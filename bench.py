@@ -2,13 +2,14 @@
 """bench.py -- the measurement contract.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload W]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the workload over one batch of synthetic input; rank 0 prints ONE JSON
-line. Every field is explained in DESIGN.md section 6.
+line; its fields are named by their keys, with units and notes beside the numbers.
 
 Workloads (config.workload):
-  quicknet         (default; BASELINE.json configs[1]) the full QuickNet `.tflite` graph, batch 256
+  quicknet         (default) the full QuickNet `.tflite` graph, batch 256
                    per GPU, through the graph host + custom-op registrations
   quicknet_large   configs[2] (batch 1024 sharded over the GPUs: --batch 128 --gpus 8)
   birealnet18      configs[3] (--batch 512)
@@ -17,14 +18,14 @@ Workloads (config.workload):
 The graph workloads take `--input-type int8` (default: the model the converter emits with
 inference_input_type=int8 -- int8 images + DEQUANTIZE in the graph, a quarter of the host-link
 bytes) or `float32`; at N = 1 the default run reports both (`f32_input`), Bi-RealNet-18 b512 and
-QuickNetLarge b128 (`other_configs`), the same graph on the two older inner products
+QuickNetLarge b128 (`other_configs`), the same graph on the other inner products
 (`legacy_paths`), and checks the GPU against the CPU checker on 4 images before it times anything.
 
-`--impl reference` times the reference's own CPU kernels (oracle/_ref: its headers compiled by
-oracle/Makefile; LCE ops: bitpack_matrix + Kernel4x2Portable indirect BGEMM + zero-padding
-correction) with PyTorch-CPU fp32 standing in for TFLite's float builtins, on the same model bytes
-and batch. It imports nothing from compute_engine_b200 (the model is synthesised by loading
-zoo.py / tflite_writer.py, pure Python, as stand-alone files).
+`--dump-outputs DIR` (GPU arm only) writes, after the timed steps, what the timed path computed
+in its last step as DIR/<name>.npy: float32, or float64 for int32 outputs. An output of more than
+DUMP_SAMPLE (3 Mi) elements is cut to at most that many, at fixed seeded positions, and the files
+of one run stay under 64 MB in all. Inputs are seeded, so two builds run with the same arguments
+can be compared output for output.
 """
 from __future__ import annotations
 
@@ -75,6 +76,8 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extras", action="store_true",
                     help="skip f32_input / other_configs / legacy_paths / parity check")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy")
     a = ap.parse_args()
     if a.batch <= 0:
         a.batch = DEFAULT_BATCH[a.workload]
@@ -87,9 +90,10 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             p = json.load(f)
-        return (float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", float(p.get("sm_max_mhz", 1965.0)),
-                float(p.get("bf16_tflops", 1590.0)), float(p.get("bf16_tflops_sustained", 1400.0)))
-    return 6650.0, "fallback (B200_PROFILING.md)", 1965.0, 1590.0, 1400.0
+        return (float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", float(p.get("sm_max_mhz", 1980.0)),
+                float(p.get("bf16_tflops", 989.0)), float(p.get("bf16_tflops_sustained", 989.0)))
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16, 1980 MHz boost
+    return 3350.0, "fallback (H100 SXM data sheet, not measured)", 1980.0, 989.0, 989.0
 
 
 class ClockSampler:
@@ -195,26 +199,8 @@ def make_stage_inputs(batch, seed):
     return [rng.standard_normal((batch, hw, hw, c), dtype=np.float32) for (hw, c) in STAGES]
 
 
-def ncu_traffic_per_launch(fname, kernel_substr=None):
-    """Mean dram__bytes_read + dram__bytes_write per launch from a committed `ncu --set full`
-    summary under profiles/ (rows of the binary-convolution kernel), or None."""
-    import csv
-    path = os.path.join(REPO, "profiles", fname)
-    try:
-        rows = list(csv.reader(open(path)))
-        hdr, units = rows[0], rows[1]
-        ir, iw = hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-        ik = hdr.index("Kernel Name") if "Kernel Name" in hdr else None
-        scale = {"Mbyte": 1e6, "Kbyte": 1e3, "Gbyte": 1e9, "byte": 1.0}
-        tot = [float(r[ir]) * scale.get(units[ir], 1.0) + float(r[iw]) * scale.get(units[iw], 1.0)
-               for r in rows[2:] if kernel_substr is None or ik is None or kernel_substr in r[ik]]
-        return sum(tot) / len(tot) if tot else None
-    except Exception:
-        return None
-
-
 def bconv_alg_bytes(in_shape, filt_shape, out_shape, out_itemsize=4):
-    """SURVEY 8(d): packed input + packed filter + output + multiplier/bias."""
+    """Algorithmic bytes: packed input + packed filter + output + multiplier/bias."""
     return (int(np.prod(in_shape)) * 4 + int(np.prod(filt_shape)) * 4 +
             int(np.prod(out_shape)) * out_itemsize + 8 * filt_shape[0])
 
@@ -303,6 +289,8 @@ def graph_config(workload, batch, world, input_type):
 
 
 def main_reference(args):
+    if args.dump_outputs:
+        raise SystemExit("--dump-outputs applies to the GPU arm only")
     if int(os.environ.get("RANK", "0")) != 0:
         return
     # The LCE kernels run on a pthread pool, the float builtins on torch's OpenMP pool. With the
@@ -335,12 +323,12 @@ def main_reference(args):
 
 
 # --------------------------------------------------------------------------- #
-# B200 arm
+# GPU arm
 # --------------------------------------------------------------------------- #
 def bind_to_gpu_numa_node(torch, index):
     """Pin this rank (and so the pinned host buffers it allocates next: first touch) to the CPUs
     of the NUMA node its GPU hangs off. Without it 8 ranks pull their images across the socket
-    link and end-to-end scaling bends (SCALE_r01: 0.76 at N = 8). Returns a description."""
+    link and end-to-end scaling bends. Returns a description."""
     try:
         p = torch.cuda.get_device_properties(index)
         bdf = f"{p.pci_domain_id:04x}:{p.pci_bus_id:02x}:{p.pci_device_id:02x}.0"
@@ -522,7 +510,8 @@ def graph_workload(D, workload, B, input_type, steps, warmup, want_e2e=True, wan
             sampler.start()
         total_ms, w0, w1 = D.timed(g.invoke, steps, sync, gs)
         clocks = sampler.stop(w0, w1) if D.rank == 0 else None
-        res = {"total_ms": total_ms, "clocks": clocks, "launches": per_step_launches * steps,
+        res = {"outputs": {f"{workload}_output": g.read(t_out)},
+               "total_ms": total_ms, "clocks": clocks, "launches": per_step_launches * steps,
                "in_bytes": in_bytes, "out_bytes": out_bytes, "fused_nodes_removed": fused,
                "graph_nodes": g.num_nodes(), "arena_bytes": g.arena_bytes(),
                "model_bytes": len(model_bytes), "e2e_ms": None}
@@ -668,7 +657,12 @@ def stack_workload(args, D):
     if D.rank == 0:
         sampler.start()
     l0 = capi.launch_count()
-    total_ms, w0, w1 = D.timed(lambda: step(True), args.steps, torch.cuda.synchronize)
+    last = {}
+
+    def timed_step():
+        last["outs"] = step(True)
+    total_ms, w0, w1 = D.timed(timed_step, args.steps, torch.cuda.synchronize)
+    outputs = {f"stage{i}_output": o for i, o in enumerate(last["outs"])}
     launches = capi.launch_count() - l0
     clocks = sampler.stop(w0, w1) if D.rank == 0 else None
     torch.cuda.synchronize()
@@ -681,7 +675,7 @@ def stack_workload(args, D):
                      for hw, c in STAGES) * LAYERS_PER_STAGE
     conv_words = sum(bconv_word_ops((B, hw, hw, c), (c, 3, 3, c // 32))
                      for hw, c in STAGES) * LAYERS_PER_STAGE
-    return {"total_ms": total_ms, "e2e_ms": e2e_ms, "clocks": clocks, "launches": launches,
+    return {"outputs": outputs, "total_ms": total_ms, "e2e_ms": e2e_ms, "clocks": clocks, "launches": launches,
             "conv_s_per_step": conv_ms * 1e-3 / args.steps, "conv_bytes": conv_bytes,
             "conv_words": conv_words, "n_conv": len(ev_pairs), "conv_share": conv_ms / total_ms,
             "in_bytes": sum(x.numel() * 4 for x in host_in),
@@ -693,12 +687,12 @@ SWEEP_K = (256, 512, 1024, 2048, 4096, 8192)
 
 
 def bgemm_sweep(args, D):
-    """BASELINE.json configs[4] / SURVEY 8(d) config 5: M, N in {256..4096}, K_bits in {256..8192},
+    """M, N in {256..4096}, K_bits in {256..8192},
     epilogues raw int32 / float / bitpacked; rows of A sharded over the ranks (W replicated).
     One JSON object per point on stderr."""
     torch = D.torch
     from compute_engine_b200 import capi
-    hbm_peak, _, sm_max, bf16_peak, _ = measured_peaks()
+    hbm_peak, _, _, bf16_peak, _ = measured_peaks()
     g = torch.Generator(device=D.dev).manual_seed(D.rank)
     flush = torch.empty(192 << 20, dtype=torch.uint8, device=D.dev)
     rows = []
@@ -727,10 +721,10 @@ def bgemm_sweep(args, D):
                         thr = np.full(N, Kb // 2, np.int32)
                         gemm, s_out = capi.BGemm(Wt, capi.OUT_BITPACKED, thresholds=thr), 1.0 / 8
                         out = torch.empty((Ml, (N + 31) // 32), dtype=torch.int32, device=D.dev)
-                    for _ in range(3):
+                    for _ in range(args.warmup):
                         gemm(A, out)
                     ts = []
-                    for _ in range(7):
+                    for _ in range(args.steps):
                         flush.zero_()                       # L2 flush between timed launches
                         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                         e0.record(); gemm(A, out); e1.record()
@@ -745,35 +739,64 @@ def bgemm_sweep(args, D):
                                  "hbm_frac": round(alg / ms / 1e6 / (hbm_peak * D.world), 4),
                                  "tensor_frac": round(tops / (2 * bf16_peak * D.world), 4)})
                     gemm.close()
+                    last_out = out
                     if D.rank == 0:
                         print(json.dumps(rows[-1]), file=sys.stderr)
-    return rows
+    return rows, {"bgemm_last_point": last_out}
 
 
-def tensor_block(conv_words, conv_s, bf16_peak, sm_max):
+DUMP_SAMPLE = 3 << 20     # elements kept of an output larger than this
+DUMP_LIMIT = 64_000_000   # bytes of all the .npy data of one run
+
+
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy in float32 (float64 for int32, which float32 cannot hold exactly). An output
+    of more than DUMP_SAMPLE elements is reduced to at most DUMP_SAMPLE of them, at indices drawn
+    from a generator seeded with the output's name, so every run samples the same positions."""
+    if not out_dir:
+        return
+    import zlib
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
+        t = t.reshape(-1)
+        if t.numel() > DUMP_SAMPLE:
+            rng = np.random.default_rng(zlib.crc32(name.encode()))
+            idx = np.unique(rng.integers(0, t.numel(), DUMP_SAMPLE))
+            t = t[torch.from_numpy(idx).to(t.device)]
+        x = t.cpu().numpy()
+        x = x.astype(np.float64 if x.dtype == np.int32 else np.float32)
+        total += x.nbytes
+        if total > DUMP_LIMIT:
+            raise SystemExit(f"--dump-outputs: the outputs exceed {DUMP_LIMIT} bytes at {name}")
+        np.save(os.path.join(out_dir, name + ".npy"), x)
+
+
+def tensor_block(conv_words, conv_s, bf16_peak):
     tops = 2 * 32 * conv_words / conv_s / 1e12
     peak = 2.0 * bf16_peak
     return {"achieved": tops, "unit": "TOP/s (int8 MAC x 2)", "peak": peak, "frac": tops / peak,
-            "peak_source": "2 x MEASURED_PEAKS.json bf16_tflops (kind::i8 issues at twice the bf16 "
-                           "rate; tools/tc_probe.cu measures 7708 MAC/clk/SM at N = 256)",
-            "legacy_mma_sync_peak": 148 * 2046.5 * sm_max * 1e6 * 2 / 1e12}
+            "peak_source": "2 x the bf16 peak (dense int8 wgmma issues at twice the bf16 rate)"}
 
 
 def main_b200(args):
     D = Dist()
     from compute_engine_b200 import capi
     capi.lib()
-    hbm_peak, peak_src, sm_max, bf16_peak, _ = measured_peaks()
+    hbm_peak, peak_src, _, bf16_peak, _ = measured_peaks()
     if args.workload == "bgemm_sweep":
-        rows = bgemm_sweep(args, D)
+        rows, outputs = bgemm_sweep(args, D)
         if D.rank == 0:
+            dump_outputs(args.dump_outputs, outputs)
             best = max(rows, key=lambda r: r["binary_TOPS"])
             best_hbm = max(rows, key=lambda r: r["hbm_frac"])
             emit({"metric": METRIC["bgemm_sweep"], "value": best["binary_TOPS"],
-                  "unit": "binary TOPS", "n_gpus": D.world, "steps": 7, "warmup": 3,
+                  "unit": "binary TOPS", "n_gpus": D.world, "steps": args.steps, "warmup": args.warmup,
                   "ms_per_step": best["ms"], "higher_is_better": True,
                   "scaling": "strong", "vs_baseline": None,
-                  "dtype": "s8 x s8 -> s32 on tcgen05 kind::i8 (== xor-popcount, bit-exact)",
+                  "dtype": "s8 x s8 -> s32 on the int8 tensor pipe (== xor-popcount, bit-exact)",
                   "data": "synthetic",
                   "roofline": {"bound": "hbm", "achieved": best_hbm["alg_GBps"], "peak": hbm_peak * D.world,
                                "unit": "GB/s", "frac": best_hbm["hbm_frac"], "traffic": None,
@@ -801,13 +824,14 @@ def main_b200(args):
     launches = int(D.sum(r["launches"]))
     multi_extra = None
     if D.world > 1 and args.workload == "quicknet" and not args.no_extras:
-        # BASELINE.json configs[2] next to configs[1]: QuickNetLarge, batch 128 per GPU (1024 at N = 8)
+        # QuickNetLarge next to QuickNet: batch 128 per GPU (1024 at N = 8)
         multi_extra = graph_workload(D, "quicknet_large", 128, input_type, max(5, min(K, 10)), 3,
                                      want_e2e=not args.no_e2e)
     if D.rank != 0:
         if D.world > 1:
             D.dist.destroy_process_group()
         return
+    dump_outputs(args.dump_outputs, r.pop("outputs"))
     ms_per_step = r["total_ms"] / K
     n_launch = max(r["n_conv"] // K, 1)
     achieved = r["conv_bytes"] / r["conv_s_per_step"] / 1e9
@@ -815,40 +839,36 @@ def main_b200(args):
            else {"workload": args.workload, "batch_per_gpu": B, "global_batch": B * D.world})
     cfg.update({"parallelism": f"dp{D.world}: batch-sharded, one NCCL broadcast of the model at load, "
                                "no collective per step",
-                "l2": "activations per step exceed the 126 MB L2 (largest tensor 205 MB)",
+                "l2": "activations per step exceed the 50 MB L2 (largest tensor 205 MB)",
                 "numa": D.numa})
     line = {
         "metric": METRIC[args.workload], "value": B * D.world / (ms_per_step * 1e-3),
         "unit": "images/s", "n_gpus": D.world, "steps": K, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None,
-        "dtype": "s8 x s8 -> s32 (binary convs on tcgen05 kind::i8, bit-exact with xor-popcount) + "
+        "dtype": "s8 x s8 -> s32 (binary convs on the int8 tensor pipe, bit-exact with xor-popcount) + "
                  "f32 (builtins, epilogue)",
         "data": "synthetic", "config": cfg, "clocks": r["clocks"], "gpu_launches": launches,
         "roofline": {
-            "kernel": "lce::tc::bconv_tc_kernel (LceBconv2d [+ADD +LceQuantize]: TMA-staged packed "
-                      "activations -> bits->bytes in TMEM -> tcgen05.mma kind::i8 -> fused "
-                      "OutputTransform epilogue -> TMA store)",
+            "kernel": "LceBconv2d [+ADD +LceQuantize]: lce::bconv_imma_kernel (mma.sync int8) where "
+                      "eligible, else lce::tc::bconv_tc_kernel (wgmma s8), bits->bytes in registers, "
+                      "fused OutputTransform epilogue",
             "bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
             "frac": achieved / hbm_peak, "peak_source": peak_src,
-            "traffic": ncu_traffic_per_launch("r02_ncu_bconv_tc_summary.csv", "bconv_tc")
-            if args.workload == "quicknet" else None,
-            "traffic_unit": "bytes per launch (mean over the binary-conv launches of one step, "
-                            "ncu --set full, profiles/r02_ncu_bconv_tc_summary.csv)",
             "alg_bytes_per_launch": r["conv_bytes"] / n_launch,
             "launches_timed": r["n_conv"],
             "avg_launch_ms": r["conv_s_per_step"] * 1e3 / n_launch,
             "share_of_step": r["conv_share"],
             "timing": "separate eager pass of the same K steps with CUDA events around every node on "
                       "the graph's stream (events cannot sit inside a replayed CUDA graph)",
-            "tensor": tensor_block(r["conv_words"], r["conv_s_per_step"], bf16_peak, sm_max)},
+            "tensor": tensor_block(r["conv_words"], r["conv_s_per_step"], bf16_peak)},
     }
     if r.get("step_alg_bytes"):
         floor_ms = r["step_alg_bytes"] / (hbm_peak * 1e9) * 1e3
         line["step_roofline"] = {"alg_bytes_per_step": r["step_alg_bytes"], "hbm_ms": floor_ms,
                                  "frac": floor_ms / (r["total_ms"] / K),
                                  "note": "all kernels of one step: operands read once + results written once "
-                                         "(binary layers: SURVEY 8d bytes) at the measured HBM rate, against "
+                                         "(binary layers: packed input + filter + output) at the HBM rate, against "
                                          "ms_per_step"}
     if r.get("e2e_ms") is not None:
         line["e2e"] = {"value": B * D.world / (r["e2e_ms"] / K * 1e-3), "unit": "images/s",
@@ -875,15 +895,15 @@ def main_b200(args):
             "unit": "images/s", "steps": Kx,
             "note": "the same graph with the other input type, same run"}
         line["legacy_paths"] = {}
-        for name, env in (("mma_sync_int8", {"LCE_B200_BCONV_TC": "0"}),
+        for name, env in (("wgmma_s8", {"LCE_B200_BCONV_IMMA": "0"}),
                           ("xor_popc", {"LCE_B200_BCONV_TC": "0", "LCE_B200_BCONV_IMMA": "0"})):
             x = graph_workload(D, args.workload, B, input_type, Kx, 3, want_e2e=False,
                                want_profile=False, model_bytes=model_bytes, env=env)
             line["legacy_paths"][name] = {"value": B / (x["total_ms"] / Kx * 1e-3), "unit": "images/s",
                                           "ms_per_step": x["total_ms"] / Kx, "env": env}
-        line["legacy_paths"]["note"] = ("same graph, same run, every LceBconv2d on the round-1 kernels: "
-                                        "int8 mma.sync (lce_b200_imma.cuh) and the XOR + POPC kernel "
-                                        "north_star describes (lce_b200_kernels.cuh)")
+        line["legacy_paths"]["note"] = ("same graph, same run, the LceBconv2d layers on the other inner "
+                                        "products: wgmma s8 (lce_b200_tc.cuh) in place of mma.sync int8, "
+                                        "and the XOR + POPC kernel (lce_b200_kernels.cuh) for all of them")
         line["other_configs"] = {}
         for wl, b in (("birealnet18", 512), ("quicknet_large", 128)):
             if wl == args.workload:

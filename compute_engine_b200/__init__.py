@@ -1,4 +1,4 @@
-"""compute_engine_b200 -- a B200-native (sm_100a) implementation of the one hot
+"""compute_engine_b200 -- an H100-native (sm_90a) implementation of the one hot
 path of larq/compute-engine: LceQuantize -> LceBconv2d (-> LceBMaxPool2d /
 LceDequantize), behind the reference's TFLite custom-op surface.
 

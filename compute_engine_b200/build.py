@@ -1,7 +1,7 @@
 """In-tree build of the native pieces (no JIT cache: the built .so files travel to
 the GPU box with the gpurun snapshot).
 
-  liblce_b200.so        CUDA kernels + C-ABI (nvcc, sm_100a only)
+  liblce_b200.so        CUDA kernels + C-ABI (nvcc, sm_90a only)
   liblce_b200_host.so   C++ TFLite-custom-op shell / graph host above the C-ABI
 """
 from __future__ import annotations
@@ -15,7 +15,7 @@ REPO = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 INC = os.path.join(REPO, "include")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 

@@ -1,5 +1,5 @@
 // builtin_ops.cc -- TfLiteRegistrations for the float builtins QuickNet /
-// QuickNetLarge / Bi-RealNet-18 use around the binary path (SURVEY 8f-1), backed by
+// QuickNetLarge / Bi-RealNet-18 use around the binary path, backed by
 // the fp32 CUDA kernels of lce_b200_builtins.cu. Shape inference follows TFLite's
 // builtin kernels (tensorflow/lite/kernels/{conv,depthwise_conv,pooling,add,mul,
 // fully_connected,softmax,reduce,reshape,activations}.cc). Device arena only.

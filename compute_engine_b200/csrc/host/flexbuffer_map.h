@@ -5,7 +5,7 @@
 // vendored and cannot be linked here. The attributes are always ONE map of integer
 // scalars written by LCE/mlir/ir/lce_ops.cc:36-64, so a map reader (and, for the
 // synthetic-model writer and the tests, a map writer) is all that is needed. The
-// wire format is restated from SURVEY.md section 9.2 and pinned by the byte blobs
+// wire format is restated from the FlexBuffers format and pinned by the byte blobs
 // the reference's own tests hold (LCE/mlir/tests/legalize-lce.mlir:9,21) in
 // tests/test_host_ops.py.
 #ifndef LCE_B200_HOST_FLEXBUFFER_MAP_H_

@@ -2,7 +2,7 @@
 // lce_b200::Graph through an OpResolver: the role FlatBufferModel +
 // InterpreterBuilder play for the reference (examples/lce_minimal.cc:31-45,
 // LCE/tflite/python/interpreter_wrapper_lite.cc:28-58). flatbuffers is not vendored,
-// so table access is hand-written from the wire format (SURVEY 9.1): uint32 root
+// so table access is hand-written from the wire format: uint32 root
 // offset, int32 back-offset from a table to its vtable, uint16 vtable slots, uint32
 // forward offsets for strings / vectors / sub-tables. Every access is bounds-checked.
 #include <algorithm>

@@ -25,7 +25,7 @@
 namespace {
 thread_local std::string g_err;
 std::atomic<uint64_t> g_launches{0};
-std::atomic<uint64_t> g_path[3] = {};   // inner-product launches: tcgen05 / mma.sync / XOR + POPC
+std::atomic<uint64_t> g_path[3] = {};   // inner-product launches: wgmma / mma.sync / XOR + POPC
 }  // namespace
 
 // shared with lce_b200_builtins.cu
@@ -76,7 +76,7 @@ struct PerDeviceOnce {
 constexpr int kChanPad = 128;
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
-int grid_for(long long work_items, int per_block, int max_blocks = 148 * 16) {
+int grid_for(long long work_items, int per_block, int max_blocks = 132 * 16) {
   long long b = (work_items + per_block - 1) / per_block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -143,7 +143,7 @@ struct GemmCore {
   int32_t* wpop = nullptr;      // popcount of each channel's filter row (padded by BN)
   int imma_Kc_v = 0, imma_chunks = 1;
   size_t imma_smem = 0;
-  // tcgen05 inner product (lce_b200_tc.cuh); absent when LCE_B200_BCONV_TC=0 or ineligible
+  // wgmma inner product (lce_b200_tc.cuh); absent when LCE_B200_BCONV_TC=0 or ineligible
   bool tc_ok = false;
   uint8_t* tc_wt = nullptr;        // [n_tiles][S_t][BN x 128 B] int8 stage images
   int32_t* tc_wpop2 = nullptr;     // 2 * popcount of each filter row, padded
@@ -228,11 +228,11 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
   const long long m_tiles = (p.M + lce::kBM - 1) / lce::kBM;
   if (m_tiles > INT_MAX) return fail("too many output pixels");
   if (p.img_words >= (1LL << 31)) return fail("input image too large (>= 2^31 packed words)");
-  if (c.tc_ok) {
-    // tcgen05 inner product: the same int32 accumulators again, persistent 128 x BN tiles
-    const int rc = tc_launch(c, p, s);
-    if (rc >= 0) return rc;
-  }
+  // Which inner product: on H100 the mma.sync int8 kernel runs the QuickNet graph faster than
+  // the wgmma kernel (bench.py reports both in one run), so it takes every
+  // plan it can (full 64-channel tiles, float or raw-accumulator output); the wgmma kernel takes
+  // the rest it is eligible for (bitpacked and int8 outputs, other channel counts), XOR + POPC
+  // what is left. All three produce the same int32 accumulators.
   if (c.wt_nat != nullptr && p.vec_store) {
     // int8 tensor-pipe inner product: 128 x 64 tiles, the same int32 accumulators as bconv_kernel
     lce::ConvKParams q = p;
@@ -248,6 +248,11 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
       default: return launch_imma_v<1>(c.out_type, q, igrid, ismem, s);
     }
   }
+  if (c.tc_ok) {
+    // wgmma inner product: persistent 128 x BN tiles
+    const int rc = tc_launch(c, p, s);
+    if (rc >= 0) return rc;
+  }
   dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(c.groups * c.tiles_per_group));
   const size_t smem = c.smem_bytes + (p.res_stage ? lce::kResStageBytes : 0);
   switch (c.V) {
@@ -259,7 +264,7 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
 
 
 // ------------------------------------------------------------------------- //
-// tcgen05 path (lce_b200_tc.cuh): plan-time weight images and the launch.
+// wgmma path (lce_b200_tc.cuh): plan-time weight images and the launch.
 // ------------------------------------------------------------------------- //
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
@@ -279,7 +284,7 @@ EncodeTiledFn tensor_map_encoder() {
 }
 int num_sms() {
   static int cache[64] = {};
-  int dev = 0, v = 148;
+  int dev = 0, v = 132;
   cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && cache[dev]) return cache[dev];
   cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
@@ -299,10 +304,11 @@ int build_tc_weights(GemmCore* c, const int32_t* d_filter, bool want_tap_popc) {
   c->tc_ok = false;
   if (!tc_enabled() || c->groups != 1 || tensor_map_encoder() == nullptr) return 0;
   if ((c->out_type == LCE_OUT_FLOAT || c->out_type == LCE_OUT_RAW_ACC) && (c->cout % 4 != 0 || c->cout < 32))
-    return 0;  // TMA store: 16-byte row pitch, 32-column boxes
+    return 0;  // two-channel stores, 32-channel sign words
   if (want_tap_popc && c->taps > 64) return 0;
   const int Cw = c->Cw_pg;
-  c->tc_BN = c->cout > 64 ? 128 : (c->cout > 32 ? 64 : 32);
+  // 64-channel tiles: their kernel fits two CTAs per SM (128-channel tiles need too many registers)
+  c->tc_BN = c->cout > 32 ? 64 : 32;
   c->tc_n_tiles = cdiv(c->cout, c->tc_BN);
   if (Cw % 4 == 0) {
     c->tc_flat = 0; c->tc_V = 4;
@@ -360,25 +366,30 @@ int tc_max_halo_px(const lce::ConvKParams& p) {
   return static_cast<int>(std::min<long long>(best, INT_MAX));
 }
 
-template <int V, int OUT>
-int launch_tc_vo(const CUtensorMap& tm_in, const CUtensorMap& tm_res, const CUtensorMap& tm_out,
-                 const lce::tc::TcParams& t, int grid, size_t smem, cudaStream_t s) {
+template <int V, int OUT, int BN>
+int launch_tc_vob(const CUtensorMap& tm_in, const lce::tc::TcParams& t, int grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::tc::bconv_tc_kernel<V, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CUDA_OK(cudaFuncSetAttribute(lce::tc::bconv_tc_kernel<V, OUT, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(kTcSmemBudget)));
-  lce::tc::bconv_tc_kernel<V, OUT><<<grid, lce::tc::kThreads, smem, s>>>(tm_in, tm_res, tm_out, t);
+  lce::tc::bconv_tc_kernel<V, OUT, BN><<<grid, lce::tc::kThreads, smem, s>>>(tm_in, t);
   g_path[0].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_tc_kernel");
 }
+template <int V, int OUT>
+int launch_tc_vo(const CUtensorMap& tm_in, const lce::tc::TcParams& t, int grid, size_t smem, cudaStream_t s) {
+  switch (t.BN) {
+    case 64: return launch_tc_vob<V, OUT, 64>(tm_in, t, grid, smem, s);
+    default: return launch_tc_vob<V, OUT, 32>(tm_in, t, grid, smem, s);
+  }
+}
 template <int V>
-int launch_tc_v(int out_type, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c,
-                const lce::tc::TcParams& t, int grid, size_t smem, cudaStream_t s) {
+int launch_tc_v(int out_type, const CUtensorMap& tm_in, const lce::tc::TcParams& t, int grid, size_t smem, cudaStream_t s) {
   switch (out_type) {
-    case LCE_OUT_FLOAT: return launch_tc_vo<V, LCE_OUT_FLOAT>(a, b, c, t, grid, smem, s);
-    case LCE_OUT_INT8: return launch_tc_vo<V, LCE_OUT_INT8>(a, b, c, t, grid, smem, s);
-    case LCE_OUT_BITPACKED: return launch_tc_vo<V, LCE_OUT_BITPACKED>(a, b, c, t, grid, smem, s);
-    default: return launch_tc_vo<V, LCE_OUT_RAW_ACC>(a, b, c, t, grid, smem, s);
+    case LCE_OUT_FLOAT: return launch_tc_vo<V, LCE_OUT_FLOAT>(tm_in, t, grid, smem, s);
+    case LCE_OUT_INT8: return launch_tc_vo<V, LCE_OUT_INT8>(tm_in, t, grid, smem, s);
+    case LCE_OUT_BITPACKED: return launch_tc_vo<V, LCE_OUT_BITPACKED>(tm_in, t, grid, smem, s);
+    default: return launch_tc_vo<V, LCE_OUT_RAW_ACC>(tm_in, t, grid, smem, s);
   }
 }
 
@@ -393,10 +404,9 @@ int tc_launch(GemmCore& c, const lce::ConvKParams& p, cudaStream_t s) {
   const long long total_words = total_px * p.Cw_total;
   if (total_words >= (1LL << 31) || total_px < 1) return -1;
   if ((reinterpret_cast<uintptr_t>(p.in) & 15u) != 0) return -1;
-  const bool tma_out = c.out_type == LCE_OUT_FLOAT || c.out_type == LCE_OUT_RAW_ACC;
-  if (tma_out && (reinterpret_cast<uintptr_t>(p.out) & 15u) != 0) return -1;
-  if (p.residual != nullptr && (reinterpret_cast<uintptr_t>(p.residual) & 15u) != 0) return -1;
-  if (c.out_type == LCE_OUT_INT8 && (reinterpret_cast<uintptr_t>(p.out) & 15u) != 0) return -1;
+  // the epilogue stores two channels at a time
+  if ((reinterpret_cast<uintptr_t>(p.out) & 7u) != 0) return -1;
+  if (p.residual != nullptr && (reinterpret_cast<uintptr_t>(p.residual) & 7u) != 0) return -1;
   if (c.tc_key_M != p.M || c.tc_key_H != p.H || c.tc_key_W != p.W) {
     c.tc_max_px = tc_max_halo_px(p);
     c.tc_key_M = p.M; c.tc_key_H = p.H; c.tc_key_W = p.W;
@@ -411,7 +421,7 @@ int tc_launch(GemmCore& c, const lce::ConvKParams& p, cudaStream_t s) {
   t.cout = c.cout; t.BN = c.tc_BN; t.n_tiles = c.tc_n_tiles;
   t.m_tiles = static_cast<int>((p.M + T::kBM - 1) / T::kBM);
   t.S_full = c.tc_S_full; t.S_last = c.tc_S_last; t.S_t = c.tc_S_t;
-  // shared memory: weights | halo stages | epilogue slots | barriers
+  // shared memory: weights | halo stages | barriers
   size_t raw_stage;
   if (c.tc_flat) raw_stage = static_cast<size_t>(cdiv(c.tc_max_px * c.Cw_pg + 3, 256)) * 1024;
   else raw_stage = static_cast<size_t>(cdiv(c.tc_max_px, 128)) * 128 * c.tc_CcB * 4;
@@ -419,56 +429,45 @@ int tc_launch(GemmCore& c, const lce::ConvKParams& p, cudaStream_t s) {
   t.raw_stage_bytes = static_cast<int>(raw_stage);
   const size_t stage_bytes = static_cast<size_t>(c.tc_BN) * 32 * T::kWS;     // one ring slot
   const size_t resident_bytes = static_cast<size_t>(c.tc_BN) * 32 * t.taps * c.Cw_pg;  // all K words, dense
-  const bool has_res = p.residual != nullptr;
-  // Epilogue staging slots (16 KB = 128 rows x 32 channels each; with a shortcut they are also the
-  // TMA landing zone of the residual tiles, so their number is the prefetch depth of that stream):
-  // as many as fit beside the weights, an even number, at most 8 with and 4 without a shortcut.
-  const int ns_max = tma_out ? (has_res ? T::kMaxNS : 4) : 0;
-  const int ns_min = tma_out ? 2 : 0;
-  const size_t fixed = T::kNR * raw_stage + T::kBarBytes + T::kTabBytes;
-  if (fixed + ns_min * T::kSlotBytes > kTcSmemBudget) return -1;
-  auto room = [&](int ns) { return kTcSmemBudget - fixed - static_cast<size_t>(ns) * T::kSlotBytes; };
-  const bool can_reside = c.tc_n_tiles == 1 && c.tc_S_t <= T::kMaxNB && room(ns_min) >= resident_bytes;
-  int nS = ns_min;
+  const size_t fixed = T::kNR * raw_stage + T::kBarBytes;
+  // two CTAs per SM where a layout fits half the shared memory, else one with all of it
+  constexpr size_t kHalfBudget = (227u * 1024u / 2 - 1024u) & ~size_t{1023};
+  const int ctas = fixed + 2 * stage_bytes <= kHalfBudget ? 2 : 1;
+  const size_t budget = ctas == 2 ? kHalfBudget : kTcSmemBudget;
+  if (fixed + 2 * stage_bytes > budget) return -1;
+  const size_t room = budget - fixed;
   size_t b_bytes;
-  if (can_reside) {
+  if (c.tc_n_tiles == 1 && c.tc_S_t <= T::kMaxNB && room >= ((resident_bytes + 1023) & ~size_t{1023})) {
     t.b_resident = 1;
     t.nB = c.tc_S_t;
     b_bytes = (resident_bytes + 1023) & ~size_t{1023};
-    while (nS + 2 <= ns_max && room(nS + 2) >= b_bytes) nS += 2;
   } else {
+    // the weights stream through a ring of as many stages as fit (2 .. kMaxRing)
     t.b_resident = 0;
-    // the weights stream through a ring whose slots are the A stages' (one barrier pair per stage)
-    t.nB = T::kNA;
-    b_bytes = T::kNA * stage_bytes;
-    if (room(ns_min) < b_bytes) return -1;
-    while (nS + 2 <= std::min(ns_max, 4) && room(nS + 2) >= b_bytes) nS += 2;
+    t.nB = static_cast<int>(std::min<size_t>(T::kMaxRing, room / stage_bytes));
+    b_bytes = t.nB * stage_bytes;
   }
-  t.nS = nS;
   t.Kw_total = t.taps * c.Cw_pg;
   t.off_raw = static_cast<int>(b_bytes);
-  t.off_slots = t.off_raw + T::kNR * t.raw_stage_bytes;
-  t.off_tab = t.off_slots + nS * T::kSlotBytes;
-  t.off_bar = t.off_tab + T::kTabBytes;
+  t.off_bar = t.off_raw + T::kNR * t.raw_stage_bytes;
   const size_t smem = static_cast<size_t>(t.off_bar) + T::kBarBytes;
   t.clamp_min = p.clamp_min; t.clamp_max = p.clamp_max;
-  t.has_res = has_res ? 1 : 0; t.residual_act = p.residual_act;
+  t.has_res = p.residual != nullptr ? 1 : 0; t.residual_act = p.residual_act;
   t.cw_out = p.cw_out; t.zp_half = p.zp_half; t.ldc = c.tc_ldc;
   t.wt = c.tc_wt; t.mul = p.mul; t.bias = p.bias; t.wpop2 = c.tc_wpop2; t.thr = p.thr;
   t.tap_popc_t = p.tap_popc != nullptr ? c.tc_tap_popc_t : nullptr;
   t.zp_float = p.zp_float; t.cin_pg = p.cin_pg;
   t.zpc_cache = c.tc_zpc_cache;
   if (t.zp_float && t.zpc_cache == nullptr) return -1;
+  t.residual = p.residual;
   t.out = p.out; t.packed_out = p.packed_out;
   t.fd_ohw = lce::make_fastdiv(static_cast<uint32_t>(ohw));
   t.fd_ow = lce::make_fastdiv(p.OW);
   t.fd_kw = lce::make_fastdiv(p.KW);
-  t.fd_cwv_full = lce::make_fastdiv(c.tc_CcB / c.tc_V);
-  t.fd_cwv_last = lce::make_fastdiv((c.Cw_pg - (c.tc_n_chunks - 1) * c.tc_CcB) / c.tc_V);
   t.fd_mt = lce::make_fastdiv(t.m_tiles);
 
   EncodeTiledFn enc = tensor_map_encoder();
-  CUtensorMap tm_in, tm_res, tm_out;
+  CUtensorMap tm_in;
   cuuint32_t es[2] = {1, 1};
   if (c.tc_flat) {
     cuuint64_t gd[1] = {static_cast<cuuint64_t>(total_words)};
@@ -487,54 +486,12 @@ int tc_launch(GemmCore& c, const lce::ConvKParams& p, cudaStream_t s) {
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return fail("cuTensorMapEncodeTiled (activations) failed");
   }
-  tm_res = tm_in;
-  tm_out = tm_in;
-  if (tma_out) {
-    cuuint64_t gd[2] = {static_cast<cuuint64_t>(c.cout), static_cast<cuuint64_t>(p.M)};
-    cuuint64_t gs[1] = {static_cast<cuuint64_t>(c.cout) * 4};
-    cuuint32_t box_st[2] = {32, 32};
-    cuuint32_t box_ld[2] = {32, 128};
-    const CUtensorMapDataType dt =
-        c.out_type == LCE_OUT_FLOAT ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_INT32;
-    if (enc(&tm_out, dt, 2, p.out, gd, gs, box_st, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return fail("cuTensorMapEncodeTiled (output) failed");
-    if (has_res &&
-        enc(&tm_res, dt, 2, const_cast<float*>(p.residual), gd, gs, box_ld, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return fail("cuTensorMapEncodeTiled (shortcut) failed");
-  }
   const long long items = static_cast<long long>(t.n_tiles) * t.m_tiles;
-  const int grid = static_cast<int>(std::min<long long>(items, num_sms()));
-  static long long* d_prof = nullptr;
-  static const bool prof_on = [] { const char* e = getenv("LCE_B200_TC_PROF"); return e && e[0] == '1'; }();
-  if (prof_on) {
-    // development aid: per-role cycle counters of block 0, printed after a synchronising copy
-    if (!d_prof) cudaMalloc(&d_prof, 20 * 8 * sizeof(long long));
-    cudaMemsetAsync(d_prof, 0, 20 * 8 * sizeof(long long), s);
-    t.prof = d_prof;
-  }
-  struct ProfDump {
-    long long* d; cudaStream_t s; const T::TcParams* t; int grid;
-    ~ProfDump() {
-      if (!d) return;
-      long long h[160];
-      cudaStreamSynchronize(s);
-      cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);
-      fprintf(stderr, "[tc prof] M=%lld BN=%d S_t=%d nB=%d res=%d resident=%d items=%d grid=%d\n", t->M, t->BN, t->S_t,
-              t->nB, t->has_res, t->b_resident, t->n_tiles * t->m_tiles, grid);
-      const char* names[20] = {"exp0", "exp1", "exp2", "exp3", "exp4", "exp5", "exp6", "exp7", "epi0", "epi1", "epi2", "epi3",
-                               "epi4", "epi5", "epi6", "epi7", "act-prod", "res-prod", "w-prod", "mma"};
-      for (int w : {16, 19, 18, 17, 0, 4, 8, 12})
-        fprintf(stderr, "[tc prof]  %-8s total=%lld  c1=%lld c2=%lld c3=%lld c4=%lld c5=%lld c6=%lld\n", names[w], h[w * 8],
-                h[w * 8 + 1], h[w * 8 + 2], h[w * 8 + 3], h[w * 8 + 4], h[w * 8 + 5], h[w * 8 + 6]);
-    }
-  } prof_dump{prof_on ? d_prof : nullptr, s, &t, grid};
+  const int grid = static_cast<int>(std::min<long long>(items, static_cast<long long>(ctas) * num_sms()));
   switch (c.tc_V) {
-    case 4: return launch_tc_v<4>(c.out_type, tm_in, tm_res, tm_out, t, grid, smem, s);
-    case 2: return launch_tc_v<2>(c.out_type, tm_in, tm_res, tm_out, t, grid, smem, s);
-    default: return launch_tc_v<1>(c.out_type, tm_in, tm_res, tm_out, t, grid, smem, s);
+    case 4: return launch_tc_v<4>(c.out_type, tm_in, t, grid, smem, s);
+    case 2: return launch_tc_v<2>(c.out_type, tm_in, t, grid, smem, s);
+    default: return launch_tc_v<1>(c.out_type, tm_in, t, grid, smem, s);
   }
 }
 
@@ -556,7 +513,7 @@ int pw_tf32_conv(const float* in, const float* filter, const float* bias, float*
   // batch mates): eligibility looks at the layer's shape only; `pairs_ok` = even pixels per image.
   const bool pairs = K == 16 && N == 64 && pairs_ok && (M & 1) == 0;
   // N: whole 128-column tiles, or (no packed output) any multiple of 4 -- TMA zero-fills the filter
-  // rows past N and clips the stores (FULLY_CONNECTED's 1000 logits)
+  // rows past N and the stores are guarded by n < N (FULLY_CONNECTED's 1000 logits)
   if (!pairs && ((K & 31) != 0 || K > 4096 || (N & 3) != 0 || ((N & 127) != 0 && packed != nullptr))) return -1;
   namespace P = lce::pw;
   P::PwParams p{};
@@ -575,9 +532,9 @@ int pw_tf32_conv(const float* in, const float* filter, const float* bias, float*
   p.bias = bias;
   p.packed = packed;
   const int Kp = pairs ? 32 : K;
-  CUtensorMap tm_a, tm_w, tm_out;
+  CUtensorMap tm_a, tm_w;
   cuuint32_t es[2] = {1, 1};
-  cuuint32_t box_ld[2] = {32, 128}, box_st[2] = {32, 32};
+  cuuint32_t box_ld[2] = {32, 128};
   {
     cuuint64_t gd[2] = {static_cast<cuuint64_t>(Kp), static_cast<cuuint64_t>(p.M)};
     cuuint64_t gs[1] = {static_cast<cuuint64_t>(Kp) * 4};
@@ -594,43 +551,17 @@ int pw_tf32_conv(const float* in, const float* filter, const float* bias, float*
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return fail("cuTensorMapEncodeTiled (pointwise filter) failed");
   }
-  {
-    cuuint64_t gd[2] = {static_cast<cuuint64_t>(p.N), static_cast<cuuint64_t>(p.M)};
-    cuuint64_t gs[1] = {static_cast<cuuint64_t>(p.N) * 4};
-    if (enc(&tm_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, out, gd, gs, box_st, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return fail("cuTensorMapEncodeTiled (pointwise output) failed");
-  }
+  p.out = out;
   static PerDeviceOnce once;
   if (once.need())
     CUDA_OK(cudaFuncSetAttribute(P::pw_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(P::kPwSmem)));
   const int grid = static_cast<int>(std::min<long long>(m_tiles * p.n_tiles, num_sms()));
-  static long long* d_prof = nullptr;
-  static const bool prof_on = [] { const char* e = getenv("LCE_B200_TC_PROF"); return e && e[0] == '1'; }();
-  if (prof_on) {
-    if (!d_prof) cudaMalloc(&d_prof, 22 * 8 * sizeof(long long));
-    cudaMemsetAsync(d_prof, 0, 22 * 8 * sizeof(long long), static_cast<cudaStream_t>(stream));
-    p.prof = d_prof;
-  }
-  P::pw_tf32_kernel<<<grid, P::kPwThreads, P::kPwSmem, static_cast<cudaStream_t>(stream)>>>(tm_a, tm_w, tm_out, p);
-  if (prof_on) {
-    // development aid (LCE_TC_PROF build): per-role cycle counters of block 0
-    long long h[22 * 8];
-    cudaStreamSynchronize(static_cast<cudaStream_t>(stream));
-    cudaMemcpy(h, d_prof, sizeof(h), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[pw prof] M=%lld N=%d KB=%d resident=%d pairs=%d items=%lld grid=%d\n", p.M, p.N, p.KB, p.w_resident, p.pairs,
-            m_tiles * p.n_tiles, grid);
-    const char* names[22] = {"split0", "split1", "split2", "split3", "epi", "epi", "epi", "epi", "epi", "epi", "epi", "epi", "epi",
-                             "epi", "epi", "epi", "epi", "epi", "epi", "epi", "tma", "mma"};
-    for (int w : {20, 21, 0, 3, 4, 11, 19})
-      fprintf(stderr, "[pw prof]  %-7s w%-2d total=%lld  c1=%lld c2=%lld c3=%lld c4=%lld n=%lld\n", names[w], w, h[w * 8], h[w * 8 + 1],
-              h[w * 8 + 2], h[w * 8 + 3], h[w * 8 + 4], h[w * 8 + 5]);
-  }
+  P::pw_tf32_kernel<<<grid, P::kPwThreads, P::kPwSmem, static_cast<cudaStream_t>(stream)>>>(tm_a, tm_w, p);
   g_pw_launches.fetch_add(1, std::memory_order_relaxed);
   return launch_check("pw_tf32_kernel");
 }
 uint64_t pw_tf32_launches() { return g_pw_launches.load(); }
-// CONV_2D 7x7 / stride 2 / 3 -> 64 (Bi-RealNet's stem) on tcgen05 kind::tf32 (lce_b200_pw.cuh):
+// CONV_2D 7x7 / stride 2 / 3 -> 64 (Bi-RealNet's stem) on wgmma tf32 (lce_b200_pw.cuh):
 // 0 = launched, -1 = not this shape, > 0 = error.
 int stem7_tf32_conv(const float* in, const float* filter, const float* bias, float* out, int B, int H, int W, int OH, int OW,
                     int ph, int pw, int act, void* stream) {
@@ -641,25 +572,18 @@ int stem7_tf32_conv(const float* in, const float* filter, const float* bias, flo
   namespace P = lce::pw;
   P::Stem7Params p{};
   p.M = static_cast<long long>(B) * OH * OW;
-  const long long m_tiles = (p.M + 127) / 128;
-  if (m_tiles > (1 << 23)) return -1;
+  const long long m_tiles = (p.M + 63) / 64;
+  if (m_tiles > (1 << 24)) return -1;
   p.H = H; p.W = W; p.OH = OH; p.OW = OW; p.ph = ph; p.pw = pw;
   p.m_tiles = static_cast<int>(m_tiles);
   p.act = act;
-  p.in = in; p.filter = filter; p.bias = bias;
-  CUtensorMap tm_out;
-  cuuint32_t es[2] = {1, 1};
-  cuuint32_t box_st[2] = {32, 32};
-  cuuint64_t gd[2] = {64, static_cast<cuuint64_t>(p.M)};
-  cuuint64_t gs[1] = {64 * 4};
-  if (enc(&tm_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, out, gd, gs, box_st, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return fail("cuTensorMapEncodeTiled (7x7 stem output) failed");
+  p.in = in; p.filter = filter; p.bias = bias; p.out = out;
   static PerDeviceOnce once;
   if (once.need())
     CUDA_OK(cudaFuncSetAttribute(P::stem7_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(P::kS7Smem)));
-  const int grid = static_cast<int>(std::min<long long>(m_tiles, num_sms()));
-  P::stem7_tf32_kernel<<<grid, P::kS7Threads, P::kS7Smem, static_cast<cudaStream_t>(stream)>>>(tm_out, p);
+  // two warpgroups per CTA, two CTAs per SM
+  const int grid = static_cast<int>(std::min<long long>((m_tiles + 1) / 2, 2LL * num_sms()));
+  P::stem7_tf32_kernel<<<grid, P::kS7Threads, P::kS7Smem, static_cast<cudaStream_t>(stream)>>>(p);
   g_pw_launches.fetch_add(1, std::memory_order_relaxed);
   return launch_check("stem7_tf32_kernel");
 }
@@ -694,8 +618,8 @@ int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
       d_filter, c->wt, c->cout_pg, c->tiles_per_group, c->taps, c->Cw_pg, c->V, c->Kv, total, 0);
   if (launch_check("tile_weights_kernel")) return 1;
   // int8 tensor-pipe inner product (lce_b200_imma.cuh) where a plan is eligible: full 64-channel
-  // tiles, float or raw-accumulator output. LCE_B200_BCONV_IMMA=0 keeps every plan on the
-  // XOR + POPC kernel (bench.py reports both).
+  // tiles, float or raw-accumulator output. LCE_B200_BCONV_IMMA=0 leaves every plan to the
+  // wgmma / XOR + POPC kernels (bench.py reports both).
   const char* imma_env = getenv("LCE_B200_BCONV_IMMA");  // read per plan: A/B in one process
   const bool imma_on = !(imma_env && imma_env[0] == '0');
   if (imma_on && c->cout_pg % lce::kBN == 0 &&
@@ -1096,7 +1020,7 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
   const bool zp_float = c.tap_popc != nullptr && plan->zp_mode == LCE_ZERO_PADDING_CORRECTION;
   if (!zp_float) return launch_conv(c, p, s);
   // the optimised kernels' zero padding: one-padding accumulators + a float correction. The
-  // tcgen05 kernel does it in its epilogue; the others run unfused and a tail pass finishes.
+  // wgmma kernel does it in its epilogue; the others run unfused and a tail pass finishes.
   p.zp_float = 1;
   p.cin_pg = d.channels_in / d.groups;
   if (c.tc_ok) {

@@ -1,14 +1,15 @@
 // lce_b200_imma.cuh -- the binary convolution's inner product on the int8 tensor pipe.
-// Used for every plan with full 64-channel tiles and float / raw-accumulator output (the three
-// model families' LceBconv2d layers, the BGEMM sweep); everything else, and every plan when
-// LCE_B200_BCONV_IMMA=0, runs the XOR + POPC kernel of lce_b200_kernels.cuh that north_star
-// describes. Both produce the reference's integers bit for bit (tests/test_gpu_parity.py runs
-// the same cases through both); bench.py reports both.
+// The default for every plan with full 64-channel tiles and float / raw-accumulator output (the
+// three model families' LceBconv2d layers, the BGEMM sweep): on H100 it runs the QuickNet graph
+// faster than the wgmma kernel of lce_b200_tc.cuh, which takes the other plans it is eligible
+// for; the rest, and every plan when LCE_B200_BCONV_IMMA=0 and ..._TC=0, run the XOR + POPC
+// kernel of lce_b200_kernels.cuh. All produce the reference's integers bit for bit
+// (tests/test_gpu_parity.py runs the same cases through each); bench.py reports them side by side.
 //
-// sm_100a has no b1 tensor instruction (ptxas lowers mma.sync ... b1 to masked int8 IMMAs that
-// are no faster than the carry-save tree: profiles/r01_microbench_mma.jsonl), but the legacy
-// int8 tensor pipe (mma.sync.m16n8k32, SASS IMMA.16832) sustains 2048 MAC/clk/SM, twice the
-// ALU/XU ceiling of XOR+POPC. HBM, L2 and shared memory keep the reference's bitpacked words;
+// The int8 tensor pipe (mma.sync.m16n8k32, SASS IMMA.16832) does the XOR + POPC sum as a signed
+// dot product. sm_90a also has a native b1 instruction (mma.sync ... b1 and.popc assembles to
+// BMMA.168256.AND.POPC); a b1 path has not been evaluated on H100. HBM, L2 and shared memory
+// keep the reference's bitpacked words;
 // only registers ever hold bytes. With activation bits a in {0,1} (u8) and weight bits mapped
 // to w' = +1 / -1 (s8):
 //     popc(a ^ w) = popc(w) + sum_k a_k * w'_k

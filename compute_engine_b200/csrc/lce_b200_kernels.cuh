@@ -1,6 +1,6 @@
-// lce_b200_kernels.cuh -- hand-written sm_100a kernels for the LCE binary-conv
-// hot path. No tensor cores by design (BASELINE.json north_star: sm_100a has no
-// b1 MMA); the inner product is XOR + POPC on the integer pipes, operands staged
+// lce_b200_kernels.cuh -- hand-written sm_90a kernels for the LCE binary-conv
+// hot path. No tensor cores: the inner product is XOR + POPC on the integer pipes
+// (the tensor-core inner products are lce_b200_imma.cuh and lce_b200_tc.cuh), operands staged
 // in shared memory as 128-bit vectors, weights brought in by the TMA bulk-copy
 // engine (cp.async.bulk -> UBLKCP) onto an mbarrier, activations gathered with
 // zero-filling cp.async (LDGSTS), and the OutputTransform fused into the epilogue.
@@ -216,7 +216,7 @@ __device__ __forceinline__ int xor_popc8_acc(const uint32_t* a, const uint32_t* 
 }
 
 // OutputTransform<float>::Run, output_transform.h:100-106: shift, int32 clamp,
-// int->float, then an UNFUSED multiply and add (two roundings, SURVEY sec. 5).
+// int->float, then an UNFUSED multiply and add (two roundings).
 __device__ __forceinline__ float transform_float(int acc, int cmin, int cmax, float mul,
                                                  float bias) {
   int x = acc << 1;
@@ -322,8 +322,7 @@ __device__ __forceinline__ void compute_chunk(const typename VecT<V>::T* A_s,
     const Vec* w_ptr = W_s + tn;
     // Main loop: 8 K-words at a time through a carry-save adder tree, so that 8
     // XOR words cost 4 POPCs (XU pipe, 16/clk/SM) + 16 LOP3s (ALU pipe, 64/clk/SM)
-    // instead of 8 POPCs -- the two pipes issue side by side (measured:
-    // profiles/r01_microbench_pipes.jsonl).
+    // instead of 8 POPCs -- the two pipes issue side by side.
     constexpr int G = 8 / V;  // smem vectors per 8-word group
     int kv = 0;
 #ifdef LCE_HALF_TILE
@@ -649,8 +648,7 @@ __device__ __forceinline__ void epilogue_tile(const ConvKParams& p, int (&acc)[k
 }
 
 // ------------------------------------------------------------------------- //
-// One CTA = one 64 x 64 tile, K staged chunk by chunk (any K). (A persistent, double-buffered
-// variant was measured slower on every layer: profiles/r01_persistent_experiment.txt.)
+// One CTA = one 64 x 64 tile, K staged chunk by chunk (any K).
 // ------------------------------------------------------------------------- //
 template <int V, int OUT>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) bconv_kernel(const ConvKParams p) {
@@ -772,7 +770,7 @@ __global__ void tap_popc_kernel(const int32_t* __restrict__ filter, int32_t* __r
 
 // ------------------------------------------------------------------------- //
 // Zero padding with the optimised reference kernels' float correction, for the plans that do not
-// run on the tcgen05 kernel (which has it in its epilogue): the convolution ran with one-padding
+// run on the wgmma kernel (which has it in its epilogue): the convolution ran with one-padding
 // and no fused tail; this pass adds the correction to the edge pixels
 // (zero_padding_correction.h:178-299, the case analysis restated literally), then the fused ADD /
 // activation / sign-pack tail if there is one. One warp per (pixel, 32 channels).

@@ -3,24 +3,18 @@
 // semantics: tensorflow/lite/kernels/internal/reference/conv.h:27; the QuickNet transition and
 // stem pointwise layers and Bi-RealNet's shortcut convolutions).
 //
-// An fp32 FMA GEMM of these shapes is issue-bound at 4-5x its HBM time. tcgen05.mma kind::tf32
-// reads fp32 operands from shared memory and TRUNCATES them to tf32 (measured: tools/tc_probe.cu
-// T7), so the kernel splits every operand once in shared memory,
+// An fp32 FMA GEMM of these shapes is issue-bound well above its HBM time. wgmma .tf32 uses only
+// the tf32 part of its operands, so the kernel splits every operand once,
 //     hi = rna_tf32(x),  lo = rna_tf32(x - hi)                (x - hi is exact in fp32)
-// and accumulates hi*hi + hi*lo + lo*hi in fp32 TMEM: the dropped terms are ~2^-22 |a||w| with
-// random sign, the same order as the rounding of an fp32 FMA chain of this length (probe T7
-// reports the measured error). Three tensor passes still leave the kernel HBM-bound.
+// and accumulates hi*hi + hi*lo + lo*hi in fp32 registers: the dropped terms are ~2^-22 |a||w|
+// with random sign, the same order as the rounding of an fp32 FMA chain of this length.
 //
 // Per CTA (persistent, one per SM), items = (128-row tile, 128-column tile):
-//   warp 20     TMA: A[128 x 32 floats] (+ W[128 x 32]) per K block, SWIZZLE_128B, 3 stages
-//   warps 0-3   row = lane: read the A row, write hi | lo to TENSOR MEMORY (tcgen05.st, 64 columns
-//               per stage) -- the A operand then costs no shared-memory bandwidth in the MMA;
-//               split the W tile hi/lo in place (elementwise, so the swizzle needs no decoding)
-//   warp 21     12 x tcgen05.mma (A from TMEM, W from shared memory; M 128, N 128, K 8) per K
-//               block into one of 2 TMEM accumulators
-//   warps 4-19  four column groups of 32: tcgen05.ld -> + bias, activation (+ LceQuantize bits)
-//               -> swizzled staging -> TMA store (one 32 x 32 box per warp and item)
-// (the single-thread roles sit at the highest warp ids: the warp scheduler favours them)
+//   warp 8      TMA: A[128 x 32 floats] (+ W[128 x 32]) per K block, SWIZZLE_128B, 3 stages
+//   warps 0-7   two math warpgroups, 64 rows each: split the W tile hi | lo in shared memory
+//               (elementwise, so the swizzle needs no decoding), read their A fragments from the
+//               swizzled tile and split them in registers, 12 x wgmma m64n128k8 per K block, then
+//               + bias, activation (+ LceQuantize bits) straight from the accumulators
 // K = 16 (QuickNet's 16 -> 64 pointwise) runs as pixel PAIRS: A'[M/2][32] is the same memory,
 // W' = diag(W, W) is built in shared memory once, out'[M/2][128] is the same memory as out.
 #ifndef LCE_B200_PW_CUH_
@@ -33,15 +27,13 @@ namespace pw {
 
 using namespace lce::tc;
 
-constexpr int kPwThreads = 704;           // 4 split + 16 epilogue + producer + MMA warps
+constexpr int kPwMathThreads = 256;       // two warpgroups
+constexpr int kPwThreads = kPwMathThreads + 32;   // + TMA producer warp
 constexpr int kPwNS = 3;                  // A / W stages
 constexpr int kPwTile = 16384;            // 128 rows x 128 B
 constexpr int kPwWStage = 2 * kPwTile;    // W: hi | lo
-constexpr int kPwNAcc = 2;                // TMEM accumulators of 128 columns (columns 0..255)
-constexpr int kPwACol = 256;              // A stages in TMEM: 64 columns each (hi 32 | lo 32)
-constexpr int kPwEpiBytes = 16 * 4096;    // 16 warps x (32 rows x 128 B)
 constexpr int kPwBarBytes = 1024;
-constexpr size_t kPwSmem = kPwNS * (kPwTile + kPwWStage) + kPwEpiBytes + kPwBarBytes + 1024;
+constexpr size_t kPwSmem = kPwNS * (kPwTile + kPwWStage) + kPwBarBytes + 1024;
 
 struct PwParams {
   long long M;          // rows (pixel pairs in pairs mode)
@@ -53,36 +45,16 @@ struct PwParams {
   int bias_mask;        // column -> bias index (pairs: & 63)
   const float* filter;  // [N][K] (read directly only in pairs mode)
   const float* bias;    // may be null
+  float* out;           // [M][N]
   int32_t* packed;      // optional LceQuantize of the output, [M][N / 32]
-  long long* prof;      // optional [22 warps][8] cycle counters of block 0 (LCE_TC_PROF build)
 };
 
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d, uint32_t a_tmem, uint32_t blo, uint32_t bhi, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\n.reg .b64 bd;\nsetp.ne.b32 p, %5, 0;\nmov.b64 bd, {%2, %3};\n"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], bd, %4, p;\n}\n" ::"r"(d), "r"(a_tmem), "r"(blo), "r"(bhi), "r"(idesc),
-               "r"(acc) : "memory");
-}
-// K-major SWIZZLE_128B operand: 8-row atoms of 1024 B (SBO), version 1, layout type 2
+// K-major SWIZZLE_128B operand: 8-row atoms of 1024 B (SBO), layout type 1 (128-byte swizzle)
 __device__ __forceinline__ uint32_t sdesc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-constexpr uint32_t kSdescHi = (1024u >> 4) | (1u << 14) | (2u << 29);
-// D = f32, A = B = tf32, K-major, N = 128, M = 128
-constexpr uint32_t kIdescTf32 = (1u << 4) | (2u << 7) | (2u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-
-__device__ __forceinline__ void tmem_ld32_async(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+constexpr uint32_t kSdescHi = (1024u >> 4) | (1u << 30);
 
 // round-to-nearest (ties away from zero) to tf32, as cvt.rna.tf32.f32 does -- but on the integer
-// ALU at full rate: the conversion instruction issues at a fraction of it, and 64 of them per
-// thread and K block made the split warps the bottleneck (profiles/r02_pw_roles.txt).
+// ALU at full rate.
 // (No Inf / NaN handling: a value within 2^-11 of FLT_MAX would round to Inf.)
 __device__ __forceinline__ float to_tf32(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
@@ -92,38 +64,69 @@ __device__ __forceinline__ void split4(float4 x, float4* hi, float4* lo) {
   *hi = h;
   *lo = make_float4(to_tf32(x.x - h.x), to_tf32(x.y - h.y), to_tf32(x.z - h.z), to_tf32(x.w - h.w));
 }
-// split one 16 KB tile in place (hi) and into the tile 16 KB above it (lo); 128 threads. All
-// loads first: the in-place stores alias the loads, and the compiler would otherwise serialise
-// load -> convert -> store eight times over.
+// split one 16 KB tile in place (hi) and into the tile 16 KB above it (lo); 256 threads. All
+// loads first: the in-place stores alias the loads.
 __device__ __forceinline__ void split_tile(unsigned char* tile, int t) {
   float4* c = reinterpret_cast<float4*>(tile) + t;
-  float4 x[8];
+  float4 x[4];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) x[j] = c[128 * j];
+  for (int j = 0; j < 4; ++j) x[j] = c[kPwMathThreads * j];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
+  for (int j = 0; j < 4; ++j) {
     float4 h, l;
     split4(x[j], &h, &l);
-    c[128 * j] = h;
-    c[128 * j + kPwTile / 16] = l;
+    c[kPwMathThreads * j] = h;
+    c[kPwMathThreads * j + kPwTile / 16] = l;
   }
+}
+// element (row, k) of a K-major SWIZZLE_128B tile of 32-float rows
+__device__ __forceinline__ float swz_at(const unsigned char* tile, int row, int k) {
+  return *reinterpret_cast<const float*>(tile + row * 128 + ((((k >> 2) ^ (row & 7))) << 4) + (k & 3) * 4);
+}
+
+__device__ __forceinline__ float apply_act(float y, int act) {
+  if (act == LCE_ACT_RELU) return fmaxf(y, 0.f);
+  if (act == LCE_ACT_RELU6) return fminf(fmaxf(y, 0.f), 6.f);
+  if (act == LCE_ACT_RELU_N1_TO_1) return fminf(fmaxf(y, -1.f), 1.f);
+  return y;
+}
+
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t desc, uint32_t scale_d) {
+  if constexpr (N == 128) wgmma_tf32_n128(d, a, desc, scale_d);
+  else wgmma_tf32_n64(d, a, desc, scale_d);
+}
+
+// The three tf32 passes of one 32-float K block: a_hi / a_lo are the warpgroup's A fragments of
+// the four k8 steps, w_lo the descriptor start of the W hi tile (its lo tile follows `lo_ofs`
+// bytes above). The small cross terms first, hi*hi last.
+template <int N>
+__device__ __forceinline__ void tf32_3pass(float (&d)[N / 2], uint32_t (&a_hi)[4][4], uint32_t (&a_lo)[4][4], uint32_t w_lo,
+                                           uint32_t lo_ofs, bool first) {
+#pragma unroll
+  for (int k8 = 0; k8 < 4; ++k8) { fence_regs(a_hi[k8]); fence_regs(a_lo[k8]); }
+  wgmma_fence();
+#pragma unroll
+  for (int pass = 0; pass < 3; ++pass) {
+    const uint32_t w = w_lo + (pass == 1 ? (lo_ofs >> 4) : 0);
+#pragma unroll
+    for (int k8 = 0; k8 < 4; ++k8)
+      wgmma_tf32<N>(d, pass == 0 ? a_lo[k8] : a_hi[k8], make_desc(w + 2 * k8, kSdescHi), (!first || pass != 0 || k8 != 0) ? 1u : 0u);
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+  fence_regs(d);
 }
 
 __global__ void __launch_bounds__(kPwThreads, 1)
-pw_tf32_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
-               const __grid_constant__ CUtensorMap tm_out, const PwParams p) {
+pw_tf32_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, const PwParams p) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   unsigned char* a_st = smem;                               // [kPwNS] raw A tiles
   unsigned char* w_st = a_st + kPwNS * kPwTile;             // [kPwNS][hi | lo]
-  unsigned char* epi = w_st + kPwNS * kPwWStage;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi + kPwEpiBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(w_st + kPwNS * kPwWStage);
   uint64_t* full = bars;                  // TMA landed                          (1 + tx)
-  uint64_t* ready = bars + kPwNS;         // A in TMEM, W hi / lo written        (128)
-  uint64_t* empty = bars + 2 * kPwNS;     // MMAs of the stage retired           (commit)
-  uint64_t* acc_full = bars + 3 * kPwNS;
-  uint64_t* acc_empty = acc_full + kPwNAcc;
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(acc_empty + kPwNAcc);
+  uint64_t* empty = bars + kPwNS;         // MMAs of the stage retired           (8 math warps)
 
   const int tid = threadIdx.x;
   const int wid = __shfl_sync(0xffffffffu, tid >> 5, 0);
@@ -131,26 +134,14 @@ pw_tf32_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
   if (tid == 0) {
     for (int i = 0; i < kPwNS; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&ready[i], 128);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < kPwNAcc; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 16);
+      mbar_init(&empty[i], 8);
     }
     fence_barrier_init();
   }
-  if (wid == 20) tmem_alloc(tmem_base_s, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_s;
   const int items = p.n_tiles * p.m_tiles;
-  const bool prof = LCE_TC_PROF != 0 && p.prof != nullptr && blockIdx.x == 0 && lane == 0;
-  long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  const long long prof_t0 = prof ? clock64() : 0;
 
-  if (wid == 20) {
+  if (wid == 8) {
     // ------------------------------------------------ TMA producer
     uint32_t cnt = 0;
     bool first = true;
@@ -158,7 +149,7 @@ pw_tf32_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
       const int mt = it / p.n_tiles, nt = it - mt * p.n_tiles;
       for (int kb = 0; kb < p.KB; ++kb, ++cnt) {
         const int s = cnt % kPwNS;
-        mbar_wait_prof(&empty[s], ((cnt / kPwNS) & 1) ^ 1, 1, prof, pc[1]);
+        mbar_wait_tc(&empty[s], ((cnt / kPwNS) & 1) ^ 1, 1);
         const bool load_w = !p.pairs && (!p.w_resident || first);
         const int ws = p.w_resident ? kb : s;
         if (elect_one()) {
@@ -170,228 +161,122 @@ pw_tf32_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
       }
       first = false;
     }
-  } else if (wid == 21) {
-    // ------------------------------------------------ MMA issuer
-    uint32_t cnt = 0, use = 0;
-    for (int it = blockIdx.x; it < items; it += gridDim.x, ++use) {
-      const int b = use % kPwNAcc;
-      mbar_wait_prof(&acc_empty[b], ((use / kPwNAcc) & 1) ^ 1, 2, prof, pc[1]);
-      tc_fence_after();
-      const uint32_t d = tmem_base + b * 128;
-      for (int kb = 0; kb < p.KB; ++kb, ++cnt) {
-        const int s = cnt % kPwNS;
-        mbar_wait_prof(&ready[s], (cnt / kPwNS) & 1, 3, prof, pc[2]);
-        tc_fence_after();
-        const int ws = p.w_resident ? kb : s;
-        const uint32_t a_hi = tmem_base + kPwACol + s * 64;
-        const uint32_t w_hi = sdesc_lo(smem_u32(w_st + ws * kPwWStage));
-        if (elect_one()) {
+    return;
+  }
+
+  // ------------------------------------------------ math warpgroups
+  const int g = lane >> 2, t = lane & 3;
+  const int r0 = (wid >> 2) * 64 + (wid & 3) * 16 + g;   // tile rows r0 and r0 + 8
+  const int pw = p.N >> 5;   // packed words per row
+  uint32_t cnt = 0;
+  bool first = true;
+  for (int it = blockIdx.x; it < items; it += gridDim.x, first = false) {
+    const int mt = it / p.n_tiles, nt = it - mt * p.n_tiles;
+    float acc[64];
 #pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            // the small cross terms first, hi*hi last
-            const uint32_t a = a_hi + (pass == 0 ? 32 : 0);
-            const uint32_t w = w_hi + (pass == 1 ? (kPwTile >> 4) : 0);
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < p.KB; ++kb, ++cnt) {
+      const int s = cnt % kPwNS;
+      const int ws = p.w_resident ? kb : s;
+      if (p.pairs && first && tid < 128) {
+        // W' = diag(W, W): row n' = tid, 32 floats (8 cells of 16 B, swizzled by row & 7)
+        unsigned char* row = w_st + ws * kPwWStage + tid * 128;
+        const float* src = p.filter + (tid & 63) * 16;
 #pragma unroll
-            for (int k8 = 0; k8 < 4; ++k8) mma_tf32_ts(d, a + 8 * k8, w + 2 * k8, kSdescHi, kIdescTf32, (kb | pass | k8) != 0);
-          }
-          tc_commit(&empty[s]);
-          if (kb == p.KB - 1) tc_commit(&acc_full[b]);
+        for (int c = 0; c < 8; ++c) {
+          float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+          if ((c >> 2) == (tid >> 6)) x = __ldg(reinterpret_cast<const float4*>(src) + (c & 3));
+          float4 h, l;
+          split4(x, &h, &l);
+          float4* cell = reinterpret_cast<float4*>(row + ((c ^ (tid & 7)) << 4));
+          *cell = h;
+          *(cell + kPwTile / 16) = l;
         }
-        __syncwarp();
       }
-    }
-  } else if (wid < 4) {
-    // ------------------------------------------------ A -> TMEM hi | lo (row = lane), W split in place
-    uint32_t cnt = 0;
-    bool first = true;
-    const uint32_t a_t0 = tmem_base + (static_cast<uint32_t>(wid * 32) << 16) + kPwACol;
-    for (int it = blockIdx.x; it < items; it += gridDim.x) {
-      for (int kb = 0; kb < p.KB; ++kb, ++cnt) {
-        const int s = cnt % kPwNS;
-        const int ws = p.w_resident ? kb : s;
-        if (p.pairs && first) {
-          // W' = diag(W, W): row n' = tid, 32 floats (8 cells of 16 B, swizzled by row & 7)
-          unsigned char* row = w_st + ws * kPwWStage + tid * 128;
-          const float* src = p.filter + (tid & 63) * 16;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if ((c >> 2) == (tid >> 6)) x = __ldg(reinterpret_cast<const float4*>(src) + (c & 3));
-            float4 h, l;
-            split4(x, &h, &l);
-            float4* cell = reinterpret_cast<float4*>(row + ((c ^ (tid & 7)) << 4));
-            *cell = h;
-            *(cell + kPwTile / 16) = l;
-          }
-        }
-        // (the stage's TMEM columns are free: the producer issued this load only after the MMAs
-        // that last read them had retired)
-        mbar_wait_prof(&full[s], (cnt / kPwNS) & 1, 4, prof, pc[1]);
-        tc_fence_after();
-        const long long ts0 = prof ? clock64() : 0;
-        {
-          const unsigned char* row = a_st + s * kPwTile + tid * 128;
-          uint32_t h[32], l[32];
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const float4 x = *reinterpret_cast<const float4*>(row + ((k ^ (tid & 7)) << 4));
-            float4 hh, ll;
-            split4(x, &hh, &ll);
-            h[4 * k] = __float_as_uint(hh.x); h[4 * k + 1] = __float_as_uint(hh.y);
-            h[4 * k + 2] = __float_as_uint(hh.z); h[4 * k + 3] = __float_as_uint(hh.w);
-            l[4 * k] = __float_as_uint(ll.x); l[4 * k + 1] = __float_as_uint(ll.y);
-            l[4 * k + 2] = __float_as_uint(ll.z); l[4 * k + 3] = __float_as_uint(ll.w);
-          }
-          tmem_st32(a_t0 + s * 64, h);
-          tmem_st32(a_t0 + s * 64 + 32, l);
-        }
-        const long long ts1 = prof ? clock64() : 0;
-        if (!p.pairs && (!p.w_resident || first)) split_tile(w_st + ws * kPwWStage, tid);
-        const long long ts2 = prof ? clock64() : 0;
-        tmem_st_wait();
-        tc_fence_before();
+      mbar_wait_tc(&full[s], (cnt / kPwNS) & 1, 4);
+      const bool split_w = !p.pairs && (!p.w_resident || first);
+      if (split_w) split_tile(w_st + ws * kPwWStage, tid);
+      if (split_w || (p.pairs && first)) {
+        // both warpgroups read the whole W tile: all of it must be split (and visible to the
+        // tensor cores' async proxy) first
         fence_proxy_async();
-        mbar_arrive(&ready[s]);
-        if (prof) { pc[2] += ts1 - ts0; pc[3] += ts2 - ts1; pc[4] += clock64() - ts2; pc[5] += 1; }
+        named_bar_sync(1, kPwMathThreads);
       }
-      first = false;
-    }
-  } else {
-    // ------------------------------------------------ epilogue: warp -> TMEM lane quarter q, 32-column group g
-    const int q = wid & 3, g = (wid - 4) >> 2;
-    unsigned char* buf = epi + (wid - 4) * 4096;
-    const int pw = p.N >> 5;   // packed words per row
-    uint32_t use = 0;
-    for (int it = blockIdx.x; it < items; it += gridDim.x, ++use) {
-      const int mt = it / p.n_tiles, nt = it - mt * p.n_tiles;
-      const int b = use % kPwNAcc;
-      const long long row = static_cast<long long>(mt) * 128 + q * 32 + lane;
-      mbar_wait_prof(&acc_full[b], (use / kPwNAcc) & 1, 5, prof, pc[1]);
-      tc_fence_after();
-      const long long te0 = prof ? clock64() : 0;
-      uint32_t v[32];
-      tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + b * 128 + g * 32, v);
-      // the accumulator is in registers: hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[b]);
-      const int n0 = nt * 128 + g * 32;
-      uint32_t bits = 0;
+      const unsigned char* at = a_st + s * kPwTile;
+      uint32_t a_hi[4][4], a_lo[4][4];
 #pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        float4 bi = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias && n0 + 4 * k < p.N) bi = __ldg(reinterpret_cast<const float4*>(p.bias + ((n0 + 4 * k) & p.bias_mask)));
-        float y0 = __fadd_rn(__uint_as_float(v[4 * k]), bi.x), y1 = __fadd_rn(__uint_as_float(v[4 * k + 1]), bi.y);
-        float y2 = __fadd_rn(__uint_as_float(v[4 * k + 2]), bi.z), y3 = __fadd_rn(__uint_as_float(v[4 * k + 3]), bi.w);
-        if (p.act == LCE_ACT_RELU) {
-          y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); y2 = fmaxf(y2, 0.f); y3 = fmaxf(y3, 0.f);
-        } else if (p.act == LCE_ACT_RELU6) {
-          y0 = fminf(fmaxf(y0, 0.f), 6.f); y1 = fminf(fmaxf(y1, 0.f), 6.f);
-          y2 = fminf(fmaxf(y2, 0.f), 6.f); y3 = fminf(fmaxf(y3, 0.f), 6.f);
-        } else if (p.act == LCE_ACT_RELU_N1_TO_1) {
-          y0 = fminf(fmaxf(y0, -1.f), 1.f); y1 = fminf(fmaxf(y1, -1.f), 1.f);
-          y2 = fminf(fmaxf(y2, -1.f), 1.f); y3 = fminf(fmaxf(y3, -1.f), 1.f);
+      for (int k8 = 0; k8 < 4; ++k8)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          // fragment register r: row r0 + 8 * (r & 1), column 8 * k8 + t + 4 * (r >> 1)
+          const float x = swz_at(at, r0 + 8 * (r & 1), 8 * k8 + t + 4 * (r >> 1));
+          const float h = to_tf32(x);
+          a_hi[k8][r] = __float_as_uint(h);
+          a_lo[k8][r] = __float_as_uint(to_tf32(x - h));
         }
-        v[4 * k] = __float_as_uint(y0); v[4 * k + 1] = __float_as_uint(y1);
-        v[4 * k + 2] = __float_as_uint(y2); v[4 * k + 3] = __float_as_uint(y3);
-        bits |= ((y0 < 0.0f ? 1u : 0u) | (y1 < 0.0f ? 2u : 0u) | (y2 < 0.0f ? 4u : 0u) | (y3 < 0.0f ? 8u : 0u)) << (4 * k);
-      }
-      const long long te1 = prof ? clock64() : 0;
-      if (lane == 0) tma_store_wait_read();   // the previous item's store has read this buffer
+      tf32_3pass<128>(acc, a_hi, a_lo, sdesc_lo(smem_u32(w_st + ws * kPwWStage)), kPwTile, kb == 0);
       __syncwarp();
-      const long long te2 = prof ? clock64() : 0;
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        *reinterpret_cast<uint4*>(buf + lane * 128 + ((k ^ (lane & 7)) << 4)) =
-            make_uint4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) tma_store_2d(&tm_out, buf, n0, mt * 128 + q * 32);
-      if (p.packed != nullptr && row < p.M) p.packed[row * pw + nt * 4 + g] = static_cast<int32_t>(bits);
-      if (prof) { pc[2] += te1 - te0; pc[3] += te2 - te1; pc[4] += clock64() - te2; pc[5] += 1; }
+      if (lane == 0) mbar_arrive(&empty[s]);
     }
-    if (lane == 0) tma_store_wait_all();
+    // epilogue: register i of block j is row r0 + 8 * ((i >> 1) & 1), column 8j + 2t + (i & 1)
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long row = static_cast<long long>(mt) * 128 + r0 + 8 * rr;
+      const bool row_ok = row < p.M;
+#pragma unroll
+      for (int gq = 0; gq < 4; ++gq) {
+        uint32_t bits = 0;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = 4 * gq + jj;
+          const int n = nt * 128 + 8 * j + 2 * t;
+          float y[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float bi = (p.bias != nullptr && n + e < p.N) ? __ldg(p.bias + ((n + e) & p.bias_mask)) : 0.f;
+            y[e] = apply_act(__fadd_rn(acc[4 * j + 2 * rr + e], bi), p.act);
+          }
+          bits |= ((y[0] < 0.0f ? 1u : 0u) | (y[1] < 0.0f ? 2u : 0u)) << (8 * jj + 2 * t);
+          if (row_ok && n < p.N) *reinterpret_cast<float2*>(p.out + row * p.N + n) = make_float2(y[0], y[1]);
+        }
+        if (p.packed != nullptr) {
+          bits = quad_or(bits);
+          if (t == 0 && row_ok) p.packed[row * pw + nt * 4 + gq] = static_cast<int32_t>(bits);
+        }
+      }
+    }
   }
-  if (prof) {
-    pc[0] = clock64() - prof_t0;
-    for (int i = 0; i < 8; ++i) p.prof[wid * 8 + i] = pc[i];
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (wid == 20) tmem_dealloc(tmem_base, 512);
 }
 
 
-// ------------------------------------------------------------------ 7x7 / stride 2 stem on kind::tf32
+// ------------------------------------------------------------------ 7x7 / stride 2 stem on wgmma .tf32
 // Bi-RealNet's first layer, CONV_2D 7x7 stride 2, 3 -> 64 channels: K = 147 (five 32-float K
-// blocks, zero-padded), N = 64. As an FMA implicit GEMM it took 3.3 ms at batch 512, more than
-// all the binary layers together. Same 3-pass split as above; what differs is the A operand: no
-// im2col tensor exists, so no TMA -- thread = output pixel = TMEM lane gathers its own 147 input
-// values (21 contiguous floats per filter row; neighbours share them through L1), splits them and
-// writes hi | lo straight to TMEM. The filter (37 KB) is split into shared memory once per CTA.
-//   warps 0-7   gather + split: two warps per TMEM lane quarter take alternate K blocks
-//   warps 8-15  epilogue: (lane quarter, 32-column half)
-//   warp 16     MMA issuer (+ TMEM allocation)
-constexpr int kS7Threads = 544;
+// blocks, zero-padded), N = 64. Same 3-pass split as above; what differs is the A operand: no
+// im2col tensor exists, so no TMA -- each thread gathers the input values of its A fragment (21
+// contiguous floats per filter row; neighbours share them through L1) and splits them in
+// registers. The filter (37 KB) is split into shared memory once per CTA. Each of the two
+// warpgroups of a CTA takes 64-pixel tiles on its own.
+constexpr int kS7Threads = 256;
 constexpr int kS7K = 147, kS7KB = 5, kS7N = 64;
 constexpr int kS7WTile = 64 * 128;                 // 64 rows x 32 floats
-constexpr int kS7NS = 3, kS7NAcc = 4;
-constexpr size_t kS7Smem = kS7KB * 2 * kS7WTile + 8 * 4096 + 1024 + 1024;
+constexpr size_t kS7Smem = kS7KB * 2 * kS7WTile + 1024;
 struct Stem7Params {
   long long M;           // output pixels
   int H, W, OH, OW, ph, pw;
-  int m_tiles, act;
+  int m_tiles, act;      // m_tiles: 64-pixel tiles
   const float* in;       // [B][H][W][3]
   const float* filter;   // [64][7][7][3]
   const float* bias;
+  float* out;            // [M][64]
 };
-constexpr uint32_t kIdescTf32N64 = (1u << 4) | (2u << 7) | (2u << 10) | ((64u >> 3) << 17) | ((128u >> 4) << 24);
 
-template <int KBI>
-__device__ __forceinline__ void stem7_gather(const float* base, int row_pitch, uint32_t rowmask, int e_lo, int e_hi,
-                                             uint32_t (&h)[32], uint32_t (&l)[32]) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    const int k = KBI * 32 + j;
-    float x = 0.0f;
-    if (k < kS7K) {
-      const int fy = k / 21, e = k - fy * 21;     // compile-time after unrolling
-      if (((rowmask >> fy) & 1u) && e >= e_lo && e < e_hi) x = __ldg(base + fy * row_pitch + e);
-    }
-    const float hi = to_tf32(x);
-    h[j] = __float_as_uint(hi);
-    l[j] = __float_as_uint(to_tf32(x - hi));
-  }
-}
-
-__global__ void __launch_bounds__(kS7Threads, 1)
-stem7_tf32_kernel(const __grid_constant__ CUtensorMap tm_out, const Stem7Params p) {
+__global__ void __launch_bounds__(kS7Threads, 2)
+stem7_tf32_kernel(const Stem7Params p) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  unsigned char* w_st = smem;                               // [kS7KB][hi | lo][64 x 128 B]
-  unsigned char* epi = w_st + kS7KB * 2 * kS7WTile;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi + 8 * 4096);
-  uint64_t* ready = bars;                 // A stage written to TMEM   (128)
-  uint64_t* empty = bars + kS7NS;         // MMAs of the stage retired (commit)
-  uint64_t* acc_full = bars + 2 * kS7NS;
-  uint64_t* acc_empty = acc_full + kS7NAcc;
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(acc_empty + kS7NAcc);
-
+  unsigned char* w_st = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int tid = threadIdx.x;
   const int wid = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const int lane = tid & 31;
-  if (tid == 0) {
-    for (int i = 0; i < kS7NS; ++i) {
-      mbar_init(&ready[i], 128);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < kS7NAcc; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 8);
-    }
-    fence_barrier_init();
-  }
-  if (wid == 16) tmem_alloc(tmem_base_s, 512);
   // the filter, split hi | lo, in the K-major SWIZZLE_128B image the MMA reads (K padded with zeros)
   for (int i = tid; i < kS7KB * 64 * 8; i += kS7Threads) {
     const int c = i & 7, row = (i >> 3) & 63, kb = i >> 9;
@@ -409,127 +294,70 @@ stem7_tf32_kernel(const __grid_constant__ CUtensorMap tm_out, const Stem7Params 
     *(cell + kS7WTile / 16) = ll;
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_s;
-  constexpr uint32_t kACol = kS7NAcc * kS7N;   // A stages behind the accumulators
 
-  if (wid == 16) {
-    // ------------------------------------------------ MMA issuer
-    uint32_t cnt = 0, use = 0;
-    for (int it = blockIdx.x; it < p.m_tiles; it += gridDim.x, ++use) {
-      const int b = use % kS7NAcc;
-      mbar_wait_tc(&acc_empty[b], ((use / kS7NAcc) & 1) ^ 1, 2);
-      tc_fence_after();
-      const uint32_t d = tmem_base + b * kS7N;
-      for (int kb = 0; kb < kS7KB; ++kb, ++cnt) {
-        const int s = cnt % kS7NS;
-        mbar_wait_tc(&ready[s], (cnt / kS7NS) & 1, 3);
-        tc_fence_after();
-        const uint32_t a_hi = tmem_base + kACol + s * 64;
-        const uint32_t w_hi = sdesc_lo(smem_u32(w_st + kb * 2 * kS7WTile));
-        if (elect_one()) {
+  const int g = lane >> 2, t = lane & 3;
+  const int r0 = (wid & 3) * 16 + g;   // rows r0 and r0 + 8 of a 64-pixel tile
+  const int row_pitch = p.W * 3;
+  const long long ohw = static_cast<long long>(p.OH) * p.OW;
+  for (int it = blockIdx.x * 2 + (wid >> 2); it < p.m_tiles; it += gridDim.x * 2) {
+    const float* base[2];
+    uint32_t rowmask[2];
+    int e_lo[2], e_hi[2];
 #pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t a = a_hi + (pass == 0 ? 32 : 0);
-            const uint32_t w = w_hi + (pass == 1 ? (kS7WTile >> 4) : 0);
-#pragma unroll
-            for (int k8 = 0; k8 < 4; ++k8) mma_tf32_ts(d, a + 8 * k8, w + 2 * k8, kSdescHi, kIdescTf32N64, (kb | pass | k8) != 0);
-          }
-          tc_commit(&empty[s]);
-          if (kb == kS7KB - 1) tc_commit(&acc_full[b]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (wid < 8) {
-    // ------------------------------------------------ gather + split: warp (quarter, parity) takes every other K block
-    const int quarter = wid & 3, parity = wid >> 2;
-    const uint32_t a_t0 = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + kACol;
-    const int row_pitch = p.W * 3;
-    const long long ohw = static_cast<long long>(p.OH) * p.OW;
-    uint32_t cnt = 0;
-    for (int it = blockIdx.x; it < p.m_tiles; it += gridDim.x) {
-      const long long m = static_cast<long long>(it) * 128 + quarter * 32 + lane;
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long m = static_cast<long long>(it) * 64 + r0 + 8 * rr;
       const long long mm = m < p.M ? m : p.M - 1;          // rows past the end gather a valid pixel; never stored
       const int bi = static_cast<int>(mm / ohw);
       const int rem = static_cast<int>(mm - bi * ohw);
       const int oy = rem / p.OW, ox = rem - oy * p.OW;
       const int iy0 = oy * 2 - p.ph, ix0 = ox * 2 - p.pw;
-      uint32_t rowmask = 0;
+      rowmask[rr] = 0;
 #pragma unroll
       for (int fy = 0; fy < 7; ++fy)
-        if (static_cast<unsigned>(iy0 + fy) < static_cast<unsigned>(p.H)) rowmask |= 1u << fy;
-      const int e_lo = 3 * max(0, -ix0), e_hi = 3 * min(7, p.W - ix0);
-      const float* base = p.in + ((static_cast<long long>(bi) * p.H + iy0) * p.W + ix0) * 3;
-      for (int kb = 0; kb < kS7KB; ++kb, ++cnt) {
-        if ((cnt & 1u) != static_cast<uint32_t>(parity)) continue;
-        const int s = cnt % kS7NS;
-        uint32_t h[32], l[32];
-        switch (kb) {
-          case 0: stem7_gather<0>(base, row_pitch, rowmask, e_lo, e_hi, h, l); break;
-          case 1: stem7_gather<1>(base, row_pitch, rowmask, e_lo, e_hi, h, l); break;
-          case 2: stem7_gather<2>(base, row_pitch, rowmask, e_lo, e_hi, h, l); break;
-          case 3: stem7_gather<3>(base, row_pitch, rowmask, e_lo, e_hi, h, l); break;
-          default: stem7_gather<4>(base, row_pitch, rowmask, e_lo, e_hi, h, l); break;
+        if (static_cast<unsigned>(iy0 + fy) < static_cast<unsigned>(p.H)) rowmask[rr] |= 1u << fy;
+      e_lo[rr] = 3 * max(0, -ix0);
+      e_hi[rr] = 3 * min(7, p.W - ix0);
+      base[rr] = p.in + ((static_cast<long long>(bi) * p.H + iy0) * p.W + ix0) * 3;
+    }
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+#pragma unroll 1
+    for (int kb = 0; kb < kS7KB; ++kb) {
+      uint32_t a_hi[4][4], a_lo[4][4];
+#pragma unroll
+      for (int k8 = 0; k8 < 4; ++k8)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int rr = r & 1;
+          const int k = kb * 32 + 8 * k8 + t + 4 * (r >> 1);
+          const int fy = k / 21, e = k - fy * 21;
+          float x = 0.0f;
+          if (k < kS7K && ((rowmask[rr] >> fy) & 1u) && e >= e_lo[rr] && e < e_hi[rr]) x = __ldg(base[rr] + fy * row_pitch + e);
+          const float h = to_tf32(x);
+          a_hi[k8][r] = __float_as_uint(h);
+          a_lo[k8][r] = __float_as_uint(to_tf32(x - h));
         }
-        mbar_wait_tc(&empty[s], ((cnt / kS7NS) & 1) ^ 1, 6);   // the MMAs that last read this TMEM stage retired
-        tc_fence_after();
-        tmem_st32(a_t0 + s * 64, h);
-        tmem_st32(a_t0 + s * 64 + 32, l);
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(&ready[s]);
+      tf32_3pass<kS7N>(acc, a_hi, a_lo, sdesc_lo(smem_u32(w_st + kb * 2 * kS7WTile)), kS7WTile, kb == 0);
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long m = static_cast<long long>(it) * 64 + r0 + 8 * rr;
+      if (m >= p.M) continue;
+#pragma unroll
+      for (int j = 0; j < kS7N / 8; ++j) {
+        const int n = 8 * j + 2 * t;
+        float y[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float bi = p.bias ? __ldg(p.bias + n + e) : 0.f;
+          y[e] = apply_act(__fadd_rn(acc[4 * j + 2 * rr + e], bi), p.act);
+        }
+        *reinterpret_cast<float2*>(p.out + m * kS7N + n) = make_float2(y[0], y[1]);
       }
     }
-  } else {
-    // ------------------------------------------------ epilogue: warp -> (TMEM lane quarter q, 32-column half g)
-    const int q = wid & 3, g = (wid - 8) >> 2;
-    unsigned char* buf = epi + (wid - 8) * 4096;
-    uint32_t use = 0;
-    for (int it = blockIdx.x; it < p.m_tiles; it += gridDim.x, ++use) {
-      const int b = use % kS7NAcc;
-      mbar_wait_tc(&acc_full[b], (use / kS7NAcc) & 1, 5);
-      tc_fence_after();
-      uint32_t v[32];
-      tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + b * kS7N + g * 32, v);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[b]);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        float4 bi = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias) bi = __ldg(reinterpret_cast<const float4*>(p.bias + g * 32 + 4 * k));
-        float y0 = __fadd_rn(__uint_as_float(v[4 * k]), bi.x), y1 = __fadd_rn(__uint_as_float(v[4 * k + 1]), bi.y);
-        float y2 = __fadd_rn(__uint_as_float(v[4 * k + 2]), bi.z), y3 = __fadd_rn(__uint_as_float(v[4 * k + 3]), bi.w);
-        if (p.act == LCE_ACT_RELU) {
-          y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); y2 = fmaxf(y2, 0.f); y3 = fmaxf(y3, 0.f);
-        } else if (p.act == LCE_ACT_RELU6) {
-          y0 = fminf(fmaxf(y0, 0.f), 6.f); y1 = fminf(fmaxf(y1, 0.f), 6.f);
-          y2 = fminf(fmaxf(y2, 0.f), 6.f); y3 = fminf(fmaxf(y3, 0.f), 6.f);
-        } else if (p.act == LCE_ACT_RELU_N1_TO_1) {
-          y0 = fminf(fmaxf(y0, -1.f), 1.f); y1 = fminf(fmaxf(y1, -1.f), 1.f);
-          y2 = fminf(fmaxf(y2, -1.f), 1.f); y3 = fminf(fmaxf(y3, -1.f), 1.f);
-        }
-        v[4 * k] = __float_as_uint(y0); v[4 * k + 1] = __float_as_uint(y1);
-        v[4 * k + 2] = __float_as_uint(y2); v[4 * k + 3] = __float_as_uint(y3);
-      }
-      if (lane == 0) tma_store_wait_read();   // the previous item's store has read this buffer
-      __syncwarp();
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        *reinterpret_cast<uint4*>(buf + lane * 128 + ((k ^ (lane & 7)) << 4)) =
-            make_uint4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) tma_store_2d(&tm_out, buf, g * 32, it * 128 + q * 32);
-    }
-    if (lane == 0) tma_store_wait_all();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (wid == 16) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace pw

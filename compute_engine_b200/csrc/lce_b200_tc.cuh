@@ -1,37 +1,29 @@
-// lce_b200_tc.cuh -- the binary convolution / BGEMM on the 5th-generation tensor cores.
+// lce_b200_tc.cuh -- the binary convolution / BGEMM on the Hopper tensor cores (wgmma).
 //
 //   acc[m][n] = sum_k popc(a[m][k] ^ w[n][k]) = popc(w[n]) + sum_k a_k * w'_k
 //   a_k in {0,1},  w'_k = +1 if w_k = 0 else -1            (same identity as lce_b200_imma.cuh)
 //
 // so the reference's integers (LCE/core/bconv2d/reference.h:35-148, bgemm/kernels.h:22-134) come
-// out of one int8 contraction, issued here as tcgen05.mma kind::i8 (SASS UTCIMMA) with the
-// accumulators in TMEM. HBM, L2 and the TMA-staged activation tiles keep the reference's BITPACKED
-// words (types.h:41-47); bytes exist only in TMEM (activations) and in a plan-time expansion of
-// the static weights.
+// out of one int8 contraction, issued here as wgmma.mma_async .s32.s8.s8 (m64 x BN x k32). HBM, L2
+// and the TMA-staged activation tiles keep the reference's BITPACKED words (types.h:41-47); bytes
+// exist only in registers (activations) and in a plan-time expansion of the static weights.
 //
-// One persistent CTA per SM, 20 warps, warp-specialised:
-//   w16       activation producer  TMA (cp.async.bulk.tensor, SASS UTMALDG) of the packed HALO
-//                                  of a 128-pixel tile: the contiguous pixel range its taps touch,
-//                                  once per tile -- no im2col replication anywhere
-//   w19       MMA issuer           the warp runs converged so every descriptor lives in uniform
-//                                  registers; one elected lane issues tcgen05.mma.cta_group::1
-//                                  .kind::i8, A from TMEM, B from shared memory, D (128 x BN int32)
-//                                  in TMEM, two D buffers
-//   w18       weight producer      cp.async.bulk of pre-expanded int8 stages (resident in shared
+// Persistent CTAs (two per SM where shared memory allows), 10 warps, warp-specialised:
+//   w8        activation producer  TMA (cp.async.bulk.tensor) of the packed HALO of a 128-pixel
+//                                  tile: the contiguous pixel range its taps touch, once per tile --
+//                                  no im2col replication anywhere
+//   w9        weight producer      cp.async.bulk of pre-expanded int8 stages (resident in shared
 //                                  memory for the whole kernel when they fit, else a ring)
-//   w17       shortcut producer    TMA tiles of the residual (fused ADD), SWIZZLE_128B
-//   w0..w7    expanders            thread = output pixel = TMEM lane: reads its taps' words from
-//                                  the halo (out-of-bounds taps read as 0 = "+1" padding,
-//                                  reference.h:106), expands bits -> bytes (9 ALU ops per word:
-//                                  bit 8i+s of a word becomes byte i of column s with VALUE
-//                                  2^(s&3); the weight byte there is +-(8 >> (s&3)), so every
-//                                  product is +-8 and D holds 8 * sum a*w') and writes them with
-//                                  tcgen05.st; two warps per TMEM lane quadrant take alternate stages
-//   w8..w15   epilogue             tcgen05.ld -> OutputTransform (output_transform.h:94-168,
-//                                  unfused fmul + fadd) [+ shortcut, activation, next layer's sign
-//                                  bits] -> swizzled shared memory -> TMA store (UTMASTG); two warps
-//                                  per TMEM lane quadrant take alternate 32-channel chunks
-// Stage = 8 K-words = 256 bits of K = eight K=32 MMAs; 4 A stages live in TMEM columns 256..511.
+//   w0..w7    two math warpgroups  warpgroup g owns pixels 64g..64g+63 of the tile. Each thread
+//                                  reads its two pixels' words from the halo (out-of-bounds taps
+//                                  read as 0 = "+1" padding, reference.h:106) and expands them
+//                                  straight into its wgmma A fragment: bit 8i+s of a word becomes
+//                                  byte i of K column group s with VALUE 2^(s&3); the weight byte
+//                                  there is +-(8 >> (s&3)), so every product is +-8 and D holds
+//                                  8 * sum a*w'. The accumulators stay in registers through the
+//                                  epilogue: OutputTransform (output_transform.h:94-168, unfused
+//                                  fmul + fadd) [+ shortcut, activation, next layer's sign bits].
+// Stage = 8 K-words = 256 bits of K = eight k32 MMAs.
 #ifndef LCE_B200_TC_CUH_
 #define LCE_B200_TC_CUH_
 
@@ -42,28 +34,14 @@
 namespace lce {
 namespace tc {
 
-#ifndef LCE_TC_PROF
-#define LCE_TC_PROF 0   // 1: per-role cycle counters (build with -DLCE_TC_PROF=1, run with LCE_B200_TC_PROF=1)
-#endif
 constexpr int kBM = 128;
-#ifndef LCE_TC_EXP_GROUPS
-#define LCE_TC_EXP_GROUPS 2   // expander warps per TMEM lane quarter (they take the A stages in turn)
-#endif
-constexpr int kExpGroups = LCE_TC_EXP_GROUPS;
-constexpr int kThreads = (4 * kExpGroups + 8 + 4) * 32;
+constexpr int kNumMathWarps = 8;  // two warpgroups of four
+constexpr int kWarpActProd = kNumMathWarps, kWarpWeightProd = kNumMathWarps + 1;
+constexpr int kThreads = (kNumMathWarps + 2) * 32;
 constexpr int kWS = 8;            // K words per stage
-constexpr int kNA = 4;            // A stages in TMEM, 64 columns each
 constexpr int kNR = 2;            // activation-halo stages
 constexpr int kMaxNB = 32;        // weight stages in shared memory (barrier array size)
-constexpr int kMaxNS = 8;         // epilogue staging slots (16 KB each)
-constexpr int kSlotBytes = kBM * 128;  // 128 rows x 32 columns x 4 B
-// Warp ids. The SM's schedulers favour the HIGHER warp id among eligible warps (measured: a
-// single-lane role at warp id 1 starved behind the busy expander / epilogue warps of its scheduler
-// and the tensor pipe idled half the time), so the latency-critical single-lane roles sit on top.
-constexpr int kFirstExpWarp = 0, kNumExpWarps = 4 * kExpGroups, kFirstEpiWarp = kNumExpWarps, kNumEpiWarps = 8;
-constexpr int kWarpActProd = kFirstEpiWarp + 8, kWarpResProd = kWarpActProd + 1, kWarpWeightProd = kWarpActProd + 2,
-              kWarpMma = kWarpActProd + 3;
-constexpr int kTabBytes = 4 * 128 * 4 * 2;   // {mul, bias, wpop2, thr} x 128 channels, double-buffered
+constexpr int kMaxRing = 4;       // weight ring slots when the weights do not stay resident
 constexpr int kBarBytes = 1024;
 
 struct TcParams {
@@ -77,9 +55,9 @@ struct TcParams {
   int mode_flat;         // 1: 1-D word map, boxes of 256 words; 0: 2-D [pixel][word] map, boxes of CcB x 128
   int cout, BN, n_tiles, m_tiles;
   int S_full, S_last, S_t;   // weight stages per full / last chunk, per tile
-  int nB, b_resident, nS;
+  int nB, b_resident;    // ring: nB slots of kWS words
   int raw_stage_bytes;
-  int off_raw, off_slots, off_tab, off_bar;   // byte offsets in dynamic shared memory (weights at 0)
+  int off_raw, off_bar;  // byte offsets in dynamic shared memory (weights at 0)
   int Kw_total;          // taps * Cw: K words per output channel
   int clamp_min, clamp_max;
   int has_res, residual_act, cw_out, zp_half, ldc;   // ldc: padded channel count of the tables
@@ -91,10 +69,10 @@ struct TcParams {
   const int32_t* thr;
   const int32_t* tap_popc_t;  // [taps][ldc] or nullptr (zero-padding correction)
   const float* zpc_cache;     // [4][eff_h][eff_w][ldc]: the optimised kernels' float corrections (zp_float)
+  const float* residual;      // [M][cout] shortcut of a fused ADD (has_res)
   void* out;
   int32_t* packed_out;
-  long long* prof;         // optional [16 warps][8] cycle counters of block 0 (LCE_B200_TC_PROF=1)
-  FastDiv fd_ohw, fd_ow, fd_kw, fd_cwv_full, fd_cwv_last, fd_mt;
+  FastDiv fd_ohw, fd_ow, fd_kw, fd_mt;
 };
 
 // ------------------------------------------------------------------ PTX
@@ -135,67 +113,11 @@ __device__ __forceinline__ void mbar_wait_tc(uint64_t* bar, uint32_t parity, int
     }
   }
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem descriptor], int8 x int8 -> int32, M = 128
-__device__ __forceinline__ void mma_i8_ts(uint32_t d, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-               "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-// Shared-memory descriptor of the B operand, K-major, no swizzle: 8 x 16 B core matrices, K-adjacent
-// ones 128 B apart (LBO), 8-row groups `sbo` bytes apart; version 1 (Blackwell). Passed as two
-// 32-bit halves so the issuing warp only does 32-bit uniform arithmetic per MMA. Layout verified
-// on hardware by tools/tc_probe.cu.
-__device__ __forceinline__ uint32_t bdesc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | ((128u >> 4) << 16); }
-__device__ __forceinline__ uint32_t bdesc_hi(uint32_t sbo) { return (sbo >> 4) | (1u << 14); }
-__device__ __forceinline__ void mma_i8_ts2(uint32_t d, uint32_t a_tmem, uint32_t blo, uint32_t bhi, uint32_t idesc,
-                                           uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\n.reg .b64 bd;\nsetp.ne.b32 p, %5, 0;\nmov.b64 bd, {%2, %3};\n"
-               "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], bd, %4, p;\n}\n" ::"r"(d), "r"(a_tmem), "r"(blo), "r"(bhi),
-               "r"(idesc), "r"(acc) : "memory");
-}
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n.reg .pred P;\nelect.sync _|P, 0xffffffff;\nselp.u32 %0, 1, 0, P;\n}\n" : "=r"(pred));
   return pred != 0;
 }
-// kind::i8 instruction descriptor: D = s32, A = B = s8, both K-major, M = 128
-__host__ __device__ inline uint32_t make_idesc(int N) {
-  return (2u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(kBM >> 4) << 24);
-}
-#define LCE_R8(a, o) "%" #a "+" #o
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void tma_load_1d(void* dst, const CUtensorMap* tm, uint64_t* bar, int c0) {
   asm volatile("cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3}], [%2];" ::"r"(smem_u32(dst)),
                "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0) : "memory");
@@ -204,28 +126,36 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tm, ui
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
                "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tm)),
-               "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// profiling aid: wait and add the cycles spent to `acc` when `on`
-__device__ __forceinline__ void mbar_wait_prof(uint64_t* bar, uint32_t parity, int tag, bool on, long long& acc) {
-  if (!on) {
-    mbar_wait_tc(bar, parity, tag);
-    return;
-  }
-  const long long t = clock64();
-  mbar_wait_tc(bar, parity, tag);
-  acc += clock64() - t;
+// wgmma: issued by all 128 threads of a warpgroup. A comes from registers, B from a shared-memory
+// descriptor, D stays in registers. The fence orders this thread's register writes (A fragments,
+// accumulators read by the previous epilogue) before the asynchronous reads; the empty asm
+// statements keep the compiler from moving register accesses across the commit / wait.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+// Shared-memory matrix descriptor (sm_90): start address, leading / stride byte offsets >> 4,
+// layout type in bits 62-63 (0 = no swizzle, 1 = 128-byte swizzle).
+__device__ __forceinline__ uint64_t make_desc(uint32_t lo, uint32_t hi) {
+  return (static_cast<uint64_t>(hi) << 32) | lo;
+}
+// B operand, K-major, no swizzle: 8 x 16 B core matrices, K-adjacent ones 128 B apart (LBO),
+// 8-row groups `sbo` bytes apart.
+__device__ __forceinline__ uint32_t bdesc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | ((128u >> 4) << 16); }
+__device__ __forceinline__ uint32_t bdesc_hi(uint32_t sbo) { return sbo >> 4; }
 
 // ------------------------------------------------------------------ index helpers
 struct Pixel { int b, oy, ox; };
@@ -255,7 +185,7 @@ __device__ __forceinline__ void tile_halo(const TcParams& p, long long m0, long 
   *px_lo = lo;
   *px_cnt = static_cast<int>(max(hi - lo, 1LL));
 }
-// first word held by the halo stage (the TMA start coordinate must be 16-byte aligned: tools/tc_probe.cu)
+// first word held by the halo stage (the TMA start coordinate must be 16-byte aligned)
 __device__ __forceinline__ long long halo_word_base(const TcParams& p, long long px_lo) {
   return p.mode_flat ? ((px_lo * p.Cw) & ~3LL) : px_lo * p.CcB;
 }
@@ -385,105 +315,106 @@ __global__ void wpop2_kernel(const int32_t* __restrict__ filter, int32_t* __rest
   out[c] = 2 * s;
 }
 
-// OutputTransform<float> (output_transform.h:94-107) of one 32-channel chunk of one pixel, the fused
-// shortcut / activation of the ADD that followed, the chunk's sign bits, and the row written into the
-// (swizzled) staging buffer. Compile-time variants keep the common path free of branches so the
-// eight 4-channel groups schedule as independent chains.
-//   RES: a shortcut row is waiting in the buffer (in place); ACT: the ADD had a fused activation;
-//   ZPF: some pixel of the warp needs the optimised kernels' float zero-padding correction.
-template <bool RES, bool ACT, bool ZPF>
-__device__ __forceinline__ uint32_t epilogue_float_chunk(const TcParams& p, const int (&x)[32], unsigned char* buf,
-                                                         int lane, const int* tab_cc, float act_lo, float act_hi,
-                                                         int zrow, int c0) {
-  uint32_t bits = 0;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    float4* cell = reinterpret_cast<float4*>(buf + ((k ^ (lane & 7)) << 4));
-    const float4 mu = reinterpret_cast<const float4*>(tab_cc + 128)[k];
-    const float4 bi = reinterpret_cast<const float4*>(tab_cc + 256)[k];
-    float y0 = transform_float_x2(x[4 * k], p.clamp_min, p.clamp_max, mu.x, bi.x);
-    float y1 = transform_float_x2(x[4 * k + 1], p.clamp_min, p.clamp_max, mu.y, bi.y);
-    float y2 = transform_float_x2(x[4 * k + 2], p.clamp_min, p.clamp_max, mu.z, bi.z);
-    float y3 = transform_float_x2(x[4 * k + 3], p.clamp_min, p.clamp_max, mu.w, bi.w);
-    if (ZPF) {
-      // edge pixels: y += cache[row][c] (zero_padding_correction.h:289-291); lanes whose pixel
-      // needs no correction (zrow < 0) keep y untouched
-      const float4 cv = __ldg(reinterpret_cast<const float4*>(p.zpc_cache + static_cast<size_t>(max(zrow, 0)) * p.ldc + c0) + k);
-      if (zrow >= 0) {
-        y0 = __fadd_rn(y0, cv.x); y1 = __fadd_rn(y1, cv.y); y2 = __fadd_rn(y2, cv.z); y3 = __fadd_rn(y3, cv.w);
-      }
-    }
-    if (RES) {
-      const float4 rv = *cell;
-      y0 = __fadd_rn(y0, rv.x); y1 = __fadd_rn(y1, rv.y); y2 = __fadd_rn(y2, rv.z); y3 = __fadd_rn(y3, rv.w);
-      if (ACT) {
-        y0 = fminf(fmaxf(y0, act_lo), act_hi); y1 = fminf(fmaxf(y1, act_lo), act_hi);
-        y2 = fminf(fmaxf(y2, act_lo), act_hi); y3 = fminf(fmaxf(y3, act_lo), act_hi);
-      }
-    }
-    *cell = make_float4(y0, y1, y2, y3);
-    // LceQuantize of the value just written: bit = value < 0 (bitpack.h:159)
-    bits |= ((y0 < 0.0f ? 1u : 0u) | (y1 < 0.0f ? 2u : 0u) | (y2 < 0.0f ? 4u : 0u) | (y3 < 0.0f ? 8u : 0u)) << (4 * k);
-  }
-  return bits;
+// ------------------------------------------------------------------ wgmma, A from registers
+__device__ __forceinline__ void wgmma_s8_n32(uint32_t (&d)[16], const uint32_t (&a)[4], uint64_t desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, "
+               "{%16,%17,%18,%19}, %20, p;\n}\n"
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+                 "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(scale_d));
 }
-template <bool RES, bool ACT>
-__device__ __forceinline__ uint32_t epilogue_float_chunk_zp(const TcParams& p, const int (&x)[32], unsigned char* buf,
-                                                            int lane, const int* tab_cc, float act_lo, float act_hi,
-                                                            int zrow, int c0) {
-  // warp-uniform choice: the correction variant only where some lane of the warp is an edge pixel
-  if (__any_sync(0xffffffffu, zrow >= 0))
-    return epilogue_float_chunk<RES, ACT, true>(p, x, buf, lane, tab_cc, act_lo, act_hi, zrow, c0);
-  return epilogue_float_chunk<RES, ACT, false>(p, x, buf, lane, tab_cc, act_lo, act_hi, zrow, c0);
+__device__ __forceinline__ void wgmma_s8_n64(uint32_t (&d)[32], const uint32_t (&a)[4], uint64_t desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+               "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+               "{%32,%33,%34,%35}, %36, p;\n}\n"
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+                 "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+                 "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+                 "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+               "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+               "{%32,%33,%34,%35}, %36, p, 1, 1;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                 "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+               "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+               "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+               "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+               "{%64,%65,%66,%67}, %68, p, 1, 1;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                 "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                 "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                 "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                 "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                 "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(scale_d));
 }
 
 // ------------------------------------------------------------------ the kernel
-template <int V, int OUT>
-__global__ void __launch_bounds__(kThreads, 1)
-bconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_res,
-                const __grid_constant__ CUtensorMap tm_out, const TcParams p) {
+template <int BN>
+__device__ __forceinline__ void wgmma_s8(uint32_t (&d)[BN / 2], const uint32_t (&a)[4], uint64_t desc, uint32_t scale_d) {
+  if constexpr (BN == 64) wgmma_s8_n64(d, a, desc, scale_d);
+  else wgmma_s8_n32(d, a, desc, scale_d);
+}
+
+// the NW k32 MMAs of one stage (K word j of the stage image starts 256 B after word j - 1)
+template <int BN, int NW>
+__device__ __forceinline__ void wgmma_stage(uint32_t (&acc)[BN / 2], uint32_t (&a)[kWS][4], uint32_t lo, uint32_t hi,
+                                            uint32_t scale_d) {
+#pragma unroll
+  for (int j = 0; j < NW; ++j) wgmma_s8<BN>(acc, a[j], make_desc(lo + j * 16, hi), j == 0 ? scale_d : 1u);
+}
+
+// OR of a 32-channel sign / threshold word over the four threads of a quad (each holds 8 channels)
+__device__ __forceinline__ uint32_t quad_or(uint32_t v) {
+  v |= __shfl_xor_sync(0xffffffffu, v, 1);
+  v |= __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
+// Compiled for two CTAs per SM: one CTA's epilogue and halo waits overlap the other's MMAs.
+template <int V, int OUT, int BN>
+__global__ void __launch_bounds__(kThreads, 2)
+bconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const TcParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.off_bar);
-  uint32_t* tmem_base_p = reinterpret_cast<uint32_t*>(smem + p.off_bar + kBarBytes - 16);
   uint64_t* b_full = bars;                     // [kMaxNB]
   uint64_t* b_empty = b_full + kMaxNB;         // [kMaxNB]
   uint64_t* raw_full = b_empty + kMaxNB;       // [kNR]
   uint64_t* raw_empty = raw_full + kNR;        // [kNR]
-  uint64_t* a_full = raw_empty + kNR;          // [kNA]
-  uint64_t* a_empty = a_full + kNA;            // [kNA]
-  uint64_t* d_full = a_empty + kNA;            // [2]
-  uint64_t* d_empty = d_full + 2;              // [2]
-  uint64_t* res_full = d_empty + 2;            // [kMaxNS]
-  uint64_t* res_empty = res_full + kMaxNS;     // [kMaxNS]
 
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform
   const int lane = tid & 31;
 
   if (tid == 0) {
-    for (int i = 0; i < kMaxNB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < kNR; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], kNumExpWarps); }
-    // a stage is full when the four expander warps of its group have written the A columns and,
-    // when the weights stream through a ring (slot = A slot), the weight producer's copy has landed
-    for (int i = 0; i < kNA; ++i) { mbar_init(&a_full[i], p.b_resident ? 4 : 5); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&d_full[i], 1); mbar_init(&d_empty[i], kNumEpiWarps); }
-    for (int i = 0; i < kMaxNS; ++i) { mbar_init(&res_full[i], 1); mbar_init(&res_empty[i], 4); }
+    for (int i = 0; i < kMaxNB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], kNumMathWarps); }
+    for (int i = 0; i < kNR; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], kNumMathWarps); }
     fence_barrier_init();
   }
-  if (warp == kWarpMma) tmem_alloc(tmem_base_p, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_base_p, 0);
-  const uint32_t tmem_a = tmem + 256;
 
   const int n_items = p.n_tiles * p.m_tiles;
   const int cc_last = p.Cw - (p.n_chunks - 1) * p.CcB;   // words per pixel in the last channel chunk
-  constexpr int VPS = kWS / V;   // vectors per stage
-  constexpr int VPH = 4 / V;     // vectors per half stage (one tcgen05.st.x32)
-  const bool prof = LCE_TC_PROF != 0 && p.prof != nullptr && blockIdx.x == 0 && lane == 0;
-  long long pw[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  const long long prof_t0 = prof ? clock64() : 0;
+  const uint32_t row32 = static_cast<uint32_t>(BN) * 32u;   // bytes of one K word of a stage image
 
   if (warp == kWarpActProd) {
     // ===== activation producer =====
@@ -498,7 +429,7 @@ bconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
         const long long wbase = halo_word_base(p, px_lo);
         for (int ch = 0; ch < p.n_chunks; ++ch, ++cnt) {
           const int rs = cnt % kNR;
-          mbar_wait_prof(&raw_empty[rs], ((cnt / kNR) & 1) ^ 1, 1, prof, pw[1]);
+          mbar_wait_tc(&raw_empty[rs], ((cnt / kNR) & 1) ^ 1, 1);
           unsigned char* dst = smem + p.off_raw + rs * p.raw_stage_bytes;
           if (p.mode_flat) {
             const int nwords = static_cast<int>((px_lo + px_cnt) * p.Cw - wbase);
@@ -515,61 +446,10 @@ bconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
         }
       }
     }
-  } else if (warp == kWarpMma) {
-    // ===== MMA issuer: the whole warp runs the loop (values stay in uniform registers), one
-    // elected lane issues =====
-    const uint32_t idesc = make_idesc(p.BN);
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t row32 = static_cast<uint32_t>(p.BN) * 32u;      // bytes of one K word of a stage image
-    uint32_t as = 0, a_par = 0, bs = 0, it = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-      const uint32_t ds = it & 1;
-      mbar_wait_prof(&d_empty[ds], ((it >> 1) & 1) ^ 1, 2, prof, pw[1]);
-      tc_fence_after();
-      const uint32_t d_addr = tmem + ds * p.BN;
-      uint32_t acc = 0;
-      uint32_t wofs = 0;   // K-word offset of the stage inside the tile's weights (resident mode)
-      for (int ch = 0; ch < p.n_chunks; ++ch) {
-        const int nq = p.taps * (ch == p.n_chunks - 1 ? cc_last : p.CcB);
-        for (int q0 = 0; q0 < nq; q0 += kWS) {
-          const int nw = min(kWS, nq - q0);
-          uint32_t b_addr;
-          if (p.b_resident) {
-            b_addr = smem_base + wofs * row32;
-            if (it == 0) mbar_wait_prof(&b_full[bs], 0, 3, prof, pw[2]);
-          } else {
-            b_addr = smem_base + as * (row32 * kWS);   // ring: the weight slot IS the A slot
-          }
-          mbar_wait_prof(&a_full[as], a_par, 4, prof, pw[3]);
-          tc_fence_after();
-          const uint32_t lo = bdesc_lo(b_addr);
-          const uint32_t hi = bdesc_hi(static_cast<uint32_t>(nw) * 256u);
-          const uint32_t a_addr = tmem_a + as * 64;
-          if (elect_one()) {
-            if (nw == kWS) {
-#pragma unroll
-              for (int j = 0; j < kWS; ++j) mma_i8_ts2(d_addr, a_addr + j * 8, lo + j * 16, hi, idesc, j == 0 ? acc : 1u);
-            } else {
-              for (int j = 0; j < nw; ++j) mma_i8_ts2(d_addr, a_addr + j * 8, lo + j * 16, hi, idesc, j == 0 ? acc : 1u);
-            }
-            tc_commit(&a_empty[as]);   // frees the A columns and (ring) the weight slot
-          }
-          __syncwarp();
-          acc = 1;
-          wofs += nw;
-          if (++as == kNA) { as = 0; a_par ^= 1; }
-          ++bs;
-        }
-      }
-      bs = 0;
-      if (elect_one()) tc_commit(&d_full[ds]);
-      __syncwarp();
-    }
   } else if (warp == kWarpWeightProd) {
     // ===== weight producer =====
     if (lane == 0) {
-      const uint32_t row32 = static_cast<uint32_t>(p.BN) * 32u;
-      uint32_t bs = 0, as = 0, a_par = 0;
+      uint32_t bs = 0, slot = 0, par = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
         const int nt = static_cast<int>(fdiv(static_cast<uint32_t>(item), p.fd_mt));
         const uint8_t* src = p.wt + static_cast<size_t>(nt) * p.Kw_total * row32;
@@ -584,11 +464,10 @@ bconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
               bulk_g2s(smem + wofs * row32, src + static_cast<size_t>(wofs) * row32, bytes, &b_full[bs]);
               ++bs;
             } else {
-              // ring: slot `as` is shared with the A stage; its a_full barrier also counts this copy
-              mbar_wait_prof(&a_empty[as], a_par ^ 1, 5, prof, pw[1]);
-              mbar_arrive_expect_tx(&a_full[as], bytes);
-              bulk_g2s(smem + as * (row32 * kWS), src + static_cast<size_t>(wofs) * row32, bytes, &a_full[as]);
-              if (++as == kNA) { as = 0; a_par ^= 1; }
+              mbar_wait_tc(&b_empty[slot], par ^ 1, 5);
+              mbar_arrive_expect_tx(&b_full[slot], bytes);
+              bulk_g2s(smem + slot * (row32 * kWS), src + static_cast<size_t>(wofs) * row32, bytes, &b_full[slot]);
+              if (++slot == static_cast<uint32_t>(p.nB)) { slot = 0; par ^= 1; }
             }
             wofs += nw;
           }
@@ -596,301 +475,214 @@ bconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
         if (p.b_resident) break;   // loaded once, kept for every tile of this CTA
       }
     }
-  } else if (warp == kWarpResProd) {
-    // ===== shortcut producer =====
-    if (lane == 0 && p.has_res) {
-      uint32_t cnt = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int nt = static_cast<int>(fdiv(static_cast<uint32_t>(item), p.fd_mt));
-        const long long m0 = static_cast<long long>(item - nt * p.m_tiles) * kBM;
-        const int c_tile = nt * p.BN;
-        const int n_cc = min(p.BN, p.cout - c_tile + 31) >> 5;
-        for (int cc = 0; cc < n_cc; ++cc, ++cnt) {
-          const int sl = cnt % p.nS;
-          mbar_wait_prof(&res_empty[sl], ((cnt / p.nS) & 1) ^ 1, 6, prof, pw[1]);
-          mbar_arrive_expect_tx(&res_full[sl], kSlotBytes);
-          tma_load_2d(smem + p.off_slots + sl * kSlotBytes, &tm_res, &res_full[sl], c_tile + cc * 32, static_cast<int>(m0));
-        }
-      }
-    }
-  } else if (warp < kFirstExpWarp + kNumExpWarps) {
-    // ===== expanders: thread = output pixel = TMEM lane =====
-    const int q = warp & 3;
-    const int group = (warp - kFirstExpWarp) >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
+  } else {
+    // ===== math warpgroups: thread (g, t) of warp w holds pixels r0 = 64 * wg + 16 * (w & 3) + g
+    // and r0 + 8, K bytes 4t..4t+3 and 16+4t..16+4t+3 of each k32 step, and channels
+    // 8j + 2t, 8j + 2t + 1 of every 8-channel block j of the accumulator.
+    const int wg = warp >> 2;
+    const int g = lane >> 2, t = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + g;
     const int pitch = p.mode_flat ? p.Cw : p.CcB;
-    uint32_t cntA = 0, cntR = 0;
-    int pend_as = -1;   // stage whose tcgen05.st is in flight (its a_full arrive is still owed)
-    auto flush = [&]() {
-      if (pend_as >= 0) {
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_full[pend_as]);
-        pend_as = -1;
-      }
-    };
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const uint32_t tmask = 0x01010101u << t;
+    const uint32_t smem_base = smem_u32(smem);
+    constexpr int VPS = kWS / V;   // vectors per stage
+    const float act_lo = p.residual_act == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
+    const float act_hi = p.residual_act == LCE_ACT_RELU ? __int_as_float(0x7f800000)
+                                                        : (p.residual_act == LCE_ACT_RELU6 ? 6.0f : 1.0f);
+    uint32_t cntR = 0, slot = 0, par = 0;
+    bool first_item = true;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x, first_item = false) {
       const int nt = static_cast<int>(fdiv(static_cast<uint32_t>(item), p.fd_mt));
       const long long m0 = static_cast<long long>(item - nt * p.m_tiles) * kBM;
       long long px_lo;
       int px_cnt;
       tile_halo(p, m0, &px_lo, &px_cnt);
       const long long wbase = halo_word_base(p, px_lo);
-      const long long m = m0 + row;
-      const bool row_ok = m < p.M;
-      int iy0 = 0, ix0 = 0, off0 = 0;
-      if (row_ok) {
-        const Pixel px = split_px(p, static_cast<uint32_t>(m));
-        iy0 = px.oy * p.sh - p.ph;
-        ix0 = px.ox * p.sw - p.pw;
-        // word offset of (this pixel's tap (0,0), channel word 0) inside the halo stage
-        off0 = static_cast<int>(((static_cast<long long>(px.b) * p.H + iy0) * p.W + ix0) * pitch - wbase);
+      long long m[2];
+      bool row_ok[2];
+      int iy0[2], ix0[2], off0[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        m[i] = m0 + r0 + 8 * i;
+        row_ok[i] = m[i] < p.M;
+        iy0[i] = ix0[i] = off0[i] = 0;
+        if (row_ok[i]) {
+          const Pixel px = split_px(p, static_cast<uint32_t>(m[i]));
+          iy0[i] = px.oy * p.sh - p.ph;
+          ix0[i] = px.ox * p.sw - p.pw;
+          // word offset of (this pixel's tap (0,0), channel word 0) inside the halo stage
+          off0[i] = static_cast<int>(((static_cast<long long>(px.b) * p.H + iy0[i]) * p.W + ix0[i]) * pitch - wbase);
+        }
       }
+      uint32_t acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
+      uint32_t scale_d = 0;
+      uint32_t wofs = 0, bs = 0;   // K-word offset / stage index inside the tile's weights
       for (int ch = 0; ch < p.n_chunks; ++ch, ++cntR) {
         const int rs = cntR % kNR;
-        const bool last = ch == p.n_chunks - 1;
-        const int cwv = (last ? cc_last : p.CcB) / V;
-        const FastDiv fd_cwv = last ? p.fd_cwv_last : p.fd_cwv_full;
+        const int cwv = (ch == p.n_chunks - 1 ? cc_last : p.CcB) / V;
         const int nvec = p.taps * cwv;
-        const int nst = (nvec + VPS - 1) / VPS;
         const uint32_t* raw = reinterpret_cast<const uint32_t*>(smem + p.off_raw + rs * p.raw_stage_bytes);
-        mbar_wait_prof(&raw_full[rs], (cntR / kNR) & 1, 7, prof, pw[1]);
-        for (int st = 0; st < nst; ++st, ++cntA) {
-          if ((cntA % kExpGroups) != static_cast<uint32_t>(group)) continue;
-          const int as = cntA % kNA;
-          uint32_t v[32];
-          const long long tb0 = prof ? clock64() : 0;
-          int kv = st * VPS;
-          int tap = static_cast<int>(fdiv(static_cast<uint32_t>(kv), fd_cwv));
-          int cv = kv - tap * cwv;
-          int fy = static_cast<int>(fdiv(static_cast<uint32_t>(tap), p.fd_kw));
-          int fx = tap - fy * p.KW;
-          auto build_half = [&]() {
-#pragma unroll
-            for (int u = 0; u < VPH; ++u, ++kv) {
-              uint32_t w[V];
-#pragma unroll
-              for (int e = 0; e < V; ++e) w[e] = 0;
-              const int iy = iy0 + fy * p.dh, ix = ix0 + fx * p.dw;
-              if (row_ok && kv < nvec && static_cast<unsigned>(iy) < static_cast<unsigned>(p.H) &&
-                  static_cast<unsigned>(ix) < static_cast<unsigned>(p.W))
-                load_words<V>(reinterpret_cast<const typename VecT<V>::T*>(raw + off0 + (fy * p.dh * p.W + fx * p.dw) * pitch + cv * V), w);
-#pragma unroll
-              for (int e = 0; e < V; ++e) expand_word(w[e], &v[(u * V + e) * 8]);
-              if (++cv == cwv) {
-                cv = 0;
-                if (++fx == p.KW) { fx = 0; ++fy; }
-              }
-            }
-          };
-          build_half();
-          if (prof) pw[3] += clock64() - tb0;
-          flush();   // the previous stage's store has had this build to complete
-          mbar_wait_prof(&a_empty[as], ((cntA / kNA) & 1) ^ 1, 8, prof, pw[2]);
-          const long long ts0 = prof ? clock64() : 0;
-          tc_fence_after();
-          tmem_st32(tmem_a + lane_base + as * 64, v);
-          if (kv < nvec) {   // second half of the stage (absent in a short last stage)
-            build_half();
-            tmem_st32(tmem_a + lane_base + as * 64 + 32, v);
+        mbar_wait_tc(&raw_full[rs], (cntR / kNR) & 1, 7);
+        int kv = 0, cv = 0, fy = 0, fx = 0;
+        while (kv < nvec) {
+          const int nw = min(kWS, (nvec - kv) * V);
+          uint32_t b_addr;
+          if (p.b_resident) {
+            b_addr = smem_base + wofs * row32;
+            if (first_item) mbar_wait_tc(&b_full[bs], 0, 3);
+          } else {
+            b_addr = smem_base + slot * (row32 * kWS);
+            mbar_wait_tc(&b_full[slot], par, 4);
           }
-          pend_as = as;
-          if (prof) { pw[4] += clock64() - ts0; pw[5] += 1; }
+          // the stage's A fragments: two pixels x kWS words, expanded in registers
+          uint32_t a[kWS][4];
+#pragma unroll
+          for (int u = 0; u < VPS; ++u, ++kv) {
+            uint32_t w[2][V];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+#pragma unroll
+              for (int e = 0; e < V; ++e) w[i][e] = 0;
+              const int iy = iy0[i] + fy * p.dh, ix = ix0[i] + fx * p.dw;
+              if (row_ok[i] && kv < nvec && static_cast<unsigned>(iy) < static_cast<unsigned>(p.H) &&
+                  static_cast<unsigned>(ix) < static_cast<unsigned>(p.W))
+                load_words<V>(reinterpret_cast<const typename VecT<V>::T*>(raw + off0[i] + (fy * p.dh * p.W + fx * p.dw) * pitch + cv * V),
+                              w[i]);
+            }
+#pragma unroll
+            for (int e = 0; e < V; ++e) {
+              uint32_t* f = a[u * V + e];
+              f[0] = w[0][e] & tmask;
+              f[1] = w[1][e] & tmask;
+              f[2] = (w[0][e] >> 4) & tmask;
+              f[3] = (w[1][e] >> 4) & tmask;
+            }
+            if (++cv == cwv) {
+              cv = 0;
+              if (++fx == p.KW) { fx = 0; ++fy; }
+            }
+          }
+#pragma unroll
+          for (int j = 0; j < kWS; ++j) fence_regs(a[j]);
+          wgmma_fence();
+          const uint32_t lo = bdesc_lo(b_addr);
+          const uint32_t hi = bdesc_hi(static_cast<uint32_t>(nw) * 256u);
+          // straight-line sequences: a predicated wgmma would make ptxas serialise the stage
+          switch (nw) {
+            case 8: wgmma_stage<BN, 8>(acc, a, lo, hi, scale_d); break;
+            case 7: wgmma_stage<BN, 7>(acc, a, lo, hi, scale_d); break;
+            case 6: wgmma_stage<BN, 6>(acc, a, lo, hi, scale_d); break;
+            case 5: wgmma_stage<BN, 5>(acc, a, lo, hi, scale_d); break;
+            case 4: wgmma_stage<BN, 4>(acc, a, lo, hi, scale_d); break;
+            case 3: wgmma_stage<BN, 3>(acc, a, lo, hi, scale_d); break;
+            case 2: wgmma_stage<BN, 2>(acc, a, lo, hi, scale_d); break;
+            default: wgmma_stage<BN, 1>(acc, a, lo, hi, scale_d); break;
+          }
+          scale_d = 1;
+          wgmma_commit();
+          wgmma_wait_all();
+          fence_regs(acc);
+          if (!p.b_resident) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&b_empty[slot]);
+            if (++slot == static_cast<uint32_t>(p.nB)) { slot = 0; par ^= 1; }
+          }
+          wofs += nw;
+          ++bs;
         }
-        flush();
         __syncwarp();
         if (lane == 0) mbar_arrive(&raw_empty[rs]);
       }
-    }
-    flush();
-  } else {
-    // ===== epilogue: thread = output pixel = TMEM lane; group g takes chunks cc with (cc & 1) == g
-    const int q = warp & 3;
-    const int group = (warp - kFirstEpiWarp) >> 2;
-    const int etid = tid - kFirstEpiWarp * 32;     // 0..255
-    const int row = q * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-    const float act_lo = p.residual_act == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
-    const float act_hi = p.residual_act == LCE_ACT_RELU ? __int_as_float(0x7f800000)
-                                                        : (p.residual_act == LCE_ACT_RELU6 ? 6.0f : 1.0f);
-    uint32_t it = 0, cntS = 0;
-    int pend_sl = -1;   // residual slot whose TMA store is still reading shared memory
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-      const int nt = static_cast<int>(fdiv(static_cast<uint32_t>(item), p.fd_mt));
-      const long long m0 = static_cast<long long>(item - nt * p.m_tiles) * kBM;
-      const int c_tile = nt * p.BN;
-      const int n_cc = min(p.BN, p.cout - c_tile + 31) >> 5;
-      const long long m = m0 + row;
-      const bool row_ok = m < p.M;
-      const uint32_t ds = it & 1;
-      // per-channel epilogue vectors of this n tile -> shared memory (once when there is one n tile)
-      int* tab = reinterpret_cast<int*>(smem + p.off_tab + (p.n_tiles > 1 ? (it & 1) * (kTabBytes / 2) : 0));
-      if (p.n_tiles > 1 || it == 0) {
-        if (etid < p.BN) {
-          const int c = c_tile + etid;
-          tab[etid] = p.wpop2[c];
-          if (OUT == LCE_OUT_BITPACKED) {
-            tab[384 + etid] = p.thr[c];
-          } else if (OUT != LCE_OUT_RAW_ACC) {
-            tab[128 + etid] = __float_as_int(p.mul[c]);
-            tab[256 + etid] = __float_as_int(p.bias[c]);
-          }
-        }
-        named_bar_sync(1, kNumEpiWarps * 32);
-      }
-      // zero padding: the reference kernel's out-of-bounds taps, or the optimised kernels' cache row
-      unsigned long long oob = 0;
-      int zrow = -1;
-      if (p.tap_popc_t != nullptr && row_ok) {
-        const Pixel px = split_px(p, static_cast<uint32_t>(m));
-        if (p.zp_float) zrow = zero_pad_cache_row(p, px.oy, px.ox);
-        else oob = zero_pad_tap_mask(p, px.oy, px.ox);
-      }
-      mbar_wait_prof(&d_full[ds], (it >> 1) & 1, 9, prof, pw[1]);
-      tc_fence_after();
-      const int last_cc = ((n_cc - 1 - group) & ~1) + group;   // this group's last chunk (< group: none)
-      if (group >= n_cc) {   // nothing to read for this group in this tile
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&d_empty[ds]);
-      }
-      for (int cc = 0; cc < n_cc; ++cc, ++cntS) {
-        if ((cc & 1) != group) continue;
-        uint32_t accu[32];
-        const long long tl0 = prof ? clock64() : 0;
-        tmem_ld32(tmem + lane_base + ds * p.BN + cc * 32, accu);
-        if (prof) { pw[3] += clock64() - tl0; pw[6] += 1; }
-        const long long tc0 = prof ? clock64() : 0;
-        if (cc == last_cc) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&d_empty[ds]);
-        }
-        const int c0 = c_tile + cc * 32;
-        // x = 2 * acc = (acc8 >> 2) + 2 * popc(w)   (acc8 is a multiple of 8)
-        int x[32];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int4 wp = reinterpret_cast<const int4*>(tab + cc * 32)[k];
-          x[4 * k] = (static_cast<int>(accu[4 * k]) >> 2) + wp.x;
-          x[4 * k + 1] = (static_cast<int>(accu[4 * k + 1]) >> 2) + wp.y;
-          x[4 * k + 2] = (static_cast<int>(accu[4 * k + 2]) >> 2) + wp.z;
-          x[4 * k + 3] = (static_cast<int>(accu[4 * k + 3]) >> 2) + wp.w;
-        }
-        if (oob != 0) {
-          for (unsigned long long mk = oob; mk != 0; mk &= mk - 1) {
-            const int t = __ffsll(static_cast<long long>(mk)) - 1;
-            const int4* tp = reinterpret_cast<const int4*>(p.tap_popc_t + static_cast<size_t>(t) * p.ldc + c0);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const int4 tv = __ldg(tp + k);
-              x[4 * k] += 2 * (p.zp_half - tv.x);
-              x[4 * k + 1] += 2 * (p.zp_half - tv.y);
-              x[4 * k + 2] += 2 * (p.zp_half - tv.z);
-              x[4 * k + 3] += 2 * (p.zp_half - tv.w);
-            }
-          }
-        }
-        if (OUT == LCE_OUT_FLOAT || OUT == LCE_OUT_RAW_ACC) {
-          const int sl = cntS % p.nS;
-          unsigned char* buf = smem + p.off_slots + sl * kSlotBytes + q * 4096 + lane * 128;
-          const bool res = OUT == LCE_OUT_FLOAT && p.has_res;
-          // the store that last read a buffer of this warp must have finished reading it
-          if (lane == 0) {
-            if (res) {
-              if (pend_sl >= 0) {
-                tma_store_wait_read();
-                mbar_arrive(&res_empty[pend_sl]);
-              }
-            } else if (p.nS >= 4) {
-              tma_store_wait_read1();
-            } else {
-              tma_store_wait_read();
-            }
-          }
-          pend_sl = -1;
-          __syncwarp();
-          if (res) mbar_wait_prof(&res_full[sl], (cntS / p.nS) & 1, 10, prof, pw[2]);
-          uint32_t bits = 0;
-          if (OUT == LCE_OUT_RAW_ACC) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-              *reinterpret_cast<uint4*>(buf + ((k ^ (lane & 7)) << 4)) =
-                  make_uint4(x[4 * k] >> 1, x[4 * k + 1] >> 1, x[4 * k + 2] >> 1, x[4 * k + 3] >> 1);
-          } else if (!res) {
-            bits = epilogue_float_chunk_zp<false, false>(p, x, buf, lane, tab + cc * 32, act_lo, act_hi, zrow, c0);
-          } else if (p.residual_act == LCE_ACT_NONE) {
-            bits = epilogue_float_chunk_zp<true, false>(p, x, buf, lane, tab + cc * 32, act_lo, act_hi, zrow, c0);
-          } else {
-            bits = epilogue_float_chunk_zp<true, true>(p, x, buf, lane, tab + cc * 32, act_lo, act_hi, zrow, c0);
-          }
-          if (prof) pw[4] += clock64() - tc0;
-          const long long tq0 = prof ? clock64() : 0;
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            if (m0 + q * 32 < p.M) tma_store_2d(&tm_out, smem + p.off_slots + sl * kSlotBytes + q * 4096, c0, static_cast<int>(m0) + q * 32);
-          }
-          if (res) pend_sl = sl;
-          __syncwarp();
-          if (prof) pw[5] += clock64() - tq0;
-          if (OUT == LCE_OUT_FLOAT && p.packed_out != nullptr && row_ok)
-            p.packed_out[static_cast<size_t>(m) * p.cw_out + (c0 >> 5)] = static_cast<int32_t>(bits);
-        } else if (OUT == LCE_OUT_INT8) {
-          if (row_ok) {
-            uint32_t pk[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const float4 mu = reinterpret_cast<const float4*>(tab + 128 + cc * 32)[k];
-              const float4 bi = reinterpret_cast<const float4*>(tab + 256 + cc * 32)[k];
-              const int q0 = round_saturate_i8(transform_float_x2(x[4 * k], p.clamp_min, p.clamp_max, mu.x, bi.x));
-              const int q1 = round_saturate_i8(transform_float_x2(x[4 * k + 1], p.clamp_min, p.clamp_max, mu.y, bi.y));
-              const int q2 = round_saturate_i8(transform_float_x2(x[4 * k + 2], p.clamp_min, p.clamp_max, mu.z, bi.z));
-              const int q3 = round_saturate_i8(transform_float_x2(x[4 * k + 3], p.clamp_min, p.clamp_max, mu.w, bi.w));
-              pk[k] = (q0 & 0xFF) | ((q1 & 0xFF) << 8) | ((q2 & 0xFF) << 16) | (static_cast<uint32_t>(q3 & 0xFF) << 24);
-            }
-            int8_t* o = static_cast<int8_t*>(p.out) + static_cast<size_t>(m) * p.cout + c0;
-            if ((p.cout & 15) == 0 && c0 + 32 <= p.cout) {
-              reinterpret_cast<uint4*>(o)[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              reinterpret_cast<uint4*>(o)[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-            } else {
-#pragma unroll
-              for (int k = 0; k < 32; ++k)
-                if (c0 + k < p.cout) o[k] = static_cast<int8_t>((pk[k >> 2] >> (8 * (k & 3))) & 0xFF);
-            }
-          }
-        } else {  // LCE_OUT_BITPACKED: bit = acc > threshold (output_transform.h:164-167)
-          uint32_t bits = 0;
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const int4 th = reinterpret_cast<const int4*>(tab + 384 + cc * 32)[k];
-            bits |= (((x[4 * k] >> 1) > th.x ? 1u : 0u) | ((x[4 * k + 1] >> 1) > th.y ? 2u : 0u) |
-                     ((x[4 * k + 2] >> 1) > th.z ? 4u : 0u) | ((x[4 * k + 3] >> 1) > th.w ? 8u : 0u)) << (4 * k);
-          }
-          const int valid = p.cout - c0;
-          if (valid < 32) bits &= (1u << valid) - 1u;
-          if (row_ok) static_cast<int32_t*>(p.out)[static_cast<size_t>(m) * p.cw_out + (c0 >> 5)] = static_cast<int32_t>(bits);
-        }
-      }
-    }
-    if (lane == 0) {
-      if (pend_sl >= 0) {
-        tma_store_wait_read();
-        mbar_arrive(&res_empty[pend_sl]);
-      }
-      tma_store_wait_all();
-    }
-  }
 
-  if (prof) {
-    pw[0] = clock64() - prof_t0;
-    for (int i = 0; i < 8; ++i) p.prof[warp * 8 + i] = pw[i];
+      // ---- epilogue, from the accumulator registers
+      const int c_tile = nt * BN;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        // zero padding: the reference kernel's out-of-bounds taps, or the optimised kernels' cache row
+        unsigned long long oob = 0;
+        int zrow = -1;
+        if (p.tap_popc_t != nullptr && row_ok[i]) {
+          const Pixel px = split_px(p, static_cast<uint32_t>(m[i]));
+          if (p.zp_float) zrow = zero_pad_cache_row(p, px.oy, px.ox);
+          else oob = zero_pad_tap_mask(p, px.oy, px.ox);
+        }
+        // x = 2 * acc = (acc8 >> 2) + 2 * popc(w)   (acc8 is a multiple of 8)
+        int x[BN / 4];
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = c_tile + 8 * j + 2 * t;
+          x[2 * j] = (static_cast<int>(acc[4 * j + 2 * i]) >> 2) + __ldg(p.wpop2 + c);
+          x[2 * j + 1] = (static_cast<int>(acc[4 * j + 2 * i + 1]) >> 2) + __ldg(p.wpop2 + c + 1);
+        }
+        for (unsigned long long mk = oob; mk != 0; mk &= mk - 1) {
+          const int tp = __ffsll(static_cast<long long>(mk)) - 1;
+          const int32_t* tpc = p.tap_popc_t + static_cast<size_t>(tp) * p.ldc + c_tile + 2 * t;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            x[2 * j] += 2 * (p.zp_half - __ldg(tpc + 8 * j));
+            x[2 * j + 1] += 2 * (p.zp_half - __ldg(tpc + 8 * j + 1));
+          }
+        }
+#pragma unroll
+        for (int cc = 0; cc < BN / 32; ++cc) {
+          const int c0 = c_tile + cc * 32;
+          if (c0 >= p.cout) break;   // warp-uniform
+          uint32_t bits = 0;
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * cc + jj;
+            const int c = c_tile + 8 * j + 2 * t;
+            const bool c_ok = row_ok[i] && c < p.cout;
+            const size_t o = static_cast<size_t>(m[i]) * p.cout + c;
+            if (OUT == LCE_OUT_RAW_ACC) {
+              if (c_ok) *reinterpret_cast<int2*>(static_cast<int32_t*>(p.out) + o) = make_int2(x[2 * j] >> 1, x[2 * j + 1] >> 1);
+            } else if (OUT == LCE_OUT_FLOAT) {
+              float y[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                y[e] = transform_float_x2(x[2 * j + e], p.clamp_min, p.clamp_max, __ldg(p.mul + c + e), __ldg(p.bias + c + e));
+                // edge pixels: y += cache[row][c] (zero_padding_correction.h:289-291)
+                if (zrow >= 0) y[e] = __fadd_rn(y[e], __ldg(p.zpc_cache + static_cast<size_t>(zrow) * p.ldc + c + e));
+              }
+              if (p.has_res && c_ok) {
+                const float2 rv = __ldg(reinterpret_cast<const float2*>(p.residual + o));
+                y[0] = __fadd_rn(y[0], rv.x);
+                y[1] = __fadd_rn(y[1], rv.y);
+                if (p.residual_act != LCE_ACT_NONE) {
+                  y[0] = fminf(fmaxf(y[0], act_lo), act_hi);
+                  y[1] = fminf(fmaxf(y[1], act_lo), act_hi);
+                }
+              }
+              if (c_ok) *reinterpret_cast<float2*>(static_cast<float*>(p.out) + o) = make_float2(y[0], y[1]);
+              // LceQuantize of the value just written: bit = value < 0 (bitpack.h:159)
+              bits |= ((y[0] < 0.0f ? 1u : 0u) | (y[1] < 0.0f ? 2u : 0u)) << (8 * jj + 2 * t);
+            } else if (OUT == LCE_OUT_INT8) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int q = round_saturate_i8(
+                    transform_float_x2(x[2 * j + e], p.clamp_min, p.clamp_max, __ldg(p.mul + c + e), __ldg(p.bias + c + e)));
+                if (row_ok[i] && c + e < p.cout) static_cast<int8_t*>(p.out)[o + e] = static_cast<int8_t>(q);
+              }
+            } else {  // LCE_OUT_BITPACKED: bit = acc > threshold (output_transform.h:164-167)
+              bits |= (((x[2 * j] >> 1) > __ldg(p.thr + c) ? 1u : 0u) | ((x[2 * j + 1] >> 1) > __ldg(p.thr + c + 1) ? 2u : 0u))
+                      << (8 * jj + 2 * t);
+            }
+          }
+          if (OUT == LCE_OUT_BITPACKED) {
+            bits = quad_or(bits);
+            const int valid = p.cout - c0;
+            if (valid < 32) bits &= (1u << valid) - 1u;
+            if (t == 0 && row_ok[i]) static_cast<int32_t*>(p.out)[static_cast<size_t>(m[i]) * p.cw_out + (c0 >> 5)] = static_cast<int32_t>(bits);
+          } else if (OUT == LCE_OUT_FLOAT && p.packed_out != nullptr) {
+            bits = quad_or(bits);
+            if (t == 0 && row_ok[i]) p.packed_out[static_cast<size_t>(m[i]) * p.cw_out + (c0 >> 5)] = static_cast<int32_t>(bits);
+          }
+        }
+      }
+    }
   }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWarpMma) tmem_dealloc(tmem, 512);
 }
 
 }  // namespace tc

@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing for the batch-sharded path (SURVEY 8e).
+"""Multi-GPU plumbing for the batch-sharded path.
 
 The path shards by image: every rank holds a full replica of the packed weights and
 processes its own slice of the batch; there is exactly ONE collective, at load time
@@ -76,7 +76,7 @@ def broadcast_model(layers, device, src=0):
 
 
 def gather_outputs(local: torch.Tensor, batch: int):
-    """Host-side concat of per-rank results in batch order (SURVEY 8e: 'outputs are
+    """Host-side concat of per-rank results in batch order ('outputs are
     copied D2H per rank and concatenated on the host' -- not a step collective)."""
     world = dist.get_world_size() if dist.is_initialized() else 1
     if world == 1:

@@ -4,7 +4,7 @@ There is no TensorFlow, no flatbuffers package and no model zoo offline, so the
 QuickNet / QuickNetLarge / Bi-RealNet-18 graphs the benchmark runs are SYNTHESISED:
 correct topology, random weights (compute_engine_b200/zoo.py), serialised here into
 real `.tflite` files that the C++ graph host reads back through its own reader.
-Field ids follow tensorflow/lite/schema/schema.fbs (SURVEY 9.1): Model :1609,
+Field ids follow tensorflow/lite/schema/schema.fbs: Model :1609,
 OperatorCode :1467, SubGraph :1540, Tensor :210, Operator :1493, Buffer :1562,
 QuantizationParameters :75, builtin option tables :806-1106.
 """
@@ -239,7 +239,7 @@ class TFLiteModel:
 
 
 # --------------------------------------------------------------------------- #
-# FlexBuffers map of integers (the LCE ops' custom_options; format: SURVEY 9.2), in pure
+# FlexBuffers map of integers (the LCE ops' custom_options), in pure
 # Python so that a model can be serialised without loading any native library. Emits the same
 # bytes as csrc/host/flexbuffer_map.cc::WriteFlexIntMap (tests/test_host_ops.py compares them,
 # and both reproduce the blobs the real flatbuffers library wrote into

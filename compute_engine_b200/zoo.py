@@ -1,10 +1,10 @@
-"""Synthetic model zoo: the three model families BASELINE.json names, emitted as real
+"""Synthetic model zoo: the three model families the benchmark runs, emitted as real
 `.tflite` graphs with the op sequence the LCE converter produces (LceQuantize ->
 LceBconv2d with folded BatchNorm multiplier/bias and fused ReLU -> ADD shortcut ...),
 random weights (seeded), correct topology.
 
 The topologies are NOT in /root/reference (they live in larq-zoo, absent offline);
-they are restated from the public QuickNet / Bi-Real Net descriptions (SURVEY 8d):
+they are restated from the public QuickNet / Bi-Real Net descriptions:
   QuickNet(-Large): stem [conv3x3 s2 -> BN/ReLU -> depthwise3x3 s2 -> conv1x1 -> BN],
     sections of residual blocks [sign -> binary conv3x3 (one-padding, ReLU fused, BN
     folded) -> + shortcut] with filters (64,128,256,512), blocks (4,4,4,4) / (6,8,12,6),

@@ -1,5 +1,5 @@
 /*
- * lce_b200.h -- the drop-in boundary: a C-ABI CUDA layer (sm_100a) for the one
+ * lce_b200.h -- the drop-in boundary: a C-ABI CUDA layer (sm_90a) for the one
  * hot path of larq/compute-engine: LceQuantize -> LceBconv2d (-> LceBMaxPool2d,
  * LceDequantize). Plain pointers and sizes only; no torch / TFLite types.
  *
@@ -135,9 +135,9 @@ void lce_b200_bgemm_destroy(lce_b200_bgemm* plan);
  * `gpu_launches`). */
 uint64_t lce_b200_launch_count(void);
 /* Diagnostics. path_counts: inner-product launches so far by kernel family
- * {tcgen05 (lce_b200_tc.cuh), mma.sync int8 (lce_b200_imma.cuh), XOR + POPC
+ * {wgmma (lce_b200_tc.cuh), mma.sync int8 (lce_b200_imma.cuh), XOR + POPC
  * (lce_b200_kernels.cuh)} -- the tests use it to prove which kernel ran.
- * tc_debug: the tcgen05 kernel's deadlock-watchdog record; out[7] != 0 means a
+ * tc_debug: the wgmma kernel's deadlock-watchdog record; out[7] != 0 means a
  * wait timed out ({barrier tag, block, thread, parity, count} in out[0..4]);
  * reading clears the flag. */
 void lce_b200_path_counts(uint64_t out[3]);

@@ -1,7 +1,7 @@
 /*
  * lce_b200_builtins.h -- C-ABI of the float TFLite builtins the three model
  * families (QuickNet, QuickNetLarge, Bi-RealNet-18) use AROUND the binary path
- * (SURVEY 8f-1). In the reference these come from stock TFLite
+ * In the reference these come from stock TFLite
  * (tensorflow/lite/kernels/internal/reference/{conv.h:27, depthwiseconv_float.h:25,
  * pooling.h:28,196, add.h, fully_connected.h:29, softmax.h:31, reduce.h}); here they
  * are plain fp32 CUDA kernels so the graph never leaves HBM between binary layers.

@@ -1,7 +1,7 @@
 // oracle/oracle_ops.cc -- TEST INFRASTRUCTURE ONLY: the CPU oracle
 // (oracle/lce_oracle.c) wrapped as TfLiteRegistrations, so that the graph host's
 // plumbing (resolver, flexbuffer attributes, init -> prepare -> invoke, resize,
-// arena) can be exercised WITHOUT a GPU: BASELINE.json configs[0], "single
+// arena) can be exercised WITHOUT a GPU: the "single
 // LceBconv2d 56x56x256->256 k3 s1 on the CPU reference interpreter (bit-exact
 // plumbing, no GPU)". Never linked into compute_engine_b200/.
 #include <cstring>

@@ -247,7 +247,7 @@ int lce_ref_bconv2d(const lce_bconv2d_desc* d, int kind, const int32_t* input,
 
 // The reference's bconv kernels are single-threaded by construction
 // (indirect_bgemm/kernel.h:180-183); a batch is run as independent per-image
-// calls spread over `threads` host threads (BASELINE.md section 3).
+// calls spread over `threads` host threads.
 int lce_ref_bconv2d_mt(const lce_bconv2d_desc* d, int kind, int threads,
                        const int32_t* input, const int32_t* filter,
                        const float* post_mul, const float* post_bias,

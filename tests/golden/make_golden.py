@@ -3,7 +3,7 @@
 
 Runs only in the build container (needs oracle/_ref/liblce_ref.so, i.e. the
 reference's own headers compiled from /root/reference by oracle/Makefile). The
-resulting ``lce_golden.npz`` is committed; the GPU box and the CPU test-suite
+resulting ``lce_golden_*.npz`` parts are committed; the GPU box and the CPU test-suite
 only read it. Inputs are regenerated from the recorded seeds by
 ``lce_testlib.make_bconv_case`` so only outputs (or, for the full-size config-1
 case, SHA-256 digests of the outputs) are stored.
@@ -15,6 +15,7 @@ bitpack_test.cc:102-109.
 
 Usage:  python tests/golden/make_golden.py
 """
+import glob
 import hashlib
 import json
 import os
@@ -66,7 +67,7 @@ def bconv_specs():
     for ot in (L.OUT_FLOAT, L.OUT_BITPACKED):
         specs.append((1, 6, 6, 3072, 5, 5, 4, 1, (1, 1), (1, 1), S, 1,
                       L.ACT_RELU, ot))
-    # QuickNet / Bi-RealNet-like layers at reduced spatial size (SURVEY 8d table)
+    # QuickNet / Bi-RealNet-like layers at reduced spatial size
     for c, hw in ((64, 14), (128, 10), (256, 7), (512, 7)):
         specs.append((2, hw, hw, c, 3, 3, c, 1, (1, 1), (1, 1), S, 1, L.ACT_RELU,
                       L.OUT_FLOAT))
@@ -117,7 +118,7 @@ def main():
         index["bconv_zpc"].append({"key": key, "seed": seed,
                                    "spec": [b, h, w, c, fh, fw, co, list(st), list(dl)]})
 
-    # config 1 (BASELINE.json configs[0]): 56x56x256 -> 256, k3 s1 SAME.
+    # config 1: 56x56x256 -> 256, k3 s1 SAME.
     # Outputs are 0.1-3.2 MB each, so only digests are stored.
     n = 0
     for pv in (1, 0):
@@ -148,7 +149,7 @@ def main():
     for rows in (1, 2, 3, 8, 10, 15, 64):
         for cols in (1, 3, 16, 32, 33, 63, 64, 128):
             xf = rng.uniform(-1.5, 1.5, (rows, cols)).astype(np.float32)
-            # sprinkle the special values the bit semantics hinge on (SURVEY 9.3-2)
+            # sprinkle the special values the bit semantics hinge on
             flat = xf.reshape(-1)
             specials = np.array([-0.0, 0.0, np.nan, -np.nan, -1e-30, -1e-45,
                                  1e-45, -np.inf, np.inf], np.float32)
@@ -202,13 +203,21 @@ def main():
                                                                    fw, sh, sw, pad]})
                     n += 1
 
-    np.savez_compressed(os.path.join(HERE, "lce_golden.npz"), **arrays)
+    # parts of under 1 MB each (tests/lce_testlib.py load_golden_arrays merges them)
+    for old in glob.glob(os.path.join(HERE, "lce_golden_*.npz")):
+        os.remove(old)
+    keys, part, n_parts = list(arrays), {}, 0
+    for i, k in enumerate(keys):
+        part[k] = arrays[k]
+        if sum(v.nbytes for v in part.values()) >= 800_000 or i == len(keys) - 1:
+            np.savez_compressed(os.path.join(HERE, f"lce_golden_{n_parts}.npz"), **part)
+            part, n_parts = {}, n_parts + 1
     with open(os.path.join(HERE, "lce_golden.json"), "w") as f:
         json.dump({"generator": "tests/golden/make_golden.py",
                    "reference": "larq/compute-engine e6860fcf core headers via "
                                 "oracle/ref_shim.cc (kReference kernel unless "
                                 "stated)", "index": index}, f, indent=1)
-    sz = os.path.getsize(os.path.join(HERE, "lce_golden.npz"))
+    sz = sum(os.path.getsize(p) for p in glob.glob(os.path.join(HERE, "lce_golden_*.npz")))
     print(f"wrote {len(arrays)} arrays, {sz/1e6:.2f} MB;",
           {k: len(v) for k, v in index.items()})
 

@@ -125,6 +125,16 @@ def ref_build_info():
                          _cache.get("ref_name"), "")}
 
 
+def load_golden_arrays(gold_dir):
+    """The committed golden vectors: tests/golden/lce_golden_*.npz merged into one dict."""
+    import glob
+    arrays = {}
+    for path in sorted(glob.glob(os.path.join(gold_dir, "lce_golden_*.npz"))):
+        with np.load(path) as z:
+            arrays.update({k: z[k] for k in z.files})
+    return arrays
+
+
 def cdiv(a, b):
     return (a + b - 1) // b
 

@@ -1,5 +1,5 @@
 """bench.py's reference arm is CPU-only, so its side of the measurement contract can be checked
-without a GPU: ONE JSON line on stdout with the agreed keys (DESIGN.md section 6)."""
+without a GPU: ONE JSON line on stdout with the agreed keys."""
 import json
 import os
 import subprocess

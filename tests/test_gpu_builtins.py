@@ -4,7 +4,7 @@
 * lce_b200_f32_stem_conv_dw == DEQUANTIZE -> CONV_2D -> DEPTHWISE_CONV_2D run one after the other,
   bit for bit (same accumulation order), over paddings, odd sizes, several column tiles and the
   unaligned loader.
-* the tcgen05 kind::tf32 pointwise convolution (csrc/lce_b200_pw.cuh) against an fp64 product:
+* the wgmma tf32 pointwise convolution (csrc/lce_b200_pw.cuh) against an fp64 product:
   |err| <= 2e-6 * sum|a||w| (the FMA kernels it replaces measure 2-4e-7, the 3-pass split 2-10e-7),
   and its fused LceQuantize words == the signs of its own float output.
 """
@@ -153,7 +153,7 @@ def test_tf32_pointwise_conv_matches_fp64_product(M, K, N, act, with_packed):
                                               (5, 64, 64, PADDING_VALID, 3)])
 def test_tf32_7x7_stem_matches_fp64_convolution(B, H, W, padding, act):
     """CONV_2D 7x7 / stride 2 / 3 -> 64 (Bi-RealNet's stem; csrc/lce_b200_pw.cuh stem7_tf32_kernel:
-    per-thread im2col gather into TMEM, 3-pass tf32) against an fp64 convolution, same error bound
+    per-thread im2col gather into the wgmma A registers, 3-pass tf32) against an fp64 convolution, same error bound
     as the pointwise kernel: 2e-6 * sum|a||w|."""
     torch, lib = _env()
     import torch.nn.functional as F

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C-ABI
+"""GPU parity tests (run on a GPU machine): the CUDA path, called through the C-ABI
 (compute_engine_b200.capi -> liblce_b200.so), against the CPU oracle on the same
 seeded inputs and against the committed golden vectors minted from the reference.
 Bar: bit-exact for bitpacked / int8 / int32 results AND for float results (the
@@ -29,7 +29,7 @@ def capi():
 def golden():
     with open(os.path.join(GOLD_DIR, "lce_golden.json")) as f:
         index = json.load(f)["index"]
-    return index, np.load(os.path.join(GOLD_DIR, "lce_golden.npz"))
+    return index, L.load_golden_arrays(GOLD_DIR)
 
 
 def dev(a):
@@ -138,7 +138,7 @@ def test_bconv_golden_zero_padding_correction(capi, golden):
 
 
 def test_bconv_config1_digests(capi, golden):
-    """BASELINE.json configs[0]: 56x56x256 -> 256, k3 s1 SAME; digests minted from the
+    """A single LceBconv2d 56x56x256 -> 256, k3 s1 SAME; digests minted from the
     reference's BConv2DReference (and equal to its indirect-BGEMM kernel for one-padding)."""
     index, _ = golden
     for e in index["bconv_full"]:
@@ -349,7 +349,7 @@ def test_bconv_fused_residual_and_pack_entry_point(capi):
 
 KERNEL_ENV = {"xor": {"LCE_B200_BCONV_TC": "0", "LCE_B200_BCONV_IMMA": "0"},
               "imma": {"LCE_B200_BCONV_TC": "0", "LCE_B200_BCONV_IMMA": "1"},
-              "tc": {"LCE_B200_BCONV_TC": "1", "LCE_B200_BCONV_IMMA": "1"}}
+              "tc": {"LCE_B200_BCONV_TC": "1", "LCE_B200_BCONV_IMMA": "0"}}
 PATH_INDEX = {"tc": 0, "imma": 1, "xor": 2}
 
 
@@ -362,8 +362,8 @@ def path_counts(capi):
 
 @pytest.mark.parametrize("imma", ["xor", "imma", "tc"])
 def test_bconv_both_inner_products_vs_oracle(capi, imma, monkeypatch):
-    """The three inner products -- XOR+POPC (north_star's), int8 mma.sync, and tcgen05 kind::i8
-    with TMEM accumulators (the default wherever a plan is eligible) -- produce the reference's
+    """The three inner products -- XOR+POPC, int8 mma.sync (the default wherever a plan is
+    eligible), and wgmma s8 with register accumulators -- produce the reference's
     integers: ones / zero padding, stride, dilation, groups, multi-chunk K, ragged M, fused tail.
     lce_b200_path_counts proves which kernel ran."""
     import ctypes as C
@@ -416,7 +416,7 @@ def test_bconv_both_inner_products_vs_oracle(capi, imma, monkeypatch):
     assert np.array_equal(got, L.bgemm(A, W, threads=4))
     ran = [b - a for a, b in zip(before, path_counts(capi))]
     # 8 plain + 8 fused convolutions + 1 BGEMM; the grouped case (2 launches) is outside the
-    # tcgen05 and (64-channel groups) inside the mma.sync kernel's reach
+    # wgmma and (64-channel groups) inside the mma.sync kernel's reach
     want_main = 17 if imma != "tc" else 15
     assert ran[PATH_INDEX[imma]] == want_main, (imma, ran)
     assert sum(ran) == 17, (imma, ran)

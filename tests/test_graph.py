@@ -1,5 +1,5 @@
 """Graph-host tests on synthesised `.tflite` models (the three model families of
-BASELINE.json; topology from the public descriptions, random weights).
+the benchmark; topology from the public descriptions, random weights).
 
 CPU: the flatbuffer writer against an independent pure-Python reader; the C++ reader
 against that reader (and against TFLite's own fixtures when /root/reference is

@@ -1,7 +1,7 @@
 """Graph-host / custom-op shell tests.
 
 CPU part (no GPU): flexbuffer attribute decoding pinned on the byte blobs the
-reference's own tests hold; BASELINE.json configs[0] -- a single LceBconv2d
+reference's own tests hold; a single LceBconv2d
 56x56x256->256 k3 s1 driven init -> prepare -> invoke through the host with the
 oracle-backed registration (bit-exact plumbing); the error behaviour of the CUDA
 registrations' Init / Prepare (which need no device).
@@ -106,7 +106,7 @@ def build_bconv_graph(case, op_name, device_arena):
 
 # ---------------------------- CPU: plumbing ------------------------------- #
 def test_config1_single_bconv_on_cpu_host_is_bit_exact():
-    """BASELINE.json configs[0]."""
+    """A single LceBconv2d 56x56x256 -> 256, k3 s1 SAME."""
     with open(os.path.join(GOLD_DIR, "lce_golden.json")) as f:
         index = json.load(f)["index"]
     for e in index["bconv_full"][:6]:

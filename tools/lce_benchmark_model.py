@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""lce_benchmark_model -- command-line timing of a `.tflite` graph on the B200 path, with
+"""lce_benchmark_model -- command-line timing of a `.tflite` graph on the GPU path, with
 the flags of the reference's benchmark tool (LCE/tflite/benchmark/lce_benchmark_tflite_model.cc:
 41-71 adds --use_reference_bconv / --use_indirect_bgemm to TFLite's benchmark_model flags
 --graph, --num_runs, --warmup_runs, --num_threads, --enable_op_profiling;

@@ -1,9 +1,8 @@
-// tools/microbench.cu -- measured denominators for the integer-pipe roofline
-// (SURVEY section 7: "sustained POPC / LOP3 / IADD3 issue rates per SM ... so
-// BASELINE.md holds measured, not assumed, peaks"). One CTA of 1024 threads per
+// tools/microbench.cu -- measured denominators for the integer-pipe roofline:
+// sustained POPC / LOP3 / IADD3 issue rates per SM. One CTA of 1024 threads per
 // SM; rates are lane-results per SM clock from in-kernel clock64() deltas, so
 // they do not depend on the DVFS state. Also times a plain HBM copy.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench tools/microbench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench tools/microbench.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>

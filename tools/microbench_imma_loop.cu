@@ -3,7 +3,7 @@
 //   mode 0: IMMA only (operands fixed in registers)
 //   mode 1: + B fragments from shared memory (one LDS.64 per two IMMAs, as in the kernel)
 //   mode 2: + A words from shared memory and the bits->bytes expansion (the full inner step)
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench_imma_loop tools/microbench_imma_loop.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench_imma_loop tools/microbench_imma_loop.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>

@@ -1,10 +1,10 @@
-// tools/microbench_mma.cu -- does sm_100a have a faster home for the binary inner product than
+// tools/microbench_mma.cu -- does the GPU have a faster home for the binary inner product than
 // the ALU/XU pipes? Measures, per SM clock (in-kernel clock64, 1024 threads per SM):
 //   (a) legacy mma.sync.m16n8k32 s8 (IMMA)            -> int8 MACs / clk / SM
-//   (b) mma.sync.m16n8k256 b1 and.popc (ptxas lowers it to masked IMMA.U8s + LOP3s: there is
-//       no b1 tensor instruction on sm_100a)           -> binary MACs / clk / SM
+//   (b) mma.sync.m16n8k256 b1 and.popc (on sm_90a a native BMMA.168256.AND.POPC)
+//                                                     -> binary MACs / clk / SM
 //   (c) the kernel's carry-save XOR/POPC tree           -> binary MACs / clk / SM
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench_mma tools/microbench_mma.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench_mma tools/microbench_mma.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>

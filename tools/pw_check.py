@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Check + time the tcgen05 kind::tf32 pointwise convolution (csrc/lce_b200_pw.cuh) against an
+"""Check + time the wgmma tf32 pointwise convolution (csrc/lce_b200_pw.cuh) against an
 fp64 product, then run the same cases on the FMA kernels it replaces (child process with
 LCE_B200_PW_TF32=0) for the error and time comparison. Usage: pw_check.py [quick]"""
 import ctypes as C

@@ -1,4 +1,4 @@
-"""Quick parity + timing sweep of the tcgen05 path against the oracle, one line per case.
+"""Quick parity + timing sweep of the wgmma path against the oracle, one line per case.
 
 Development tool (not collected by pytest): runs from simple to complex so that a failure
 localises itself, reads the kernel's deadlock-watchdog record after every case, and compares each
