@@ -102,7 +102,7 @@ def _dev(t, dtype=None):
 
 
 def path_counts():
-    """Launches per binary inner product so far: [wgmma, legacy mma.sync int8, XOR + POPC]."""
+    """Launches per binary inner product so far: [wgmma, mma.sync (b1 or int8), XOR + POPC]."""
     a = (C.c_uint64 * 3)()
     lib().lce_b200_path_counts(a)
     return [int(v) for v in a]

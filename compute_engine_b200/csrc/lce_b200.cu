@@ -138,9 +138,10 @@ struct GemmCore {
   int32_t* thr = nullptr;
   int32_t* tap_popc = nullptr;  // zero-padding correction table
   size_t smem_bytes = 0;
-  // int8 tensor-pipe inner product (lce_b200_imma.cuh); absent when LCE_B200_BCONV_IMMA=0 or ineligible
-  int32_t* wt_nat = nullptr;    // weights expanded to int8 mma B fragments (8x the packed bytes)
+  // mma.sync inner product (lce_b200_imma.cuh); absent when LCE_B200_BCONV_IMMA=0 or ineligible
+  int32_t* wt_nat = nullptr;    // weights in mma B-fragment order: packed b1, or expanded to int8
   int32_t* wpop = nullptr;      // popcount of each channel's filter row (padded by BN)
+  bool imma_b1 = false;         // b1 fragments (default) or int8 ones (LCE_B200_BCONV_B1=0)
   int imma_Kc_v = 0, imma_chunks = 1;
   size_t imma_smem = 0;
   // wgmma inner product (lce_b200_tc.cuh); absent when LCE_B200_BCONV_TC=0 or ineligible
@@ -181,27 +182,31 @@ int launch_conv_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream
   g_path[2].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_kernel");
 }
-size_t imma_smem_budget(int V) {
-  const int ctas = lce::imma_ctas_per_sm(V);
+size_t imma_smem_budget(int V, bool b1) {
+  const int ctas = b1 ? lce::kB1SmemCtas : lce::imma_ctas_per_sm(V);
   return (227u * 1024u / ctas - 1024u - 256u) & ~size_t{127};
 }
 
-template <int V, int OUT>
+template <int V, int OUT, bool B1>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 static_cast<int>(imma_smem_budget(V))));
-  lce::bconv_imma_kernel<V, OUT><<<grid, lce::kIThreads, smem, s>>>(p);
+                                 static_cast<int>(imma_smem_budget(V, B1))));
+  lce::bconv_imma_kernel<V, OUT, B1><<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
 template <int V>
-int launch_imma_v(int out_type, const lce::ConvKParams& p, dim3 grid, size_t smem,
+int launch_imma_v(int out_type, bool b1, const lce::ConvKParams& p, dim3 grid, size_t smem,
                   cudaStream_t s) {
-  if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT>(p, grid, smem, s);
-  return launch_imma_vo<V, LCE_OUT_RAW_ACC>(p, grid, smem, s);
+  if (b1) {
+    if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, true>(p, grid, smem, s);
+    return launch_imma_vo<V, LCE_OUT_RAW_ACC, true>(p, grid, smem, s);
+  }
+  if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, false>(p, grid, smem, s);
+  return launch_imma_vo<V, LCE_OUT_RAW_ACC, false>(p, grid, smem, s);
 }
 
 template <int V>
@@ -228,13 +233,14 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
   const long long m_tiles = (p.M + lce::kBM - 1) / lce::kBM;
   if (m_tiles > INT_MAX) return fail("too many output pixels");
   if (p.img_words >= (1LL << 31)) return fail("input image too large (>= 2^31 packed words)");
-  // Which inner product: on H100 the mma.sync int8 kernel runs the QuickNet graph faster than
-  // the wgmma kernel (bench.py reports both in one run), so it takes every
-  // plan it can (full 64-channel tiles, float or raw-accumulator output); the wgmma kernel takes
-  // the rest it is eligible for (bitpacked and int8 outputs, other channel counts), XOR + POPC
-  // what is left. All three produce the same int32 accumulators.
+  // Which inner product: on H100 the mma.sync kernel (native b1 BMMA, or int8 fragments with
+  // LCE_B200_BCONV_B1=0) runs the QuickNet graph faster than the wgmma kernel (bench.py reports
+  // both in one run), so it takes every plan it can (full 64-channel tiles, float or
+  // raw-accumulator output); the wgmma kernel takes the rest it is eligible for (bitpacked and
+  // int8 outputs, other channel counts), XOR + POPC what is left. All produce the same int32
+  // accumulators.
   if (c.wt_nat != nullptr && p.vec_store) {
-    // int8 tensor-pipe inner product: 128 x 64 tiles, the same int32 accumulators as bconv_kernel
+    // mma.sync inner product: 128 x 64 tiles, the same int32 accumulators as bconv_kernel
     lce::ConvKParams q = p;
     q.wt = c.wt_nat; q.wpop = c.wpop;
     q.Kc_v = c.imma_Kc_v; q.n_chunks = c.imma_chunks;
@@ -243,9 +249,9 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
     dim3 igrid(static_cast<unsigned>((p.M + lce::kIBM - 1) / lce::kIBM),
                static_cast<unsigned>(c.groups * c.tiles_per_group));
     switch (c.V) {
-      case 4: return launch_imma_v<4>(c.out_type, q, igrid, ismem, s);
-      case 2: return launch_imma_v<2>(c.out_type, q, igrid, ismem, s);
-      default: return launch_imma_v<1>(c.out_type, q, igrid, ismem, s);
+      case 4: return launch_imma_v<4>(c.out_type, c.imma_b1, q, igrid, ismem, s);
+      case 2: return launch_imma_v<2>(c.out_type, c.imma_b1, q, igrid, ismem, s);
+      default: return launch_imma_v<1>(c.out_type, c.imma_b1, q, igrid, ismem, s);
     }
   }
   if (c.tc_ok) {
@@ -617,34 +623,61 @@ int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
   lce::tile_weights_kernel<<<grid_for(total, 256, 1 << 20), 256>>>(
       d_filter, c->wt, c->cout_pg, c->tiles_per_group, c->taps, c->Cw_pg, c->V, c->Kv, total, 0);
   if (launch_check("tile_weights_kernel")) return 1;
-  // int8 tensor-pipe inner product (lce_b200_imma.cuh) where a plan is eligible: full 64-channel
+  // mma.sync inner product (lce_b200_imma.cuh) where a plan is eligible: full 64-channel
   // tiles, float or raw-accumulator output. LCE_B200_BCONV_IMMA=0 leaves every plan to the
-  // wgmma / XOR + POPC kernels (bench.py reports both).
+  // wgmma / XOR + POPC kernels (bench.py reports both). LCE_B200_BCONV_B1=0 keeps the int8
+  // fragments instead of the packed b1 ones; both give the same accumulators.
   const char* imma_env = getenv("LCE_B200_BCONV_IMMA");  // read per plan: A/B in one process
   const bool imma_on = !(imma_env && imma_env[0] == '0');
+  const char* b1_env = getenv("LCE_B200_BCONV_B1");
   if (imma_on && c->cout_pg % lce::kBN == 0 &&
       (c->out_type == LCE_OUT_FLOAT || c->out_type == LCE_OUT_RAW_ACC)) {
-    const long long Kw = static_cast<long long>(c->taps) * c->Cw_pg;
-    const long long xtotal = static_cast<long long>(c->groups) * c->tiles_per_group * Kw * 256;
-    CUDA_OK(cudaMalloc(&c->wt_nat, xtotal * 8));
-    lce::expand_weights_imma_kernel<<<grid_for(xtotal, 256, 1 << 22), 256>>>(
-        d_filter, reinterpret_cast<uint2*>(c->wt_nat), c->cout_pg, c->tiles_per_group, c->taps,
-        c->Cw_pg, xtotal);
-    if (launch_check("expand_weights_imma_kernel")) return 1;
+    const int Kw = c->taps * c->Cw_pg;
+    c->imma_b1 = !(b1_env && b1_env[0] == '0');
+    const size_t budget = imma_smem_budget(c->V, c->imma_b1);
+    if (c->imma_b1) {
+      const int n_slices = cdiv(Kw, 8);  // 8-word k-slices, the last one padded to 4 or 8 words
+      const long long total = static_cast<long long>(c->groups) * c->tiles_per_group * n_slices * 256;
+      CUDA_OK(cudaMalloc(&c->wt_nat, total * 8));
+      lce::pack_weights_b1_kernel<<<grid_for(total, 256, 1 << 22), 256>>>(
+          d_filter, reinterpret_cast<uint2*>(c->wt_nat), c->cout_pg, c->tiles_per_group, Kw,
+          n_slices, total);
+      if (launch_check("pack_weights_b1_kernel")) return 1;
+      // K staging: one chunk when it fits kB1SmemCtas CTAs per SM, else a two-deep ring of
+      // chunks of whole 8-word slices
+      const int Kvp = lce::b1_padded_vectors(c->Kv, c->V);
+      const size_t slice_bytes = lce::kB1BytesPerSlice;
+      if (n_slices * slice_bytes <= budget) {
+        c->imma_chunks = 1;
+        c->imma_Kc_v = Kvp;
+        c->imma_smem = n_slices * slice_bytes;
+      } else {
+        const int ring_slices = std::max(static_cast<int>(budget / (2 * slice_bytes)), 1);
+        c->imma_chunks = cdiv(n_slices, ring_slices);
+        const int chunk_slices = cdiv(n_slices, c->imma_chunks);
+        c->imma_Kc_v = chunk_slices * 8 / c->V;
+        c->imma_smem = 2 * chunk_slices * slice_bytes;
+      }
+    } else {
+      const long long xtotal = static_cast<long long>(c->groups) * c->tiles_per_group * Kw * 256;
+      CUDA_OK(cudaMalloc(&c->wt_nat, xtotal * 8));
+      lce::expand_weights_imma_kernel<<<grid_for(xtotal, 256, 1 << 22), 256>>>(
+          d_filter, reinterpret_cast<uint2*>(c->wt_nat), c->cout_pg, c->tiles_per_group, c->taps,
+          c->Cw_pg, xtotal);
+      if (launch_check("expand_weights_imma_kernel")) return 1;
+      // K staging: everything in one chunk when it fits the CTA's shared-memory share, else a
+      // two-deep ring of equal chunks. 3 CTAs per SM for uint4 operands, 4 otherwise (registers).
+      const int single_max = static_cast<int>(budget / lce::kIBytesPerWord) / c->V;      // vectors
+      const int ring_max = static_cast<int>(budget / (2 * lce::kIBytesPerWord)) / c->V;
+      c->imma_chunks = c->Kv <= single_max ? 1 : cdiv(c->Kv, std::max(ring_max, 1));
+      c->imma_Kc_v = cdiv(c->Kv, c->imma_chunks);
+      c->imma_smem = static_cast<size_t>(c->imma_Kc_v) * c->V * lce::kIBytesPerWord *
+                     (c->imma_chunks > 1 ? 2 : 1);  // two-deep ring
+    }
     CUDA_OK(cudaMalloc(&c->wpop, static_cast<size_t>(c->cout + lce::kBN) * 4));
     CUDA_OK(cudaMemset(c->wpop, 0, static_cast<size_t>(c->cout + lce::kBN) * 4));
-    lce::tap_popc_kernel<<<cdiv(c->cout, 256), 256>>>(d_filter, c->wpop, c->cout, 1,
-                                                      c->taps * c->Cw_pg);
+    lce::tap_popc_kernel<<<cdiv(c->cout, 256), 256>>>(d_filter, c->wpop, c->cout, 1, Kw);
     if (launch_check("tap_popc_kernel")) return 1;
-    // K staging: everything in one chunk when it fits the CTA's shared-memory share, else a
-    // two-deep ring of equal chunks. 3 CTAs per SM for uint4 operands, 4 otherwise (registers).
-    const size_t budget = imma_smem_budget(c->V);
-    const int single_max = static_cast<int>(budget / lce::kIBytesPerWord) / c->V;      // vectors
-    const int ring_max = static_cast<int>(budget / (2 * lce::kIBytesPerWord)) / c->V;
-    c->imma_chunks = c->Kv <= single_max ? 1 : cdiv(c->Kv, std::max(ring_max, 1));
-    c->imma_Kc_v = cdiv(c->Kv, c->imma_chunks);
-    c->imma_smem = static_cast<size_t>(c->imma_Kc_v) * c->V * lce::kIBytesPerWord *
-                   (c->imma_chunks > 1 ? 2 : 1);  // two-deep ring
   }
   if (build_tc_weights(c, d_filter, want_tap_popc)) return 1;
   if (want_tap_popc) {

@@ -1,4 +1,4 @@
-// lce_b200_imma.cuh -- the binary convolution's inner product on the int8 tensor pipe.
+// lce_b200_imma.cuh -- the binary convolution's inner product on the mma.sync tensor pipe.
 // The default for every plan with full 64-channel tiles and float / raw-accumulator output (the
 // three model families' LceBconv2d layers, the BGEMM sweep): on H100 it runs the QuickNet graph
 // faster than the wgmma kernel of lce_b200_tc.cuh, which takes the other plans it is eligible
@@ -6,10 +6,18 @@
 // kernel of lce_b200_kernels.cuh. All produce the reference's integers bit for bit
 // (tests/test_gpu_parity.py runs the same cases through each); bench.py reports them side by side.
 //
+// Two inner products share the kernel's gather, TMA weight staging, zero-padding correction and
+// epilogue (template parameter B1):
+//  - b1 (default): the native binary instruction, mma.sync m16n8k256 b1 and.popc (SASS
+//    BMMA.168256.AND.POPC; .xor.popc is lowered to two of them). Operands stay packed, so the
+//    weights cost 256 B per K word per 64-channel tile in L2 and shared memory instead of 2048 B,
+//    and one BMMA does the work of 8 IMMA.16832. Measured on an H100 80GB HBM3 at a 400 W power
+//    limit (tools/microbench_mma.cu): 19.9 k binary MACs / clk / SM against IMMA's 2.5 k int8
+//    MACs / clk / SM. See compute_chunk_b1 for the identity and fragment layout.
+//  - int8 (LCE_B200_BCONV_B1=0), described below, kept for A/B runs.
+//
 // The int8 tensor pipe (mma.sync.m16n8k32, SASS IMMA.16832) does the XOR + POPC sum as a signed
-// dot product. sm_90a also has a native b1 instruction (mma.sync ... b1 and.popc assembles to
-// BMMA.168256.AND.POPC); a b1 path has not been evaluated on H100. HBM, L2 and shared memory
-// keep the reference's bitpacked words;
+// dot product. HBM, L2 and shared memory keep the reference's bitpacked words;
 // only registers ever hold bytes. With activation bits a in {0,1} (u8) and weight bits mapped
 // to w' = +1 / -1 (s8):
 //     popc(a ^ w) = popc(w) + sum_k a_k * w'_k
@@ -47,6 +55,14 @@ constexpr int kIBytesPerWord = kIBM * 4 + 8 * 32 * 8;  // smem per K word: packe
 // K is staged in one chunk when it fits, else through a TWO-deep ring: chunk c+1 is gathered /
 // TMA-copied while chunk c is multiplied. The host sizes the chunks (imma_smem_budget):
 // 3 CTAs per SM for the uint4 instances (153 registers), 4 for the narrower ones (128).
+// b1 inner product: smem per 8-word k-slice (A rows [128][8 words] + B fragments [8][32] x 8 B),
+// 768 B per K word. The host stages K in one chunk when it fits kB1SmemCtas CTAs per SM, which
+// holds for every QuickNet layer; the register cap allows kB1Ctas.
+constexpr int kB1BytesPerSlice = kIBM * 32 + 8 * 32 * 8;
+constexpr int kB1Ctas = 4;
+constexpr int kB1SmemCtas = 2;
+// K words padded up to the b1 instructions' granularity (4 words = m16n8k128), in vectors of V
+__host__ __device__ constexpr int b1_padded_vectors(int Kv, int V) { return ((Kv * V + 3) & ~3) / V; }
 
 // byte `tig` of w -> two registers of four u8 each: bit i of the low / high nibble -> byte i with
 // value 2^i (sel = tig * 0x1111 replicates the byte; 4 ALU instructions, no multiplies)
@@ -143,9 +159,107 @@ __device__ __forceinline__ void compute_chunk_imma(const typename VecT<V>::T* A_
   }
 }
 
+// ---- b1 inner product: popc(a ^ w) = popc(w) + popc(a) - 2 * popc(a & w) ----
+// BMMA.168256.AND.POPC sums popc(a & w) over 256 k; one more per m16 tile against an all-ones B
+// fragment gives popc(a) per pixel row. Operands stay packed: A rows [k-slice][pixel][8 words],
+// thread (gid, tig) holds words 2*tig (a0 / a1, b0) and 2*tig + 1 (a2 / a3, b1) of its rows. A
+// K tail of 4 words runs as m16n8k128, thread tig holding word tig. Padding words are 0 in A and
+// B and add nothing.
+__device__ __forceinline__ void bmma_k256(int (&c)[4], const uint32_t (&a)[4], uint32_t b0,
+                                          uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k256.row.col.s32.b1.b1.s32.and.popc {%0,%1,%2,%3}, {%4,%5,%6,%7}, "
+      "{%8,%9}, {%0,%1,%2,%3};"
+      : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void bmma_k128(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t b0) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k128.row.col.s32.b1.b1.s32.and.popc {%0,%1,%2,%3}, {%4,%5}, {%6}, "
+      "{%0,%1,%2,%3};"
+      : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+      : "r"(a0), "r"(a1), "r"(b0));
+}
+
+// Plan-time: wtb[n_tile][k-slice][ns / 2][lane][ns & 1] = {b0, b1}, the packed filter words of
+// channel ns*8 + lane/4 that `lane` feeds to the b1 mma (see above); two neighbouring sub-tiles
+// side by side so one 128-bit LDS fetches both. A k128 tail slice has {word tig, 0}. Words past
+// Kw and channels past the group's end are 0.
+__global__ void pack_weights_b1_kernel(const int32_t* __restrict__ filter, uint2* __restrict__ wtb,
+                                       int cout_pg, int tiles_per_group, int Kw, int n_slices,
+                                       long long total) {
+  const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (idx >= total) return;
+  const int ns = static_cast<int>(((idx >> 6) & 3) * 2 + (idx & 1));
+  const int lane = static_cast<int>((idx >> 1) & 31);
+  const long long r = idx >> 8;
+  const int s = static_cast<int>(r % n_slices);
+  const int nt = static_cast<int>(r / n_slices);
+  const int g = nt / tiles_per_group, tg = nt - g * tiles_per_group;
+  const int ch = tg * kBN + ns * 8 + (lane >> 2);
+  const int tig = lane & 3;
+  const bool tail = s * 8 + 4 >= ((Kw + 3) & ~3);
+  const int k0 = s * 8 + (tail ? tig : 2 * tig);
+  const int32_t* row = filter + (static_cast<long long>(g) * cout_pg + ch) * Kw;
+  const bool ch_ok = ch < cout_pg;
+  const uint32_t w0 = ch_ok && k0 < Kw ? static_cast<uint32_t>(row[k0]) : 0u;
+  const uint32_t w1 = ch_ok && !tail && k0 + 1 < Kw ? static_cast<uint32_t>(row[k0 + 1]) : 0u;
+  wtb[idx] = make_uint2(w0, w1);
+}
+
+// acc += popc(a & w) and pa += popc(a) over `words` K words (a multiple of 4) of one chunk
+__device__ __forceinline__ void compute_chunk_b1(const uint32_t* A_s, const uint2* B_s, int words,
+                                                 int warp, int gid, int tig, int lane,
+                                                 int (&acc)[2][8][4], int (&pa)[2][4]) {
+  const uint4* b4 = reinterpret_cast<const uint4*>(B_s) + lane;
+  const uint2* a2 = reinterpret_cast<const uint2*>(A_s) + (warp * 32 + gid) * 4 + tig;
+  const int full = words >> 3;
+#pragma unroll 2
+  for (int s = 0; s < full; ++s) {
+    uint32_t a[2][4];
+#pragma unroll
+    for (int ms = 0; ms < 2; ++ms) {
+      const uint2 lo = a2[(s * kIBM + ms * 16) * 4];
+      const uint2 hi = a2[(s * kIBM + ms * 16 + 8) * 4];
+      a[ms][0] = lo.x; a[ms][1] = hi.x; a[ms][2] = lo.y; a[ms][3] = hi.y;
+    }
+#pragma unroll
+    for (int np = 0; np < 4; ++np) {
+      const uint4 b = b4[(s * 4 + np) * 32];
+      bmma_k256(acc[0][2 * np], a[0], b.x, b.y);
+      bmma_k256(acc[1][2 * np], a[1], b.x, b.y);
+      bmma_k256(acc[0][2 * np + 1], a[0], b.z, b.w);
+      bmma_k256(acc[1][2 * np + 1], a[1], b.z, b.w);
+    }
+    bmma_k256(pa[0], a[0], ~0u, ~0u);
+    bmma_k256(pa[1], a[1], ~0u, ~0u);
+  }
+  if (words & 4) {
+    const uint32_t* a1 = A_s + (full * kIBM + warp * 32 + gid) * 8 + tig;
+    uint32_t lo[2], hi[2];
+#pragma unroll
+    for (int ms = 0; ms < 2; ++ms) {
+      lo[ms] = a1[(ms * 16) * 8];
+      hi[ms] = a1[(ms * 16 + 8) * 8];
+    }
+#pragma unroll
+    for (int np = 0; np < 4; ++np) {
+      const uint4 b = b4[(full * 4 + np) * 32];
+#pragma unroll
+      for (int ms = 0; ms < 2; ++ms) {
+        bmma_k128(acc[ms][2 * np], lo[ms], hi[ms], b.x);
+        bmma_k128(acc[ms][2 * np + 1], lo[ms], hi[ms], b.z);
+      }
+    }
+#pragma unroll
+    for (int ms = 0; ms < 2; ++ms) bmma_k128(pa[ms], lo[ms], hi[ms], ~0u);
+  }
+}
+
 // SAME padding with pad value 0 (reference.h:100-103), for this kernel's accumulator layout:
-// an out-of-bounds tap contributes channels_in_per_group / 2 instead of popc(0 ^ w) -- times 8,
-// the accumulators' scale.
+// an out-of-bounds tap contributes channels_in_per_group / 2 instead of popc(0 ^ w) -- times
+// 2^S, the accumulators' scale (8 for the int8 inner product, 1 for b1).
+template <int S>
 __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
                                                          int (&acc)[2][8][4], long long m0,
                                                          int c_tile, int warp, int gid, int tig) {
@@ -173,9 +287,10 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns) {
             const int c = c_tile + ns * 8 + tig * 2;
-            acc[ms][ns][h * 2] += 8 * (p.zp_half - p.tap_popc[static_cast<size_t>(c) * taps + t]);
+            acc[ms][ns][h * 2] +=
+                (1 << S) * (p.zp_half - p.tap_popc[static_cast<size_t>(c) * taps + t]);
             acc[ms][ns][h * 2 + 1] +=
-                8 * (p.zp_half - p.tap_popc[static_cast<size_t>(c + 1) * taps + t]);
+                (1 << S) * (p.zp_half - p.tap_popc[static_cast<size_t>(c + 1) * taps + t]);
           }
         }
       }
@@ -184,8 +299,9 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 }
 
 // Accumulator (ms, ns, e) of thread (gid, tig): pixel m0 + warp*32 + ms*16 + (e/2)*8 + gid,
-// channel c_tile + ns*8 + tig*2 + (e & 1). Full 64-channel tiles only (host-checked).
-template <int OUT>
+// channel c_tile + ns*8 + tig*2 + (e & 1), at scale 2^S. Full 64-channel tiles only
+// (host-checked).
+template <int OUT, int S>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
                                               int tig) {
@@ -219,7 +335,7 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns)
             *reinterpret_cast<int2*>(o + ns * 8) =
-                make_int2(acc[ms][ns][h * 2] >> 3, acc[ms][ns][h * 2 + 1] >> 3);
+                make_int2(acc[ms][ns][h * 2] >> S, acc[ms][ns][h * 2 + 1] >> S);
         }
         continue;
       }
@@ -228,11 +344,16 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
         float y[16];
 #pragma unroll
         for (int ns = 0; ns < 8; ++ns) {
-          // accumulators hold 8 * acc: OutputTransform's (acc << 1) is (acc8 >> 2), exactly
-          y[2 * ns] = transform_float_x2(acc[ms][ns][h * 2] >> 2, p.clamp_min, p.clamp_max,
-                                         mul_r[ns].x, bias_r[ns].x);
-          y[2 * ns + 1] = transform_float_x2(acc[ms][ns][h * 2 + 1] >> 2, p.clamp_min, p.clamp_max,
-                                            mul_r[ns].y, bias_r[ns].y);
+          // OutputTransform's (acc << 1); at scale 8 that is (acc8 >> 2), exactly
+          int x0 = acc[ms][ns][h * 2], x1 = acc[ms][ns][h * 2 + 1];
+          if constexpr (S > 0) {
+            x0 >>= S - 1; x1 >>= S - 1;
+          } else {
+            x0 <<= 1; x1 <<= 1;
+          }
+          y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mul_r[ns].x, bias_r[ns].x);
+          y[2 * ns + 1] =
+              transform_float_x2(x1, p.clamp_min, p.clamp_max, mul_r[ns].y, bias_r[ns].y);
         }
         if (has_res) {
           // (A TMA-staged copy of the shortcut tile was measured slower on every layer: the
@@ -281,12 +402,15 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
   }
 }
 
-template <int V, int OUT>
-__global__ void __launch_bounds__(kIThreads, imma_ctas_per_sm(V))
+// B1 selects the inner product: packed b1 fragments (accumulators at scale 1) or int8 ones
+// (scale 8). Both produce the same int32 accumulators.
+template <int V, int OUT, bool B1>
+__global__ void __launch_bounds__(kIThreads, B1 ? kB1Ctas : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
   using Vec = typename VecT<V>::T;
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  // two buffers of { A: [Kc_v][128] packed vectors, B: [Kc_v*V][8][32] int8 fragments }
+  // two buffers of { A: [Kc_v][128] packed vectors, B: [Kc_v*V][8][32] int8 fragments }, or for
+  // B1 { A: [slices][128][8 words], B: [slices][8][32] b1 fragments }
   __shared__ __align__(8) uint64_t wbar[2];
 
   const int tid = threadIdx.x;
@@ -297,6 +421,10 @@ bconv_imma_kernel(const ConvKParams p) {
   const int tg = nt - g * p.tiles_per_group;
   const long long m0 = static_cast<long long>(blockIdx.x) * kIBM;
   const int c_tile = g * p.cout_pg + tg * kBN;
+  // B1: K runs to the padded vector count, in 8-word slices (the last may be a 4-word one)
+  const int Kv_end = B1 ? b1_padded_vectors(p.Kv, V) : p.Kv;
+  const int n_slices = (Kv_end * V + 7) >> 3;
+  const int chunk_slices = (p.Kc_v * V + 7) >> 3;
 
   if (tid == 0) {
     mbar_init(&wbar[0], 1);
@@ -305,11 +433,14 @@ bconv_imma_kernel(const ConvKParams p) {
   }
   __syncthreads();
 
-  // accumulators start at 8 * popc(filter row): acc8 = 8 * (popc(w) + sum a * w')
+  // int8: accumulators start at 8 * popc(filter row): acc8 = 8 * (popc(w) + sum a * w').
+  // B1: they sum popc(a & w), and pa sums popc(a) of each row.
   int acc[2][8][4];
+  int pa[2][4] = {};
 #pragma unroll
   for (int ns = 0; ns < 8; ++ns) {
-    const int2 pw = *reinterpret_cast<const int2*>(p.wpop + c_tile + ns * 8 + tig * 2);
+    const int2 pw = B1 ? make_int2(0, 0)
+                       : *reinterpret_cast<const int2*>(p.wpop + c_tile + ns * 8 + tig * 2);
 #pragma unroll
     for (int ms = 0; ms < 2; ++ms) {
       acc[ms][ns][0] = pw.x * 8; acc[ms][ns][1] = pw.y * 8;
@@ -324,21 +455,27 @@ bconv_imma_kernel(const ConvKParams p) {
     }
   }
 
-  const size_t chunk_bytes = static_cast<size_t>(p.Kc_v) * V * kIBytesPerWord;
+  const size_t a_bytes = B1 ? static_cast<size_t>(chunk_slices) * kIBM * 32
+                            : static_cast<size_t>(p.Kc_v) * kIBM * sizeof(Vec);
+  const size_t chunk_bytes = B1 ? static_cast<size_t>(chunk_slices) * kB1BytesPerSlice
+                                : static_cast<size_t>(p.Kc_v) * V * kIBytesPerWord;
   auto stage = [&](int ch) {
     unsigned char* base = smem_raw + (ch & 1) * chunk_bytes;
     Vec* A_b = reinterpret_cast<Vec*>(base);
-    uint2* B_b = reinterpret_cast<uint2*>(A_b + static_cast<size_t>(p.Kc_v) * kIBM);
+    uint2* B_b = reinterpret_cast<uint2*>(base + a_bytes);
     const int kv0 = ch * p.Kc_v;
-    const int kv1 = min(kv0 + p.Kc_v, p.Kv);
+    const int kv1 = min(kv0 + p.Kc_v, Kv_end);
     if (tid == 0) {
-      const uint32_t bytes = static_cast<uint32_t>(kv1 - kv0) * V * (8 * 32 * 8);
+      // B fragments: 8 * 32 uint2 per K word (int8) or per 8-word slice (b1)
+      const size_t frag0 = B1 ? static_cast<size_t>(nt) * n_slices + (kv0 * V >> 3)
+                              : (static_cast<size_t>(nt) * p.Kv + kv0) * V;
+      const uint32_t nfrag = B1 ? static_cast<uint32_t>(((kv1 - kv0) * V + 7) >> 3)
+                                : static_cast<uint32_t>(kv1 - kv0) * V;
+      const uint32_t bytes = nfrag * (8 * 32 * 8);
       mbar_arrive_expect_tx(&wbar[ch & 1], bytes);
-      bulk_g2s(B_b, reinterpret_cast<const uint2*>(p.wt) +
-                        (static_cast<size_t>(nt) * p.Kv + kv0) * V * (8 * 32),
-               bytes, &wbar[ch & 1]);
+      bulk_g2s(B_b, reinterpret_cast<const uint2*>(p.wt) + frag0 * (8 * 32), bytes, &wbar[ch & 1]);
     }
-    gather_tile<V, kIBM, kIThreads>(p, A_b, m0, g, kv0, kv1, tid);
+    gather_tile<V, kIBM, kIThreads, B1>(p, A_b, m0, g, kv0, kv1, tid);
     cp_async_commit();
   };
   stage(0);
@@ -350,14 +487,32 @@ bconv_imma_kernel(const ConvKParams p) {
     mbar_wait(&wbar[ch & 1], (ch >> 1) & 1);
     __syncthreads();
     unsigned char* base = smem_raw + (ch & 1) * chunk_bytes;
-    const Vec* A_b = reinterpret_cast<const Vec*>(base);
-    const uint2* B_b = reinterpret_cast<const uint2*>(A_b + static_cast<size_t>(p.Kc_v) * kIBM);
+    const uint2* B_b = reinterpret_cast<const uint2*>(base + a_bytes);
     const int kv0 = ch * p.Kc_v;
-    compute_chunk_imma<V>(A_b, B_b, min(kv0 + p.Kc_v, p.Kv) - kv0, warp, gid, tig, lane, acc);
+    const int nkv = min(kv0 + p.Kc_v, Kv_end) - kv0;
+    if constexpr (B1)
+      compute_chunk_b1(reinterpret_cast<const uint32_t*>(base), B_b, nkv * V, warp, gid, tig,
+                       lane, acc, pa);
+    else
+      compute_chunk_imma<V>(reinterpret_cast<const Vec*>(base), B_b, nkv, warp, gid, tig, lane,
+                            acc);
     __syncthreads();
   }
-  if (p.tap_popc != nullptr) zero_pad_correction_imma(p, acc, m0, c_tile, warp, gid, tig);
-  epilogue_imma<OUT>(p, acc, m0, c_tile, warp, gid, tig);
+  constexpr int S = B1 ? 0 : 3;
+  if constexpr (B1) {
+    // popc(a ^ w) = popc(w) + popc(a) - 2 * popc(a & w); out-of-bounds taps (a = 0) give popc(w)
+#pragma unroll
+    for (int ns = 0; ns < 8; ++ns) {
+      const int2 pw = *reinterpret_cast<const int2*>(p.wpop + c_tile + ns * 8 + tig * 2);
+#pragma unroll
+      for (int ms = 0; ms < 2; ++ms)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          acc[ms][ns][e] = (e & 1 ? pw.y : pw.x) + pa[ms][e] - 2 * acc[ms][ns][e];
+    }
+  }
+  if (p.tap_popc != nullptr) zero_pad_correction_imma<S>(p, acc, m0, c_tile, warp, gid, tig);
+  epilogue_imma<OUT, S>(p, acc, m0, c_tile, warp, gid, tig);
 }
 
 }  // namespace lce

@@ -268,7 +268,9 @@ __device__ __forceinline__ void split_pixel(const ConvKParams& p, long long m, l
 
 // Gather one K chunk of the im2col rows of tile `m0` into A_buf[kv - kv0][pixel] with
 // zero-filling cp.async. Thread t handles pixel t % BM and every second k-vector.
-template <int V, int BM_ = kBM, int NT_ = kThreads>
+// kSliceRows: the layout is A_buf[k-slice][pixel][8 words] instead (k = (kv - kv0) * V words into
+// the chunk), and vectors at kv >= p.Kv -- the K tail padding -- are zero-filled.
+template <int V, int BM_ = kBM, int NT_ = kThreads, bool kSliceRows = false>
 __device__ __forceinline__ void gather_tile(const ConvKParams& p, typename VecT<V>::T* A_buf,
                                             long long m0, int g, int kv0, int kv1, int tid) {
   using Vec = typename VecT<V>::T;
@@ -296,12 +298,18 @@ __device__ __forceinline__ void gather_tile(const ConvKParams& p, typename VecT<
   for (; kv < kv1; kv += kStep, dst += kStep * BM_ * static_cast<uint32_t>(sizeof(Vec))) {
     const int iy = iy0 + fy * p.dh;
     const int ix = ix0 + fx * p.dw;
-    const bool inside = pix_valid && static_cast<unsigned>(iy) < static_cast<unsigned>(p.H) &&
+    const bool inside = pix_valid && (!kSliceRows || kv < p.Kv) &&
+                        static_cast<unsigned>(iy) < static_cast<unsigned>(p.H) &&
                         static_cast<unsigned>(ix) < static_cast<unsigned>(p.W);
     // offsets inside one image fit 32 bits (img_words < 2^31)
     const int off = (iy * p.W + ix) * p.Cw_total + cv * V;
     const int32_t* src = inside ? img + off : p.in;
-    cp_async_zfill_u32<V * 4>(dst, src, inside ? V * 4 : 0);
+    uint32_t d = dst;
+    if constexpr (kSliceRows) {
+      const uint32_t k = static_cast<uint32_t>(kv - kv0) * V;
+      d = smem_u32(A_buf) + (k >> 3) * (BM_ * 32) + lp * 32 + (k & 7) * 4;
+    }
+    cp_async_zfill_u32<V * 4>(d, src, inside ? V * 4 : 0);
     cv += kStep;
     while (cv >= p.CwV) {
       cv -= p.CwV;

@@ -135,7 +135,7 @@ void lce_b200_bgemm_destroy(lce_b200_bgemm* plan);
  * `gpu_launches`). */
 uint64_t lce_b200_launch_count(void);
 /* Diagnostics. path_counts: inner-product launches so far by kernel family
- * {wgmma (lce_b200_tc.cuh), mma.sync int8 (lce_b200_imma.cuh), XOR + POPC
+ * {wgmma (lce_b200_tc.cuh), mma.sync b1 or int8 (lce_b200_imma.cuh), XOR + POPC
  * (lce_b200_kernels.cuh)} -- the tests use it to prove which kernel ran.
  * tc_debug: the wgmma kernel's deadlock-watchdog record; out[7] != 0 means a
  * wait timed out ({barrier tag, block, thread, parity, count} in out[0..4]);

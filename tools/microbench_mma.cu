@@ -95,7 +95,7 @@ int main() {
   int sms = prop.multiProcessorCount;
   printf("{\"device\": \"%s\", \"sms\": %d}\n", prop.name, sms);
   run<0>("mma.sync m16n8k32 s8 (legacy IMMA), int8 MACs", 16.0 * 8 * 32, 0, sms);
-  run<1>("mma.sync m16n8k256 b1 and.popc (ptxas emulation), binary MACs", 16.0 * 8 * 256, 0, sms);
+  run<1>("mma.sync m16n8k256 b1 and.popc (native BMMA on sm_90a), binary MACs", 16.0 * 8 * 256, 0, sms);
   run<2>("carry-save XOR/POPC tree (this kernel), binary MACs", 0, 8.0 * 4, sms);
   return 0;
 }
