@@ -44,6 +44,17 @@ class BMaxPoolDesc(C.Structure):
         "stride_h", "stride_w", "padding")]
 
 
+class ChainDesc(C.Structure):
+    """lce_chain_desc: device pointers of the per-channel vectors; None = the op is absent."""
+    _fields_ = [("shift_in", C.c_void_p), ("alpha", C.c_void_p), ("shift_out", C.c_void_p),
+                ("sign_shift", C.c_void_p)]
+
+
+def _chain_desc(shift_in=None, alpha=None, shift_out=None, sign_shift=None):
+    vecs = [None if v is None else _dev(v, torch.float32) for v in (shift_in, alpha, shift_out, sign_shift)]
+    return ChainDesc(*[None if v is None else v.data_ptr() for v in vecs]), vecs
+
+
 class BgemmEpilogue(C.Structure):
     _fields_ = [("out_type", C.c_int32), ("clamp_min", C.c_int32),
                 ("clamp_max", C.c_int32), ("multiplier", C.c_void_p),
@@ -56,7 +67,9 @@ EXPORTS = [
     "lce_b200_bmaxpool", "lce_b200_bconv2d_out_shape", "lce_b200_bconv2d_create",
     "lce_b200_bconv2d_set_input_shape", "lce_b200_bconv2d_get_desc",
     "lce_b200_bconv2d_set_zero_padding_mode", "lce_b200_path_counts", "lce_b200_tc_debug",
-    "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
+    "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_fused_chain",
+    "lce_b200_f32_chain_sign",
+    "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
 ]
@@ -166,6 +179,23 @@ def bmaxpool(x: torch.Tensor, filter_hw, stride_hw, padding=PADDING_SAME):
     return out
 
 
+def chain_sign(x: torch.Tensor, shift_in=None, alpha=None, shift_out=None, sign_shift=None,
+               out=True, packed=True, channels=None):
+    """ReActNet's per-channel chain (RPReLU, then RSign's signs) over the last axis of x, or over
+    `channels` trailing elements (PRELU with a trailing-shape alpha). Returns (out | None,
+    packed | None)."""
+    x = _dev(x, torch.float32)
+    ch = channels or x.shape[-1]
+    rows = x.numel() // ch
+    desc, _keep = _chain_desc(shift_in, alpha, shift_out, sign_shift)
+    o = torch.empty_like(x) if out else None
+    pk = torch.empty(x.shape[:-1] + (cdiv(x.shape[-1], 32),), dtype=torch.int32,
+                     device=x.device) if packed else None
+    _check(lib().lce_b200_f32_chain_sign(_p(x), C.byref(desc), C.c_int64(rows), C.c_int(ch), _p(o),
+                                         _p(pk), _stream()))
+    return o, pk
+
+
 class BConv2d:
     """LceBconv2d plan: constructor = Init + Prepare + OneTimeSetup
     (LCE/tflite/kernels/bconv2d.cc:85-392), ``__call__`` = Eval (:551-564)."""
@@ -234,6 +264,21 @@ class BConv2d:
         else:
             raise LceError(f"LceBconv2d: unsupported input type {x.dtype}")
         return out
+
+    def run_fused_chain(self, x: torch.Tensor, residual=None, add_activation=0, shift_in=None,
+                        alpha=None, shift_out=None, sign_shift=None, packed=True):
+        """lce_b200_bconv2d_run_fused_chain on bitpacked x: returns (float out, packed signs | None)."""
+        x = _dev(x, torch.int32)
+        if tuple(x.shape[:3]) != (self.desc.batch, self.desc.in_h, self.desc.in_w):
+            self.set_input_shape(*x.shape[:3])
+        out = self._alloc(x, None)
+        pk = torch.empty(out.shape[:3] + (cdiv(out.shape[3], 32),), dtype=torch.int32,
+                         device=x.device) if packed else None
+        res = None if residual is None else _dev(residual, torch.float32)
+        desc, _keep = _chain_desc(shift_in, alpha, shift_out, sign_shift)
+        _check(lib().lce_b200_bconv2d_run_fused_chain(self._h, _p(x), _p(res), C.c_int(add_activation),
+                                                      C.byref(desc), _p(out), _p(pk), _stream()))
+        return out, pk
 
     def run_host(self, x_host, out_host):
         """Host-buffer call (numpy arrays): H2D + kernel + D2H, synchronised."""

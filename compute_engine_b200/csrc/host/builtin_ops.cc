@@ -1,5 +1,5 @@
 // builtin_ops.cc -- TfLiteRegistrations for the float builtins QuickNet /
-// QuickNetLarge / Bi-RealNet-18 use around the binary path, backed by
+// QuickNetLarge / Bi-RealNet-18 / ReActNet-A use around the binary path, backed by
 // the fp32 CUDA kernels of lce_b200_builtins.cu. Shape inference follows TFLite's
 // builtin kernels (tensorflow/lite/kernels/{conv,depthwise_conv,pooling,add,mul,
 // fully_connected,softmax,reduce,reshape,activations}.cc). Device arena only.
@@ -362,6 +362,88 @@ TfLiteStatus ReluInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// ----------------------------------- PRELU ----------------------------------- //
+// out = x >= 0 ? x : x * alpha (TF/lite/kernels/internal/reference/prelu.h). Alpha broadcasts by
+// element index modulo its size, so its shape with leading 1s dropped must be x's trailing
+// dimensions (per-channel [1, 1, C] among them). Returns that size, or 0 for any other shape.
+int64_t PreluAlphaCount(const TfLiteTensor* x, const TfLiteTensor* a) {
+  int lead = 0;
+  while (lead < a->dims->size && a->dims->data[lead] == 1) ++lead;
+  const int r = a->dims->size - lead;
+  if (r > x->dims->size) return 0;
+  int64_t n = 1;
+  for (int i = 0; i < r; ++i) {
+    if (a->dims->data[lead + i] != x->dims->data[x->dims->size - r + i]) return 0;
+    n *= a->dims->data[lead + i];
+  }
+  return n;
+}
+TfLiteStatus PreluPrepare(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const TfLiteTensor* a = T(c, n->inputs, 1);
+  B_ENSURE(c, x && a && x->type == kTfLiteFloat32 && a->type == kTfLiteFloat32,
+           "PRELU: float32 input and alpha expected");
+  const int64_t na = PreluAlphaCount(x, a);
+  B_ENSURE(c, na > 0 && na <= INT32_MAX,
+           "PRELU: alpha must have the shape of the input's trailing dimensions (leading 1s "
+           "allowed); other broadcasts are not supported");
+  return SameShapePrepare(c, n);
+}
+TfLiteStatus PreluInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const TfLiteTensor* a = T(c, n->inputs, 1);
+  B_ENSURE(c, OnDevice(a->data.raw), "PRELU: alpha must be device-resident");
+  const int64_t na = PreluAlphaCount(x, a);
+  const lce_chain_desc chain{nullptr, a->data.f, nullptr, nullptr};
+  B_CAPI(c, lce_b200_f32_chain_sign(x->data.f, &chain, Count(x) / na, static_cast<int>(na),
+                                    T(c, n->outputs, 0)->data.f, nullptr, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// ------------------ ADD / PRELU / ADD [/ ADD -> LceQuantize] chain ------------------ //
+// Created by Graph::FuseActivationChains where no binary convolution precedes the chain.
+// inputs [x, shift_in, alpha, shift_out, sign_shift] (absent = -1), each constant [C] for
+// x [..., C]; outputs [o (-1 when only the signs are read), packed signs?].
+TfLiteStatus ChainPrepare(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  B_ENSURE(c, x && x->type == kTfLiteFloat32 && x->dims->size >= 1 && n->inputs->size == 5,
+           "activation chain: float32 input and four optional constants expected");
+  const int ch = x->dims->data[x->dims->size - 1];
+  for (int k = 1; k < 5; ++k) {
+    const TfLiteTensor* v = T(c, n->inputs, k);
+    B_ENSURE(c, !v || (v->type == kTfLiteFloat32 && Count(v) == ch),
+             "activation chain: the constants must be float32 with one value per channel");
+  }
+  TfLiteTensor* o = T(c, n->outputs, 0);
+  if (o && SameShapePrepare(c, n) != kTfLiteOk) return kTfLiteError;
+  if (n->outputs->size > 1) {
+    TfLiteTensor* pk = T(c, n->outputs, 1);
+    B_ENSURE(c, pk && pk->type == kTfLiteInt32, "activation chain: packed output must be int32");
+    TfLiteIntArray* dims = LceB200IntArrayCreate(x->dims->size);
+    for (int i = 0; i < x->dims->size; ++i) dims->data[i] = x->dims->data[i];
+    dims->data[x->dims->size - 1] = (ch + 31) / 32;
+    if (c->ResizeTensor(c, pk, dims) != kTfLiteOk) return kTfLiteError;
+  }
+  return kTfLiteOk;
+}
+TfLiteStatus ChainInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const float* v[4];
+  for (int k = 0; k < 4; ++k) {
+    const TfLiteTensor* t = T(c, n->inputs, k + 1);
+    v[k] = t ? t->data.f : nullptr;
+    B_ENSURE(c, !t || OnDevice(t->data.raw), "activation chain: constants must be device-resident");
+  }
+  const lce_chain_desc chain{v[0], v[1], v[2], v[3]};
+  const int ch = x->dims->data[x->dims->size - 1];
+  TfLiteTensor* o = T(c, n->outputs, 0);
+  TfLiteTensor* pk = n->outputs->size > 1 ? T(c, n->outputs, 1) : nullptr;
+  B_CAPI(c, lce_b200_f32_chain_sign(x->data.f, &chain, ch ? Count(x) / ch : 0, ch,
+                                    o ? o->data.f : nullptr, pk ? pk->data.i32 : nullptr,
+                                    lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // --------------------------------- DEQUANTIZE -------------------------------- //
 // int8 / uint8 -> float32 with the input tensor's (scale, zero_point): TF/lite/kernels/dequantize.cc.
 TfLiteStatus DequantPrepare(TfLiteContext* c, TfLiteNode* n) {
@@ -553,6 +635,10 @@ const TfLiteRegistration* FusedPoolDepthwiseRegistration() {
   static TfLiteRegistration r = {PoolDwInit, PoolDwFree, PoolDwPrepare, PoolDwInvoke};
   return &r;
 }
+const TfLiteRegistration* ActivationChainRegistration() {
+  static TfLiteRegistration r = {Init, Free, ChainPrepare, ChainInvoke};
+  return &r;
+}
 
 void RegisterBuiltinOps(OpResolver* r) {
   static TfLiteRegistration conv = {Init, Free, ConvPrepare<false>, ConvInvoke<false>};
@@ -585,6 +671,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(2, &concat);  // CONCATENATION
   static TfLiteRegistration dequant = {Init, Free, DequantPrepare, DequantInvoke};
   r->AddBuiltin(6, &dequant);  // DEQUANTIZE
+  static TfLiteRegistration prelu = {Init, Free, PreluPrepare, PreluInvoke};
+  r->AddBuiltin(54, &prelu);   // PRELU
 }
 
 }  // namespace lce_b200

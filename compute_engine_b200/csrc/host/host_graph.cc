@@ -398,6 +398,151 @@ int Graph::FuseResidualBlocks() {
 
 const TfLiteRegistration* FusedPoolDepthwiseRegistration();  // builtin_ops.cc
 const TfLiteRegistration* FusedStemRegistration();
+const TfLiteRegistration* ActivationChainRegistration();
+
+int Graph::FuseActivationChains() {
+  if (!device_arena_) return 0;
+  const size_t none = nodes_.size() + 1;   // "no such node" (compared before nodes are erased)
+  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
+  auto consumers = [&](int t) {
+    std::vector<size_t> c;
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
+    return c;
+  };
+  // the node that alone reads t, when t is an intermediate the chain may absorb
+  auto sole_consumer = [&](int t) {
+    if (is_output(t)) return none;
+    const std::vector<size_t> c = consumers(t);
+    return c.size() == 1 ? c[0] : none;
+  };
+  // node k is op(x, v) with v a per-channel constant of x's C channels (float, kTfLiteMmapRo,
+  // shape [1, ..., 1, C]) and no fused activation: returns v, else -1
+  auto const_op = [&](size_t k, const char* name, int x, int C) {
+    if (k >= nodes_.size()) return -1;
+    const NodeRecord& n = *nodes_[k];
+    if (n.name != name || n.initialized || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
+        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32 ||
+        n.builtin_blob.size() < sizeof(BuiltinParams) ||
+        reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())->activation != 0)
+      return -1;
+    const int v = n.node.inputs->data[1];
+    if (v < 0) return -1;
+    const TfLiteTensor& t = tensors_[v];
+    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
+        t.dims->data[t.dims->size - 1] != C)
+      return -1;
+    for (int d = 0; d + 1 < t.dims->size; ++d)
+      if (t.dims->data[d] != 1) return -1;
+    return v;
+  };
+  // node k's output is read only by an LceQuantize: returns that node, else none
+  auto quantize_of = [&](size_t k) {
+    const int y = nodes_[k]->node.outputs->data[0];
+    const size_t q = sole_consumer(y);
+    if (q >= nodes_.size()) return none;
+    const NodeRecord& n = *nodes_[q];
+    return n.name == "LceQuantize" && !n.initialized && n.node.inputs->size == 1 &&
+                   n.node.outputs->size == 1 && tensors_[n.node.outputs->data[0]].type == kTfLiteInt32
+               ? q
+               : none;
+  };
+  auto free_node = [&](NodeRecord& n) {
+    LceB200IntArrayFree(n.node.inputs);
+    LceB200IntArrayFree(n.node.outputs);
+    LceB200IntArrayFree(n.node.temporaries);
+    LceB200IntArrayFree(n.node.intermediates);
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    NodeRecord& a = *nodes_[i];
+    if (a.initialized) continue;
+    // after a fused residual block the chain starts on the sum; elsewhere node i is its first op
+    const bool after_bconv = a.name == "LceBconv2d+ADD" && a.node.inputs->size == 6 &&
+                             a.node.outputs->size == 1;
+    if (!after_bconv && a.name != "builtin:0" && a.name != "builtin:54") continue;
+    int cur = after_bconv ? a.node.outputs->data[0] : a.node.inputs->data[0];
+    if (cur < 0 || tensors_[cur].type != kTfLiteFloat32 || tensors_[cur].dims->size < 1) continue;
+    const int C = tensors_[cur].dims->data[tensors_[cur].dims->size - 1];
+    std::vector<size_t> absorbed;
+    int vec[4] = {-1, -1, -1, -1};   // shift_in, alpha, shift_out, sign_shift
+    size_t k = after_bconv ? sole_consumer(cur) : i;
+    // RPReLU: ADD? -> PRELU? -> ADD?; an ADD read only by an LceQuantize is the RSign's instead
+    const char* steps[3] = {"builtin:0", "builtin:54", "builtin:0"};
+    for (int s = 0; s < 3 && k < nodes_.size(); ++s) {
+      const int v = const_op(k, steps[s], cur, C);
+      if (v < 0 || (s != 1 && quantize_of(k) < nodes_.size())) continue;
+      vec[s] = v;
+      absorbed.push_back(k);
+      cur = nodes_[k]->node.outputs->data[0];
+      k = sole_consumer(cur);
+    }
+    const bool any_float = !absorbed.empty();
+    // RSign of the next binary layer: [ADD(sign_shift) ->] LceQuantize of the chain's result
+    int packed = -1;
+    for (size_t c : consumers(cur)) {
+      if (!any_float && !after_bconv && c != i) continue;   // stand-alone: node i must start it
+      const NodeRecord& n = *nodes_[c];
+      if (n.name == "LceQuantize" && !n.initialized && n.node.inputs->size == 1 &&
+          n.node.outputs->size == 1 && tensors_[n.node.outputs->data[0]].type == kTfLiteInt32) {
+        packed = n.node.outputs->data[0];
+        absorbed.push_back(c);
+        break;
+      }
+      const int v = const_op(c, "builtin:0", cur, C);
+      const size_t q = v >= 0 ? quantize_of(c) : none;
+      if (q < nodes_.size()) {
+        vec[3] = v;
+        packed = nodes_[q]->node.outputs->data[0];
+        absorbed.push_back(c);
+        absorbed.push_back(q);
+        break;
+      }
+    }
+    // a stand-alone chain must replace at least two nodes (node i is one of them)
+    if (absorbed.size() < (after_bconv ? 1u : 2u)) continue;
+    std::string name;
+    if (vec[0] >= 0 && vec[1] >= 0 && vec[2] >= 0) {
+      name = "+RPReLU";
+    } else {
+      if (vec[0] >= 0) name += "+ADD";
+      if (vec[1] >= 0) name += "+PRELU";
+      if (vec[2] >= 0) name += "+ADD";
+    }
+    if (packed >= 0) name += vec[3] >= 0 ? "+ADD+LceQuantize" : "+LceQuantize";
+    // the float result stays a tensor when something else reads it; a stand-alone chain without
+    // float steps would only copy its input
+    const std::vector<size_t> readers = consumers(cur);
+    const bool keep_out = after_bconv || (any_float && (is_output(cur) ||
+                                                        readers.size() > (packed >= 0 ? 1u : 0u)));
+    std::vector<int> ins, outs{keep_out ? cur : -1};
+    if (packed >= 0) outs.push_back(packed);
+    if (after_bconv) {
+      ins.assign(a.node.inputs->data, a.node.inputs->data + 6);
+      a.name += name;
+    } else {
+      ins.push_back(a.node.inputs->data[0]);
+      a.registration = ActivationChainRegistration();
+      a.name = name.substr(1);
+    }
+    ins.insert(ins.end(), vec, vec + 4);
+    LceB200IntArrayFree(a.node.inputs);
+    LceB200IntArrayFree(a.node.outputs);
+    a.node.inputs = MakeDims(ins);
+    a.node.outputs = MakeDims(outs);
+    // drop the absorbed nodes (all after node i), the highest index first
+    std::sort(absorbed.begin(), absorbed.end());
+    for (auto it = absorbed.rbegin(); it != absorbed.rend(); ++it) {
+      if (*it == i) continue;
+      free_node(*nodes_[*it]);
+      nodes_.erase(nodes_.begin() + *it);
+      ++removed;
+    }
+  }
+  allocated_ = false;
+  return removed;
+}
 
 // [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> 16) -> DEPTHWISE_CONV_2D(3x3, stride 2, multiplier 1),
 // each intermediate consumed once: one node (QuickNet's stem). The image is read once, as the

@@ -73,6 +73,16 @@ class Graph {
   // Returns the number of (ADD, LceQuantize) nodes removed. Call before AllocateTensors.
   int FuseResidualBlocks();
 
+  // ReActNet's per-channel chain: RPReLU (ADD(const) -> PRELU(const) -> ADD(const)) and the next
+  // layer's RSign ([ADD(const) ->] LceQuantize), each step optional:
+  //   after a "LceBconv2d+ADD" node (FuseResidualBlocks first) it moves into that node's epilogue
+  //   (inputs 6..9 = shift_in, alpha, shift_out, sign_shift; lce_b200_bconv2d_run_fused_chain);
+  //   elsewhere it becomes one node (lce_b200_f32_chain_sign) that replaces at least two.
+  // Only float constants of shape [1, ..., 1, C] (kTfLiteMmapRo), ADDs without fused activation,
+  // and intermediates with a single consumer that are not graph outputs are absorbed; otherwise
+  // the graph is left as it is. Bit-identical. Returns the number of nodes removed.
+  int FuseActivationChains();
+
   // Fusions among the float builtins around the binary path:
   //   MAX_POOL_2D(2x2, stride 1, VALID) -> DEPTHWISE_CONV_2D(3x3)  =>  one node
   //   CONV_2D(3x3 s2 -> 16) -> DEPTHWISE_CONV_2D(3x3 s2) -> CONV_2D(1x1 -> 64)  =>  one node (opt-in)

@@ -212,7 +212,9 @@ TfLiteStatus BconvPrepare(TfLiteContext* context, TfLiteNode* node) {
   if (!op->successfully_initialized) return kTfLiteError;
   lce_bconv2d_desc& d = op->desc;
 
-  LCE_ENSURE(context, node->inputs->size == (FUSED ? 6 : 5));
+  // fused: 6 inputs, or 10 with the activation chain (inputs 6..9, Graph::FuseActivationChains)
+  LCE_ENSURE(context, FUSED ? (node->inputs->size == 6 || node->inputs->size == 10)
+                            : node->inputs->size == 5);
   const TfLiteTensor* input = GetInput(context, node, 0);
   const TfLiteTensor* filter = GetInput(context, node, 1);
   const TfLiteTensor* post_mul = GetInput(context, node, 2);
@@ -322,6 +324,12 @@ TfLiteStatus BconvPrepare(TfLiteContext* context, TfLiteNode* node) {
     LCE_ENSURE(context, residual->type == kTfLiteFloat32 && NumDims(residual) == 4);
     LCE_ENSURE(context, Dim(residual, 0) == d.batch && Dim(residual, 1) == out_h &&
                             Dim(residual, 2) == out_w && Dim(residual, 3) == d.channels_out);
+    // the chain's per-channel constants: shift_in, alpha, shift_out, sign_shift (absent = -1)
+    for (int k = 6; k < node->inputs->size; ++k) {
+      const TfLiteTensor* v = GetInput(context, node, k);
+      LCE_ENSURE(context, v == nullptr || (v->type == kTfLiteFloat32 &&
+                                           NumElements(v) == d.channels_out));
+    }
     if (node->outputs->size > 1) {
       LCE_ENSURE(context, d.groups == 1);
       TfLiteIntArray* packed_shape = LceB200IntArrayCreate(4);
@@ -342,7 +350,8 @@ TfLiteStatus BconvPrepare(TfLiteContext* context, TfLiteNode* node) {
 
 TfLiteStatus BconvEnsurePlan(TfLiteContext* context, TfLiteNode* node);
 
-// Fused node: [in, filter, mul, bias, thr, residual] -> [out, packed_out?]; device arena only.
+// Fused node: [in, filter, mul, bias, thr, residual (, shift_in, alpha, shift_out, sign_shift)]
+// -> [out, packed_out?]; device arena only.
 TfLiteStatus BconvFusedEval(TfLiteContext* context, TfLiteNode* node) {
   auto* op = static_cast<BconvOpData*>(node->user_data);
   if (BconvEnsurePlan(context, node) != kTfLiteOk) return kTfLiteError;
@@ -355,6 +364,17 @@ TfLiteStatus BconvFusedEval(TfLiteContext* context, TfLiteNode* node) {
   LCE_ENSURE_MSG(context, OnDevice(input->data.raw) && OnDevice(output->data.raw) &&
                               OnDevice(residual->data.raw),
                  "fused LceBconv2d needs a device arena");
+  if (node->inputs->size == 10) {
+    auto vec = [&](int k) {
+      const TfLiteTensor* v = GetInput(context, node, k);
+      return v ? v->data.f : nullptr;
+    };
+    const lce_chain_desc chain{vec(6), vec(7), vec(8), vec(9)};
+    LCE_ENSURE_CAPI(context, lce_b200_bconv2d_run_fused_chain(
+                                 op->plan, input->data.i32, residual->data.f, add_act, &chain,
+                                 output->data.f, packed ? packed->data.i32 : nullptr, g_stream));
+    return kTfLiteOk;
+  }
   LCE_ENSURE_CAPI(context,
                   lce_b200_bconv2d_run_fused(op->plan, input->data.i32, residual->data.f, add_act,
                                              output->data.f, packed ? packed->data.i32 : nullptr,

@@ -187,20 +187,25 @@ size_t imma_smem_budget(int V, bool b1) {
   return (227u * 1024u / ctas - 1024u - 256u) & ~size_t{127};
 }
 
-template <int V, int OUT, bool B1>
+template <int V, int OUT, bool B1, bool CHAIN = false>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(imma_smem_budget(V, B1))));
-  lce::bconv_imma_kernel<V, OUT, B1><<<grid, lce::kIThreads, smem, s>>>(p);
+  lce::bconv_imma_kernel<V, OUT, B1, CHAIN><<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
+// chain: float output with p.chain applied in the epilogue (bconv_run_impl decides)
 template <int V>
-int launch_imma_v(int out_type, bool b1, const lce::ConvKParams& p, dim3 grid, size_t smem,
-                  cudaStream_t s) {
+int launch_imma_v(int out_type, bool b1, bool chain, const lce::ConvKParams& p, dim3 grid,
+                  size_t smem, cudaStream_t s) {
+  if (chain) {
+    if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, true>(p, grid, smem, s);
+    return launch_imma_vo<V, LCE_OUT_FLOAT, false, true>(p, grid, smem, s);
+  }
   if (b1) {
     if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, true>(p, grid, smem, s);
     return launch_imma_vo<V, LCE_OUT_RAW_ACC, true>(p, grid, smem, s);
@@ -222,7 +227,10 @@ int launch_conv_v(int out_type, const lce::ConvKParams& p, dim3 grid, size_t sme
 }
 int tc_launch(GemmCore& c, const lce::ConvKParams& p, cudaStream_t s);
 
-int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
+// The plan's float output goes through the mma.sync kernel (launch_conv's first choice).
+bool takes_imma(const GemmCore& c, const lce::ConvKParams& p) { return c.wt_nat != nullptr && p.vec_store; }
+
+int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, bool chain = false) {
   p.fd_ohw = lce::make_fastdiv(static_cast<uint32_t>(p.OH) * p.OW);
   p.fd_ow = lce::make_fastdiv(p.OW);
   p.fd_cwv = lce::make_fastdiv(p.CwV);
@@ -239,7 +247,7 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
   // raw-accumulator output); the wgmma kernel takes the rest it is eligible for (bitpacked and
   // int8 outputs, other channel counts), XOR + POPC what is left. All produce the same int32
   // accumulators.
-  if (c.wt_nat != nullptr && p.vec_store) {
+  if (takes_imma(c, p)) {
     // mma.sync inner product: 128 x 64 tiles, the same int32 accumulators as bconv_kernel
     lce::ConvKParams q = p;
     q.wt = c.wt_nat; q.wpop = c.wpop;
@@ -249,11 +257,12 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s) {
     dim3 igrid(static_cast<unsigned>((p.M + lce::kIBM - 1) / lce::kIBM),
                static_cast<unsigned>(c.groups * c.tiles_per_group));
     switch (c.V) {
-      case 4: return launch_imma_v<4>(c.out_type, c.imma_b1, q, igrid, ismem, s);
-      case 2: return launch_imma_v<2>(c.out_type, c.imma_b1, q, igrid, ismem, s);
-      default: return launch_imma_v<1>(c.out_type, c.imma_b1, q, igrid, ismem, s);
+      case 4: return launch_imma_v<4>(c.out_type, c.imma_b1, chain, q, igrid, ismem, s);
+      case 2: return launch_imma_v<2>(c.out_type, c.imma_b1, chain, q, igrid, ismem, s);
+      default: return launch_imma_v<1>(c.out_type, c.imma_b1, chain, q, igrid, ismem, s);
     }
   }
+  if (chain) return fail("bconv2d: the chain epilogue needs the mma.sync kernel");
   if (c.tc_ok) {
     // wgmma inner product: persistent 128 x BN tiles
     const int rc = tc_launch(c, p, s);
@@ -1008,7 +1017,7 @@ static size_t bconv_out_bytes(const lce_b200_bconv2d* plan) {
 
 static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* out_dev,
                           const float* residual, int residual_act, int32_t* packed_out,
-                          void* stream) {
+                          const lce_chain_desc* chain, void* stream) {
   const lce_bconv2d_desc& d = plan->d;
   GemmCore& c = plan->core;
   cudaStream_t s = as_stream(stream);
@@ -1051,6 +1060,18 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
   if (d.out_type == LCE_OUT_BITPACKED && !p.bp_fast)
     CUDA_OK(cudaMemsetAsync(out_dev, 0, bconv_out_bytes(plan), s));
   const bool zp_float = c.tap_popc != nullptr && plan->zp_mode == LCE_ZERO_PADDING_CORRECTION;
+  if (chain != nullptr) {
+    if (!zp_float && takes_imma(c, p)) {
+      p.chain = *chain;
+      return launch_conv(c, p, s, /*chain=*/true);
+    }
+    // every other kernel: the fused tail without the pack, then the chain pass in place
+    const int rc = bconv_run_impl(plan, in_dev, out_dev, residual, residual_act, nullptr, nullptr,
+                                  stream);
+    if (rc) return rc;
+    float* out = static_cast<float*>(out_dev);
+    return lce_b200_f32_chain_sign(out, chain, p.M, c.cout, out, packed_out, stream);
+  }
   if (!zp_float) return launch_conv(c, p, s);
   // the optimised kernels' zero padding: one-padding accumulators + a float correction. The
   // wgmma kernel does it in its epilogue; the others run unfused and a tail pass finishes.
@@ -1079,7 +1100,7 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
 
 int lce_b200_bconv2d_run(lce_b200_bconv2d* plan, const int32_t* in_dev, void* out_dev,
                          void* stream) {
-  return bconv_run_impl(plan, in_dev, out_dev, nullptr, LCE_ACT_NONE, nullptr, stream);
+  return bconv_run_impl(plan, in_dev, out_dev, nullptr, LCE_ACT_NONE, nullptr, nullptr, stream);
 }
 
 int lce_b200_bconv2d_run_fused(lce_b200_bconv2d* plan, const int32_t* in_dev,
@@ -1092,6 +1113,23 @@ int lce_b200_bconv2d_run_fused(lce_b200_bconv2d* plan, const int32_t* in_dev,
   if (residual_dev && (reinterpret_cast<uintptr_t>(residual_dev) & 15u) != 0)
     return fail("bconv2d_run_fused: residual must be 16-byte aligned");
   return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev,
+                        nullptr, stream);
+}
+
+int lce_b200_bconv2d_run_fused_chain(lce_b200_bconv2d* plan, const int32_t* in_dev,
+                                     const float* residual_dev, int add_activation,
+                                     const lce_chain_desc* chain, float* out_dev,
+                                     int32_t* packed_out_dev, void* stream) {
+  if (plan->d.out_type != LCE_OUT_FLOAT)
+    return fail("bconv2d_run_fused_chain: only float-output plans can take a chain");
+  if (packed_out_dev && plan->d.groups != 1)
+    return fail("bconv2d_run_fused_chain: packed output needs groups == 1");
+  if (residual_dev && (reinterpret_cast<uintptr_t>(residual_dev) & 15u) != 0)
+    return fail("bconv2d_run_fused_chain: residual must be 16-byte aligned");
+  if (chain)
+    for (const float* v : {chain->shift_in, chain->alpha, chain->shift_out, chain->sign_shift})
+      if (v && !is_device_ptr(v)) return fail("bconv2d_run_fused_chain: chain vectors must be device memory");
+  return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev, chain,
                         stream);
 }
 

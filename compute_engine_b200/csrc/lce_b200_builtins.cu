@@ -14,6 +14,7 @@
 
 #include "lce_b200.h"
 #include "lce_b200_builtins.h"
+#include "lce_b200_chain.cuh"
 
 namespace lce_b200_internal {
 int fail(const char* fmt, ...);       // lce_b200.cu
@@ -990,6 +991,37 @@ __global__ void __launch_bounds__(256) eltwise_kernel(const float* __restrict__ 
   }
 }
 
+// lce_b200_f32_chain_sign: one pass of the per-channel chain (lce_b200_chain.cuh). PACK: one thread
+// per (row, channel slot of a sign word), so each warp owns one packed word and ballots it (slots
+// past `channels` give 0 bits); else one thread per element. x and out may be the same buffer.
+template <bool PACK, typename I>
+__global__ void __launch_bounds__(256) chain_sign_kernel(const float* x, const lce_chain_desc ch,
+                                                         I rows, int channels, int cw, float* out,
+                                                         int32_t* __restrict__ packed) {
+  const bool has_si = ch.shift_in != nullptr, has_a = ch.alpha != nullptr;
+  const bool has_so = ch.shift_out != nullptr, has_ss = ch.sign_shift != nullptr;
+  const I span = PACK ? static_cast<I>(cw) * 32 : static_cast<I>(channels);
+  const I n = rows * span;
+  const I stride = static_cast<I>(gridDim.x) * blockDim.x;   // a multiple of 32: warps stay whole
+  for (I i = static_cast<I>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const I row = i / span;
+    const int c = static_cast<int>(i - row * span);
+    bool bit = false;
+    if (!PACK || c < channels) {
+      const I e = row * channels + c;
+      const float o = lce::chain_rprelu(x[e], has_si, has_si ? __ldg(ch.shift_in + c) : 0.0f, has_a,
+                                        has_a ? __ldg(ch.alpha + c) : 0.0f, has_so,
+                                        has_so ? __ldg(ch.shift_out + c) : 0.0f);
+      if (out) out[e] = o;
+      if (PACK) bit = lce::chain_sign(o, has_ss, has_ss ? __ldg(ch.sign_shift + c) : 0.0f);
+    }
+    if (PACK) {
+      const unsigned word = __ballot_sync(0xffffffffu, bit);
+      if ((threadIdx.x & 31) == 0) packed[i >> 5] = static_cast<int32_t>(word);
+    }
+  }
+}
+
 // mean over H*W: one thread per (b, c), c fastest => coalesced rows.
 __global__ void __launch_bounds__(256) mean_hw_kernel(const float* __restrict__ in,
                                                       float* __restrict__ out, int B, int HW,
@@ -1773,6 +1805,32 @@ int lce_b200_f32_activation(const float* in, float* out, int64_t n, int act, voi
   eltwise_kernel<2><<<grid_for(n / 4 + 1, 256), 256, 0, as_stream(stream)>>>(
       in, in, out, n, n, act, vec4_ok(in, in, out, n, n));
   return launch_check("eltwise_kernel<act>");
+}
+
+int lce_b200_f32_chain_sign(const float* x, const lce_chain_desc* chain, int64_t rows, int channels,
+                            float* out, int32_t* packed, void* stream) {
+  if (rows < 0 || channels <= 0) return fail("chain_sign: bad shape (%lld rows, %d channels)",
+                                             static_cast<long long>(rows), channels);
+  if (rows == 0 || (out == nullptr && packed == nullptr)) return 0;
+  const lce_chain_desc ch = chain ? *chain : lce_chain_desc{nullptr, nullptr, nullptr, nullptr};
+  const int cw = (channels + 31) / 32;
+  const long long n = packed ? rows * cw * 32 : rows * static_cast<long long>(channels);
+  const int grid = grid_for(n, 256);
+  cudaStream_t s = as_stream(stream);
+  // 32-bit index arithmetic where it fits (the row / channel split is a division per element)
+  const bool narrow = n + 256LL * grid < (1LL << 31);
+  if (packed) {
+    if (narrow)
+      chain_sign_kernel<true, int><<<grid, 256, 0, s>>>(x, ch, static_cast<int>(rows), channels, cw, out, packed);
+    else
+      chain_sign_kernel<true, long long><<<grid, 256, 0, s>>>(x, ch, rows, channels, cw, out, packed);
+  } else {
+    if (narrow)
+      chain_sign_kernel<false, int><<<grid, 256, 0, s>>>(x, ch, static_cast<int>(rows), channels, cw, out, packed);
+    else
+      chain_sign_kernel<false, long long><<<grid, 256, 0, s>>>(x, ch, rows, channels, cw, out, packed);
+  }
+  return launch_check("chain_sign_kernel");
 }
 
 int lce_b200_f32_mean_hw_act(const float* in, float* out, int batch, int h, int w, int c, int pre_activation,

@@ -39,6 +39,7 @@
 #ifndef LCE_B200_IMMA_CUH_
 #define LCE_B200_IMMA_CUH_
 
+#include "lce_b200_chain.cuh"
 #include "lce_b200_kernels.cuh"
 
 namespace lce {
@@ -300,14 +301,17 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 
 // Accumulator (ms, ns, e) of thread (gid, tig): pixel m0 + warp*32 + ms*16 + (e/2)*8 + gid,
 // channel c_tile + ns*8 + tig*2 + (e & 1), at scale 2^S. Full 64-channel tiles only
-// (host-checked).
-template <int OUT, int S>
+// (host-checked). CHAIN (float output): ReActNet's chain on the fused sum. Its four vectors and
+// the output transform's multiplier and bias are read per row from chain_s = [shift_in | alpha |
+// shift_out | sign_shift | mul | bias] x 64 channels in shared memory: holding them all in
+// registers would exceed the b1 instances' 128-register cap.
+template <int OUT, int S, bool CHAIN = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
-                                              int tig) {
+                                              int tig, const float* chain_s = nullptr) {
   const int cth = c_tile + tig * 2;
   float2 mul_r[8], bias_r[8];
-  if (OUT == LCE_OUT_FLOAT) {
+  if (OUT == LCE_OUT_FLOAT && !CHAIN) {
 #pragma unroll
     for (int ns = 0; ns < 8; ++ns) {
       mul_r[ns] = *reinterpret_cast<const float2*>(p.mul + cth + ns * 8);
@@ -351,9 +355,16 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           } else {
             x0 <<= 1; x1 <<= 1;
           }
-          y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mul_r[ns].x, bias_r[ns].x);
-          y[2 * ns + 1] =
-              transform_float_x2(x1, p.clamp_min, p.clamp_max, mul_r[ns].y, bias_r[ns].y);
+          if constexpr (CHAIN) {
+            const float2 mu = *reinterpret_cast<const float2*>(chain_s + 4 * kBN + tig * 2 + ns * 8);
+            const float2 bi = *reinterpret_cast<const float2*>(chain_s + 5 * kBN + tig * 2 + ns * 8);
+            y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mu.x, bi.x);
+            y[2 * ns + 1] = transform_float_x2(x1, p.clamp_min, p.clamp_max, mu.y, bi.y);
+          } else {
+            y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mul_r[ns].x, bias_r[ns].x);
+            y[2 * ns + 1] =
+                transform_float_x2(x1, p.clamp_min, p.clamp_max, mul_r[ns].y, bias_r[ns].y);
+          }
         }
         if (has_res) {
           // (A TMA-staged copy of the shortcut tile was measured slower on every layer: the
@@ -372,16 +383,44 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
             for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], act_lo), act_hi);
           }
         }
+        if constexpr (CHAIN) {
+          const bool has_si = p.chain.shift_in != nullptr, has_a = p.chain.alpha != nullptr;
+          const bool has_so = p.chain.shift_out != nullptr;
+#pragma unroll
+          for (int ns = 0; ns < 8; ++ns) {
+            const int k = tig * 2 + ns * 8;
+            const float2 si = *reinterpret_cast<const float2*>(chain_s + k);
+            const float2 al = *reinterpret_cast<const float2*>(chain_s + kBN + k);
+            const float2 so = *reinterpret_cast<const float2*>(chain_s + 2 * kBN + k);
+            y[2 * ns] = chain_rprelu(y[2 * ns], has_si, si.x, has_a, al.x, has_so, so.x);
+            y[2 * ns + 1] = chain_rprelu(y[2 * ns + 1], has_si, si.y, has_a, al.y, has_so, so.y);
+          }
+        }
         float* o = static_cast<float*>(p.out) + e0;
 #pragma unroll
         for (int ns = 0; ns < 8; ++ns)
           *reinterpret_cast<float2*>(o + ns * 8) = make_float2(y[2 * ns], y[2 * ns + 1]);
         if (has_pk) {
-          // LceQuantize of the value just written: bit = value < 0 (bitpack.h:159)
+          if constexpr (CHAIN) {
+            // RSign: LceQuantize of the value just written plus sign_shift
+            const bool has_ss = p.chain.sign_shift != nullptr;
+            const float* ss = chain_s + 3 * kBN + tig * 2;
 #pragma unroll
-          for (int ns = 0; ns < 4; ++ns) {
-            bits0 |= ((y[2 * ns] < 0.0f ? 1u : 0u) | (y[2 * ns + 1] < 0.0f ? 2u : 0u)) << (ns * 8);
-            bits1 |= ((y[2 * ns + 8] < 0.0f ? 1u : 0u) | (y[2 * ns + 9] < 0.0f ? 2u : 0u)) << (ns * 8);
+            for (int ns = 0; ns < 4; ++ns) {
+              const float2 s0 = *reinterpret_cast<const float2*>(ss + ns * 8);
+              const float2 s1 = *reinterpret_cast<const float2*>(ss + ns * 8 + 32);
+              bits0 |= ((chain_sign(y[2 * ns], has_ss, s0.x) ? 1u : 0u) |
+                        (chain_sign(y[2 * ns + 1], has_ss, s0.y) ? 2u : 0u)) << (ns * 8);
+              bits1 |= ((chain_sign(y[2 * ns + 8], has_ss, s1.x) ? 1u : 0u) |
+                        (chain_sign(y[2 * ns + 9], has_ss, s1.y) ? 2u : 0u)) << (ns * 8);
+            }
+          } else {
+            // LceQuantize of the value just written: bit = value < 0 (bitpack.h:159)
+#pragma unroll
+            for (int ns = 0; ns < 4; ++ns) {
+              bits0 |= ((y[2 * ns] < 0.0f ? 1u : 0u) | (y[2 * ns + 1] < 0.0f ? 2u : 0u)) << (ns * 8);
+              bits1 |= ((y[2 * ns + 8] < 0.0f ? 1u : 0u) | (y[2 * ns + 9] < 0.0f ? 2u : 0u)) << (ns * 8);
+            }
           }
           bits0 <<= tig * 2;
           bits1 <<= tig * 2;
@@ -403,8 +442,9 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 }
 
 // B1 selects the inner product: packed b1 fragments (accumulators at scale 1) or int8 ones
-// (scale 8). Both produce the same int32 accumulators.
-template <int V, int OUT, bool B1>
+// (scale 8). Both produce the same int32 accumulators. CHAIN (float output): the epilogue also
+// applies p.chain (lce_b200_bconv2d_run_fused_chain); the other instances compile as without it.
+template <int V, int OUT, bool B1, bool CHAIN = false>
 __global__ void __launch_bounds__(kIThreads, B1 ? kB1Ctas : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
   using Vec = typename VecT<V>::T;
@@ -512,7 +552,25 @@ bconv_imma_kernel(const ConvKParams p) {
     }
   }
   if (p.tap_popc != nullptr) zero_pad_correction_imma<S>(p, acc, m0, c_tile, warp, gid, tig);
-  epilogue_imma<OUT, S>(p, acc, m0, c_tile, warp, gid, tig);
+  if constexpr (CHAIN) {
+    // the chain's four 64-channel slices and the tile's multiplier / bias go to the shared memory
+    // the last K chunk released (the loop ended on a barrier)
+    float* cs = reinterpret_cast<float*>(smem_raw);
+    for (int i = tid; i < 6 * kBN; i += kIThreads) {
+      const int k = i / kBN;
+      const float* v = k == 0   ? p.chain.shift_in
+                       : k == 1 ? p.chain.alpha
+                       : k == 2 ? p.chain.shift_out
+                       : k == 3 ? p.chain.sign_shift
+                       : k == 4 ? p.mul
+                                : p.bias;
+      cs[i] = v != nullptr ? __ldg(v + c_tile + (i & (kBN - 1))) : 0.0f;
+    }
+    __syncthreads();
+    epilogue_imma<OUT, S, true>(p, acc, m0, c_tile, warp, gid, tig, cs);
+  } else {
+    epilogue_imma<OUT, S>(p, acc, m0, c_tile, warp, gid, tig);
+  }
 }
 
 }  // namespace lce

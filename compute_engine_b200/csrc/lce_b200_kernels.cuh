@@ -92,6 +92,9 @@ struct ConvKParams {
   int zp_float, cin_pg; // zero padding with the optimised kernels' float correction (host-side switch)
   FastDiv fd_ohw, fd_ow, fd_cwv, fd_kw, fd_tpg;  // / (OH*OW), / OW, / CwV, / KW, / tiles_per_group
   long long img_words;  // H * W * Cw_total (< 2^31, checked by the host)
+  // mma.sync kernel, CHAIN instances only: ReActNet's per-channel chain on the fused sum
+  // (lce_b200_chain.cuh); packed_out then holds the signs of o + sign_shift
+  lce_chain_desc chain;
 };
 
 // --------------------------- PTX helpers ---------------------------------- //

@@ -186,8 +186,14 @@ class HostGraph:
         """MAX_POOL_2D(2x2 s1 VALID) -> DEPTHWISE_CONV_2D(3x3) => one node."""
         return lib().lce_host_fuse_float_glue(self._g)
 
+    def fuse_activation_chains(self):
+        """ADD -> PRELU -> ADD [-> ADD -> LceQuantize] (ReActNet's RPReLU / RSign, each step
+        optional) => the epilogue of the preceding fused LceBconv2d+ADD node, or one node.
+        Call after fuse_residual_blocks and before allocate_tensors."""
+        return lib().lce_host_fuse_activation_chains(self._g)
+
     def fuse_all(self):
-        return self.fuse_residual_blocks() + self.fuse_float_glue()
+        return self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_activation_chains()
 
     # ---- profiling / async IO (bench.py) ----
     def enable_profiling(self, on=True):

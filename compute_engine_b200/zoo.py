@@ -228,4 +228,57 @@ def birealnet18(batch=1, seed=0, image=224, input_type="float32"):
     return g.m.serialize()
 
 
-MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "birealnet18": birealnet18}
+def reactnet_a(batch=1, seed=0, image=224, input_type="float32"):
+    """ReActNet-A, restated from the public description (Liu et al., ECCV 2020): MobileNet-V1
+    shaped. Stem CONV_2D 3x3/s2 3 -> 32 (BN folded, no activation), then 13 blocks with output
+    widths [64, 128, 128, 256, 256, 512 x 6, 1024, 1024], stride 2 where the width changes (not
+    32 -> 64). Each block, in the converter's op order:
+      RSign [ADD(shift) -> LceQuantize] -> LceBconv2d 3x3 C -> C (pad_values 1, BN folded, no
+      activation) -> ADD(shortcut; AVERAGE_POOL_2D 2x2/s2 VALID of x at stride 2) -> RPReLU
+      [ADD(shift) -> PRELU(alpha [1,1,C]) -> ADD(shift)] = out1 -> RSign -> 1x1 LceBconv2d C -> C
+      -> ADD(out1) (width doubling: two such 1x1 convolutions on the same signs, each + out1,
+      then CONCATENATION on channels) -> RPReLU.
+    Head MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX. 31 LceBconv2d, 26 PRELU."""
+    g = _Builder(seed, batch, "ReActNetA")
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+    x, xs = g.conv(x, xs, 32, 3, 2)
+
+    def shift(t, ts):
+        return g.add(t, g.const(g.rng.uniform(-0.2, 0.2, ts[3]).astype(np.float32), name="shift"), ts)
+
+    def rsign(t, ts):
+        return g.quantize(shift(t, ts), ts)
+
+    def rprelu(t, ts):
+        u = g.act(ts)
+        alpha = g.const(g.rng.uniform(0.05, 0.5, (1, 1, ts[3])).astype(np.float32), name="alpha")
+        g.m.add_op("PRELU", [shift(t, ts), alpha], [u])
+        return shift(u, ts)
+
+    widths = [32, 64, 128, 128, 256, 256] + [512] * 6 + [1024, 1024]
+    for cin, cout in zip(widths[:-1], widths[1:]):
+        stride = 2 if cout != cin and cin != 32 else 1
+        # the shortcut first: the convolution's epilogue can then add it (Graph::FuseResidualBlocks)
+        sc = x if stride == 1 else g.pool("AVERAGE_POOL_2D", x, xs, 2, 2, "VALID")[0]
+        y, ys = g.bconv(rsign(x, xs), xs, cin, stride=stride, pad_values=1, activation="NONE")
+        out1 = rprelu(g.add(y, sc, ys), ys)
+        q = rsign(out1, ys)
+        halves = []
+        for _ in range(cout // cin):
+            z, _ = g.bconv(q, ys, cin, k=1, pad_values=1, activation="NONE")
+            halves.append(g.add(z, out1, ys))
+        xs = ys[:3] + (cout,)
+        if len(halves) == 1:
+            z = halves[0]
+        else:
+            z = g.act(xs)
+            g.m.add_op("CONCATENATION", halves, [z], axis=3)
+        x = rprelu(z, xs)
+    probs = g.head(x, xs, relu=False)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
+MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "birealnet18": birealnet18,
+          "reactnet_a": reactnet_a}

@@ -113,6 +113,24 @@ int lce_b200_bconv2d_run_f32(lce_b200_bconv2d* plan, const float* in_dev,
 int lce_b200_bconv2d_run_fused(lce_b200_bconv2d* plan, const int32_t* in_dev,
                                const float* residual_dev, int add_activation,
                                float* out_dev, int32_t* packed_out_dev, void* stream);
+/* run_fused followed by ReActNet's per-channel chain (lce_chain_desc, lce_b200_types.h) on every
+ * output: out = o, packed_out = bitpack(o + sign_shift) (optional). Each chain vector holds
+ * channels_out floats on the device; chain may be NULL (then this is run_fused). The mma.sync
+ * kernel applies the chain in its epilogue; plans that run on another kernel, or that finish
+ * zero padding with the float correction pass, run run_fused and then lce_b200_f32_chain_sign in
+ * place. Bit-identical to the op sequence either way. */
+int lce_b200_bconv2d_run_fused_chain(lce_b200_bconv2d* plan, const int32_t* in_dev,
+                                     const float* residual_dev, int add_activation,
+                                     const lce_chain_desc* chain, float* out_dev,
+                                     int32_t* packed_out_dev, void* stream);
+/* The same chain without a convolution, in one pass over a float [rows, channels] tensor
+ * (ReActNet's chains after a CONCATENATION, a lone RSign; the PRELU builtin): element i takes
+ * channel i % channels of every present vector. out = o (may be NULL when nothing else reads it;
+ * may be x_dev), packed_out[row][ceil(channels/32)] = bitpack(o + sign_shift) (may be NULL). With
+ * only `alpha` set this is PRELU (TF/lite/kernels/internal/reference/prelu.h),
+ * out = x >= 0 ? x : x * alpha, and `channels` may be any alpha size dividing the element count. */
+int lce_b200_f32_chain_sign(const float* x_dev, const lce_chain_desc* chain, int64_t rows,
+                            int channels, float* out_dev, int32_t* packed_out_dev, void* stream);
 int lce_b200_bconv2d_run_host(lce_b200_bconv2d* plan, const int32_t* in_host,
                               void* out_host);
 void lce_b200_bconv2d_destroy(lce_b200_bconv2d* plan);

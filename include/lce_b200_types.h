@@ -82,6 +82,19 @@ typedef struct lce_bgemm_epilogue {
 } lce_bgemm_epilogue;
 #define LCE_OUT_RAW_ACC 3
 
+/* The per-channel float chain ReActNet puts behind a binary convolution: RPReLU
+ * (ADD(shift_in) -> PRELU(alpha) -> ADD(shift_out)), then the next layer's RSign
+ * (ADD(sign_shift) -> LceQuantize). Each pointer is a device vector with one float per channel;
+ * NULL means the op is absent, which is not the same as adding zeros (-0 + 0 = +0). Per element,
+ * in TFLite's order and rounding:
+ *   t = s + shift_in;  u = t >= 0 ? t : t * alpha;  o = u + shift_out;  bit = (o + sign_shift) < 0 */
+typedef struct lce_chain_desc {
+  const float* shift_in;
+  const float* alpha;
+  const float* shift_out;
+  const float* sign_shift;
+} lce_chain_desc;
+
 #ifdef __cplusplus
 }
 #endif
