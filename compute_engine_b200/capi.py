@@ -68,6 +68,7 @@ EXPORTS = [
     "lce_b200_bconv2d_set_input_shape", "lce_b200_bconv2d_get_desc",
     "lce_b200_bconv2d_set_zero_padding_mode", "lce_b200_path_counts", "lce_b200_tc_debug",
     "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_fused_chain",
+    "lce_b200_bconv2d_run_fused_pair",
     "lce_b200_f32_chain_sign",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
@@ -278,6 +279,23 @@ class BConv2d:
         desc, _keep = _chain_desc(shift_in, alpha, shift_out, sign_shift)
         _check(lib().lce_b200_bconv2d_run_fused_chain(self._h, _p(x), _p(res), C.c_int(add_activation),
                                                       C.byref(desc), _p(out), _p(pk), _stream()))
+        return out, pk
+
+    def run_fused_pair(self, second, x: torch.Tensor, residual: torch.Tensor, act1=0, act2=0,
+                       packed=True):
+        """lce_b200_bconv2d_run_fused_pair: this layer, then `second`, as two residual blocks on
+        bitpacked x and shortcut residual. Returns (float x2, packed signs of x2 | None)."""
+        x = _dev(x, torch.int32)
+        for plan in (self, second):
+            if tuple(x.shape[:3]) != (plan.desc.batch, plan.desc.in_h, plan.desc.in_w):
+                plan.set_input_shape(*x.shape[:3])
+        res = _dev(residual, torch.float32)
+        out = torch.empty_like(res)
+        pk = torch.empty(res.shape[:3] + (cdiv(res.shape[3], 32),), dtype=torch.int32,
+                         device=x.device) if packed else None
+        _check(lib().lce_b200_bconv2d_run_fused_pair(self._h, second._h, _p(x), _p(res),
+                                                     C.c_int(act1), C.c_int(act2), _p(out),
+                                                     _p(pk), _stream()))
         return out, pk
 
     def run_host(self, x_host, out_host):

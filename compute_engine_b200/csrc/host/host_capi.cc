@@ -143,6 +143,7 @@ int lce_host_enable_cuda_graph(void* g, int on) {
 int lce_host_fuse_residual_blocks(void* g) { return static_cast<Graph*>(g)->FuseResidualBlocks(); }
 int lce_host_fuse_float_glue(void* g) { return static_cast<Graph*>(g)->FuseFloatGlue(); }
 int lce_host_fuse_activation_chains(void* g) { return static_cast<Graph*>(g)->FuseActivationChains(); }
+int lce_host_fuse_residual_pairs(void* g) { return static_cast<Graph*>(g)->FuseResidualPairs(); }
 void lce_host_enable_profiling(void* g, int on) { static_cast<Graph*>(g)->EnableProfiling(on != 0); }
 void lce_host_reset_profile(void* g) { static_cast<Graph*>(g)->ResetProfile(); }
 double lce_host_node_time_ms(void* g, int node) { return static_cast<Graph*>(g)->NodeTimeMs(node); }

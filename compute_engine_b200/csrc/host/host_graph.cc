@@ -1,6 +1,8 @@
 #include "host_graph.h"
 
 #include "builtin_params.h"
+#include "flexbuffer_map.h"
+#include "lce_b200_types.h"
 
 #include <cuda_runtime.h>
 
@@ -391,6 +393,88 @@ int Graph::FuseResidualBlocks() {
     };
     if (qi < nodes_.size()) drop(qi);
     drop(ai);
+  }
+  allocated_ = false;
+  return removed;
+}
+
+extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_PAIR(const TfLiteRegistration* fused);
+extern "C" int lce_b200_internal_pair_pays_off(const lce_bconv2d_desc* d);   // lce_b200.cu
+
+int Graph::FuseResidualPairs() {
+  if (!device_arena_) return 0;
+  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
+  auto consumers = [&](int t) {
+    std::vector<size_t> c;
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
+    return c;
+  };
+  // the channel count of a fused residual block (no chain) whose layer the pair kernel takes and
+  // runs faster than two blocks at the input's current spatial size, or 0
+  auto pair_channels = [&](const NodeRecord& n) {
+    if (n.initialized || n.node.inputs->size != 6) return 0;
+    const TfLiteIntArray* xd = tensors_[n.node.inputs->data[0]].dims;
+    const TfLiteIntArray* fd = tensors_[n.node.inputs->data[1]].dims;
+    if (xd->size != 4 || fd->size != 4) return 0;
+    FlexMap m(n.custom_options.data(), n.custom_options.size());
+    lce_bconv2d_desc d{};
+    d.batch = xd->data[0]; d.in_h = xd->data[1]; d.in_w = xd->data[2];
+    d.channels_in = m.AsInt32("channels_in");
+    d.channels_out = fd->data[0]; d.filter_h = fd->data[1]; d.filter_w = fd->data[2];
+    d.groups = fd->data[3] == (d.channels_in + 31) / 32 && xd->data[3] == fd->data[3] ? 1 : 0;
+    d.stride_h = m.AsInt32("stride_height"); d.stride_w = m.AsInt32("stride_width");
+    d.dilation_h = m.AsInt32("dilation_height_factor");
+    d.dilation_w = m.AsInt32("dilation_width_factor");
+    d.padding = m.AsInt32("padding"); d.pad_value = m.AsInt32("pad_values");
+    d.out_type = tensors_[n.node.outputs->data[0]].type == kTfLiteFloat32 ? LCE_OUT_FLOAT : -1;
+    return lce_b200_internal_pair_pays_off(&d) ? d.channels_out : 0;
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    NodeRecord& a = *nodes_[i];
+    if (a.name != "LceBconv2d+ADD+LceQuantize" || a.node.outputs->size != 2) continue;
+    TfLiteRegistration* pair_reg = lce_b200_internal_Register_BCONV_2D_PAIR(a.registration);
+    if (pair_reg == nullptr) continue;
+    // x1 and its signs feed the next block alone
+    const int x1 = a.node.outputs->data[0], p1 = a.node.outputs->data[1];
+    if (is_output(x1) || is_output(p1)) continue;
+    const std::vector<size_t> cx = consumers(x1);
+    if (cx.size() != 1 || consumers(p1) != cx || cx[0] <= i) continue;
+    NodeRecord& b = *nodes_[cx[0]];
+    if ((b.name != "LceBconv2d+ADD" && b.name != "LceBconv2d+ADD+LceQuantize") ||
+        b.registration != a.registration || b.node.inputs->data[0] != p1 ||
+        b.node.inputs->data[5] != x1)
+      continue;
+    const int C = pair_channels(a);
+    if (C == 0 || pair_channels(b) != C) continue;
+    std::vector<int> ins(a.node.inputs->data, a.node.inputs->data + 6);
+    ins.insert(ins.end(), b.node.inputs->data + 1, b.node.inputs->data + 5);
+    std::vector<int> outs(b.node.outputs->data, b.node.outputs->data + b.node.outputs->size);
+    const int32_t acts[2] = {*reinterpret_cast<const int32_t*>(a.builtin_blob.data()),
+                             *reinterpret_cast<const int32_t*>(b.builtin_blob.data())};
+    const uint32_t n = static_cast<uint32_t>(a.custom_options.size());
+    std::vector<uint8_t> opts(reinterpret_cast<const uint8_t*>(&n), reinterpret_cast<const uint8_t*>(&n) + 4);
+    opts.insert(opts.end(), a.custom_options.begin(), a.custom_options.end());
+    opts.insert(opts.end(), b.custom_options.begin(), b.custom_options.end());
+    LceB200IntArrayFree(a.node.inputs);
+    LceB200IntArrayFree(a.node.outputs);
+    a.node.inputs = MakeDims(ins);
+    a.node.outputs = MakeDims(outs);
+    a.custom_options = opts;
+    a.node.custom_initial_data = a.custom_options.data();
+    a.node.custom_initial_data_size = static_cast<int>(a.custom_options.size());
+    a.builtin_blob.assign(reinterpret_cast<const uint8_t*>(acts), reinterpret_cast<const uint8_t*>(acts) + 8);
+    a.node.builtin_data = a.builtin_blob.data();
+    a.registration = pair_reg;
+    a.name = "LceBconv2d+ADD+" + b.name;
+    LceB200IntArrayFree(b.node.inputs);
+    LceB200IntArrayFree(b.node.outputs);
+    LceB200IntArrayFree(b.node.temporaries);
+    LceB200IntArrayFree(b.node.intermediates);
+    nodes_.erase(nodes_.begin() + cx[0]);
+    ++removed;
   }
   allocated_ = false;
   return removed;

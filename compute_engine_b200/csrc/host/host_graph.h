@@ -83,6 +83,17 @@ class Graph {
   // the graph is left as it is. Bit-identical. Returns the number of nodes removed.
   int FuseActivationChains();
 
+  // Two consecutive residual blocks x1 = x0 + f1(sign x0), x2 = x1 + f2(sign x1) -- a
+  // "LceBconv2d+ADD+LceQuantize" node whose two outputs only the next "LceBconv2d+ADD[+LceQuantize]"
+  // node reads, as its packed input and its shortcut -- become one node
+  // "LceBconv2d+ADD+LceBconv2d+ADD[+LceQuantize]" (lce_b200_bconv2d_run_fused_pair): x1 stays on
+  // chip. Inputs [x0 packed, f1, mul1, bias1, thr1, x0, f2, mul2, bias2, thr2], outputs
+  // [x2, packed x2?]. Both layers must be ones the pair kernel takes (3x3, stride 1, one-padding,
+  // C -> C, C = 64 or 128), on an image its tiles cover at least half full at the tensors' shapes
+  // when the pass runs (smaller images run faster unpaired); pairing is greedy in graph order. Call
+  // after FuseResidualBlocks and FuseActivationChains. Bit-identical. Returns the nodes removed.
+  int FuseResidualPairs();
+
   // Fusions among the float builtins around the binary path:
   //   MAX_POOL_2D(2x2, stride 1, VALID) -> DEPTHWISE_CONV_2D(3x3)  =>  one node
   //   CONV_2D(3x3 s2 -> 16) -> DEPTHWISE_CONV_2D(3x3 s2) -> CONV_2D(1x1 -> 64)  =>  one node (opt-in)

@@ -607,6 +607,109 @@ TfLiteStatus BMaxPoolEval(TfLiteContext* context, TfLiteNode* node) {
                       });
 }
 
+// ------------------------------------------------------------------------- //
+// Two residual blocks in one node (Graph::FuseResidualPairs):
+// [x0 packed, f1, mul1, bias1, thr1, x0, f2, mul2, bias2, thr2] -> [x2, packed x2?].
+// Options: [uint32 n][layer 1's n option bytes][layer 2's option bytes]; builtin_data: the two
+// ADD activations (int32[2]). Each layer keeps the op data of a plain LceBconv2d.
+// ------------------------------------------------------------------------- //
+struct PairOpData {
+  BconvOpData* layer[2] = {nullptr, nullptr};
+  ~PairOpData() {
+    delete layer[0];
+    delete layer[1];
+  }
+};
+
+void* PairInit(TfLiteContext* context, const char* buffer, size_t length) {
+  auto* op = new PairOpData();
+  uint32_t n = 0;
+  if (length >= 4) memcpy(&n, buffer, 4);
+  if (length < 4 || n > length - 4) {
+    context->ReportError(context, "LceBconv2d pair: malformed options");
+    op->layer[0] = new BconvOpData();
+    op->layer[1] = new BconvOpData();
+    return op;
+  }
+  op->layer[0] = static_cast<BconvOpData*>(BconvInit(context, buffer + 4, n));
+  op->layer[1] = static_cast<BconvOpData*>(BconvInit(context, buffer + 4 + n, length - 4 - n));
+  return op;
+}
+void PairFree(TfLiteContext*, void* buffer) { delete static_cast<PairOpData*>(buffer); }
+
+// Layer k of a pair node seen as a plain LceBconv2d node [x0 packed, filter, mul, bias, thr] ->
+// [x2]: x1 has x2's shape and x0's packed shape, so both layers check against the same tensors.
+struct PairLayerView {
+  TfLiteNode node{};
+  PairLayerView(const TfLiteNode* pair, int k, void* user_data) {
+    node.inputs = LceB200IntArrayCreate(5);
+    node.inputs->data[0] = pair->inputs->data[0];
+    for (int i = 1; i < 5; ++i) node.inputs->data[i] = pair->inputs->data[5 * k + i];
+    node.outputs = LceB200IntArrayCreate(1);
+    node.outputs->data[0] = pair->outputs->data[0];
+    node.user_data = user_data;
+  }
+  ~PairLayerView() {
+    LceB200IntArrayFree(node.inputs);
+    LceB200IntArrayFree(node.outputs);
+  }
+};
+
+template <KernelType kt>
+TfLiteStatus PairPrepare(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<PairOpData*>(node->user_data);
+  LCE_ENSURE(context, node->inputs->size == 10);
+  LCE_ENSURE(context, node->outputs->size == 1 || node->outputs->size == 2);
+  for (int k = 0; k < 2; ++k) {
+    PairLayerView v(node, k, op->layer[k]);
+    if (BconvPrepare<kt>(context, &v.node) != kTfLiteOk) return kTfLiteError;
+  }
+  const lce_bconv2d_desc& d = op->layer[1]->desc;
+  const TfLiteTensor* residual = GetInput(context, node, 5);
+  LCE_ENSURE(context, GetOutput(context, node, 0)->type == kTfLiteFloat32);
+  LCE_ENSURE(context, residual != nullptr && residual->type == kTfLiteFloat32 && NumDims(residual) == 4);
+  LCE_ENSURE(context, Dim(residual, 0) == d.batch && Dim(residual, 1) == d.in_h &&
+                          Dim(residual, 2) == d.in_w && Dim(residual, 3) == d.channels_out);
+  if (node->outputs->size > 1) {
+    TfLiteIntArray* packed_shape = LceB200IntArrayCreate(4);
+    packed_shape->data[0] = d.batch;
+    packed_shape->data[1] = d.in_h;
+    packed_shape->data[2] = d.in_w;
+    packed_shape->data[3] = BitpackedSize(d.channels_out);
+    if (context->ResizeTensor(context, GetOutput(context, node, 1), packed_shape) != kTfLiteOk)
+      return kTfLiteError;
+  }
+  return kTfLiteOk;
+}
+
+TfLiteStatus PairEval(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<PairOpData*>(node->user_data);
+  for (int k = 0; k < 2; ++k) {
+    PairLayerView v(node, k, op->layer[k]);
+    if (BconvEnsurePlan(context, &v.node) != kTfLiteOk) return kTfLiteError;
+  }
+  const TfLiteTensor* input = GetInput(context, node, 0);
+  const TfLiteTensor* residual = GetInput(context, node, 5);
+  TfLiteTensor* output = GetOutput(context, node, 0);
+  TfLiteTensor* packed = node->outputs->size > 1 ? GetOutput(context, node, 1) : nullptr;
+  const int32_t* act = static_cast<const int32_t*>(node->builtin_data);
+  LCE_ENSURE(context, act != nullptr);
+  LCE_ENSURE_MSG(context, OnDevice(input->data.raw) && OnDevice(output->data.raw) &&
+                              OnDevice(residual->data.raw),
+                 "fused LceBconv2d pair needs a device arena");
+  LCE_ENSURE_CAPI(context, lce_b200_bconv2d_run_fused_pair(
+                               op->layer[0]->plan, op->layer[1]->plan, input->data.i32,
+                               residual->data.f, act[0], act[1], output->data.f,
+                               packed ? packed->data.i32 : nullptr, g_stream));
+  return kTfLiteOk;
+}
+
+template <KernelType kt>
+TfLiteRegistration* BconvPairRegistration() {
+  static TfLiteRegistration r = {PairInit, PairFree, PairPrepare<kt>, PairEval};
+  return &r;
+}
+
 template <KernelType kt>
 TfLiteRegistration* BconvFusedRegistration() {
   static TfLiteRegistration r = {BconvInit, BconvFree, BconvPrepare<kt, true>, BconvFusedEval};
@@ -644,6 +747,19 @@ TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_FUSED(const TfLiteRegist
     return BconvFusedRegistration<KernelType::kOptimizedBGEMM>();
   if (original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
     return BconvFusedRegistration<KernelType::kOptimizedIndirectBGEMM>();
+  return nullptr;
+}
+
+// host-internal: the two-block node created by Graph::FuseResidualPairs from two fused nodes of
+// this registration (nullptr: not one of this library's fused LceBconv2d registrations)
+TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_PAIR(const TfLiteRegistration* fused) {
+  if (fused == BconvFusedRegistration<KernelType::kCuda>()) return BconvPairRegistration<KernelType::kCuda>();
+  if (fused == BconvFusedRegistration<KernelType::kReference>())
+    return BconvPairRegistration<KernelType::kReference>();
+  if (fused == BconvFusedRegistration<KernelType::kOptimizedBGEMM>())
+    return BconvPairRegistration<KernelType::kOptimizedBGEMM>();
+  if (fused == BconvFusedRegistration<KernelType::kOptimizedIndirectBGEMM>())
+    return BconvPairRegistration<KernelType::kOptimizedIndirectBGEMM>();
   return nullptr;
 }
 

@@ -19,6 +19,7 @@
 #include "lce_b200.h"
 #include "lce_b200_kernels.cuh"
 #include "lce_b200_imma.cuh"
+#include "lce_b200_pair.cuh"
 #include "lce_b200_tc.cuh"
 #include "lce_b200_pw.cuh"
 
@@ -605,6 +606,12 @@ int stem7_tf32_conv(const float* in, const float* filter, const float* bias, flo
 }  // namespace lce_b200_internal
 namespace {
 
+// A kernel-selection switch set to 0 (read per plan: A/B in one process)
+bool env_off(const char* name) {
+  const char* e = getenv(name);
+  return e && e[0] == '0';
+}
+
 // Build the tiled weights (+ optional tap popcounts) from an OHWI-packed filter
 // [cout][taps][Cw_pg] that may live on the host or the device.
 int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
@@ -636,13 +643,10 @@ int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
   // tiles, float or raw-accumulator output. LCE_B200_BCONV_IMMA=0 leaves every plan to the
   // wgmma / XOR + POPC kernels (bench.py reports both). LCE_B200_BCONV_B1=0 keeps the int8
   // fragments instead of the packed b1 ones; both give the same accumulators.
-  const char* imma_env = getenv("LCE_B200_BCONV_IMMA");  // read per plan: A/B in one process
-  const bool imma_on = !(imma_env && imma_env[0] == '0');
-  const char* b1_env = getenv("LCE_B200_BCONV_B1");
-  if (imma_on && c->cout_pg % lce::kBN == 0 &&
+  if (!env_off("LCE_B200_BCONV_IMMA") && c->cout_pg % lce::kBN == 0 &&
       (c->out_type == LCE_OUT_FLOAT || c->out_type == LCE_OUT_RAW_ACC)) {
     const int Kw = c->taps * c->Cw_pg;
-    c->imma_b1 = !(b1_env && b1_env[0] == '0');
+    c->imma_b1 = !env_off("LCE_B200_BCONV_B1");
     const size_t budget = imma_smem_budget(c->V, c->imma_b1);
     if (c->imma_b1) {
       const int n_slices = cdiv(Kw, 8);  // 8-word k-slices, the last one padded to 4 or 8 words
@@ -703,6 +707,40 @@ int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// What keeps a layer off the pair kernel (lce_b200_pair.cuh), or nullptr: it takes 3x3, stride 1,
+// dilation 1, ungrouped, SAME one-padded layers with float output and channels_in ==
+// channels_out in {64, 128}, on the b1 mma.sync inner product.
+const char* pair_layer_refusal(const lce_bconv2d_desc& d) {
+  if (d.out_type != LCE_OUT_FLOAT) return "float output";
+  if (d.filter_h != 3 || d.filter_w != 3 || d.stride_h != 1 || d.stride_w != 1 ||
+      d.dilation_h != 1 || d.dilation_w != 1 || d.groups != 1)
+    return "an ungrouped 3x3 filter with stride 1 and dilation 1";
+  if (d.padding != LCE_PADDING_SAME || d.pad_value != 1) return "SAME padding with pad_values = 1";
+  if (d.channels_in != d.channels_out || (d.channels_out != 64 && d.channels_out != 128))
+    return "channels_in == channels_out, 64 or 128";
+  if (env_off("LCE_B200_BCONV_IMMA") || env_off("LCE_B200_BCONV_B1"))
+    return "the b1 mma.sync inner product (LCE_B200_BCONV_IMMA / _B1 are 0)";
+  return nullptr;
+}
+
+// the pair kernel's output tile for C channels (64 or 128)
+void pair_tile(int C, int* th, int* tw) {
+  *th = C == 64 ? lce::PairShape<2>::TH : lce::PairShape<4>::TH;
+  *tw = C == 64 ? lce::PairShape<2>::TW : lce::PairShape<4>::TW;
+}
+
+template <int CW>
+int launch_pair(const lce::PairParams& p, int grid, cudaStream_t s) {
+  constexpr int smem = lce::PairShape<CW>::smem_bytes;
+  static PerDeviceOnce once;
+  if (once.need())
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_pair_kernel<CW>,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  lce::bconv_pair_kernel<CW><<<grid, lce::kPThreads, smem, s>>>(p);
+  g_path[1].fetch_add(1, std::memory_order_relaxed);
+  return launch_check("bconv_pair_kernel");
+}
 
 }  // namespace
 
@@ -1131,6 +1169,75 @@ int lce_b200_bconv2d_run_fused_chain(lce_b200_bconv2d* plan, const int32_t* in_d
       if (v && !is_device_ptr(v)) return fail("bconv2d_run_fused_chain: chain vectors must be device memory");
   return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev, chain,
                         stream);
+}
+
+int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* plan2,
+                                    const int32_t* in_dev, const float* residual_dev,
+                                    int act1, int act2, float* out_dev, int32_t* packed_out_dev,
+                                    void* stream) {
+  if (!plan1 || !plan2 || !in_dev || !residual_dev || !out_dev)
+    return fail("bconv2d_run_fused_pair: plans, input, residual and output are required");
+  for (const lce_b200_bconv2d* pl : {plan1, plan2}) {
+    if (const char* why = pair_layer_refusal(pl->d))
+      return fail("bconv2d_run_fused_pair: each layer needs %s", why);
+    if (!pl->core.imma_b1 || pl->core.wt_nat == nullptr)
+      return fail("bconv2d_run_fused_pair: each plan needs the b1 mma.sync weight fragments");
+  }
+  const lce_bconv2d_desc& d = plan1->d;
+  const lce_bconv2d_desc& d2 = plan2->d;
+  if (d2.channels_in != d.channels_out || d2.batch != d.batch || d2.in_h != d.in_h ||
+      d2.in_w != d.in_w)
+    return fail("bconv2d_run_fused_pair: the second layer must take the first one's output shape");
+  for (int a : {act1, act2})
+    if (a < LCE_ACT_NONE || a > LCE_ACT_RELU6)
+      return fail("bconv2d_run_fused_pair: unknown ADD activation %d", a);
+  const int C = d.channels_out, CW = C / 32;
+  if ((reinterpret_cast<uintptr_t>(in_dev) & (4u * CW - 1)) != 0)
+    return fail("bconv2d_run_fused_pair: input pointer must be %d-byte aligned", 4 * CW);
+  if (!aligned16(residual_dev) || !aligned16(out_dev))
+    return fail("bconv2d_run_fused_pair: residual and output must be 16-byte aligned");
+  const long long px = static_cast<long long>(d.batch) * d.in_h * d.in_w;
+  if (px == 0) return 0;
+  // a CTA reads the shortcut of its neighbours' tiles: writing x2 over x0 would race
+  const uintptr_t r0 = reinterpret_cast<uintptr_t>(residual_dev), o0 = reinterpret_cast<uintptr_t>(out_dev);
+  const uintptr_t bytes = static_cast<uintptr_t>(px) * C * 4;
+  if (r0 < o0 + bytes && o0 < r0 + bytes)
+    return fail("bconv2d_run_fused_pair: output must not overlap the residual");
+  lce::PairParams p;
+  memset(&p, 0, sizeof(p));
+  p.in = in_dev; p.residual = residual_dev; p.out = out_dev; p.packed_out = packed_out_dev;
+  const lce_b200_bconv2d* plans[2] = {plan1, plan2};
+  for (int k = 0; k < 2; ++k) {
+    const GemmCore& c = plans[k]->core;
+    p.wt[k] = reinterpret_cast<const uint2*>(c.wt_nat);
+    p.wpop[k] = c.wpop; p.mul[k] = c.mul; p.bias[k] = c.bias;
+    p.clamp_min[k] = c.clamp_min; p.clamp_max[k] = c.clamp_max;
+  }
+  p.act[0] = act1; p.act[1] = act2;
+  p.H = d.in_h; p.W = d.in_w;
+  int th, tw;
+  pair_tile(C, &th, &tw);
+  p.tiles_x = cdiv(d.in_w, tw);
+  p.tiles_per_img = p.tiles_x * cdiv(d.in_h, th);
+  const long long grid = static_cast<long long>(d.batch) * p.tiles_per_img;
+  if (grid > INT_MAX) return fail("bconv2d_run_fused_pair: too many tiles");
+  cudaStream_t s = as_stream(stream);
+  if (CW == 2) return launch_pair<2>(p, static_cast<int>(grid), s);
+  return launch_pair<4>(p, static_cast<int>(grid), s);
+}
+
+// Whether Graph::FuseResidualPairs should pair two such layers at this image size: the pair kernel
+// takes them and at least half of its tiles' pixels are the image's. Measured on an H100 80GB
+// HBM3, batch 256 (tools/pair_bench.py), pair time over two run_fused calls: whole tiles 0.65 -
+// 0.77 (56x56x64, 28x28x128, 42x42x64, 14x14x64 and x128); 22x22x64 (62 % used) 0.80, 32x32x64
+// (58 %) 0.95, 11x11x128 (62 %) 0.97, 7x7x128 (50 %) 0.88; 16x16x64 and 8x8x128 (33 %) 1.26 and
+// 1.73: there the ring recompute and the empty tile area cost more than x1's round trip saves.
+int lce_b200_internal_pair_pays_off(const lce_bconv2d_desc* d) {
+  if (pair_layer_refusal(*d) != nullptr || d->in_h < 1 || d->in_w < 1) return 0;
+  int th, tw;
+  pair_tile(d->channels_out, &th, &tw);
+  const long long tiled = static_cast<long long>(cdiv(d->in_h, th)) * th * cdiv(d->in_w, tw) * tw;
+  return 2LL * d->in_h * d->in_w >= tiled;
 }
 
 int lce_b200_bconv2d_run_f32(lce_b200_bconv2d* plan, const float* in_dev, void* out_dev,

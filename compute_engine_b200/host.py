@@ -192,8 +192,14 @@ class HostGraph:
         Call after fuse_residual_blocks and before allocate_tensors."""
         return lib().lce_host_fuse_activation_chains(self._g)
 
+    def fuse_residual_pairs(self):
+        """Two consecutive LceBconv2d+ADD[+LceQuantize] blocks whose intermediate nothing else
+        reads => one node that keeps it on chip. Call after the other fusions."""
+        return lib().lce_host_fuse_residual_pairs(self._g)
+
     def fuse_all(self):
-        return self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_activation_chains()
+        return (self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_activation_chains()
+                + self.fuse_residual_pairs())
 
     # ---- profiling / async IO (bench.py) ----
     def enable_profiling(self, on=True):

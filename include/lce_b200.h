@@ -123,6 +123,17 @@ int lce_b200_bconv2d_run_fused_chain(lce_b200_bconv2d* plan, const int32_t* in_d
                                      const float* residual_dev, int add_activation,
                                      const lce_chain_desc* chain, float* out_dev,
                                      int32_t* packed_out_dev, void* stream);
+/* Two consecutive fused residual blocks in one kernel:
+ *   x1 = act1(OutputTransform1(conv1(x0 packed)) + x0);  out = act2(OutputTransform2(conv2(bitpack(x1))) + x1);
+ *   packed_out = bitpack(out) (optional, may be NULL).
+ * Bit-identical to two run_fused calls, but x1 and its signs stay on chip. Both plans must be
+ * ungrouped 3x3 / stride 1 / dilation 1 SAME layers with pad_values = 1, float output,
+ * channels_in == channels_out == 64 or 128, on the b1 mma.sync kernel, and plan2 must take plan1's
+ * output shape; anything else is refused with a message. out must not overlap residual. */
+int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* plan2,
+                                    const int32_t* in_dev, const float* residual_dev,
+                                    int act1, int act2, float* out_dev,
+                                    int32_t* packed_out_dev, void* stream);
 /* The same chain without a convolution, in one pass over a float [rows, channels] tensor
  * (ReActNet's chains after a CONCATENATION, a lone RSign; the PRELU builtin): element i takes
  * channel i % channels of every present vector. out = o (may be NULL when nothing else reads it;
