@@ -55,6 +55,17 @@ def _chain_desc(shift_in=None, alpha=None, shift_out=None, sign_shift=None):
     return ChainDesc(*[None if v is None else v.data_ptr() for v in vecs]), vecs
 
 
+class GateDesc(C.Structure):
+    """lce_gate_desc: device pointers; gate [batch, C] is required, None = the op is absent."""
+    _fields_ = [("gate", C.c_void_p), ("alpha", C.c_void_p), ("sign_scale", C.c_void_p),
+                ("sign_shift", C.c_void_p)]
+
+
+def _gate_desc(gate, alpha=None, sign_scale=None, sign_shift=None):
+    vecs = [None if v is None else _dev(v, torch.float32) for v in (gate, alpha, sign_scale, sign_shift)]
+    return GateDesc(*[None if v is None else v.data_ptr() for v in vecs]), vecs
+
+
 class BgemmEpilogue(C.Structure):
     _fields_ = [("out_type", C.c_int32), ("clamp_min", C.c_int32),
                 ("clamp_max", C.c_int32), ("multiplier", C.c_void_p),
@@ -69,7 +80,8 @@ EXPORTS = [
     "lce_b200_bconv2d_set_zero_padding_mode", "lce_b200_path_counts", "lce_b200_tc_debug",
     "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_fused_chain",
     "lce_b200_bconv2d_run_fused_pair",
-    "lce_b200_f32_chain_sign",
+    "lce_b200_bconv2d_run_fused_gate",
+    "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_logistic",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -197,6 +209,24 @@ def chain_sign(x: torch.Tensor, shift_in=None, alpha=None, shift_out=None, sign_
     return o, pk
 
 
+def gate_sign(x: torch.Tensor, gate, residual=None, activation=0, alpha=None, sign_scale=None,
+              sign_shift=None, out=True, packed=True):
+    """Real-to-Binary's gated tail over x [B, H, W, C] with gate [B, C] (or [B, 1, 1, C]):
+    act(prelu(x * gate, alpha) + residual), and the signs of that * sign_scale + sign_shift.
+    Returns (out | None, packed | None)."""
+    x = _dev(x, torch.float32)
+    b, ch = x.shape[0], x.shape[-1]
+    desc, _keep = _gate_desc(gate, alpha, sign_scale, sign_shift)
+    res = None if residual is None else _dev(residual, torch.float32)
+    o = torch.empty_like(x) if out else None
+    pk = torch.empty(x.shape[:-1] + (cdiv(ch, 32),), dtype=torch.int32,
+                     device=x.device) if packed else None
+    _check(lib().lce_b200_f32_gate_sign(_p(x), C.byref(desc), _p(res), C.c_int(activation),
+                                        C.c_int64(b), C.c_int64(x.numel() // max(b * ch, 1)),
+                                        C.c_int(ch), _p(o), _p(pk), _stream()))
+    return o, pk
+
+
 class BConv2d:
     """LceBconv2d plan: constructor = Init + Prepare + OneTimeSetup
     (LCE/tflite/kernels/bconv2d.cc:85-392), ``__call__`` = Eval (:551-564)."""
@@ -279,6 +309,24 @@ class BConv2d:
         desc, _keep = _chain_desc(shift_in, alpha, shift_out, sign_shift)
         _check(lib().lce_b200_bconv2d_run_fused_chain(self._h, _p(x), _p(res), C.c_int(add_activation),
                                                       C.byref(desc), _p(out), _p(pk), _stream()))
+        return out, pk
+
+    def run_fused_gate(self, x: torch.Tensor, gate, residual=None, add_activation=0, alpha=None,
+                       sign_scale=None, sign_shift=None, packed=True, out=None):
+        """lce_b200_bconv2d_run_fused_gate on bitpacked x with gate [batch, C] (or [batch, 1, 1, C]):
+        returns (float out, packed signs | None). `out` may be given (the C-ABI refuses one that
+        overlaps the residual or the gate)."""
+        x = _dev(x, torch.int32)
+        if tuple(x.shape[:3]) != (self.desc.batch, self.desc.in_h, self.desc.in_w):
+            self.set_input_shape(*x.shape[:3])
+        out = self._alloc(x, out)
+        pk = torch.empty(out.shape[:3] + (cdiv(out.shape[3], 32),), dtype=torch.int32,
+                         device=x.device) if packed else None
+        res = None if residual is None else _dev(residual, torch.float32)
+        desc, _keep = _gate_desc(gate, alpha, sign_scale, sign_shift)
+        _check(lib().lce_b200_bconv2d_run_fused_gate(self._h, _p(x), C.byref(desc), _p(res),
+                                                     C.c_int(add_activation), _p(out), _p(pk),
+                                                     _stream()))
         return out, pk
 
     def run_fused_pair(self, second, x: torch.Tensor, residual: torch.Tensor, act1=0, act2=0,

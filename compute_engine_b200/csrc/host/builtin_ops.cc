@@ -1,8 +1,8 @@
 // builtin_ops.cc -- TfLiteRegistrations for the float builtins QuickNet /
-// QuickNetLarge / Bi-RealNet-18 / ReActNet-A use around the binary path, backed by
+// QuickNetLarge / Bi-RealNet-18 / ReActNet-A / Real-to-Binary Net use around the binary path, backed by
 // the fp32 CUDA kernels of lce_b200_builtins.cu. Shape inference follows TFLite's
 // builtin kernels (tensorflow/lite/kernels/{conv,depthwise_conv,pooling,add,mul,
-// fully_connected,softmax,reduce,reshape,activations}.cc). Device arena only.
+// fully_connected,softmax,reduce,reshape,activations,logistic}.cc). Device arena only.
 #include <cuda_runtime.h>
 
 #include <cstring>
@@ -325,14 +325,24 @@ TfLiteStatus StemInvoke(TfLiteContext* c, TfLiteNode* n) {
 }
 
 // ------------------------------ ADD / MUL / RELU ------------------------------ //
+// MUL's one further broadcast: a [B,H,W,C] tensor by a per-image, per-channel [B,1,1,C] one (the
+// channel gate of Real-to-Binary Net); runs as lce_b200_f32_gate_sign with only the gate set.
+bool ImageChannelBroadcast(const TfLiteTensor* a, const TfLiteTensor* b) {
+  return a->dims->size == 4 && b->dims->size == 4 && b->dims->data[0] == a->dims->data[0] &&
+         b->dims->data[1] == 1 && b->dims->data[2] == 1 && b->dims->data[3] == a->dims->data[3];
+}
+template <bool MUL>
 TfLiteStatus EltPrepare(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* a = T(c, n->inputs, 0);
   const TfLiteTensor* b = T(c, n->inputs, 1);
   B_ENSURE(c, a && b, "ADD/MUL: two inputs required");
   const int64_t na = Count(a), nb = Count(b);
-  B_ENSURE(c, nb > 0 && na % nb == 0 &&
-                  (na == nb || nb == a->dims->data[a->dims->size - 1]),
-           "ADD/MUL: only same-shape or last-dimension broadcast is supported");
+  const bool plain = nb > 0 && na % nb == 0 && (na == nb || nb == a->dims->data[a->dims->size - 1]);
+  if (MUL)
+    B_ENSURE(c, plain || (nb > 0 && ImageChannelBroadcast(a, b)),
+             "MUL: only same-shape, last-dimension or [B,H,W,C] x [B,1,1,C] broadcast is supported");
+  else
+    B_ENSURE(c, plain, "ADD/MUL: only same-shape or last-dimension broadcast is supported");
   TfLiteIntArray* dims = LceB200IntArrayCreate(a->dims->size);
   for (int i = 0; i < a->dims->size; ++i) dims->data[i] = a->dims->data[i];
   return c->ResizeTensor(c, T(c, n->outputs, 0), dims);
@@ -343,6 +353,15 @@ TfLiteStatus EltInvoke(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* b = T(c, n->inputs, 1);
   TfLiteTensor* out = T(c, n->outputs, 0);
   B_ENSURE(c, OnDevice(b->data.raw), "float builtins need device-resident operands");
+  const int64_t na = Count(a), nb = Count(b);
+  if (MUL && na != nb && nb != a->dims->data[a->dims->size - 1]) {   // [B,1,1,C] (EltPrepare)
+    const lce_gate_desc gate{b->data.f, nullptr, nullptr, nullptr};
+    const int ch = a->dims->data[3];
+    B_CAPI(c, lce_b200_f32_gate_sign(a->data.f, &gate, nullptr, P(n).activation, a->dims->data[0],
+                                     na / (static_cast<int64_t>(a->dims->data[0]) * ch), ch,
+                                     out->data.f, nullptr, lce_b200_get_stream()));
+    return kTfLiteOk;
+  }
   if (MUL) B_CAPI(c, lce_b200_f32_mul(a->data.f, b->data.f, out->data.f, Count(a), Count(b),
                                       P(n).activation, lce_b200_get_stream()));
   else B_CAPI(c, lce_b200_f32_add(a->data.f, b->data.f, out->data.f, Count(a), Count(b),
@@ -359,6 +378,18 @@ TfLiteStatus ReluInvoke(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* a = T(c, n->inputs, 0);
   B_CAPI(c, lce_b200_f32_activation(a->data.f, T(c, n->outputs, 0)->data.f, Count(a), LCE_ACT_RELU,
                                     lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+TfLiteStatus LogisticPrepare(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  B_ENSURE(c, x && x->type == kTfLiteFloat32, "LOGISTIC: only float32 is supported");
+  return SameShapePrepare(c, n);
+}
+TfLiteStatus LogisticInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  B_CAPI(c, lce_b200_f32_logistic(x->data.f, T(c, n->outputs, 0)->data.f, Count(x),
+                                  lce_b200_get_stream()));
   return kTfLiteOk;
 }
 
@@ -646,8 +677,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   static TfLiteRegistration fc = {Init, Free, FcPrepare, FcInvoke};
   static TfLiteRegistration maxp = {Init, Free, PoolPrepare, PoolInvoke<true>};
   static TfLiteRegistration avgp = {Init, Free, PoolPrepare, PoolInvoke<false>};
-  static TfLiteRegistration add = {Init, Free, EltPrepare, EltInvoke<false>};
-  static TfLiteRegistration mul = {Init, Free, EltPrepare, EltInvoke<true>};
+  static TfLiteRegistration add = {Init, Free, EltPrepare<false>, EltInvoke<false>};
+  static TfLiteRegistration mul = {Init, Free, EltPrepare<true>, EltInvoke<true>};
   static TfLiteRegistration relu = {Init, Free, SameShapePrepare, ReluInvoke};
   static TfLiteRegistration mean = {Init, Free, MeanPrepare, MeanInvoke};
   static TfLiteRegistration softmax = {Init, Free, SameShapePrepare, SoftmaxInvoke};
@@ -673,6 +704,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(6, &dequant);  // DEQUANTIZE
   static TfLiteRegistration prelu = {Init, Free, PreluPrepare, PreluInvoke};
   r->AddBuiltin(54, &prelu);   // PRELU
+  static TfLiteRegistration logistic = {Init, Free, LogisticPrepare, LogisticInvoke};
+  r->AddBuiltin(14, &logistic);  // LOGISTIC
 }
 
 }  // namespace lce_b200

@@ -480,6 +480,160 @@ int Graph::FuseResidualPairs() {
   return removed;
 }
 
+extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_GATE(const TfLiteRegistration* original);
+
+int Graph::FuseChannelGates() {
+  if (!device_arena_) return 0;
+  const size_t none = nodes_.size() + 1;
+  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
+  auto consumers = [&](int t) {
+    std::vector<size_t> c;
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
+    return c;
+  };
+  auto sole_consumer = [&](int t) {
+    if (is_output(t)) return none;
+    const std::vector<size_t> c = consumers(t);
+    return c.size() == 1 ? c[0] : none;
+  };
+  auto activation = [&](const NodeRecord& n) {
+    return n.builtin_blob.size() >= sizeof(BuiltinParams)
+               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())->activation
+               : 0;
+  };
+  // node k is the builtin `name` with two inputs, the first x, and one float output
+  auto binary = [&](size_t k, const char* name, int x) {
+    if (k >= nodes_.size()) return false;
+    const NodeRecord& n = *nodes_[k];
+    return n.name == name && !n.initialized && n.node.inputs->size == 2 && n.node.outputs->size == 1 &&
+           n.node.inputs->data[0] == x && tensors_[n.node.outputs->data[0]].type == kTfLiteFloat32;
+  };
+  // node k is op(x, v) with v a per-channel float constant ([1, ..., 1, C]) and no fused
+  // activation: returns v, else -1
+  auto const_op = [&](size_t k, const char* name, int x, int C) {
+    if (!binary(k, name, x) || activation(*nodes_[k]) != 0) return -1;
+    const int v = nodes_[k]->node.inputs->data[1];
+    if (v < 0) return -1;
+    const TfLiteTensor& t = tensors_[v];
+    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
+        t.dims->data[t.dims->size - 1] != C)
+      return -1;
+    for (int d = 0; d + 1 < t.dims->size; ++d)
+      if (t.dims->data[d] != 1) return -1;
+    return v;
+  };
+  // tensor t exists before node i runs
+  auto ready_before = [&](int t, size_t i) {
+    if (std::find(inputs_.begin(), inputs_.end(), t) != inputs_.end()) return true;
+    for (size_t k = 0; k < i; ++k)
+      for (int q = 0; q < nodes_[k]->node.outputs->size; ++q)
+        if (nodes_[k]->node.outputs->data[q] == t) return true;
+    return false;
+  };
+  auto same_dims = [](const TfLiteIntArray* a, const TfLiteIntArray* b) {
+    if (!a || !b || a->size != b->size) return false;
+    for (int k = 0; k < a->size; ++k)
+      if (a->data[k] != b->data[k]) return false;
+    return true;
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    NodeRecord& b = *nodes_[i];
+    if (b.name != "LceBconv2d" || b.initialized || b.node.inputs->size != 5 || b.node.outputs->size != 1)
+      continue;
+    TfLiteRegistration* gate_reg = lce_b200_internal_Register_BCONV_2D_GATE(b.registration);
+    if (gate_reg == nullptr) continue;
+    const int y = b.node.outputs->data[0];
+    const TfLiteIntArray* yd = tensors_[y].dims;
+    if (tensors_[y].type != kTfLiteFloat32 || !yd || yd->size != 4) continue;
+    const int C = yd->data[3];
+    // MUL(y, g): g a computed float [B, 1, 1, C]
+    const size_t km = sole_consumer(y);
+    if (!binary(km, "builtin:18", y) || activation(*nodes_[km]) != 0) continue;
+    const int g = nodes_[km]->node.inputs->data[1];
+    if (g < 0 || g == y) continue;
+    const TfLiteTensor& gt = tensors_[g];
+    if (gt.type != kTfLiteFloat32 || gt.allocation_type == kTfLiteMmapRo || !gt.dims || gt.dims->size != 4 ||
+        gt.dims->data[0] != yd->data[0] || gt.dims->data[1] != 1 || gt.dims->data[2] != 1 ||
+        gt.dims->data[3] != C || !ready_before(g, i))
+      continue;
+    // PRELU(t, alpha [1, ..., 1, C])
+    const int t1 = nodes_[km]->node.outputs->data[0];
+    const size_t kp = sole_consumer(t1);
+    const int alpha = const_op(kp, "builtin:54", t1, C);
+    if (alpha < 0) continue;
+    // ADD(u, shortcut), the shortcut a computed float tensor of y's shape; its activation applies
+    const int t2 = nodes_[kp]->node.outputs->data[0];
+    const size_t ka = sole_consumer(t2);
+    if (ka >= nodes_.size()) continue;
+    const NodeRecord& a = *nodes_[ka];
+    if (a.name != "builtin:0" || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1)
+      continue;
+    const int in0 = a.node.inputs->data[0], in1 = a.node.inputs->data[1];
+    if (in0 == in1 || (in0 != t2 && in1 != t2)) continue;
+    const int r = in0 == t2 ? in1 : in0;
+    if (r < 0 || tensors_[r].type != kTfLiteFloat32 || tensors_[r].allocation_type == kTfLiteMmapRo ||
+        !same_dims(tensors_[r].dims, yd) || !ready_before(r, i))
+      continue;
+    const int o = a.node.outputs->data[0];
+    if (tensors_[o].type != kTfLiteFloat32) continue;
+    const int32_t add_act = activation(a);
+    std::vector<size_t> absorbed{km, kp, ka};
+    // the next block's BatchNorm and sign: MUL(o, scale) -> ADD(shift) -> LceQuantize, when the
+    // convolution is ungrouped (the fused sign-pack needs groups == 1)
+    int sc = -1, sh = -1, packed = -1;
+    const TfLiteIntArray* xs = tensors_[b.node.inputs->data[0]].dims;
+    const TfLiteIntArray* fs = tensors_[b.node.inputs->data[1]].dims;
+    const bool ungrouped = xs && fs && xs->size == 4 && fs->size == 4 && xs->data[3] == fs->data[3];
+    for (size_t c : consumers(o)) {
+      if (!ungrouped) break;
+      const int v1 = const_op(c, "builtin:18", o, C);
+      if (v1 < 0) continue;
+      const int t3 = nodes_[c]->node.outputs->data[0];
+      const size_t k2 = sole_consumer(t3);
+      const int v2 = const_op(k2, "builtin:0", t3, C);
+      if (v2 < 0) continue;
+      const size_t kq = sole_consumer(nodes_[k2]->node.outputs->data[0]);
+      if (kq >= nodes_.size()) continue;
+      const NodeRecord& q = *nodes_[kq];
+      if (q.name != "LceQuantize" || q.initialized || q.node.inputs->size != 1 || q.node.outputs->size != 1 ||
+          tensors_[q.node.outputs->data[0]].type != kTfLiteInt32)
+        continue;
+      sc = v1; sh = v2; packed = q.node.outputs->data[0];
+      absorbed.insert(absorbed.end(), {c, k2, kq});
+      break;
+    }
+    std::vector<int> ins(b.node.inputs->data, b.node.inputs->data + 5);
+    ins.insert(ins.end(), {r, g, alpha, sc, sh});
+    std::vector<int> outs{o};
+    if (packed >= 0) outs.push_back(packed);
+    LceB200IntArrayFree(b.node.inputs);
+    LceB200IntArrayFree(b.node.outputs);
+    b.node.inputs = MakeDims(ins);
+    b.node.outputs = MakeDims(outs);
+    b.registration = gate_reg;
+    b.builtin_blob.assign(reinterpret_cast<const uint8_t*>(&add_act),
+                          reinterpret_cast<const uint8_t*>(&add_act) + 4);
+    b.node.builtin_data = b.builtin_blob.data();
+    b.name = packed >= 0 ? "LceBconv2d+MUL+PRELU+ADD+MUL+ADD+LceQuantize" : "LceBconv2d+MUL+PRELU+ADD";
+    // drop the absorbed nodes (all after node i), the highest index first
+    std::sort(absorbed.begin(), absorbed.end());
+    for (auto it = absorbed.rbegin(); it != absorbed.rend(); ++it) {
+      NodeRecord& n = *nodes_[*it];
+      LceB200IntArrayFree(n.node.inputs);
+      LceB200IntArrayFree(n.node.outputs);
+      LceB200IntArrayFree(n.node.temporaries);
+      LceB200IntArrayFree(n.node.intermediates);
+      nodes_.erase(nodes_.begin() + *it);
+      ++removed;
+    }
+  }
+  allocated_ = false;
+  return removed;
+}
+
 const TfLiteRegistration* FusedPoolDepthwiseRegistration();  // builtin_ops.cc
 const TfLiteRegistration* FusedStemRegistration();
 const TfLiteRegistration* ActivationChainRegistration();

@@ -83,6 +83,20 @@ class Graph {
   // the graph is left as it is. Bit-identical. Returns the number of nodes removed.
   int FuseActivationChains();
 
+  // Real-to-Binary Net's gated block tail
+  //   LceBconv2d(float y) -> MUL(y, g [B,1,1,C]) -> PRELU(alpha) -> ADD(shortcut)
+  //     [-> MUL(scale) -> ADD(shift) -> LceQuantize, the next block's BatchNorm and sign]
+  // becomes one node "LceBconv2d+MUL+PRELU+ADD[+MUL+ADD+LceQuantize]"
+  // (lce_b200_bconv2d_run_fused_gate): inputs [in, filter, mul, bias, thr, shortcut, g, alpha,
+  // scale, shift (-1 when the sign tail is absent)], outputs [sum, packed signs?]. Only when g is
+  // a computed float [B,1,1,C] tensor, alpha / scale / shift are float constants of shape
+  // [1, ..., 1, C], the MULs and the BatchNorm ADD have no fused activation (the shortcut ADD's is
+  // applied), every intermediate has a single consumer and is not a graph output, and g and the
+  // shortcut exist before the convolution runs. Run before FuseActivationChains, which would
+  // otherwise take the BatchNorm's ADD -> LceQuantize as a lone RSign. Bit-identical. Returns the
+  // number of nodes removed.
+  int FuseChannelGates();
+
   // Two consecutive residual blocks x1 = x0 + f1(sign x0), x2 = x1 + f2(sign x1) -- a
   // "LceBconv2d+ADD+LceQuantize" node whose two outputs only the next "LceBconv2d+ADD[+LceQuantize]"
   // node reads, as its packed input and its shortcut -- become one node

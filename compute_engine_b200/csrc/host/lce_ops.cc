@@ -704,6 +704,76 @@ TfLiteStatus PairEval(TfLiteContext* context, TfLiteNode* node) {
   return kTfLiteOk;
 }
 
+// ------------------------------------------------------------------------- //
+// Real-to-Binary's gated block in one node (Graph::FuseChannelGates):
+// [in, filter, mul, bias, thr, residual, gate [B,1,1,C], alpha, sign_scale, sign_shift]
+// -> [out, packed_out?]; absent vectors are -1; builtin_data: the shortcut ADD's activation.
+// ------------------------------------------------------------------------- //
+// The node seen as a fused residual block [in, filter, mul, bias, thr, residual] -> its outputs.
+struct GateBlockView {
+  TfLiteNode node{};
+  explicit GateBlockView(const TfLiteNode* gated) {
+    node.inputs = LceB200IntArrayCreate(6);
+    for (int i = 0; i < 6; ++i) node.inputs->data[i] = gated->inputs->data[i];
+    node.outputs = LceB200IntArrayCreate(gated->outputs->size);
+    for (int i = 0; i < gated->outputs->size; ++i) node.outputs->data[i] = gated->outputs->data[i];
+    node.user_data = gated->user_data;
+  }
+  ~GateBlockView() {
+    LceB200IntArrayFree(node.inputs);
+    LceB200IntArrayFree(node.outputs);
+  }
+};
+
+template <KernelType kt>
+TfLiteStatus GatePrepare(TfLiteContext* context, TfLiteNode* node) {
+  LCE_ENSURE(context, node->inputs->size == 10);
+  GateBlockView v(node);
+  if (BconvPrepare<kt, true>(context, &v.node) != kTfLiteOk) return kTfLiteError;
+  const lce_bconv2d_desc& d = static_cast<BconvOpData*>(node->user_data)->desc;
+  const TfLiteTensor* gate = GetInput(context, node, 6);
+  LCE_ENSURE_MSG(context,
+                 gate != nullptr && gate->type == kTfLiteFloat32 && NumDims(gate) == 4 &&
+                     Dim(gate, 0) == d.batch && Dim(gate, 1) == 1 && Dim(gate, 2) == 1 &&
+                     Dim(gate, 3) == d.channels_out,
+                 "gated LceBconv2d: the gate must be a float32 [batch, 1, 1, channels_out] tensor");
+  for (int k = 7; k < 10; ++k) {
+    const TfLiteTensor* t = GetInput(context, node, k);
+    LCE_ENSURE(context, t == nullptr || (t->type == kTfLiteFloat32 && NumElements(t) == d.channels_out));
+  }
+  return kTfLiteOk;
+}
+
+TfLiteStatus GateEval(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<BconvOpData*>(node->user_data);
+  if (BconvEnsurePlan(context, node) != kTfLiteOk) return kTfLiteError;
+  const TfLiteTensor* input = GetInput(context, node, 0);
+  const TfLiteTensor* residual = GetInput(context, node, 5);
+  const TfLiteTensor* gate = GetInput(context, node, 6);
+  TfLiteTensor* output = GetOutput(context, node, 0);
+  TfLiteTensor* packed = node->outputs->size > 1 ? GetOutput(context, node, 1) : nullptr;
+  int add_act = LCE_ACT_NONE;
+  if (node->builtin_data) add_act = *static_cast<const int32_t*>(node->builtin_data);
+  LCE_ENSURE_MSG(context, OnDevice(input->data.raw) && OnDevice(output->data.raw) &&
+                              OnDevice(residual->data.raw) && OnDevice(gate->data.raw),
+                 "gated LceBconv2d needs a device arena");
+  auto vec = [&](int k) {
+    const TfLiteTensor* v = GetInput(context, node, k);
+    return v ? v->data.f : nullptr;
+  };
+  const lce_gate_desc gd{gate->data.f, vec(7), vec(8), vec(9)};
+  LCE_ENSURE_CAPI(context, lce_b200_bconv2d_run_fused_gate(
+                               op->plan, input->data.i32, &gd, residual->data.f, add_act,
+                               output->data.f, packed ? packed->data.i32 : nullptr, g_stream));
+  return kTfLiteOk;
+}
+
+template <KernelType kt>
+TfLiteRegistration* BconvGateRegistration() {
+  static TfLiteRegistration r = {BconvInit, BconvFree, GatePrepare<kt>, GateEval};
+  return &r;
+}
+
 template <KernelType kt>
 TfLiteRegistration* BconvPairRegistration() {
   static TfLiteRegistration r = {PairInit, PairFree, PairPrepare<kt>, PairEval};
@@ -760,6 +830,19 @@ TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_PAIR(const TfLiteRegistr
     return BconvPairRegistration<KernelType::kOptimizedBGEMM>();
   if (fused == BconvFusedRegistration<KernelType::kOptimizedIndirectBGEMM>())
     return BconvPairRegistration<KernelType::kOptimizedIndirectBGEMM>();
+  return nullptr;
+}
+
+// host-internal: the gated-block node created by Graph::FuseChannelGates from a plain LceBconv2d
+// node of this registration (nullptr: not one of this library's LceBconv2d registrations)
+TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_GATE(const TfLiteRegistration* original) {
+  if (original == BconvRegistration<KernelType::kCuda>()) return BconvGateRegistration<KernelType::kCuda>();
+  if (original == BconvRegistration<KernelType::kReference>())
+    return BconvGateRegistration<KernelType::kReference>();
+  if (original == BconvRegistration<KernelType::kOptimizedBGEMM>())
+    return BconvGateRegistration<KernelType::kOptimizedBGEMM>();
+  if (original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
+    return BconvGateRegistration<KernelType::kOptimizedIndirectBGEMM>();
   return nullptr;
 }
 

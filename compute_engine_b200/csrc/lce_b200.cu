@@ -188,24 +188,30 @@ size_t imma_smem_budget(int V, bool b1) {
   return (227u * 1024u / ctas - 1024u - 256u) & ~size_t{127};
 }
 
-template <int V, int OUT, bool B1, bool CHAIN = false>
+template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(imma_smem_budget(V, B1))));
-  lce::bconv_imma_kernel<V, OUT, B1, CHAIN><<<grid, lce::kIThreads, smem, s>>>(p);
+  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE><<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
-// chain: float output with p.chain applied in the epilogue (bconv_run_impl decides)
+// Epilogue tails of the float output beyond run_fused's (bconv_run_impl decides).
+enum class Tail { kNone, kChain, kGate };   // p.chain / p.gate applied in the epilogue
+
 template <int V>
-int launch_imma_v(int out_type, bool b1, bool chain, const lce::ConvKParams& p, dim3 grid,
+int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, dim3 grid,
                   size_t smem, cudaStream_t s) {
-  if (chain) {
+  if (tail == Tail::kChain) {
     if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, true>(p, grid, smem, s);
     return launch_imma_vo<V, LCE_OUT_FLOAT, false, true>(p, grid, smem, s);
+  }
+  if (tail == Tail::kGate) {
+    if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, true>(p, grid, smem, s);
+    return launch_imma_vo<V, LCE_OUT_FLOAT, false, false, true>(p, grid, smem, s);
   }
   if (b1) {
     if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, true>(p, grid, smem, s);
@@ -231,7 +237,7 @@ int tc_launch(GemmCore& c, const lce::ConvKParams& p, cudaStream_t s);
 // The plan's float output goes through the mma.sync kernel (launch_conv's first choice).
 bool takes_imma(const GemmCore& c, const lce::ConvKParams& p) { return c.wt_nat != nullptr && p.vec_store; }
 
-int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, bool chain = false) {
+int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, Tail tail = Tail::kNone) {
   p.fd_ohw = lce::make_fastdiv(static_cast<uint32_t>(p.OH) * p.OW);
   p.fd_ow = lce::make_fastdiv(p.OW);
   p.fd_cwv = lce::make_fastdiv(p.CwV);
@@ -258,12 +264,12 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, bool chain = f
     dim3 igrid(static_cast<unsigned>((p.M + lce::kIBM - 1) / lce::kIBM),
                static_cast<unsigned>(c.groups * c.tiles_per_group));
     switch (c.V) {
-      case 4: return launch_imma_v<4>(c.out_type, c.imma_b1, chain, q, igrid, ismem, s);
-      case 2: return launch_imma_v<2>(c.out_type, c.imma_b1, chain, q, igrid, ismem, s);
-      default: return launch_imma_v<1>(c.out_type, c.imma_b1, chain, q, igrid, ismem, s);
+      case 4: return launch_imma_v<4>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
+      case 2: return launch_imma_v<2>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
+      default: return launch_imma_v<1>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
     }
   }
-  if (chain) return fail("bconv2d: the chain epilogue needs the mma.sync kernel");
+  if (tail != Tail::kNone) return fail("bconv2d: the chain and gate epilogues need the mma.sync kernel");
   if (c.tc_ok) {
     // wgmma inner product: persistent 128 x BN tiles
     const int rc = tc_launch(c, p, s);
@@ -1055,7 +1061,8 @@ static size_t bconv_out_bytes(const lce_b200_bconv2d* plan) {
 
 static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* out_dev,
                           const float* residual, int residual_act, int32_t* packed_out,
-                          const lce_chain_desc* chain, void* stream) {
+                          const lce_chain_desc* chain, void* stream,
+                          const lce_gate_desc* gate = nullptr) {
   const lce_bconv2d_desc& d = plan->d;
   GemmCore& c = plan->core;
   cudaStream_t s = as_stream(stream);
@@ -1101,7 +1108,7 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
   if (chain != nullptr) {
     if (!zp_float && takes_imma(c, p)) {
       p.chain = *chain;
-      return launch_conv(c, p, s, /*chain=*/true);
+      return launch_conv(c, p, s, Tail::kChain);
     }
     // every other kernel: the fused tail without the pack, then the chain pass in place
     const int rc = bconv_run_impl(plan, in_dev, out_dev, residual, residual_act, nullptr, nullptr,
@@ -1109,6 +1116,19 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     if (rc) return rc;
     float* out = static_cast<float*>(out_dev);
     return lce_b200_f32_chain_sign(out, chain, p.M, c.cout, out, packed_out, stream);
+  }
+  if (gate != nullptr) {
+    if (!zp_float && takes_imma(c, p) && p.M < (1LL << 31)) {   // the epilogue's 32-bit image index
+      p.gate = *gate;
+      return launch_conv(c, p, s, Tail::kGate);
+    }
+    // every other kernel: the convolution alone, then the whole tail in one pass in place
+    const int rc = bconv_run_impl(plan, in_dev, out_dev, nullptr, LCE_ACT_NONE, nullptr, nullptr,
+                                  stream);
+    if (rc) return rc;
+    float* out = static_cast<float*>(out_dev);
+    return lce_b200_f32_gate_sign(out, gate, residual, residual_act, d.batch,
+                                  static_cast<int64_t>(p.OH) * p.OW, c.cout, out, packed_out, stream);
   }
   if (!zp_float) return launch_conv(c, p, s);
   // the optimised kernels' zero padding: one-padding accumulators + a float correction. The
@@ -1169,6 +1189,39 @@ int lce_b200_bconv2d_run_fused_chain(lce_b200_bconv2d* plan, const int32_t* in_d
       if (v && !is_device_ptr(v)) return fail("bconv2d_run_fused_chain: chain vectors must be device memory");
   return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev, chain,
                         stream);
+}
+
+int lce_b200_bconv2d_run_fused_gate(lce_b200_bconv2d* plan, const int32_t* in_dev,
+                                    const lce_gate_desc* gate, const float* residual_dev,
+                                    int add_activation, float* out_dev, int32_t* packed_out_dev,
+                                    void* stream) {
+  const lce_bconv2d_desc& d = plan->d;
+  if (d.out_type != LCE_OUT_FLOAT)
+    return fail("bconv2d_run_fused_gate: only float-output plans can take a gate");
+  if (packed_out_dev && d.groups != 1)
+    return fail("bconv2d_run_fused_gate: packed output needs groups == 1");
+  if (!gate || !gate->gate) return fail("bconv2d_run_fused_gate: the gate tensor is required");
+  if (add_activation < LCE_ACT_NONE || add_activation > LCE_ACT_RELU6)
+    return fail("bconv2d_run_fused_gate: unknown ADD activation %d", add_activation);
+  if (residual_dev && !aligned16(residual_dev))
+    return fail("bconv2d_run_fused_gate: residual must be 16-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(gate->gate) & 7u) != 0)
+    return fail("bconv2d_run_fused_gate: the gate must be 8-byte aligned");
+  for (const float* v : {gate->gate, gate->alpha, gate->sign_scale, gate->sign_shift})
+    if (v && !is_device_ptr(v)) return fail("bconv2d_run_fused_gate: gate vectors must be device memory");
+  // the epilogue reads the shortcut and the gate of rows other CTAs write: out must not alias them
+  const uintptr_t o0 = reinterpret_cast<uintptr_t>(out_dev);
+  const uintptr_t o1 = o0 + bconv_out_bytes(plan);
+  auto overlaps = [&](const void* v, size_t bytes) {
+    const uintptr_t v0 = reinterpret_cast<uintptr_t>(v);
+    return v != nullptr && v0 < o1 && o0 < v0 + bytes;
+  };
+  if (overlaps(residual_dev, bconv_out_bytes(plan)))
+    return fail("bconv2d_run_fused_gate: output must not overlap the residual");
+  if (overlaps(gate->gate, static_cast<size_t>(d.batch) * d.channels_out * sizeof(float)))
+    return fail("bconv2d_run_fused_gate: output must not overlap the gate");
+  return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev,
+                        nullptr, stream, gate);
 }
 
 int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* plan2,

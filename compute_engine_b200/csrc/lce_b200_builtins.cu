@@ -1022,6 +1022,55 @@ __global__ void __launch_bounds__(256) chain_sign_kernel(const float* x, const l
   }
 }
 
+// lce_b200_f32_gate_sign: one pass of the gated tail (lce_b200_chain.cuh) over [batch][pixels][C],
+// threads laid out as in chain_sign_kernel. x and out may be the same buffer.
+template <bool PACK, typename I>
+__global__ void __launch_bounds__(256) gate_sign_kernel(const float* x, const lce_gate_desc gd,
+                                                        const float* __restrict__ residual, int act,
+                                                        I rows, I pixels, int channels, int cw,
+                                                        float* out, int32_t* __restrict__ packed) {
+  const bool has_a = gd.alpha != nullptr;
+  const bool has_sc = gd.sign_scale != nullptr, has_sh = gd.sign_shift != nullptr;
+  const I span = PACK ? static_cast<I>(cw) * 32 : static_cast<I>(channels);
+  const I n = rows * span;
+  const I stride = static_cast<I>(gridDim.x) * blockDim.x;   // a multiple of 32: warps stay whole
+  for (I i = static_cast<I>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const I row = i / span;
+    const int c = static_cast<int>(i - row * span);
+    bool bit = false;
+    if (!PACK || c < channels) {
+      const I e = row * channels + c;
+      const I b = row / pixels;
+      float o = lce::gate_prelu(x[e], __ldg(gd.gate + b * channels + c), has_a,
+                                has_a ? __ldg(gd.alpha + c) : 0.0f);
+      if (residual) o = __fadd_rn(o, residual[e]);
+      o = apply_act(o, act);
+      if (out) out[e] = o;
+      if (PACK)
+        bit = lce::affine_sign(o, has_sc, has_sc ? __ldg(gd.sign_scale + c) : 0.0f, has_sh,
+                               has_sh ? __ldg(gd.sign_shift + c) : 0.0f);
+    }
+    if (PACK) {
+      const unsigned word = __ballot_sync(0xffffffffu, bit);
+      if ((threadIdx.x & 31) == 0) packed[i >> 5] = static_cast<int32_t>(word);
+    }
+  }
+}
+
+// LOGISTIC, TFLite's float reference (reference/logistic.h) with CUDA's expf
+__global__ void __launch_bounds__(256) logistic_kernel(const float* __restrict__ in,
+                                                       float* __restrict__ out, long long n) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += stride) {
+    const float x = in[i];
+    float r;
+    if (x > 16.619047164916992188f) r = 1.0f;
+    else if (x < -9.0f) r = expf(x);
+    else r = 1.0f / (1.0f + expf(-x));
+    out[i] = r;
+  }
+}
+
 // mean over H*W: one thread per (b, c), c fastest => coalesced rows.
 __global__ void __launch_bounds__(256) mean_hw_kernel(const float* __restrict__ in,
                                                       float* __restrict__ out, int B, int HW,
@@ -1831,6 +1880,46 @@ int lce_b200_f32_chain_sign(const float* x, const lce_chain_desc* chain, int64_t
       chain_sign_kernel<false, long long><<<grid, 256, 0, s>>>(x, ch, rows, channels, cw, out, packed);
   }
   return launch_check("chain_sign_kernel");
+}
+
+int lce_b200_f32_gate_sign(const float* x, const lce_gate_desc* gate, const float* residual, int act,
+                           int64_t batch, int64_t pixels, int channels, float* out, int32_t* packed,
+                           void* stream) {
+  if (batch < 0 || pixels < 0 || channels <= 0)
+    return fail("gate_sign: bad shape (%lld images, %lld pixels, %d channels)",
+                static_cast<long long>(batch), static_cast<long long>(pixels), channels);
+  if (!gate || !gate->gate) return fail("gate_sign: the gate tensor is required");
+  if (act < LCE_ACT_NONE || act > LCE_ACT_RELU6) return fail("gate_sign: unknown activation %d", act);
+  const long long rows = batch * pixels;
+  if (rows == 0 || (out == nullptr && packed == nullptr)) return 0;
+  const int cw = (channels + 31) / 32;
+  const long long n = packed ? rows * cw * 32 : rows * static_cast<long long>(channels);
+  const int grid = grid_for(n, 256);
+  cudaStream_t s = as_stream(stream);
+  const bool narrow = n + 256LL * grid < (1LL << 31) && batch * static_cast<long long>(channels) < (1LL << 31);
+  if (packed) {
+    if (narrow)
+      gate_sign_kernel<true, int><<<grid, 256, 0, s>>>(x, *gate, residual, act, static_cast<int>(rows),
+                                                       static_cast<int>(pixels), channels, cw, out, packed);
+    else
+      gate_sign_kernel<true, long long><<<grid, 256, 0, s>>>(x, *gate, residual, act, rows, pixels, channels,
+                                                             cw, out, packed);
+  } else {
+    if (narrow)
+      gate_sign_kernel<false, int><<<grid, 256, 0, s>>>(x, *gate, residual, act, static_cast<int>(rows),
+                                                        static_cast<int>(pixels), channels, cw, out, packed);
+    else
+      gate_sign_kernel<false, long long><<<grid, 256, 0, s>>>(x, *gate, residual, act, rows, pixels, channels,
+                                                              cw, out, packed);
+  }
+  return launch_check("gate_sign_kernel");
+}
+
+int lce_b200_f32_logistic(const float* in, float* out, int64_t n, void* stream) {
+  if (n < 0) return fail("logistic: bad size %lld", static_cast<long long>(n));
+  if (n == 0) return 0;
+  logistic_kernel<<<grid_for(n, 256), 256, 0, as_stream(stream)>>>(in, out, n);
+  return launch_check("logistic_kernel");
 }
 
 int lce_b200_f32_mean_hw_act(const float* in, float* out, int batch, int h, int w, int c, int pre_activation,

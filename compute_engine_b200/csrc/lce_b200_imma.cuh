@@ -304,14 +304,18 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // (host-checked). CHAIN (float output): ReActNet's chain on the fused sum. Its four vectors and
 // the output transform's multiplier and bias are read per row from chain_s = [shift_in | alpha |
 // shift_out | sign_shift | mul | bias] x 64 channels in shared memory: holding them all in
-// registers would exceed the b1 instances' 128-register cap.
-template <int OUT, int S, bool CHAIN = false>
+// registers would exceed the b1 instances' 128-register cap. GATE (float output): Real-to-Binary's
+// gated tail (p.gate) before the shortcut ADD, from chain_s = [- | alpha | sign_scale | sign_shift
+// | mul | bias]; the gate row is each row's own image's (a tile can span several images).
+template <int OUT, int S, bool CHAIN = false, bool GATE = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
                                               int tig, const float* chain_s = nullptr) {
+  static_assert(!(CHAIN && GATE), "one epilogue tail at a time");
+  constexpr bool STAGED = CHAIN || GATE;
   const int cth = c_tile + tig * 2;
   float2 mul_r[8], bias_r[8];
-  if (OUT == LCE_OUT_FLOAT && !CHAIN) {
+  if (OUT == LCE_OUT_FLOAT && !STAGED) {
 #pragma unroll
     for (int ns = 0; ns < 8; ++ns) {
       mul_r[ns] = *reinterpret_cast<const float2*>(p.mul + cth + ns * 8);
@@ -355,7 +359,7 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           } else {
             x0 <<= 1; x1 <<= 1;
           }
-          if constexpr (CHAIN) {
+          if constexpr (STAGED) {
             const float2 mu = *reinterpret_cast<const float2*>(chain_s + 4 * kBN + tig * 2 + ns * 8);
             const float2 bi = *reinterpret_cast<const float2*>(chain_s + 5 * kBN + tig * 2 + ns * 8);
             y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mu.x, bi.x);
@@ -364,6 +368,19 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
             y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mul_r[ns].x, bias_r[ns].x);
             y[2 * ns + 1] =
                 transform_float_x2(x1, p.clamp_min, p.clamp_max, mul_r[ns].y, bias_r[ns].y);
+          }
+        }
+        if constexpr (GATE) {
+          // MUL(gate) -> PRELU(alpha): gate row b = m / (OH * OW) (M < 2^31, host-checked)
+          const uint32_t b = fdiv(static_cast<uint32_t>(m), p.fd_ohw);
+          const float* gr = p.gate.gate + static_cast<size_t>(b) * p.cout + cth;
+          const bool has_a = p.gate.alpha != nullptr;
+#pragma unroll
+          for (int ns = 0; ns < 8; ++ns) {
+            const float2 gv = __ldg(reinterpret_cast<const float2*>(gr + ns * 8));
+            const float2 al = *reinterpret_cast<const float2*>(chain_s + kBN + tig * 2 + ns * 8);
+            y[2 * ns] = gate_prelu(y[2 * ns], gv.x, has_a, al.x);
+            y[2 * ns + 1] = gate_prelu(y[2 * ns + 1], gv.y, has_a, al.y);
           }
         }
         if (has_res) {
@@ -379,6 +396,13 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
             y[2 * ns + 1] = __fadd_rn(y[2 * ns + 1], rv[ns].y);
           }
           if (ract != LCE_ACT_NONE) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], act_lo), act_hi);
+          }
+        }
+        if constexpr (GATE) {
+          // the gated tail applies the activation with or without a shortcut
+          if (!has_res && ract != LCE_ACT_NONE) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], act_lo), act_hi);
           }
@@ -414,6 +438,22 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
               bits1 |= ((chain_sign(y[2 * ns + 8], has_ss, s1.x) ? 1u : 0u) |
                         (chain_sign(y[2 * ns + 9], has_ss, s1.y) ? 2u : 0u)) << (ns * 8);
             }
+          } else if constexpr (GATE) {
+            // the next block's BatchNorm and sign: bit of o * sign_scale + sign_shift
+            const bool has_sc = p.gate.sign_scale != nullptr, has_sh = p.gate.sign_shift != nullptr;
+            const float* sc = chain_s + 2 * kBN + tig * 2;
+            const float* sh = chain_s + 3 * kBN + tig * 2;
+#pragma unroll
+            for (int ns = 0; ns < 4; ++ns) {
+              const float2 c0 = *reinterpret_cast<const float2*>(sc + ns * 8);
+              const float2 c1 = *reinterpret_cast<const float2*>(sc + ns * 8 + 32);
+              const float2 h0 = *reinterpret_cast<const float2*>(sh + ns * 8);
+              const float2 h1 = *reinterpret_cast<const float2*>(sh + ns * 8 + 32);
+              bits0 |= ((affine_sign(y[2 * ns], has_sc, c0.x, has_sh, h0.x) ? 1u : 0u) |
+                        (affine_sign(y[2 * ns + 1], has_sc, c0.y, has_sh, h0.y) ? 2u : 0u)) << (ns * 8);
+              bits1 |= ((affine_sign(y[2 * ns + 8], has_sc, c1.x, has_sh, h1.x) ? 1u : 0u) |
+                        (affine_sign(y[2 * ns + 9], has_sc, c1.y, has_sh, h1.y) ? 2u : 0u)) << (ns * 8);
+            }
           } else {
             // LceQuantize of the value just written: bit = value < 0 (bitpack.h:159)
 #pragma unroll
@@ -443,8 +483,9 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 
 // B1 selects the inner product: packed b1 fragments (accumulators at scale 1) or int8 ones
 // (scale 8). Both produce the same int32 accumulators. CHAIN (float output): the epilogue also
-// applies p.chain (lce_b200_bconv2d_run_fused_chain); the other instances compile as without it.
-template <int V, int OUT, bool B1, bool CHAIN = false>
+// applies p.chain (lce_b200_bconv2d_run_fused_chain); GATE (float output): p.gate
+// (lce_b200_bconv2d_run_fused_gate). The other instances compile as without them.
+template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false>
 __global__ void __launch_bounds__(kIThreads, B1 ? kB1Ctas : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
   using Vec = typename VecT<V>::T;
@@ -568,6 +609,22 @@ bconv_imma_kernel(const ConvKParams p) {
     }
     __syncthreads();
     epilogue_imma<OUT, S, true>(p, acc, m0, c_tile, warp, gid, tig, cs);
+  } else if constexpr (GATE) {
+    // likewise the gated tail's per-channel vectors (slot 0 unused); the gate itself is per image
+    // and is read per row
+    float* cs = reinterpret_cast<float*>(smem_raw);
+    for (int i = tid; i < 6 * kBN; i += kIThreads) {
+      const int k = i / kBN;
+      const float* v = k == 1   ? p.gate.alpha
+                       : k == 2 ? p.gate.sign_scale
+                       : k == 3 ? p.gate.sign_shift
+                       : k == 4 ? p.mul
+                       : k == 5 ? p.bias
+                                : nullptr;
+      cs[i] = v != nullptr ? __ldg(v + c_tile + (i & (kBN - 1))) : 0.0f;
+    }
+    __syncthreads();
+    epilogue_imma<OUT, S, false, true>(p, acc, m0, c_tile, warp, gid, tig, cs);
   } else {
     epilogue_imma<OUT, S>(p, acc, m0, c_tile, warp, gid, tig);
   }

@@ -95,6 +95,9 @@ struct ConvKParams {
   // mma.sync kernel, CHAIN instances only: ReActNet's per-channel chain on the fused sum
   // (lce_b200_chain.cuh); packed_out then holds the signs of o + sign_shift
   lce_chain_desc chain;
+  // GATE instances only: Real-to-Binary's gated tail before the shortcut ADD; packed_out then
+  // holds the signs of o * sign_scale + sign_shift
+  lce_gate_desc gate;
 };
 
 // --------------------------- PTX helpers ---------------------------------- //

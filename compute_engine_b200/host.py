@@ -186,6 +186,12 @@ class HostGraph:
         """MAX_POOL_2D(2x2 s1 VALID) -> DEPTHWISE_CONV_2D(3x3) => one node."""
         return lib().lce_host_fuse_float_glue(self._g)
 
+    def fuse_channel_gates(self):
+        """LceBconv2d -> MUL(gate [B,1,1,C]) -> PRELU -> ADD(shortcut) [-> MUL -> ADD -> LceQuantize]
+        (Real-to-Binary Net's gated block and the next block's BatchNorm and sign) => one node.
+        Call before fuse_activation_chains and allocate_tensors."""
+        return lib().lce_host_fuse_channel_gates(self._g)
+
     def fuse_activation_chains(self):
         """ADD -> PRELU -> ADD [-> ADD -> LceQuantize] (ReActNet's RPReLU / RSign, each step
         optional) => the epilogue of the preceding fused LceBconv2d+ADD node, or one node.
@@ -198,8 +204,8 @@ class HostGraph:
         return lib().lce_host_fuse_residual_pairs(self._g)
 
     def fuse_all(self):
-        return (self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_activation_chains()
-                + self.fuse_residual_pairs())
+        return (self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_channel_gates()
+                + self.fuse_activation_chains() + self.fuse_residual_pairs())
 
     # ---- profiling / async IO (bench.py) ----
     def enable_profiling(self, on=True):

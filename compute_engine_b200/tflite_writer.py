@@ -111,7 +111,7 @@ TENSOR_TYPE = {np.dtype(np.float32): 0, np.dtype(np.int32): 2, np.dtype(np.uint8
 OP = {"ADD": 0, "AVERAGE_POOL_2D": 1, "CONV_2D": 3, "DEPTHWISE_CONV_2D": 4,
       "FULLY_CONNECTED": 9, "MAX_POOL_2D": 17, "MUL": 18, "RELU": 19, "RESHAPE": 22,
       "SOFTMAX": 25, "MEAN": 40, "CUSTOM": 32, "CONCATENATION": 2, "PAD": 34, "PADV2": 60,
-      "DEQUANTIZE": 6, "PRELU": 54}
+      "DEQUANTIZE": 6, "PRELU": 54, "LOGISTIC": 14}
 # BuiltinOptions union tags (schema_generated.h:1652-1694)
 OPT_TAG = {"CONV_2D": 1, "DEPTHWISE_CONV_2D": 2, "AVERAGE_POOL_2D": 5, "MAX_POOL_2D": 5,
            "FULLY_CONNECTED": 8, "SOFTMAX": 9, "ADD": 11, "MUL": 21, "RESHAPE": 17, "MEAN": 27,

@@ -1,4 +1,4 @@
-"""Synthetic model zoo: the three model families the benchmark runs, emitted as real
+"""Synthetic model zoo: the model families the graph host runs, emitted as real
 `.tflite` graphs with the op sequence the LCE converter produces (LceQuantize ->
 LceBconv2d with folded BatchNorm multiplier/bias and fused ReLU -> ADD shortcut ...),
 random weights (seeded), correct topology.
@@ -280,5 +280,74 @@ def reactnet_a(batch=1, seed=0, image=224, input_type="float32"):
     return g.m.serialize()
 
 
+def realtobinarynet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    """Real-to-Binary Net, restated from the paper (Martinez et al., ICLR 2020): ResNet-18 with
+    Bi-Real's one shortcut per binary convolution, 4 stages x 4 blocks at 64 / 128 / 256 / 512
+    channels (16 LceBconv2d), each binary convolution's output scaled by a gate computed from the
+    block's real-valued input. In the converter's op order:
+      stem CONV_2D 7x7/s2 3 -> 64 (BN folded) -> PRELU -> MAX_POOL_2D 3x3/s2 SAME;
+      block x [B,H,W,Cin] -> [B,H',W',Cout] (stride 2 and Cout = 2 Cin on the first block of
+      stages 2-4): the shortcut first (x, or AVERAGE_POOL_2D 2x2/s2 VALID -> CONV_2D 1x1, BN
+      folded); the gate MEAN(x, [1, 2]) -> FULLY_CONNECTED Cin -> Cin/8 (RELU, no bias) ->
+      FULLY_CONNECTED Cin/8 -> Cout (no bias) -> LOGISTIC -> RESHAPE [-1, 1, 1, Cout]; the main
+      path MUL(x, bn_scale) -> ADD(bn_shift) -> LceQuantize -> LceBconv2d 3x3 (stride s,
+      `pad_values`, no fused activation) -> MUL(gate) -> PRELU(alpha [1, 1, Cout]) -> ADD(shortcut);
+      head PRELU -> MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX.
+    The BatchNorm after each binary convolution is folded into its post_activation multiplier and
+    bias, before the gate: a simplification of the paper's block, which changes nothing measured
+    with synthetic weights. The RESHAPE's -1 batch dimension keeps the graph resizable."""
+    g = _Builder(seed, batch, "RealToBinaryNet")
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+
+    def prelu(t, ts):
+        u = g.act(ts)
+        alpha = g.const(g.rng.uniform(0.05, 0.5, (1, 1, ts[3])).astype(np.float32), name="alpha")
+        g.m.add_op("PRELU", [t, alpha], [u])
+        return u
+
+    def dense(t, cin, cout, activation="NONE"):
+        wt = g.rng.standard_normal((cout, cin)).astype(np.float32) / np.float32(np.sqrt(cin))
+        y = g.act((batch, cout))
+        g.m.add_op("FULLY_CONNECTED", [t, g.const(wt), -1], [y], activation=activation)
+        return y
+
+    def gate(t, ts, cout):
+        axes = g.const(np.array([1, 2], np.int32), np.int32, "axes")
+        pooled = g.act((batch, ts[3]))
+        g.m.add_op("MEAN", [t, axes], [pooled], keep_dims=False)
+        z = dense(dense(pooled, ts[3], ts[3] // 8, "RELU"), ts[3] // 8, cout)
+        s = g.act((batch, cout))
+        g.m.add_op("LOGISTIC", [z], [s])
+        r = g.act((batch, 1, 1, cout))
+        g.m.add_op("RESHAPE", [s], [r], new_shape=[-1, 1, 1, cout])
+        return r
+
+    x, xs = g.conv(x, xs, 64, 7, 2)
+    x = prelu(x, xs)
+    x, xs = g.pool("MAX_POOL_2D", x, xs, 3, 2, "SAME")
+    for stage, cout in enumerate((64, 128, 256, 512)):
+        for blk in range(4):
+            stride = 2 if (stage > 0 and blk == 0) else 1
+            if stride == 2:
+                s, ss = g.pool("AVERAGE_POOL_2D", x, xs, 2, 2, "VALID")
+                s, _ = g.conv(s, ss, cout, 1, 1)
+            else:
+                s = x
+            gt = gate(x, xs, cout)
+            scale, shift = g.bn(xs[3])
+            t = g.act(xs)
+            g.m.add_op("MUL", [x, g.const(scale, name="bn_scale")], [t])
+            t = g.add(t, g.const(shift, name="bn_shift"), xs)
+            y, ys = g.bconv(g.quantize(t, xs), xs, cout, stride=stride, pad_values=pad_values,
+                            activation="NONE")
+            u = g.act(ys)
+            g.m.add_op("MUL", [y, gt], [u])
+            x, xs = g.add(prelu(u, ys), s, ys), ys
+    probs = g.head(prelu(x, xs), xs, relu=False)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
 MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "birealnet18": birealnet18,
-          "reactnet_a": reactnet_a}
+          "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet}

@@ -142,6 +142,33 @@ int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* p
  * out = x >= 0 ? x : x * alpha, and `channels` may be any alpha size dividing the element count. */
 int lce_b200_f32_chain_sign(const float* x_dev, const lce_chain_desc* chain, int64_t rows,
                             int channels, float* out_dev, int32_t* packed_out_dev, void* stream);
+/* Real-to-Binary Net's gated block tail (lce_gate_desc, lce_b200_types.h) behind the convolution:
+ *   out = act(prelu(OutputTransform(acc) * gate[b][c], alpha) + residual),
+ *   packed_out = bitpack(out * sign_scale + sign_shift) (optional),
+ * with b the output pixel's image. residual may be NULL (then act applies to the PRELU result);
+ * add_activation is an LCE_ACT_* code. gate_desc and gate_desc->gate are required. Float-output
+ * plans only; packed_out needs groups == 1; out must not overlap residual or the gate. The mma.sync
+ * kernel applies the tail in its epilogue; plans on another kernel, or that finish zero padding
+ * with the float correction pass, run run_fused without a residual and then
+ * lce_b200_f32_gate_sign in place. Bit-identical to the op sequence either way. */
+int lce_b200_bconv2d_run_fused_gate(lce_b200_bconv2d* plan, const int32_t* in_dev,
+                                    const lce_gate_desc* gate_desc, const float* residual_dev,
+                                    int add_activation, float* out_dev, int32_t* packed_out_dev,
+                                    void* stream);
+/* The same tail without a convolution, in one pass over a float [batch, pixels, channels] tensor:
+ * element (b, p, c) takes gate[b][c] and channel c of the other present vectors. residual (same
+ * shape as x, may be NULL), out (may be NULL when only the signs are read; may be x_dev) and
+ * packed_out[b][p][ceil(channels/32)] (may be NULL) as in run_fused_gate. With only `gate` set
+ * this is the MUL builtin of a [B,H,W,C] tensor by a [B,1,1,C] one, out = act(x * gate). */
+int lce_b200_f32_gate_sign(const float* x_dev, const lce_gate_desc* gate_desc,
+                           const float* residual_dev, int activation, int64_t batch,
+                           int64_t pixels, int channels, float* out_dev, int32_t* packed_out_dev,
+                           void* stream);
+/* The sigmoid that ends Real-to-Binary Net's gate, TFLite's LOGISTIC
+ * (TF/lite/kernels/internal/reference/logistic.h): out = 1 above 16.619047164916992188, exp(x)
+ * below -9, else 1 / (1 + exp(-x)). CUDA's expf is not libm's: within 4 ulp of the formula, not
+ * bit-identical to a CPU run. */
+int lce_b200_f32_logistic(const float* in_dev, float* out_dev, int64_t n, void* stream);
 int lce_b200_bconv2d_run_host(lce_b200_bconv2d* plan, const int32_t* in_host,
                               void* out_host);
 void lce_b200_bconv2d_destroy(lce_b200_bconv2d* plan);

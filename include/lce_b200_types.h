@@ -95,6 +95,21 @@ typedef struct lce_chain_desc {
   const float* sign_shift;
 } lce_chain_desc;
 
+/* The gated block tail of Real-to-Binary Net behind a binary convolution: MUL by a per-image,
+ * per-channel gate (the sigmoid of a squeeze-excitation branch), PRELU(alpha), the shortcut ADD,
+ * then the next block's BatchNorm and sign (MUL(sign_scale) -> ADD(sign_shift) -> LceQuantize).
+ * `gate` is a device tensor [batch][channels] and is required; the other pointers are device
+ * vectors with one float per channel, NULL when the op is absent (as in lce_chain_desc). Per
+ * element of image b, channel c, in TFLite's order and rounding:
+ *   t = s * gate[b][c];  u = t >= 0 ? t : t * alpha;  o = act(u + residual);
+ *   bit = (o * sign_scale + sign_shift) < 0 */
+typedef struct lce_gate_desc {
+  const float* gate;
+  const float* alpha;
+  const float* sign_scale;
+  const float* sign_shift;
+} lce_gate_desc;
+
 #ifdef __cplusplus
 }
 #endif
