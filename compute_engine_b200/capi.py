@@ -80,8 +80,9 @@ EXPORTS = [
     "lce_b200_bconv2d_set_zero_padding_mode", "lce_b200_path_counts", "lce_b200_tc_debug",
     "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_fused_chain",
     "lce_b200_bconv2d_run_fused_pair",
-    "lce_b200_bconv2d_run_fused_gate",
+    "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_slice",
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_logistic",
+    "lce_b200_f32_affine_sign",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -227,6 +228,25 @@ def gate_sign(x: torch.Tensor, gate, residual=None, activation=0, alpha=None, si
     return o, pk
 
 
+def affine_sign(x: torch.Tensor, channels=None, scale=None, shift=None, copy_to=None):
+    """The signs of x[..., :channels] * scale + shift over x's pixels (the last axis is the pixel
+    stride, so x may be the leading channels of a wider map). copy_to (optional): a float tensor
+    with x's pixels whose leading `channels` receive x's, bit for bit. Returns the packed signs."""
+    x = _dev(x, torch.float32)
+    ch = channels or x.shape[-1]
+    rows = x.numel() // x.shape[-1]
+    vecs = [None if v is None else _dev(v, torch.float32) for v in (scale, shift)]
+    pk = torch.empty(x.shape[:-1] + (cdiv(ch, 32),), dtype=torch.int32, device=x.device)
+    if copy_to is not None and (not copy_to.is_cuda or copy_to.dtype != torch.float32 or
+                                not copy_to.is_contiguous()):
+        raise LceError("affine_sign: copy_to must be a contiguous CUDA float32 tensor")
+    _check(lib().lce_b200_f32_affine_sign(_p(x), C.c_int64(x.shape[-1]), C.c_int64(rows), C.c_int(ch),
+                                          _p(vecs[0]), _p(vecs[1]), _p(pk), _p(copy_to),
+                                          C.c_int64(0 if copy_to is None else copy_to.shape[-1]),
+                                          _stream()))
+    return pk
+
+
 class BConv2d:
     """LceBconv2d plan: constructor = Init + Prepare + OneTimeSetup
     (LCE/tflite/kernels/bconv2d.cc:85-392), ``__call__`` = Eval (:551-564)."""
@@ -328,6 +348,20 @@ class BConv2d:
                                                      C.c_int(add_activation), _p(out), _p(pk),
                                                      _stream()))
         return out, pk
+
+    def run_slice(self, x: torch.Tensor, out: torch.Tensor, offset: int = 0):
+        """lce_b200_bconv2d_run_slice on bitpacked x: writes the float output into channels
+        [offset, offset + channels_out) of `out`, a contiguous float32 [B, OH, OW, C] map (or any
+        tensor whose last axis is the pixel stride), and nothing else. Returns out."""
+        x = _dev(x, torch.int32)
+        if tuple(x.shape[:3]) != (self.desc.batch, self.desc.in_h, self.desc.in_w):
+            self.set_input_shape(*x.shape[:3])
+        if not out.is_cuda or out.dtype != torch.float32 or not out.is_contiguous():
+            raise LceError("run_slice: out must be a contiguous CUDA float32 tensor")
+        ptr = C.c_void_p(out.data_ptr() + 4 * offset)
+        _check(lib().lce_b200_bconv2d_run_slice(self._h, _p(x), ptr, C.c_int64(out.shape[-1]),
+                                                _stream()))
+        return out
 
     def run_fused_pair(self, second, x: torch.Tensor, residual: torch.Tensor, act1=0, act2=0,
                        packed=True):

@@ -634,6 +634,181 @@ int Graph::FuseChannelGates() {
   return removed;
 }
 
+extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_DENSE(const TfLiteRegistration* original);
+extern "C" int lce_b200_internal_slice_takes(const lce_bconv2d_desc* d);   // lce_b200.cu
+
+int Graph::FuseDenseBlocks() {
+  if (!device_arena_) return 0;
+  const size_t none = nodes_.size() + 1;
+  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
+  auto consumers = [&](int t) {
+    std::vector<size_t> c;
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
+    return c;
+  };
+  auto sole_consumer = [&](int t) {
+    if (is_output(t)) return none;
+    const std::vector<size_t> c = consumers(t);
+    return c.size() == 1 ? c[0] : none;
+  };
+  auto params = [&](const NodeRecord& n) {
+    return n.builtin_blob.size() >= sizeof(BuiltinParams)
+               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())
+               : nullptr;
+  };
+  auto dims4 = [&](int t) {
+    const TfLiteIntArray* d = tensors_[t].dims;
+    return d && d->size == 4 ? d : nullptr;
+  };
+  // node k is the builtin op(x, v), v a float constant [C] or [1, ..., 1, C], with no fused
+  // activation and a float output: returns v, else -1
+  auto const_op = [&](size_t k, const char* name, int x, int C) {
+    if (k >= nodes_.size()) return -1;
+    const NodeRecord& n = *nodes_[k];
+    if (n.name != name || n.initialized || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
+        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32 ||
+        !params(n) || params(n)->activation != 0)
+      return -1;
+    const int v = n.node.inputs->data[1];
+    if (v < 0) return -1;
+    const TfLiteTensor& t = tensors_[v];
+    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
+        t.dims->data[t.dims->size - 1] != C)
+      return -1;
+    for (int d = 0; d + 1 < t.dims->size; ++d)
+      if (t.dims->data[d] != 1) return -1;
+    return v;
+  };
+  // One dense layer read from the MUL at node i: x -> MUL(scale) -> ADD(shift) -> LceQuantize ->
+  // LceBconv2d (float y, one that run_slice takes, same image size) -> CONCATENATION([x, y], last
+  // axis) = out, every intermediate read once and not a graph output.
+  struct Layer {
+    size_t mul, add, quant, conv, cat;
+    int x, scale, shift, packed, out;
+    const TfLiteRegistration* reg;
+  };
+  auto match = [&](size_t i, Layer* L) {
+    const NodeRecord& m = *nodes_[i];
+    if (m.name != "builtin:18" || m.node.inputs->size != 2) return false;
+    const int x = m.node.inputs->data[0];
+    const TfLiteIntArray* xd = x >= 0 && tensors_[x].type == kTfLiteFloat32 ? dims4(x) : nullptr;
+    if (!xd || xd->data[3] % 4 != 0) return false;
+    const int C = xd->data[3];
+    L->mul = i; L->x = x;
+    L->scale = const_op(i, "builtin:18", x, C);
+    if (L->scale < 0) return false;
+    const int t1 = m.node.outputs->data[0];
+    L->add = sole_consumer(t1);
+    L->shift = const_op(L->add, "builtin:0", t1, C);
+    if (L->shift < 0) return false;
+    const int t2 = nodes_[L->add]->node.outputs->data[0];
+    L->quant = sole_consumer(t2);
+    if (L->quant >= nodes_.size()) return false;
+    const NodeRecord& q = *nodes_[L->quant];
+    if (q.name != "LceQuantize" || q.initialized || q.node.inputs->size != 1 || q.node.outputs->size != 1)
+      return false;
+    L->packed = q.node.outputs->data[0];
+    if (tensors_[L->packed].type != kTfLiteInt32) return false;
+    L->conv = sole_consumer(L->packed);
+    if (L->conv >= nodes_.size()) return false;
+    const NodeRecord& b = *nodes_[L->conv];
+    if (b.name != "LceBconv2d" || b.initialized || b.node.inputs->size != 5 || b.node.outputs->size != 1 ||
+        b.node.inputs->data[0] != L->packed)
+      return false;
+    L->reg = lce_b200_internal_Register_BCONV_2D_DENSE(b.registration);
+    if (L->reg == nullptr) return false;   // a foreign "LceBconv2d" (e.g. the CPU test double)
+    const int y = b.node.outputs->data[0];
+    const TfLiteIntArray* yd = tensors_[y].type == kTfLiteFloat32 ? dims4(y) : nullptr;
+    const TfLiteIntArray* pd = dims4(L->packed);
+    const TfLiteIntArray* fd = dims4(b.node.inputs->data[1]);
+    if (!yd || !pd || !fd || yd->data[0] != xd->data[0] || yd->data[1] != xd->data[1] ||
+        yd->data[2] != xd->data[2])
+      return false;
+    FlexMap opts(b.custom_options.data(), b.custom_options.size());
+    lce_bconv2d_desc d{};
+    d.batch = xd->data[0]; d.in_h = xd->data[1]; d.in_w = xd->data[2];
+    d.channels_in = opts.AsInt32("channels_in");
+    d.channels_out = fd->data[0];
+    d.groups = fd->data[3] == (d.channels_in + 31) / 32 && pd->data[3] == fd->data[3] ? 1 : 0;
+    d.out_type = LCE_OUT_FLOAT;
+    if (d.channels_in != C || d.groups != 1 || yd->data[3] != d.channels_out ||
+        !lce_b200_internal_slice_takes(&d))
+      return false;
+    L->cat = sole_consumer(y);
+    if (L->cat >= nodes_.size()) return false;
+    const NodeRecord& c = *nodes_[L->cat];
+    if (c.name != "builtin:2" || c.initialized || c.node.inputs->size != 2 || c.node.outputs->size != 1 ||
+        c.node.inputs->data[0] != x || c.node.inputs->data[1] != y || !params(c) ||
+        params(c)->activation != 0 || (params(c)->axis != 3 && params(c)->axis != -1))
+      return false;
+    L->out = c.node.outputs->data[0];
+    const TfLiteIntArray* od = tensors_[L->out].type == kTfLiteFloat32 ? dims4(L->out) : nullptr;
+    return od && od->data[0] == xd->data[0] && od->data[1] == xd->data[1] && od->data[2] == xd->data[2] &&
+           od->data[3] == C + d.channels_out && i < L->add && L->add < L->quant &&
+           L->quant < L->conv && L->conv < L->cat;
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    Layer first;
+    if (nodes_[i]->initialized || !match(i, &first)) continue;
+    // the block: each map x_j (j >= 1) read only by the next layer's MUL and CONCATENATION
+    std::vector<Layer> block{first};
+    for (;;) {
+      const int xj = block.back().out;
+      if (is_output(xj)) break;
+      const std::vector<size_t> readers = consumers(xj);
+      Layer next;
+      if (readers.size() != 2 || !match(readers[0], &next) || next.x != xj || next.cat != readers[1])
+        break;
+      block.push_back(next);
+    }
+    const int X = block.back().out;
+    const int c_total = tensors_[X].dims->data[3];
+    std::vector<size_t> absorbed;
+    for (size_t j = 0; j < block.size(); ++j) {
+      const Layer& L = block[j];
+      const TfLiteIntArray* pd = tensors_[L.packed].dims;
+      const std::string tmp_name = names_[L.packed];   // AddTensor appends to names_
+      const int tmp = AddTensor(kTfLiteInt32, std::vector<int>(pd->data, pd->data + 4), nullptr, 0, false,
+                                0.f, 0, tmp_name);
+      NodeRecord& conv = *nodes_[L.conv];
+      NodeRecord& n = *nodes_[L.mul];
+      std::vector<int> ins{j == 0 ? L.x : X, L.scale, L.shift};
+      ins.insert(ins.end(), conv.node.inputs->data + 1, conv.node.inputs->data + 5);
+      LceB200IntArrayFree(n.node.inputs);
+      LceB200IntArrayFree(n.node.outputs);
+      LceB200IntArrayFree(n.node.temporaries);
+      n.node.inputs = MakeDims(ins);
+      n.node.outputs = MakeDims({X});
+      n.node.temporaries = MakeDims({tmp});
+      n.custom_options = conv.custom_options;
+      n.node.custom_initial_data = n.custom_options.data();
+      n.node.custom_initial_data_size = static_cast<int>(n.custom_options.size());
+      n.builtin_blob.assign(reinterpret_cast<const uint8_t*>(&c_total),
+                            reinterpret_cast<const uint8_t*>(&c_total) + 4);
+      n.node.builtin_data = n.builtin_blob.data();
+      n.registration = L.reg;
+      n.name = "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION";
+      absorbed.insert(absorbed.end(), {L.add, L.quant, L.conv, L.cat});
+    }
+    // drop the absorbed nodes (all after node i), the highest index first
+    std::sort(absorbed.begin(), absorbed.end());
+    for (auto it = absorbed.rbegin(); it != absorbed.rend(); ++it) {
+      NodeRecord& n = *nodes_[*it];
+      LceB200IntArrayFree(n.node.inputs);
+      LceB200IntArrayFree(n.node.outputs);
+      LceB200IntArrayFree(n.node.temporaries);
+      LceB200IntArrayFree(n.node.intermediates);
+      nodes_.erase(nodes_.begin() + *it);
+      ++removed;
+    }
+  }
+  allocated_ = false;
+  return removed;
+}
+
 const TfLiteRegistration* FusedPoolDepthwiseRegistration();  // builtin_ops.cc
 const TfLiteRegistration* FusedStemRegistration();
 const TfLiteRegistration* ActivationChainRegistration();

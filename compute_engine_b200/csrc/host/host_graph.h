@@ -97,6 +97,24 @@ class Graph {
   // number of nodes removed.
   int FuseChannelGates();
 
+  // BinaryDenseNet's dense layers
+  //   x_j [B,H,W,C_j] -> MUL(scale) -> ADD(shift) -> LceQuantize -> LceBconv2d (float y_j)
+  //   x_{j+1} = CONCATENATION([x_j, y_j], last axis)
+  // become one node each, "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION": inputs [src, scale,
+  // shift, filter, mul, bias, thr], outputs [X], one temporary for the packed signs. A chain of such
+  // layers shares one tensor X, the block's final map [B,H,W,C_L]; each layer reads X's first C_j
+  // channels and writes its new ones into X[..., C_j : C_j + C_out] (lce_b200_f32_affine_sign,
+  // lce_b200_bconv2d_run_slice), so no x_j and no concatenation copy exists. src is x_0 for the
+  // block's first layer, which also copies x_0 into X, and X for the others. Only when scale and
+  // shift are float constants [C] or [1, ..., 1, C], the MUL and ADD have no fused activation, the
+  // LceBconv2d is a plain node with float output that run_slice takes (same image size), the
+  // CONCATENATION is exactly [x_j, y_j] on the last axis with no activation, C_j and C_L are
+  // multiples of 4, every intermediate has one consumer and is not a graph output, and each x_j
+  // with j >= 1 is read only by its layer's MUL and CONCATENATION. Run before FuseChannelGates and
+  // FuseActivationChains, which would otherwise take the ADD -> LceQuantize as a lone RSign.
+  // Bit-identical. Returns the number of nodes removed.
+  int FuseDenseBlocks();
+
   // Two consecutive residual blocks x1 = x0 + f1(sign x0), x2 = x1 + f2(sign x1) -- a
   // "LceBconv2d+ADD+LceQuantize" node whose two outputs only the next "LceBconv2d+ADD[+LceQuantize]"
   // node reads, as its packed input and its shortcut -- become one node

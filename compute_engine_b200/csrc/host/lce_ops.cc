@@ -768,6 +768,106 @@ TfLiteStatus GateEval(TfLiteContext* context, TfLiteNode* node) {
   return kTfLiteOk;
 }
 
+// ------------------------------------------------------------------------- //
+// A BinaryDenseNet dense layer in one node (Graph::FuseDenseBlocks):
+// [src, scale, shift, filter, mul, bias, thr] -> [X], temporaries [the packed signs]. X is the
+// block's final map [B, H, W, C_L] (builtin_data: int32 C_L); options are the layer's LceBconv2d
+// options, so C_j = channels_in. The node packs the signs of src[..., :C_j] * scale + shift and
+// writes the convolution's channels_out new channels to X[..., C_j : C_j + channels_out]. src is
+// x_0 for a block's first layer, which also copies x_0 into X[..., :C_j] and sets X's shape, and X
+// for the others.
+// ------------------------------------------------------------------------- //
+// The node seen as a plain LceBconv2d node [packed signs, filter, mul, bias, thr] -> [X].
+struct DenseLayerView {
+  TfLiteNode node{};
+  explicit DenseLayerView(const TfLiteNode* dense) {
+    node.inputs = LceB200IntArrayCreate(5);
+    node.inputs->data[0] = dense->temporaries->data[0];
+    for (int i = 1; i < 5; ++i) node.inputs->data[i] = dense->inputs->data[2 + i];
+    node.outputs = LceB200IntArrayCreate(1);
+    node.outputs->data[0] = dense->outputs->data[0];
+    node.user_data = dense->user_data;
+  }
+  ~DenseLayerView() {
+    LceB200IntArrayFree(node.inputs);
+    LceB200IntArrayFree(node.outputs);
+  }
+};
+
+TfLiteStatus ResizeTo(TfLiteContext* context, TfLiteTensor* t, int b, int h, int w, int c) {
+  TfLiteIntArray* dims = LceB200IntArrayCreate(4);
+  dims->data[0] = b;
+  dims->data[1] = h;
+  dims->data[2] = w;
+  dims->data[3] = c;
+  return context->ResizeTensor(context, t, dims);
+}
+
+template <KernelType kt>
+TfLiteStatus DensePrepare(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<BconvOpData*>(node->user_data);
+  if (!op->successfully_initialized) return kTfLiteError;
+  LCE_ENSURE(context, node->inputs->size == 7 && node->outputs->size == 1 &&
+                          node->temporaries->size == 1 && node->builtin_data != nullptr);
+  const int c_total = *static_cast<const int32_t*>(node->builtin_data);
+  const int c_in = op->desc.channels_in;
+  const TfLiteTensor* src = GetInput(context, node, 0);
+  TfLiteTensor* x = GetOutput(context, node, 0);
+  TfLiteTensor* packed = context->GetTensor ? context->GetTensor(context, node->temporaries->data[0])
+                                            : &context->tensors[node->temporaries->data[0]];
+  LCE_ENSURE(context, src != nullptr && src->type == kTfLiteFloat32 && NumDims(src) == 4);
+  LCE_ENSURE(context, x->type == kTfLiteFloat32 && packed->type == kTfLiteInt32);
+  const int b = Dim(src, 0), h = Dim(src, 1), w = Dim(src, 2);
+  if (node->inputs->data[0] != node->outputs->data[0]) {
+    // the block's first layer: X takes x_0's pixels
+    LCE_ENSURE(context, Dim(src, 3) == c_in);
+  } else {
+    LCE_ENSURE_MSG(context, Dim(x, 3) == c_total, "dense layer: the block's map has another channel count");
+  }
+  for (int k = 1; k < 3; ++k) {
+    const TfLiteTensor* v = GetInput(context, node, k);
+    LCE_ENSURE(context, v == nullptr || (v->type == kTfLiteFloat32 && NumElements(v) == c_in));
+  }
+  if (ResizeTo(context, packed, b, h, w, BitpackedSize(c_in)) != kTfLiteOk) return kTfLiteError;
+  DenseLayerView v(node);
+  if (BconvPrepare<kt>(context, &v.node) != kTfLiteOk) return kTfLiteError;
+  // BconvPrepare gave X the convolution's output shape: the layer keeps the image size and its new
+  // channels fit X; then X takes the block's shape again
+  LCE_ENSURE(context, op->desc.out_type == LCE_OUT_FLOAT && Dim(x, 1) == h && Dim(x, 2) == w &&
+                          c_in + op->desc.channels_out <= c_total);
+  return ResizeTo(context, x, b, h, w, c_total);
+}
+
+TfLiteStatus DenseEval(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<BconvOpData*>(node->user_data);
+  DenseLayerView v(node);
+  if (BconvEnsurePlan(context, &v.node) != kTfLiteOk) return kTfLiteError;
+  const TfLiteTensor* src = GetInput(context, node, 0);
+  const TfLiteTensor* scale = GetInput(context, node, 1);
+  const TfLiteTensor* shift = GetInput(context, node, 2);
+  TfLiteTensor* x = GetOutput(context, node, 0);
+  TfLiteTensor* packed = context->GetTensor ? context->GetTensor(context, node->temporaries->data[0])
+                                            : &context->tensors[node->temporaries->data[0]];
+  LCE_ENSURE_MSG(context, OnDevice(src->data.raw) && OnDevice(x->data.raw) && OnDevice(packed->data.raw),
+                 "dense LceBconv2d needs a device arena");
+  const int c_in = op->desc.channels_in, c_total = Dim(x, 3);
+  const bool first = node->inputs->data[0] != node->outputs->data[0];
+  const int64_t rows = static_cast<int64_t>(Dim(x, 0)) * Dim(x, 1) * Dim(x, 2);
+  LCE_ENSURE_CAPI(context, lce_b200_f32_affine_sign(src->data.f, Dim(src, 3), rows, c_in,
+                                                    scale ? scale->data.f : nullptr,
+                                                    shift ? shift->data.f : nullptr, packed->data.i32,
+                                                    first ? x->data.f : nullptr, c_total, g_stream));
+  LCE_ENSURE_CAPI(context, lce_b200_bconv2d_run_slice(op->plan, packed->data.i32, x->data.f + c_in,
+                                                      c_total, g_stream));
+  return kTfLiteOk;
+}
+
+template <KernelType kt>
+TfLiteRegistration* BconvDenseRegistration() {
+  static TfLiteRegistration r = {BconvInit, BconvFree, DensePrepare<kt>, DenseEval};
+  return &r;
+}
+
 template <KernelType kt>
 TfLiteRegistration* BconvGateRegistration() {
   static TfLiteRegistration r = {BconvInit, BconvFree, GatePrepare<kt>, GateEval};
@@ -843,6 +943,19 @@ TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_GATE(const TfLiteRegistr
     return BconvGateRegistration<KernelType::kOptimizedBGEMM>();
   if (original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
     return BconvGateRegistration<KernelType::kOptimizedIndirectBGEMM>();
+  return nullptr;
+}
+
+// host-internal: the dense-layer node created by Graph::FuseDenseBlocks from a plain LceBconv2d
+// node of this registration (nullptr: not one of this library's LceBconv2d registrations)
+TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_DENSE(const TfLiteRegistration* original) {
+  if (original == BconvRegistration<KernelType::kCuda>()) return BconvDenseRegistration<KernelType::kCuda>();
+  if (original == BconvRegistration<KernelType::kReference>())
+    return BconvDenseRegistration<KernelType::kReference>();
+  if (original == BconvRegistration<KernelType::kOptimizedBGEMM>())
+    return BconvDenseRegistration<KernelType::kOptimizedBGEMM>();
+  if (original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
+    return BconvDenseRegistration<KernelType::kOptimizedIndirectBGEMM>();
   return nullptr;
 }
 

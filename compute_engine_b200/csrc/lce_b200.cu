@@ -188,19 +188,19 @@ size_t imma_smem_budget(int V, bool b1) {
   return (227u * 1024u / ctas - 1024u - 256u) & ~size_t{127};
 }
 
-template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false>
+template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(imma_smem_budget(V, B1))));
-  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE><<<grid, lce::kIThreads, smem, s>>>(p);
+  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE><<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
 // Epilogue tails of the float output beyond run_fused's (bconv_run_impl decides).
-enum class Tail { kNone, kChain, kGate };   // p.chain / p.gate applied in the epilogue
+enum class Tail { kNone, kChain, kGate, kSlice };   // p.chain / p.gate / p.out_stride in the epilogue
 
 template <int V>
 int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, dim3 grid,
@@ -212,6 +212,10 @@ int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, d
   if (tail == Tail::kGate) {
     if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, true>(p, grid, smem, s);
     return launch_imma_vo<V, LCE_OUT_FLOAT, false, false, true>(p, grid, smem, s);
+  }
+  if (tail == Tail::kSlice) {
+    if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, false, true>(p, grid, smem, s);
+    return launch_imma_vo<V, LCE_OUT_FLOAT, false, false, false, true>(p, grid, smem, s);
   }
   if (b1) {
     if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, true>(p, grid, smem, s);
@@ -269,7 +273,7 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, Tail tail = Ta
       default: return launch_imma_v<1>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
     }
   }
-  if (tail != Tail::kNone) return fail("bconv2d: the chain and gate epilogues need the mma.sync kernel");
+  if (tail != Tail::kNone) return fail("bconv2d: the chain, gate and slice epilogues need the mma.sync kernel");
   if (c.tc_ok) {
     // wgmma inner product: persistent 128 x BN tiles
     const int rc = tc_launch(c, p, s);
@@ -736,6 +740,19 @@ void pair_tile(int C, int* th, int* tw) {
   *tw = C == 64 ? lce::PairShape<2>::TW : lce::PairShape<4>::TW;
 }
 
+// What keeps a plan off lce_b200_bconv2d_run_slice, or nullptr: float output and the mma.sync
+// weight fragments, which a plan has when it was created with LCE_B200_BCONV_IMMA not 0 and full
+// 64-channel tiles. c == nullptr: for a plan not created yet.
+const char* slice_refusal(const lce_bconv2d_desc& d, const GemmCore* c) {
+  if (d.out_type != LCE_OUT_FLOAT) return "float output";
+  const bool imma = c != nullptr ? c->wt_nat != nullptr
+                                 : !env_off("LCE_B200_BCONV_IMMA") && d.groups > 0 &&
+                                       (d.channels_out / d.groups) % lce::kBN == 0;
+  if (!imma)
+    return "the mma.sync weight fragments (channels_out a multiple of 64, LCE_B200_BCONV_IMMA not 0)";
+  return nullptr;
+}
+
 template <int CW>
 int launch_pair(const lce::PairParams& p, int grid, cudaStream_t s) {
   constexpr int smem = lce::PairShape<CW>::smem_bytes;
@@ -1062,7 +1079,7 @@ static size_t bconv_out_bytes(const lce_b200_bconv2d* plan) {
 static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* out_dev,
                           const float* residual, int residual_act, int32_t* packed_out,
                           const lce_chain_desc* chain, void* stream,
-                          const lce_gate_desc* gate = nullptr) {
+                          const lce_gate_desc* gate = nullptr, int64_t out_stride = 0) {
   const lce_bconv2d_desc& d = plan->d;
   GemmCore& c = plan->core;
   cudaStream_t s = as_stream(stream);
@@ -1130,12 +1147,16 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     return lce_b200_f32_gate_sign(out, gate, residual, residual_act, d.batch,
                                   static_cast<int64_t>(p.OH) * p.OW, c.cout, out, packed_out, stream);
   }
-  if (!zp_float) return launch_conv(c, p, s);
+  // run_slice: the mma.sync kernel's strided store (the caller checked that it takes the plan)
+  const bool slice = out_stride != 0;
+  const Tail plain = slice ? Tail::kSlice : Tail::kNone;
+  p.out_stride = slice ? out_stride : c.cout;
+  if (!zp_float) return launch_conv(c, p, s, plain);
   // the optimised kernels' zero padding: one-padding accumulators + a float correction. The
   // wgmma kernel does it in its epilogue; the others run unfused and a tail pass finishes.
   p.zp_float = 1;
   p.cin_pg = d.channels_in / d.groups;
-  if (c.tc_ok) {
+  if (c.tc_ok && !slice) {
     const int rc = tc_launch(c, p, s);
     if (rc >= 0) return rc;
   }
@@ -1143,12 +1164,12 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
   q.tap_popc = nullptr; q.residual = nullptr; q.packed_out = nullptr; q.res_stage = 0; q.zp_float = 0;
   const bool tc_was = c.tc_ok;
   c.tc_ok = false;
-  const int rc = launch_conv(c, q, s);
+  const int rc = launch_conv(c, q, s, plain);
   c.tc_ok = tc_was;
   if (rc) return rc;
   lce::ZpcTailParams z;
   z.out = static_cast<float*>(out_dev); z.mul = c.mul; z.tap_popc = c.tap_popc;
-  z.residual = residual; z.packed_out = packed_out; z.M = p.M;
+  z.residual = residual; z.packed_out = packed_out; z.M = p.M; z.out_stride = p.out_stride;
   z.H = p.H; z.W = p.W; z.OH = p.OH; z.OW = p.OW; z.KH = p.KH; z.KW = p.KW;
   z.sh = p.sh; z.sw = p.sw; z.dh = p.dh; z.dw = p.dw;
   z.cout = c.cout; z.cin_pg = p.cin_pg; z.cw_out = p.cw_out; z.residual_act = residual_act;
@@ -1222,6 +1243,33 @@ int lce_b200_bconv2d_run_fused_gate(lce_b200_bconv2d* plan, const int32_t* in_de
     return fail("bconv2d_run_fused_gate: output must not overlap the gate");
   return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev,
                         nullptr, stream, gate);
+}
+
+int lce_b200_bconv2d_run_slice(lce_b200_bconv2d* plan, const int32_t* in_dev, float* out_dev,
+                               int64_t out_pixel_stride, void* stream) {
+  const lce_bconv2d_desc& d = plan->d;
+  if (const char* why = slice_refusal(d, &plan->core))
+    return fail("bconv2d_run_slice: the plan needs %s", why);
+  if (out_pixel_stride < d.channels_out || out_pixel_stride % 4 != 0)
+    return fail("bconv2d_run_slice: the output pixel stride %lld must be a multiple of 4 and at "
+                "least channels_out %d", static_cast<long long>(out_pixel_stride), d.channels_out);
+  if (!aligned16(out_dev)) return fail("bconv2d_run_slice: output must be 16-byte aligned");
+  const long long px = static_cast<long long>(d.batch) * plan->out_h * plan->out_w;
+  if (px == 0) return 0;
+  // the output's span, first float of pixel 0 to the last of pixel px - 1, against the packed input
+  const uintptr_t o0 = reinterpret_cast<uintptr_t>(out_dev);
+  const uintptr_t o1 = o0 + (static_cast<uintptr_t>(px - 1) * out_pixel_stride + d.channels_out) * 4;
+  const uintptr_t i0 = reinterpret_cast<uintptr_t>(in_dev);
+  const uintptr_t i1 = i0 + static_cast<uintptr_t>(d.batch) * d.in_h * d.in_w * cdiv(d.channels_in, 32) * 4;
+  if (o0 < i1 && i0 < o1) return fail("bconv2d_run_slice: output must not overlap the input");
+  return bconv_run_impl(plan, in_dev, out_dev, nullptr, LCE_ACT_NONE, nullptr, nullptr, stream,
+                        nullptr, out_pixel_stride);
+}
+
+// Whether lce_b200_bconv2d_run_slice will take a plan created now from *d
+// (Graph::FuseDenseBlocks asks before it rewrites the graph).
+int lce_b200_internal_slice_takes(const lce_bconv2d_desc* d) {
+  return slice_refusal(*d, nullptr) == nullptr;
 }
 
 int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* plan2,

@@ -1057,6 +1057,34 @@ __global__ void __launch_bounds__(256) gate_sign_kernel(const float* x, const lc
   }
 }
 
+// lce_b200_f32_affine_sign: the signs of x * scale + shift over a strided [rows][channels] map,
+// threads laid out as in chain_sign_kernel with the packed output; copy (optional) receives x.
+template <typename I>
+__global__ void __launch_bounds__(256) affine_sign_kernel(const float* __restrict__ x, I x_stride,
+                                                          I rows, int channels, int cw,
+                                                          const float* __restrict__ scale,
+                                                          const float* __restrict__ shift,
+                                                          int32_t* __restrict__ packed,
+                                                          float* __restrict__ copy, I copy_stride) {
+  const bool has_sc = scale != nullptr, has_sh = shift != nullptr;
+  const I span = static_cast<I>(cw) * 32;
+  const I n = rows * span;
+  const I stride = static_cast<I>(gridDim.x) * blockDim.x;   // a multiple of 32: warps stay whole
+  for (I i = static_cast<I>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const I row = i / span;
+    const int c = static_cast<int>(i - row * span);
+    bool bit = false;
+    if (c < channels) {
+      const float v = x[row * x_stride + c];
+      if (copy) copy[row * copy_stride + c] = v;
+      bit = lce::affine_sign(v, has_sc, has_sc ? __ldg(scale + c) : 0.0f, has_sh,
+                             has_sh ? __ldg(shift + c) : 0.0f);
+    }
+    const unsigned word = __ballot_sync(0xffffffffu, bit);
+    if ((threadIdx.x & 31) == 0) packed[i >> 5] = static_cast<int32_t>(word);
+  }
+}
+
 // LOGISTIC, TFLite's float reference (reference/logistic.h) with CUDA's expf
 __global__ void __launch_bounds__(256) logistic_kernel(const float* __restrict__ in,
                                                        float* __restrict__ out, long long n) {
@@ -1913,6 +1941,32 @@ int lce_b200_f32_gate_sign(const float* x, const lce_gate_desc* gate, const floa
                                                               cw, out, packed);
   }
   return launch_check("gate_sign_kernel");
+}
+
+int lce_b200_f32_affine_sign(const float* x, int64_t x_pixel_stride, int64_t rows, int channels,
+                             const float* scale, const float* shift, int32_t* packed, float* copy,
+                             int64_t copy_pixel_stride, void* stream) {
+  if (rows < 0 || channels <= 0 || x_pixel_stride < channels ||
+      (copy != nullptr && copy_pixel_stride < channels))
+    return fail("affine_sign: bad shape (%lld rows, %d channels, pixel strides %lld and %lld)",
+                static_cast<long long>(rows), channels, static_cast<long long>(x_pixel_stride),
+                static_cast<long long>(copy_pixel_stride));
+  if (packed == nullptr) return fail("affine_sign: the packed output is required");
+  if (rows == 0) return 0;
+  const int cw = (channels + 31) / 32;
+  const long long n = rows * cw * 32;
+  const int grid = grid_for(n, 256);
+  cudaStream_t s = as_stream(stream);
+  // 32-bit index arithmetic where it fits (the row / channel split is a division per element)
+  const long long widest = std::max<long long>(x_pixel_stride, copy ? copy_pixel_stride : 0);
+  if (n + 256LL * grid < (1LL << 31) && rows * widest < (1LL << 31))
+    affine_sign_kernel<int><<<grid, 256, 0, s>>>(x, static_cast<int>(x_pixel_stride), static_cast<int>(rows),
+                                                 channels, cw, scale, shift, packed, copy,
+                                                 static_cast<int>(copy_pixel_stride));
+  else
+    affine_sign_kernel<long long><<<grid, 256, 0, s>>>(x, x_pixel_stride, rows, channels, cw, scale, shift,
+                                                       packed, copy, copy_pixel_stride);
+  return launch_check("affine_sign_kernel");
 }
 
 int lce_b200_f32_logistic(const float* in, float* out, int64_t n, void* stream) {

@@ -307,11 +307,14 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // registers would exceed the b1 instances' 128-register cap. GATE (float output): Real-to-Binary's
 // gated tail (p.gate) before the shortcut ADD, from chain_s = [- | alpha | sign_scale | sign_shift
 // | mul | bias]; the gate row is each row's own image's (a tile can span several images).
-template <int OUT, int S, bool CHAIN = false, bool GATE = false>
+// SLICE (float output, no shortcut or signs): row m goes to out + m * p.out_stride, a channel
+// slice of a wider map.
+template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
                                               int tig, const float* chain_s = nullptr) {
   static_assert(!(CHAIN && GATE), "one epilogue tail at a time");
+  static_assert(!SLICE || (OUT == LCE_OUT_FLOAT && !CHAIN && !GATE), "a plain float slice");
   constexpr bool STAGED = CHAIN || GATE;
   const int cth = c_tile + tig * 2;
   float2 mul_r[8], bias_r[8];
@@ -322,8 +325,8 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
       bias_r[ns] = *reinterpret_cast<const float2*>(p.bias + cth + ns * 8);
     }
   }
-  const bool has_res = OUT == LCE_OUT_FLOAT && p.residual != nullptr;
-  const bool has_pk = OUT == LCE_OUT_FLOAT && p.packed_out != nullptr;
+  const bool has_res = OUT == LCE_OUT_FLOAT && !SLICE && p.residual != nullptr;
+  const bool has_pk = OUT == LCE_OUT_FLOAT && !SLICE && p.packed_out != nullptr;
   // fused activation of the ADD as one clamp: y = min(max(y, lo), hi) (kernel_util.h:285-300)
   const int ract = p.residual_act;
   const float act_lo = ract == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
@@ -336,7 +339,8 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
       const int lrow = warp * 32 + ms * 16 + h * 8 + gid;
       const long long m = m0 + lrow;
       const bool row_ok = m < p.M;
-      const size_t e0 = static_cast<size_t>(m) * p.cout + cth;
+      const size_t e0 = SLICE ? static_cast<size_t>(m) * p.out_stride + cth
+                              : static_cast<size_t>(m) * p.cout + cth;
       if (OUT == LCE_OUT_RAW_ACC) {
         if (row_ok) {
           int* o = static_cast<int*>(p.out) + e0;
@@ -484,8 +488,9 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 // B1 selects the inner product: packed b1 fragments (accumulators at scale 1) or int8 ones
 // (scale 8). Both produce the same int32 accumulators. CHAIN (float output): the epilogue also
 // applies p.chain (lce_b200_bconv2d_run_fused_chain); GATE (float output): p.gate
-// (lce_b200_bconv2d_run_fused_gate). The other instances compile as without them.
-template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false>
+// (lce_b200_bconv2d_run_fused_gate); SLICE (float output): the strided store of
+// lce_b200_bconv2d_run_slice. The other instances compile as without them.
+template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false>
 __global__ void __launch_bounds__(kIThreads, B1 ? kB1Ctas : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
   using Vec = typename VecT<V>::T;
@@ -528,7 +533,7 @@ bconv_imma_kernel(const ConvKParams p) {
       acc[ms][ns][2] = pw.x * 8; acc[ms][ns][3] = pw.y * 8;
     }
   }
-  if (OUT == LCE_OUT_FLOAT && p.residual != nullptr) {
+  if (OUT == LCE_OUT_FLOAT && !SLICE && p.residual != nullptr) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const long long m = m0 + warp * 32 + i * 8 + gid;
@@ -626,7 +631,7 @@ bconv_imma_kernel(const ConvKParams p) {
     __syncthreads();
     epilogue_imma<OUT, S, false, true>(p, acc, m0, c_tile, warp, gid, tig, cs);
   } else {
-    epilogue_imma<OUT, S>(p, acc, m0, c_tile, warp, gid, tig);
+    epilogue_imma<OUT, S, false, false, SLICE>(p, acc, m0, c_tile, warp, gid, tig);
   }
 }
 

@@ -98,6 +98,9 @@ struct ConvKParams {
   // GATE instances only: Real-to-Binary's gated tail before the shortcut ADD; packed_out then
   // holds the signs of o * sign_scale + sign_shift
   lce_gate_desc gate;
+  // SLICE instances only: output pixel m's cout floats start at out + m * out_stride
+  // (lce_b200_bconv2d_run_slice)
+  long long out_stride;
 };
 
 // --------------------------- PTX helpers ---------------------------------- //
@@ -796,6 +799,7 @@ struct ZpcTailParams {
   const float* residual;
   int32_t* packed_out;
   long long M;
+  long long out_stride;      // floats from one output pixel to the next (cout unless strided)
   int H, W, OH, OW, KH, KW, sh, sw, dh, dw;
   int cout, cin_pg, cw_out, residual_act;
 };
@@ -826,7 +830,7 @@ __global__ void __launch_bounds__(256) zpc_tail_kernel(const ZpcTailParams p) {
     float y = 0.0f;
     const bool ok = c < p.cout;
     if (ok) {
-      y = p.out[m * p.cout + c];
+      y = p.out[m * p.out_stride + c];
       if (cs >= 0) {
         int corr = 0;
         for (int fy = 0; fy < p.KH; ++fy)
@@ -847,7 +851,7 @@ __global__ void __launch_bounds__(256) zpc_tail_kernel(const ZpcTailParams p) {
         else if (p.residual_act == LCE_ACT_RELU6) y = fminf(fmaxf(y, 0.0f), 6.0f);
         else if (p.residual_act == LCE_ACT_RELU_N1_TO_1) y = fminf(fmaxf(y, -1.0f), 1.0f);
       }
-      p.out[m * p.cout + c] = y;
+      p.out[m * p.out_stride + c] = y;
     }
     if (p.packed_out != nullptr) {
       const uint32_t word = __ballot_sync(0xffffffffu, ok && y < 0.0f);

@@ -186,6 +186,12 @@ class HostGraph:
         """MAX_POOL_2D(2x2 s1 VALID) -> DEPTHWISE_CONV_2D(3x3) => one node."""
         return lib().lce_host_fuse_float_glue(self._g)
 
+    def fuse_dense_blocks(self):
+        """BinaryDenseNet's MUL -> ADD -> LceQuantize -> LceBconv2d -> CONCATENATION layers => one
+        node each, writing into the block's final map in place. Call before fuse_channel_gates,
+        fuse_activation_chains and allocate_tensors."""
+        return lib().lce_host_fuse_dense_blocks(self._g)
+
     def fuse_channel_gates(self):
         """LceBconv2d -> MUL(gate [B,1,1,C]) -> PRELU -> ADD(shortcut) [-> MUL -> ADD -> LceQuantize]
         (Real-to-Binary Net's gated block and the next block's BatchNorm and sign) => one node.
@@ -204,8 +210,8 @@ class HostGraph:
         return lib().lce_host_fuse_residual_pairs(self._g)
 
     def fuse_all(self):
-        return (self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_channel_gates()
-                + self.fuse_activation_chains() + self.fuse_residual_pairs())
+        return (self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_dense_blocks()
+                + self.fuse_channel_gates() + self.fuse_activation_chains() + self.fuse_residual_pairs())
 
     # ---- profiling / async IO (bench.py) ----
     def enable_profiling(self, on=True):

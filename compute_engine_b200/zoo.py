@@ -76,7 +76,8 @@ class _Builder:
         return scale, shift
 
     # ---- float builtins ----
-    def conv(self, x, xs, cout, k, stride, padding="SAME", activation="NONE", bn=True):
+    def conv(self, x, xs, cout, k, stride, padding="SAME", activation="NONE", bn=True,
+             use_bias=True):
         b, h, w, cin = xs
         wt = self.rng.standard_normal((cout, k, k, cin)).astype(np.float32) * np.float32(
             1.0 / np.sqrt(k * k * cin))
@@ -88,8 +89,8 @@ class _Builder:
         oh = -(-h // stride) if padding == "SAME" else (h - k) // stride + 1
         ow = -(-w // stride) if padding == "SAME" else (w - k) // stride + 1
         y = self.act((b, oh, ow, cout))
-        self.m.add_op("CONV_2D", [x, self.const(wt), self.const(bias, name="b")], [y],
-                      padding=padding, stride=(stride, stride), activation=activation)
+        self.m.add_op("CONV_2D", [x, self.const(wt), self.const(bias, name="b") if use_bias else -1],
+                      [y], padding=padding, stride=(stride, stride), activation=activation)
         return y, (b, oh, ow, cout)
 
     def depthwise(self, x, xs, k, stride, padding="SAME", blur=False, bn=False):
@@ -137,7 +138,7 @@ class _Builder:
         self.m.add_op("LceQuantize", [x], [y], custom_options=b"")
         return y
 
-    def bconv(self, xq, xs, cout, k=3, stride=1, pad_values=1, activation="RELU"):
+    def bconv(self, xq, xs, cout, k=3, stride=1, pad_values=1, activation="RELU", dilation=1):
         """LceBconv2d with float output; BN (and for Bi-RealNet the kernel scale)
         folded into post_activation_multiplier / bias like the converter does
         (LCE/mlir/transforms/optimize_patterns_common.td:39-113)."""
@@ -152,7 +153,7 @@ class _Builder:
         oh, ow = -(-h // stride), -(-w // stride)
         y = self.act((b, oh, ow, cout))
         act_code = {"NONE": 0, "RELU": 1}[activation]
-        opts = bconv2d_options(cin, (stride, stride), (1, 1), 0, pad_values, act_code)
+        opts = bconv2d_options(cin, (stride, stride), (dilation, dilation), 0, pad_values, act_code)
         self.m.add_op("LceBconv2d",
                       [xq, self.const(filt, np.int32, "bfilter"), self.const(mul, name="pmul"),
                        self.const(t, name="pbias"), -1], [y], custom_options=opts)
@@ -349,5 +350,73 @@ def realtobinarynet(batch=1, seed=0, image=224, input_type="float32", pad_values
     return g.m.serialize()
 
 
+def binarydensenet(batch=1, seed=0, image=224, input_type="float32", pad_values=0,
+                   layers=(6, 6, 6, 5), reduction=(2.7, 2.7, 2.2), dilation=(1, 1, 1, 1),
+                   name="BinaryDenseNet28"):
+    """BinaryDenseNet, restated from the paper (Bethge et al., 2019) with the block parameters of
+    its 28 / 37 / 37-Dilated / 45 variants. In the converter's op order:
+      stem CONV_2D 7x7/s2 3 -> 64 (BN folded, RELU) -> MAX_POOL_2D 3x3/s2 SAME;
+      dense layer x_j [B,H,W,C_j] -> MUL(bn_scale) -> ADD(bn_shift) -> LceQuantize -> LceBconv2d
+      3x3 (C_j -> 64, stride 1, SAME, `pad_values`, the block's dilation, no activation) = y_j,
+      x_{j+1} = CONCATENATION([x_j, y_j], axis 3);
+      transition MUL -> ADD (BN) -> MAX_POOL_2D 2x2/s2 VALID (not before a dilated block) -> RELU
+      -> CONV_2D 1x1 to round(C // reduction / 32) * 32 channels, no bias;
+      head MUL -> ADD (BN) -> RELU -> MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX."""
+    g = _Builder(seed, batch, name)
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+
+    def batchnorm(t, ts):
+        scale, shift = g.bn(ts[3])
+        u = g.act(ts)
+        g.m.add_op("MUL", [t, g.const(scale, name="bn_scale")], [u])
+        return g.add(u, g.const(shift, name="bn_shift"), ts)
+
+    x, xs = g.conv(x, xs, 64, 7, 2, activation="RELU")
+    x, xs = g.pool("MAX_POOL_2D", x, xs, 3, 2, "SAME")
+    for blk, n in enumerate(layers):
+        if blk > 0:
+            cout = int(round(xs[3] // reduction[blk - 1] / 32)) * 32
+            x = batchnorm(x, xs)
+            if dilation[blk] == 1:
+                x, xs = g.pool("MAX_POOL_2D", x, xs, 2, 2, "VALID")
+            x = g.relu(x, xs)
+            x, xs = g.conv(x, xs, cout, 1, 1, bn=False, use_bias=False)
+        for _ in range(n):
+            t = batchnorm(x, xs)
+            y, _ = g.bconv(g.quantize(t, xs), xs, 64, pad_values=pad_values, activation="NONE",
+                           dilation=dilation[blk])
+            xs = xs[:3] + (xs[3] + 64,)
+            z = g.act(xs)
+            g.m.add_op("CONCATENATION", [x, y], [z], axis=3)
+            x = z
+    probs = g.head(batchnorm(x, xs), xs)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
+def binarydensenet28(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    return binarydensenet(batch, seed, image, input_type, pad_values)
+
+
+def binarydensenet37(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    return binarydensenet(batch, seed, image, input_type, pad_values, layers=(6, 8, 12, 6),
+                          reduction=(3.3, 3.3, 4), name="BinaryDenseNet37")
+
+
+def binarydensenet37_dilated(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    return binarydensenet(batch, seed, image, input_type, pad_values, layers=(6, 8, 12, 6),
+                          reduction=(3.3, 3.3, 4), dilation=(1, 1, 2, 4),
+                          name="BinaryDenseNet37Dilated")
+
+
+def binarydensenet45(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    return binarydensenet(batch, seed, image, input_type, pad_values, layers=(6, 12, 14, 8),
+                          reduction=(2.7, 3.3, 4), name="BinaryDenseNet45")
+
+
 MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "birealnet18": birealnet18,
-          "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet}
+          "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet,
+          "binarydensenet28": binarydensenet28, "binarydensenet37": binarydensenet37,
+          "binarydensenet37_dilated": binarydensenet37_dilated,
+          "binarydensenet45": binarydensenet45}

@@ -169,6 +169,26 @@ int lce_b200_f32_gate_sign(const float* x_dev, const lce_gate_desc* gate_desc,
  * below -9, else 1 / (1 + exp(-x)). CUDA's expf is not libm's: within 4 ulp of the formula, not
  * bit-identical to a CPU run. */
 int lce_b200_f32_logistic(const float* in_dev, float* out_dev, int64_t n, void* stream);
+/* BinaryDenseNet's dense layer writes its new channels into the block's map in place:
+ * run, but output pixel m's channels_out floats go to out_dev + m * out_pixel_stride, and nothing
+ * else is written. Float-output plans on the mma.sync kernel only (created with
+ * LCE_B200_BCONV_IMMA not 0 and channels_out a multiple of 64); REFERENCE zero padding stays in
+ * the kernel, CORRECTION plans finish with the float correction pass on the same strided rows.
+ * Refuses, with a message, other plans, a stride below channels_out or not a multiple of 4, an
+ * out_dev that is not 16-byte aligned, and an output span that overlaps the input. Bit-identical
+ * to run followed by a copy of each pixel's row. */
+int lce_b200_bconv2d_run_slice(lce_b200_bconv2d* plan, const int32_t* in_dev, float* out_dev,
+                               int64_t out_pixel_stride, void* stream);
+/* The signs of a dense layer's BatchNorm in one pass over a strided float [rows, channels] map
+ * (row r starts at x_dev + r * x_pixel_stride):
+ *   packed_out[r][ceil(channels/32)] = bitpack(x * scale[c] + shift[c]),
+ * rounded after the multiply and again after the add, as TFLite's MUL then ADD. scale or shift
+ * may be NULL (that op is absent). copy_out (may be NULL) receives x bit for bit, row r at
+ * copy_out + r * copy_pixel_stride. */
+int lce_b200_f32_affine_sign(const float* x_dev, int64_t x_pixel_stride, int64_t rows,
+                             int channels, const float* scale, const float* shift,
+                             int32_t* packed_out_dev, float* copy_out_dev,
+                             int64_t copy_pixel_stride, void* stream);
 int lce_b200_bconv2d_run_host(lce_b200_bconv2d* plan, const int32_t* in_host,
                               void* out_host);
 void lce_b200_bconv2d_destroy(lce_b200_bconv2d* plan);
