@@ -80,7 +80,7 @@ EXPORTS = [
     "lce_b200_bconv2d_set_zero_padding_mode", "lce_b200_path_counts", "lce_b200_tc_debug",
     "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_fused_chain",
     "lce_b200_bconv2d_run_fused_pair",
-    "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_slice",
+    "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add",
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_logistic",
     "lce_b200_f32_affine_sign",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
@@ -361,6 +361,23 @@ class BConv2d:
         ptr = C.c_void_p(out.data_ptr() + 4 * offset)
         _check(lib().lce_b200_bconv2d_run_slice(self._h, _p(x), ptr, C.c_int64(out.shape[-1]),
                                                 _stream()))
+        return out
+
+    def run_slice_add(self, x: torch.Tensor, out: torch.Tensor, offset: int = 0, scratch=None):
+        """lce_b200_bconv2d_run_slice_add on bitpacked x: adds the float output to channels
+        [offset, offset + channels_out) of `out`, a contiguous float32 [B, OH, OW, C] map (or any
+        tensor whose last axis is the pixel stride), in place, and writes nothing else. scratch: a
+        contiguous CUDA float32 tensor of pixels * channels_out elements, required by CORRECTION
+        plans (zero padding with the float correction). Returns out."""
+        x = _dev(x, torch.int32)
+        if tuple(x.shape[:3]) != (self.desc.batch, self.desc.in_h, self.desc.in_w):
+            self.set_input_shape(*x.shape[:3])
+        for name, t in (("out", out), ("scratch", scratch)):
+            if t is not None and (not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()):
+                raise LceError(f"run_slice_add: {name} must be a contiguous CUDA float32 tensor")
+        ptr = C.c_void_p(out.data_ptr() + 4 * offset)
+        _check(lib().lce_b200_bconv2d_run_slice_add(self._h, _p(x), ptr, C.c_int64(out.shape[-1]),
+                                                    _p(scratch), _stream()))
         return out
 
     def run_fused_pair(self, second, x: torch.Tensor, residual: torch.Tensor, act1=0, act2=0,

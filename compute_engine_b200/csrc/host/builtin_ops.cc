@@ -5,6 +5,7 @@
 // fully_connected,softmax,reduce,reshape,activations,logistic}.cc). Device arena only.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstring>
 
 #include "builtin_params.h"
@@ -656,7 +657,137 @@ TfLiteStatus ConcatInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// ----------------------------- STRIDED_SLICE / SPLIT ----------------------------- //
+// One strided device copy per output, as CONCATENATION: no kernel of ours. Every index vector is a
+// host constant. The copy of outer rows of `width` bytes, each `pitch` bytes apart in x.
+TfLiteStatus CopyRows(TfLiteContext* c, void* dst, const void* src, size_t width, size_t pitch,
+                      size_t rows, const char* what) {
+  if (width && rows &&
+      cudaMemcpy2DAsync(dst, width, src, pitch, width, rows, cudaMemcpyDeviceToDevice,
+                        static_cast<cudaStream_t>(lce_b200_get_stream())) != cudaSuccess) {
+    c->ReportError(c, "%s: device copy failed", what);
+    return kTfLiteError;
+  }
+  return kTfLiteOk;
+}
+// A constant int32 tensor in host memory (the model's own buffer), or nullptr.
+const int32_t* HostInts(const TfLiteTensor* t) {
+  return t && t->type == kTfLiteInt32 && t->data.raw && !OnDevice(t->data.raw) ? t->data.i32 : nullptr;
+}
+// inputs [x (float32 / int32), begin, end, strides]
+const char* SliceGeometry(TfLiteContext* c, TfLiteNode* n, SliceBounds* sb) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  if (n->inputs->size != 4 || !x || (x->type != kTfLiteFloat32 && x->type != kTfLiteInt32))
+    return "STRIDED_SLICE: a float32 or int32 input, then begin, end and strides, expected";
+  const TfLiteTensor* v[3] = {T(c, n->inputs, 1), T(c, n->inputs, 2), T(c, n->inputs, 3)};
+  for (const TfLiteTensor* t : v)
+    if (!HostInts(t) || t->dims->size != 1 || t->dims->data[0] != v[0]->dims->data[0])
+      return "STRIDED_SLICE: begin, end and strides must be constant int32 vectors of one length";
+  return StridedSliceBounds(x->dims->data, x->dims->size, v[0]->data.i32, v[1]->data.i32,
+                            v[2]->data.i32, v[0]->dims->data[0], P(n), sb);
+}
+TfLiteStatus StridedSlicePrepare(TfLiteContext* c, TfLiteNode* n) {
+  SliceBounds sb;
+  const char* why = SliceGeometry(c, n, &sb);
+  B_ENSURE(c, why == nullptr, why);
+  TfLiteIntArray* dims = LceB200IntArrayCreate(sb.rank);
+  for (int k = 0; k < sb.rank; ++k) dims->data[k] = sb.end[k] - sb.begin[k];
+  return c->ResizeTensor(c, T(c, n->outputs, 0), dims);
+}
+TfLiteStatus StridedSliceInvoke(TfLiteContext* c, TfLiteNode* n) {
+  SliceBounds sb;
+  const char* why = SliceGeometry(c, n, &sb);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  int a = 0;   // the sliced axis (axis 0 when the slice is the whole of x)
+  while (a + 1 < sb.rank && sb.begin[a] == 0 && sb.end[a] == x->dims->data[a]) ++a;
+  size_t outer = 1, inner = 4;
+  for (int k = 0; k < a; ++k) outer *= x->dims->data[k];
+  for (int k = a + 1; k < sb.rank; ++k) inner *= x->dims->data[k];
+  return CopyRows(c, T(c, n->outputs, 0)->data.raw, x->data.raw + sb.begin[a] * inner,
+                  (sb.end[a] - sb.begin[a]) * inner, x->dims->data[a] * inner, outer, "STRIDED_SLICE");
+}
+
+// inputs [axis (constant int32 scalar, negative counts from the end), x (float32 / int32)];
+// num_splits outputs of equal size along the axis
+bool SplitGeometry(TfLiteContext* c, TfLiteNode* n, int* axis, size_t* outer, size_t* inner) {
+  const TfLiteTensor* ax = T(c, n->inputs, 0);
+  const TfLiteTensor* x = T(c, n->inputs, 1);
+  if (n->inputs->size != 2 || !HostInts(ax) || Count(ax) != 1 || !x ||
+      (x->type != kTfLiteFloat32 && x->type != kTfLiteInt32) || x->dims->size < 1 || x->dims->size > 4)
+    return false;
+  const int r = x->dims->size;
+  *axis = ax->data.i32[0] < 0 ? ax->data.i32[0] + r : ax->data.i32[0];
+  if (*axis < 0 || *axis >= r) return false;
+  *outer = 1;
+  *inner = 4;
+  for (int k = 0; k < *axis; ++k) *outer *= x->dims->data[k];
+  for (int k = *axis + 1; k < r; ++k) *inner *= x->dims->data[k];
+  return true;
+}
+TfLiteStatus SplitPrepare(TfLiteContext* c, TfLiteNode* n) {
+  int axis;
+  size_t outer, inner;
+  B_ENSURE(c, SplitGeometry(c, n, &axis, &outer, &inner),
+           "SPLIT: a constant int32 axis within the input's rank, and a float32 or int32 input of "
+           "rank 1 to 4, expected");
+  const TfLiteTensor* x = T(c, n->inputs, 1);
+  const int parts = P(n).num_splits;
+  B_ENSURE(c, parts > 0 && n->outputs->size == parts, "SPLIT: num_splits must equal the output count");
+  B_ENSURE(c, x->dims->data[axis] % parts == 0, "SPLIT: num_splits must divide the axis");
+  for (int k = 0; k < parts; ++k) {
+    TfLiteIntArray* dims = LceB200IntArrayCreate(x->dims->size);
+    for (int i = 0; i < x->dims->size; ++i)
+      dims->data[i] = i == axis ? x->dims->data[i] / parts : x->dims->data[i];
+    if (c->ResizeTensor(c, T(c, n->outputs, k), dims) != kTfLiteOk) return kTfLiteError;
+  }
+  return kTfLiteOk;
+}
+TfLiteStatus SplitInvoke(TfLiteContext* c, TfLiteNode* n) {
+  int axis;
+  size_t outer, inner;
+  B_ENSURE(c, SplitGeometry(c, n, &axis, &outer, &inner), "SPLIT: bad axis or input");
+  const TfLiteTensor* x = T(c, n->inputs, 1);
+  const size_t pitch = x->dims->data[axis] * inner, width = pitch / n->outputs->size;
+  for (int k = 0; k < n->outputs->size; ++k)
+    if (CopyRows(c, T(c, n->outputs, k)->data.raw, x->data.raw + k * width, width, pitch, outer,
+                 "SPLIT") != kTfLiteOk)
+      return kTfLiteError;
+  return kTfLiteOk;
+}
+
 }  // namespace
+
+const char* StridedSliceBounds(const int32_t* dims, int rank, const int32_t* begin, const int32_t* end,
+                               const int32_t* strides, int n, const BuiltinParams& p, SliceBounds* out) {
+  if (rank < 1 || rank > 4) return "STRIDED_SLICE: the input's rank must be 1 to 4";
+  if (n < 1 || n > rank) return "STRIDED_SLICE: begin, end and strides need 1 to rank values";
+  if (p.ellipsis_mask || p.new_axis_mask || p.shrink_axis_mask)
+    return "STRIDED_SLICE: ellipsis_mask, new_axis_mask and shrink_axis_mask are not supported";
+  if (p.offset) return "STRIDED_SLICE: offset is not supported";
+  out->rank = rank;
+  int sliced = 0;
+  for (int k = 0; k < rank; ++k) {
+    const int64_t size = dims[k];
+    int64_t b = 0, e = size;
+    if (k < n) {   // the axes beyond n are whole
+      if (strides[k] != 1) return "STRIDED_SLICE: only unit strides are supported";
+      // strided_slice_logic.h StartForAxis / EndForAxis at stride 1: a mask bit takes the whole
+      // side, a negative index counts from the end, then both clamp to [0, size]
+      b = (p.begin_mask >> k) & 1 ? 0 : begin[k];
+      e = (p.end_mask >> k) & 1 ? size : end[k];
+      if (b < 0) b += size;
+      if (e < 0) e += size;
+      b = std::min(std::max<int64_t>(b, 0), size);
+      e = std::min(std::max(e, b), size);
+    }
+    out->begin[k] = static_cast<int>(b);
+    out->end[k] = static_cast<int>(e);
+    if (b != 0 || e != size) ++sliced;
+  }
+  if (sliced > 1) return "STRIDED_SLICE: at most one axis may be sliced";
+  return nullptr;
+}
 
 const TfLiteRegistration* FusedStemRegistration() {
   static TfLiteRegistration r = {StemInit, StemFree, StemPrepare, StemInvoke};
@@ -706,6 +837,10 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(54, &prelu);   // PRELU
   static TfLiteRegistration logistic = {Init, Free, LogisticPrepare, LogisticInvoke};
   r->AddBuiltin(14, &logistic);  // LOGISTIC
+  static TfLiteRegistration strided_slice = {Init, Free, StridedSlicePrepare, StridedSliceInvoke};
+  r->AddBuiltin(45, &strided_slice);  // STRIDED_SLICE
+  static TfLiteRegistration split = {Init, Free, SplitPrepare, SplitInvoke};
+  r->AddBuiltin(49, &split);  // SPLIT
 }
 
 }  // namespace lce_b200

@@ -17,6 +17,21 @@ struct BuiltinParams {
   float beta;
   int32_t n_new_shape;
   int32_t new_shape[8];
+  // STRIDED_SLICE (StridedSliceOptions) and SPLIT (SplitOptions)
+  int32_t begin_mask, end_mask, ellipsis_mask, new_axis_mask, shrink_axis_mask, offset;
+  int32_t num_splits;
 };
+
+// STRIDED_SLICE's bounds for an input of dims[0..rank) and n = the length of begin / end / strides,
+// normalised as TFLite's strided_slice.cc does (masks, negative indices, clamping): the output is
+// dims with axis k cut to [begin[k], end[k]). Only the form x[..., a:b] lowers to is taken: unit
+// strides and at most one axis not whole. Returns nullptr, or why the slice is refused.
+// builtin_ops.cc; Graph::FuseDenseBlocks matches slices through it too.
+struct SliceBounds {
+  int rank;
+  int begin[4], end[4];
+};
+const char* StridedSliceBounds(const int32_t* dims, int rank, const int32_t* begin, const int32_t* end,
+                               const int32_t* strides, int n, const BuiltinParams& p, SliceBounds* out);
 }  // namespace lce_b200
 #endif

@@ -681,13 +681,51 @@ int Graph::FuseDenseBlocks() {
       if (t.dims->data[d] != 1) return -1;
     return v;
   };
-  // One dense layer read from the MUL at node i: x -> MUL(scale) -> ADD(shift) -> LceQuantize ->
-  // LceBconv2d (float y, one that run_slice takes, same image size) -> CONCATENATION([x, y], last
-  // axis) = out, every intermediate read once and not a graph output.
+  auto producer = [&](int t) {
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.outputs->size; ++q)
+        if (nodes_[k]->node.outputs->data[q] == t) return k;
+    return none;
+  };
+  // node k is a STRIDED_SLICE of x [B,H,W,C] (through the builtin's own normalisation) to the
+  // channels [lo, hi), the other axes whole, with a float output read once and not a graph output
+  auto channel_slice = [&](size_t k, int x, const TfLiteIntArray* xd, int lo, int hi) {
+    if (k >= nodes_.size()) return false;
+    const NodeRecord& n = *nodes_[k];
+    if (n.name != "builtin:45" || n.initialized || !params(n) || n.node.inputs->size != 4 ||
+        n.node.outputs->size != 1 || n.node.inputs->data[0] != x)
+      return false;
+    const int32_t* v[3];
+    for (int q = 0; q < 3; ++q) {
+      const int t = n.node.inputs->data[1 + q];
+      if (t < 0 || tensors_[t].type != kTfLiteInt32 || tensors_[t].allocation_type != kTfLiteMmapRo ||
+          !tensors_[t].data.raw || tensors_[t].dims->size != 1 ||
+          tensors_[t].dims->data[0] != tensors_[n.node.inputs->data[1]].dims->data[0])
+        return false;
+      v[q] = tensors_[t].data.i32;
+    }
+    SliceBounds sb;
+    if (StridedSliceBounds(xd->data, 4, v[0], v[1], v[2], tensors_[n.node.inputs->data[1]].dims->data[0],
+                           *params(n), &sb) != nullptr)
+      return false;
+    for (int d = 0; d < 3; ++d)
+      if (sb.begin[d] != 0 || sb.end[d] != xd->data[d]) return false;
+    const int out = n.node.outputs->data[0];
+    return sb.begin[3] == lo && sb.end[3] == hi && tensors_[out].type == kTfLiteFloat32 &&
+           sole_consumer(out) != none;
+  };
+  // One layer read from the MUL at node i: x -> MUL(scale) -> ADD(shift) -> LceQuantize ->
+  // LceBconv2d (float y, one that run_slice takes, same image size), then either
+  //   dense: CONCATENATION([x, y], last axis) = out, or
+  //   improvement: ADD(b, y) or ADD(y, b) with no activation = sum and CONCATENATION([a, sum], last
+  //   axis) = out, a and b the STRIDED_SLICEs x[..., :C - C_out] and x[..., C - C_out:],
+  // every intermediate read once and not a graph output.
   struct Layer {
-    size_t mul, add, quant, conv, cat;
-    int x, scale, shift, packed, out;
+    int kind;   // DensePrepare's layer kind: 0 dense, 1 improvement
+    size_t mul, add, quant, conv, cat, sum, slice_a, slice_b;
+    int x, scale, shift, packed, out, c_out;
     const TfLiteRegistration* reg;
+    std::vector<size_t> x_readers;   // the layer's nodes that read x, in graph order
   };
   auto match = [&](size_t i, Layer* L) {
     const NodeRecord& m = *nodes_[i];
@@ -736,32 +774,70 @@ int Graph::FuseDenseBlocks() {
     if (d.channels_in != C || d.groups != 1 || yd->data[3] != d.channels_out ||
         !lce_b200_internal_slice_takes(&d))
       return false;
-    L->cat = sole_consumer(y);
-    if (L->cat >= nodes_.size()) return false;
+    L->c_out = d.channels_out;
+    const size_t next = sole_consumer(y);
+    if (next >= nodes_.size()) return false;
+    std::vector<int> cat_ins{x, y};
+    int c_cat = C + d.channels_out;
+    L->kind = nodes_[next]->name == "builtin:2" ? 0 : 1;
+    if (L->kind == 0) {
+      L->cat = next;
+      L->x_readers = {L->mul, L->cat};
+    } else {
+      // the improvement layer's tail
+      L->sum = next;
+      const NodeRecord& a = *nodes_[L->sum];
+      if (a.name != "builtin:0" || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1 ||
+          !params(a) || params(a)->activation != 0 || d.channels_out > C)
+        return false;
+      const int bt = a.node.inputs->data[a.node.inputs->data[0] == y ? 1 : 0];
+      const int sum = a.node.outputs->data[0];
+      const TfLiteIntArray* sd = tensors_[sum].type == kTfLiteFloat32 ? dims4(sum) : nullptr;
+      if (bt < 0 || bt == y || !sd || sd->data[3] != d.channels_out) return false;
+      L->slice_b = producer(bt);
+      if (!channel_slice(L->slice_b, x, xd, C - d.channels_out, C)) return false;
+      L->cat = sole_consumer(sum);
+      if (L->cat >= nodes_.size() || nodes_[L->cat]->node.inputs->size != 2) return false;
+      const int at = nodes_[L->cat]->node.inputs->data[0];
+      L->slice_a = at >= 0 ? producer(at) : none;
+      if (!channel_slice(L->slice_a, x, xd, 0, C - d.channels_out) || L->slice_b >= L->sum ||
+          L->slice_a >= L->cat || L->conv >= L->sum || L->sum >= L->cat)
+        return false;
+      cat_ins = {at, sum};
+      c_cat = C;
+      L->x_readers = {L->mul, L->slice_a, L->slice_b};
+      std::sort(L->x_readers.begin(), L->x_readers.end());
+    }
     const NodeRecord& c = *nodes_[L->cat];
     if (c.name != "builtin:2" || c.initialized || c.node.inputs->size != 2 || c.node.outputs->size != 1 ||
-        c.node.inputs->data[0] != x || c.node.inputs->data[1] != y || !params(c) ||
+        c.node.inputs->data[0] != cat_ins[0] || c.node.inputs->data[1] != cat_ins[1] || !params(c) ||
         params(c)->activation != 0 || (params(c)->axis != 3 && params(c)->axis != -1))
       return false;
     L->out = c.node.outputs->data[0];
     const TfLiteIntArray* od = tensors_[L->out].type == kTfLiteFloat32 ? dims4(L->out) : nullptr;
     return od && od->data[0] == xd->data[0] && od->data[1] == xd->data[1] && od->data[2] == xd->data[2] &&
-           od->data[3] == C + d.channels_out && i < L->add && L->add < L->quant &&
-           L->quant < L->conv && L->conv < L->cat;
+           od->data[3] == c_cat && i < L->add && L->add < L->quant && L->quant < L->conv &&
+           L->conv < L->cat;
   };
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
     Layer first;
     if (nodes_[i]->initialized || !match(i, &first)) continue;
-    // the block: each map x_j (j >= 1) read only by the next layer's MUL and CONCATENATION
+    // the block: each map x_j (j >= 1) read only by the next layer's nodes (a dense layer's MUL and
+    // CONCATENATION, an improvement layer's MUL and two STRIDED_SLICEs)
     std::vector<Layer> block{first};
     for (;;) {
       const int xj = block.back().out;
       if (is_output(xj)) break;
       const std::vector<size_t> readers = consumers(xj);
       Layer next;
-      if (readers.size() != 2 || !match(readers[0], &next) || next.x != xj || next.cat != readers[1])
-        break;
+      bool found = false;
+      for (size_t r : readers)
+        if (match(r, &next) && next.x == xj && next.x_readers == readers) {
+          found = true;
+          break;
+        }
+      if (!found) break;
       block.push_back(next);
     }
     const int X = block.back().out;
@@ -771,8 +847,15 @@ int Graph::FuseDenseBlocks() {
       const Layer& L = block[j];
       const TfLiteIntArray* pd = tensors_[L.packed].dims;
       const std::string tmp_name = names_[L.packed];   // AddTensor appends to names_
-      const int tmp = AddTensor(kTfLiteInt32, std::vector<int>(pd->data, pd->data + 4), nullptr, 0, false,
-                                0.f, 0, tmp_name);
+      std::vector<int> tmps{AddTensor(kTfLiteInt32, std::vector<int>(pd->data, pd->data + 4), nullptr, 0,
+                                      false, 0.f, 0, tmp_name)};
+      if (L.kind == 1) {
+        // the convolution's own output when a CORRECTION plan needs it (DensePrepare sizes it)
+        const TfLiteIntArray* xd = tensors_[L.x].dims;
+        const std::string y_name = names_[nodes_[L.conv]->node.outputs->data[0]];
+        tmps.push_back(AddTensor(kTfLiteFloat32, {xd->data[0], xd->data[1], xd->data[2], L.c_out}, nullptr,
+                                 0, false, 0.f, 0, y_name));
+      }
       NodeRecord& conv = *nodes_[L.conv];
       NodeRecord& n = *nodes_[L.mul];
       std::vector<int> ins{j == 0 ? L.x : X, L.scale, L.shift};
@@ -782,18 +865,25 @@ int Graph::FuseDenseBlocks() {
       LceB200IntArrayFree(n.node.temporaries);
       n.node.inputs = MakeDims(ins);
       n.node.outputs = MakeDims({X});
-      n.node.temporaries = MakeDims({tmp});
+      n.node.temporaries = MakeDims(tmps);
       n.custom_options = conv.custom_options;
       n.node.custom_initial_data = n.custom_options.data();
       n.node.custom_initial_data_size = static_cast<int>(n.custom_options.size());
-      n.builtin_blob.assign(reinterpret_cast<const uint8_t*>(&c_total),
-                            reinterpret_cast<const uint8_t*>(&c_total) + 4);
+      const int32_t blob[2] = {c_total, L.kind};   // DensePrepare
+      n.builtin_blob.assign(reinterpret_cast<const uint8_t*>(blob),
+                            reinterpret_cast<const uint8_t*>(blob) + sizeof(blob));
       n.node.builtin_data = n.builtin_blob.data();
       n.registration = L.reg;
-      n.name = "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION";
-      absorbed.insert(absorbed.end(), {L.add, L.quant, L.conv, L.cat});
+      if (L.kind == 0) {
+        n.name = "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION";
+        absorbed.insert(absorbed.end(), {L.add, L.quant, L.conv, L.cat});
+      } else {
+        n.name = "MUL+ADD+LceQuantize+LceBconv2d+STRIDED_SLICE+ADD+CONCATENATION";
+        absorbed.insert(absorbed.end(), {L.add, L.quant, L.conv, L.slice_a, L.slice_b, L.sum, L.cat});
+      }
     }
-    // drop the absorbed nodes (all after node i), the highest index first
+    // drop the absorbed nodes, the highest index first; a first improvement layer's slices may
+    // precede its MUL, and node i moves back by their number
     std::sort(absorbed.begin(), absorbed.end());
     for (auto it = absorbed.rbegin(); it != absorbed.rend(); ++it) {
       NodeRecord& n = *nodes_[*it];
@@ -803,6 +893,7 @@ int Graph::FuseDenseBlocks() {
       LceB200IntArrayFree(n.node.intermediates);
       nodes_.erase(nodes_.begin() + *it);
       ++removed;
+      if (*it < i) --i;
     }
   }
   allocated_ = false;

@@ -100,19 +100,29 @@ class Graph {
   // BinaryDenseNet's dense layers
   //   x_j [B,H,W,C_j] -> MUL(scale) -> ADD(shift) -> LceQuantize -> LceBconv2d (float y_j)
   //   x_{j+1} = CONCATENATION([x_j, y_j], last axis)
-  // become one node each, "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION": inputs [src, scale,
-  // shift, filter, mul, bias, thr], outputs [X], one temporary for the packed signs. A chain of such
-  // layers shares one tensor X, the block's final map [B,H,W,C_L]; each layer reads X's first C_j
-  // channels and writes its new ones into X[..., C_j : C_j + C_out] (lce_b200_f32_affine_sign,
-  // lce_b200_bconv2d_run_slice), so no x_j and no concatenation copy exists. src is x_0 for the
-  // block's first layer, which also copies x_0 into X, and X for the others. Only when scale and
-  // shift are float constants [C] or [1, ..., 1, C], the MUL and ADD have no fused activation, the
-  // LceBconv2d is a plain node with float output that run_slice takes (same image size), the
-  // CONCATENATION is exactly [x_j, y_j] on the last axis with no activation, C_j and C_L are
-  // multiples of 4, every intermediate has one consumer and is not a graph output, and each x_j
-  // with j >= 1 is read only by its layer's MUL and CONCATENATION. Run before FuseChannelGates and
-  // FuseActivationChains, which would otherwise take the ADD -> LceQuantize as a lone RSign.
-  // Bit-identical. Returns the number of nodes removed.
+  // and MeliusNet's improvement layers
+  //   x_j -> MUL(scale) -> ADD(shift) -> LceQuantize -> LceBconv2d (float y_j, C_out channels)
+  //   a = STRIDED_SLICE(x_j)[..., :C_j - C_out], b = STRIDED_SLICE(x_j)[..., C_j - C_out:]
+  //   x_{j+1} = CONCATENATION([a, ADD(b, y_j)], last axis)
+  // become one node each, "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION" or
+  // "MUL+ADD+LceQuantize+LceBconv2d+STRIDED_SLICE+ADD+CONCATENATION": inputs [src, scale, shift,
+  // filter, mul, bias, thr], outputs [X], temporaries [packed signs] or [packed signs, scratch]. A
+  // chain of such layers shares one tensor X, the block's final map [B,H,W,C_L]; each layer reads
+  // X's first C_j channels; a dense layer writes its new ones into X[..., C_j : C_j + C_out]
+  // (lce_b200_f32_affine_sign, lce_b200_bconv2d_run_slice), an improvement layer adds its own to
+  // X[..., C_j - C_out : C_j] (lce_b200_bconv2d_run_slice_add, through the scratch [B,H,W,C_out]
+  // for a zero-padding CORRECTION plan), so no x_j and no slice or concatenation copy exists. src
+  // is x_0 for the block's first layer, which also copies x_0 into X, and X for the others. Only
+  // when scale and shift are float constants [C] or [1, ..., 1, C], the MUL and ADDs have no fused
+  // activation, the LceBconv2d is a plain node with float output that run_slice takes (same image
+  // size), the CONCATENATION is exactly [x_j, y_j] / [a, sum] on the last axis with no activation,
+  // the slices cover exactly those channels with every other axis whole and unit strides (the
+  // STRIDED_SLICE builtin's own normalisation decides), C_j and C_L are multiples of 4, every
+  // intermediate has one consumer and is not a graph output, and each x_j with j >= 1 is read only
+  // by the next layer's nodes (a dense layer's MUL and CONCATENATION, an improvement layer's MUL
+  // and two STRIDED_SLICEs). Run first: FuseResidualBlocks would otherwise take an improvement
+  // layer's LceBconv2d -> ADD(b), and FuseChannelGates / FuseActivationChains the ADD ->
+  // LceQuantize as a lone RSign. Bit-identical. Returns the number of nodes removed.
   int FuseDenseBlocks();
 
   // Two consecutive residual blocks x1 = x0 + f1(sign x0), x2 = x1 + f2(sign x1) -- a

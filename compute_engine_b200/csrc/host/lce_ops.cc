@@ -769,14 +769,21 @@ TfLiteStatus GateEval(TfLiteContext* context, TfLiteNode* node) {
 }
 
 // ------------------------------------------------------------------------- //
-// A BinaryDenseNet dense layer in one node (Graph::FuseDenseBlocks):
-// [src, scale, shift, filter, mul, bias, thr] -> [X], temporaries [the packed signs]. X is the
-// block's final map [B, H, W, C_L] (builtin_data: int32 C_L); options are the layer's LceBconv2d
-// options, so C_j = channels_in. The node packs the signs of src[..., :C_j] * scale + shift and
-// writes the convolution's channels_out new channels to X[..., C_j : C_j + channels_out]. src is
-// x_0 for a block's first layer, which also copies x_0 into X[..., :C_j] and sets X's shape, and X
-// for the others.
+// A BinaryDenseNet dense layer or a MeliusNet improvement layer in one node
+// (Graph::FuseDenseBlocks): [src, scale, shift, filter, mul, bias, thr] -> [X]. X is the block's
+// final map [B, H, W, C_L]; builtin_data: int32 {C_L, the layer kind (kDenseLayer /
+// kImprovementLayer)}; options are the layer's LceBconv2d options, so C_j = channels_in. The node
+// packs the signs of src[..., :C_j] * scale + shift, then
+//   dense layer, temporaries [packed signs]: writes the convolution's channels_out new channels to
+//     X[..., C_j : C_j + channels_out];
+//   improvement layer, temporaries [packed signs, scratch]: adds them to X[..., C_j - channels_out :
+//     C_j] in place; the scratch is [B, H, W, channels_out] for a zero-padding CORRECTION plan
+//     (lce_b200_bconv2d_run_slice_add) and empty otherwise.
+// src is x_0 for a block's first layer, which also copies x_0 into X[..., :C_j] and sets X's
+// shape, and X for the others.
 // ------------------------------------------------------------------------- //
+enum { kDenseLayer = 0, kImprovementLayer = 1 };
+
 // The node seen as a plain LceBconv2d node [packed signs, filter, mul, bias, thr] -> [X].
 struct DenseLayerView {
   TfLiteNode node{};
@@ -803,18 +810,24 @@ TfLiteStatus ResizeTo(TfLiteContext* context, TfLiteTensor* t, int b, int h, int
   return context->ResizeTensor(context, t, dims);
 }
 
+TfLiteTensor* Temporary(TfLiteContext* context, TfLiteNode* node, int k) {
+  return context->GetTensor ? context->GetTensor(context, node->temporaries->data[k])
+                            : &context->tensors[node->temporaries->data[k]];
+}
+
 template <KernelType kt>
 TfLiteStatus DensePrepare(TfLiteContext* context, TfLiteNode* node) {
   auto* op = static_cast<BconvOpData*>(node->user_data);
   if (!op->successfully_initialized) return kTfLiteError;
-  LCE_ENSURE(context, node->inputs->size == 7 && node->outputs->size == 1 &&
-                          node->temporaries->size == 1 && node->builtin_data != nullptr);
-  const int c_total = *static_cast<const int32_t*>(node->builtin_data);
+  LCE_ENSURE(context, node->inputs->size == 7 && node->outputs->size == 1 && node->builtin_data != nullptr);
+  const int c_total = static_cast<const int32_t*>(node->builtin_data)[0];
+  const int kind = static_cast<const int32_t*>(node->builtin_data)[1];
+  LCE_ENSURE(context, (kind == kDenseLayer && node->temporaries->size == 1) ||
+                          (kind == kImprovementLayer && node->temporaries->size == 2));
   const int c_in = op->desc.channels_in;
   const TfLiteTensor* src = GetInput(context, node, 0);
   TfLiteTensor* x = GetOutput(context, node, 0);
-  TfLiteTensor* packed = context->GetTensor ? context->GetTensor(context, node->temporaries->data[0])
-                                            : &context->tensors[node->temporaries->data[0]];
+  TfLiteTensor* packed = Temporary(context, node, 0);
   LCE_ENSURE(context, src != nullptr && src->type == kTfLiteFloat32 && NumDims(src) == 4);
   LCE_ENSURE(context, x->type == kTfLiteFloat32 && packed->type == kTfLiteInt32);
   const int b = Dim(src, 0), h = Dim(src, 1), w = Dim(src, 2);
@@ -832,9 +845,17 @@ TfLiteStatus DensePrepare(TfLiteContext* context, TfLiteNode* node) {
   DenseLayerView v(node);
   if (BconvPrepare<kt>(context, &v.node) != kTfLiteOk) return kTfLiteError;
   // BconvPrepare gave X the convolution's output shape: the layer keeps the image size and its new
-  // channels fit X; then X takes the block's shape again
+  // channels fit X (a dense layer's after C_j, an improvement layer's before); then X takes the
+  // block's shape again
+  const int c_out = op->desc.channels_out;
   LCE_ENSURE(context, op->desc.out_type == LCE_OUT_FLOAT && Dim(x, 1) == h && Dim(x, 2) == w &&
-                          c_in + op->desc.channels_out <= c_total);
+                          (kind == kDenseLayer ? c_in + c_out <= c_total : c_out <= c_in && c_in <= c_total));
+  if (kind == kImprovementLayer) {
+    TfLiteTensor* scratch = Temporary(context, node, 1);
+    LCE_ENSURE(context, scratch->type == kTfLiteFloat32);
+    const bool corr = op->zp_mode == LCE_ZERO_PADDING_CORRECTION;
+    if (ResizeTo(context, scratch, b, h, w, corr ? c_out : 0) != kTfLiteOk) return kTfLiteError;
+  }
   return ResizeTo(context, x, b, h, w, c_total);
 }
 
@@ -846,8 +867,7 @@ TfLiteStatus DenseEval(TfLiteContext* context, TfLiteNode* node) {
   const TfLiteTensor* scale = GetInput(context, node, 1);
   const TfLiteTensor* shift = GetInput(context, node, 2);
   TfLiteTensor* x = GetOutput(context, node, 0);
-  TfLiteTensor* packed = context->GetTensor ? context->GetTensor(context, node->temporaries->data[0])
-                                            : &context->tensors[node->temporaries->data[0]];
+  TfLiteTensor* packed = Temporary(context, node, 0);
   LCE_ENSURE_MSG(context, OnDevice(src->data.raw) && OnDevice(x->data.raw) && OnDevice(packed->data.raw),
                  "dense LceBconv2d needs a device arena");
   const int c_in = op->desc.channels_in, c_total = Dim(x, 3);
@@ -857,6 +877,13 @@ TfLiteStatus DenseEval(TfLiteContext* context, TfLiteNode* node) {
                                                     scale ? scale->data.f : nullptr,
                                                     shift ? shift->data.f : nullptr, packed->data.i32,
                                                     first ? x->data.f : nullptr, c_total, g_stream));
+  if (static_cast<const int32_t*>(node->builtin_data)[1] == kImprovementLayer) {
+    TfLiteTensor* scratch = Temporary(context, node, 1);
+    LCE_ENSURE_CAPI(context, lce_b200_bconv2d_run_slice_add(
+                                 op->plan, packed->data.i32, x->data.f + c_in - op->desc.channels_out,
+                                 c_total, scratch->bytes ? scratch->data.f : nullptr, g_stream));
+    return kTfLiteOk;
+  }
   LCE_ENSURE_CAPI(context, lce_b200_bconv2d_run_slice(op->plan, packed->data.i32, x->data.f + c_in,
                                                       c_total, g_stream));
   return kTfLiteOk;
@@ -946,8 +973,8 @@ TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_GATE(const TfLiteRegistr
   return nullptr;
 }
 
-// host-internal: the dense-layer node created by Graph::FuseDenseBlocks from a plain LceBconv2d
-// node of this registration (nullptr: not one of this library's LceBconv2d registrations)
+// host-internal: the dense- or improvement-layer node created by Graph::FuseDenseBlocks from a plain
+// LceBconv2d node of this registration (nullptr: not one of this library's LceBconv2d registrations)
 TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_DENSE(const TfLiteRegistration* original) {
   if (original == BconvRegistration<KernelType::kCuda>()) return BconvDenseRegistration<KernelType::kCuda>();
   if (original == BconvRegistration<KernelType::kReference>())

@@ -305,6 +305,17 @@ bool BuildGraphFromTflite(const uint8_t* data, size_t size, const OpResolver& re
         for (int k = 0; k < bp.n_new_shape; ++k) bp.new_shape[k] = ns.at<int32_t>(k);
         break;
       }
+      case 45:  // STRIDED_SLICE: StridedSliceOptions
+        bp.begin_mask = o.scalar<int32_t>(0, 0);
+        bp.end_mask = o.scalar<int32_t>(1, 0);
+        bp.ellipsis_mask = o.scalar<int32_t>(2, 0);
+        bp.new_axis_mask = o.scalar<int32_t>(3, 0);
+        bp.shrink_axis_mask = o.scalar<int32_t>(4, 0);
+        bp.offset = o.scalar<int8_t>(5, 0);
+        break;
+      case 49:  // SPLIT: SplitOptions
+        bp.num_splits = o.scalar<int32_t>(0, 0);
+        break;
       default:
         break;
     }

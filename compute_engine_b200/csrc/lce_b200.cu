@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "lce_b200.h"
@@ -1079,7 +1080,8 @@ static size_t bconv_out_bytes(const lce_b200_bconv2d* plan) {
 static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* out_dev,
                           const float* residual, int residual_act, int32_t* packed_out,
                           const lce_chain_desc* chain, void* stream,
-                          const lce_gate_desc* gate = nullptr, int64_t out_stride = 0) {
+                          const lce_gate_desc* gate = nullptr, int64_t out_stride = 0,
+                          float* scratch = nullptr) {
   const lce_bconv2d_desc& d = plan->d;
   GemmCore& c = plan->core;
   cudaStream_t s = as_stream(stream);
@@ -1147,7 +1149,8 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     return lce_b200_f32_gate_sign(out, gate, residual, residual_act, d.batch,
                                   static_cast<int64_t>(p.OH) * p.OW, c.cout, out, packed_out, stream);
   }
-  // run_slice: the mma.sync kernel's strided store (the caller checked that it takes the plan)
+  // run_slice / run_slice_add: the mma.sync kernel's strided store, and the residual read at the
+  // same strided address (the caller checked that the kernel takes the plan)
   const bool slice = out_stride != 0;
   const Tail plain = slice ? Tail::kSlice : Tail::kNone;
   p.out_stride = slice ? out_stride : c.cout;
@@ -1160,8 +1163,16 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     const int rc = tc_launch(c, p, s);
     if (rc >= 0) return rc;
   }
+  // run_slice_add: the strided residual is the output itself, whose old values the tail still
+  // needs, so the convolution writes [M][cout] to the scratch and the tail reads it from there
+  if (slice && residual != nullptr && scratch == nullptr)
+    return fail("bconv2d: a strided residual with the zero-padding correction needs a scratch");
   lce::ConvKParams q = p;
   q.tap_popc = nullptr; q.residual = nullptr; q.packed_out = nullptr; q.res_stage = 0; q.zp_float = 0;
+  if (scratch != nullptr) {
+    q.out = scratch;
+    q.out_stride = c.cout;
+  }
   const bool tc_was = c.tc_ok;
   c.tc_ok = false;
   const int rc = launch_conv(c, q, s, plain);
@@ -1169,6 +1180,7 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
   if (rc) return rc;
   lce::ZpcTailParams z;
   z.out = static_cast<float*>(out_dev); z.mul = c.mul; z.tap_popc = c.tap_popc;
+  z.src = static_cast<const float*>(q.out); z.src_stride = q.out_stride;
   z.residual = residual; z.packed_out = packed_out; z.M = p.M; z.out_stride = p.out_stride;
   z.H = p.H; z.W = p.W; z.OH = p.OH; z.OW = p.OW; z.KH = p.KH; z.KW = p.KW;
   z.sh = p.sh; z.sw = p.sw; z.dh = p.dh; z.dw = p.dw;
@@ -1264,6 +1276,42 @@ int lce_b200_bconv2d_run_slice(lce_b200_bconv2d* plan, const int32_t* in_dev, fl
   if (o0 < i1 && i0 < o1) return fail("bconv2d_run_slice: output must not overlap the input");
   return bconv_run_impl(plan, in_dev, out_dev, nullptr, LCE_ACT_NONE, nullptr, nullptr, stream,
                         nullptr, out_pixel_stride);
+}
+
+int lce_b200_bconv2d_run_slice_add(lce_b200_bconv2d* plan, const int32_t* in_dev, float* io_dev,
+                                   int64_t io_pixel_stride, float* scratch_dev, void* stream) {
+  const lce_bconv2d_desc& d = plan->d;
+  if (const char* why = slice_refusal(d, &plan->core))
+    return fail("bconv2d_run_slice_add: the plan needs %s", why);
+  if (io_pixel_stride < d.channels_out || io_pixel_stride % 4 != 0)
+    return fail("bconv2d_run_slice_add: the pixel stride %lld must be a multiple of 4 and at "
+                "least channels_out %d", static_cast<long long>(io_pixel_stride), d.channels_out);
+  if (!aligned16(io_dev)) return fail("bconv2d_run_slice_add: io must be 16-byte aligned");
+  const long long px = static_cast<long long>(d.batch) * plan->out_h * plan->out_w;
+  const bool corr = plan->core.tap_popc != nullptr && plan->zp_mode == LCE_ZERO_PADDING_CORRECTION;
+  if (corr && scratch_dev == nullptr)
+    return fail("bconv2d_run_slice_add: a zero-padding CORRECTION plan needs the scratch "
+                "([pixels, channels_out] floats)");
+  if (corr && !aligned16(scratch_dev)) return fail("bconv2d_run_slice_add: scratch must be 16-byte aligned");
+  if (px == 0) return 0;
+  // the spans: io from the first float of pixel 0 to the last of pixel px - 1, the packed input,
+  // the scratch
+  auto span = [](const void* p, uintptr_t bytes) {
+    return std::make_pair(reinterpret_cast<uintptr_t>(p), reinterpret_cast<uintptr_t>(p) + bytes);
+  };
+  auto overlap = [](std::pair<uintptr_t, uintptr_t> a, std::pair<uintptr_t, uintptr_t> b) {
+    return a.first < b.second && b.first < a.second;
+  };
+  const auto io = span(io_dev, (static_cast<uintptr_t>(px - 1) * io_pixel_stride + d.channels_out) * 4);
+  const auto in = span(in_dev, static_cast<uintptr_t>(d.batch) * d.in_h * d.in_w * cdiv(d.channels_in, 32) * 4);
+  if (overlap(io, in)) return fail("bconv2d_run_slice_add: io must not overlap the input");
+  if (corr) {
+    const auto sc = span(scratch_dev, static_cast<uintptr_t>(px) * d.channels_out * 4);
+    if (overlap(sc, io) || overlap(sc, in))
+      return fail("bconv2d_run_slice_add: scratch must not overlap io or the input");
+  }
+  return bconv_run_impl(plan, in_dev, io_dev, io_dev, LCE_ACT_NONE, nullptr, nullptr, stream, nullptr,
+                        io_pixel_stride, corr ? scratch_dev : nullptr);
 }
 
 // Whether lce_b200_bconv2d_run_slice will take a plan created now from *d

@@ -307,8 +307,8 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // registers would exceed the b1 instances' 128-register cap. GATE (float output): Real-to-Binary's
 // gated tail (p.gate) before the shortcut ADD, from chain_s = [- | alpha | sign_scale | sign_shift
 // | mul | bias]; the gate row is each row's own image's (a tile can span several images).
-// SLICE (float output, no shortcut or signs): row m goes to out + m * p.out_stride, a channel
-// slice of a wider map.
+// SLICE (float output, no signs): row m goes to out + m * p.out_stride, a channel slice of a
+// wider map; a shortcut is read at the same strided address, which may be the output itself.
 template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
@@ -325,7 +325,7 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
       bias_r[ns] = *reinterpret_cast<const float2*>(p.bias + cth + ns * 8);
     }
   }
-  const bool has_res = OUT == LCE_OUT_FLOAT && !SLICE && p.residual != nullptr;
+  const bool has_res = OUT == LCE_OUT_FLOAT && p.residual != nullptr;
   const bool has_pk = OUT == LCE_OUT_FLOAT && !SLICE && p.packed_out != nullptr;
   // fused activation of the ADD as one clamp: y = min(max(y, lo), hi) (kernel_util.h:285-300)
   const int ract = p.residual_act;
@@ -392,8 +392,12 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           // extra 36 KB of shared memory cost a resident CTA. The rows are already in L2.)
           float2 rv[8];
           const float* r = p.residual + e0;
+          // SLICE: the residual may be the output this kernel writes, so not the read-only
+          // (non-coherent) path
 #pragma unroll
-          for (int ns = 0; ns < 8; ++ns) rv[ns] = __ldg(reinterpret_cast<const float2*>(r + ns * 8));
+          for (int ns = 0; ns < 8; ++ns)
+            rv[ns] = SLICE ? __ldcg(reinterpret_cast<const float2*>(r + ns * 8))
+                           : __ldg(reinterpret_cast<const float2*>(r + ns * 8));
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns) {
             y[2 * ns] = __fadd_rn(y[2 * ns], rv[ns].x);
@@ -489,7 +493,8 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 // (scale 8). Both produce the same int32 accumulators. CHAIN (float output): the epilogue also
 // applies p.chain (lce_b200_bconv2d_run_fused_chain); GATE (float output): p.gate
 // (lce_b200_bconv2d_run_fused_gate); SLICE (float output): the strided store of
-// lce_b200_bconv2d_run_slice. The other instances compile as without them.
+// lce_b200_bconv2d_run_slice, and its read-add-write in lce_b200_bconv2d_run_slice_add. The other
+// instances compile as without them.
 template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false>
 __global__ void __launch_bounds__(kIThreads, B1 ? kB1Ctas : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {

@@ -98,8 +98,8 @@ struct ConvKParams {
   // GATE instances only: Real-to-Binary's gated tail before the shortcut ADD; packed_out then
   // holds the signs of o * sign_scale + sign_shift
   lce_gate_desc gate;
-  // SLICE instances only: output pixel m's cout floats start at out + m * out_stride
-  // (lce_b200_bconv2d_run_slice)
+  // SLICE instances only: output pixel m's cout floats start at out + m * out_stride, and so do
+  // the residual's (lce_b200_bconv2d_run_slice, lce_b200_bconv2d_run_slice_add)
   long long out_stride;
 };
 
@@ -794,12 +794,15 @@ __global__ void tap_popc_kernel(const int32_t* __restrict__ filter, int32_t* __r
 // ------------------------------------------------------------------------- //
 struct ZpcTailParams {
   float* out;
+  const float* src;          // the convolution's uncorrected output: out, or (with a residual) a
+                             // separate buffer
   const float* mul;          // folded multiplier = -post_activation_multiplier
   const int32_t* tap_popc;   // [cout][taps]
-  const float* residual;
+  const float* residual;     // pixel m at residual + m * out_stride; may be out itself
   int32_t* packed_out;
   long long M;
   long long out_stride;      // floats from one output pixel to the next (cout unless strided)
+  long long src_stride;      // the same for src
   int H, W, OH, OW, KH, KW, sh, sw, dh, dw;
   int cout, cin_pg, cw_out, residual_act;
 };
@@ -830,7 +833,7 @@ __global__ void __launch_bounds__(256) zpc_tail_kernel(const ZpcTailParams p) {
     float y = 0.0f;
     const bool ok = c < p.cout;
     if (ok) {
-      y = p.out[m * p.out_stride + c];
+      y = p.src[m * p.src_stride + c];
       if (cs >= 0) {
         int corr = 0;
         for (int fy = 0; fy < p.KH; ++fy)
@@ -846,7 +849,7 @@ __global__ void __launch_bounds__(256) zpc_tail_kernel(const ZpcTailParams p) {
         y = __fadd_rn(y, __fmul_rn(p.mul[c], static_cast<float>(corr)));
       }
       if (p.residual != nullptr) {
-        y = __fadd_rn(y, p.residual[m * p.cout + c]);
+        y = __fadd_rn(y, p.residual[m * p.out_stride + c]);
         if (p.residual_act == LCE_ACT_RELU) y = fmaxf(y, 0.0f);
         else if (p.residual_act == LCE_ACT_RELU6) y = fminf(fmaxf(y, 0.0f), 6.0f);
         else if (p.residual_act == LCE_ACT_RELU_N1_TO_1) y = fminf(fmaxf(y, -1.0f), 1.0f);

@@ -187,9 +187,11 @@ class HostGraph:
         return lib().lce_host_fuse_float_glue(self._g)
 
     def fuse_dense_blocks(self):
-        """BinaryDenseNet's MUL -> ADD -> LceQuantize -> LceBconv2d -> CONCATENATION layers => one
-        node each, writing into the block's final map in place. Call before fuse_channel_gates,
-        fuse_activation_chains and allocate_tensors."""
+        """BinaryDenseNet's MUL -> ADD -> LceQuantize -> LceBconv2d -> CONCATENATION layers and
+        MeliusNet's improvement layers (the same up to LceBconv2d, whose output is added to the
+        map's last channels through STRIDED_SLICE -> ADD -> CONCATENATION) => one node each, writing
+        into the block's final map in place. Call before the other passes (fuse_residual_blocks
+        would take an improvement layer's LceBconv2d -> ADD) and allocate_tensors."""
         return lib().lce_host_fuse_dense_blocks(self._g)
 
     def fuse_channel_gates(self):
@@ -210,7 +212,7 @@ class HostGraph:
         return lib().lce_host_fuse_residual_pairs(self._g)
 
     def fuse_all(self):
-        return (self.fuse_residual_blocks() + self.fuse_float_glue() + self.fuse_dense_blocks()
+        return (self.fuse_dense_blocks() + self.fuse_residual_blocks() + self.fuse_float_glue()
                 + self.fuse_channel_gates() + self.fuse_activation_chains() + self.fuse_residual_pairs())
 
     # ---- profiling / async IO (bench.py) ----

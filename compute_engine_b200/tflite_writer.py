@@ -111,11 +111,11 @@ TENSOR_TYPE = {np.dtype(np.float32): 0, np.dtype(np.int32): 2, np.dtype(np.uint8
 OP = {"ADD": 0, "AVERAGE_POOL_2D": 1, "CONV_2D": 3, "DEPTHWISE_CONV_2D": 4,
       "FULLY_CONNECTED": 9, "MAX_POOL_2D": 17, "MUL": 18, "RELU": 19, "RESHAPE": 22,
       "SOFTMAX": 25, "MEAN": 40, "CUSTOM": 32, "CONCATENATION": 2, "PAD": 34, "PADV2": 60,
-      "DEQUANTIZE": 6, "PRELU": 54, "LOGISTIC": 14}
+      "DEQUANTIZE": 6, "PRELU": 54, "LOGISTIC": 14, "STRIDED_SLICE": 45, "SPLIT": 49}
 # BuiltinOptions union tags (schema_generated.h:1652-1694)
 OPT_TAG = {"CONV_2D": 1, "DEPTHWISE_CONV_2D": 2, "AVERAGE_POOL_2D": 5, "MAX_POOL_2D": 5,
            "FULLY_CONNECTED": 8, "SOFTMAX": 9, "ADD": 11, "MUL": 21, "RESHAPE": 17, "MEAN": 27,
-           "CONCATENATION": 10, "PAD": 22, "PADV2": 43}
+           "CONCATENATION": 10, "PAD": 22, "PADV2": 43, "STRIDED_SLICE": 32, "SPLIT": 35}
 PADDING = {"SAME": 0, "VALID": 1}
 ACT = {"NONE": 0, "RELU": 1, "RELU_N1_TO_1": 2, "RELU6": 3}
 
@@ -172,6 +172,13 @@ class TFLiteModel:
             return fb.table({0: ("i", int(o.get("axis", 0))), 1: ("b", act)})
         if kind in ("PAD", "PADV2"):
             return fb.table({})
+        if kind == "STRIDED_SLICE":   # StridedSliceOptions
+            return fb.table({0: ("i", o.get("begin_mask", 0)), 1: ("i", o.get("end_mask", 0)),
+                             2: ("i", o.get("ellipsis_mask", 0)), 3: ("i", o.get("new_axis_mask", 0)),
+                             4: ("i", o.get("shrink_axis_mask", 0)),
+                             5: ("b", 1) if o.get("offset") else None})
+        if kind == "SPLIT":           # SplitOptions
+            return fb.table({0: ("i", o["num_splits"])})
         return None
 
     def serialize(self) -> bytes:

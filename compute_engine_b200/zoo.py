@@ -75,6 +75,13 @@ class _Builder:
         shift = self.rng.uniform(-0.5, 0.5, c).astype(np.float32)
         return scale, shift
 
+    def batchnorm(self, t, ts, activation="NONE"):
+        """An unfolded BatchNorm as the converter leaves it: MUL(scale) -> ADD(shift)."""
+        scale, shift = self.bn(ts[3])
+        u = self.act(ts)
+        self.m.add_op("MUL", [t, self.const(scale, name="bn_scale")], [u])
+        return self.add(u, self.const(shift, name="bn_shift"), ts, activation)
+
     # ---- float builtins ----
     def conv(self, x, xs, cout, k, stride, padding="SAME", activation="NONE", bn=True,
              use_bias=True):
@@ -365,13 +372,7 @@ def binarydensenet(batch=1, seed=0, image=224, input_type="float32", pad_values=
     g = _Builder(seed, batch, name)
     xs = (batch, image, image, 3)
     x = g.image_input(xs, input_type)
-
-    def batchnorm(t, ts):
-        scale, shift = g.bn(ts[3])
-        u = g.act(ts)
-        g.m.add_op("MUL", [t, g.const(scale, name="bn_scale")], [u])
-        return g.add(u, g.const(shift, name="bn_shift"), ts)
-
+    batchnorm = g.batchnorm
     x, xs = g.conv(x, xs, 64, 7, 2, activation="RELU")
     x, xs = g.pool("MAX_POOL_2D", x, xs, 3, 2, "SAME")
     for blk, n in enumerate(layers):
@@ -415,8 +416,91 @@ def binarydensenet45(batch=1, seed=0, image=224, input_type="float32", pad_value
                           reduction=(2.7, 3.3, 4), name="BinaryDenseNet45")
 
 
+def meliusnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0, blocks=(4, 5, 4, 6),
+              transitions=(160, 224, 256), name="MeliusNet22"):
+    """MeliusNet, restated from the paper (Bethge et al., 2020) and larq-zoo's MeliusNet22 with
+    synthetic weights, in the converter's op order:
+      stem CONV_2D 3x3/s2 3 -> 32 (BN folded, RELU); a grouped convolution 32 -> 32 in 4 groups,
+      built as larq-zoo's group_conv builds it (tf.split -> one Conv2D per group -> concat):
+      SPLIT(axis 3, 4) -> 4x CONV_2D 3x3 SAME 8 -> 8 (no bias) -> CONCATENATION -> MUL -> ADD(RELU),
+      the BatchNorm and activation after the concatenation; the same 32 -> 64 in 8 groups (8x
+      CONV_2D 4 -> 8); MAX_POOL_2D 3x3/s2 SAME;
+      sections of `blocks` MeliusBlocks (64 -> 320, 160 -> 480, 224 -> 480, 256 -> 640 channels
+      at the default), each a dense layer and then an improvement layer on the map x [B,H,W,C]:
+        dense layer MUL(bn_scale) -> ADD(bn_shift) -> LceQuantize -> LceBconv2d 3x3 C -> 64
+        (`pad_values`, no activation) = y, CONCATENATION([x, y], axis 3), as BinaryDenseNet's;
+        improvement layer MUL -> ADD -> LceQuantize, then a = STRIDED_SLICE(x)[..., :C-64] and
+        b = STRIDED_SLICE(x)[..., C-64:] (constant int32 begin / end / strides, begin_mask and
+        end_mask on the whole axes, the channel bound -64), then LceBconv2d 3x3 C -> 64 = y,
+        ADD(b, y) and CONCATENATION([a, ADD], axis 3): y is added to the map's last 64 channels;
+      transition after every section but the last: MUL -> ADD (BN) -> MAX_POOL_2D 2x2/s2 VALID ->
+      RELU -> CONV_2D 1x1 to `transitions[i]` channels, no bias;
+      head MUL -> ADD (BN) -> RELU -> MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX.
+    Simplifications: larq-zoo's transition convolutions are grouped; these are ungrouped. The
+    slices come before the binary convolution, an order the converter may emit. 38 LceBconv2d,
+    38 STRIDED_SLICE, 2 SPLIT, 16 CONV_2D and 40 CONCATENATION at the default."""
+    g = _Builder(seed, batch, name)
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+
+    def group_conv(t, ts, cout, groups):
+        axis = g.const(np.array(3, np.int32), np.int32, "axis")
+        parts = [g.act(ts[:3] + (ts[3] // groups,)) for _ in range(groups)]
+        g.m.add_op("SPLIT", [axis, t], parts, num_splits=groups)
+        ys = [g.conv(p, ts[:3] + (ts[3] // groups,), cout // groups, 3, 1, bn=False, use_bias=False)[0]
+              for p in parts]
+        ts = ts[:3] + (cout,)
+        z = g.act(ts)
+        g.m.add_op("CONCATENATION", ys, [z], axis=3)
+        return g.batchnorm(z, ts, "RELU"), ts
+
+    def last_channels(t, ts, first):
+        """t[..., :C-64] (first) or t[..., C-64:]: the channel bound is -64, begin_mask /
+        end_mask cover the whole axes."""
+        out = g.act(ts[:3] + (ts[3] - 64 if first else 64,))
+        vec = lambda v: g.const(np.array(v, np.int32), np.int32, "ss")
+        lo, hi = (0, -64) if first else (-64, 0)
+        g.m.add_op("STRIDED_SLICE", [t, vec([0, 0, 0, lo]), vec([0, 0, 0, hi]), vec([1, 1, 1, 1])], [out],
+                   begin_mask=0b1111 if first else 0b0111, end_mask=0b0111 if first else 0b1111)
+        return out
+
+    x, xs = g.conv(x, xs, 32, 3, 2, activation="RELU")
+    x, xs = group_conv(x, xs, 32, 4)
+    x, xs = group_conv(x, xs, 64, 8)
+    x, xs = g.pool("MAX_POOL_2D", x, xs, 3, 2, "SAME")
+    for sec, n in enumerate(blocks):
+        if sec > 0:
+            x = g.batchnorm(x, xs)
+            x, xs = g.pool("MAX_POOL_2D", x, xs, 2, 2, "VALID")
+            x = g.relu(x, xs)
+            x, xs = g.conv(x, xs, transitions[sec - 1], 1, 1, bn=False, use_bias=False)
+        for _ in range(n):
+            # dense layer
+            y, _ = g.bconv(g.quantize(g.batchnorm(x, xs), xs), xs, 64, pad_values=pad_values,
+                           activation="NONE")
+            xs = xs[:3] + (xs[3] + 64,)
+            z = g.act(xs)
+            g.m.add_op("CONCATENATION", [x, y], [z], axis=3)
+            x = z
+            # improvement layer, the slices before the convolution
+            q = g.quantize(g.batchnorm(x, xs), xs)
+            a, b = last_channels(x, xs, True), last_channels(x, xs, False)
+            y, _ = g.bconv(q, xs, 64, pad_values=pad_values, activation="NONE")
+            s = g.add(b, y, xs[:3] + (64,))
+            z = g.act(xs)
+            g.m.add_op("CONCATENATION", [a, s], [z], axis=3)
+            x = z
+    probs = g.head(g.batchnorm(x, xs), xs)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
+def meliusnet22(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    return meliusnet(batch, seed, image, input_type, pad_values)
+
+
 MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "birealnet18": birealnet18,
           "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet,
           "binarydensenet28": binarydensenet28, "binarydensenet37": binarydensenet37,
           "binarydensenet37_dilated": binarydensenet37_dilated,
-          "binarydensenet45": binarydensenet45}
+          "binarydensenet45": binarydensenet45, "meliusnet22": meliusnet22}

@@ -179,6 +179,17 @@ int lce_b200_f32_logistic(const float* in_dev, float* out_dev, int64_t n, void* 
  * to run followed by a copy of each pixel's row. */
 int lce_b200_bconv2d_run_slice(lce_b200_bconv2d* plan, const int32_t* in_dev, float* out_dev,
                                int64_t out_pixel_stride, void* stream);
+/* MeliusNet's improvement layer adds its new channels to a channel slice of the block's map in
+ * place: for every output pixel m and c < channels_out,
+ *   io_dev[m * io_pixel_stride + c] = io_dev[m * io_pixel_stride + c] + y[m][c]
+ * (one __fadd_rn, TFLite's ADD), y being exactly what run computes; nothing else in io is written.
+ * Takes the plans run_slice takes, with its stride, alignment and input-overlap refusals. One-
+ * padding and REFERENCE zero-padding plans run it in one mma.sync launch. A CORRECTION plan (zero
+ * padding with the float correction) writes y to scratch_dev ([pixels, channels_out] floats,
+ * 16-byte aligned, overlapping neither io nor the input) and the correction pass adds it to io;
+ * refuses such a plan without a scratch. Other plans ignore scratch_dev, which may be NULL. */
+int lce_b200_bconv2d_run_slice_add(lce_b200_bconv2d* plan, const int32_t* in_dev, float* io_dev,
+                                   int64_t io_pixel_stride, float* scratch_dev, void* stream);
 /* The signs of a dense layer's BatchNorm in one pass over a strided float [rows, channels] map
  * (row r starts at x_dev + r * x_pixel_stride):
  *   packed_out[r][ceil(channels/32)] = bitpack(x * scale[c] + shift[c]),

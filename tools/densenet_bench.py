@@ -1,18 +1,20 @@
-"""BinaryDenseNet throughput on one GPU, with and without the dense-block fusion.
+"""BinaryDenseNet and MeliusNet throughput on one GPU, with and without the dense-block fusion.
 
-  python tools/densenet_bench.py [--model binarydensenet28] [--batch 256] [--image 224]
+  python tools/densenet_bench.py [--model binarydensenet28|...|meliusnet22] [--batch 256] [--image 224]
                                  [--pad-values 0] [--runs 5] [--steps 20] [--warmup 3]
 
 Two arms on the same int8-input model (synthetic weights, compute_engine_b200/zoo.py):
   base  : fuse_all() without fuse_dense_blocks() -- each dense layer runs as MUL, ADD, LceQuantize,
-          LceBconv2d and a CONCATENATION that copies the whole map
+          LceBconv2d and a CONCATENATION that copies the whole map; each MeliusNet improvement
+          layer as MUL, ADD, LceQuantize, two STRIDED_SLICE copies, LceBconv2d + ADD and a
+          CONCATENATION
   dense : fuse_all() -- each layer packs its signs in one pass and writes its new channels into
-          the block's final map in place
+          the block's final map in place (an improvement layer adds them to the map's last ones)
 Both graphs replay as CUDA graphs with the images already in HBM (the graph's compute, not the
 host link). The arms alternate, `--runs` times each; the JSON line gives each arm's median and
 range in images/s, the card's name, power limit and max SM clock (read with nvidia-smi in the same
-run), per-node-name summed times of one profiled step of each arm with the dense layers' share of it,
-and whether both arms give
+run), per-node-name summed times of one profiled step of each arm with the dense and improvement
+layers' share of it, and whether both arms give
 identical output bits on the same seeded input: with every tensor kept (no arena reuse, so both
 arms lay tensors out alike) and with the arenas the timed graphs use. Needs a GPU; there is no CPU
 path.
@@ -82,7 +84,7 @@ def profile(blob, arm, x):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", default="binarydensenet28",
-                    choices=[m for m in zoo.MODELS if m.startswith("binarydensenet")])
+                    choices=[m for m in zoo.MODELS if m.startswith(("binarydensenet", "meliusnet"))])
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--image", type=int, default=224)
     ap.add_argument("--pad-values", type=int, default=0, choices=(0, 1))
@@ -130,15 +132,24 @@ def main():
         r = sorted(rates[arm])
         out[arm] = {"median": round(float(np.median(r)), 1), "min": round(r[0], 1), "max": round(r[-1], 1)}
     out["profile_ms_per_step"] = prof
-    # the dense layers' nodes: the fused ones, or the five ops each replaces (in the base arm this
-    # also counts the transitions' and the head's BatchNorm MUL and ADD)
-    layer_ops = ("builtin:18", "builtin:0", "LceQuantize", "LceBconv2d", "builtin:2")
+    # the dense and improvement layers' nodes: the fused ones, or the ops each replaces (in the base
+    # arm this also counts the stem's, transitions' and head's BatchNorm MUL and ADD). The
+    # improvement layers alone: their fused nodes (dense arm), or the ops only they have (base arm:
+    # the slices and the convolution with its ADD).
+    dense_node = "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION"
+    improvement_node = "MUL+ADD+LceQuantize+LceBconv2d+STRIDED_SLICE+ADD+CONCATENATION"
+    layer_ops = ("builtin:18", "builtin:0", "LceQuantize", "ADD+LceQuantize", "LceBconv2d", "builtin:2",
+                 "builtin:45", "LceBconv2d+ADD")
     for arm in arms:
         total = sum(prof[arm].values())
-        dense = sum(v for k, v in prof[arm].items()
-                    if k == "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION" or (arm == "base" and k in layer_ops))
+        fused = (dense_node, improvement_node)
+        dense = sum(v for k, v in prof[arm].items() if k in fused or (arm == "base" and k in layer_ops))
+        impr = sum(v for k, v in prof[arm].items()
+                   if k == improvement_node or (arm == "base" and k in ("builtin:45", "LceBconv2d+ADD")))
         out[arm]["dense_layers_ms"] = round(dense, 4)
         out[arm]["dense_layers_share"] = round(dense / total, 3) if total else None
+        out[arm]["improvement_layers_ms"] = round(impr, 4)
+        out[arm]["improvement_layers_share"] = round(impr / total, 3) if total else None
     print(json.dumps(out))
     return 0 if out["identical_outputs"] else 1
 
