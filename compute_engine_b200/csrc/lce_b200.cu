@@ -220,9 +220,11 @@ int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, d
   }
   if (b1) {
     if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, true>(p, grid, smem, s);
+    if (out_type == LCE_OUT_BITPACKED) return launch_imma_vo<V, LCE_OUT_BITPACKED, true>(p, grid, smem, s);
     return launch_imma_vo<V, LCE_OUT_RAW_ACC, true>(p, grid, smem, s);
   }
   if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, false>(p, grid, smem, s);
+  if (out_type == LCE_OUT_BITPACKED) return launch_imma_vo<V, LCE_OUT_BITPACKED, false>(p, grid, smem, s);
   return launch_imma_vo<V, LCE_OUT_RAW_ACC, false>(p, grid, smem, s);
 }
 
@@ -239,7 +241,7 @@ int launch_conv_v(int out_type, const lce::ConvKParams& p, dim3 grid, size_t sme
 }
 int tc_launch(GemmCore& c, const lce::ConvKParams& p, cudaStream_t s);
 
-// The plan's float output goes through the mma.sync kernel (launch_conv's first choice).
+// The plan's output goes through the mma.sync kernel (launch_conv's first choice).
 bool takes_imma(const GemmCore& c, const lce::ConvKParams& p) { return c.wt_nat != nullptr && p.vec_store; }
 
 int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, Tail tail = Tail::kNone) {
@@ -255,10 +257,9 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, Tail tail = Ta
   if (p.img_words >= (1LL << 31)) return fail("input image too large (>= 2^31 packed words)");
   // Which inner product: on H100 the mma.sync kernel (native b1 BMMA, or int8 fragments with
   // LCE_B200_BCONV_B1=0) runs the QuickNet graph faster than the wgmma kernel (bench.py reports
-  // both in one run), so it takes every plan it can (full 64-channel tiles, float or
-  // raw-accumulator output); the wgmma kernel takes the rest it is eligible for (bitpacked and
-  // int8 outputs, other channel counts), XOR + POPC what is left. All produce the same int32
-  // accumulators.
+  // both in one run), so it takes every plan it can (full 64-channel tiles, float, bitpacked or
+  // raw-accumulator output); the wgmma kernel takes the rest it is eligible for (int8 outputs,
+  // other channel counts), XOR + POPC what is left. All produce the same int32 accumulators.
   if (takes_imma(c, p)) {
     // mma.sync inner product: 128 x 64 tiles, the same int32 accumulators as bconv_kernel
     lce::ConvKParams q = p;
@@ -651,11 +652,10 @@ int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
       d_filter, c->wt, c->cout_pg, c->tiles_per_group, c->taps, c->Cw_pg, c->V, c->Kv, total, 0);
   if (launch_check("tile_weights_kernel")) return 1;
   // mma.sync inner product (lce_b200_imma.cuh) where a plan is eligible: full 64-channel
-  // tiles, float or raw-accumulator output. LCE_B200_BCONV_IMMA=0 leaves every plan to the
-  // wgmma / XOR + POPC kernels (bench.py reports both). LCE_B200_BCONV_B1=0 keeps the int8
-  // fragments instead of the packed b1 ones; both give the same accumulators.
-  if (!env_off("LCE_B200_BCONV_IMMA") && c->cout_pg % lce::kBN == 0 &&
-      (c->out_type == LCE_OUT_FLOAT || c->out_type == LCE_OUT_RAW_ACC)) {
+  // tiles, float, bitpacked or raw-accumulator output. LCE_B200_BCONV_IMMA=0 leaves every plan
+  // to the wgmma / XOR + POPC kernels (bench.py reports both). LCE_B200_BCONV_B1=0 keeps the
+  // int8 fragments instead of the packed b1 ones; both give the same accumulators.
+  if (!env_off("LCE_B200_BCONV_IMMA") && c->cout_pg % lce::kBN == 0 && c->out_type != LCE_OUT_INT8) {
     const int Kw = c->taps * c->Cw_pg;
     c->imma_b1 = !env_off("LCE_B200_BCONV_B1");
     const size_t budget = imma_smem_budget(c->V, c->imma_b1);

@@ -1,8 +1,8 @@
 // lce_b200_imma.cuh -- the binary convolution's inner product on the mma.sync tensor pipe.
-// The default for every plan with full 64-channel tiles and float / raw-accumulator output (the
-// three model families' LceBconv2d layers, the BGEMM sweep): on H100 it runs the QuickNet graph
-// faster than the wgmma kernel of lce_b200_tc.cuh, which takes the other plans it is eligible
-// for; the rest, and every plan when LCE_B200_BCONV_IMMA=0 and ..._TC=0, run the XOR + POPC
+// The default for every plan with full 64-channel tiles and float, bitpacked or raw-accumulator
+// output (the model families' LceBconv2d layers, the BGEMM sweep): on H100 it runs the QuickNet
+// graph faster than the wgmma kernel of lce_b200_tc.cuh, which takes the other plans it is
+// eligible for; the rest, and every plan when LCE_B200_BCONV_IMMA=0 and ..._TC=0, run the XOR + POPC
 // kernel of lce_b200_kernels.cuh. All produce the reference's integers bit for bit
 // (tests/test_gpu_parity.py runs the same cases through each); bench.py reports them side by side.
 //
@@ -309,15 +309,18 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // | mul | bias]; the gate row is each row's own image's (a tile can span several images).
 // SLICE (float output, no signs): row m goes to out + m * p.out_stride, a channel slice of a
 // wider map; a shortcut is read at the same strided address, which may be the output itself.
+// BITPACKED: the row's two output words, bit = acc > p.thr[c], packed like the float output's signs.
 template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
                                               int tig, const float* chain_s = nullptr) {
   static_assert(!(CHAIN && GATE), "one epilogue tail at a time");
   static_assert(!SLICE || (OUT == LCE_OUT_FLOAT && !CHAIN && !GATE), "a plain float slice");
+  static_assert(OUT != LCE_OUT_BITPACKED || !(CHAIN || GATE || SLICE), "float tails only");
   constexpr bool STAGED = CHAIN || GATE;
   const int cth = c_tile + tig * 2;
   float2 mul_r[8], bias_r[8];
+  int2 thr_r[8];
   if (OUT == LCE_OUT_FLOAT && !STAGED) {
 #pragma unroll
     for (int ns = 0; ns < 8; ++ns) {
@@ -325,8 +328,12 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
       bias_r[ns] = *reinterpret_cast<const float2*>(p.bias + cth + ns * 8);
     }
   }
+  if (OUT == LCE_OUT_BITPACKED) {
+#pragma unroll
+    for (int ns = 0; ns < 8; ++ns) thr_r[ns] = __ldg(reinterpret_cast<const int2*>(p.thr + cth + ns * 8));
+  }
   const bool has_res = OUT == LCE_OUT_FLOAT && p.residual != nullptr;
-  const bool has_pk = OUT == LCE_OUT_FLOAT && !SLICE && p.packed_out != nullptr;
+  const bool has_pk = OUT == LCE_OUT_BITPACKED || (OUT == LCE_OUT_FLOAT && !SLICE && p.packed_out != nullptr);
   // fused activation of the ADD as one clamp: y = min(max(y, lo), hi) (kernel_util.h:285-300)
   const int ract = p.residual_act;
   const float act_lo = ract == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
@@ -352,7 +359,18 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
         continue;
       }
       uint32_t bits0 = 0, bits1 = 0;
-      if (row_ok) {
+      if (OUT == LCE_OUT_BITPACKED && row_ok) {
+        // OutputTransform<TBitpacked>: bit = acc > threshold (output_transform.h:164-167)
+#pragma unroll
+        for (int ns = 0; ns < 4; ++ns) {
+          bits0 |= (((acc[ms][ns][h * 2] >> S) > thr_r[ns].x ? 1u : 0u) |
+                    ((acc[ms][ns][h * 2 + 1] >> S) > thr_r[ns].y ? 2u : 0u)) << (ns * 8);
+          bits1 |= (((acc[ms][ns + 4][h * 2] >> S) > thr_r[ns + 4].x ? 1u : 0u) |
+                    ((acc[ms][ns + 4][h * 2 + 1] >> S) > thr_r[ns + 4].y ? 2u : 0u)) << (ns * 8);
+        }
+        bits0 <<= tig * 2;
+        bits1 <<= tig * 2;
+      } else if (OUT != LCE_OUT_BITPACKED && row_ok) {
         float y[16];
 #pragma unroll
         for (int ns = 0; ns < 8; ++ns) {
@@ -480,7 +498,8 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
         bits0 |= __shfl_xor_sync(0xffffffffu, bits0, 2);
         bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 2);
         if (row_ok && tig == 0) {
-          int32_t* pk = p.packed_out + static_cast<size_t>(m) * p.cw_out + (c_tile >> 5);
+          int32_t* pk = (OUT == LCE_OUT_BITPACKED ? static_cast<int32_t*>(p.out) : p.packed_out) +
+                        static_cast<size_t>(m) * p.cw_out + (c_tile >> 5);
           pk[0] = static_cast<int32_t>(bits0);
           pk[1] = static_cast<int32_t>(bits1);
         }
