@@ -325,9 +325,27 @@ TfLiteStatus StemInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// The size of `a` when its shape with leading 1s dropped is `x`'s trailing dimensions, else 0. A
+// kernel that reads a[i % size] for element i of x then broadcasts `a` as TFLite does.
+int64_t PreluAlphaCount(const TfLiteTensor* x, const TfLiteTensor* a) {
+  int lead = 0;
+  while (lead < a->dims->size && a->dims->data[lead] == 1) ++lead;
+  const int r = a->dims->size - lead;
+  if (r > x->dims->size) return 0;
+  int64_t n = 1;
+  for (int i = 0; i < r; ++i) {
+    if (a->dims->data[lead + i] != x->dims->data[x->dims->size - r + i]) return 0;
+    n *= a->dims->data[lead + i];
+  }
+  return n;
+}
+
 // ------------------------------ ADD / MUL / RELU ------------------------------ //
-// MUL's one further broadcast: a [B,H,W,C] tensor by a per-image, per-channel [B,1,1,C] one (the
-// channel gate of Real-to-Binary Net); runs as lce_b200_f32_gate_sign with only the gate set.
+// The kernels compute out[i] = a[i] (op) b[i % Count(b)], which is TFLite's broadcast for two shapes
+// of b only: a's own shape, and [C] (a's last dimension) with any leading 1s. A b of higher rank
+// would make the output's rank b's. MUL's one further broadcast: a [B,H,W,C] tensor by a per-image,
+// per-channel [B,1,1,C] one (the channel gate of Real-to-Binary Net); runs as
+// lce_b200_f32_gate_sign with only the gate set.
 bool ImageChannelBroadcast(const TfLiteTensor* a, const TfLiteTensor* b) {
   return a->dims->size == 4 && b->dims->size == 4 && b->dims->data[0] == a->dims->data[0] &&
          b->dims->data[1] == 1 && b->dims->data[2] == 1 && b->dims->data[3] == a->dims->data[3];
@@ -337,10 +355,11 @@ TfLiteStatus EltPrepare(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* a = T(c, n->inputs, 0);
   const TfLiteTensor* b = T(c, n->inputs, 1);
   B_ENSURE(c, a && b, "ADD/MUL: two inputs required");
-  const int64_t na = Count(a), nb = Count(b);
-  const bool plain = nb > 0 && na % nb == 0 && (na == nb || nb == a->dims->data[a->dims->size - 1]);
+  const int64_t na = Count(a), nb = PreluAlphaCount(a, b);
+  const bool plain = a->dims->size > 0 && b->dims->size <= a->dims->size && nb > 0 &&
+                     (nb == na || nb == a->dims->data[a->dims->size - 1]);
   if (MUL)
-    B_ENSURE(c, plain || (nb > 0 && ImageChannelBroadcast(a, b)),
+    B_ENSURE(c, plain || (Count(b) > 0 && ImageChannelBroadcast(a, b)),
              "MUL: only same-shape, last-dimension or [B,H,W,C] x [B,1,1,C] broadcast is supported");
   else
     B_ENSURE(c, plain, "ADD/MUL: only same-shape or last-dimension broadcast is supported");
@@ -396,20 +415,7 @@ TfLiteStatus LogisticInvoke(TfLiteContext* c, TfLiteNode* n) {
 
 // ----------------------------------- PRELU ----------------------------------- //
 // out = x >= 0 ? x : x * alpha (TF/lite/kernels/internal/reference/prelu.h). Alpha broadcasts by
-// element index modulo its size, so its shape with leading 1s dropped must be x's trailing
-// dimensions (per-channel [1, 1, C] among them). Returns that size, or 0 for any other shape.
-int64_t PreluAlphaCount(const TfLiteTensor* x, const TfLiteTensor* a) {
-  int lead = 0;
-  while (lead < a->dims->size && a->dims->data[lead] == 1) ++lead;
-  const int r = a->dims->size - lead;
-  if (r > x->dims->size) return 0;
-  int64_t n = 1;
-  for (int i = 0; i < r; ++i) {
-    if (a->dims->data[lead + i] != x->dims->data[x->dims->size - r + i]) return 0;
-    n *= a->dims->data[lead + i];
-  }
-  return n;
-}
+// element index modulo its size (PreluAlphaCount), per-channel [1, 1, C] among the shapes.
 TfLiteStatus PreluPrepare(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* x = T(c, n->inputs, 0);
   const TfLiteTensor* a = T(c, n->inputs, 1);

@@ -239,6 +239,51 @@ def test_mul_image_channel_broadcast_rule():
     g.close()
 
 
+# b shapes the ADD / MUL kernels (out[i] = a[i] op b[i % Count(b)]) compute as TFLite broadcasts
+ELT_BROADCASTS = [((2, 8, 8, 8), (8,)), ((2, 8, 8, 8), (1, 1, 1, 8)), ((2, 8, 8, 8), (1, 8)),
+                  ((2, 8, 8, 8), (2, 8, 8, 8)), ((1, 8, 8, 8), (8, 8, 8)), ((3, 5, 7, 1), (1,))]
+# b's element count is C or a's, but TFLite broadcasts it over other axes, or to a 5-D output, or
+# not at all: a kernel reading b[i % Count(b)] would return a wrong result or shape
+ELT_WRONG_BROADCASTS = [((2, 8, 8, 8), (1, 8, 1, 1)), ((2, 8, 8, 8), (1, 1, 8, 1)), ((2, 8, 8, 8), (8, 1, 1, 1)),
+                        ((2, 4, 4, 2), (2, 1, 1, 1)), ((2, 8, 8, 8), (1, 1, 1, 1, 8)), ((2, 8, 8, 8), (8, 8, 8, 2)),
+                        ((1, 8, 8, 8), (1, 1, 8, 8, 8))]
+
+
+@pytest.mark.parametrize("op", ["ADD", "MUL"])
+def test_eltwise_broadcast_rule_looks_at_dimensions(op):
+    for a_shape, b_shape in ELT_BROADCASTS:
+        g = H.HostGraph.from_tflite(_binary_graph(op, a_shape, b_shape), device_arena=False)
+        g.allocate_tensors()
+        assert g.shape(g.outputs()[0]) == a_shape
+        g.close()
+    msg = ("MUL: only same-shape, last-dimension or [B,H,W,C] x [B,1,1,C] broadcast is supported" if op == "MUL"
+           else "ADD/MUL: only same-shape or last-dimension broadcast is supported")
+    for a_shape, b_shape in ELT_WRONG_BROADCASTS:
+        g = H.HostGraph.from_tflite(_binary_graph(op, a_shape, b_shape), device_arena=False)
+        with pytest.raises(H.HostError, match=re.escape(msg)):
+            g.allocate_tensors()
+        g.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("op", ["ADD", "MUL"])
+@pytest.mark.parametrize("a_shape,b_shape", ELT_BROADCASTS)
+def test_gpu_eltwise_broadcast_matches_numpy(op, a_shape, b_shape):
+    """One IEEE operation per element: bit-exact against numpy's broadcast in float32."""
+    rng = np.random.default_rng(len(b_shape) * 10 + b_shape[-1])
+    a = rng.standard_normal(a_shape).astype(np.float32)
+    b = rng.standard_normal(b_shape).astype(np.float32)
+    want = (a + b if op == "ADD" else a * b).astype(np.float32)
+    g = H.HostGraph.from_tflite(_binary_graph(op, a_shape, b_shape), device_arena=True)
+    g.allocate_tensors()
+    g.write(g.inputs()[0], a)
+    g.write(g.inputs()[1], b)
+    g.invoke()
+    got = g.read(g.outputs()[0])
+    g.close()
+    assert got.shape == want.shape and np.array_equal(got.view(np.uint32), want.view(np.uint32))
+
+
 def test_gate_instances_compile_without_spills(tmp_path):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
