@@ -44,6 +44,13 @@ class BMaxPoolDesc(C.Structure):
         "stride_h", "stride_w", "padding")]
 
 
+class PoolDesc(C.Structure):
+    """``lce_f32_pool_desc`` (include/lce_b200_builtins.h)."""
+    _fields_ = [(n, C.c_int32) for n in (
+        "batch", "in_h", "in_w", "channels", "filter_h", "filter_w", "stride_h", "stride_w",
+        "padding", "activation")]
+
+
 class ChainDesc(C.Structure):
     """lce_chain_desc: device pointers of the per-channel vectors; None = the op is absent."""
     _fields_ = [("shift_in", C.c_void_p), ("alpha", C.c_void_p), ("shift_out", C.c_void_p),
@@ -82,7 +89,7 @@ EXPORTS = [
     "lce_b200_bconv2d_run_fused_pair",
     "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add",
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_logistic",
-    "lce_b200_f32_affine_sign",
+    "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -244,6 +251,24 @@ def affine_sign(x: torch.Tensor, channels=None, scale=None, shift=None, copy_to=
                                           _p(vecs[0]), _p(vecs[1]), _p(pk), _p(copy_to),
                                           C.c_int64(0 if copy_to is None else copy_to.shape[-1]),
                                           _stream()))
+    return pk
+
+
+def maxpool_affine_sign(x: torch.Tensor, filter_hw, stride_hw, padding=PADDING_VALID, activation=ACT_NONE,
+                        scale=None, shift=None):
+    """MAX_POOL_2D (with its fused activation) -> MUL(scale) -> ADD(shift) -> LceQuantize in one
+    pass over a float NHWC map: the packed signs [B, OH, OW, ceil(C / 32)]. scale / shift: [C]
+    float32 CUDA tensors, or None where that op is absent."""
+    x = _dev(x, torch.float32)
+    b, h, w, c = x.shape
+    vecs = [None if v is None else _dev(v, torch.float32) for v in (scale, shift)]
+    d = PoolDesc(b, h, w, c, filter_hw[0], filter_hw[1], stride_hw[0], stride_hw[1], padding, activation)
+    oh, ow = C.c_int(), C.c_int()
+    _check(lib().lce_b200_f32_pool_out_shape(C.byref(d), C.byref(oh), C.byref(ow)))
+    pk = torch.empty((b, max(oh.value, 0), max(ow.value, 0), cdiv(c, 32)), dtype=torch.int32, device=x.device)
+    _check(lib().lce_b200_f32_maxpool_affine_sign(_p(x), b, h, w, c, filter_hw[0], filter_hw[1], stride_hw[0],
+                                                  stride_hw[1], padding, activation, _p(vecs[0]), _p(vecs[1]),
+                                                  _p(pk), _stream()))
     return pk
 
 

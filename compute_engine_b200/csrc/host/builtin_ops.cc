@@ -184,6 +184,39 @@ TfLiteStatus PoolInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// --------------- fused MAX_POOL_2D -> MUL(scale) -> ADD(shift) -> LceQuantize --------------- //
+// Created by Graph::FusePooledSigns; builtin_data = the pool's BuiltinParams; inputs [x, scale,
+// shift], each constant [C] (or [1, ..., 1, C]) for x [B,H,W,C]; output the packed signs
+// [B,OH,OW,ceil(C/32)].
+TfLiteStatus PooledSignPrepare(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_pool_desc d;
+  B_ENSURE(c, n->inputs->size == 3 && PoolDesc(c, n, &d) && T(c, n->inputs, 0)->type == kTfLiteFloat32,
+           "MAX_POOL_2D+MUL+ADD+LceQuantize: a 4-D float32 input and two constants expected");
+  for (int k = 1; k < 3; ++k) {
+    const TfLiteTensor* v = T(c, n->inputs, k);
+    B_ENSURE(c, v && v->type == kTfLiteFloat32 && Count(v) == d.channels,
+             "MAX_POOL_2D+MUL+ADD+LceQuantize: scale and shift must be float32 with one value per channel");
+  }
+  TfLiteTensor* pk = T(c, n->outputs, 0);
+  B_ENSURE(c, pk && pk->type == kTfLiteInt32, "MAX_POOL_2D+MUL+ADD+LceQuantize: packed output must be int32");
+  int oh, ow;
+  B_CAPI(c, lce_b200_f32_pool_out_shape(&d, &oh, &ow));
+  return Resize(c, pk, {d.batch, oh, ow, (d.channels + 31) / 32});
+}
+TfLiteStatus PooledSignInvoke(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_pool_desc d;
+  PoolDesc(c, n, &d);
+  const TfLiteTensor* scale = T(c, n->inputs, 1);
+  const TfLiteTensor* shift = T(c, n->inputs, 2);
+  B_ENSURE(c, OnDevice(scale->data.raw) && OnDevice(shift->data.raw),
+           "MAX_POOL_2D+MUL+ADD+LceQuantize: constants must be device-resident");
+  B_CAPI(c, lce_b200_f32_maxpool_affine_sign(T(c, n->inputs, 0)->data.f, d.batch, d.in_h, d.in_w, d.channels,
+                                             d.filter_h, d.filter_w, d.stride_h, d.stride_w, d.padding,
+                                             d.activation, scale->data.f, shift->data.f,
+                                             T(c, n->outputs, 0)->data.i32, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // ------------- fused MAX_POOL_2D(2x2 s1 VALID) + DEPTHWISE_CONV_2D(3x3) ------------- //
 // Created by Graph::FuseFloatGlue; builtin_data = { BuiltinParams pool, BuiltinParams dw }.
 struct PoolDwParams {
@@ -805,6 +838,10 @@ const TfLiteRegistration* FusedPoolDepthwiseRegistration() {
 }
 const TfLiteRegistration* ActivationChainRegistration() {
   static TfLiteRegistration r = {Init, Free, ChainPrepare, ChainInvoke};
+  return &r;
+}
+const TfLiteRegistration* PooledSignRegistration() {
+  static TfLiteRegistration r = {Init, Free, PooledSignPrepare, PooledSignInvoke};
   return &r;
 }
 

@@ -903,6 +903,7 @@ int Graph::FuseDenseBlocks() {
 const TfLiteRegistration* FusedPoolDepthwiseRegistration();  // builtin_ops.cc
 const TfLiteRegistration* FusedStemRegistration();
 const TfLiteRegistration* ActivationChainRegistration();
+const TfLiteRegistration* PooledSignRegistration();
 
 int Graph::FuseActivationChains() {
   if (!device_arena_) return 0;
@@ -1041,6 +1042,84 @@ int Graph::FuseActivationChains() {
       if (*it == i) continue;
       free_node(*nodes_[*it]);
       nodes_.erase(nodes_.begin() + *it);
+      ++removed;
+    }
+  }
+  allocated_ = false;
+  return removed;
+}
+
+int Graph::FusePooledSigns() {
+  if (!device_arena_) return 0;
+  const size_t none = nodes_.size() + 1;
+  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
+  auto sole_consumer = [&](int t) {
+    if (is_output(t)) return none;
+    size_t found = none;
+    int n = 0;
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+        if (nodes_[k]->node.inputs->data[q] == t) { ++n; found = k; break; }
+    return n == 1 ? found : none;
+  };
+  // node k (after node `after`) is op(x, v) with v a per-channel float constant ([1, ..., 1, C]) and
+  // no fused activation: returns v, else -1
+  auto const_op = [&](size_t k, size_t after, const char* name, int x, int C) {
+    if (k >= nodes_.size() || k <= after) return -1;
+    const NodeRecord& n = *nodes_[k];
+    if (n.name != name || n.initialized || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
+        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32 ||
+        n.builtin_blob.size() < sizeof(BuiltinParams) ||
+        reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())->activation != 0)
+      return -1;
+    const int v = n.node.inputs->data[1];
+    if (v < 0) return -1;
+    const TfLiteTensor& t = tensors_[v];
+    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
+        t.dims->data[t.dims->size - 1] != C)
+      return -1;
+    for (int d = 0; d + 1 < t.dims->size; ++d)
+      if (t.dims->data[d] != 1) return -1;
+    return v;
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    NodeRecord& p = *nodes_[i];
+    if (p.name != "builtin:17" || p.initialized || p.node.inputs->size != 1 || p.node.outputs->size != 1 ||
+        p.builtin_blob.size() < sizeof(BuiltinParams))
+      continue;
+    const int x = p.node.inputs->data[0], y = p.node.outputs->data[0];
+    const TfLiteIntArray* xd = tensors_[x].dims;
+    if (tensors_[x].type != kTfLiteFloat32 || tensors_[y].type != kTfLiteFloat32 || !xd || xd->size != 4)
+      continue;
+    const int C = xd->data[3];
+    const size_t km = sole_consumer(y);
+    const int scale = const_op(km, i, "builtin:18", y, C);
+    if (scale < 0) continue;
+    const int t1 = nodes_[km]->node.outputs->data[0];
+    const size_t ka = sole_consumer(t1);
+    const int shift = const_op(ka, km, "builtin:0", t1, C);
+    if (shift < 0) continue;
+    const size_t kq = sole_consumer(nodes_[ka]->node.outputs->data[0]);
+    if (kq >= nodes_.size() || kq <= ka) continue;
+    const NodeRecord& q = *nodes_[kq];
+    if (q.name != "LceQuantize" || q.initialized || q.node.inputs->size != 1 || q.node.outputs->size != 1 ||
+        tensors_[q.node.outputs->data[0]].type != kTfLiteInt32)
+      continue;
+    std::vector<int> ins{x, scale, shift}, outs{q.node.outputs->data[0]};
+    LceB200IntArrayFree(p.node.inputs);
+    LceB200IntArrayFree(p.node.outputs);
+    p.node.inputs = MakeDims(ins);
+    p.node.outputs = MakeDims(outs);
+    p.registration = PooledSignRegistration();   // builtin_data stays the pool's parameters
+    p.name = "MAX_POOL_2D+MUL+ADD+LceQuantize";
+    for (size_t k : {kq, ka, km}) {   // the highest index first
+      NodeRecord& n = *nodes_[k];
+      LceB200IntArrayFree(n.node.inputs);
+      LceB200IntArrayFree(n.node.outputs);
+      LceB200IntArrayFree(n.node.temporaries);
+      LceB200IntArrayFree(n.node.intermediates);
+      nodes_.erase(nodes_.begin() + k);
       ++removed;
     }
   }

@@ -97,6 +97,18 @@ class Graph {
   // number of nodes removed.
   int FuseChannelGates();
 
+  // BinaryAlexNet's and XNOR-Net's pooled BatchNorm and sign
+  //   MAX_POOL_2D(x) -> MUL(scale) -> ADD(shift) -> LceQuantize
+  // becomes one node "MAX_POOL_2D+MUL+ADD+LceQuantize" (lce_b200_f32_maxpool_affine_sign): inputs
+  // [x, scale, shift], output [packed signs], builtin_data the pool's parameters; the float map is
+  // read once and only the signs are written. Only when scale and shift are float constants of shape
+  // [C] or [1, ..., 1, C] and the second operand of their op, the MUL and ADD have no fused
+  // activation (the pool's own is applied), and the pool, MUL and ADD outputs each have one consumer
+  // and are not graph outputs; otherwise the graph is left as it is. Run before FuseChannelGates /
+  // FuseActivationChains, which would otherwise take the ADD -> LceQuantize as a lone RSign.
+  // Bit-identical. Returns the number of nodes removed (3 per pooled layer).
+  int FusePooledSigns();
+
   // BinaryDenseNet's dense layers
   //   x_j [B,H,W,C_j] -> MUL(scale) -> ADD(shift) -> LceQuantize -> LceBconv2d (float y_j)
   //   x_{j+1} = CONCATENATION([x_j, y_j], last axis)

@@ -1085,6 +1085,51 @@ __global__ void __launch_bounds__(256) affine_sign_kernel(const float* __restric
   }
 }
 
+// lce_b200_f32_maxpool_affine_sign: MAX_POOL_2D -> MUL -> ADD -> LceQuantize in one pass. One warp
+// per (output pixel, 32-channel word): lane l owns channel 32 * word + l, so every tap is one
+// coalesced 128-byte read, and the ballot of the lanes' signs is the packed word (lanes past C vote
+// 0). The window is visited in pool_kernel's order (rows, then columns, in-bounds taps only) from
+// -FLT_MAX with fmaxf, then the pool's activation; FHW > 0 fixes a square window so the taps unroll.
+template <int FHW, typename I>
+__global__ void __launch_bounds__(256) maxpool_affine_sign_kernel(
+    const float* __restrict__ x, int H, int W, int C, int OH, int OW, int cw, int fh_, int fw_, int sh,
+    int sw, int ph, int pw, int act, const float* __restrict__ scale, const float* __restrict__ shift,
+    int32_t* __restrict__ packed, I words) {
+  const bool has_sc = scale != nullptr, has_sh = shift != nullptr;
+  const int fh = FHW ? FHW : fh_, fw = FHW ? FHW : fw_;
+  const int lane = threadIdx.x & 31;
+  const I warps = static_cast<I>(gridDim.x) * (blockDim.x >> 5);
+  for (I wi = static_cast<I>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); wi < words; wi += warps) {
+    const I pix = wi / cw;
+    const int c = static_cast<int>(wi - pix * cw) * 32 + lane;
+    const int ox = static_cast<int>(pix % OW);
+    const I r = pix / OW;
+    const int oy = static_cast<int>(r % OH);
+    const I b = r / OH;
+    bool bit = false;
+    if (c < C) {
+      const int y0 = oy * sh - ph, x0 = ox * sw - pw;
+      const float* img = x + b * H * W * C + c;
+      float v = -FLT_MAX;
+#pragma unroll
+      for (int fy = 0; fy < fh; ++fy) {
+        const int y = y0 + fy;
+        if (static_cast<unsigned>(y) >= static_cast<unsigned>(H)) continue;
+#pragma unroll
+        for (int fx = 0; fx < fw; ++fx) {
+          const int xx = x0 + fx;
+          if (static_cast<unsigned>(xx) >= static_cast<unsigned>(W)) continue;
+          v = fmaxf(v, __ldg(img + (static_cast<I>(y) * W + xx) * C));
+        }
+      }
+      bit = lce::affine_sign(apply_act(v, act), has_sc, has_sc ? __ldg(scale + c) : 0.0f, has_sh,
+                             has_sh ? __ldg(shift + c) : 0.0f);
+    }
+    const unsigned word = __ballot_sync(0xffffffffu, bit);
+    if (lane == 0) packed[wi] = static_cast<int32_t>(word);
+  }
+}
+
 // LOGISTIC, TFLite's float reference (reference/logistic.h) with CUDA's expf
 __global__ void __launch_bounds__(256) logistic_kernel(const float* __restrict__ in,
                                                        float* __restrict__ out, long long n) {
@@ -1967,6 +2012,44 @@ int lce_b200_f32_affine_sign(const float* x, int64_t x_pixel_stride, int64_t row
     affine_sign_kernel<long long><<<grid, 256, 0, s>>>(x, x_pixel_stride, rows, channels, cw, scale, shift,
                                                        packed, copy, copy_pixel_stride);
   return launch_check("affine_sign_kernel");
+}
+
+int lce_b200_f32_maxpool_affine_sign(const float* x, int batch, int in_h, int in_w, int channels,
+                                     int filter_h, int filter_w, int stride_h, int stride_w, int padding,
+                                     int activation, const float* scale, const float* shift,
+                                     int32_t* packed, void* stream) {
+  if (batch < 0 || in_h <= 0 || in_w <= 0 || channels <= 0)
+    return fail("maxpool_affine_sign: bad shape (%d x %d x %d x %d)", batch, in_h, in_w, channels);
+  if (padding != LCE_PADDING_SAME && padding != LCE_PADDING_VALID)
+    return fail("maxpool_affine_sign: unknown padding %d", padding);
+  if (packed == nullptr) return fail("maxpool_affine_sign: the packed output is required");
+  const lce_f32_pool_desc d{batch, in_h, in_w, channels, filter_h, filter_w, stride_h, stride_w, padding,
+                            activation};
+  int oh, ow;
+  if (lce_b200_f32_pool_out_shape(&d, &oh, &ow)) return 1;
+  if (batch == 0 || oh <= 0 || ow <= 0) return 0;
+  const int ph = pad_before(stride_h, 1, in_h, filter_h, oh);
+  const int pw = pad_before(stride_w, 1, in_w, filter_w, ow);
+  const int cw = (channels + 31) / 32;
+  const long long words = static_cast<long long>(batch) * oh * ow * cw;
+  const int grid = grid_for(words * 32, 256);
+  cudaStream_t s = as_stream(stream);
+  const int f = filter_h == filter_w && (filter_h == 2 || filter_h == 3) ? filter_h : 0;
+  // 32-bit index arithmetic where the input and the word count fit
+  const bool narrow = static_cast<long long>(batch) * in_h * in_w * channels < (1LL << 31) &&
+                      words + 8LL * grid < (1LL << 31);
+#define LCE_MAXPOOL_SIGN(F, I)                                                                            \
+  maxpool_affine_sign_kernel<F, I><<<grid, 256, 0, s>>>(x, in_h, in_w, channels, oh, ow, cw, filter_h,   \
+                                                        filter_w, stride_h, stride_w, ph, pw, activation, \
+                                                        scale, shift, packed, static_cast<I>(words))
+  if (narrow) {
+    if (f == 2) LCE_MAXPOOL_SIGN(2, int); else if (f == 3) LCE_MAXPOOL_SIGN(3, int); else LCE_MAXPOOL_SIGN(0, int);
+  } else {
+    if (f == 2) LCE_MAXPOOL_SIGN(2, long long); else if (f == 3) LCE_MAXPOOL_SIGN(3, long long);
+    else LCE_MAXPOOL_SIGN(0, long long);
+  }
+#undef LCE_MAXPOOL_SIGN
+  return launch_check("maxpool_affine_sign_kernel");
 }
 
 int lce_b200_f32_logistic(const float* in, float* out, int64_t n, void* stream) {

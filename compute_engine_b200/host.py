@@ -200,6 +200,12 @@ class HostGraph:
         Call before fuse_activation_chains and allocate_tensors."""
         return lib().lce_host_fuse_channel_gates(self._g)
 
+    def fuse_pooled_signs(self):
+        """MAX_POOL_2D -> MUL(scale) -> ADD(shift) -> LceQuantize (BinaryAlexNet's and XNOR-Net's
+        pooled BatchNorm and sign) => one node that writes only the signs. Call before
+        fuse_channel_gates, fuse_activation_chains and allocate_tensors."""
+        return lib().lce_host_fuse_pooled_signs(self._g)
+
     def fuse_activation_chains(self):
         """ADD -> PRELU -> ADD [-> ADD -> LceQuantize] (ReActNet's RPReLU / RSign, each step
         optional) => the epilogue of the preceding fused LceBconv2d+ADD node, or one node.
@@ -213,7 +219,8 @@ class HostGraph:
 
     def fuse_all(self):
         return (self.fuse_dense_blocks() + self.fuse_residual_blocks() + self.fuse_float_glue()
-                + self.fuse_channel_gates() + self.fuse_activation_chains() + self.fuse_residual_pairs())
+                + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
+                + self.fuse_residual_pairs())
 
     # ---- profiling / async IO (bench.py) ----
     def enable_profiling(self, on=True):

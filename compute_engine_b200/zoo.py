@@ -84,10 +84,14 @@ class _Builder:
 
     # ---- float builtins ----
     def conv(self, x, xs, cout, k, stride, padding="SAME", activation="NONE", bn=True,
-             use_bias=True):
+             use_bias=True, binary=False):
+        """binary: +-1 weights, what the converter leaves of a binary kernel on a float input."""
         b, h, w, cin = xs
-        wt = self.rng.standard_normal((cout, k, k, cin)).astype(np.float32) * np.float32(
-            1.0 / np.sqrt(k * k * cin))
+        if binary:
+            wt = (self.rng.integers(0, 2, (cout, k, k, cin), dtype=np.int8) * 2 - 1).astype(np.float32)
+        else:
+            wt = self.rng.standard_normal((cout, k, k, cin)).astype(np.float32) * np.float32(
+                1.0 / np.sqrt(k * k * cin))
         bias = np.zeros(cout, np.float32)
         if bn:
             s, t = self.bn(cout)
@@ -145,22 +149,36 @@ class _Builder:
         self.m.add_op("LceQuantize", [x], [y], custom_options=b"")
         return y
 
-    def bconv(self, xq, xs, cout, k=3, stride=1, pad_values=1, activation="RELU", dilation=1):
+    def bconv(self, xq, xs, cout, k=3, stride=1, pad_values=1, activation="RELU", dilation=1,
+              padding="SAME", bitpacked=False):
         """LceBconv2d with float output; BN (and for Bi-RealNet the kernel scale)
         folded into post_activation_multiplier / bias like the converter does
-        (LCE/mlir/transforms/optimize_patterns_common.td:39-113)."""
+        (LCE/mlir/transforms/optimize_patterns_common.td:39-113). bitpacked: int32 output, the
+        signs the next binary layer reads, with synthetic int32 thresholds [cout] around half the
+        accumulators' range K = k * k * cin (inputs 2 and 3 absent) in place of the BN."""
         b, h, w, cin = xs
         signs = self.rng.integers(0, 2, (cout, k, k, cin), dtype=np.int8) * 2 - 1
         bits = np.zeros((cout, k, k, ((cin + 31) // 32) * 32), np.uint32)
         bits[..., :cin] = signs < 0
         filt = (bits.reshape(cout, k, k, -1, 32) << np.arange(32, dtype=np.uint32)).sum(
             -1, dtype=np.uint64).astype(np.uint32).view(np.int32)
+        if padding == "SAME":
+            oh, ow = -(-h // stride), -(-w // stride)
+        else:
+            oh, ow = (h - k) // stride + 1, (w - k) // stride + 1
+        act_code = {"NONE": 0, "RELU": 1}[activation]
+        opts = bconv2d_options(cin, (stride, stride), (dilation, dilation), {"SAME": 0, "VALID": 1}[padding],
+                               pad_values, act_code)
+        if bitpacked:
+            kk = k * k * cin
+            thr = np.rint(kk / 2 + self.rng.standard_normal(cout) * np.sqrt(kk) * 0.75).astype(np.int32)
+            y = self.act((b, oh, ow, (cout + 31) // 32), np.int32)
+            self.m.add_op("LceBconv2d", [xq, self.const(filt, np.int32, "bfilter"), -1, -1,
+                                         self.const(thr, np.int32, "thr")], [y], custom_options=opts)
+            return y, (b, oh, ow, cout)
         s, t = self.bn(cout)
         mul = (s / np.float32(k * k * cin) * np.float32(4.0)).astype(np.float32)
-        oh, ow = -(-h // stride), -(-w // stride)
         y = self.act((b, oh, ow, cout))
-        act_code = {"NONE": 0, "RELU": 1}[activation]
-        opts = bconv2d_options(cin, (stride, stride), (dilation, dilation), 0, pad_values, act_code)
         self.m.add_op("LceBconv2d",
                       [xq, self.const(filt, np.int32, "bfilter"), self.const(mul, name="pmul"),
                        self.const(t, name="pbias"), -1], [y], custom_options=opts)
@@ -499,8 +517,98 @@ def meliusnet22(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
     return meliusnet(batch, seed, image, input_type, pad_values)
 
 
+def _alexnet(g, x, xs, widths, pad_values):
+    """The binary trunk BinaryAlexNet and XNOR-Net share, after the stem's map x: pooled sign ->
+    LceBconv2d 5x5 (float) -> pooled sign -> two LceBconv2d 3x3 with bitpacked output -> LceBconv2d
+    3x3 (float) -> pooled sign -> LceBconv2d VALID over the whole pooled map (bitpacked). A pooled
+    sign is MAX_POOL_2D 3x3/s2 VALID -> MUL(bn_scale) -> ADD(bn_shift) -> LceQuantize. Returns the
+    packed signs of the last layer and their shape."""
+    def pooled_sign(t, ts):
+        t, ts = g.pool("MAX_POOL_2D", t, ts, 3, 2, "VALID")
+        return g.quantize(g.batchnorm(t, ts), ts), ts
+
+    c2, c3, c4, c5, c6 = widths
+    q, qs = pooled_sign(x, xs)
+    y, ys = g.bconv(q, qs, c2, k=5, pad_values=pad_values, activation="NONE")
+    q, qs = pooled_sign(y, ys)
+    q, qs = g.bconv(q, qs, c3, pad_values=pad_values, activation="NONE", bitpacked=True)
+    q, qs = g.bconv(q, qs, c4, pad_values=pad_values, activation="NONE", bitpacked=True)
+    y, ys = g.bconv(q, qs, c5, pad_values=pad_values, activation="NONE")
+    q, qs = pooled_sign(y, ys)
+    return g.bconv(q, qs, c6, k=qs[1], pad_values=pad_values, activation="NONE", padding="VALID",
+                   bitpacked=True)
+
+
+def binaryalexnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    """BinaryAlexNet, restated from larq-zoo with synthetic weights, in the converter's op order
+    (shapes at 224):
+      stem CONV_2D 11x11/s4 SAME 3 -> 64 with +-1 float weights (a binary kernel on the float image,
+      which the converter leaves a float convolution), no bias, no activation -> [B,56,56,64];
+      MAX_POOL_2D 3x3/s2 VALID -> MUL -> ADD (the BatchNorm after the pool) -> LceQuantize;
+      LceBconv2d 5x5 SAME 64 -> 192 (float output, `pad_values`, no activation) -> pooled sign
+      as above -> 13x13;
+      LceBconv2d 3x3 192 -> 384 and 384 -> 384 with bitpacked output (int32 signs, inputs 2 and 3
+      absent, input 4 the int32 thresholds [C_out]);
+      LceBconv2d 3x3 384 -> 256 (float) -> pooled sign -> 6x6;
+      the dense blocks as convolutions: LceBconv2d VALID with a filter covering the pooled map
+      (6x6 at 224) 256 -> 4096, bitpacked; 1x1 4096 -> 4096, bitpacked; 1x1 4096 -> 1000, float;
+      RESHAPE [-1, 1000] -> SOFTMAX.
+    Simplification: larq-zoo flattens the pooled map and applies dense layers; flattening an NHWC
+    map and a dense layer over it is exactly a VALID convolution over the whole map, which keeps
+    those layers binary. The BatchNorm that follows each binary layer with bitpacked output is
+    folded into its thresholds. 7 LceBconv2d (4 bitpacked), 3 pooled signs."""
+    g = _Builder(seed, batch, "BinaryAlexNet")
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+    x, xs = g.conv(x, xs, 64, 11, 4, bn=False, use_bias=False, binary=True)
+    q, qs = _alexnet(g, x, xs, (192, 384, 384, 256, 4096), pad_values)
+    q, qs = g.bconv(q, qs, 4096, k=1, pad_values=pad_values, activation="NONE", padding="VALID",
+                    bitpacked=True)
+    y, ys = g.bconv(q, qs, 1000, k=1, pad_values=pad_values, activation="NONE", padding="VALID")
+    logits = g.act((batch, 1000))
+    g.m.add_op("RESHAPE", [y], [logits], new_shape=[-1, 1000])
+    probs = g.act((batch, 1000))
+    g.m.add_op("SOFTMAX", [logits], [probs], beta=1.0)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
+def xnornet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    """XNOR-Net, restated from larq-zoo with synthetic weights, in the converter's op order (shapes
+    at 224):
+      stem CONV_2D 11x11/s4 SAME 3 -> 96 (BN folded, RELU) -> [B,56,56,96];
+      MAX_POOL_2D 3x3/s2 VALID -> MUL -> ADD (BN) -> LceQuantize;
+      LceBconv2d 5x5 SAME 96 -> 256 (float output, `pad_values`, no activation) -> pooled sign;
+      LceBconv2d 3x3 256 -> 384 and 384 -> 384, bitpacked (int32 thresholds [C_out]);
+      LceBconv2d 3x3 384 -> 256 (float) -> pooled sign -> 6x6;
+      LceBconv2d 6x6 VALID 256 -> 4096, bitpacked; LceBconv2d 1x1 4096 -> 4096, float with fused
+      RELU (BN folded);
+      RESHAPE [-1, 4096] -> FULLY_CONNECTED 1000 (BN folded into its weights and bias) -> SOFTMAX.
+    The per-channel weight scale of XNOR-Net's binary layers folds into each post-activation
+    multiplier, so with synthetic weights it changes nothing. The first dense layer is restated as
+    a VALID convolution over the whole pooled map, as in binaryalexnet. 6 LceBconv2d (3
+    bitpacked), 3 pooled signs."""
+    g = _Builder(seed, batch, "XNORNet")
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+    x, xs = g.conv(x, xs, 96, 11, 4, activation="RELU")
+    q, qs = _alexnet(g, x, xs, (256, 384, 384, 256, 4096), pad_values)
+    y, ys = g.bconv(q, qs, 4096, k=1, pad_values=pad_values, activation="RELU", padding="VALID")
+    flat = g.act((batch, 4096))
+    g.m.add_op("RESHAPE", [y], [flat], new_shape=[-1, 4096])
+    wt = g.rng.standard_normal((1000, 4096)).astype(np.float32) / np.float32(np.sqrt(4096))
+    s, t = g.bn(1000)
+    logits = g.act((batch, 1000))
+    g.m.add_op("FULLY_CONNECTED", [flat, g.const(wt * s[:, None]), g.const(t, name="b")], [logits])
+    probs = g.act((batch, 1000))
+    g.m.add_op("SOFTMAX", [logits], [probs], beta=1.0)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
 MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "birealnet18": birealnet18,
           "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet,
           "binarydensenet28": binarydensenet28, "binarydensenet37": binarydensenet37,
           "binarydensenet37_dilated": binarydensenet37_dilated,
-          "binarydensenet45": binarydensenet45, "meliusnet22": meliusnet22}
+          "binarydensenet45": binarydensenet45, "meliusnet22": meliusnet22,
+          "binaryalexnet": binaryalexnet, "xnornet": xnornet}

@@ -200,6 +200,19 @@ int lce_b200_f32_affine_sign(const float* x_dev, int64_t x_pixel_stride, int64_t
                              int channels, const float* scale, const float* shift,
                              int32_t* packed_out_dev, float* copy_out_dev,
                              int64_t copy_pixel_stride, void* stream);
+/* BinaryAlexNet's and XNOR-Net's pooled BatchNorm and sign, MAX_POOL_2D -> MUL(scale) -> ADD(shift)
+ * -> LceQuantize, in one pass over a float NHWC map [batch, in_h, in_w, channels]:
+ *   packed_out[b][oy][ox][ceil(channels/32)] bit c =
+ *     bitpack(act(max over the in-bounds window) * scale[c] + shift[c]),
+ * the max taken as the MAX_POOL_2D builtin takes it (from -FLT_MAX with fmaxf, then the pool's
+ * fused activation `activation`, an LCE_ACT_* code), the affine step rounded after the multiply and
+ * again after the add, as TFLite's MUL then ADD. Tail bits are 0. padding is LCE_PADDING_SAME or
+ * LCE_PADDING_VALID with the pool's output size; scale or shift may be NULL (that op is absent).
+ * Bit-identical to the four ops one after the other. */
+int lce_b200_f32_maxpool_affine_sign(const float* x_dev, int batch, int in_h, int in_w, int channels,
+                                     int filter_h, int filter_w, int stride_h, int stride_w,
+                                     int padding, int activation, const float* scale,
+                                     const float* shift, int32_t* packed_out_dev, void* stream);
 int lce_b200_bconv2d_run_host(lce_b200_bconv2d* plan, const int32_t* in_host,
                               void* out_host);
 void lce_b200_bconv2d_destroy(lce_b200_bconv2d* plan);
