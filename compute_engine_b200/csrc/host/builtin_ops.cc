@@ -269,7 +269,7 @@ TfLiteStatus PoolDwInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
-// ---- fused stem [DEQUANTIZE +] CONV_2D(3x3 s2, 3 -> 16) + DEPTHWISE_CONV_2D(3x3 s2) ---- //
+// ---- fused stem [DEQUANTIZE +] CONV_2D(3x3 s2, 3 -> 16 or 8) + DEPTHWISE_CONV_2D(3x3 s2) ---- //
 // Created by Graph::FuseStem; builtin_data = { conv1, depthwise } BuiltinParams;
 // inputs [x (float32, or the int8 / uint8 input of the removed DEQUANTIZE), w1, b1, w2, b2].
 struct StemBlob {
@@ -333,12 +333,14 @@ TfLiteStatus StemPrepare(TfLiteContext* c, TfLiteNode* n) {
   B_ENSURE(c, in->type == kTfLiteFloat32 || in->type == kTfLiteInt8 || in->type == kTfLiteUInt8,
            "fused stem: the input must be float32, int8 or uint8");
   B_ENSURE(c, d1.in_c == 3, "fused stem: three input channels expected");
+  const size_t c1 = static_cast<size_t>(d1.out_c);
+  B_ENSURE(c, (c1 == 16 || c1 == 8) && d2.out_c == d1.out_c, "fused stem: 16 or 8 first-conv channels expected");
   auto& sp = *static_cast<StemParams*>(n->user_data);
   if (sp.w1.empty()) {
     B_ENSURE(c, HostCopy(T(c, n->inputs, 1), &sp.w1) && HostCopy(T(c, n->inputs, 2), &sp.b1) &&
                     HostCopy(T(c, n->inputs, 3), &sp.w2) && HostCopy(T(c, n->inputs, 4), &sp.b2) &&
-                    sp.w1.size() == 16 * 27 && sp.w2.size() == 9 * 16 && (sp.b1.empty() || sp.b1.size() == 16) &&
-                    (sp.b2.empty() || sp.b2.size() == 16),
+                    sp.w1.size() == c1 * 27 && sp.w2.size() == 9 * c1 && (sp.b1.empty() || sp.b1.size() == c1) &&
+                    (sp.b2.empty() || sp.b2.size() == c1),
              "fused stem: the filters and biases must be constant float tensors");
   }
   int oh, ow;

@@ -1127,9 +1127,10 @@ int Graph::FusePooledSigns() {
   return removed;
 }
 
-// [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> 16) -> DEPTHWISE_CONV_2D(3x3, stride 2, multiplier 1),
-// each intermediate consumed once: one node (QuickNet's stem). The image is read once, as the
-// bytes the host shipped; the dequantised image and the first conv's map never reach HBM.
+// [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> 16 or 8) -> DEPTHWISE_CONV_2D(3x3, stride 2,
+// multiplier 1), each intermediate consumed once: one node (the stem of QuickNet and QuickNetLarge,
+// 16, and of QuickNetSmall, 8). The image is read once, as the bytes the host shipped; the
+// dequantised image and the first conv's map never reach HBM.
 int Graph::FuseStem() {
   auto sole_consumer = [&](int t, size_t after) -> size_t {
     if (std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end()) return nodes_.size();
@@ -1160,7 +1161,8 @@ int Graph::FuseStem() {
       continue;
     const int w1 = c1.node.inputs->data[1];
     const int x = c1.node.inputs->data[0];
-    if (dims4(w1, 0) != 16 || dims4(w1, 1) != 3 || dims4(w1, 2) != 3 || dims4(w1, 3) != 3 ||
+    const int c1_out = dims4(w1, 0);
+    if ((c1_out != 16 && c1_out != 8) || dims4(w1, 1) != 3 || dims4(w1, 2) != 3 || dims4(w1, 3) != 3 ||
         bp(c1)->stride_h != 2 || bp(c1)->stride_w != 2 || bp(c1)->dilation_h != 1 ||
         bp(c1)->dilation_w != 1 || tensors_[x].type != kTfLiteFloat32 ||
         tensors_[c1.node.outputs->data[0]].type != kTfLiteFloat32)
@@ -1172,7 +1174,7 @@ int Graph::FuseStem() {
         dw.builtin_blob.size() < sizeof(BuiltinParams))
       continue;
     const int w2 = dw.node.inputs->data[1];
-    if (dims4(w2, 1) != 3 || dims4(w2, 2) != 3 || dims4(w2, 3) != 16 || bp(dw)->stride_h != 2 ||
+    if (dims4(w2, 1) != 3 || dims4(w2, 2) != 3 || dims4(w2, 3) != c1_out || bp(dw)->stride_h != 2 ||
         bp(dw)->stride_w != 2 || bp(dw)->dilation_h != 1 || bp(dw)->dilation_w != 1 ||
         bp(dw)->depth_multiplier != 1)
       continue;
@@ -1219,8 +1221,12 @@ int Graph::FuseStem() {
   return 0;
 }
 
+extern "C" int lce_b200_internal_conv_packs_alike(int filter_h, int filter_w, int stride_h,
+                                                  int stride_w, int in_c, int out_c);   // lce_b200_builtins.cu
+
 // CONV_2D (float) whose output also feeds an LceQuantize: the conv emits the packed signs from its
-// epilogue as a second output and the LceQuantize node disappears (first layer of every stage).
+// epilogue as a second output and the LceQuantize node disappears (first layer of every stage),
+// where the signs leave the kernel that computes the floats unchanged.
 int Graph::FuseConvQuantize() {
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
@@ -1228,6 +1234,14 @@ int Graph::FuseConvQuantize() {
     if (conv.name != "builtin:3" || conv.initialized || conv.node.outputs->size != 1) continue;
     const int y = conv.node.outputs->data[0];
     if (tensors_[y].type != kTfLiteFloat32) continue;
+    if (conv.node.inputs->size >= 2 && conv.builtin_blob.size() >= sizeof(BuiltinParams)) {
+      const TfLiteIntArray* fd = tensors_[conv.node.inputs->data[1]].dims;
+      const auto* bp = reinterpret_cast<const BuiltinParams*>(conv.builtin_blob.data());
+      if (fd && fd->size == 4 &&
+          !lce_b200_internal_conv_packs_alike(fd->data[1], fd->data[2], bp->stride_h, bp->stride_w,
+                                              fd->data[3], fd->data[0]))
+        continue;
+    }
     for (size_t k = i + 1; k < nodes_.size(); ++k) {
       NodeRecord& q = *nodes_[k];
       if (q.name != "LceQuantize" || q.initialized || q.node.inputs->size != 1 ||

@@ -144,6 +144,9 @@ struct GemmCore {
   int32_t* wt_nat = nullptr;    // weights in mma B-fragment order: packed b1, or expanded to int8
   int32_t* wpop = nullptr;      // popcount of each channel's filter row (padded by BN)
   bool imma_b1 = false;         // b1 fragments (default) or int8 ones (LCE_B200_BCONV_B1=0)
+  // a 32-channel layer the pair kernel takes: its b1 fragments for that kernel alone (wpop filled
+  // too); the plan's own launches stay on the kernels below, which take every other channel count
+  int32_t* pair_wt = nullptr;
   int imma_Kc_v = 0, imma_chunks = 1;
   size_t imma_smem = 0;
   // wgmma inner product (lce_b200_tc.cuh); absent when LCE_B200_BCONV_TC=0 or ineligible
@@ -160,9 +163,9 @@ struct GemmCore {
 
   void release() {
     cudaFree(wt); cudaFree(mul); cudaFree(bias); cudaFree(thr); cudaFree(tap_popc);
-    cudaFree(wt_nat); cudaFree(wpop);
+    cudaFree(wt_nat); cudaFree(wpop); cudaFree(pair_wt);
     cudaFree(tc_wt); cudaFree(tc_wpop2); cudaFree(tc_tap_popc_t); cudaFree(tc_zpc_cache);
-    wt = wt_nat = wpop = nullptr; mul = bias = nullptr; thr = tap_popc = nullptr;
+    wt = wt_nat = wpop = pair_wt = nullptr; mul = bias = nullptr; thr = tap_popc = nullptr;
     tc_wt = nullptr; tc_wpop2 = tc_tap_popc_t = nullptr; tc_zpc_cache = nullptr; tc_ok = false;
   }
 };
@@ -625,8 +628,9 @@ bool env_off(const char* name) {
 }
 
 // Build the tiled weights (+ optional tap popcounts) from an OHWI-packed filter
-// [cout][taps][Cw_pg] that may live on the host or the device.
-int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
+// [cout][taps][Cw_pg] that may live on the host or the device. pair_b1: a 32-channel layer the
+// pair kernel takes (pair_layer_refusal), which gets the pair kernel's fragments as well.
+int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc, bool pair_b1 = false) {
   const size_t filter_words = static_cast<size_t>(c->cout) * c->taps * c->Cw_pg;
   int32_t* d_filter = nullptr;
   const bool on_dev = is_device_ptr(filter);
@@ -702,6 +706,19 @@ int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc) {
     CUDA_OK(cudaMemset(c->wpop, 0, static_cast<size_t>(c->cout + lce::kBN) * 4));
     lce::tap_popc_kernel<<<cdiv(c->cout, 256), 256>>>(d_filter, c->wpop, c->cout, 1, Kw);
     if (launch_check("tap_popc_kernel")) return 1;
+  } else if (pair_b1) {
+    // one 64-channel tile of b1 fragments whose channels 32-63 are zero (PairShape<1>)
+    const int Kw = c->taps * c->Cw_pg;
+    const int n_slices = cdiv(Kw, 8);
+    const long long total = static_cast<long long>(n_slices) * 256;
+    CUDA_OK(cudaMalloc(&c->pair_wt, total * 8));
+    lce::pack_weights_b1_kernel<<<grid_for(total, 256, 1 << 22), 256>>>(
+        d_filter, reinterpret_cast<uint2*>(c->pair_wt), c->cout_pg, 1, Kw, n_slices, total);
+    if (launch_check("pack_weights_b1_kernel")) return 1;
+    CUDA_OK(cudaMalloc(&c->wpop, static_cast<size_t>(c->cout + lce::kBN) * 4));
+    CUDA_OK(cudaMemset(c->wpop, 0, static_cast<size_t>(c->cout + lce::kBN) * 4));
+    lce::tap_popc_kernel<<<cdiv(c->cout, 256), 256>>>(d_filter, c->wpop, c->cout, 1, Kw);
+    if (launch_check("tap_popc_kernel")) return 1;
   }
   if (build_tc_weights(c, d_filter, want_tap_popc)) return 1;
   if (want_tap_popc) {
@@ -721,24 +738,25 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) ==
 
 // What keeps a layer off the pair kernel (lce_b200_pair.cuh), or nullptr: it takes 3x3, stride 1,
 // dilation 1, ungrouped, SAME one-padded layers with float output and channels_in ==
-// channels_out in {64, 128}, on the b1 mma.sync inner product.
+// channels_out in {32, 64, 128}, on the b1 mma.sync inner product.
 const char* pair_layer_refusal(const lce_bconv2d_desc& d) {
   if (d.out_type != LCE_OUT_FLOAT) return "float output";
   if (d.filter_h != 3 || d.filter_w != 3 || d.stride_h != 1 || d.stride_w != 1 ||
       d.dilation_h != 1 || d.dilation_w != 1 || d.groups != 1)
     return "an ungrouped 3x3 filter with stride 1 and dilation 1";
   if (d.padding != LCE_PADDING_SAME || d.pad_value != 1) return "SAME padding with pad_values = 1";
-  if (d.channels_in != d.channels_out || (d.channels_out != 64 && d.channels_out != 128))
-    return "channels_in == channels_out, 64 or 128";
+  if (d.channels_in != d.channels_out ||
+      (d.channels_out != 32 && d.channels_out != 64 && d.channels_out != 128))
+    return "channels_in == channels_out, 32, 64 or 128";
   if (env_off("LCE_B200_BCONV_IMMA") || env_off("LCE_B200_BCONV_B1"))
     return "the b1 mma.sync inner product (LCE_B200_BCONV_IMMA / _B1 are 0)";
   return nullptr;
 }
 
-// the pair kernel's output tile for C channels (64 or 128)
+// the pair kernel's output tile for C channels (32, 64 or 128)
 void pair_tile(int C, int* th, int* tw) {
-  *th = C == 64 ? lce::PairShape<2>::TH : lce::PairShape<4>::TH;
-  *tw = C == 64 ? lce::PairShape<2>::TW : lce::PairShape<4>::TW;
+  *th = C == 32 ? lce::PairShape<1>::TH : C == 64 ? lce::PairShape<2>::TH : lce::PairShape<4>::TH;
+  *tw = C == 32 ? lce::PairShape<1>::TW : C == 64 ? lce::PairShape<2>::TW : lce::PairShape<4>::TW;
 }
 
 // What keeps a plan off lce_b200_bconv2d_run_slice, or nullptr: float output and the mma.sync
@@ -970,7 +988,8 @@ int lce_b200_bconv2d_create(const lce_bconv2d_desc* d, const int32_t* filter,
   c.Cw_pg = cdiv(d->channels_in / d->groups, 32);
   c.taps = d->filter_h * d->filter_w;
   c.out_type = d->out_type;
-  int rc = build_core_weights(&c, filter, zero_pad);
+  int rc = build_core_weights(&c, filter, zero_pad,
+                              d->channels_out == 32 && pair_layer_refusal(*d) == nullptr);
 
   const size_t padded = static_cast<size_t>(c.cout) + kChanPad;
   if (!rc && d->out_type != LCE_OUT_BITPACKED) {
@@ -1329,7 +1348,7 @@ int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* p
   for (const lce_b200_bconv2d* pl : {plan1, plan2}) {
     if (const char* why = pair_layer_refusal(pl->d))
       return fail("bconv2d_run_fused_pair: each layer needs %s", why);
-    if (!pl->core.imma_b1 || pl->core.wt_nat == nullptr)
+    if (pl->core.pair_wt == nullptr && (!pl->core.imma_b1 || pl->core.wt_nat == nullptr))
       return fail("bconv2d_run_fused_pair: each plan needs the b1 mma.sync weight fragments");
   }
   const lce_bconv2d_desc& d = plan1->d;
@@ -1358,7 +1377,7 @@ int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* p
   const lce_b200_bconv2d* plans[2] = {plan1, plan2};
   for (int k = 0; k < 2; ++k) {
     const GemmCore& c = plans[k]->core;
-    p.wt[k] = reinterpret_cast<const uint2*>(c.wt_nat);
+    p.wt[k] = reinterpret_cast<const uint2*>(c.pair_wt != nullptr ? c.pair_wt : c.wt_nat);
     p.wpop[k] = c.wpop; p.mul[k] = c.mul; p.bias[k] = c.bias;
     p.clamp_min[k] = c.clamp_min; p.clamp_max[k] = c.clamp_max;
   }
@@ -1371,6 +1390,7 @@ int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* p
   const long long grid = static_cast<long long>(d.batch) * p.tiles_per_img;
   if (grid > INT_MAX) return fail("bconv2d_run_fused_pair: too many tiles");
   cudaStream_t s = as_stream(stream);
+  if (CW == 1) return launch_pair<1>(p, static_cast<int>(grid), s);
   if (CW == 2) return launch_pair<2>(p, static_cast<int>(grid), s);
   return launch_pair<4>(p, static_cast<int>(grid), s);
 }
@@ -1381,6 +1401,8 @@ int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* p
 // 0.77 (56x56x64, 28x28x128, 42x42x64, 14x14x64 and x128); 22x22x64 (62 % used) 0.80, 32x32x64
 // (58 %) 0.95, 11x11x128 (62 %) 0.97, 7x7x128 (50 %) 0.88; 16x16x64 and 8x8x128 (33 %) 1.26 and
 // 1.73: there the ring recompute and the empty tile area cost more than x1's round trip saves.
+// The 32-channel instance follows the same rule with the 64-channel tile; it is measured at
+// 56x56 only (QuickNetSmall), not at partial tiles.
 int lce_b200_internal_pair_pays_off(const lce_bconv2d_desc* d) {
   if (pair_layer_refusal(*d) != nullptr || d->in_h < 1 || d->in_w < 1) return 0;
   int th, tw;

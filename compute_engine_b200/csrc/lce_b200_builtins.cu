@@ -1235,10 +1235,11 @@ __global__ void __launch_bounds__(256) pad4d32_kernel(const uint32_t* __restrict
   out[i] = v;
 }
 
-// ---- fused stem: [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> 16) -> DEPTHWISE_CONV_2D(3x3,
-// stride 2) in one pass (QuickNet's stem). Unfused, the dequantised image (154 MB at batch 256) and
-// the first conv's map (205 MB) each make a round trip through HBM; fused, a step reads the int8
-// image and writes the 51 MB depthwise map.
+// ---- fused stem: [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> C1) -> DEPTHWISE_CONV_2D(3x3,
+// stride 2) in one pass, C1 = 16 (QuickNet, QuickNetLarge) or 8 (QuickNetSmall). Unfused, the
+// dequantised image (154 MB at batch 256) and the first conv's map (205 MB at C1 = 16, 103 MB at 8)
+// each make a round trip through HBM; fused, a step reads the int8 image and writes the depthwise
+// map. The text below counts C1 = 16; at C1 = 8 each first-conv pixel is two 16-byte cells.
 //   Persistent CTAs (one per SM, 512 threads). A tile = 4 output rows x <= 56 output columns of
 // one image. Its 19 x 227 x 3 input patch is fetched as raw bytes (cp.async, double-buffered: the
 // next tile's patch arrives while this one computes), padded in the QUANTISED domain (zero point;
@@ -1273,13 +1274,14 @@ struct Stem2Geom {
   int in_zero_point;
   double in_scale;
 };
+template <int C1>
 struct StemWeights {
-  float w1[27][16];   // [tap * 3 + ci][co]
-  float b1[16];
-  float w2[9][16];    // [tap][c]
-  float b2[16];
+  float w1[27][C1];   // [tap * 3 + ci][co]
+  float b1[C1];
+  float w2[9][C1];    // [tap][c]
+  float b2[C1];
 };
-template <typename TIn>
+template <typename TIn, int C1>
 struct Stem2Layout {
   static constexpr int kRawPitch = kS2RawCols * 3 * static_cast<int>(sizeof(TIn));          // 720 / 2880 B
   static constexpr int kLutBytes = sizeof(TIn) == 1 ? 256 * 32 * 4 : 0;
@@ -1290,34 +1292,36 @@ struct Stem2Layout {
   static constexpr int kGroups = sizeof(TIn) == 1 ? 2 : 1;
   static constexpr int kC1Bufs = 1;
   static constexpr size_t kGroupRawBytes = 2 * static_cast<size_t>(kS2R0) * kRawPitch + 64;
-  static constexpr size_t kSmemBytes = kGroups * (kGroupRawBytes + kC1Bufs * kS2R1 * kS2C1 * 64) + (9 * 16 + 16) * 4 + kLutBytes;
+  static constexpr size_t kSmemBytes = kGroups * (kGroupRawBytes + kC1Bufs * kS2R1 * kS2C1 * C1 * 4) + (9 * C1 + C1) * 4 + kLutBytes;
 };
 
-template <typename TIn, bool kUnsigned>
+template <typename TIn, bool kUnsigned, int C1>
 __global__ void __launch_bounds__(kS2Threads, 1)
-stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const __grid_constant__ StemWeights Wt,
+stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const __grid_constant__ StemWeights<C1> Wt,
                     const Stem2Geom s) {
+  static_assert(C1 == 8 || C1 == 16, "the fused stem takes 8 or 16 first-conv channels");
   extern __shared__ __align__(16) unsigned char sm_raw[];
-  constexpr int kRawPitch = Stem2Layout<TIn>::kRawPitch;
+  using Lay = Stem2Layout<TIn, C1>;
+  constexpr int kRawPitch = Lay::kRawPitch;
   constexpr bool kQuant = sizeof(TIn) == 1;
-  using Lay = Stem2Layout<TIn>;
   constexpr int kGroups = Lay::kGroups, kG = kS2Threads / kGroups;                // threads per group
   constexpr int kC1Bufs = Lay::kC1Bufs;
-  constexpr int kC1Floats = kS2R1 * kS2C1 * 16;
+  constexpr int kC1Floats = kS2R1 * kS2C1 * C1;
+  constexpr int kQ = C1 / 4;                                                      // 16-byte cells per pixel
   const int gid = threadIdx.x / kG, tid = threadIdx.x - gid * kG, lane = threadIdx.x & 31;   // tid: inside the group
   unsigned char* raw0 = sm_raw + gid * Lay::kGroupRawBytes;                       // [2][19][kRawPitch] (+ slack)
   float* c1_all = reinterpret_cast<float*>(sm_raw + kGroups * Lay::kGroupRawBytes);
-  float* c1_0 = c1_all + gid * kC1Bufs * kC1Floats;                               // [kC1Bufs][9][113][16], swizzled
-  float* w2s = c1_all + kGroups * kC1Bufs * kC1Floats;                            // [9][16]
-  float* b2s = w2s + 9 * 16;
-  float* lut = b2s + 16;                                                          // [256][32]
+  float* c1_0 = c1_all + gid * kC1Bufs * kC1Floats;                               // [kC1Bufs][9][113][C1], swizzled
+  float* w2s = c1_all + kGroups * kC1Bufs * kC1Floats;                            // [9][C1]
+  float* b2s = w2s + 9 * C1;
+  float* lut = b2s + C1;                                                          // [256][32]
   auto group_barrier = [&]() {
     if (kGroups == 1) __syncthreads();
     else asm volatile("bar.sync %0, %1;" ::"r"(1 + gid), "r"(kG) : "memory");
   };
 
-  for (int i = threadIdx.x; i < 9 * 16; i += kS2Threads) w2s[i] = Wt.w2[i >> 4][i & 15];
-  if (threadIdx.x < 16) b2s[threadIdx.x] = Wt.b2[threadIdx.x];
+  for (int i = threadIdx.x; i < 9 * C1; i += kS2Threads) w2s[i] = Wt.w2[i / C1][i % C1];
+  if (threadIdx.x < C1) b2s[threadIdx.x] = Wt.b2[threadIdx.x];
   if (kQuant) {
     for (int i = threadIdx.x; i < 256 * 32; i += kS2Threads) {
       const int byte = i >> 5;
@@ -1399,11 +1403,11 @@ stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const _
     for (int task = tid; task < tasks; task += kG) {
       const int rr = task / tpr, tt = task - rr * tpr;
       const int l1 = l1_lo + rr, cg = cl_lo + 2 * tt;
-      float2 acc[2][8];
+      float2 acc[2][C1 / 2];
 #pragma unroll
       for (int p = 0; p < 2; ++p)
 #pragma unroll
-        for (int c = 0; c < 8; ++c) acc[p][c] = make_float2(0.0f, 0.0f);
+        for (int c = 0; c < C1 / 2; ++c) acc[p][c] = make_float2(0.0f, 0.0f);
       const unsigned char* row0 = raw + (2 * l1) * kRawPitch + 6 * cg * static_cast<int>(sizeof(TIn));
       // byte images: all 12 words of the three patch rows are requested before the first lookup
       uint32_t rw[3][4];
@@ -1441,7 +1445,7 @@ stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const _
           for (int ci = 0; ci < 3; ++ci) {
             const int kk = (fy * 3 + fx) * 3 + ci;
 #pragma unroll
-            for (int c = 0; c < 8; ++c) {
+            for (int c = 0; c < C1 / 2; ++c) {
               const float2 w = make_float2(Wt.w1[kk][2 * c], Wt.w1[kk][2 * c + 1]);
 #pragma unroll
               for (int p = 0; p < 2; ++p) {
@@ -1455,10 +1459,10 @@ stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const _
       for (int p = 0; p < 2; ++p) {
         const int cl = cg + p;
         if (cl >= cl_hi) continue;
-        float* dst = c1 + (l1 * kS2C1 + cl) * 16;
-        const int sw = (cl >> 1) & 3;   // 16-byte cell swizzle: neighbouring tasks hit different banks
+        float* dst = c1 + (l1 * kS2C1 + cl) * C1;
+        const int sw = (cl >> 1) & (kQ - 1);   // 16-byte cell swizzle: neighbouring tasks hit different banks
 #pragma unroll
-        for (int q = 0; q < 4; ++q)
+        for (int q = 0; q < kQ; ++q)
           *reinterpret_cast<float4*>(dst + ((q ^ sw) << 2)) =
               make_float4(apply_act(acc[p][2 * q].x + Wt.b1[4 * q], s.act1), apply_act(acc[p][2 * q].y + Wt.b1[4 * q + 1], s.act1),
                           apply_act(acc[p][2 * q + 1].x + Wt.b1[4 * q + 2], s.act1),
@@ -1470,32 +1474,32 @@ stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const _
   // column offsets, their validity and the 9 weight vectors are per-thread constants;
   // out-of-range taps are skipped like depthwise_v4_kernel skips them.
   auto stage2 = [&](const Tile& T, const float* c1) {
-    const int n2 = T.tw * 4;
+    const int n2 = T.tw * kQ;
     for (int task = tid; task < 2 * n2; task += kG) {
     const int half = task >= n2 ? 1 : 0;
     const int r2 = task - half * n2;
-    const int lx = r2 >> 2, q = r2 & 3;
+    const int lx = r2 / kQ, q = r2 % kQ;
     int off[3];
     bool cok[3];
 #pragma unroll
     for (int fx = 0; fx < 3; ++fx) {
       const int cl = 2 * lx + fx;
       cok[fx] = static_cast<unsigned>(T.x1_0 + cl) < static_cast<unsigned>(s.OW1);
-      off[fx] = cl * 16 + ((q ^ ((cl >> 1) & 3)) << 2);
+      off[fx] = cl * C1 + ((q ^ ((cl >> 1) & (kQ - 1))) << 2);
     }
     float4 wv[9];
 #pragma unroll
-    for (int k = 0; k < 9; ++k) wv[k] = *reinterpret_cast<const float4*>(w2s + k * 16 + q * 4);
+    for (int k = 0; k < 9; ++k) wv[k] = *reinterpret_cast<const float4*>(w2s + k * C1 + q * 4);
     const float4 bb = *reinterpret_cast<const float4*>(b2s + q * 4);
     float4* o = reinterpret_cast<float4*>(out) +
-                ((static_cast<long long>(T.b) * s.OH2 + T.oy2_0) * s.OW2 + T.ox2_0 + lx) * 4 + q;
+                ((static_cast<long long>(T.b) * s.OH2 + T.oy2_0) * s.OW2 + T.ox2_0 + lx) * kQ + q;
     for (int ly = 2 * half; ly < 2 * half + 2 && T.oy2_0 + ly < s.OH2; ++ly) {
       float2 a0 = make_float2(0.f, 0.f), a1 = make_float2(0.f, 0.f);
 #pragma unroll
       for (int fy = 0; fy < 3; ++fy) {
         const int l1 = 2 * ly + fy;
         if (static_cast<unsigned>(T.y1_0 + l1) >= static_cast<unsigned>(s.OH1)) continue;
-        const float* rowp = c1 + l1 * (kS2C1 * 16);
+        const float* rowp = c1 + l1 * (kS2C1 * C1);
 #pragma unroll
         for (int fx = 0; fx < 3; ++fx) {
           if (!cok[fx]) continue;
@@ -1505,7 +1509,7 @@ stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const _
           a1 = fma2_rn(make_float2(x.z, x.w), make_float2(w.z, w.w), a1);
         }
       }
-      o[static_cast<long long>(ly) * s.OW2 * 4] =
+      o[static_cast<long long>(ly) * s.OW2 * kQ] =
           make_float4(apply_act(a0.x + bb.x, s.act2), apply_act(a0.y + bb.y, s.act2),
                       apply_act(a1.x + bb.z, s.act2), apply_act(a1.y + bb.w, s.act2));
     }
@@ -1538,14 +1542,14 @@ stem_conv_dw_kernel(const TIn* __restrict__ in, float* __restrict__ out, const _
   }
 }
 
-template <typename TIn, bool kUnsigned>
-int launch_stem2(const void* in, const StemWeights& wt, float* out, const Stem2Geom& s, void* stream) {
+template <typename TIn, bool kUnsigned, int C1>
+int launch_stem2(const void* in, const StemWeights<C1>& wt, float* out, const Stem2Geom& s, void* stream) {
   static bool attr_dev[64] = {};   // the attribute is per device
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
-  constexpr size_t smem = Stem2Layout<TIn>::kSmemBytes;
+  constexpr size_t smem = Stem2Layout<TIn, C1>::kSmemBytes;
   if (!(dev >= 0 && dev < 64 && attr_dev[dev])) {
-    if (cudaFuncSetAttribute(stem_conv_dw_kernel<TIn, kUnsigned>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    if (cudaFuncSetAttribute(stem_conv_dw_kernel<TIn, kUnsigned, C1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              static_cast<int>(smem)) != cudaSuccess)
       return fail("stem_conv_dw: cannot raise the shared-memory limit");
     if (dev >= 0 && dev < 64) attr_dev[dev] = true;
@@ -1553,10 +1557,27 @@ int launch_stem2(const void* in, const StemWeights& wt, float* out, const Stem2G
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long tiles = static_cast<long long>(s.B) * s.n_rt * s.n_ct;
   if (tiles > (1LL << 29)) return fail("stem_conv_dw: too many tiles");
-  constexpr int groups = Stem2Layout<TIn>::kGroups;
+  constexpr int groups = Stem2Layout<TIn, C1>::kGroups;
   const unsigned grid = static_cast<unsigned>(std::min<long long>((tiles + groups - 1) / groups, sms));
-  stem_conv_dw_kernel<TIn, kUnsigned><<<grid, kS2Threads, smem, as_stream(stream)>>>(static_cast<const TIn*>(in), out, wt, s);
+  stem_conv_dw_kernel<TIn, kUnsigned, C1><<<grid, kS2Threads, smem, as_stream(stream)>>>(static_cast<const TIn*>(in), out, wt, s);
   return launch_check("stem_conv_dw_kernel");
+}
+
+// The filters in the kernel's order, then the launch for the image's element type.
+template <int C1>
+int stem2_run(int in_type, const void* in, const float* w1, const float* b1, const float* w2, const float* b2,
+              float* out, const Stem2Geom& s, void* stream) {
+  StemWeights<C1> wt;
+  for (int k = 0; k < 27; ++k)
+    for (int c = 0; c < C1; ++c) wt.w1[k][c] = w1[c * 27 + k];   // OHWI [C1][3][3][3] -> [k][co]
+  for (int i = 0; i < 9 * C1; ++i) wt.w2[i / C1][i % C1] = w2[i];
+  for (int c = 0; c < C1; ++c) {
+    wt.b1[c] = b1 ? b1[c] : 0.0f;
+    wt.b2[c] = b2 ? b2[c] : 0.0f;
+  }
+  if (in_type == LCE_T_FLOAT) return launch_stem2<float, false, C1>(in, wt, out, s, stream);
+  if (in_type == LCE_T_INT8) return launch_stem2<int8_t, false, C1>(in, wt, out, s, stream);
+  return launch_stem2<uint8_t, true, C1>(in, wt, out, s, stream);
 }
 
 int make_geom(const lce_f32_conv_desc* d, ConvGeom* g) {
@@ -1614,6 +1635,19 @@ int lce_b200_f32_conv_out_shape(const lce_f32_conv_desc* d, int* out_h, int* out
   *out_h = g.OH;
   *out_w = g.OW;
   return 0;
+}
+
+// Whether conv2d_impl computes a convolution's floats on the same kernel with and without the
+// signs of its output (Graph::FuseConvQuantize asks before it rewrites the graph, so that
+// CONV_2D+LceQuantize equals CONV_2D then LceQuantize bit for bit). The tensor-core pointwise
+// kernel packs whole 128-column tiles only: a 1x1 stride-1 convolution it takes without the signs
+// (K a multiple of 32) but of another width, such as QuickNetSmall's 32 -> 64 transition, would
+// run on another kernel with them.
+int lce_b200_internal_conv_packs_alike(int filter_h, int filter_w, int stride_h, int stride_w,
+                                       int in_c, int out_c) {
+  const bool pw = filter_h == 1 && filter_w == 1 && stride_h == 1 && stride_w == 1 &&
+                  in_c % 32 == 0 && in_c <= 4096;
+  return !(pw && out_c % 32 == 0 && out_c % 128 != 0);
 }
 
 // `packed` (optional): LceQuantize of the output. Kernels that can emit it in their epilogue do
@@ -1876,9 +1910,10 @@ int lce_b200_f32_stem_conv_dw(const lce_f32_conv_desc* conv1, const lce_f32_conv
   ConvGeom g1, g2;
   if (make_geom(conv1, &g1) || make_geom(dw, &g2)) return 1;
   const bool ok = g1.KH == 3 && g1.KW == 3 && g1.sh == 2 && g1.sw == 2 && g1.dh == 1 && g1.dw == 1 && g1.Cin == 3 &&
-                  g1.Cout == 16 && g2.KH == 3 && g2.KW == 3 && g2.sh == 2 && g2.sw == 2 && g2.dh == 1 && g2.dw == 1 &&
-                  g2.Cin == 16 && g2.Cout == 16 && g2.H == g1.OH && g2.W == g1.OW && g2.B == g1.B;
-  if (!ok) return fail("stem_conv_dw: unsupported shapes (3x3/s2 3 -> 16, depthwise 3x3/s2)");
+                  (g1.Cout == 8 || g1.Cout == 16) && g2.KH == 3 && g2.KW == 3 && g2.sh == 2 && g2.sw == 2 &&
+                  g2.dh == 1 && g2.dw == 1 && g2.Cin == g1.Cout && g2.Cout == g1.Cout && g2.H == g1.OH &&
+                  g2.W == g1.OW && g2.B == g1.B;
+  if (!ok) return fail("stem_conv_dw: unsupported shapes (3x3/s2 3 -> 8 or 16, depthwise 3x3/s2)");
   if (in_type != LCE_T_FLOAT && in_type != LCE_T_INT8 && in_type != LCE_T_BOOL) return fail("stem_conv_dw: bad input type");
   if ((uintptr_t)out & 15) return fail("stem_conv_dw: unaligned output");
   if (g1.B == 0 || g2.OH == 0 || g2.OW == 0) return 0;
@@ -1893,17 +1928,8 @@ int lce_b200_f32_stem_conv_dw(const lce_f32_conv_desc* conv1, const lce_f32_conv
   // at the row's end or 240 columns on is a whole number of 16-byte chunks
   s.aligned = (((uintptr_t)in & 15) == 0 && (static_cast<long long>(g1.W) * 3 * es) % 16 == 0) ? 1 : 0;
   if (!w1 || !w2) return fail("stem_conv_dw: the filters must be host pointers");
-  StemWeights wt;
-  for (int k = 0; k < 27; ++k)
-    for (int c = 0; c < 16; ++c) wt.w1[k][c] = w1[c * 27 + k];   // OHWI [16][3][3][3] -> [k][co]
-  for (int i = 0; i < 9 * 16; ++i) wt.w2[i / 16][i % 16] = w2[i];
-  for (int c = 0; c < 16; ++c) {
-    wt.b1[c] = b1 ? b1[c] : 0.0f;
-    wt.b2[c] = b2 ? b2[c] : 0.0f;
-  }
-  if (in_type == LCE_T_FLOAT) return launch_stem2<float, false>(in, wt, out, s, stream);
-  if (in_type == LCE_T_INT8) return launch_stem2<int8_t, false>(in, wt, out, s, stream);
-  return launch_stem2<uint8_t, true>(in, wt, out, s, stream);
+  if (g1.Cout == 8) return stem2_run<8>(in_type, in, w1, b1, w2, b2, out, s, stream);
+  return stem2_run<16>(in_type, in, w1, b1, w2, b2, out, s, stream);
 }
 
 int lce_b200_f32_add(const float* a, const float* b, float* out, int64_t n, int64_t b_len,

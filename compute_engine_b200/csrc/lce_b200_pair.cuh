@@ -15,16 +15,26 @@
 //     x2 and, optionally, its packed signs.
 // The inner product is lce_b200_imma.cuh's b1 one (BMMA.168256.AND.POPC plus the popc(a) row),
 // on the same plan-time fragments (wt_nat), so the integers and then the floats are those of two
-// run_fused calls bit for bit. Warp task = 32 pixels x 64 channels, as in bconv_imma_kernel.
+// run_fused calls bit for bit. Warp task = 32 pixels x 64 channels, as in bconv_imma_kernel (32
+// pixels x 32 channels at C = 32).
 //
 // Tiles (8 warps, __launch_bounds__(256, 2): 128 registers, no spills with -Xptxas -v):
+//   C = 32 : 14 x 14 (region 16 x 16 = 8 warp tasks), 42 KB of shared memory
 //   C = 64 : 14 x 14 (region 16 x 16 = 8 warp tasks), 73 KB of shared memory
 //   C = 128:  7 x 14 (region  9 x 16, 10 warp tasks), 99 KB
+// At C = 32 (QuickNetSmall's 56 x 56 section) a tap is one word, so a 3 x 3 layer's K is 9 words:
+// taps 0-7 fill one k256 slice (thread tig holds taps 2 tig and 2 tig + 1, two separate words of
+// the packed tile) and tap 8 with three zero words is a k128 tail (thread 0 holds it). The plan's
+// fragments are those of a 64-channel tile whose channels 32-63 are zero; only the first two
+// 16-channel pairs are issued. Per 16 x 8 output fragment that is 2 BMMAs (one k256, one k128) for
+// 288 bits of K, against 3 (two k256, one k128) for the 576 bits of C = 64.
 // so two CTAs share an SM, and a 56 x 56 or 28 x 28 image splits into whole tiles. Larger C
 // would need smaller tiles (more ring recompute and x0 ring re-reads) or a cluster; those stages
 // stay on two run_fused calls. Measured on an H100 80GB HBM3 at a 400 W power limit, QuickNet
 // batch 256, per profiled step: the 56 x 56 x 64 stage's four blocks 0.695 ms as four nodes,
-// 0.449 ms as two pairs; the 28 x 28 x 128 stage's 0.393 ms, 0.300 ms.
+// 0.449 ms as two pairs; the 28 x 28 x 128 stage's 0.393 ms, 0.300 ms. At a 700 W power limit,
+// QuickNetSmall batch 256 (tools/quicknet_small_bench.py): the 56 x 56 x 32 stage's four blocks
+// 0.686 ms as four nodes (on the wgmma kernel), 0.217 ms as two pairs.
 #ifndef LCE_B200_PAIR_CUH_
 #define LCE_B200_PAIR_CUH_
 
@@ -49,11 +59,13 @@ struct PairParams {
 };
 
 template <int CW> struct PairShape {
-  static_assert(CW == 2 || CW == 4, "the pair kernel takes 64 or 128 channels");
+  static_assert(CW == 1 || CW == 2 || CW == 4, "the pair kernel takes 32, 64 or 128 channels");
   static constexpr int C = 32 * CW;
-  static constexpr int TH = CW == 2 ? 14 : 7, TW = 14;  // output tile
+  static constexpr int TH = CW == 4 ? 7 : 14, TW = 14;  // output tile
   static constexpr int RH = TH + 2, RW = TW + 2;        // layer 1's region: the tile plus a ring
-  static constexpr int NT = C / kBN;                    // 64-channel tiles
+  static constexpr int NW = C < kBN ? C : kBN;          // channels of a warp task
+  static constexpr int NS = NW / 8;                     // its 8-channel n sub-tiles
+  static constexpr int NT = C / NW;                     // warp tasks per pixel group
   static constexpr int Kw = 9 * CW;                     // K words of a 3x3 layer
   static constexpr int Kw4 = (Kw + 3) & ~3;             // padded to the k128 granularity
   static constexpr int n_full = Kw4 >> 3;               // 8-word slices
@@ -88,20 +100,30 @@ __device__ __forceinline__ void pair_conv_b1(const uint32_t* src, int ow, int n_
     }
 #pragma unroll 1
   for (int s = 0; s < S::n_full; ++s) {
-    // words 2 tig, 2 tig + 1 of the slice: one tap (CW is even), channels word cw, cw + 1
     const int kw = s * 8 + 2 * tig;
-    const int t = kw / CW;
-    const int off = ((t / 3) * sw + t % 3) * CW + kw % CW;
-    const bool live = kw < S::Kw;
     uint32_t a[2][4];
+    if constexpr (CW == 1) {
+      // words 2 tig, 2 tig + 1 of the slice: taps kw and kw + 1 (both < 8 < Kw)
+      const int off0 = (kw / 3) * sw + kw % 3, off1 = ((kw + 1) / 3) * sw + (kw + 1) % 3;
 #pragma unroll
-    for (int ms = 0; ms < 2; ++ms) {
-      const uint2 lo = live ? *reinterpret_cast<const uint2*>(src + base[ms][0] + off) : make_uint2(0, 0);
-      const uint2 hi = live ? *reinterpret_cast<const uint2*>(src + base[ms][1] + off) : make_uint2(0, 0);
-      a[ms][0] = lo.x; a[ms][1] = hi.x; a[ms][2] = lo.y; a[ms][3] = hi.y;
+      for (int ms = 0; ms < 2; ++ms) {
+        a[ms][0] = src[base[ms][0] + off0]; a[ms][1] = src[base[ms][1] + off0];
+        a[ms][2] = src[base[ms][0] + off1]; a[ms][3] = src[base[ms][1] + off1];
+      }
+    } else {
+      // words 2 tig, 2 tig + 1 of the slice: one tap (CW is even), channels word cw, cw + 1
+      const int t = kw / CW;
+      const int off = ((t / 3) * sw + t % 3) * CW + kw % CW;
+      const bool live = kw < S::Kw;
+#pragma unroll
+      for (int ms = 0; ms < 2; ++ms) {
+        const uint2 lo = live ? *reinterpret_cast<const uint2*>(src + base[ms][0] + off) : make_uint2(0, 0);
+        const uint2 hi = live ? *reinterpret_cast<const uint2*>(src + base[ms][1] + off) : make_uint2(0, 0);
+        a[ms][0] = lo.x; a[ms][1] = hi.x; a[ms][2] = lo.y; a[ms][3] = hi.y;
+      }
     }
 #pragma unroll
-    for (int np = 0; np < 4; ++np) {
+    for (int np = 0; np < S::NS / 2; ++np) {
       const uint4 b = b4[(s * 4 + np) * 32];
       bmma_k256(acc[0][2 * np], a[0], b.x, b.y);
       bmma_k256(acc[1][2 * np], a[1], b.x, b.y);
@@ -124,7 +146,7 @@ __device__ __forceinline__ void pair_conv_b1(const uint32_t* src, int ow, int n_
       hi[ms] = live ? src[base[ms][1] + off] : 0u;
     }
 #pragma unroll
-    for (int np = 0; np < 4; ++np) {
+    for (int np = 0; np < S::NS / 2; ++np) {
       const uint4 b = b4[(S::n_full * 4 + np) * 32];
 #pragma unroll
       for (int ms = 0; ms < 2; ++ms) {
@@ -138,7 +160,7 @@ __device__ __forceinline__ void pair_conv_b1(const uint32_t* src, int ow, int n_
 }
 
 // One warp task of a layer: the accumulators of output pixels [m0, m0 + 32) x channels
-// [c_tile, c_tile + 64), turned into popc(a ^ w) exactly as bconv_imma_kernel does.
+// [c_tile, c_tile + NW), turned into popc(a ^ w) exactly as bconv_imma_kernel does.
 // ch_s: the layer's [mul | bias | wpop] x C in shared memory.
 template <int CW>
 __device__ __forceinline__ void pair_task_acc(const float* ch_s, const uint32_t* src,
@@ -150,14 +172,14 @@ __device__ __forceinline__ void pair_task_acc(const float* ch_s, const uint32_t*
 #pragma unroll
   for (int ms = 0; ms < 2; ++ms)
 #pragma unroll
-    for (int ns = 0; ns < 8; ++ns)
+    for (int ns = 0; ns < S::NS; ++ns)
 #pragma unroll
       for (int e = 0; e < 4; ++e) acc[ms][ns][e] = 0;
   const uint4* b4 = reinterpret_cast<const uint4*>(wt_s) + nt * S::n_slices * 128 + lane;
   pair_conv_b1<CW>(src, ow, n_out, m0, b4, gid, tig, acc, pa);
-  const int c_tile = nt * kBN;
+  const int c_tile = nt * S::NW;
 #pragma unroll
-  for (int ns = 0; ns < 8; ++ns) {
+  for (int ns = 0; ns < S::NS; ++ns) {
     const int2 pw = *reinterpret_cast<const int2*>(ch_s + 2 * S::C + c_tile + ns * 8 + tig * 2);
 #pragma unroll
     for (int ms = 0; ms < 2; ++ms)
@@ -167,8 +189,8 @@ __device__ __forceinline__ void pair_task_acc(const float* ch_s, const uint32_t*
   }
 }
 
-// epilogue_imma's float path for one accumulator row: y = act(T(acc) + res)
-template <int C>
+// epilogue_imma's float path for one accumulator row: y = act(T(acc) + res), y[0, 2 NS)
+template <int C, int NS>
 __device__ __forceinline__ void pair_row(const PairParams& p, int L, const float* ch_s,
                                          const int (&acc)[2][8][4], int ms, int h,
                                          const float* res, int cth, float (&y)[16]) {
@@ -177,7 +199,7 @@ __device__ __forceinline__ void pair_row(const PairParams& p, int L, const float
   const float act_hi = ract == LCE_ACT_RELU ? __int_as_float(0x7f800000)
                                             : (ract == LCE_ACT_RELU6 ? 6.0f : 1.0f);
 #pragma unroll
-  for (int ns = 0; ns < 8; ++ns) {
+  for (int ns = 0; ns < NS; ++ns) {
     const float2 mu = *reinterpret_cast<const float2*>(ch_s + cth + ns * 8);
     const float2 bi = *reinterpret_cast<const float2*>(ch_s + C + cth + ns * 8);
     const float2 rv = *reinterpret_cast<const float2*>(res + ns * 8);
@@ -188,11 +210,13 @@ __device__ __forceinline__ void pair_row(const PairParams& p, int L, const float
   }
   if (ract != LCE_ACT_NONE) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], act_lo), act_hi);
+    for (int j = 0; j < 2 * NS; ++j) y[j] = fminf(fmaxf(y[j], act_lo), act_hi);
   }
 }
 
-// LceQuantize of the row's 16 values, gathered over the quad: words (c_tile >> 5) and + 1
+// LceQuantize of the row's 2 NS values, gathered over the quad: words (c_tile >> 5) and, at
+// NS = 8, + 1 (bits1 stays 0 at NS = 4)
+template <int NS>
 __device__ __forceinline__ void pair_signs(const float (&y)[16], bool ok, int tig, uint32_t& bits0,
                                            uint32_t& bits1) {
   bits0 = bits1 = 0;
@@ -200,15 +224,16 @@ __device__ __forceinline__ void pair_signs(const float (&y)[16], bool ok, int ti
 #pragma unroll
     for (int ns = 0; ns < 4; ++ns) {
       bits0 |= ((y[2 * ns] < 0.0f ? 1u : 0u) | (y[2 * ns + 1] < 0.0f ? 2u : 0u)) << (ns * 8);
-      bits1 |= ((y[2 * ns + 8] < 0.0f ? 1u : 0u) | (y[2 * ns + 9] < 0.0f ? 2u : 0u)) << (ns * 8);
+      if (NS == 8)
+        bits1 |= ((y[2 * ns + 8] < 0.0f ? 1u : 0u) | (y[2 * ns + 9] < 0.0f ? 2u : 0u)) << (ns * 8);
     }
     bits0 <<= tig * 2;
     bits1 <<= tig * 2;
   }
   bits0 |= __shfl_xor_sync(0xffffffffu, bits0, 1);
-  bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 1);
+  if (NS == 8) bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 1);
   bits0 |= __shfl_xor_sync(0xffffffffu, bits0, 2);
-  bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 2);
+  if (NS == 8) bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 2);
 }
 
 template <int CW>
@@ -276,7 +301,7 @@ __global__ void __launch_bounds__(kPThreads, 2) bconv_pair_kernel(const PairPara
     for (int task = warp; task < n_tasks; task += kPThreads / 32) {
       const int nt = task % S::NT, m0 = (task / S::NT) * 32;
       pair_task_acc<CW>(ch_s, x0p_s, wt_s, RW, n_out, m0, nt, lane, acc);
-      const int cth = nt * kBN + tig * 2;
+      const int cth = nt * S::NW + tig * 2;
 #pragma unroll
       for (int ms = 0; ms < 2; ++ms)
 #pragma unroll
@@ -290,20 +315,20 @@ __global__ void __launch_bounds__(kPThreads, 2) bconv_pair_kernel(const PairPara
           if (ok) {
             const float* res = p.residual +
                 ((static_cast<long long>(img) * p.H + gy) * p.W + gx) * S::C + cth;
-            pair_row<S::C>(p, 0, ch_s, acc, ms, h, res, cth, y);
+            pair_row<S::C, S::NS>(p, 0, ch_s, acc, ms, h, res, cth, y);
             if (ry >= 1 && ry <= TH && rx >= 1 && rx <= TW) {
               float* o = x1_s + ((ry - 1) * TW + (rx - 1)) * S::x1_stride + cth;
 #pragma unroll
-              for (int ns = 0; ns < 8; ++ns)
+              for (int ns = 0; ns < S::NS; ++ns)
                 *reinterpret_cast<float2*>(o + ns * 8) = make_float2(y[2 * ns], y[2 * ns + 1]);
             }
           }
           uint32_t bits0, bits1;
-          pair_signs(y, ok, tig, bits0, bits1);
+          pair_signs<S::NS>(y, ok, tig, bits0, bits1);
           if (r < n_out && tig == 0) {
-            uint32_t* w = s1_s + r * CW + (nt * kBN >> 5);
+            uint32_t* w = s1_s + r * CW + (nt * S::NW >> 5);
             w[0] = bits0;
-            w[1] = bits1;
+            if (S::NS == 8) w[1] = bits1;
           }
         }
     }
@@ -319,7 +344,7 @@ __global__ void __launch_bounds__(kPThreads, 2) bconv_pair_kernel(const PairPara
     for (int task = warp; task < n_tasks; task += kPThreads / 32) {
       const int nt = task % S::NT, m0 = (task / S::NT) * 32;
       pair_task_acc<CW>(ch2_s, s1_s, wt2_s, TW, n_out, m0, nt, lane, acc);
-      const int cth = nt * kBN + tig * 2;
+      const int cth = nt * S::NW + tig * 2;
 #pragma unroll
       for (int ms = 0; ms < 2; ++ms)
 #pragma unroll
@@ -331,19 +356,19 @@ __global__ void __launch_bounds__(kPThreads, 2) bconv_pair_kernel(const PairPara
           float y[16];
           const long long px = (static_cast<long long>(img) * p.H + gy) * p.W + gx;
           if (ok) {
-            pair_row<S::C>(p, 1, ch2_s, acc, ms, h, x1_s + i * S::x1_stride + cth, cth, y);
+            pair_row<S::C, S::NS>(p, 1, ch2_s, acc, ms, h, x1_s + i * S::x1_stride + cth, cth, y);
             float* o = p.out + px * S::C + cth;
 #pragma unroll
-            for (int ns = 0; ns < 8; ++ns)
+            for (int ns = 0; ns < S::NS; ++ns)
               *reinterpret_cast<float2*>(o + ns * 8) = make_float2(y[2 * ns], y[2 * ns + 1]);
           }
           if (p.packed_out != nullptr) {   // uniform across the CTA: every lane shuffles
             uint32_t bits0, bits1;
-            pair_signs(y, ok, tig, bits0, bits1);
+            pair_signs<S::NS>(y, ok, tig, bits0, bits1);
             if (ok && tig == 0) {
-              int32_t* pk = p.packed_out + px * CW + (nt * kBN >> 5);
+              int32_t* pk = p.packed_out + px * CW + (nt * S::NW >> 5);
               pk[0] = static_cast<int32_t>(bits0);
-              pk[1] = static_cast<int32_t>(bits1);
+              if (S::NS == 8) pk[1] = static_cast<int32_t>(bits1);
             }
           }
         }

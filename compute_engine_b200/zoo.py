@@ -5,9 +5,11 @@ random weights (seeded), correct topology.
 
 The topologies are NOT in /root/reference (they live in larq-zoo, absent offline);
 they are restated from the public QuickNet / Bi-Real Net descriptions:
-  QuickNet(-Large): stem [conv3x3 s2 -> BN/ReLU -> depthwise3x3 s2 -> conv1x1 -> BN],
-    sections of residual blocks [sign -> binary conv3x3 (one-padding, ReLU fused, BN
-    folded) -> + shortcut] with filters (64,128,256,512), blocks (4,4,4,4) / (6,8,12,6),
+  QuickNet(-Large, -Small): stem [conv3x3 s2 -> BN/ReLU -> depthwise3x3 s2 -> conv1x1 -> BN],
+    the first conv filters[0] // 4 wide, sections of residual blocks [sign -> binary conv3x3
+    (one-padding, ReLU fused, BN folded) -> + shortcut] with filters (64,128,256,512) and blocks
+    (4,4,4,4) / (6,8,12,6), or filters (32,64,256,512) and blocks (4,4,4,4) for QuickNetSmall
+    (larq-zoo's QuickNetSmallFactory),
     transitions [ReLU? no: maxpool2x2 s1 -> blur depthwise3x3 s2 -> conv1x1 -> BN],
     head [ReLU -> global average pool -> dense 1000 -> softmax].
   Bi-RealNet-18: conv7x7 s2 + BN + maxpool3x3 s2; 16 binary conv3x3 (zero padding,
@@ -227,6 +229,14 @@ def quicknet(batch=1, blocks=(4, 4, 4, 4), filters=(64, 128, 256, 512), seed=0, 
 
 def quicknet_large(batch=1, seed=0, image=224, input_type="float32"):
     return quicknet(batch, blocks=(6, 8, 12, 6), seed=seed, image=image, name="QuickNetLarge",
+                    input_type=input_type)
+
+
+def quicknet_small(batch=1, seed=0, image=224, input_type="float32"):
+    """QuickNetSmall, restated from larq-zoo (sota/quicknet.py, QuickNetSmallFactory): QuickNet
+    with section filters (32, 64, 256, 512) and four blocks per section, so the stem is CONV_2D
+    3x3/s2 3 -> 8 (filters[0] // 4) -> DEPTHWISE 3x3/s2 -> CONV_2D 1x1 8 -> 32. 16 LceBconv2d."""
+    return quicknet(batch, filters=(32, 64, 256, 512), seed=seed, image=image, name="QuickNetSmall",
                     input_type=input_type)
 
 
@@ -606,7 +616,8 @@ def xnornet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
     return g.m.serialize()
 
 
-MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "birealnet18": birealnet18,
+MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "quicknet_small": quicknet_small,
+          "birealnet18": birealnet18,
           "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet,
           "binarydensenet28": binarydensenet28, "binarydensenet37": binarydensenet37,
           "binarydensenet37_dilated": binarydensenet37_dilated,

@@ -128,8 +128,10 @@ int lce_b200_bconv2d_run_fused_chain(lce_b200_bconv2d* plan, const int32_t* in_d
  *   packed_out = bitpack(out) (optional, may be NULL).
  * Bit-identical to two run_fused calls, but x1 and its signs stay on chip. Both plans must be
  * ungrouped 3x3 / stride 1 / dilation 1 SAME layers with pad_values = 1, float output,
- * channels_in == channels_out == 64 or 128, on the b1 mma.sync kernel, and plan2 must take plan1's
- * output shape; anything else is refused with a message. out must not overlap residual. */
+ * channels_in == channels_out == 32, 64 or 128, on the b1 mma.sync kernel (32-channel plans get
+ * the pair kernel's fragments at creation and otherwise run on the wgmma kernel), and plan2 must
+ * take plan1's output shape; anything else is refused with a message. out must not overlap
+ * residual. */
 int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* plan2,
                                     const int32_t* in_dev, const float* residual_dev,
                                     int act1, int act2, float* out_dev,

@@ -62,13 +62,14 @@ int lce_b200_f32_avg_pool(const lce_f32_pool_desc* d, const float* in_dev, float
 int lce_b200_f32_maxpool2x2_depthwise3x3(const lce_f32_pool_desc* pool, const lce_f32_conv_desc* dw,
                                          const float* in_dev, const float* filter_dev,
                                          const float* bias_dev, float* out_dev, void* stream);
-/* Fused stem [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> 16) -> DEPTHWISE_CONV_2D(3x3, stride 2)
- * (QuickNet's stem): one pass over the image; the dequantised image and the first conv's map stay
+/* Fused stem [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> C1) -> DEPTHWISE_CONV_2D(3x3, stride 2),
+ * C1 = 16 (QuickNet, QuickNetLarge) or 8 (QuickNetSmall); other widths are refused. One pass over
+ * the image; the dequantised image and the first conv's map stay
  * in shared memory. in_type LCE_T_FLOAT: `in_dev` is the float image (scale / zero point unused);
  * LCE_T_INT8 / LCE_T_BOOL (= uint8): the quantised image, dequantised as float(scale * (q - zp))
  * like lce_b200_dequantize_affine. `dw` describes the depthwise conv on the first conv's output.
- * The filters and biases are HOST pointers (w1 OHWI [16][3][3][3], w2 [1][3][3][16]; biases may be
- * NULL): 2.4 KB that travel by value in the kernel's parameter bank, where every FMA reads its
+ * The filters and biases are HOST pointers (w1 OHWI [C1][3][3][3], w2 [1][3][3][C1]; biases may be
+ * NULL): 2.4 KB at C1 = 16 that travel by value in the kernel's parameter bank, where every FMA reads its
  * weight as a constant operand. Bit-identical to the separate kernels run one after the other. */
 int lce_b200_f32_stem_conv_dw(const lce_f32_conv_desc* conv1, const lce_f32_conv_desc* dw, int in_type,
                               const void* in_dev, double in_scale, int32_t in_zero_point,

@@ -27,7 +27,7 @@ def _bool(v):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--graph", default="")
-    ap.add_argument("--zoo", default="", help="quicknet | quicknet_large | birealnet18 | reactnet_a | realtobinarynet | "
+    ap.add_argument("--zoo", default="", help="quicknet | quicknet_large | quicknet_small | birealnet18 | reactnet_a | realtobinarynet | "
                     "binarydensenet28 | binarydensenet37 | binarydensenet37_dilated | binarydensenet45 | meliusnet22 | "
                     "binaryalexnet | xnornet")
     ap.add_argument("--num_runs", type=int, default=50)
