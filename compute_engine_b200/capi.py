@@ -90,6 +90,8 @@ EXPORTS = [
     "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add",
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_logistic",
     "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
+    "lce_b200_f32_maximum", "lce_b200_f32_minimum", "lce_b200_f32_div", "lce_b200_f32_round",
+    "lce_b200_f32_quant2_planes",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -270,6 +272,23 @@ def maxpool_affine_sign(x: torch.Tensor, filter_hw, stride_hw, padding=PADDING_V
                                                   stride_hw[1], padding, activation, _p(vecs[0]), _p(vecs[1]),
                                                   _p(pk), _stream()))
     return pk
+
+
+def quant2_planes(x: torch.Tensor, pool=None):
+    """DoReFaNet's 2-bit quantiser q = round(clip(x, 0, 1) * 3) of a float NHWC map, as int32 bit
+    planes [B, OH, OW, 3 * C / 32] = [bit 0 | bit 1 | bit 1] (C % 32 == 0). pool: None, or
+    (filter_hw, stride_hw, padding, activation) of a MAX_POOL_2D applied first."""
+    x = _dev(x, torch.float32)
+    b, h, w, c = x.shape
+    (fh, fw), (sh, sw), padding, activation = pool if pool is not None else ((0, 0), (1, 1), PADDING_VALID, ACT_NONE)
+    oh, ow = C.c_int(h), C.c_int(w)
+    if pool is not None:
+        d = PoolDesc(b, h, w, c, fh, fw, sh, sw, padding, activation)
+        _check(lib().lce_b200_f32_pool_out_shape(C.byref(d), C.byref(oh), C.byref(ow)))
+    planes = torch.empty((b, max(oh.value, 0), max(ow.value, 0), 3 * (c // 32)), dtype=torch.int32, device=x.device)
+    _check(lib().lce_b200_f32_quant2_planes(_p(x), b, h, w, c, fh, fw, sh, sw, padding, activation, _p(planes),
+                                            _stream()))
+    return planes
 
 
 class BConv2d:

@@ -378,21 +378,27 @@ int64_t PreluAlphaCount(const TfLiteTensor* x, const TfLiteTensor* a) {
 // ------------------------------ ADD / MUL / RELU ------------------------------ //
 // The kernels compute out[i] = a[i] (op) b[i % Count(b)], which is TFLite's broadcast for two shapes
 // of b only: a's own shape, and [C] (a's last dimension) with any leading 1s. A b of higher rank
-// would make the output's rank b's. MUL's one further broadcast: a [B,H,W,C] tensor by a per-image,
+// would make the output's rank b's. A b of one element (a scalar, or all dimensions 1) is read as
+// b[0] for every element. MUL's one further broadcast: a [B,H,W,C] tensor by a per-image,
 // per-channel [B,1,1,C] one (the channel gate of Real-to-Binary Net); runs as
 // lce_b200_f32_gate_sign with only the gate set.
 bool ImageChannelBroadcast(const TfLiteTensor* a, const TfLiteTensor* b) {
   return a->dims->size == 4 && b->dims->size == 4 && b->dims->data[0] == a->dims->data[0] &&
          b->dims->data[1] == 1 && b->dims->data[2] == 1 && b->dims->data[3] == a->dims->data[3];
 }
+// b is a's own shape, [C] with any leading 1s, or one element: what out[i] = a[i] op b[i % Count(b)]
+// computes as TFLite broadcasts it
+bool PlainBroadcast(const TfLiteTensor* a, const TfLiteTensor* b) {
+  const int64_t nb = PreluAlphaCount(a, b);
+  return a->dims->size > 0 && b->dims->size <= a->dims->size && nb > 0 &&
+         (nb == Count(a) || nb == a->dims->data[a->dims->size - 1] || nb == 1);
+}
 template <bool MUL>
 TfLiteStatus EltPrepare(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* a = T(c, n->inputs, 0);
   const TfLiteTensor* b = T(c, n->inputs, 1);
   B_ENSURE(c, a && b, "ADD/MUL: two inputs required");
-  const int64_t na = Count(a), nb = PreluAlphaCount(a, b);
-  const bool plain = a->dims->size > 0 && b->dims->size <= a->dims->size && nb > 0 &&
-                     (nb == na || nb == a->dims->data[a->dims->size - 1]);
+  const bool plain = PlainBroadcast(a, b);
   if (MUL)
     B_ENSURE(c, plain || (Count(b) > 0 && ImageChannelBroadcast(a, b)),
              "MUL: only same-shape, last-dimension or [B,H,W,C] x [B,1,1,C] broadcast is supported");
@@ -408,8 +414,8 @@ TfLiteStatus EltInvoke(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* b = T(c, n->inputs, 1);
   TfLiteTensor* out = T(c, n->outputs, 0);
   B_ENSURE(c, OnDevice(b->data.raw), "float builtins need device-resident operands");
-  const int64_t na = Count(a), nb = Count(b);
-  if (MUL && na != nb && nb != a->dims->data[a->dims->size - 1]) {   // [B,1,1,C] (EltPrepare)
+  const int64_t na = Count(a);
+  if (MUL && !PlainBroadcast(a, b)) {   // [B,1,1,C] (EltPrepare)
     const lce_gate_desc gate{b->data.f, nullptr, nullptr, nullptr};
     const int ch = a->dims->data[3];
     B_CAPI(c, lce_b200_f32_gate_sign(a->data.f, &gate, nullptr, P(n).activation, a->dims->data[0],
@@ -433,6 +439,82 @@ TfLiteStatus ReluInvoke(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* a = T(c, n->inputs, 0);
   B_CAPI(c, lce_b200_f32_activation(a->data.f, T(c, n->outputs, 0)->data.f, Count(a), LCE_ACT_RELU,
                                     lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// MAXIMUM (55), MINIMUM (57), DIV (42): float32, b of the shapes ADD takes
+template <int CODE>
+TfLiteStatus MinMaxDivPrepare(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* a = T(c, n->inputs, 0);
+  const TfLiteTensor* b = T(c, n->inputs, 1);
+  B_ENSURE(c, a && b && a->type == kTfLiteFloat32 && b->type == kTfLiteFloat32,
+           "MAXIMUM/MINIMUM/DIV: two float32 inputs required");
+  B_ENSURE(c, PlainBroadcast(a, b),
+           "MAXIMUM/MINIMUM/DIV: only same-shape, last-dimension or single-element broadcast is supported");
+  return SameShapePrepare(c, n);
+}
+template <int CODE>
+TfLiteStatus MinMaxDivInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* a = T(c, n->inputs, 0);
+  const TfLiteTensor* b = T(c, n->inputs, 1);
+  float* out = T(c, n->outputs, 0)->data.f;
+  B_ENSURE(c, OnDevice(b->data.raw), "float builtins need device-resident operands");
+  if (CODE == 55)
+    B_CAPI(c, lce_b200_f32_maximum(a->data.f, b->data.f, out, Count(a), Count(b), lce_b200_get_stream()));
+  else if (CODE == 57)
+    B_CAPI(c, lce_b200_f32_minimum(a->data.f, b->data.f, out, Count(a), Count(b), lce_b200_get_stream()));
+  else
+    B_CAPI(c, lce_b200_f32_div(a->data.f, b->data.f, out, Count(a), Count(b), P(n).activation,
+                               lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+TfLiteStatus RoundPrepare(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  B_ENSURE(c, x && x->type == kTfLiteFloat32, "ROUND: only float32 is supported");
+  return SameShapePrepare(c, n);
+}
+TfLiteStatus RoundInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  B_CAPI(c, lce_b200_f32_round(x->data.f, T(c, n->outputs, 0)->data.f, Count(x), lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// ------------- fused [MAX_POOL_2D ->] MAXIMUM(0) -> MINIMUM(1) -> MUL(3) -> ROUND [-> DIV(3)] ------------- //
+// Created by Graph::FuseQuantizedActivations; builtin_data = the pool's BuiltinParams, or with
+// filter_h == 0 no pool; input x [B,H,W,C] (without a pool also [rows, C], taken as [rows,1,1,C]),
+// C % 32 == 0; output the level's bit planes [B,OH,OW,3*C/32] (lce_b200_f32_quant2_planes).
+bool Quant2Desc(TfLiteContext* c, TfLiteNode* n, lce_f32_pool_desc* d) {
+  const TfLiteTensor* in = T(c, n->inputs, 0);
+  if (!in || in->type != kTfLiteFloat32 || in->dims->size < 1) return false;
+  const BuiltinParams& p = P(n);
+  if (p.filter_h != 0) return PoolDesc(c, n, d);
+  const int C = in->dims->data[in->dims->size - 1];
+  if (C <= 0) return false;
+  memset(d, 0, sizeof(*d));
+  d->channels = C;
+  if (in->dims->size == 4) {
+    d->batch = in->dims->data[0]; d->in_h = in->dims->data[1]; d->in_w = in->dims->data[2];
+  } else {
+    d->batch = static_cast<int>(Count(in) / C); d->in_h = d->in_w = 1;
+  }
+  return true;
+}
+TfLiteStatus Quant2Prepare(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_pool_desc d;
+  B_ENSURE(c, n->inputs->size == 1 && Quant2Desc(c, n, &d), "Quant2: a float32 input [..., C] expected");
+  B_ENSURE(c, d.channels % 32 == 0, "Quant2: the channel count must be a multiple of 32");
+  TfLiteTensor* pk = T(c, n->outputs, 0);
+  B_ENSURE(c, pk && pk->type == kTfLiteInt32, "Quant2: the planes output must be int32");
+  int oh = d.in_h, ow = d.in_w;
+  if (d.filter_h != 0) B_CAPI(c, lce_b200_f32_pool_out_shape(&d, &oh, &ow));
+  return Resize(c, pk, {d.batch, oh, ow, 3 * (d.channels / 32)});
+}
+TfLiteStatus Quant2Invoke(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_pool_desc d;
+  Quant2Desc(c, n, &d);
+  B_CAPI(c, lce_b200_f32_quant2_planes(T(c, n->inputs, 0)->data.f, d.batch, d.in_h, d.in_w, d.channels,
+                                       d.filter_h, d.filter_w, d.stride_h, d.stride_w, d.padding,
+                                       d.activation, T(c, n->outputs, 0)->data.i32, lce_b200_get_stream()));
   return kTfLiteOk;
 }
 
@@ -842,6 +924,10 @@ const TfLiteRegistration* ActivationChainRegistration() {
   static TfLiteRegistration r = {Init, Free, ChainPrepare, ChainInvoke};
   return &r;
 }
+const TfLiteRegistration* Quant2Registration() {
+  static TfLiteRegistration r = {Init, Free, Quant2Prepare, Quant2Invoke};
+  return &r;
+}
 const TfLiteRegistration* PooledSignRegistration() {
   static TfLiteRegistration r = {Init, Free, PooledSignPrepare, PooledSignInvoke};
   return &r;
@@ -882,6 +968,14 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(54, &prelu);   // PRELU
   static TfLiteRegistration logistic = {Init, Free, LogisticPrepare, LogisticInvoke};
   r->AddBuiltin(14, &logistic);  // LOGISTIC
+  static TfLiteRegistration maximum = {Init, Free, MinMaxDivPrepare<55>, MinMaxDivInvoke<55>};
+  static TfLiteRegistration minimum = {Init, Free, MinMaxDivPrepare<57>, MinMaxDivInvoke<57>};
+  static TfLiteRegistration div = {Init, Free, MinMaxDivPrepare<42>, MinMaxDivInvoke<42>};
+  static TfLiteRegistration round = {Init, Free, RoundPrepare, RoundInvoke};
+  r->AddBuiltin(55, &maximum);   // MAXIMUM
+  r->AddBuiltin(57, &minimum);   // MINIMUM
+  r->AddBuiltin(42, &div);       // DIV
+  r->AddBuiltin(116, &round);    // ROUND
   static TfLiteRegistration strided_slice = {Init, Free, StridedSlicePrepare, StridedSliceInvoke};
   r->AddBuiltin(45, &strided_slice);  // STRIDED_SLICE
   static TfLiteRegistration split = {Init, Free, SplitPrepare, SplitInvoke};

@@ -144,6 +144,9 @@ int lce_host_fuse_residual_blocks(void* g) { return static_cast<Graph*>(g)->Fuse
 int lce_host_fuse_float_glue(void* g) { return static_cast<Graph*>(g)->FuseFloatGlue(); }
 int lce_host_fuse_channel_gates(void* g) { return static_cast<Graph*>(g)->FuseChannelGates(); }
 int lce_host_fuse_pooled_signs(void* g) { return static_cast<Graph*>(g)->FusePooledSigns(); }
+int lce_host_fuse_quantized_activations(void* g) {
+  return static_cast<Graph*>(g)->FuseQuantizedActivations();
+}
 int lce_host_fuse_dense_blocks(void* g) { return static_cast<Graph*>(g)->FuseDenseBlocks(); }
 int lce_host_fuse_activation_chains(void* g) { return static_cast<Graph*>(g)->FuseActivationChains(); }
 int lce_host_fuse_residual_pairs(void* g) { return static_cast<Graph*>(g)->FuseResidualPairs(); }

@@ -2,6 +2,7 @@
 
 #include "builtin_params.h"
 #include "flexbuffer_map.h"
+#include "lce_b200.h"
 #include "lce_b200_types.h"
 
 #include <cuda_runtime.h>
@@ -904,6 +905,7 @@ const TfLiteRegistration* FusedPoolDepthwiseRegistration();  // builtin_ops.cc
 const TfLiteRegistration* FusedStemRegistration();
 const TfLiteRegistration* ActivationChainRegistration();
 const TfLiteRegistration* PooledSignRegistration();
+const TfLiteRegistration* Quant2Registration();
 
 int Graph::FuseActivationChains() {
   if (!device_arena_) return 0;
@@ -1122,6 +1124,234 @@ int Graph::FusePooledSigns() {
       nodes_.erase(nodes_.begin() + k);
       ++removed;
     }
+  }
+  allocated_ = false;
+  return removed;
+}
+
+int Graph::FuseQuantizedActivations() {
+  const size_t none = nodes_.size() + 1;
+  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
+  auto consumers = [&](int t) {
+    std::vector<size_t> c;
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
+    return c;
+  };
+  auto sole_consumer = [&](int t) {
+    if (is_output(t)) return none;
+    const std::vector<size_t> c = consumers(t);
+    return c.size() == 1 ? c[0] : none;
+  };
+  auto params = [&](const NodeRecord& n) {
+    return n.builtin_blob.size() >= sizeof(BuiltinParams)
+               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())
+               : nullptr;
+  };
+  // the host copy of a float constant, else nullptr (data.raw may be its device copy)
+  auto float_const = [&](int t) -> const float* {
+    if (t < 0 || tensors_[t].type != kTfLiteFloat32 || tensors_[t].allocation_type != kTfLiteMmapRo)
+      return nullptr;
+    return reinterpret_cast<const float*>(const_host_[t].data());
+  };
+  auto count = [&](int t) {
+    int64_t n = 1;
+    for (int d = 0; d < tensors_[t].dims->size; ++d) n *= tensors_[t].dims->data[d];
+    return n;
+  };
+  // node k (after node `after`) is the builtin `name` of x [and a one-element float constant equal to
+  // `value`], with no fused activation and a float output: returns that output, else -1
+  auto step = [&](size_t k, long long after, const char* name, int x, bool binary, float value) {
+    if (k >= nodes_.size() || static_cast<long long>(k) <= after) return -1;
+    const NodeRecord& n = *nodes_[k];
+    if (n.name != name || n.initialized || n.node.inputs->size != (binary ? 2 : 1) ||
+        n.node.outputs->size != 1 || n.node.inputs->data[0] != x || !params(n) || params(n)->activation != 0 ||
+        tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32)
+      return -1;
+    if (binary) {
+      const int v = n.node.inputs->data[1];
+      const float* c = float_const(v);
+      if (!c || count(v) != 1 || memcmp(c, &value, sizeof(float)) != 0) return -1;
+    }
+    return n.node.outputs->data[0];
+  };
+  // One consumer of the quantised tensor: CONV_2D or FULLY_CONNECTED with constant +-alpha weights.
+  struct Layer {
+    size_t node;
+    int N, kh, kw;
+    BuiltinParams p;
+    std::vector<int32_t> filter;
+    std::vector<float> mul, bias;
+  };
+  // fills `l` when node k qualifies (see host_graph.h)
+  auto layer = [&](size_t k, size_t after, int t, int C, Layer* l) {
+    if (k >= nodes_.size() || k <= after) return false;
+    const NodeRecord& n = *nodes_[k];
+    const bool fc = n.name == "builtin:9";
+    if ((!fc && n.name != "builtin:3") || n.initialized || !params(n) || params(n)->activation != 0 ||
+        n.node.inputs->size < 2 || n.node.inputs->size > 3 || n.node.outputs->size != 1 ||
+        n.node.inputs->data[0] != t || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32)
+      return false;
+    const int wt = n.node.inputs->data[1], bt = n.node.inputs->size > 2 ? n.node.inputs->data[2] : -1;
+    const float* w = float_const(wt);
+    const float* b = bt < 0 ? nullptr : float_const(bt);
+    if (!w || (bt >= 0 && !b)) return false;
+    const TfLiteIntArray* wd = tensors_[wt].dims;
+    if (wd->size != (fc ? 2 : 4) || wd->data[wd->size - 1] != C) return false;
+    // a FULLY_CONNECTED output becomes [rows,1,1,N]: the same bytes, but not the shape a caller reads
+    if (fc && is_output(n.node.outputs->data[0])) return false;
+    l->node = k;
+    l->N = wd->data[0];
+    l->kh = fc ? 1 : wd->data[1];
+    l->kw = fc ? 1 : wd->data[2];
+    l->p = *params(n);
+    if (fc) {
+      l->p.padding = LCE_PADDING_VALID;
+      l->p.stride_h = l->p.stride_w = l->p.dilation_h = l->p.dilation_w = 1;
+    }
+    const int64_t taps = static_cast<int64_t>(l->kh) * l->kw, K = taps * C;
+    if (l->N < 1 || taps < 1 || 3 * K >= (1 << 24) || (b && count(bt) != l->N)) return false;
+    lce_bconv2d_desc d{};
+    d.batch = d.in_h = d.in_w = 1;
+    d.channels_in = 3 * C; d.channels_out = l->N; d.groups = 1;
+    d.filter_h = l->kh; d.filter_w = l->kw;
+    d.stride_h = l->p.stride_h; d.stride_w = l->p.stride_w;
+    d.dilation_h = l->p.dilation_h; d.dilation_w = l->p.dilation_w;
+    d.padding = l->p.padding; d.pad_value = 1; d.out_type = LCE_OUT_FLOAT;
+    int oh, ow, ph, pw;
+    if (lce_b200_bconv2d_out_shape(&d, &oh, &ow, &ph, &pw) != 0) return false;
+    const int cw = C / 32;
+    l->filter.assign(static_cast<size_t>(l->N) * taps * 3 * cw, 0);
+    l->mul.resize(l->N);
+    l->bias.resize(l->N);
+    for (int o = 0; o < l->N; ++o) {
+      const float* wo = w + static_cast<int64_t>(o) * K;
+      uint32_t mag;
+      memcpy(&mag, wo, 4);
+      mag &= 0x7fffffffu;
+      if (mag == 0 || mag >= 0x7f800000u) return false;
+      int64_t sum = 0;   // W_o: the sum of the filter's signs
+      for (int64_t tap = 0; tap < taps; ++tap)
+        for (int c = 0; c < C; ++c) {
+          uint32_t bits;
+          memcpy(&bits, wo + tap * C + c, 4);
+          if ((bits & 0x7fffffffu) != mag) return false;
+          const bool neg = bits >> 31;
+          sum += neg ? -1 : 1;
+          if (neg)
+            for (int plane = 0; plane < 3; ++plane)
+              l->filter[((static_cast<size_t>(o) * taps + tap) * 3 + plane) * cw + c / 32] |=
+                  static_cast<int32_t>(1u << (c % 32));
+        }
+      float alpha_f;
+      memcpy(&alpha_f, &mag, 4);
+      const double alpha = alpha_f;
+      l->mul[o] = static_cast<float>(-alpha / 6.0);
+      l->bias[o] = static_cast<float>(alpha * static_cast<double>(sum) / 2.0 + (b ? static_cast<double>(b[o]) : 0.0));
+    }
+    return true;
+  };
+  auto free_arrays = [&](NodeRecord& n) {
+    LceB200IntArrayFree(n.node.inputs);
+    LceB200IntArrayFree(n.node.outputs);
+    LceB200IntArrayFree(n.node.temporaries);
+    LceB200IntArrayFree(n.node.intermediates);
+  };
+
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    if (nodes_[i]->name != "builtin:55" || nodes_[i]->node.inputs->size != 2) continue;
+    const int x = nodes_[i]->node.inputs->data[0];
+    if (x < 0 || tensors_[x].type != kTfLiteFloat32 || !tensors_[x].dims || tensors_[x].dims->size < 1) continue;
+    const int C = tensors_[x].dims->data[tensors_[x].dims->size - 1];
+    if (C <= 0 || C % 32 != 0) continue;
+    const int t1 = step(i, -1, "builtin:55", x, true, 0.0f);
+    if (t1 < 0) continue;
+    const size_t kmin = sole_consumer(t1);
+    const int t2 = step(kmin, i, "builtin:57", t1, true, 1.0f);
+    if (t2 < 0) continue;
+    const size_t kmul = sole_consumer(t2);
+    const int t3 = step(kmul, kmin, "builtin:18", t2, true, 3.0f);
+    if (t3 < 0) continue;
+    const size_t kround = sole_consumer(t3);
+    const int t4 = step(kround, kmul, "builtin:116", t3, false, 0.0f);
+    if (t4 < 0) continue;
+    const size_t kdiv = sole_consumer(t4);
+    const int t5 = step(kdiv, kround, "builtin:42", t4, true, 3.0f);
+    if (t5 < 0 || is_output(t5)) continue;
+    const std::vector<size_t> users = consumers(t5);
+    if (users.empty()) continue;
+    std::vector<Layer> layers(users.size());
+    bool ok = true;
+    for (size_t u = 0; u < users.size() && ok; ++u) ok = layer(users[u], kdiv, t5, C, &layers[u]);
+    if (!ok) continue;
+    // the optional pool in front: x is read by the quantiser only
+    size_t head = i;
+    int src = x;
+    if (!is_output(x) && consumers(x).size() == 1 && tensors_[x].dims->size == 4)
+      for (size_t k = 0; k < i; ++k) {
+        const NodeRecord& p = *nodes_[k];
+        if (p.name == "builtin:17" && !p.initialized && params(p) && p.node.inputs->size == 1 &&
+            p.node.outputs->size == 1 && p.node.outputs->data[0] == x &&
+            tensors_[p.node.inputs->data[0]].type == kTfLiteFloat32) {
+          head = k;
+          src = p.node.inputs->data[0];
+        }
+      }
+    const std::vector<int> xdims(tensors_[x].dims->data, tensors_[x].dims->data + tensors_[x].dims->size);
+    std::vector<int> pdims = xdims.size() == 4 ? xdims : std::vector<int>{static_cast<int>(count(x) / C), 1, 1, C};
+    pdims[3] = 3 * (C / 32);
+    const int planes = AddTensor(kTfLiteInt32, pdims, nullptr, 0, false, 0.0f, 0, names_[t5] + "_planes");
+    NodeRecord& h = *nodes_[head];
+    if (head == i) {   // no pool: filter_h == 0 tells the node so
+      BuiltinParams bp;
+      memset(&bp, 0, sizeof(bp));
+      h.builtin_blob.assign(reinterpret_cast<const uint8_t*>(&bp), reinterpret_cast<const uint8_t*>(&bp) + sizeof(bp));
+      h.node.builtin_data = h.builtin_blob.data();
+    }
+    LceB200IntArrayFree(h.node.inputs);
+    LceB200IntArrayFree(h.node.outputs);
+    h.node.inputs = MakeDims({src});
+    h.node.outputs = MakeDims({planes});
+    h.registration = Quant2Registration();
+    h.name = head == i ? "Quant2" : "MAX_POOL_2D+Quant2";
+    for (const Layer& l : layers) {
+      const int f = AddTensor(kTfLiteInt32, {l.N, l.kh, l.kw, 3 * (C / 32)}, l.filter.data(),
+                              l.filter.size() * sizeof(int32_t), false, 0.0f, 0, names_[t5] + "_bfilter");
+      const int m = AddTensor(kTfLiteFloat32, {l.N}, l.mul.data(), l.mul.size() * sizeof(float), false, 0.0f, 0,
+                              names_[t5] + "_pmul");
+      const int b = AddTensor(kTfLiteFloat32, {l.N}, l.bias.data(), l.bias.size() * sizeof(float), false, 0.0f, 0,
+                              names_[t5] + "_pbias");
+      NodeRecord& n = *nodes_[l.node];
+      const int out = n.node.outputs->data[0];
+      LceB200IntArrayFree(n.node.inputs);
+      LceB200IntArrayFree(n.node.outputs);
+      n.node.inputs = MakeDims({planes, f, m, b, -1});
+      n.node.outputs = MakeDims({out});
+      n.custom_options = WriteFlexIntMap({{"channels_in", 3 * C},
+                                          {"dilation_height_factor", l.p.dilation_h},
+                                          {"dilation_width_factor", l.p.dilation_w},
+                                          {"fused_activation_function", 0},
+                                          {"pad_values", 1},
+                                          {"padding", l.p.padding},
+                                          {"stride_height", l.p.stride_h},
+                                          {"stride_width", l.p.stride_w}});
+      n.builtin_blob.clear();
+      n.node.builtin_data = nullptr;
+      n.node.custom_initial_data = n.custom_options.data();
+      n.node.custom_initial_data_size = static_cast<int>(n.custom_options.size());
+      n.registration = lce_b200_Register_BCONV_2D();
+      n.name = "LceBconv2d";
+    }
+    std::vector<size_t> gone{kdiv, kround, kmul, kmin};   // the highest index first
+    if (head != i) gone.push_back(i);
+    for (size_t k : gone) {
+      free_arrays(*nodes_[k]);
+      nodes_.erase(nodes_.begin() + k);
+      ++removed;
+    }
+    i = head;
   }
   allocated_ = false;
   return removed;

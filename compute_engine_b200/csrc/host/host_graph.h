@@ -109,6 +109,33 @@ class Graph {
   // Bit-identical. Returns the number of nodes removed (3 per pooled layer).
   int FusePooledSigns();
 
+  // DoReFaNet's 2-bit activations: the quantiser a = round(clip(x, 0, 1) * 3) / 3 in front of a float
+  // convolution or dense layer whose weights are +-alpha_o,
+  //   [MAX_POOL_2D ->] MAXIMUM(0) -> MINIMUM(1) -> MUL(3) -> ROUND -> DIV(3) -> CONV_2D | FULLY_CONNECTED
+  // becomes two nodes: "[MAX_POOL_2D+]Quant2" (lce_b200_f32_quant2_planes), which writes the level
+  // q = 3 a as the int32 bit planes [plane 0 | plane 1 | plane 1], [B,H,W,3*C/32], and a plain
+  // "LceBconv2d" over channels_in = 3 * C with pad_values 1 and the layer's stride, padding and
+  // dilation, whose constants the pass synthesises: the filter's sign words (bit set = negative
+  // weight) repeated three times per tap, post_mul[o] = fl(-alpha_o / 6) and post_bias[o] =
+  // fl(alpha_o * W_o / 2 + bias_o), W_o the sum of filter o's signs, both computed in double. With
+  // t = 1 - 2 bit the convolution's accumulator is D = sum s * (3 - 2 q), a padded tap counting as
+  // q = 0, so y = alpha/3 * sum s * q + bias = -alpha/6 * D + alpha * W / 2 + bias: CONV_2D's zero
+  // padding is one-padding here. FULLY_CONNECTED [rows,K] -> [rows,N] is the 1x1 VALID case; its output
+  // tensor becomes [rows,1,1,N], the same bytes. Only when the four constants have one element and
+  // are exactly 0, 1, 3 and 3; MUL and DIV have no fused activation; every layer that reads the
+  // quantised tensor qualifies (several may): float constant weights whose magnitude is bitwise
+  // one non-zero finite value per output channel, a float constant bias or none, no fused
+  // activation (LCE clamps before the multiplier, TFLite after the bias), C % 32 == 0,
+  // 3 * k * k * C < 2^24 (so float(D) is exact), parameters lce_b200_bconv2d_out_shape accepts, and for
+  // FULLY_CONNECTED an output that is not a graph output; every intermediate has one consumer and
+  // none is a graph output. The pool is absorbed when only the quantiser reads it. Otherwise the
+  // graph is left as it is. The levels are the unfused ops' bit for bit and D is an exact integer,
+  // so y is the real-valued result rounded twice; TFLite's float CONV_2D rounds after each of its
+  // K = k * k * C terms, so the two differ by up to about K * 2^-24 * sum |a| |w|: NOT bit-identical
+  // to the float ops, and a difference can flip a level of the next quantiser at a near-tie. Returns
+  // the number of nodes removed (4, or 5 with the pool, per quantiser).
+  int FuseQuantizedActivations();
+
   // BinaryDenseNet's dense layers
   //   x_j [B,H,W,C_j] -> MUL(scale) -> ADD(shift) -> LceQuantize -> LceBconv2d (float y_j)
   //   x_{j+1} = CONCATENATION([x_j, y_j], last axis)

@@ -289,7 +289,8 @@ bool BuildGraphFromTflite(const uint8_t* data, size_t size, const OpResolver& re
         bp.beta = o.scalar<float>(0, 1.0f);
         break;
       case 0:
-      case 18:  // ADD / MUL (schema.fbs:939,945)
+      case 18:
+      case 42:  // ADD / MUL / DIV (schema.fbs:939,945; DivOptions)
         bp.activation = o.scalar<int8_t>(0, 0);
         break;
       case 2:  // CONCATENATION (schema.fbs:934)

@@ -960,7 +960,25 @@ __global__ void __launch_bounds__(256) pool_kernel(const float* __restrict__ in,
   }
 }
 
-template <int OP>  // 0 add, 1 mul, 2 activation only
+// TFLite's MAXIMUM and MINIMUM (reference/maximum_minimum.h): a comparison and a select, so a NaN in
+// `a` gives b, and max(-0, +0) is the second operand
+__device__ __forceinline__ float tfl_maximum(float a, float b) { return a > b ? a : b; }
+__device__ __forceinline__ float tfl_minimum(float a, float b) { return a < b ? a : b; }
+
+// OP 0 add, 1 mul, 2 activation only, 3 MAXIMUM, 4 MINIMUM, 5 DIV (IEEE division), 6 ROUND (halves
+// to even, reference/round.h; b unused, no activation)
+template <int OP>
+__device__ __forceinline__ float eltwise_op(float x, float y) {
+  if (OP == 0) return x + y;
+  if (OP == 1) return x * y;
+  if (OP == 3) return tfl_maximum(x, y);
+  if (OP == 4) return tfl_minimum(x, y);
+  if (OP == 5) return __fdiv_rn(x, y);
+  if (OP == 6) return rintf(x);
+  return x;
+}
+
+template <int OP>
 __global__ void __launch_bounds__(256) eltwise_kernel(const float* __restrict__ a,
                                                       const float* __restrict__ b,
                                                       float* __restrict__ out, long long n,
@@ -974,20 +992,23 @@ __global__ void __launch_bounds__(256) eltwise_kernel(const float* __restrict__ 
     for (long long i = t0; i < (n >> 2); i += stride) {
       float4 x = a4[i];
       if (OP != 2) {
-        const float4 y = b4[i];
-        if (OP == 0) { x.x += y.x; x.y += y.y; x.z += y.z; x.w += y.w; }
-        else { x.x *= y.x; x.y *= y.y; x.z *= y.z; x.w *= y.w; }
+        const float4 y = OP == 6 ? x : b4[i];
+        x = make_float4(eltwise_op<OP>(x.x, y.x), eltwise_op<OP>(x.y, y.y), eltwise_op<OP>(x.z, y.z),
+                        eltwise_op<OP>(x.w, y.w));
       }
       o4[i] = make_float4(apply_act(x.x, act), apply_act(x.y, act), apply_act(x.z, act),
                           apply_act(x.w, act));
     }
     return;
   }
+  if (OP != 2 && OP != 6 && b_len == 1) {   // a single-element b: one read, no index arithmetic
+    const float y = __ldg(b);
+    for (long long i = t0; i < n; i += stride) out[i] = apply_act(eltwise_op<OP>(a[i], y), act);
+    return;
+  }
   for (long long i = t0; i < n; i += stride) {
-    float x = a[i];
-    if (OP == 0) x += b[i % b_len];
-    if (OP == 1) x *= b[i % b_len];
-    out[i] = apply_act(x, act);
+    const float x = a[i];
+    out[i] = apply_act(OP == 2 || OP == 6 ? eltwise_op<OP>(x, x) : eltwise_op<OP>(x, b[i % b_len]), act);
   }
 }
 
@@ -1090,6 +1111,26 @@ __global__ void __launch_bounds__(256) affine_sign_kernel(const float* __restric
 // coalesced 128-byte read, and the ballot of the lanes' signs is the packed word (lanes past C vote
 // 0). The window is visited in pool_kernel's order (rows, then columns, in-bounds taps only) from
 // -FLT_MAX with fmaxf, then the pool's activation; FHW > 0 fixes a square window so the taps unroll.
+// The max of channel `img[0]`'s in-bounds taps of the fh x fw window at (y0, x0) of an H x W x C map,
+// visited in pool_kernel's order from -FLT_MAX with fmaxf.
+template <typename I>
+__device__ __forceinline__ float window_max(const float* __restrict__ img, int y0, int x0, int fh, int fw,
+                                            int H, int W, int C) {
+  float v = -FLT_MAX;
+#pragma unroll
+  for (int fy = 0; fy < fh; ++fy) {
+    const int y = y0 + fy;
+    if (static_cast<unsigned>(y) >= static_cast<unsigned>(H)) continue;
+#pragma unroll
+    for (int fx = 0; fx < fw; ++fx) {
+      const int xx = x0 + fx;
+      if (static_cast<unsigned>(xx) >= static_cast<unsigned>(W)) continue;
+      v = fmaxf(v, __ldg(img + (static_cast<I>(y) * W + xx) * C));
+    }
+  }
+  return v;
+}
+
 template <int FHW, typename I>
 __global__ void __launch_bounds__(256) maxpool_affine_sign_kernel(
     const float* __restrict__ x, int H, int W, int C, int OH, int OW, int cw, int fh_, int fw_, int sh,
@@ -1109,24 +1150,47 @@ __global__ void __launch_bounds__(256) maxpool_affine_sign_kernel(
     bool bit = false;
     if (c < C) {
       const int y0 = oy * sh - ph, x0 = ox * sw - pw;
-      const float* img = x + b * H * W * C + c;
-      float v = -FLT_MAX;
-#pragma unroll
-      for (int fy = 0; fy < fh; ++fy) {
-        const int y = y0 + fy;
-        if (static_cast<unsigned>(y) >= static_cast<unsigned>(H)) continue;
-#pragma unroll
-        for (int fx = 0; fx < fw; ++fx) {
-          const int xx = x0 + fx;
-          if (static_cast<unsigned>(xx) >= static_cast<unsigned>(W)) continue;
-          v = fmaxf(v, __ldg(img + (static_cast<I>(y) * W + xx) * C));
-        }
-      }
+      const float v = window_max<I>(x + b * H * W * C + c, y0, x0, fh, fw, H, W, C);
       bit = lce::affine_sign(apply_act(v, act), has_sc, has_sc ? __ldg(scale + c) : 0.0f, has_sh,
                              has_sh ? __ldg(shift + c) : 0.0f);
     }
     const unsigned word = __ballot_sync(0xffffffffu, bit);
     if (lane == 0) packed[wi] = static_cast<int32_t>(word);
+  }
+}
+
+// lce_b200_f32_quant2_planes: [MAX_POOL_2D ->] the 2-bit DoReFa quantiser in one pass, threads laid
+// out as in maxpool_affine_sign_kernel (C % 32 == 0, so every lane owns a channel). The level
+// q = rint(min(max(v, 0), 1) * 3) in {0, 1, 2, 3} is computed with the float operations of the MAXIMUM
+// -> MINIMUM -> MUL -> ROUND builtins; the ballots of its two bits are the word of plane 0 and of
+// plane 1, and a pixel's 3 * cw output words are [plane 0 | plane 1 | plane 1], so a binary
+// convolution over 3 * C channels with each tap's filter words repeated three times accumulates
+// plane 0 + 2 * plane 1. FHW == 1 is the quantiser alone (no window, no pool activation).
+template <int FHW, typename I>
+__global__ void __launch_bounds__(256) quant2_planes_kernel(
+    const float* __restrict__ x, int H, int W, int C, int OH, int OW, int cw, int fh_, int fw_, int sh,
+    int sw, int ph, int pw, int act, int32_t* __restrict__ planes, I words) {
+  const int fh = FHW ? FHW : fh_, fw = FHW ? FHW : fw_;
+  const int lane = threadIdx.x & 31;
+  const I warps = static_cast<I>(gridDim.x) * (blockDim.x >> 5);
+  for (I wi = static_cast<I>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); wi < words; wi += warps) {
+    const I pix = wi / cw;
+    const int word = static_cast<int>(wi - pix * cw);
+    float v;
+    if (FHW == 1) {
+      v = __ldg(x + pix * C + word * 32 + lane);
+    } else {
+      const int ox = static_cast<int>(pix % OW);
+      const I r = pix / OW;
+      const int oy = static_cast<int>(r % OH);
+      const I b = r / OH;
+      v = apply_act(window_max<I>(x + b * H * W * C + word * 32 + lane, oy * sh - ph, ox * sw - pw, fh, fw,
+                                  H, W, C), act);
+    }
+    const int q = static_cast<int>(rintf(__fmul_rn(tfl_minimum(tfl_maximum(v, 0.0f), 1.0f), 3.0f)));
+    const unsigned p0 = __ballot_sync(0xffffffffu, q & 1);
+    const unsigned p1 = __ballot_sync(0xffffffffu, q & 2);
+    if (lane < 3) planes[pix * (3 * cw) + lane * cw + word] = static_cast<int32_t>(lane == 0 ? p0 : p1);
   }
 }
 
@@ -1764,6 +1828,19 @@ static int conv2d_impl(const lce_f32_conv_desc* d, const float* in, const float*
       const char* e = getenv("LCE_B200_IGEMM_8X4");
       return e && e[0] == '1';
     }();
+    // with the kernels' static tiles, the offset table of a K above about 3000 (DoReFaNet's 3x3x384
+    // layers as float convolutions) passes the 48 KB a launch gets without opting in
+    {
+      static bool attr[64] = {};   // the attribute is per device
+      int dev = 0;
+      cudaGetDevice(&dev);
+      if (dev < 0 || dev >= 64 || !attr[dev]) {
+        const int most = kIKMax * 2 * static_cast<int>(sizeof(int));
+        cudaFuncSetAttribute(conv_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+        cudaFuncSetAttribute(conv_igemm8x8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+        if (dev >= 0 && dev < 64) attr[dev] = true;
+      }
+    }
     if (use8x4) {
       conv_igemm_kernel<<<igrid, 256, ksmem, as_stream(stream)>>>(in, filter, bias, out, g, M);
       return launch_check("conv_igemm_kernel");
@@ -1955,6 +2032,37 @@ int lce_b200_f32_activation(const float* in, float* out, int64_t n, int act, voi
   return launch_check("eltwise_kernel<act>");
 }
 
+int lce_b200_f32_maximum(const float* a, const float* b, float* out, int64_t n, int64_t b_len,
+                         void* stream) {
+  if (n <= 0) return 0;
+  if (b_len <= 0 || n % b_len) return fail("maximum: operand shapes do not broadcast");
+  eltwise_kernel<3><<<grid_for(n / 4 + 1, 256), 256, 0, as_stream(stream)>>>(
+      a, b, out, n, b_len, LCE_ACT_NONE, vec4_ok(a, b, out, n, b_len));
+  return launch_check("eltwise_kernel<maximum>");
+}
+int lce_b200_f32_minimum(const float* a, const float* b, float* out, int64_t n, int64_t b_len,
+                         void* stream) {
+  if (n <= 0) return 0;
+  if (b_len <= 0 || n % b_len) return fail("minimum: operand shapes do not broadcast");
+  eltwise_kernel<4><<<grid_for(n / 4 + 1, 256), 256, 0, as_stream(stream)>>>(
+      a, b, out, n, b_len, LCE_ACT_NONE, vec4_ok(a, b, out, n, b_len));
+  return launch_check("eltwise_kernel<minimum>");
+}
+int lce_b200_f32_div(const float* a, const float* b, float* out, int64_t n, int64_t b_len, int act,
+                     void* stream) {
+  if (n <= 0) return 0;
+  if (b_len <= 0 || n % b_len) return fail("div: operand shapes do not broadcast");
+  eltwise_kernel<5><<<grid_for(n / 4 + 1, 256), 256, 0, as_stream(stream)>>>(
+      a, b, out, n, b_len, act, vec4_ok(a, b, out, n, b_len));
+  return launch_check("eltwise_kernel<div>");
+}
+int lce_b200_f32_round(const float* in, float* out, int64_t n, void* stream) {
+  if (n <= 0) return 0;
+  eltwise_kernel<6><<<grid_for(n / 4 + 1, 256), 256, 0, as_stream(stream)>>>(
+      in, in, out, n, n, LCE_ACT_NONE, vec4_ok(in, in, out, n, n));
+  return launch_check("eltwise_kernel<round>");
+}
+
 int lce_b200_f32_chain_sign(const float* x, const lce_chain_desc* chain, int64_t rows, int channels,
                             float* out, int32_t* packed, void* stream) {
   if (rows < 0 || channels <= 0) return fail("chain_sign: bad shape (%lld rows, %d channels)",
@@ -2076,6 +2184,47 @@ int lce_b200_f32_maxpool_affine_sign(const float* x, int batch, int in_h, int in
   }
 #undef LCE_MAXPOOL_SIGN
   return launch_check("maxpool_affine_sign_kernel");
+}
+
+int lce_b200_f32_quant2_planes(const float* x, int batch, int in_h, int in_w, int channels, int filter_h,
+                               int filter_w, int stride_h, int stride_w, int padding, int activation,
+                               int32_t* planes, void* stream) {
+  if (batch < 0 || in_h <= 0 || in_w <= 0 || channels <= 0)
+    return fail("quant2_planes: bad shape (%d x %d x %d x %d)", batch, in_h, in_w, channels);
+  if (channels % 32) return fail("quant2_planes: channels (%d) must be a multiple of 32", channels);
+  if (planes == nullptr) return fail("quant2_planes: the planes output is required");
+  const bool pooled = filter_h != 0 || filter_w != 0;
+  int oh = in_h, ow = in_w, ph = 0, pw = 0;
+  if (pooled) {
+    if (padding != LCE_PADDING_SAME && padding != LCE_PADDING_VALID)
+      return fail("quant2_planes: unknown padding %d", padding);
+    const lce_f32_pool_desc d{batch, in_h, in_w, channels, filter_h, filter_w, stride_h, stride_w, padding,
+                              activation};
+    if (lce_b200_f32_pool_out_shape(&d, &oh, &ow)) return 1;
+    ph = pad_before(stride_h, 1, in_h, filter_h, oh);
+    pw = pad_before(stride_w, 1, in_w, filter_w, ow);
+  }
+  if (batch == 0 || oh <= 0 || ow <= 0) return 0;
+  const int cw = channels / 32;
+  const long long words = static_cast<long long>(batch) * oh * ow * cw;
+  const int grid = grid_for(words * 32, 256);
+  cudaStream_t s = as_stream(stream);
+  const int f = !pooled ? 1 : filter_h == 3 && filter_w == 3 ? 3 : 0;
+  // 32-bit index arithmetic where the input, the output and the word count fit
+  const bool narrow = static_cast<long long>(batch) * in_h * in_w * channels < (1LL << 31) &&
+                      3 * words + 8LL * grid < (1LL << 31);
+#define LCE_QUANT2(F, I)                                                                                  \
+  quant2_planes_kernel<F, I><<<grid, 256, 0, s>>>(x, in_h, in_w, channels, oh, ow, cw, filter_h, filter_w, \
+                                                  stride_h, stride_w, ph, pw, activation, planes,         \
+                                                  static_cast<I>(words))
+  if (narrow) {
+    if (f == 1) LCE_QUANT2(1, int); else if (f == 3) LCE_QUANT2(3, int); else LCE_QUANT2(0, int);
+  } else {
+    if (f == 1) LCE_QUANT2(1, long long); else if (f == 3) LCE_QUANT2(3, long long);
+    else LCE_QUANT2(0, long long);
+  }
+#undef LCE_QUANT2
+  return launch_check("quant2_planes_kernel");
 }
 
 int lce_b200_f32_logistic(const float* in, float* out, int64_t n, void* stream) {

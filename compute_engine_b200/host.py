@@ -206,6 +206,14 @@ class HostGraph:
         fuse_channel_gates, fuse_activation_chains and allocate_tensors."""
         return lib().lce_host_fuse_pooled_signs(self._g)
 
+    def fuse_quantized_activations(self):
+        """[MAX_POOL_2D ->] MAXIMUM(0) -> MINIMUM(1) -> MUL(3) -> ROUND -> DIV(3) -> CONV_2D or
+        FULLY_CONNECTED with +-alpha weights (DoReFaNet's 2-bit activations) => a node that writes the
+        level's bit planes and a plain LceBconv2d over three planes. Exact integer arithmetic, so not
+        bit-identical to the float convolution it replaces (Graph::FuseQuantizedActivations states
+        the bound). Call before allocate_tensors."""
+        return lib().lce_host_fuse_quantized_activations(self._g)
+
     def fuse_activation_chains(self):
         """ADD -> PRELU -> ADD [-> ADD -> LceQuantize] (ReActNet's RPReLU / RSign, each step
         optional) => the epilogue of the preceding fused LceBconv2d+ADD node, or one node.
@@ -219,7 +227,7 @@ class HostGraph:
 
     def fuse_all(self):
         return (self.fuse_dense_blocks() + self.fuse_residual_blocks() + self.fuse_float_glue()
-                + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
+                + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
                 + self.fuse_residual_pairs())
 
     # ---- profiling / async IO (bench.py) ----

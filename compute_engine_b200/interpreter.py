@@ -42,7 +42,12 @@ class Interpreter:
         (the optimised kernels' rules and their float zero-padding correction).
         batch_size: mini-batch used by predict (default: all). fuse: apply the graph-level fusions
         (residual-block tail into LceBconv2d's epilogue, max-pool + blur-pool); the outputs are
-        bit-identical either way. devices: CUDA device indices to shard mini-batches over
+        bit-identical either way, with one exception: a 2-bit-activation layer (DoReFaNet's quantiser
+        in front of a float CONV_2D or FULLY_CONNECTED with +-alpha weights) runs fused as an exact
+        integer binary convolution over bit planes, whose result is the real value rounded twice,
+        where the float layer rounds after each of its K terms; the two differ by up to about
+        K * 2^-24 * sum |a| |w| per output, which can flip a level of the next quantiser at a near-tie
+        (HostGraph.fuse_quantized_activations). devices: CUDA device indices to shard mini-batches over
         (default: the current device only)."""
         if use_reference_bconv and use_indirect_bgemm:
             import warnings

@@ -111,11 +111,12 @@ TENSOR_TYPE = {np.dtype(np.float32): 0, np.dtype(np.int32): 2, np.dtype(np.uint8
 OP = {"ADD": 0, "AVERAGE_POOL_2D": 1, "CONV_2D": 3, "DEPTHWISE_CONV_2D": 4,
       "FULLY_CONNECTED": 9, "MAX_POOL_2D": 17, "MUL": 18, "RELU": 19, "RESHAPE": 22,
       "SOFTMAX": 25, "MEAN": 40, "CUSTOM": 32, "CONCATENATION": 2, "PAD": 34, "PADV2": 60,
-      "DEQUANTIZE": 6, "PRELU": 54, "LOGISTIC": 14, "STRIDED_SLICE": 45, "SPLIT": 49}
+      "DEQUANTIZE": 6, "PRELU": 54, "LOGISTIC": 14, "STRIDED_SLICE": 45, "SPLIT": 49,
+      "DIV": 42, "MAXIMUM": 55, "MINIMUM": 57, "ROUND": 116}
 # BuiltinOptions union tags (schema_generated.h:1652-1694)
 OPT_TAG = {"CONV_2D": 1, "DEPTHWISE_CONV_2D": 2, "AVERAGE_POOL_2D": 5, "MAX_POOL_2D": 5,
            "FULLY_CONNECTED": 8, "SOFTMAX": 9, "ADD": 11, "MUL": 21, "RESHAPE": 17, "MEAN": 27,
-           "CONCATENATION": 10, "PAD": 22, "PADV2": 43, "STRIDED_SLICE": 32, "SPLIT": 35}
+           "CONCATENATION": 10, "PAD": 22, "PADV2": 43, "STRIDED_SLICE": 32, "SPLIT": 35, "DIV": 29}
 PADDING = {"SAME": 0, "VALID": 1}
 ACT = {"NONE": 0, "RELU": 1, "RELU_N1_TO_1": 2, "RELU6": 3}
 
@@ -162,7 +163,7 @@ class TFLiteModel:
             return fb.table({0: ("b", act)})
         if kind == "SOFTMAX":
             return fb.table({0: ("f", float(o.get("beta", 1.0)))})
-        if kind in ("ADD", "MUL"):
+        if kind in ("ADD", "MUL", "DIV"):
             return fb.table({0: ("b", act)})
         if kind == "RESHAPE":
             return fb.table({0: ("o", fb.scalar_vector("i", o["new_shape"]))})

@@ -616,10 +616,89 @@ def xnornet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
     return g.m.serialize()
 
 
+def dorefanet(batch=1, seed=0, image=224, input_type="float32"):
+    """DoReFaNet (Zhou et al., 2016: 1-bit weights, 2-bit activations), restated from larq-zoo's
+    DoReFaNet with synthetic weights; larq-zoo's source is not available offline, so the topology is
+    restated from its public description. In the converter's op order (shapes at 224):
+      stem CONV_2D 12x12/s4 VALID 3 -> 96 (BN folded into weights and bias, no activation) ->
+      [B,54,54,96];
+      quantised block Q(C_out, k, pool): the 2-bit activation quantiser round(clip(x, 0, 1) * 3) / 3 as
+      MAXIMUM(x, 0) -> MINIMUM(., 1) -> MUL(., 3) -> ROUND -> DIV(., 3) with one-element constants, then
+      CONV_2D k x k SAME stride 1 with no fused activation, whose weights are +-alpha_o: the
+      magnitude-aware sign's per-channel scale times the folded BatchNorm scale, one float32 value
+      per output channel, so |w| is bitwise constant within a channel and the converter cannot emit
+      an LceBconv2d (the input is not binary); the bias is the folded BatchNorm shift; then, if
+      `pool`, MAX_POOL_2D 3x3/s2;
+      Q(256, 5, SAME pool) -> 27x27, Q(384, 3, SAME pool) -> 14x14, Q(384, 3), Q(256, 3, VALID pool)
+      -> [B,6,6,256];
+      RESHAPE [-1, 9216] -> quantiser -> FULLY_CONNECTED 9216 -> 4096 (+-alpha_o, bias) -> quantiser
+      -> FULLY_CONNECTED 4096 -> 4096 (+-alpha_o, bias) -> MAXIMUM(0) -> MINIMUM(1) (a clip, not a
+      quantiser) -> FULLY_CONNECTED 4096 -> 1000 with float weights -> SOFTMAX.
+    6 quantisers, 5 CONV_2D, 3 FULLY_CONNECTED, 3 MAX_POOL_2D."""
+    g = _Builder(seed, batch, "DoReFaNet")
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+
+    def scalar_op(kind, t, ts, value):
+        y = g.act(ts)
+        g.m.add_op(kind, [t, g.const(np.array(value, np.float32), name="q")], [y])
+        return y
+
+    def clip(t, ts):
+        return scalar_op("MINIMUM", scalar_op("MAXIMUM", t, ts, 0.0), ts, 1.0)
+
+    def quantiser(t, ts):
+        t = scalar_op("MUL", clip(t, ts), ts, 3.0)
+        r = g.act(ts)
+        g.m.add_op("ROUND", [t], [r])
+        return scalar_op("DIV", r, ts, 3.0)
+
+    def binary_weights(shape):
+        """+-alpha_o of `shape` [C_out, ...], and the bias: pre-activations spread around [0, 1]."""
+        fan_in = int(np.prod(shape[1:]))
+        s, t = g.bn(shape[0])
+        alpha = (g.rng.uniform(0.5, 1.5, shape[0]).astype(np.float32) * s / np.float32(np.sqrt(fan_in)))
+        sign = (g.rng.integers(0, 2, shape, dtype=np.int8) * 2 - 1).astype(np.float32)
+        return sign * alpha.reshape((-1,) + (1,) * (len(shape) - 1)), t + np.float32(0.5)
+
+    def qconv(t, ts, cout, k, pool):
+        b, h, w, cin = ts
+        wt, bias = binary_weights((cout, k, k, cin))
+        y = g.act((b, h, w, cout))
+        g.m.add_op("CONV_2D", [quantiser(t, ts), g.const(wt), g.const(bias, name="b")], [y], padding="SAME",
+                   stride=(1, 1), activation="NONE")
+        ys = (b, h, w, cout)
+        return g.pool("MAX_POOL_2D", y, ys, 3, 2, pool) if pool else (y, ys)
+
+    def qdense(t, cin, cout):
+        wt, bias = binary_weights((cout, cin))
+        y = g.act((batch, cout))
+        g.m.add_op("FULLY_CONNECTED", [quantiser(t, (batch, cin)), g.const(wt), g.const(bias, name="b")], [y])
+        return y
+
+    x, xs = g.conv(x, xs, 96, 12, 4, padding="VALID")
+    x, xs = qconv(x, xs, 256, 5, "SAME")
+    x, xs = qconv(x, xs, 384, 3, "SAME")
+    x, xs = qconv(x, xs, 384, 3, None)
+    x, xs = qconv(x, xs, 256, 3, "VALID")
+    flat_c = xs[1] * xs[2] * xs[3]
+    flat = g.act((batch, flat_c))
+    g.m.add_op("RESHAPE", [x], [flat], new_shape=[-1, flat_c])
+    x = qdense(qdense(flat, flat_c, 4096), 4096, 4096)
+    x = clip(x, (batch, 4096))
+    wt = g.rng.standard_normal((1000, 4096)).astype(np.float32) / np.float32(np.sqrt(4096))
+    logits = g.act((batch, 1000))
+    g.m.add_op("FULLY_CONNECTED", [x, g.const(wt), g.const(np.zeros(1000, np.float32), name="b")], [logits])
+    probs = g.act((batch, 1000))
+    g.m.add_op("SOFTMAX", [logits], [probs], beta=1.0)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
 MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "quicknet_small": quicknet_small,
           "birealnet18": birealnet18,
           "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet,
           "binarydensenet28": binarydensenet28, "binarydensenet37": binarydensenet37,
           "binarydensenet37_dilated": binarydensenet37_dilated,
           "binarydensenet45": binarydensenet45, "meliusnet22": meliusnet22,
-          "binaryalexnet": binaryalexnet, "xnornet": xnornet}
+          "binaryalexnet": binaryalexnet, "xnornet": xnornet, "dorefanet": dorefanet}

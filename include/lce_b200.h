@@ -215,6 +215,32 @@ int lce_b200_f32_maxpool_affine_sign(const float* x_dev, int batch, int in_h, in
                                      int filter_h, int filter_w, int stride_h, int stride_w,
                                      int padding, int activation, const float* scale,
                                      const float* shift, int32_t* packed_out_dev, void* stream);
+/* MAXIMUM / MINIMUM (TF/lite/kernels/internal/reference/maximum_minimum.h: a > b ? a : b and
+ * a < b ? a : b), DIV (reference/div.h: one IEEE division, then the fused activation) and ROUND
+ * (reference/round.h: halves to even), on device pointers: out[i] = a[i] (op) b[i % b_len], with b_len == n (same
+ * shape), the last dimension, or 1. Bit-identical to numpy float32. */
+int lce_b200_f32_maximum(const float* a_dev, const float* b_dev, float* out_dev, int64_t n,
+                         int64_t b_len, void* stream);
+int lce_b200_f32_minimum(const float* a_dev, const float* b_dev, float* out_dev, int64_t n,
+                         int64_t b_len, void* stream);
+int lce_b200_f32_div(const float* a_dev, const float* b_dev, float* out_dev, int64_t n, int64_t b_len,
+                     int activation, void* stream);
+int lce_b200_f32_round(const float* in_dev, float* out_dev, int64_t n, void* stream);
+/* DoReFaNet's 2-bit activation quantiser, [MAX_POOL_2D ->] MAXIMUM(0) -> MINIMUM(1) -> MUL(3) ->
+ * ROUND [-> DIV(3)], in one pass over a float NHWC map [batch, in_h, in_w, channels], written as the
+ * bit planes of the level q = rint(min(max(v, 0), 1) * 3) in {0, 1, 2, 3}:
+ *   planes_out[b][oy][ox][3 * channels/32] = [bit 0 of q | bit 1 of q | bit 1 of q],
+ * each part channels/32 words packed as LceQuantize packs signs (bit c % 32 of word c / 32). A binary
+ * convolution with channels_in = 3 * channels, one-padding and each tap's filter words repeated
+ * three times then accumulates D = sum s * (3 - 2 q) over real taps (and sum 3 s over padded ones),
+ * so sum s * q / 3 = (3 W - D) / 6 with W the sum of a filter's signs. v is x, or with filter_h and
+ * filter_w not 0 the max over the in-bounds pool window taken as the MAX_POOL_2D builtin takes it
+ * (from -FLT_MAX with fmaxf, then `activation`); with both 0 the pool arguments are ignored and
+ * the output has the input's size. q uses the float operations of the MAXIMUM, MINIMUM, MUL and
+ * ROUND builtins, so the levels are theirs bit for bit. channels must be a multiple of 32. */
+int lce_b200_f32_quant2_planes(const float* x_dev, int batch, int in_h, int in_w, int channels,
+                               int filter_h, int filter_w, int stride_h, int stride_w, int padding,
+                               int activation, int32_t* planes_out_dev, void* stream);
 int lce_b200_bconv2d_run_host(lce_b200_bconv2d* plan, const int32_t* in_host,
                               void* out_host);
 void lce_b200_bconv2d_destroy(lce_b200_bconv2d* plan);

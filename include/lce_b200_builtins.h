@@ -75,7 +75,7 @@ int lce_b200_f32_stem_conv_dw(const lce_f32_conv_desc* conv1, const lce_f32_conv
                               const void* in_dev, double in_scale, int32_t in_zero_point,
                               const float* w1_host, const float* b1_host, const float* w2_host,
                               const float* b2_host, float* out_dev, void* stream);
-/* out[i] = act(a[i] (op) b[i % b_len]); b_len == n (same shape) or the last dim. */
+/* out[i] = act(a[i] (op) b[i % b_len]); b_len == n (same shape), the last dim, or 1. */
 int lce_b200_f32_add(const float* a_dev, const float* b_dev, float* out_dev, int64_t n,
                      int64_t b_len, int activation, void* stream);
 int lce_b200_f32_mul(const float* a_dev, const float* b_dev, float* out_dev, int64_t n,

@@ -29,7 +29,7 @@ def main():
     ap.add_argument("--graph", default="")
     ap.add_argument("--zoo", default="", help="quicknet | quicknet_large | quicknet_small | birealnet18 | reactnet_a | realtobinarynet | "
                     "binarydensenet28 | binarydensenet37 | binarydensenet37_dilated | binarydensenet45 | meliusnet22 | "
-                    "binaryalexnet | xnornet")
+                    "binaryalexnet | xnornet | dorefanet")
     ap.add_argument("--num_runs", type=int, default=50)
     ap.add_argument("--warmup_runs", type=int, default=5)
     ap.add_argument("--num_threads", type=int, default=1)
