@@ -91,7 +91,7 @@ EXPORTS = [
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_logistic",
     "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
     "lce_b200_f32_maximum", "lce_b200_f32_minimum", "lce_b200_f32_div", "lce_b200_f32_round",
-    "lce_b200_f32_quant2_planes",
+    "lce_b200_f32_quant2_planes", "lce_b200_f32_grouped_conv2d",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -289,6 +289,38 @@ def quant2_planes(x: torch.Tensor, pool=None):
     _check(lib().lce_b200_f32_quant2_planes(_p(x), b, h, w, c, fh, fw, sh, sw, padding, activation, _p(planes),
                                             _stream()))
     return planes
+
+
+class ConvDesc(C.Structure):
+    """``lce_f32_conv_desc`` (include/lce_b200_builtins.h)."""
+    _fields_ = [(n, C.c_int32) for n in (
+        "batch", "in_h", "in_w", "in_c", "filter_h", "filter_w", "out_c", "stride_h", "stride_w",
+        "dilation_h", "dilation_w", "padding", "activation")]
+
+
+def grouped_conv2d(x: torch.Tensor, filt: torch.Tensor, bias=None, stride=(1, 1), dilation=(1, 1),
+                   padding=PADDING_SAME, activation=ACT_NONE, scale=None, shift=None,
+                   post_activation=ACT_NONE, out: torch.Tensor | None = None):
+    """Grouped CONV_2D of a float NHWC map x [B, H, W, C_in] with an OHWI filter [C_out, kh, kw,
+    C_in / groups] (groups = C_in / filter_in, as TFLite infers it), then the optional BatchNorm
+    epilogue fl(fl(act(y) * scale) + shift) and post_activation. bias / scale / shift: [C_out]
+    float32 CUDA tensors or None. `out` may be given (a view at any 4-byte offset)."""
+    x = _dev(x, torch.float32)
+    filt = _dev(filt, torch.float32)
+    b, h, w, cin = x.shape
+    cout, kh, kw, fin = filt.shape
+    if fin < 1 or cin % fin:
+        raise LceError(f"grouped_conv2d: the filter's {fin} input channels do not divide {cin}")
+    vecs = [None if v is None else _dev(v, torch.float32) for v in (bias, scale, shift)]
+    d = ConvDesc(b, h, w, cin, kh, kw, cout, stride[0], stride[1], dilation[0], dilation[1], padding, activation)
+    oh, ow = C.c_int(), C.c_int()
+    _check(lib().lce_b200_f32_conv_out_shape(C.byref(d), C.byref(oh), C.byref(ow)))
+    if out is None:
+        out = torch.empty((b, oh.value, ow.value, cout), dtype=torch.float32, device=x.device)
+    _check(lib().lce_b200_f32_grouped_conv2d(C.byref(d), C.c_int(cin // fin), _p(x), _p(filt), _p(vecs[0]),
+                                             _p(vecs[1]), _p(vecs[2]), C.c_int(post_activation), _p(out),
+                                             _stream()))
+    return out
 
 
 class BConv2d:

@@ -65,10 +65,13 @@ void Free(TfLiteContext*, void* p) { delete static_cast<BuiltinParams*>(p); }
 const BuiltinParams& P(TfLiteNode* n) { return *static_cast<BuiltinParams*>(n->user_data); }
 
 // ---------------------------- CONV_2D / DEPTHWISE ---------------------------- //
-bool ConvDesc(TfLiteContext* c, TfLiteNode* n, bool depthwise, lce_f32_conv_desc* d) {
+// groups (CONV_2D only): TFLite's conv.cc infers groups = in_c / filter_in from a filter
+// [out_c, fh, fw, filter_in]; ConvGroupChecks tells whether that division and out_c / groups are exact.
+bool ConvDesc(TfLiteContext* c, TfLiteNode* n, bool depthwise, lce_f32_conv_desc* d, int* groups = nullptr) {
   const TfLiteTensor* in = T(c, n->inputs, 0);
   const TfLiteTensor* f = T(c, n->inputs, 1);
   if (!in || !f || in->dims->size != 4 || f->dims->size != 4) return false;
+  if (groups) *groups = 1;
   const BuiltinParams& p = P(n);
   d->batch = in->dims->data[0];
   d->in_h = in->dims->data[1];
@@ -83,19 +86,34 @@ bool ConvDesc(TfLiteContext* c, TfLiteNode* n, bool depthwise, lce_f32_conv_desc
   d->dilation_w = p.dilation_w;
   d->padding = p.padding;
   d->activation = p.activation;
-  if (!depthwise && f->dims->data[3] != d->in_c) return false;
+  if (!depthwise && f->dims->data[3] != d->in_c) {
+    if (!groups || f->dims->data[3] < 1) return false;
+    *groups = d->in_c / f->dims->data[3];
+  }
   return true;
+}
+TfLiteStatus ConvGroupChecks(TfLiteContext* c, TfLiteNode* n, const lce_f32_conv_desc& d) {
+  const int filter_in = T(c, n->inputs, 1)->dims->data[3];
+  if (filter_in == d.in_c) return kTfLiteOk;
+  B_ENSURE(c, d.in_c % filter_in == 0,
+           "CONV_2D: the input's channels must be a multiple of the filter's input channels");
+  B_ENSURE(c, d.out_c % (d.in_c / filter_in) == 0,
+           "CONV_2D: the filter count must be a multiple of the group count");
+  return kTfLiteOk;
 }
 template <bool DW>
 TfLiteStatus ConvPrepare(TfLiteContext* c, TfLiteNode* n) {
   lce_f32_conv_desc d;
-  B_ENSURE(c, ConvDesc(c, n, DW, &d), "CONV_2D: bad input / filter shapes");
+  int groups = 1;
+  B_ENSURE(c, ConvDesc(c, n, DW, &d, DW ? nullptr : &groups), "CONV_2D: bad input / filter shapes");
   B_ENSURE(c, T(c, n->inputs, 0)->type == kTfLiteFloat32, "CONV_2D: only float32 is supported");
   if (DW) B_ENSURE(c, P(n).depth_multiplier == 1 && d.out_c == d.in_c,
                    "DEPTHWISE_CONV_2D: depth_multiplier must be 1");
+  if (!DW && ConvGroupChecks(c, n, d) != kTfLiteOk) return kTfLiteError;
   int oh, ow;
   B_CAPI(c, lce_b200_f32_conv_out_shape(&d, &oh, &ow));
   if (!DW && n->outputs->size == 2) {
+    B_ENSURE(c, groups == 1, "CONV_2D+LceQuantize: grouped convolutions are not supported");
     // fused LceQuantize (Graph::FuseFloatGlue): second output = bitpacked signs of the first
     TfLiteTensor* pk = T(c, n->outputs, 1);
     B_ENSURE(c, pk && pk->type == kTfLiteInt32, "CONV_2D+LceQuantize: packed output must be int32");
@@ -106,14 +124,18 @@ TfLiteStatus ConvPrepare(TfLiteContext* c, TfLiteNode* n) {
 template <bool DW>
 TfLiteStatus ConvInvoke(TfLiteContext* c, TfLiteNode* n) {
   lce_f32_conv_desc d;
-  ConvDesc(c, n, DW, &d);
+  int groups = 1;
+  ConvDesc(c, n, DW, &d, DW ? nullptr : &groups);
   const TfLiteTensor* in = T(c, n->inputs, 0);
   const TfLiteTensor* f = T(c, n->inputs, 1);
   const TfLiteTensor* bias = T(c, n->inputs, 2);
   TfLiteTensor* out = T(c, n->outputs, 0);
   B_ENSURE(c, OnDevice(in->data.raw) && OnDevice(f->data.raw) && OnDevice(out->data.raw),
            "float builtins need a device arena (no CPU path)");
-  if (DW)
+  if (groups != 1)
+    B_CAPI(c, lce_b200_f32_grouped_conv2d(&d, groups, in->data.f, f->data.f, bias ? bias->data.f : nullptr,
+                                          nullptr, nullptr, LCE_ACT_NONE, out->data.f, lce_b200_get_stream()));
+  else if (DW)
     B_CAPI(c, lce_b200_f32_depthwise_conv2d(&d, in->data.f, f->data.f, bias ? bias->data.f : nullptr,
                                              out->data.f, lce_b200_get_stream()));
   else if (n->outputs->size == 2)
@@ -123,6 +145,54 @@ TfLiteStatus ConvInvoke(TfLiteContext* c, TfLiteNode* n) {
   else
     B_CAPI(c, lce_b200_f32_conv2d(&d, in->data.f, f->data.f, bias ? bias->data.f : nullptr,
                                   out->data.f, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// -------------- fused grouped CONV_2D -> MUL(scale) -> ADD(shift): a BatchNorm after the conv -------------- //
+// Created by Graph::FuseGroupedConvAffine; builtin_data = { BuiltinParams conv, BuiltinParams add };
+// inputs [x, filter, bias (-1 when absent), scale, shift], scale and shift constants of out_c floats.
+// Runs lce_b200_f32_grouped_conv2d with the epilogue, the ADD's activation as the post activation.
+struct ConvAffineParams {
+  BuiltinParams conv, add;
+};
+void* ConvAffineInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* p = new ConvAffineParams();
+  memset(p, 0, sizeof(*p));
+  if (buffer && length >= sizeof(ConvAffineParams)) memcpy(p, buffer, sizeof(ConvAffineParams));
+  return p;
+}
+void ConvAffineFree(TfLiteContext*, void* p) { delete static_cast<ConvAffineParams*>(p); }
+TfLiteStatus ConvAffinePrepare(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_conv_desc d;
+  int groups = 1;
+  B_ENSURE(c, n->inputs->size == 5 && n->outputs->size == 1 && ConvDesc(c, n, false, &d, &groups),
+           "CONV_2D+MUL+ADD: bad input / filter shapes");
+  B_ENSURE(c, T(c, n->inputs, 0)->type == kTfLiteFloat32, "CONV_2D: only float32 is supported");
+  if (ConvGroupChecks(c, n, d) != kTfLiteOk) return kTfLiteError;
+  for (int k = 3; k < 5; ++k) {
+    const TfLiteTensor* v = T(c, n->inputs, k);
+    B_ENSURE(c, v && v->type == kTfLiteFloat32 && Count(v) == d.out_c,
+             "CONV_2D+MUL+ADD: scale and shift must be float32 with one value per output channel");
+  }
+  int oh, ow;
+  B_CAPI(c, lce_b200_f32_conv_out_shape(&d, &oh, &ow));
+  return Resize(c, T(c, n->outputs, 0), {d.batch, oh, ow, d.out_c});
+}
+TfLiteStatus ConvAffineInvoke(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_conv_desc d;
+  int groups = 1;
+  ConvDesc(c, n, false, &d, &groups);
+  const TfLiteTensor* bias = T(c, n->inputs, 2);
+  const TfLiteTensor* scale = T(c, n->inputs, 3);
+  const TfLiteTensor* shift = T(c, n->inputs, 4);
+  TfLiteTensor* out = T(c, n->outputs, 0);
+  B_ENSURE(c, OnDevice(T(c, n->inputs, 0)->data.raw) && OnDevice(out->data.raw) && OnDevice(scale->data.raw) &&
+                  OnDevice(shift->data.raw),
+           "float builtins need a device arena (no CPU path)");
+  B_CAPI(c, lce_b200_f32_grouped_conv2d(&d, groups, T(c, n->inputs, 0)->data.f, T(c, n->inputs, 1)->data.f,
+                                        bias ? bias->data.f : nullptr, scale->data.f, shift->data.f,
+                                        static_cast<const ConvAffineParams*>(n->user_data)->add.activation,
+                                        out->data.f, lce_b200_get_stream()));
   return kTfLiteOk;
 }
 
@@ -930,6 +1000,10 @@ const TfLiteRegistration* Quant2Registration() {
 }
 const TfLiteRegistration* PooledSignRegistration() {
   static TfLiteRegistration r = {Init, Free, PooledSignPrepare, PooledSignInvoke};
+  return &r;
+}
+const TfLiteRegistration* GroupedConvAffineRegistration() {
+  static TfLiteRegistration r = {ConvAffineInit, ConvAffineFree, ConvAffinePrepare, ConvAffineInvoke};
   return &r;
 }
 

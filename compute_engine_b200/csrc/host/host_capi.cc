@@ -147,6 +147,7 @@ int lce_host_fuse_pooled_signs(void* g) { return static_cast<Graph*>(g)->FusePoo
 int lce_host_fuse_quantized_activations(void* g) {
   return static_cast<Graph*>(g)->FuseQuantizedActivations();
 }
+int lce_host_fuse_grouped_conv_affine(void* g) { return static_cast<Graph*>(g)->FuseGroupedConvAffine(); }
 int lce_host_fuse_dense_blocks(void* g) { return static_cast<Graph*>(g)->FuseDenseBlocks(); }
 int lce_host_fuse_activation_chains(void* g) { return static_cast<Graph*>(g)->FuseActivationChains(); }
 int lce_host_fuse_residual_pairs(void* g) { return static_cast<Graph*>(g)->FuseResidualPairs(); }

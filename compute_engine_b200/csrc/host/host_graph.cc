@@ -906,6 +906,7 @@ const TfLiteRegistration* FusedStemRegistration();
 const TfLiteRegistration* ActivationChainRegistration();
 const TfLiteRegistration* PooledSignRegistration();
 const TfLiteRegistration* Quant2Registration();
+const TfLiteRegistration* GroupedConvAffineRegistration();
 
 int Graph::FuseActivationChains() {
   if (!device_arena_) return 0;
@@ -1357,6 +1358,88 @@ int Graph::FuseQuantizedActivations() {
   return removed;
 }
 
+int Graph::FuseGroupedConvAffine() {
+  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
+  // the node that alone reads t (as its first input), when t is not a graph output; else nodes_.size()
+  auto sole_consumer = [&](int t) {
+    if (is_output(t)) return nodes_.size();
+    size_t found = nodes_.size();
+    int n = 0;
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+        if (nodes_[k]->node.inputs->data[q] == t) { ++n; found = k; }
+    return (n == 1 && nodes_[found]->node.inputs->data[0] == t) ? found : nodes_.size();
+  };
+  auto params = [&](const NodeRecord& n) {
+    return n.builtin_blob.size() >= sizeof(BuiltinParams)
+               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())
+               : nullptr;
+  };
+  // node k (after `after`) is the builtin `name` of x and a float constant of C values, shape [C] or
+  // [1, ..., 1, C], with a float output: returns that output, else -1
+  auto const_op = [&](size_t k, size_t after, const char* name, int x, int C) {
+    if (k >= nodes_.size() || k <= after) return -1;
+    const NodeRecord& n = *nodes_[k];
+    if (n.name != name || n.initialized || !params(n) || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
+        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32)
+      return -1;
+    const int v = n.node.inputs->data[1];
+    if (v < 0) return -1;
+    const TfLiteTensor& t = tensors_[v];
+    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
+        t.dims->data[t.dims->size - 1] != C)
+      return -1;
+    for (int d = 0; d + 1 < t.dims->size; ++d)
+      if (t.dims->data[d] != 1) return -1;
+    return n.node.outputs->data[0];
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    NodeRecord& conv = *nodes_[i];
+    if (conv.name != "builtin:3" || conv.initialized || !params(conv) || params(conv)->activation != 0 ||
+        conv.node.inputs->size < 2 || conv.node.inputs->size > 3 || conv.node.outputs->size != 1)
+      continue;
+    const int x = conv.node.inputs->data[0], w = conv.node.inputs->data[1];
+    const int y = conv.node.outputs->data[0];
+    if (x < 0 || w < 0 || tensors_[x].dims->size != 4 || tensors_[w].dims->size != 4 ||
+        tensors_[x].type != kTfLiteFloat32 || tensors_[y].type != kTfLiteFloat32)
+      continue;
+    // grouped only: TFLite's groups = C_in / filter_in, exact, and dividing C_out
+    const int cin = tensors_[x].dims->data[3], fin = tensors_[w].dims->data[3], C = tensors_[w].dims->data[0];
+    if (fin < 1 || fin == cin || cin % fin != 0 || C % (cin / fin) != 0) continue;
+    const size_t km = sole_consumer(y);
+    const int u = const_op(km, i, "builtin:18", y, C);
+    if (u < 0 || params(*nodes_[km])->activation != 0) continue;
+    const size_t ka = sole_consumer(u);
+    const int z = const_op(ka, km, "builtin:0", u, C);
+    if (z < 0) continue;
+    std::vector<uint8_t> blob(2 * sizeof(BuiltinParams));
+    memcpy(blob.data(), params(conv), sizeof(BuiltinParams));
+    memcpy(blob.data() + sizeof(BuiltinParams), params(*nodes_[ka]), sizeof(BuiltinParams));
+    const std::vector<int> ins{x, w, conv.node.inputs->size > 2 ? conv.node.inputs->data[2] : -1,
+                               nodes_[km]->node.inputs->data[1], nodes_[ka]->node.inputs->data[1]};
+    LceB200IntArrayFree(conv.node.inputs);
+    LceB200IntArrayFree(conv.node.outputs);
+    conv.node.inputs = MakeDims(ins);
+    conv.node.outputs = MakeDims({z});
+    conv.builtin_blob = blob;
+    conv.node.builtin_data = conv.builtin_blob.data();
+    conv.registration = GroupedConvAffineRegistration();
+    conv.name = "CONV_2D+MUL+ADD";
+    for (size_t k : {ka, km}) {   // the later node first
+      NodeRecord& v = *nodes_[k];
+      LceB200IntArrayFree(v.node.inputs);
+      LceB200IntArrayFree(v.node.outputs);
+      LceB200IntArrayFree(v.node.temporaries);
+      LceB200IntArrayFree(v.node.intermediates);
+      nodes_.erase(nodes_.begin() + k);
+      ++removed;
+    }
+  }
+  allocated_ = false;
+  return removed;
+}
+
 // [DEQUANTIZE ->] CONV_2D(3x3, stride 2, 3 -> 16 or 8) -> DEPTHWISE_CONV_2D(3x3, stride 2,
 // multiplier 1), each intermediate consumed once: one node (the stem of QuickNet and QuickNetLarge,
 // 16, and of QuickNetSmall, 8). The image is read once, as the bytes the host shipped; the
@@ -1392,7 +1475,9 @@ int Graph::FuseStem() {
     const int w1 = c1.node.inputs->data[1];
     const int x = c1.node.inputs->data[0];
     const int c1_out = dims4(w1, 0);
+    // dims4(x, 3) != 3: a grouped convolution's filter has fewer input channels than x
     if ((c1_out != 16 && c1_out != 8) || dims4(w1, 1) != 3 || dims4(w1, 2) != 3 || dims4(w1, 3) != 3 ||
+        dims4(x, 3) != 3 ||
         bp(c1)->stride_h != 2 || bp(c1)->stride_w != 2 || bp(c1)->dilation_h != 1 ||
         bp(c1)->dilation_w != 1 || tensors_[x].type != kTfLiteFloat32 ||
         tensors_[c1.node.outputs->data[0]].type != kTfLiteFloat32)
@@ -1466,6 +1551,9 @@ int Graph::FuseConvQuantize() {
     if (tensors_[y].type != kTfLiteFloat32) continue;
     if (conv.node.inputs->size >= 2 && conv.builtin_blob.size() >= sizeof(BuiltinParams)) {
       const TfLiteIntArray* fd = tensors_[conv.node.inputs->data[1]].dims;
+      const TfLiteIntArray* xd = tensors_[conv.node.inputs->data[0]].dims;
+      // a grouped convolution (filter_in != the input's channels) runs its own kernel, without signs
+      if (fd && xd && fd->size == 4 && xd->size == 4 && fd->data[3] != xd->data[3]) continue;
       const auto* bp = reinterpret_cast<const BuiltinParams*>(conv.builtin_blob.data());
       if (fd && fd->size == 4 &&
           !lce_b200_internal_conv_packs_alike(fd->data[1], fd->data[2], bp->stride_h, bp->stride_w,

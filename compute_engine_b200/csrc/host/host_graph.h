@@ -136,6 +136,17 @@ class Graph {
   // the number of nodes removed (4, or 5 with the pool, per quantiser).
   int FuseQuantizedActivations();
 
+  // A BatchNorm behind a grouped convolution (Keras Conv2D(groups=g), or MeliusNet's stem with each
+  // group convolution as one op)
+  //   CONV_2D(filter [C, kh, kw, C_in / g], no fused activation) -> MUL(scale) -> ADD(shift, any activation)
+  // becomes one node "CONV_2D+MUL+ADD" (lce_b200_f32_grouped_conv2d with the epilogue): inputs [x,
+  // filter, bias (-1 when absent), scale, shift], builtin_data { the conv's, the ADD's BuiltinParams }.
+  // Only when g = C_in / filter_in is an exact division other than 1 and divides C, scale and shift
+  // are float constants of shape [C] or [1, ..., 1, C] and the second operand of their op, the MUL
+  // has no fused activation, and the conv and MUL outputs each have one consumer and are not graph
+  // outputs; an ungrouped CONV_2D is never matched. Bit-identical. Returns the nodes removed (2 each).
+  int FuseGroupedConvAffine();
+
   // BinaryDenseNet's dense layers
   //   x_j [B,H,W,C_j] -> MUL(scale) -> ADD(shift) -> LceQuantize -> LceBconv2d (float y_j)
   //   x_{j+1} = CONCATENATION([x_j, y_j], last axis)

@@ -1662,6 +1662,137 @@ int make_geom(const lce_f32_conv_desc* d, ConvGeom* g) {
   return 0;
 }
 
+// ---- grouped convolution (lce_b200_f32_grouped_conv2d): filter [Cout, KH, KW, Cin / G] ----
+// Output channel o reads input channels [(o / (Cout / G)) * Cin / G, ...). Each output is the chain
+// the other FMA convolution kernels run over its group's channels: acc = 0, fmaf over (fy, fx, ci)
+// in that order, padded taps as fmaf(0, w, acc); then the bias once if present, the activation, and
+// the optional BatchNorm behind it in the MUL and ADD builtins' roundings.
+struct GroupedEpilogue {
+  const float* bias;    // may be null
+  const float* scale;   // may be null (no MUL)
+  const float* shift;   // may be null (no ADD)
+  int act, post_act;
+};
+
+__device__ __forceinline__ float grouped_epilogue(float acc, int o, const GroupedEpilogue& e) {
+  float y = e.bias ? __fadd_rn(acc, __ldg(e.bias + o)) : acc;
+  y = apply_act(y, e.act);
+  if (e.scale) y = __fmul_rn(y, __ldg(e.scale + o));
+  if (e.shift) y = __fadd_rn(y, __ldg(e.shift + o));
+  return apply_act(y, e.post_act);
+}
+
+// Any shape: one thread per output element, operands straight from global memory.
+__global__ void __launch_bounds__(256) grouped_conv_any_kernel(const float* __restrict__ in,
+                                                               const float* __restrict__ filter,
+                                                               float* __restrict__ out, ConvGeom g, int cin_g,
+                                                               int cout_g, GroupedEpilogue e, long long n) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += stride) {
+    const int o = static_cast<int>(i % g.Cout);
+    long long r = i / g.Cout;
+    const int ox = static_cast<int>(r % g.OW);
+    r /= g.OW;
+    const int oy = static_cast<int>(r % g.OH);
+    const long long b = r / g.OH;
+    const float* wp = filter + static_cast<long long>(o) * g.KH * g.KW * cin_g;
+    const int c0 = (o / cout_g) * cin_g;
+    float acc = 0.0f;
+    for (int fy = 0; fy < g.KH; ++fy) {
+      const int iy = oy * g.sh - g.ph + fy * g.dh;
+      for (int fx = 0; fx < g.KW; ++fx) {
+        const int ix = ox * g.sw - g.pw + fx * g.dw;
+        const bool inside = static_cast<unsigned>(iy) < static_cast<unsigned>(g.H) &&
+                            static_cast<unsigned>(ix) < static_cast<unsigned>(g.W);
+        const float* src = in + ((b * g.H + (inside ? iy : 0)) * g.W + (inside ? ix : 0)) * g.Cin + c0;
+        for (int ci = 0; ci < cin_g; ++ci) acc = fmaf(inside ? __ldg(src + ci) : 0.0f, __ldg(wp++), acc);
+      }
+    }
+    out[i] = grouped_epilogue(acc, o, e);
+  }
+}
+
+// 3x3, stride 1, dilation 1, CG -> OG channels in each of G groups (MeliusNet's stem: 8 -> 8 in 4
+// groups, 4 -> 8 in 8). A block takes a 16 x 8 pixel tile of one image: the tile and its halo for all
+// channels, and every group's weights, are staged in shared memory once. A warp takes two rows of
+// the tile and one group, so its weight reads are one broadcast address; each lane owns one pixel and
+// the group's OG outputs and stores them as float4. Input pixels sit CIN + 4 floats apart, so the
+// float4 reads of eight consecutive lanes hit distinct banks. Padded taps read zeros from the tile.
+constexpr int kGTW = 16, kGTH = 8;
+template <int CG, int OG, int G>
+__global__ void __launch_bounds__(256) grouped_conv3x3_kernel(const float* __restrict__ in,
+                                                              const float* __restrict__ filter,
+                                                              float* __restrict__ out, ConvGeom g,
+                                                              GroupedEpilogue e) {
+  constexpr int CIN = CG * G, COUT = OG * G, PS = CIN + 4, Q = OG / 4;
+  constexpr int HW = kGTW + 2, HH = kGTH + 2;
+  static_assert(CG % 4 == 0 && OG % 4 == 0, "whole float4s per group");
+  __shared__ __align__(16) float x_s[HH * HW * PS];
+  __shared__ __align__(16) float w_s[9 * CG * OG * G];   // [tap][ci][q][g][4]
+  const int b = blockIdx.z;
+  const int oy0 = blockIdx.y * kGTH, ox0 = blockIdx.x * kGTW;
+  for (int i = threadIdx.x; i < 9 * CG * COUT; i += blockDim.x) {
+    const int o = i / (9 * CG), rem = i - o * (9 * CG);
+    const int gi = o / OG, oo = o - gi * OG;
+    w_s[((rem * Q + (oo >> 2)) * G + gi) * 4 + (oo & 3)] = __ldg(filter + i);
+  }
+  const long long img = static_cast<long long>(b) * g.H * g.W;
+  for (int i = threadIdx.x; i < HH * HW * (CIN / 4); i += blockDim.x) {
+    const int p = i / (CIN / 4), c4 = i - p * (CIN / 4);
+    const int py = p / HW, px = p - py * HW;
+    const int iy = oy0 - g.ph + py, ix = ox0 - g.pw + px;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (static_cast<unsigned>(iy) < static_cast<unsigned>(g.H) && static_cast<unsigned>(ix) < static_cast<unsigned>(g.W))
+      v = __ldg(reinterpret_cast<const float4*>(in + (img + static_cast<long long>(iy) * g.W + ix) * CIN) + c4);
+    *reinterpret_cast<float4*>(x_s + p * PS + c4 * 4) = v;
+  }
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int col = lane & (kGTW - 1);
+  // (row pair, group) tasks: kGTH / 2 * G of them over the block's 8 warps
+  for (int task = warp; task < (kGTH / 2) * G; task += 8) {
+    const int gi = task % G, row = (task / G) * 2 + (lane >> 4);
+    float acc[OG];
+#pragma unroll
+    for (int k = 0; k < OG; ++k) acc[k] = 0.0f;
+#pragma unroll
+    for (int fy = 0; fy < 3; ++fy)
+#pragma unroll
+      for (int fx = 0; fx < 3; ++fx) {
+        const float* xp = x_s + ((row + fy) * HW + col + fx) * PS + gi * CG;
+#pragma unroll
+        for (int c4 = 0; c4 < CG / 4; ++c4) {
+          const float4 v = *reinterpret_cast<const float4*>(xp + c4 * 4);
+          const float xv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float4* wq =
+                reinterpret_cast<const float4*>(w_s + (((fy * 3 + fx) * CG + c4 * 4 + k) * Q * G + gi) * 4);
+#pragma unroll
+            for (int q = 0; q < Q; ++q) {
+              const float4 w = wq[q * G];
+              acc[4 * q] = fmaf(xv[k], w.x, acc[4 * q]);
+              acc[4 * q + 1] = fmaf(xv[k], w.y, acc[4 * q + 1]);
+              acc[4 * q + 2] = fmaf(xv[k], w.z, acc[4 * q + 2]);
+              acc[4 * q + 3] = fmaf(xv[k], w.w, acc[4 * q + 3]);
+            }
+          }
+        }
+      }
+    const int oy = oy0 + row, ox = ox0 + col;
+    if (oy < g.OH && ox < g.OW) {
+      float4* o4 = reinterpret_cast<float4*>(out + ((static_cast<long long>(b) * g.OH + oy) * g.OW + ox) * COUT +
+                                             gi * OG);
+#pragma unroll
+      for (int q = 0; q < Q; ++q) {
+        const int o = gi * OG + 4 * q;
+        o4[q] = make_float4(grouped_epilogue(acc[4 * q], o, e), grouped_epilogue(acc[4 * q + 1], o + 1, e),
+                            grouped_epilogue(acc[4 * q + 2], o + 2, e), grouped_epilogue(acc[4 * q + 3], o + 3, e));
+      }
+    }
+  }
+}
+
 }  // namespace
 
 // DEQUANTIZE (TF/lite/kernels/internal/reference/dequantize.h:32-49): out = float(scale * (q - zp)),
@@ -2225,6 +2356,38 @@ int lce_b200_f32_quant2_planes(const float* x, int batch, int in_h, int in_w, in
   }
 #undef LCE_QUANT2
   return launch_check("quant2_planes_kernel");
+}
+
+int lce_b200_f32_grouped_conv2d(const lce_f32_conv_desc* d, int groups, const float* in, const float* filter,
+                                const float* bias, const float* scale, const float* shift, int post_activation,
+                                float* out, void* stream) {
+  ConvGeom g;
+  if (d == nullptr) return fail("grouped conv: no descriptor");
+  if (make_geom(d, &g)) return 1;
+  if (groups < 1 || g.Cin % groups || g.Cout % groups)
+    return fail("grouped conv: %d groups must divide the %d input and %d output channels", groups, g.Cin, g.Cout);
+  if (d->padding != LCE_PADDING_SAME && d->padding != LCE_PADDING_VALID)
+    return fail("grouped conv: unknown padding %d", d->padding);
+  const long long n = static_cast<long long>(g.B) * g.OH * g.OW * g.Cout;
+  if (n == 0) return 0;
+  if (in == nullptr || filter == nullptr || out == nullptr) return fail("grouped conv: null tensor");
+  const int cg = g.Cin / groups, og = g.Cout / groups;
+  const GroupedEpilogue e{bias, scale, shift, g.act, post_activation};
+  cudaStream_t s = as_stream(stream);
+  const bool a16 = !((uintptr_t)in & 15) && !((uintptr_t)out & 15);
+  if (g.KH == 3 && g.KW == 3 && g.sh == 1 && g.sw == 1 && g.dh == 1 && g.dw == 1 && a16 && g.B <= 65535) {
+    const dim3 grid((g.OW + kGTW - 1) / kGTW, (g.OH + kGTH - 1) / kGTH, g.B);
+    if (cg == 8 && og == 8 && groups == 4) {
+      grouped_conv3x3_kernel<8, 8, 4><<<grid, 256, 0, s>>>(in, filter, out, g, e);
+      return launch_check("grouped_conv3x3_kernel");
+    }
+    if (cg == 4 && og == 8 && groups == 8) {
+      grouped_conv3x3_kernel<4, 8, 8><<<grid, 256, 0, s>>>(in, filter, out, g, e);
+      return launch_check("grouped_conv3x3_kernel");
+    }
+  }
+  grouped_conv_any_kernel<<<grid_for(n, 256), 256, 0, s>>>(in, filter, out, g, cg, og, e, n);
+  return launch_check("grouped_conv_any_kernel");
 }
 
 int lce_b200_f32_logistic(const float* in, float* out, int64_t n, void* stream) {

@@ -214,6 +214,12 @@ class HostGraph:
         the bound). Call before allocate_tensors."""
         return lib().lce_host_fuse_quantized_activations(self._g)
 
+    def fuse_grouped_conv_affine(self):
+        """A grouped CONV_2D (filter [C, kh, kw, C_in / g], g > 1) -> MUL(scale [C]) -> ADD(shift [C])
+        => one node whose kernel applies the BatchNorm in its epilogue. Bit-identical; an ungrouped
+        CONV_2D is never matched. Call before allocate_tensors."""
+        return lib().lce_host_fuse_grouped_conv_affine(self._g)
+
     def fuse_activation_chains(self):
         """ADD -> PRELU -> ADD [-> ADD -> LceQuantize] (ReActNet's RPReLU / RSign, each step
         optional) => the epilogue of the preceding fused LceBconv2d+ADD node, or one node.
@@ -227,7 +233,7 @@ class HostGraph:
 
     def fuse_all(self):
         return (self.fuse_dense_blocks() + self.fuse_residual_blocks() + self.fuse_float_glue()
-                + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
+                + self.fuse_grouped_conv_affine() + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
                 + self.fuse_residual_pairs())
 
     # ---- profiling / async IO (bench.py) ----

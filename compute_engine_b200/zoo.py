@@ -445,7 +445,7 @@ def binarydensenet45(batch=1, seed=0, image=224, input_type="float32", pad_value
 
 
 def meliusnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0, blocks=(4, 5, 4, 6),
-              transitions=(160, 224, 256), name="MeliusNet22"):
+              transitions=(160, 224, 256), name="MeliusNet22", group_conv="split"):
     """MeliusNet, restated from the paper (Bethge et al., 2020) and larq-zoo's MeliusNet22 with
     synthetic weights, in the converter's op order:
       stem CONV_2D 3x3/s2 3 -> 32 (BN folded, RELU); a grouped convolution 32 -> 32 in 4 groups,
@@ -453,6 +453,11 @@ def meliusnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0, bl
       SPLIT(axis 3, 4) -> 4x CONV_2D 3x3 SAME 8 -> 8 (no bias) -> CONCATENATION -> MUL -> ADD(RELU),
       the BatchNorm and activation after the concatenation; the same 32 -> 64 in 8 groups (8x
       CONV_2D 4 -> 8); MAX_POOL_2D 3x3/s2 SAME;
+      with group_conv="native" each of the two grouped convolutions is instead one grouped CONV_2D
+      (filter [32, 3, 3, 8] and [64, 3, 3, 4], what Keras Conv2D(groups=g) converts to), then the same
+      MUL -> ADD(RELU): its filter is the split form's per-group filters, drawn in the same order and
+      concatenated along the output channels, and every other tensor is the split form's, so both
+      forms compute the same function (the default "split" model's bytes are unchanged);
       sections of `blocks` MeliusBlocks (64 -> 320, 160 -> 480, 224 -> 480, 256 -> 640 channels
       at the default), each a dense layer and then an improvement layer on the map x [B,H,W,C]:
         dense layer MUL(bn_scale) -> ADD(bn_shift) -> LceQuantize -> LceBconv2d 3x3 C -> 64
@@ -466,12 +471,25 @@ def meliusnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0, bl
       head MUL -> ADD (BN) -> RELU -> MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX.
     Simplifications: larq-zoo's transition convolutions are grouped; these are ungrouped. The
     slices come before the binary convolution, an order the converter may emit. 38 LceBconv2d,
-    38 STRIDED_SLICE, 2 SPLIT, 16 CONV_2D and 40 CONCATENATION at the default."""
+    38 STRIDED_SLICE, 2 SPLIT, 16 CONV_2D and 40 CONCATENATION at the default; with
+    group_conv="native" no SPLIT, 6 CONV_2D and 38 CONCATENATION."""
+    if group_conv not in ("split", "native"):
+        raise ValueError(f"group_conv must be 'split' or 'native', not {group_conv!r}")
+    native = group_conv == "native"
     g = _Builder(seed, batch, name)
     xs = (batch, image, image, 3)
     x = g.image_input(xs, input_type)
 
     def group_conv(t, ts, cout, groups):
+        if native:
+            cin = ts[3] // groups
+            # the split form's g.conv draws, group by group, concatenated along O
+            wt = np.concatenate([g.rng.standard_normal((cout // groups, 3, 3, cin)).astype(np.float32) *
+                                 np.float32(1.0 / np.sqrt(9 * cin)) for _ in range(groups)])
+            y = g.act(ts[:3] + (cout,))
+            g.m.add_op("CONV_2D", [t, g.const(wt), -1], [y], padding="SAME", stride=(1, 1), activation="NONE")
+            ts = ts[:3] + (cout,)
+            return g.batchnorm(y, ts, "RELU"), ts
         axis = g.const(np.array(3, np.int32), np.int32, "axis")
         parts = [g.act(ts[:3] + (ts[3] // groups,)) for _ in range(groups)]
         g.m.add_op("SPLIT", [axis, t], parts, num_splits=groups)

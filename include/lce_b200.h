@@ -241,6 +241,23 @@ int lce_b200_f32_round(const float* in_dev, float* out_dev, int64_t n, void* str
 int lce_b200_f32_quant2_planes(const float* x_dev, int batch, int in_h, int in_w, int channels,
                                int filter_h, int filter_w, int stride_h, int stride_w, int padding,
                                int activation, int32_t* planes_out_dev, void* stream);
+/* Grouped CONV_2D (TF/lite/kernels/conv.cc with groups = in_c / filter_in): x NHWC [batch, in_h,
+ * in_w, d->in_c], filter OHWI [d->out_c, filter_h, filter_w, d->in_c / groups]; output channel o reads
+ * the input channels [(o / (out_c / groups)) * in_c / groups, ...). `groups` must divide in_c and
+ * out_c; any stride, dilation and SAME / VALID padding. Each output is the fmaf chain of
+ * lce_b200_f32_conv2d over its group's channels (acc = 0, then (fy, fx, ci) in order, padded taps as
+ * fma(0, w, acc)), then
+ *   y = act(acc [+ bias[o]]),  y = fl(y * scale[o]),  y = fl(y + shift[o]),  out = post_act(y)
+ * with act = d->activation and post_activation an LCE_ACT_* code: a BatchNorm folded as MUL then ADD
+ * behind the convolution, rounded as those ops round. bias, scale and shift may be NULL (that step is
+ * absent). So the result equals one lce_b200_f32_conv2d per group on the channel slices, concatenated
+ * (then MUL and ADD), bit for bit. 3x3 stride-1 convolutions of 8 -> 8 channels in 4 groups and 4 -> 8
+ * in 8 groups on 16-byte aligned tensors run a tiled kernel; other shapes a direct one. */
+struct lce_f32_conv_desc; /* lce_b200_builtins.h */
+int lce_b200_f32_grouped_conv2d(const struct lce_f32_conv_desc* d, int groups, const float* in_dev,
+                                const float* filter_dev, const float* bias_dev, const float* scale_dev,
+                                const float* shift_dev, int post_activation, float* out_dev,
+                                void* stream);
 int lce_b200_bconv2d_run_host(lce_b200_bconv2d* plan, const int32_t* in_host,
                               void* out_host);
 void lce_b200_bconv2d_destroy(lce_b200_bconv2d* plan);
