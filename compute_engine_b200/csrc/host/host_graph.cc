@@ -300,35 +300,162 @@ TfLiteStatus Graph::PlanArena() {
   return kTfLiteOk;
 }
 
+// ------------------------------ graph fusion ------------------------------ //
+namespace {
+// The names of the builtin nodes the passes match: "builtin:<BuiltinOperator code>", as
+// BuildGraphFromTflite gives them (tflite_model.cc:323). Custom nodes carry their op's name.
+constexpr const char* kAdd = "builtin:0";
+constexpr const char* kConcatenation = "builtin:2";
+constexpr const char* kConv2d = "builtin:3";
+constexpr const char* kDepthwiseConv2d = "builtin:4";
+constexpr const char* kDequantize = "builtin:6";
+constexpr const char* kFullyConnected = "builtin:9";
+constexpr const char* kMaxPool2d = "builtin:17";
+constexpr const char* kMul = "builtin:18";
+constexpr const char* kRelu = "builtin:19";
+constexpr const char* kMean = "builtin:40";
+constexpr const char* kDiv = "builtin:42";
+constexpr const char* kStridedSlice = "builtin:45";
+constexpr const char* kPrelu = "builtin:54";
+constexpr const char* kMaximum = "builtin:55";
+constexpr const char* kMinimum = "builtin:57";
+constexpr const char* kRound = "builtin:116";
+
+std::vector<int> Ints(const TfLiteIntArray* a) { return std::vector<int>(a->data, a->data + a->size); }
+}  // namespace
+
+bool Graph::IsGraphOutput(int t) const {
+  return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end();
+}
+
+std::vector<size_t> Graph::Consumers(int t) const {
+  std::vector<size_t> c;
+  for (size_t k = 0; k < nodes_.size(); ++k)
+    for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+      if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
+  return c;
+}
+
+size_t Graph::SoleConsumer(int t) const {
+  if (IsGraphOutput(t)) return kNoNode;
+  const std::vector<size_t> c = Consumers(t);
+  return c.size() == 1 ? c[0] : kNoNode;
+}
+
+size_t Graph::SoleReaderAsFirstInput(int t) const {
+  if (IsGraphOutput(t)) return kNoNode;
+  size_t found = kNoNode;
+  int slots = 0;
+  for (size_t k = 0; k < nodes_.size(); ++k)
+    for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
+      if (nodes_[k]->node.inputs->data[q] == t) { ++slots; found = k; }
+  return slots == 1 && nodes_[found]->node.inputs->data[0] == t ? found : kNoNode;
+}
+
+bool Graph::ReadyBefore(int t, size_t i) const {
+  if (std::find(inputs_.begin(), inputs_.end(), t) != inputs_.end()) return true;
+  for (size_t k = 0; k < i; ++k)
+    for (int q = 0; q < nodes_[k]->node.outputs->size; ++q)
+      if (nodes_[k]->node.outputs->data[q] == t) return true;
+  return false;
+}
+
+bool Graph::SameDims(const TfLiteIntArray* a, const TfLiteIntArray* b) {
+  if (!a || !b || a->size != b->size) return false;
+  for (int k = 0; k < a->size; ++k)
+    if (a->data[k] != b->data[k]) return false;
+  return true;
+}
+
+const BuiltinParams* Graph::Params(const NodeRecord& n) {
+  return n.builtin_blob.size() >= sizeof(BuiltinParams)
+             ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())
+             : nullptr;
+}
+
+int32_t Graph::Activation(const NodeRecord& n) { return Params(n) ? Params(n)->activation : 0; }
+
+int Graph::PerChannelConstOp(size_t k, const char* op, int x, int C, bool any_activation) const {
+  if (k >= nodes_.size()) return -1;
+  const NodeRecord& n = *nodes_[k];
+  if (n.name != op || n.initialized || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
+      n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32 ||
+      !Params(n) || (!any_activation && Params(n)->activation != 0))
+    return -1;
+  const int v = n.node.inputs->data[1];
+  if (v < 0) return -1;
+  const TfLiteTensor& t = tensors_[v];
+  if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
+      t.dims->data[t.dims->size - 1] != C)
+    return -1;
+  for (int d = 0; d + 1 < t.dims->size; ++d)
+    if (t.dims->data[d] != 1) return -1;
+  return v;
+}
+
+bool Graph::IsQuantize(size_t k) const {
+  if (k >= nodes_.size()) return false;
+  const NodeRecord& n = *nodes_[k];
+  return n.name == "LceQuantize" && !n.initialized && n.node.inputs->size == 1 &&
+         n.node.outputs->size == 1 && tensors_[n.node.outputs->data[0]].type == kTfLiteInt32;
+}
+
+void Graph::EraseNode(size_t k) {
+  TfLiteNode& n = nodes_[k]->node;
+  LceB200IntArrayFree(n.inputs);
+  LceB200IntArrayFree(n.outputs);
+  LceB200IntArrayFree(n.temporaries);
+  LceB200IntArrayFree(n.intermediates);
+  nodes_.erase(nodes_.begin() + k);
+  allocated_ = false;
+}
+
+void Graph::EraseNodes(std::vector<size_t> ks) {
+  std::sort(ks.begin(), ks.end());
+  for (auto it = ks.rbegin(); it != ks.rend(); ++it) EraseNode(*it);   // the highest index first
+}
+
+void Graph::SetNodeIO(NodeRecord& n, const std::vector<int>& inputs, const std::vector<int>& outputs,
+                      const std::vector<int>& temporaries) {
+  LceB200IntArrayFree(n.node.inputs);
+  LceB200IntArrayFree(n.node.outputs);
+  LceB200IntArrayFree(n.node.temporaries);
+  n.node.inputs = MakeDims(inputs);
+  n.node.outputs = MakeDims(outputs);
+  n.node.temporaries = MakeDims(temporaries);
+  allocated_ = false;
+}
+
+void Graph::SetBuiltinBlob(NodeRecord& n, const void* bytes, size_t len) {
+  const uint8_t* b = static_cast<const uint8_t*>(bytes);
+  n.builtin_blob.assign(b, b + len);
+  n.node.builtin_data = n.builtin_blob.empty() ? nullptr : n.builtin_blob.data();
+  allocated_ = false;
+}
+
+void Graph::SetCustomOptions(NodeRecord& n, std::vector<uint8_t> options) {
+  n.custom_options = std::move(options);
+  n.node.custom_initial_data = n.custom_options.data();
+  n.node.custom_initial_data_size = static_cast<int>(n.custom_options.size());
+  allocated_ = false;
+}
+
 extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_FUSED(const TfLiteRegistration* original);
 
 int Graph::FuseResidualBlocks() {
   if (!device_arena_) return 0;
   int removed = 0;
-  auto consumers = [&](int t) {
-    std::vector<size_t> c;
-    for (size_t i = 0; i < nodes_.size(); ++i) {
-      const TfLiteIntArray* in = nodes_[i]->node.inputs;
-      for (int k = 0; k < in->size; ++k)
-        if (in->data[k] == t) { c.push_back(i); break; }
-    }
-    return c;
-  };
-  auto is_graph_output = [&](int t) {
-    return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end();
-  };
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& b = *nodes_[i];
     if (b.name != "LceBconv2d" || b.initialized || b.node.inputs->size != 5) continue;
     TfLiteRegistration* fused_reg = lce_b200_internal_Register_BCONV_2D_FUSED(b.registration);
     if (fused_reg == nullptr) continue;   // a foreign "LceBconv2d" (e.g. the CPU test double)
     const int y = b.node.outputs->data[0];
-    if (tensors_[y].type != kTfLiteFloat32 || is_graph_output(y)) continue;
-    std::vector<size_t> cy = consumers(y);
-    if (cy.size() != 1) continue;
-    const size_t ai = cy[0];
+    if (tensors_[y].type != kTfLiteFloat32) continue;
+    const size_t ai = SoleConsumer(y);
+    if (ai == kNoNode) continue;
     NodeRecord& a = *nodes_[ai];
-    if (a.name != "builtin:0" || a.node.inputs->size != 2 || ai <= i) continue;  // ADD
+    if (a.name != kAdd || a.node.inputs->size != 2 || ai <= i) continue;
     const int in0 = a.node.inputs->data[0], in1 = a.node.inputs->data[1];
     if (in0 == in1) continue;
     const int r = in0 == y ? in1 : in0;
@@ -337,63 +464,35 @@ int Graph::FuseResidualBlocks() {
     // run correctly unfused): the shortcut has exactly the convolution's shape (ADD would also
     // accept a broadcast over the last dimension), and the convolution is not grouped (the fused
     // sign-pack needs groups == 1): filter words per pixel == input words per pixel.
-    {
-      const TfLiteIntArray* ys = tensors_[y].dims;
-      const TfLiteIntArray* rs = tensors_[r].dims;
-      bool same = ys && rs && ys->size == rs->size;
-      for (int k = 0; same && k < ys->size; ++k) same = ys->data[k] == rs->data[k];
-      if (!same) continue;
-      const TfLiteIntArray* xs = tensors_[b.node.inputs->data[0]].dims;
-      const TfLiteIntArray* fs = tensors_[b.node.inputs->data[1]].dims;
-      if (!xs || !fs || xs->size != 4 || fs->size != 4 || xs->data[3] != fs->data[3]) continue;
-    }
+    if (!SameDims(tensors_[y].dims, tensors_[r].dims)) continue;
+    const TfLiteIntArray* xs = tensors_[b.node.inputs->data[0]].dims;
+    const TfLiteIntArray* fs = tensors_[b.node.inputs->data[1]].dims;
+    if (!xs || !fs || xs->size != 4 || fs->size != 4 || xs->data[3] != fs->data[3]) continue;
     // the shortcut must already exist when the bconv runs
-    bool r_ready = std::find(inputs_.begin(), inputs_.end(), r) != inputs_.end();
-    for (size_t k = 0; k < i && !r_ready; ++k)
-      for (int q = 0; q < nodes_[k]->node.outputs->size; ++q)
-        if (nodes_[k]->node.outputs->data[q] == r) r_ready = true;
-    if (!r_ready) continue;
+    if (!ReadyBefore(r, i)) continue;
     const int o = a.node.outputs->data[0];
-    int32_t add_act = 0;
-    if (a.builtin_blob.size() >= sizeof(BuiltinParams))
-      add_act = reinterpret_cast<const BuiltinParams*>(a.builtin_blob.data())->activation;
+    const int32_t add_act = Activation(a);
+    std::vector<size_t> absorbed{ai};
     // optional: the LceQuantize that consumes the sum
     int packed = -1;
-    size_t qi = nodes_.size();
-    for (size_t c : consumers(o)) {
+    for (size_t c : Consumers(o)) {
       NodeRecord& q = *nodes_[c];
       if (q.name == "LceQuantize" && c > ai && tensors_[o].type == kTfLiteFloat32) {
         packed = q.node.outputs->data[0];
-        qi = c;
+        absorbed.push_back(c);
         break;
       }
     }
-    // rewrite node i
-    std::vector<int> ins(b.node.inputs->data, b.node.inputs->data + 5);
+    std::vector<int> ins = Ints(b.node.inputs);
     ins.push_back(r);
     std::vector<int> outs{o};
     if (packed >= 0) outs.push_back(packed);
-    LceB200IntArrayFree(b.node.inputs);
-    LceB200IntArrayFree(b.node.outputs);
-    b.node.inputs = MakeDims(ins);
-    b.node.outputs = MakeDims(outs);
+    SetNodeIO(b, ins, outs);
     b.registration = fused_reg;
-    b.builtin_blob.assign(reinterpret_cast<const uint8_t*>(&add_act),
-                          reinterpret_cast<const uint8_t*>(&add_act) + 4);
-    b.node.builtin_data = b.builtin_blob.data();
+    SetBuiltinBlob(b, &add_act, sizeof(add_act));
     b.name = packed >= 0 ? "LceBconv2d+ADD+LceQuantize" : "LceBconv2d+ADD";
-    // drop the absorbed nodes (higher index first)
-    auto drop = [&](size_t idx) {
-      NodeRecord& n = *nodes_[idx];
-      LceB200IntArrayFree(n.node.inputs);
-      LceB200IntArrayFree(n.node.outputs);
-      LceB200IntArrayFree(n.node.temporaries);
-      LceB200IntArrayFree(n.node.intermediates);
-      nodes_.erase(nodes_.begin() + idx);
-      ++removed;
-    };
-    if (qi < nodes_.size()) drop(qi);
-    drop(ai);
+    removed += static_cast<int>(absorbed.size());
+    EraseNodes(absorbed);
   }
   allocated_ = false;
   return removed;
@@ -404,14 +503,6 @@ extern "C" int lce_b200_internal_pair_pays_off(const lce_bconv2d_desc* d);   // 
 
 int Graph::FuseResidualPairs() {
   if (!device_arena_) return 0;
-  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
-  auto consumers = [&](int t) {
-    std::vector<size_t> c;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
-    return c;
-  };
   // the channel count of a fused residual block (no chain) whose layer the pair kernel takes and
   // runs faster than two blocks at the input's current spatial size, or 0
   auto pair_channels = [&](const NodeRecord& n) {
@@ -440,41 +531,30 @@ int Graph::FuseResidualPairs() {
     if (pair_reg == nullptr) continue;
     // x1 and its signs feed the next block alone
     const int x1 = a.node.outputs->data[0], p1 = a.node.outputs->data[1];
-    if (is_output(x1) || is_output(p1)) continue;
-    const std::vector<size_t> cx = consumers(x1);
-    if (cx.size() != 1 || consumers(p1) != cx || cx[0] <= i) continue;
-    NodeRecord& b = *nodes_[cx[0]];
+    const size_t bi = SoleConsumer(x1);
+    if (bi == kNoNode || SoleConsumer(p1) != bi || bi <= i) continue;
+    NodeRecord& b = *nodes_[bi];
     if ((b.name != "LceBconv2d+ADD" && b.name != "LceBconv2d+ADD+LceQuantize") ||
         b.registration != a.registration || b.node.inputs->data[0] != p1 ||
         b.node.inputs->data[5] != x1)
       continue;
     const int C = pair_channels(a);
     if (C == 0 || pair_channels(b) != C) continue;
-    std::vector<int> ins(a.node.inputs->data, a.node.inputs->data + 6);
+    std::vector<int> ins = Ints(a.node.inputs);
     ins.insert(ins.end(), b.node.inputs->data + 1, b.node.inputs->data + 5);
-    std::vector<int> outs(b.node.outputs->data, b.node.outputs->data + b.node.outputs->size);
+    // each block's blob is its ADD's activation
     const int32_t acts[2] = {*reinterpret_cast<const int32_t*>(a.builtin_blob.data()),
                              *reinterpret_cast<const int32_t*>(b.builtin_blob.data())};
     const uint32_t n = static_cast<uint32_t>(a.custom_options.size());
     std::vector<uint8_t> opts(reinterpret_cast<const uint8_t*>(&n), reinterpret_cast<const uint8_t*>(&n) + 4);
     opts.insert(opts.end(), a.custom_options.begin(), a.custom_options.end());
     opts.insert(opts.end(), b.custom_options.begin(), b.custom_options.end());
-    LceB200IntArrayFree(a.node.inputs);
-    LceB200IntArrayFree(a.node.outputs);
-    a.node.inputs = MakeDims(ins);
-    a.node.outputs = MakeDims(outs);
-    a.custom_options = opts;
-    a.node.custom_initial_data = a.custom_options.data();
-    a.node.custom_initial_data_size = static_cast<int>(a.custom_options.size());
-    a.builtin_blob.assign(reinterpret_cast<const uint8_t*>(acts), reinterpret_cast<const uint8_t*>(acts) + 8);
-    a.node.builtin_data = a.builtin_blob.data();
+    SetNodeIO(a, ins, Ints(b.node.outputs));
+    SetCustomOptions(a, opts);
+    SetBuiltinBlob(a, acts, sizeof(acts));
     a.registration = pair_reg;
     a.name = "LceBconv2d+ADD+" + b.name;
-    LceB200IntArrayFree(b.node.inputs);
-    LceB200IntArrayFree(b.node.outputs);
-    LceB200IntArrayFree(b.node.temporaries);
-    LceB200IntArrayFree(b.node.intermediates);
-    nodes_.erase(nodes_.begin() + cx[0]);
+    EraseNode(bi);
     ++removed;
   }
   allocated_ = false;
@@ -485,60 +565,6 @@ extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_GATE(const Tf
 
 int Graph::FuseChannelGates() {
   if (!device_arena_) return 0;
-  const size_t none = nodes_.size() + 1;
-  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
-  auto consumers = [&](int t) {
-    std::vector<size_t> c;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
-    return c;
-  };
-  auto sole_consumer = [&](int t) {
-    if (is_output(t)) return none;
-    const std::vector<size_t> c = consumers(t);
-    return c.size() == 1 ? c[0] : none;
-  };
-  auto activation = [&](const NodeRecord& n) {
-    return n.builtin_blob.size() >= sizeof(BuiltinParams)
-               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())->activation
-               : 0;
-  };
-  // node k is the builtin `name` with two inputs, the first x, and one float output
-  auto binary = [&](size_t k, const char* name, int x) {
-    if (k >= nodes_.size()) return false;
-    const NodeRecord& n = *nodes_[k];
-    return n.name == name && !n.initialized && n.node.inputs->size == 2 && n.node.outputs->size == 1 &&
-           n.node.inputs->data[0] == x && tensors_[n.node.outputs->data[0]].type == kTfLiteFloat32;
-  };
-  // node k is op(x, v) with v a per-channel float constant ([1, ..., 1, C]) and no fused
-  // activation: returns v, else -1
-  auto const_op = [&](size_t k, const char* name, int x, int C) {
-    if (!binary(k, name, x) || activation(*nodes_[k]) != 0) return -1;
-    const int v = nodes_[k]->node.inputs->data[1];
-    if (v < 0) return -1;
-    const TfLiteTensor& t = tensors_[v];
-    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
-        t.dims->data[t.dims->size - 1] != C)
-      return -1;
-    for (int d = 0; d + 1 < t.dims->size; ++d)
-      if (t.dims->data[d] != 1) return -1;
-    return v;
-  };
-  // tensor t exists before node i runs
-  auto ready_before = [&](int t, size_t i) {
-    if (std::find(inputs_.begin(), inputs_.end(), t) != inputs_.end()) return true;
-    for (size_t k = 0; k < i; ++k)
-      for (int q = 0; q < nodes_[k]->node.outputs->size; ++q)
-        if (nodes_[k]->node.outputs->data[q] == t) return true;
-    return false;
-  };
-  auto same_dims = [](const TfLiteIntArray* a, const TfLiteIntArray* b) {
-    if (!a || !b || a->size != b->size) return false;
-    for (int k = 0; k < a->size; ++k)
-      if (a->data[k] != b->data[k]) return false;
-    return true;
-  };
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& b = *nodes_[i];
@@ -551,36 +577,41 @@ int Graph::FuseChannelGates() {
     if (tensors_[y].type != kTfLiteFloat32 || !yd || yd->size != 4) continue;
     const int C = yd->data[3];
     // MUL(y, g): g a computed float [B, 1, 1, C]
-    const size_t km = sole_consumer(y);
-    if (!binary(km, "builtin:18", y) || activation(*nodes_[km]) != 0) continue;
-    const int g = nodes_[km]->node.inputs->data[1];
+    const size_t km = SoleConsumer(y);
+    if (km == kNoNode) continue;
+    const NodeRecord& m = *nodes_[km];
+    if (m.name != kMul || m.initialized || m.node.inputs->size != 2 || m.node.outputs->size != 1 ||
+        m.node.inputs->data[0] != y || tensors_[m.node.outputs->data[0]].type != kTfLiteFloat32 ||
+        Activation(m) != 0)
+      continue;
+    const int g = m.node.inputs->data[1];
     if (g < 0 || g == y) continue;
     const TfLiteTensor& gt = tensors_[g];
     if (gt.type != kTfLiteFloat32 || gt.allocation_type == kTfLiteMmapRo || !gt.dims || gt.dims->size != 4 ||
         gt.dims->data[0] != yd->data[0] || gt.dims->data[1] != 1 || gt.dims->data[2] != 1 ||
-        gt.dims->data[3] != C || !ready_before(g, i))
+        gt.dims->data[3] != C || !ReadyBefore(g, i))
       continue;
     // PRELU(t, alpha [1, ..., 1, C])
-    const int t1 = nodes_[km]->node.outputs->data[0];
-    const size_t kp = sole_consumer(t1);
-    const int alpha = const_op(kp, "builtin:54", t1, C);
+    const int t1 = m.node.outputs->data[0];
+    const size_t kp = SoleConsumer(t1);
+    const int alpha = PerChannelConstOp(kp, kPrelu, t1, C);
     if (alpha < 0) continue;
     // ADD(u, shortcut), the shortcut a computed float tensor of y's shape; its activation applies
     const int t2 = nodes_[kp]->node.outputs->data[0];
-    const size_t ka = sole_consumer(t2);
-    if (ka >= nodes_.size()) continue;
+    const size_t ka = SoleConsumer(t2);
+    if (ka == kNoNode) continue;
     const NodeRecord& a = *nodes_[ka];
-    if (a.name != "builtin:0" || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1)
+    if (a.name != kAdd || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1)
       continue;
     const int in0 = a.node.inputs->data[0], in1 = a.node.inputs->data[1];
     if (in0 == in1 || (in0 != t2 && in1 != t2)) continue;
     const int r = in0 == t2 ? in1 : in0;
     if (r < 0 || tensors_[r].type != kTfLiteFloat32 || tensors_[r].allocation_type == kTfLiteMmapRo ||
-        !same_dims(tensors_[r].dims, yd) || !ready_before(r, i))
+        !SameDims(tensors_[r].dims, yd) || !ReadyBefore(r, i))
       continue;
     const int o = a.node.outputs->data[0];
     if (tensors_[o].type != kTfLiteFloat32) continue;
-    const int32_t add_act = activation(a);
+    const int32_t add_act = Activation(a);
     std::vector<size_t> absorbed{km, kp, ka};
     // the next block's BatchNorm and sign: MUL(o, scale) -> ADD(shift) -> LceQuantize, when the
     // convolution is ungrouped (the fused sign-pack needs groups == 1)
@@ -588,48 +619,30 @@ int Graph::FuseChannelGates() {
     const TfLiteIntArray* xs = tensors_[b.node.inputs->data[0]].dims;
     const TfLiteIntArray* fs = tensors_[b.node.inputs->data[1]].dims;
     const bool ungrouped = xs && fs && xs->size == 4 && fs->size == 4 && xs->data[3] == fs->data[3];
-    for (size_t c : consumers(o)) {
+    for (size_t c : Consumers(o)) {
       if (!ungrouped) break;
-      const int v1 = const_op(c, "builtin:18", o, C);
+      const int v1 = PerChannelConstOp(c, kMul, o, C);
       if (v1 < 0) continue;
       const int t3 = nodes_[c]->node.outputs->data[0];
-      const size_t k2 = sole_consumer(t3);
-      const int v2 = const_op(k2, "builtin:0", t3, C);
+      const size_t k2 = SoleConsumer(t3);
+      const int v2 = PerChannelConstOp(k2, kAdd, t3, C);
       if (v2 < 0) continue;
-      const size_t kq = sole_consumer(nodes_[k2]->node.outputs->data[0]);
-      if (kq >= nodes_.size()) continue;
-      const NodeRecord& q = *nodes_[kq];
-      if (q.name != "LceQuantize" || q.initialized || q.node.inputs->size != 1 || q.node.outputs->size != 1 ||
-          tensors_[q.node.outputs->data[0]].type != kTfLiteInt32)
-        continue;
-      sc = v1; sh = v2; packed = q.node.outputs->data[0];
+      const size_t kq = SoleConsumer(nodes_[k2]->node.outputs->data[0]);
+      if (!IsQuantize(kq)) continue;
+      sc = v1; sh = v2; packed = nodes_[kq]->node.outputs->data[0];
       absorbed.insert(absorbed.end(), {c, k2, kq});
       break;
     }
-    std::vector<int> ins(b.node.inputs->data, b.node.inputs->data + 5);
+    std::vector<int> ins = Ints(b.node.inputs);
     ins.insert(ins.end(), {r, g, alpha, sc, sh});
     std::vector<int> outs{o};
     if (packed >= 0) outs.push_back(packed);
-    LceB200IntArrayFree(b.node.inputs);
-    LceB200IntArrayFree(b.node.outputs);
-    b.node.inputs = MakeDims(ins);
-    b.node.outputs = MakeDims(outs);
+    SetNodeIO(b, ins, outs);
     b.registration = gate_reg;
-    b.builtin_blob.assign(reinterpret_cast<const uint8_t*>(&add_act),
-                          reinterpret_cast<const uint8_t*>(&add_act) + 4);
-    b.node.builtin_data = b.builtin_blob.data();
+    SetBuiltinBlob(b, &add_act, sizeof(add_act));
     b.name = packed >= 0 ? "LceBconv2d+MUL+PRELU+ADD+MUL+ADD+LceQuantize" : "LceBconv2d+MUL+PRELU+ADD";
-    // drop the absorbed nodes (all after node i), the highest index first
-    std::sort(absorbed.begin(), absorbed.end());
-    for (auto it = absorbed.rbegin(); it != absorbed.rend(); ++it) {
-      NodeRecord& n = *nodes_[*it];
-      LceB200IntArrayFree(n.node.inputs);
-      LceB200IntArrayFree(n.node.outputs);
-      LceB200IntArrayFree(n.node.temporaries);
-      LceB200IntArrayFree(n.node.intermediates);
-      nodes_.erase(nodes_.begin() + *it);
-      ++removed;
-    }
+    removed += static_cast<int>(absorbed.size());
+    EraseNodes(absorbed);   // all after node i
   }
   allocated_ = false;
   return removed;
@@ -640,60 +653,22 @@ extern "C" int lce_b200_internal_slice_takes(const lce_bconv2d_desc* d);   // lc
 
 int Graph::FuseDenseBlocks() {
   if (!device_arena_) return 0;
-  const size_t none = nodes_.size() + 1;
-  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
-  auto consumers = [&](int t) {
-    std::vector<size_t> c;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
-    return c;
-  };
-  auto sole_consumer = [&](int t) {
-    if (is_output(t)) return none;
-    const std::vector<size_t> c = consumers(t);
-    return c.size() == 1 ? c[0] : none;
-  };
-  auto params = [&](const NodeRecord& n) {
-    return n.builtin_blob.size() >= sizeof(BuiltinParams)
-               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())
-               : nullptr;
-  };
   auto dims4 = [&](int t) {
     const TfLiteIntArray* d = tensors_[t].dims;
     return d && d->size == 4 ? d : nullptr;
-  };
-  // node k is the builtin op(x, v), v a float constant [C] or [1, ..., 1, C], with no fused
-  // activation and a float output: returns v, else -1
-  auto const_op = [&](size_t k, const char* name, int x, int C) {
-    if (k >= nodes_.size()) return -1;
-    const NodeRecord& n = *nodes_[k];
-    if (n.name != name || n.initialized || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
-        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32 ||
-        !params(n) || params(n)->activation != 0)
-      return -1;
-    const int v = n.node.inputs->data[1];
-    if (v < 0) return -1;
-    const TfLiteTensor& t = tensors_[v];
-    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
-        t.dims->data[t.dims->size - 1] != C)
-      return -1;
-    for (int d = 0; d + 1 < t.dims->size; ++d)
-      if (t.dims->data[d] != 1) return -1;
-    return v;
   };
   auto producer = [&](int t) {
     for (size_t k = 0; k < nodes_.size(); ++k)
       for (int q = 0; q < nodes_[k]->node.outputs->size; ++q)
         if (nodes_[k]->node.outputs->data[q] == t) return k;
-    return none;
+    return kNoNode;
   };
   // node k is a STRIDED_SLICE of x [B,H,W,C] (through the builtin's own normalisation) to the
   // channels [lo, hi), the other axes whole, with a float output read once and not a graph output
   auto channel_slice = [&](size_t k, int x, const TfLiteIntArray* xd, int lo, int hi) {
     if (k >= nodes_.size()) return false;
     const NodeRecord& n = *nodes_[k];
-    if (n.name != "builtin:45" || n.initialized || !params(n) || n.node.inputs->size != 4 ||
+    if (n.name != kStridedSlice || n.initialized || !Params(n) || n.node.inputs->size != 4 ||
         n.node.outputs->size != 1 || n.node.inputs->data[0] != x)
       return false;
     const int32_t* v[3];
@@ -707,13 +682,13 @@ int Graph::FuseDenseBlocks() {
     }
     SliceBounds sb;
     if (StridedSliceBounds(xd->data, 4, v[0], v[1], v[2], tensors_[n.node.inputs->data[1]].dims->data[0],
-                           *params(n), &sb) != nullptr)
+                           *Params(n), &sb) != nullptr)
       return false;
     for (int d = 0; d < 3; ++d)
       if (sb.begin[d] != 0 || sb.end[d] != xd->data[d]) return false;
     const int out = n.node.outputs->data[0];
     return sb.begin[3] == lo && sb.end[3] == hi && tensors_[out].type == kTfLiteFloat32 &&
-           sole_consumer(out) != none;
+           SoleConsumer(out) != kNoNode;
   };
   // One layer read from the MUL at node i: x -> MUL(scale) -> ADD(shift) -> LceQuantize ->
   // LceBconv2d (float y, one that run_slice takes, same image size), then either
@@ -730,28 +705,23 @@ int Graph::FuseDenseBlocks() {
   };
   auto match = [&](size_t i, Layer* L) {
     const NodeRecord& m = *nodes_[i];
-    if (m.name != "builtin:18" || m.node.inputs->size != 2) return false;
+    if (m.name != kMul || m.node.inputs->size != 2) return false;
     const int x = m.node.inputs->data[0];
     const TfLiteIntArray* xd = x >= 0 && tensors_[x].type == kTfLiteFloat32 ? dims4(x) : nullptr;
     if (!xd || xd->data[3] % 4 != 0) return false;
     const int C = xd->data[3];
     L->mul = i; L->x = x;
-    L->scale = const_op(i, "builtin:18", x, C);
+    L->scale = PerChannelConstOp(i, kMul, x, C);
     if (L->scale < 0) return false;
     const int t1 = m.node.outputs->data[0];
-    L->add = sole_consumer(t1);
-    L->shift = const_op(L->add, "builtin:0", t1, C);
+    L->add = SoleConsumer(t1);
+    L->shift = PerChannelConstOp(L->add, kAdd, t1, C);
     if (L->shift < 0) return false;
-    const int t2 = nodes_[L->add]->node.outputs->data[0];
-    L->quant = sole_consumer(t2);
-    if (L->quant >= nodes_.size()) return false;
-    const NodeRecord& q = *nodes_[L->quant];
-    if (q.name != "LceQuantize" || q.initialized || q.node.inputs->size != 1 || q.node.outputs->size != 1)
-      return false;
-    L->packed = q.node.outputs->data[0];
-    if (tensors_[L->packed].type != kTfLiteInt32) return false;
-    L->conv = sole_consumer(L->packed);
-    if (L->conv >= nodes_.size()) return false;
+    L->quant = SoleConsumer(nodes_[L->add]->node.outputs->data[0]);
+    if (!IsQuantize(L->quant)) return false;
+    L->packed = nodes_[L->quant]->node.outputs->data[0];
+    L->conv = SoleConsumer(L->packed);
+    if (L->conv == kNoNode) return false;
     const NodeRecord& b = *nodes_[L->conv];
     if (b.name != "LceBconv2d" || b.initialized || b.node.inputs->size != 5 || b.node.outputs->size != 1 ||
         b.node.inputs->data[0] != L->packed)
@@ -776,11 +746,11 @@ int Graph::FuseDenseBlocks() {
         !lce_b200_internal_slice_takes(&d))
       return false;
     L->c_out = d.channels_out;
-    const size_t next = sole_consumer(y);
-    if (next >= nodes_.size()) return false;
+    const size_t next = SoleConsumer(y);
+    if (next == kNoNode) return false;
     std::vector<int> cat_ins{x, y};
     int c_cat = C + d.channels_out;
-    L->kind = nodes_[next]->name == "builtin:2" ? 0 : 1;
+    L->kind = nodes_[next]->name == kConcatenation ? 0 : 1;
     if (L->kind == 0) {
       L->cat = next;
       L->x_readers = {L->mul, L->cat};
@@ -788,8 +758,8 @@ int Graph::FuseDenseBlocks() {
       // the improvement layer's tail
       L->sum = next;
       const NodeRecord& a = *nodes_[L->sum];
-      if (a.name != "builtin:0" || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1 ||
-          !params(a) || params(a)->activation != 0 || d.channels_out > C)
+      if (a.name != kAdd || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1 ||
+          !Params(a) || Params(a)->activation != 0 || d.channels_out > C)
         return false;
       const int bt = a.node.inputs->data[a.node.inputs->data[0] == y ? 1 : 0];
       const int sum = a.node.outputs->data[0];
@@ -797,10 +767,10 @@ int Graph::FuseDenseBlocks() {
       if (bt < 0 || bt == y || !sd || sd->data[3] != d.channels_out) return false;
       L->slice_b = producer(bt);
       if (!channel_slice(L->slice_b, x, xd, C - d.channels_out, C)) return false;
-      L->cat = sole_consumer(sum);
-      if (L->cat >= nodes_.size() || nodes_[L->cat]->node.inputs->size != 2) return false;
+      L->cat = SoleConsumer(sum);
+      if (L->cat == kNoNode || nodes_[L->cat]->node.inputs->size != 2) return false;
       const int at = nodes_[L->cat]->node.inputs->data[0];
-      L->slice_a = at >= 0 ? producer(at) : none;
+      L->slice_a = at >= 0 ? producer(at) : kNoNode;
       if (!channel_slice(L->slice_a, x, xd, 0, C - d.channels_out) || L->slice_b >= L->sum ||
           L->slice_a >= L->cat || L->conv >= L->sum || L->sum >= L->cat)
         return false;
@@ -810,9 +780,9 @@ int Graph::FuseDenseBlocks() {
       std::sort(L->x_readers.begin(), L->x_readers.end());
     }
     const NodeRecord& c = *nodes_[L->cat];
-    if (c.name != "builtin:2" || c.initialized || c.node.inputs->size != 2 || c.node.outputs->size != 1 ||
-        c.node.inputs->data[0] != cat_ins[0] || c.node.inputs->data[1] != cat_ins[1] || !params(c) ||
-        params(c)->activation != 0 || (params(c)->axis != 3 && params(c)->axis != -1))
+    if (c.name != kConcatenation || c.initialized || c.node.inputs->size != 2 || c.node.outputs->size != 1 ||
+        c.node.inputs->data[0] != cat_ins[0] || c.node.inputs->data[1] != cat_ins[1] || !Params(c) ||
+        Params(c)->activation != 0 || (Params(c)->axis != 3 && Params(c)->axis != -1))
       return false;
     L->out = c.node.outputs->data[0];
     const TfLiteIntArray* od = tensors_[L->out].type == kTfLiteFloat32 ? dims4(L->out) : nullptr;
@@ -829,8 +799,8 @@ int Graph::FuseDenseBlocks() {
     std::vector<Layer> block{first};
     for (;;) {
       const int xj = block.back().out;
-      if (is_output(xj)) break;
-      const std::vector<size_t> readers = consumers(xj);
+      if (IsGraphOutput(xj)) break;
+      const std::vector<size_t> readers = Consumers(xj);
       Layer next;
       bool found = false;
       for (size_t r : readers)
@@ -861,19 +831,10 @@ int Graph::FuseDenseBlocks() {
       NodeRecord& n = *nodes_[L.mul];
       std::vector<int> ins{j == 0 ? L.x : X, L.scale, L.shift};
       ins.insert(ins.end(), conv.node.inputs->data + 1, conv.node.inputs->data + 5);
-      LceB200IntArrayFree(n.node.inputs);
-      LceB200IntArrayFree(n.node.outputs);
-      LceB200IntArrayFree(n.node.temporaries);
-      n.node.inputs = MakeDims(ins);
-      n.node.outputs = MakeDims({X});
-      n.node.temporaries = MakeDims(tmps);
-      n.custom_options = conv.custom_options;
-      n.node.custom_initial_data = n.custom_options.data();
-      n.node.custom_initial_data_size = static_cast<int>(n.custom_options.size());
+      SetNodeIO(n, ins, {X}, tmps);
+      SetCustomOptions(n, conv.custom_options);
       const int32_t blob[2] = {c_total, L.kind};   // DensePrepare
-      n.builtin_blob.assign(reinterpret_cast<const uint8_t*>(blob),
-                            reinterpret_cast<const uint8_t*>(blob) + sizeof(blob));
-      n.node.builtin_data = n.builtin_blob.data();
+      SetBuiltinBlob(n, blob, sizeof(blob));
       n.registration = L.reg;
       if (L.kind == 0) {
         n.name = "MUL+ADD+LceQuantize+LceBconv2d+CONCATENATION";
@@ -883,19 +844,11 @@ int Graph::FuseDenseBlocks() {
         absorbed.insert(absorbed.end(), {L.add, L.quant, L.conv, L.slice_a, L.slice_b, L.sum, L.cat});
       }
     }
-    // drop the absorbed nodes, the highest index first; a first improvement layer's slices may
-    // precede its MUL, and node i moves back by their number
-    std::sort(absorbed.begin(), absorbed.end());
-    for (auto it = absorbed.rbegin(); it != absorbed.rend(); ++it) {
-      NodeRecord& n = *nodes_[*it];
-      LceB200IntArrayFree(n.node.inputs);
-      LceB200IntArrayFree(n.node.outputs);
-      LceB200IntArrayFree(n.node.temporaries);
-      LceB200IntArrayFree(n.node.intermediates);
-      nodes_.erase(nodes_.begin() + *it);
-      ++removed;
-      if (*it < i) --i;
-    }
+    // a first improvement layer's slices may precede its MUL, and node i moves back by their number
+    const size_t before_i = std::count_if(absorbed.begin(), absorbed.end(), [&](size_t k) { return k < i; });
+    removed += static_cast<int>(absorbed.size());
+    EraseNodes(absorbed);
+    i -= before_i;
   }
   allocated_ = false;
   return removed;
@@ -910,58 +863,6 @@ const TfLiteRegistration* GroupedConvAffineRegistration();
 
 int Graph::FuseActivationChains() {
   if (!device_arena_) return 0;
-  const size_t none = nodes_.size() + 1;   // "no such node" (compared before nodes are erased)
-  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
-  auto consumers = [&](int t) {
-    std::vector<size_t> c;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
-    return c;
-  };
-  // the node that alone reads t, when t is an intermediate the chain may absorb
-  auto sole_consumer = [&](int t) {
-    if (is_output(t)) return none;
-    const std::vector<size_t> c = consumers(t);
-    return c.size() == 1 ? c[0] : none;
-  };
-  // node k is op(x, v) with v a per-channel constant of x's C channels (float, kTfLiteMmapRo,
-  // shape [1, ..., 1, C]) and no fused activation: returns v, else -1
-  auto const_op = [&](size_t k, const char* name, int x, int C) {
-    if (k >= nodes_.size()) return -1;
-    const NodeRecord& n = *nodes_[k];
-    if (n.name != name || n.initialized || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
-        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32 ||
-        n.builtin_blob.size() < sizeof(BuiltinParams) ||
-        reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())->activation != 0)
-      return -1;
-    const int v = n.node.inputs->data[1];
-    if (v < 0) return -1;
-    const TfLiteTensor& t = tensors_[v];
-    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
-        t.dims->data[t.dims->size - 1] != C)
-      return -1;
-    for (int d = 0; d + 1 < t.dims->size; ++d)
-      if (t.dims->data[d] != 1) return -1;
-    return v;
-  };
-  // node k's output is read only by an LceQuantize: returns that node, else none
-  auto quantize_of = [&](size_t k) {
-    const int y = nodes_[k]->node.outputs->data[0];
-    const size_t q = sole_consumer(y);
-    if (q >= nodes_.size()) return none;
-    const NodeRecord& n = *nodes_[q];
-    return n.name == "LceQuantize" && !n.initialized && n.node.inputs->size == 1 &&
-                   n.node.outputs->size == 1 && tensors_[n.node.outputs->data[0]].type == kTfLiteInt32
-               ? q
-               : none;
-  };
-  auto free_node = [&](NodeRecord& n) {
-    LceB200IntArrayFree(n.node.inputs);
-    LceB200IntArrayFree(n.node.outputs);
-    LceB200IntArrayFree(n.node.temporaries);
-    LceB200IntArrayFree(n.node.intermediates);
-  };
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& a = *nodes_[i];
@@ -969,38 +870,36 @@ int Graph::FuseActivationChains() {
     // after a fused residual block the chain starts on the sum; elsewhere node i is its first op
     const bool after_bconv = a.name == "LceBconv2d+ADD" && a.node.inputs->size == 6 &&
                              a.node.outputs->size == 1;
-    if (!after_bconv && a.name != "builtin:0" && a.name != "builtin:54") continue;
+    if (!after_bconv && a.name != kAdd && a.name != kPrelu) continue;
     int cur = after_bconv ? a.node.outputs->data[0] : a.node.inputs->data[0];
     if (cur < 0 || tensors_[cur].type != kTfLiteFloat32 || tensors_[cur].dims->size < 1) continue;
     const int C = tensors_[cur].dims->data[tensors_[cur].dims->size - 1];
     std::vector<size_t> absorbed;
     int vec[4] = {-1, -1, -1, -1};   // shift_in, alpha, shift_out, sign_shift
-    size_t k = after_bconv ? sole_consumer(cur) : i;
+    size_t k = after_bconv ? SoleConsumer(cur) : i;
     // RPReLU: ADD? -> PRELU? -> ADD?; an ADD read only by an LceQuantize is the RSign's instead
-    const char* steps[3] = {"builtin:0", "builtin:54", "builtin:0"};
+    const char* steps[3] = {kAdd, kPrelu, kAdd};
     for (int s = 0; s < 3 && k < nodes_.size(); ++s) {
-      const int v = const_op(k, steps[s], cur, C);
-      if (v < 0 || (s != 1 && quantize_of(k) < nodes_.size())) continue;
+      const int v = PerChannelConstOp(k, steps[s], cur, C);
+      if (v < 0 || (s != 1 && IsQuantize(SoleConsumer(nodes_[k]->node.outputs->data[0])))) continue;
       vec[s] = v;
       absorbed.push_back(k);
       cur = nodes_[k]->node.outputs->data[0];
-      k = sole_consumer(cur);
+      k = SoleConsumer(cur);
     }
     const bool any_float = !absorbed.empty();
     // RSign of the next binary layer: [ADD(sign_shift) ->] LceQuantize of the chain's result
     int packed = -1;
-    for (size_t c : consumers(cur)) {
+    for (size_t c : Consumers(cur)) {
       if (!any_float && !after_bconv && c != i) continue;   // stand-alone: node i must start it
-      const NodeRecord& n = *nodes_[c];
-      if (n.name == "LceQuantize" && !n.initialized && n.node.inputs->size == 1 &&
-          n.node.outputs->size == 1 && tensors_[n.node.outputs->data[0]].type == kTfLiteInt32) {
-        packed = n.node.outputs->data[0];
+      if (IsQuantize(c)) {
+        packed = nodes_[c]->node.outputs->data[0];
         absorbed.push_back(c);
         break;
       }
-      const int v = const_op(c, "builtin:0", cur, C);
-      const size_t q = v >= 0 ? quantize_of(c) : none;
-      if (q < nodes_.size()) {
+      const int v = PerChannelConstOp(c, kAdd, cur, C);
+      const size_t q = v >= 0 ? SoleConsumer(nodes_[c]->node.outputs->data[0]) : kNoNode;
+      if (IsQuantize(q)) {
         vec[3] = v;
         packed = nodes_[q]->node.outputs->data[0];
         absorbed.push_back(c);
@@ -1021,13 +920,13 @@ int Graph::FuseActivationChains() {
     if (packed >= 0) name += vec[3] >= 0 ? "+ADD+LceQuantize" : "+LceQuantize";
     // the float result stays a tensor when something else reads it; a stand-alone chain without
     // float steps would only copy its input
-    const std::vector<size_t> readers = consumers(cur);
-    const bool keep_out = after_bconv || (any_float && (is_output(cur) ||
+    const std::vector<size_t> readers = Consumers(cur);
+    const bool keep_out = after_bconv || (any_float && (IsGraphOutput(cur) ||
                                                         readers.size() > (packed >= 0 ? 1u : 0u)));
     std::vector<int> ins, outs{keep_out ? cur : -1};
     if (packed >= 0) outs.push_back(packed);
     if (after_bconv) {
-      ins.assign(a.node.inputs->data, a.node.inputs->data + 6);
+      ins = Ints(a.node.inputs);
       a.name += name;
     } else {
       ins.push_back(a.node.inputs->data[0]);
@@ -1035,18 +934,11 @@ int Graph::FuseActivationChains() {
       a.name = name.substr(1);
     }
     ins.insert(ins.end(), vec, vec + 4);
-    LceB200IntArrayFree(a.node.inputs);
-    LceB200IntArrayFree(a.node.outputs);
-    a.node.inputs = MakeDims(ins);
-    a.node.outputs = MakeDims(outs);
-    // drop the absorbed nodes (all after node i), the highest index first
-    std::sort(absorbed.begin(), absorbed.end());
-    for (auto it = absorbed.rbegin(); it != absorbed.rend(); ++it) {
-      if (*it == i) continue;
-      free_node(*nodes_[*it]);
-      nodes_.erase(nodes_.begin() + *it);
-      ++removed;
-    }
+    SetNodeIO(a, ins, outs);
+    // node i, when the chain starts on it, is the node just rewritten; the others are all after it
+    absorbed.erase(std::remove(absorbed.begin(), absorbed.end(), i), absorbed.end());
+    removed += static_cast<int>(absorbed.size());
+    EraseNodes(absorbed);
   }
   allocated_ = false;
   return removed;
@@ -1054,102 +946,37 @@ int Graph::FuseActivationChains() {
 
 int Graph::FusePooledSigns() {
   if (!device_arena_) return 0;
-  const size_t none = nodes_.size() + 1;
-  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
-  auto sole_consumer = [&](int t) {
-    if (is_output(t)) return none;
-    size_t found = none;
-    int n = 0;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { ++n; found = k; break; }
-    return n == 1 ? found : none;
-  };
-  // node k (after node `after`) is op(x, v) with v a per-channel float constant ([1, ..., 1, C]) and
-  // no fused activation: returns v, else -1
-  auto const_op = [&](size_t k, size_t after, const char* name, int x, int C) {
-    if (k >= nodes_.size() || k <= after) return -1;
-    const NodeRecord& n = *nodes_[k];
-    if (n.name != name || n.initialized || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
-        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32 ||
-        n.builtin_blob.size() < sizeof(BuiltinParams) ||
-        reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())->activation != 0)
-      return -1;
-    const int v = n.node.inputs->data[1];
-    if (v < 0) return -1;
-    const TfLiteTensor& t = tensors_[v];
-    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
-        t.dims->data[t.dims->size - 1] != C)
-      return -1;
-    for (int d = 0; d + 1 < t.dims->size; ++d)
-      if (t.dims->data[d] != 1) return -1;
-    return v;
-  };
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& p = *nodes_[i];
-    if (p.name != "builtin:17" || p.initialized || p.node.inputs->size != 1 || p.node.outputs->size != 1 ||
-        p.builtin_blob.size() < sizeof(BuiltinParams))
+    if (p.name != kMaxPool2d || p.initialized || p.node.inputs->size != 1 || p.node.outputs->size != 1 ||
+        !Params(p))
       continue;
     const int x = p.node.inputs->data[0], y = p.node.outputs->data[0];
     const TfLiteIntArray* xd = tensors_[x].dims;
     if (tensors_[x].type != kTfLiteFloat32 || tensors_[y].type != kTfLiteFloat32 || !xd || xd->size != 4)
       continue;
     const int C = xd->data[3];
-    const size_t km = sole_consumer(y);
-    const int scale = const_op(km, i, "builtin:18", y, C);
-    if (scale < 0) continue;
+    const size_t km = SoleConsumer(y);
+    const int scale = PerChannelConstOp(km, kMul, y, C);
+    if (scale < 0 || km <= i) continue;
     const int t1 = nodes_[km]->node.outputs->data[0];
-    const size_t ka = sole_consumer(t1);
-    const int shift = const_op(ka, km, "builtin:0", t1, C);
-    if (shift < 0) continue;
-    const size_t kq = sole_consumer(nodes_[ka]->node.outputs->data[0]);
-    if (kq >= nodes_.size() || kq <= ka) continue;
-    const NodeRecord& q = *nodes_[kq];
-    if (q.name != "LceQuantize" || q.initialized || q.node.inputs->size != 1 || q.node.outputs->size != 1 ||
-        tensors_[q.node.outputs->data[0]].type != kTfLiteInt32)
-      continue;
-    std::vector<int> ins{x, scale, shift}, outs{q.node.outputs->data[0]};
-    LceB200IntArrayFree(p.node.inputs);
-    LceB200IntArrayFree(p.node.outputs);
-    p.node.inputs = MakeDims(ins);
-    p.node.outputs = MakeDims(outs);
+    const size_t ka = SoleConsumer(t1);
+    const int shift = PerChannelConstOp(ka, kAdd, t1, C);
+    if (shift < 0 || ka <= km) continue;
+    const size_t kq = SoleConsumer(nodes_[ka]->node.outputs->data[0]);
+    if (!IsQuantize(kq) || kq <= ka) continue;
+    SetNodeIO(p, {x, scale, shift}, {nodes_[kq]->node.outputs->data[0]});
     p.registration = PooledSignRegistration();   // builtin_data stays the pool's parameters
     p.name = "MAX_POOL_2D+MUL+ADD+LceQuantize";
-    for (size_t k : {kq, ka, km}) {   // the highest index first
-      NodeRecord& n = *nodes_[k];
-      LceB200IntArrayFree(n.node.inputs);
-      LceB200IntArrayFree(n.node.outputs);
-      LceB200IntArrayFree(n.node.temporaries);
-      LceB200IntArrayFree(n.node.intermediates);
-      nodes_.erase(nodes_.begin() + k);
-      ++removed;
-    }
+    EraseNodes({km, ka, kq});
+    removed += 3;
   }
   allocated_ = false;
   return removed;
 }
 
 int Graph::FuseQuantizedActivations() {
-  const size_t none = nodes_.size() + 1;
-  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
-  auto consumers = [&](int t) {
-    std::vector<size_t> c;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { c.push_back(k); break; }
-    return c;
-  };
-  auto sole_consumer = [&](int t) {
-    if (is_output(t)) return none;
-    const std::vector<size_t> c = consumers(t);
-    return c.size() == 1 ? c[0] : none;
-  };
-  auto params = [&](const NodeRecord& n) {
-    return n.builtin_blob.size() >= sizeof(BuiltinParams)
-               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())
-               : nullptr;
-  };
   // the host copy of a float constant, else nullptr (data.raw may be its device copy)
   auto float_const = [&](int t) -> const float* {
     if (t < 0 || tensors_[t].type != kTfLiteFloat32 || tensors_[t].allocation_type != kTfLiteMmapRo)
@@ -1167,7 +994,7 @@ int Graph::FuseQuantizedActivations() {
     if (k >= nodes_.size() || static_cast<long long>(k) <= after) return -1;
     const NodeRecord& n = *nodes_[k];
     if (n.name != name || n.initialized || n.node.inputs->size != (binary ? 2 : 1) ||
-        n.node.outputs->size != 1 || n.node.inputs->data[0] != x || !params(n) || params(n)->activation != 0 ||
+        n.node.outputs->size != 1 || n.node.inputs->data[0] != x || !Params(n) || Params(n)->activation != 0 ||
         tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32)
       return -1;
     if (binary) {
@@ -1189,8 +1016,8 @@ int Graph::FuseQuantizedActivations() {
   auto layer = [&](size_t k, size_t after, int t, int C, Layer* l) {
     if (k >= nodes_.size() || k <= after) return false;
     const NodeRecord& n = *nodes_[k];
-    const bool fc = n.name == "builtin:9";
-    if ((!fc && n.name != "builtin:3") || n.initialized || !params(n) || params(n)->activation != 0 ||
+    const bool fc = n.name == kFullyConnected;
+    if ((!fc && n.name != kConv2d) || n.initialized || !Params(n) || Params(n)->activation != 0 ||
         n.node.inputs->size < 2 || n.node.inputs->size > 3 || n.node.outputs->size != 1 ||
         n.node.inputs->data[0] != t || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32)
       return false;
@@ -1201,12 +1028,12 @@ int Graph::FuseQuantizedActivations() {
     const TfLiteIntArray* wd = tensors_[wt].dims;
     if (wd->size != (fc ? 2 : 4) || wd->data[wd->size - 1] != C) return false;
     // a FULLY_CONNECTED output becomes [rows,1,1,N]: the same bytes, but not the shape a caller reads
-    if (fc && is_output(n.node.outputs->data[0])) return false;
+    if (fc && IsGraphOutput(n.node.outputs->data[0])) return false;
     l->node = k;
     l->N = wd->data[0];
     l->kh = fc ? 1 : wd->data[1];
     l->kw = fc ? 1 : wd->data[2];
-    l->p = *params(n);
+    l->p = *Params(n);
     if (fc) {
       l->p.padding = LCE_PADDING_VALID;
       l->p.stride_h = l->p.stride_w = l->p.dilation_h = l->p.dilation_w = 1;
@@ -1253,35 +1080,29 @@ int Graph::FuseQuantizedActivations() {
     }
     return true;
   };
-  auto free_arrays = [&](NodeRecord& n) {
-    LceB200IntArrayFree(n.node.inputs);
-    LceB200IntArrayFree(n.node.outputs);
-    LceB200IntArrayFree(n.node.temporaries);
-    LceB200IntArrayFree(n.node.intermediates);
-  };
 
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
-    if (nodes_[i]->name != "builtin:55" || nodes_[i]->node.inputs->size != 2) continue;
+    if (nodes_[i]->name != kMaximum || nodes_[i]->node.inputs->size != 2) continue;
     const int x = nodes_[i]->node.inputs->data[0];
     if (x < 0 || tensors_[x].type != kTfLiteFloat32 || !tensors_[x].dims || tensors_[x].dims->size < 1) continue;
     const int C = tensors_[x].dims->data[tensors_[x].dims->size - 1];
     if (C <= 0 || C % 32 != 0) continue;
-    const int t1 = step(i, -1, "builtin:55", x, true, 0.0f);
+    const int t1 = step(i, -1, kMaximum, x, true, 0.0f);
     if (t1 < 0) continue;
-    const size_t kmin = sole_consumer(t1);
-    const int t2 = step(kmin, i, "builtin:57", t1, true, 1.0f);
+    const size_t kmin = SoleConsumer(t1);
+    const int t2 = step(kmin, i, kMinimum, t1, true, 1.0f);
     if (t2 < 0) continue;
-    const size_t kmul = sole_consumer(t2);
-    const int t3 = step(kmul, kmin, "builtin:18", t2, true, 3.0f);
+    const size_t kmul = SoleConsumer(t2);
+    const int t3 = step(kmul, kmin, kMul, t2, true, 3.0f);
     if (t3 < 0) continue;
-    const size_t kround = sole_consumer(t3);
-    const int t4 = step(kround, kmul, "builtin:116", t3, false, 0.0f);
+    const size_t kround = SoleConsumer(t3);
+    const int t4 = step(kround, kmul, kRound, t3, false, 0.0f);
     if (t4 < 0) continue;
-    const size_t kdiv = sole_consumer(t4);
-    const int t5 = step(kdiv, kround, "builtin:42", t4, true, 3.0f);
-    if (t5 < 0 || is_output(t5)) continue;
-    const std::vector<size_t> users = consumers(t5);
+    const size_t kdiv = SoleConsumer(t4);
+    const int t5 = step(kdiv, kround, kDiv, t4, true, 3.0f);
+    if (t5 < 0 || IsGraphOutput(t5)) continue;
+    const std::vector<size_t> users = Consumers(t5);
     if (users.empty()) continue;
     std::vector<Layer> layers(users.size());
     bool ok = true;
@@ -1290,17 +1111,17 @@ int Graph::FuseQuantizedActivations() {
     // the optional pool in front: x is read by the quantiser only
     size_t head = i;
     int src = x;
-    if (!is_output(x) && consumers(x).size() == 1 && tensors_[x].dims->size == 4)
+    if (SoleConsumer(x) == i && tensors_[x].dims->size == 4)
       for (size_t k = 0; k < i; ++k) {
         const NodeRecord& p = *nodes_[k];
-        if (p.name == "builtin:17" && !p.initialized && params(p) && p.node.inputs->size == 1 &&
+        if (p.name == kMaxPool2d && !p.initialized && Params(p) && p.node.inputs->size == 1 &&
             p.node.outputs->size == 1 && p.node.outputs->data[0] == x &&
             tensors_[p.node.inputs->data[0]].type == kTfLiteFloat32) {
           head = k;
           src = p.node.inputs->data[0];
         }
       }
-    const std::vector<int> xdims(tensors_[x].dims->data, tensors_[x].dims->data + tensors_[x].dims->size);
+    const std::vector<int> xdims = Ints(tensors_[x].dims);
     std::vector<int> pdims = xdims.size() == 4 ? xdims : std::vector<int>{static_cast<int>(count(x) / C), 1, 1, C};
     pdims[3] = 3 * (C / 32);
     const int planes = AddTensor(kTfLiteInt32, pdims, nullptr, 0, false, 0.0f, 0, names_[t5] + "_planes");
@@ -1308,13 +1129,9 @@ int Graph::FuseQuantizedActivations() {
     if (head == i) {   // no pool: filter_h == 0 tells the node so
       BuiltinParams bp;
       memset(&bp, 0, sizeof(bp));
-      h.builtin_blob.assign(reinterpret_cast<const uint8_t*>(&bp), reinterpret_cast<const uint8_t*>(&bp) + sizeof(bp));
-      h.node.builtin_data = h.builtin_blob.data();
+      SetBuiltinBlob(h, &bp, sizeof(bp));
     }
-    LceB200IntArrayFree(h.node.inputs);
-    LceB200IntArrayFree(h.node.outputs);
-    h.node.inputs = MakeDims({src});
-    h.node.outputs = MakeDims({planes});
+    SetNodeIO(h, {src}, {planes});
     h.registration = Quant2Registration();
     h.name = head == i ? "Quant2" : "MAX_POOL_2D+Quant2";
     for (const Layer& l : layers) {
@@ -1325,33 +1142,23 @@ int Graph::FuseQuantizedActivations() {
       const int b = AddTensor(kTfLiteFloat32, {l.N}, l.bias.data(), l.bias.size() * sizeof(float), false, 0.0f, 0,
                               names_[t5] + "_pbias");
       NodeRecord& n = *nodes_[l.node];
-      const int out = n.node.outputs->data[0];
-      LceB200IntArrayFree(n.node.inputs);
-      LceB200IntArrayFree(n.node.outputs);
-      n.node.inputs = MakeDims({planes, f, m, b, -1});
-      n.node.outputs = MakeDims({out});
-      n.custom_options = WriteFlexIntMap({{"channels_in", 3 * C},
-                                          {"dilation_height_factor", l.p.dilation_h},
-                                          {"dilation_width_factor", l.p.dilation_w},
-                                          {"fused_activation_function", 0},
-                                          {"pad_values", 1},
-                                          {"padding", l.p.padding},
-                                          {"stride_height", l.p.stride_h},
-                                          {"stride_width", l.p.stride_w}});
-      n.builtin_blob.clear();
-      n.node.builtin_data = nullptr;
-      n.node.custom_initial_data = n.custom_options.data();
-      n.node.custom_initial_data_size = static_cast<int>(n.custom_options.size());
+      SetNodeIO(n, {planes, f, m, b, -1}, {n.node.outputs->data[0]});
+      SetCustomOptions(n, WriteFlexIntMap({{"channels_in", 3 * C},
+                                           {"dilation_height_factor", l.p.dilation_h},
+                                           {"dilation_width_factor", l.p.dilation_w},
+                                           {"fused_activation_function", 0},
+                                           {"pad_values", 1},
+                                           {"padding", l.p.padding},
+                                           {"stride_height", l.p.stride_h},
+                                           {"stride_width", l.p.stride_w}}));
+      SetBuiltinBlob(n, nullptr, 0);
       n.registration = lce_b200_Register_BCONV_2D();
       n.name = "LceBconv2d";
     }
-    std::vector<size_t> gone{kdiv, kround, kmul, kmin};   // the highest index first
+    std::vector<size_t> gone{kmin, kmul, kround, kdiv};
     if (head != i) gone.push_back(i);
-    for (size_t k : gone) {
-      free_arrays(*nodes_[k]);
-      nodes_.erase(nodes_.begin() + k);
-      ++removed;
-    }
+    removed += static_cast<int>(gone.size());
+    EraseNodes(gone);
     i = head;
   }
   allocated_ = false;
@@ -1359,44 +1166,10 @@ int Graph::FuseQuantizedActivations() {
 }
 
 int Graph::FuseGroupedConvAffine() {
-  auto is_output = [&](int t) { return std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end(); };
-  // the node that alone reads t (as its first input), when t is not a graph output; else nodes_.size()
-  auto sole_consumer = [&](int t) {
-    if (is_output(t)) return nodes_.size();
-    size_t found = nodes_.size();
-    int n = 0;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { ++n; found = k; }
-    return (n == 1 && nodes_[found]->node.inputs->data[0] == t) ? found : nodes_.size();
-  };
-  auto params = [&](const NodeRecord& n) {
-    return n.builtin_blob.size() >= sizeof(BuiltinParams)
-               ? reinterpret_cast<const BuiltinParams*>(n.builtin_blob.data())
-               : nullptr;
-  };
-  // node k (after `after`) is the builtin `name` of x and a float constant of C values, shape [C] or
-  // [1, ..., 1, C], with a float output: returns that output, else -1
-  auto const_op = [&](size_t k, size_t after, const char* name, int x, int C) {
-    if (k >= nodes_.size() || k <= after) return -1;
-    const NodeRecord& n = *nodes_[k];
-    if (n.name != name || n.initialized || !params(n) || n.node.inputs->size != 2 || n.node.outputs->size != 1 ||
-        n.node.inputs->data[0] != x || tensors_[n.node.outputs->data[0]].type != kTfLiteFloat32)
-      return -1;
-    const int v = n.node.inputs->data[1];
-    if (v < 0) return -1;
-    const TfLiteTensor& t = tensors_[v];
-    if (t.type != kTfLiteFloat32 || t.allocation_type != kTfLiteMmapRo || t.dims->size < 1 ||
-        t.dims->data[t.dims->size - 1] != C)
-      return -1;
-    for (int d = 0; d + 1 < t.dims->size; ++d)
-      if (t.dims->data[d] != 1) return -1;
-    return n.node.outputs->data[0];
-  };
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& conv = *nodes_[i];
-    if (conv.name != "builtin:3" || conv.initialized || !params(conv) || params(conv)->activation != 0 ||
+    if (conv.name != kConv2d || conv.initialized || !Params(conv) || Params(conv)->activation != 0 ||
         conv.node.inputs->size < 2 || conv.node.inputs->size > 3 || conv.node.outputs->size != 1)
       continue;
     const int x = conv.node.inputs->data[0], w = conv.node.inputs->data[1];
@@ -1407,34 +1180,22 @@ int Graph::FuseGroupedConvAffine() {
     // grouped only: TFLite's groups = C_in / filter_in, exact, and dividing C_out
     const int cin = tensors_[x].dims->data[3], fin = tensors_[w].dims->data[3], C = tensors_[w].dims->data[0];
     if (fin < 1 || fin == cin || cin % fin != 0 || C % (cin / fin) != 0) continue;
-    const size_t km = sole_consumer(y);
-    const int u = const_op(km, i, "builtin:18", y, C);
-    if (u < 0 || params(*nodes_[km])->activation != 0) continue;
-    const size_t ka = sole_consumer(u);
-    const int z = const_op(ka, km, "builtin:0", u, C);
-    if (z < 0) continue;
-    std::vector<uint8_t> blob(2 * sizeof(BuiltinParams));
-    memcpy(blob.data(), params(conv), sizeof(BuiltinParams));
-    memcpy(blob.data() + sizeof(BuiltinParams), params(*nodes_[ka]), sizeof(BuiltinParams));
-    const std::vector<int> ins{x, w, conv.node.inputs->size > 2 ? conv.node.inputs->data[2] : -1,
-                               nodes_[km]->node.inputs->data[1], nodes_[ka]->node.inputs->data[1]};
-    LceB200IntArrayFree(conv.node.inputs);
-    LceB200IntArrayFree(conv.node.outputs);
-    conv.node.inputs = MakeDims(ins);
-    conv.node.outputs = MakeDims({z});
-    conv.builtin_blob = blob;
-    conv.node.builtin_data = conv.builtin_blob.data();
+    // the fused node takes over y and the MUL's output as the first operand alone
+    const size_t km = SoleReaderAsFirstInput(y);
+    const int scale = PerChannelConstOp(km, kMul, y, C);
+    if (scale < 0 || km <= i) continue;
+    const int u = nodes_[km]->node.outputs->data[0];
+    const size_t ka = SoleReaderAsFirstInput(u);
+    const int shift = PerChannelConstOp(ka, kAdd, u, C, /*any_activation=*/true);
+    if (shift < 0 || ka <= km) continue;
+    const BuiltinParams two[2] = {*Params(conv), *Params(*nodes_[ka])};
+    SetNodeIO(conv, {x, w, conv.node.inputs->size > 2 ? conv.node.inputs->data[2] : -1, scale, shift},
+              {nodes_[ka]->node.outputs->data[0]});
+    SetBuiltinBlob(conv, two, sizeof(two));
     conv.registration = GroupedConvAffineRegistration();
     conv.name = "CONV_2D+MUL+ADD";
-    for (size_t k : {ka, km}) {   // the later node first
-      NodeRecord& v = *nodes_[k];
-      LceB200IntArrayFree(v.node.inputs);
-      LceB200IntArrayFree(v.node.outputs);
-      LceB200IntArrayFree(v.node.temporaries);
-      LceB200IntArrayFree(v.node.intermediates);
-      nodes_.erase(nodes_.begin() + k);
-      ++removed;
-    }
+    EraseNodes({km, ka});
+    removed += 2;
   }
   allocated_ = false;
   return removed;
@@ -1445,53 +1206,28 @@ int Graph::FuseGroupedConvAffine() {
 // 16, and of QuickNetSmall, 8). The image is read once, as the bytes the host shipped; the
 // dequantised image and the first conv's map never reach HBM.
 int Graph::FuseStem() {
-  auto sole_consumer = [&](int t, size_t after) -> size_t {
-    if (std::find(outputs_.begin(), outputs_.end(), t) != outputs_.end()) return nodes_.size();
-    size_t found = nodes_.size();
-    int n = 0;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == t) { ++n; found = k; }
-    return (n == 1 && found > after && nodes_[found]->node.inputs->data[0] == t) ? found
-                                                                                 : nodes_.size();
-  };
-  auto bp = [](const NodeRecord& r) {
-    return reinterpret_cast<const BuiltinParams*>(r.builtin_blob.data());
-  };
   auto dims4 = [&](int t, int d) { return tensors_[t].dims->size == 4 ? tensors_[t].dims->data[d] : -1; };
-  auto erase_node = [&](size_t victim) {
-    NodeRecord& v = *nodes_[victim];
-    LceB200IntArrayFree(v.node.inputs);
-    LceB200IntArrayFree(v.node.outputs);
-    LceB200IntArrayFree(v.node.temporaries);
-    LceB200IntArrayFree(v.node.intermediates);
-    nodes_.erase(nodes_.begin() + victim);
-  };
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& c1 = *nodes_[i];
-    if (c1.name != "builtin:3" || c1.initialized || c1.node.inputs->size < 3 ||
-        c1.builtin_blob.size() < sizeof(BuiltinParams))
-      continue;
+    if (c1.name != kConv2d || c1.initialized || c1.node.inputs->size < 3 || !Params(c1)) continue;
+    const BuiltinParams p1 = *Params(c1);
     const int w1 = c1.node.inputs->data[1];
     const int x = c1.node.inputs->data[0];
     const int c1_out = dims4(w1, 0);
     // dims4(x, 3) != 3: a grouped convolution's filter has fewer input channels than x
     if ((c1_out != 16 && c1_out != 8) || dims4(w1, 1) != 3 || dims4(w1, 2) != 3 || dims4(w1, 3) != 3 ||
-        dims4(x, 3) != 3 ||
-        bp(c1)->stride_h != 2 || bp(c1)->stride_w != 2 || bp(c1)->dilation_h != 1 ||
-        bp(c1)->dilation_w != 1 || tensors_[x].type != kTfLiteFloat32 ||
+        dims4(x, 3) != 3 || p1.stride_h != 2 || p1.stride_w != 2 || p1.dilation_h != 1 ||
+        p1.dilation_w != 1 || tensors_[x].type != kTfLiteFloat32 ||
         tensors_[c1.node.outputs->data[0]].type != kTfLiteFloat32)
       continue;
-    const size_t di = sole_consumer(c1.node.outputs->data[0], i);
-    if (di >= nodes_.size()) continue;
+    const size_t di = SoleReaderAsFirstInput(c1.node.outputs->data[0]);
+    if (di == kNoNode || di <= i) continue;
     NodeRecord& dw = *nodes_[di];
-    if (dw.name != "builtin:4" || dw.initialized || dw.node.inputs->size < 3 ||
-        dw.builtin_blob.size() < sizeof(BuiltinParams))
-      continue;
+    if (dw.name != kDepthwiseConv2d || dw.initialized || dw.node.inputs->size < 3 || !Params(dw)) continue;
+    const BuiltinParams p2 = *Params(dw);
     const int w2 = dw.node.inputs->data[1];
-    if (dims4(w2, 1) != 3 || dims4(w2, 2) != 3 || dims4(w2, 3) != c1_out || bp(dw)->stride_h != 2 ||
-        bp(dw)->stride_w != 2 || bp(dw)->dilation_h != 1 || bp(dw)->dilation_w != 1 ||
-        bp(dw)->depth_multiplier != 1)
+    if (dims4(w2, 1) != 3 || dims4(w2, 2) != 3 || dims4(w2, 3) != c1_out || p2.stride_h != 2 ||
+        p2.stride_w != 2 || p2.dilation_h != 1 || p2.dilation_w != 1 || p2.depth_multiplier != 1)
       continue;
     // the kernel takes the filters and biases by value: they must be constants
     bool consts = true;
@@ -1500,38 +1236,26 @@ int Graph::FuseStem() {
     if (!consts) continue;
     // a DEQUANTIZE that feeds only this conv is folded in: the kernel reads the quantised image
     int src = x;
-    size_t qi = nodes_.size();
+    size_t qi = kNoNode;
     for (size_t k = 0; k < i; ++k) {
       NodeRecord& dq = *nodes_[k];
-      if (dq.name == "builtin:6" && !dq.initialized && dq.node.outputs->size == 1 &&
-          dq.node.outputs->data[0] == x && dq.node.inputs->size == 1 && sole_consumer(x, k) == i &&
+      if (dq.name == kDequantize && !dq.initialized && dq.node.outputs->size == 1 &&
+          dq.node.outputs->data[0] == x && dq.node.inputs->size == 1 && SoleReaderAsFirstInput(x) == i &&
           (tensors_[dq.node.inputs->data[0]].type == kTfLiteInt8 ||
            tensors_[dq.node.inputs->data[0]].type == kTfLiteUInt8)) {
         qi = k;
         src = dq.node.inputs->data[0];
       }
     }
-    std::vector<uint8_t> blob(2 * sizeof(BuiltinParams));
-    memcpy(blob.data(), bp(c1), sizeof(BuiltinParams));
-    memcpy(blob.data() + sizeof(BuiltinParams), bp(dw), sizeof(BuiltinParams));
-    std::vector<int> ins{src, w1, c1.node.inputs->data[2], w2, dw.node.inputs->data[2]};
-    std::vector<int> outs{dw.node.outputs->data[0]};
-    LceB200IntArrayFree(c1.node.inputs);
-    LceB200IntArrayFree(c1.node.outputs);
-    c1.node.inputs = MakeDims(ins);
-    c1.node.outputs = MakeDims(outs);
-    c1.builtin_blob = blob;
-    c1.node.builtin_data = c1.builtin_blob.data();
+    const BuiltinParams two[2] = {p1, p2};
+    SetNodeIO(c1, {src, w1, c1.node.inputs->data[2], w2, dw.node.inputs->data[2]}, {dw.node.outputs->data[0]});
+    SetBuiltinBlob(c1, two, sizeof(two));
     c1.registration = FusedStemRegistration();
-    c1.name = qi < nodes_.size() ? "DEQUANTIZE+CONV_2D+DEPTHWISE_CONV_2D" : "CONV_2D+DEPTHWISE_CONV_2D";
-    erase_node(di);                         // the later node first
-    int removed = 1;
-    if (qi < nodes_.size()) {
-      erase_node(qi);
-      ++removed;
-    }
-    allocated_ = false;
-    return removed;
+    c1.name = qi != kNoNode ? "DEQUANTIZE+CONV_2D+DEPTHWISE_CONV_2D" : "CONV_2D+DEPTHWISE_CONV_2D";
+    std::vector<size_t> absorbed{di};
+    if (qi != kNoNode) absorbed.push_back(qi);
+    EraseNodes(absorbed);
+    return static_cast<int>(absorbed.size());
   }
   return 0;
 }
@@ -1546,15 +1270,15 @@ int Graph::FuseConvQuantize() {
   int removed = 0;
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& conv = *nodes_[i];
-    if (conv.name != "builtin:3" || conv.initialized || conv.node.outputs->size != 1) continue;
+    if (conv.name != kConv2d || conv.initialized || conv.node.outputs->size != 1) continue;
     const int y = conv.node.outputs->data[0];
     if (tensors_[y].type != kTfLiteFloat32) continue;
-    if (conv.node.inputs->size >= 2 && conv.builtin_blob.size() >= sizeof(BuiltinParams)) {
+    if (conv.node.inputs->size >= 2 && Params(conv)) {
       const TfLiteIntArray* fd = tensors_[conv.node.inputs->data[1]].dims;
       const TfLiteIntArray* xd = tensors_[conv.node.inputs->data[0]].dims;
       // a grouped convolution (filter_in != the input's channels) runs its own kernel, without signs
       if (fd && xd && fd->size == 4 && xd->size == 4 && fd->data[3] != xd->data[3]) continue;
-      const auto* bp = reinterpret_cast<const BuiltinParams*>(conv.builtin_blob.data());
+      const BuiltinParams* bp = Params(conv);
       if (fd && fd->size == 4 &&
           !lce_b200_internal_conv_packs_alike(fd->data[1], fd->data[2], bp->stride_h, bp->stride_w,
                                               fd->data[3], fd->data[0]))
@@ -1567,17 +1291,10 @@ int Graph::FuseConvQuantize() {
         continue;
       const int packed = q.node.outputs->data[0];
       if (tensors_[packed].type != kTfLiteInt32) break;
-      std::vector<int> outs{y, packed};
-      LceB200IntArrayFree(conv.node.outputs);
-      conv.node.outputs = MakeDims(outs);
+      SetNodeIO(conv, Ints(conv.node.inputs), {y, packed});
       conv.name = "CONV_2D+LceQuantize";
-      LceB200IntArrayFree(q.node.inputs);
-      LceB200IntArrayFree(q.node.outputs);
-      LceB200IntArrayFree(q.node.temporaries);
-      LceB200IntArrayFree(q.node.intermediates);
-      nodes_.erase(nodes_.begin() + k);
+      EraseNode(k);
       ++removed;
-      allocated_ = false;
       break;
     }
   }
@@ -1596,80 +1313,49 @@ int Graph::FuseFloatGlue() {
   // RELU -> MEAN (the model heads): the mean applies the activation as it reads
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& relu = *nodes_[i];
-    if (relu.name != "builtin:19" || relu.initialized || relu.node.inputs->size != 1 || relu.node.outputs->size != 1)
+    if (relu.name != kRelu || relu.initialized || relu.node.inputs->size != 1 || relu.node.outputs->size != 1)
       continue;
     const int y = relu.node.outputs->data[0];
-    if (std::find(outputs_.begin(), outputs_.end(), y) != outputs_.end()) continue;
-    size_t mi = nodes_.size();
-    int n_cons = 0;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == y) { ++n_cons; mi = k; }
-    if (n_cons != 1 || mi <= i) continue;
+    const size_t mi = SoleReaderAsFirstInput(y);
+    if (mi == kNoNode || mi <= i) continue;
     NodeRecord& mean = *nodes_[mi];
-    if (mean.name != "builtin:40" || mean.initialized || mean.node.inputs->data[0] != y ||
-        mean.builtin_blob.size() < sizeof(BuiltinParams))
-      continue;
-    reinterpret_cast<BuiltinParams*>(mean.builtin_blob.data())->activation = 1;   // kTfLiteActRelu
-    mean.node.builtin_data = mean.builtin_blob.data();
+    if (mean.name != kMean || mean.initialized || !Params(mean)) continue;
+    BuiltinParams mp = *Params(mean);
+    mp.activation = 1;   // kTfLiteActRelu
+    SetBuiltinBlob(mean, &mp, sizeof(mp));
     mean.node.inputs->data[0] = relu.node.inputs->data[0];
     mean.name = "RELU+MEAN";
-    LceB200IntArrayFree(relu.node.inputs);
-    LceB200IntArrayFree(relu.node.outputs);
-    LceB200IntArrayFree(relu.node.temporaries);
-    LceB200IntArrayFree(relu.node.intermediates);
-    nodes_.erase(nodes_.begin() + i);
+    EraseNode(i);
     ++removed;
-    allocated_ = false;
     break;
   }
   for (size_t i = 0; i < nodes_.size(); ++i) {
     NodeRecord& pool = *nodes_[i];
-    if (pool.name != "builtin:17" || pool.initialized ||
-        pool.builtin_blob.size() < sizeof(BuiltinParams))
-      continue;
-    const auto* pp = reinterpret_cast<const BuiltinParams*>(pool.builtin_blob.data());
+    if (pool.name != kMaxPool2d || pool.initialized || !Params(pool)) continue;
+    const BuiltinParams* pp = Params(pool);
     if (pp->filter_h != 2 || pp->filter_w != 2 || pp->stride_h != 1 || pp->stride_w != 1 ||
         pp->padding != 1 /* VALID */ || pp->activation != 0)
       continue;
     const int y = pool.node.outputs->data[0];
-    if (std::find(outputs_.begin(), outputs_.end(), y) != outputs_.end()) continue;
-    size_t di = nodes_.size();
-    int n_cons = 0;
-    for (size_t k = 0; k < nodes_.size(); ++k)
-      for (int q = 0; q < nodes_[k]->node.inputs->size; ++q)
-        if (nodes_[k]->node.inputs->data[q] == y) { ++n_cons; di = k; }
-    if (n_cons != 1 || di <= i) continue;
+    const size_t di = SoleReaderAsFirstInput(y);
+    if (di == kNoNode || di <= i) continue;
     NodeRecord& dw = *nodes_[di];
-    if (dw.name != "builtin:4" || dw.node.inputs->data[0] != y ||
-        dw.builtin_blob.size() < sizeof(BuiltinParams))
-      continue;
-    const auto* dp = reinterpret_cast<const BuiltinParams*>(dw.builtin_blob.data());
+    if (dw.name != kDepthwiseConv2d || !Params(dw)) continue;
+    const BuiltinParams* dp = Params(dw);
     const TfLiteTensor& f = tensors_[dw.node.inputs->data[1]];
     if (f.dims->size != 4 || f.dims->data[1] != 3 || f.dims->data[2] != 3 ||
         (f.dims->data[3] & 3) || dp->dilation_h != 1 || dp->dilation_w != 1 ||
         dp->depth_multiplier != 1 || tensors_[y].type != kTfLiteFloat32)
       continue;
     // rewrite the pool node into the fused node; it takes the depthwise node's constants / output
-    std::vector<uint8_t> blob(2 * sizeof(BuiltinParams));
-    memcpy(blob.data(), pp, sizeof(BuiltinParams));
-    memcpy(blob.data() + sizeof(BuiltinParams), dp, sizeof(BuiltinParams));
-    std::vector<int> ins{pool.node.inputs->data[0], dw.node.inputs->data[1],
-                         dw.node.inputs->size > 2 ? dw.node.inputs->data[2] : -1};
-    std::vector<int> outs{dw.node.outputs->data[0]};
-    LceB200IntArrayFree(pool.node.inputs);
-    LceB200IntArrayFree(pool.node.outputs);
-    pool.node.inputs = MakeDims(ins);
-    pool.node.outputs = MakeDims(outs);
-    pool.builtin_blob = blob;
-    pool.node.builtin_data = pool.builtin_blob.data();
+    const BuiltinParams two[2] = {*pp, *dp};
+    SetNodeIO(pool, {pool.node.inputs->data[0], dw.node.inputs->data[1],
+                     dw.node.inputs->size > 2 ? dw.node.inputs->data[2] : -1},
+              {dw.node.outputs->data[0]});
+    SetBuiltinBlob(pool, two, sizeof(two));
     pool.registration = FusedPoolDepthwiseRegistration();
     pool.name = "MAX_POOL_2D+DEPTHWISE_CONV_2D";
-    LceB200IntArrayFree(dw.node.inputs);
-    LceB200IntArrayFree(dw.node.outputs);
-    LceB200IntArrayFree(dw.node.temporaries);
-    LceB200IntArrayFree(dw.node.intermediates);
-    nodes_.erase(nodes_.begin() + di);
+    EraseNode(di);
     ++removed;
   }
   allocated_ = false;

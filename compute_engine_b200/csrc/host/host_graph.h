@@ -21,6 +21,8 @@
 
 namespace lce_b200 {
 
+struct BuiltinParams;   // builtin_params.h
+
 // MutableOpResolver stand-in (tensorflow/lite/mutable_op_resolver.h:83): custom ops
 // by name, builtins by schema BuiltinOperator code.
 class OpResolver {
@@ -237,6 +239,36 @@ class Graph {
   TfLiteStatus PlanArena();
   void FreeArena();
   void RefreshContext();
+
+  // What the fusion passes ask of the graph. "No such node" is kNoNode, which no index equals and
+  // every `k < nodes_.size()` test refuses, before and after nodes are erased.
+  static constexpr size_t kNoNode = SIZE_MAX;
+  bool IsGraphOutput(int t) const;
+  std::vector<size_t> Consumers(int t) const;   // the nodes that read t, each once, in graph order
+  // The one node that reads t (in any of its inputs, in several of them too), t not a graph output.
+  size_t SoleConsumer(int t) const;
+  // The node that reads t when t is read by exactly one input of one node, that node's first, and
+  // is not a graph output: what a pass needs whose fused node takes over input 0 alone.
+  size_t SoleReaderAsFirstInput(int t) const;
+  bool ReadyBefore(int t, size_t i) const;      // t is a graph input or an output of a node before i
+  static bool SameDims(const TfLiteIntArray* a, const TfLiteIntArray* b);
+  static const BuiltinParams* Params(const NodeRecord& n);   // nullptr when the blob is too short
+  static int32_t Activation(const NodeRecord& n);            // 0 for a node without parameters
+  // Node k is the unprepared builtin `op`(x, v) with one float output, parameters, no fused
+  // activation (unless any_activation) and v a float constant of shape [C] or [1, ..., 1, C]:
+  // returns v, else -1 (also for k = kNoNode).
+  int PerChannelConstOp(size_t k, const char* op, int x, int C, bool any_activation = false) const;
+  // Node k is an unprepared LceQuantize with one input and one int32 output (false for kNoNode).
+  bool IsQuantize(size_t k) const;
+
+  // How the passes rewrite it. Each clears allocated_. A node they rewrite has not been prepared,
+  // so its temporaries are the ones its pass gives it.
+  void EraseNode(size_t k);
+  void EraseNodes(std::vector<size_t> ks);   // in any order, without duplicates
+  void SetNodeIO(NodeRecord& n, const std::vector<int>& inputs, const std::vector<int>& outputs,
+                 const std::vector<int>& temporaries = {});
+  void SetBuiltinBlob(NodeRecord& n, const void* bytes, size_t len);   // and node.builtin_data
+  void SetCustomOptions(NodeRecord& n, std::vector<uint8_t> options);  // and node.custom_initial_data
 
   bool device_arena_;
   std::vector<TfLiteTensor> tensors_;

@@ -193,8 +193,9 @@ def test_grouped_refusals(x_shape, w_shape, message):
 
 def _block(x_shape=(2, 10, 9, 32), filt=(32, 3, 3, 8), conv_act="NONE", mul_act="NONE", add_act="RELU",
            scale_shape=None, shift_shape=None, bias=False, conv_out_read_twice=False, conv_out_is_output=False,
-           mul_out_read_twice=False, mul_out_is_output=False, const_first=False):
-    """x -> CONV_2D -> MUL(scale) -> ADD(shift) [-> extra readers]"""
+           mul_out_read_twice=False, mul_out_is_output=False, const_first=False, square=False):
+    """x -> CONV_2D -> MUL(scale) -> ADD(shift) [-> extra readers]; `square` makes the MUL read the
+    convolution's output as both operands (one reading node, two reading inputs)."""
     rng = np.random.default_rng(3)
     C = filt[0]
     m = TFLiteModel()
@@ -208,7 +209,7 @@ def _block(x_shape=(2, 10, 9, 32), filt=(32, 3, 3, 8), conv_act="NONE", mul_act=
     shift = rng.uniform(-0.5, 0.5, shift_shape or (C,)).astype(F32)
     u = m.add_tensor("u", x_shape[:3] + (C,))
     sc = m.add_tensor("scale", None, data=scale)
-    m.add_op("MUL", [sc, y] if const_first else [y, sc], [u], activation=mul_act)
+    m.add_op("MUL", [y, y] if square else [sc, y] if const_first else [y, sc], [u], activation=mul_act)
     z = m.add_tensor("z", x_shape[:3] + (C,))
     m.add_op("ADD", [u, m.add_tensor("shift", None, data=shift)], [z], activation=add_act)
     m.outputs = [z]
@@ -245,14 +246,15 @@ def test_block_fuses(kw):
 
 @pytest.mark.parametrize("variant", ["ungrouped", "conv_activation", "mul_activation", "scale_not_per_channel",
                                      "shift_not_per_channel", "scale_2d", "conv_out_read_twice", "conv_out_is_output",
-                                     "mul_out_read_twice", "mul_out_is_output", "constant_first"])
+                                     "mul_out_read_twice", "mul_out_is_output", "constant_first",
+                                     "mul_reads_conv_out_twice"])
 def test_block_refusals(variant):
     kw = {"ungrouped": dict(filt=(32, 3, 3, 32)), "conv_activation": dict(conv_act="RELU"),
           "mul_activation": dict(mul_act="RELU"), "scale_not_per_channel": dict(scale_shape=(1,)),
           "shift_not_per_channel": dict(shift_shape=(1,)), "scale_2d": dict(scale_shape=(2, 32)),
           "conv_out_read_twice": dict(conv_out_read_twice=True), "conv_out_is_output": dict(conv_out_is_output=True),
           "mul_out_read_twice": dict(mul_out_read_twice=True), "mul_out_is_output": dict(mul_out_is_output=True),
-          "constant_first": dict(const_first=True)}[variant]
+          "constant_first": dict(const_first=True), "mul_reads_conv_out_twice": dict(square=True)}[variant]
     g = H.HostGraph.from_tflite(_block(**kw), device_arena=False)
     before = _names(g)
     assert g.fuse_grouped_conv_affine() == 0 and _names(g) == before

@@ -210,9 +210,10 @@ def test_other_models_bytes_are_unchanged():
 
 
 def _pooled_block(x_shape=(2, 9, 9, 40), kind="MAX_POOL_2D", k=3, s=2, padding="VALID", pool_act="NONE",
-                  scale_shape=None, mul_act="NONE", add_act="NONE", output=None, extra_reader=None):
+                  scale_shape=None, mul_act="NONE", add_act="NONE", output=None, extra_reader=None, square=False):
     """x -> pool -> MUL(scale) -> ADD(shift) -> LceQuantize; `output` makes "y" (pool), "u" (MUL) or
-    "v" (ADD) a graph output too, `extra_reader` gives that tensor a RELU reader."""
+    "v" (ADD) a graph output too, `extra_reader` gives that tensor a RELU reader, `square` makes the
+    MUL read the pool's output as both operands (one reading node, two reading inputs)."""
     rng = np.random.default_rng(5)
     b, h, w, c = x_shape
     oh = -(-h // s) if padding == "SAME" else (h - k) // s + 1
@@ -225,7 +226,7 @@ def _pooled_block(x_shape=(2, 9, 9, 40), kind="MAX_POOL_2D", k=3, s=2, padding="
     shift = m.add_tensor("shift", None, data=rng.uniform(-0.5, 0.5, (c,)).astype(np.float32))
     q = m.add_tensor("q", ys[:3] + (L.cdiv(c, 32),), np.int32)
     m.add_op(kind, [x], [t["y"]], padding=padding, stride=(s, s), filter=(k, k), activation=pool_act)
-    m.add_op("MUL", [t["y"], scale], [t["u"]], activation=mul_act)
+    m.add_op("MUL", [t["y"], t["y"] if square else scale], [t["u"]], activation=mul_act)
     m.add_op("ADD", [t["u"], shift], [t["v"]], activation=add_act)
     m.add_op("LceQuantize", [t["v"]], [q], custom_options=b"")
     m.inputs, m.outputs = [x], [q]
@@ -246,7 +247,7 @@ def test_pooled_block_fuses():
 
 @pytest.mark.parametrize("variant", ["pool_read_twice", "scale_not_per_channel", "mul_activation",
                                      "add_activation", "pool_is_a_graph_output", "mul_is_a_graph_output",
-                                     "add_is_a_graph_output", "average_pool"])
+                                     "add_is_a_graph_output", "average_pool", "mul_reads_pool_twice"])
 def test_pooled_block_refusals(variant):
     kw = {"pool_read_twice": dict(extra_reader="y"),
           "scale_not_per_channel": dict(scale_shape=(2, 4, 4, 40)),
@@ -255,7 +256,8 @@ def test_pooled_block_refusals(variant):
           "pool_is_a_graph_output": dict(output="y"),
           "mul_is_a_graph_output": dict(output="u"),
           "add_is_a_graph_output": dict(output="v"),
-          "average_pool": dict(kind="AVERAGE_POOL_2D")}[variant]
+          "average_pool": dict(kind="AVERAGE_POOL_2D"),
+          "mul_reads_pool_twice": dict(square=True)}[variant]
     blob = _pooled_block(**kw)
     g = H.HostGraph.from_tflite(blob, device_arena=True)
     before = _names(g)
