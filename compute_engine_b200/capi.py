@@ -73,6 +73,16 @@ def _gate_desc(gate, alpha=None, sign_scale=None, sign_shift=None):
     return GateDesc(*[None if v is None else v.data_ptr() for v in vecs]), vecs
 
 
+class ScaleDesc(C.Structure):
+    """lce_scale_desc: device pointers; scale [OH * OW, C] is required, None = the op is absent."""
+    _fields_ = [("scale", C.c_void_p), ("sign_scale", C.c_void_p), ("sign_shift", C.c_void_p)]
+
+
+def _scale_desc(scale, sign_scale=None, sign_shift=None):
+    vecs = [None if v is None else _dev(v, torch.float32) for v in (scale, sign_scale, sign_shift)]
+    return ScaleDesc(*[None if v is None else v.data_ptr() for v in vecs]), vecs
+
+
 class BgemmEpilogue(C.Structure):
     _fields_ = [("out_type", C.c_int32), ("clamp_min", C.c_int32),
                 ("clamp_max", C.c_int32), ("multiplier", C.c_void_p),
@@ -87,8 +97,9 @@ EXPORTS = [
     "lce_b200_bconv2d_set_zero_padding_mode", "lce_b200_path_counts", "lce_b200_tc_debug",
     "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_fused_chain",
     "lce_b200_bconv2d_run_fused_pair",
-    "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add",
-    "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_logistic",
+    "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_fused_scale",
+    "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add",
+    "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_scale_sign", "lce_b200_f32_logistic",
     "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
     "lce_b200_f32_maximum", "lce_b200_f32_minimum", "lce_b200_f32_div", "lce_b200_f32_round",
     "lce_b200_f32_quant2_planes", "lce_b200_f32_grouped_conv2d",
@@ -234,6 +245,24 @@ def gate_sign(x: torch.Tensor, gate, residual=None, activation=0, alpha=None, si
     _check(lib().lce_b200_f32_gate_sign(_p(x), C.byref(desc), _p(res), C.c_int(activation),
                                         C.c_int64(b), C.c_int64(x.numel() // max(b * ch, 1)),
                                         C.c_int(ch), _p(o), _p(pk), _stream()))
+    return o, pk
+
+
+def scale_sign(x: torch.Tensor, scale, residual=None, activation=0, sign_scale=None, sign_shift=None,
+               out=True, packed=True):
+    """XNOR-Net++'s scaled tail over x [B, H, W, C] with scale [H, W, C] (or [1, H, W, C]):
+    act(x * scale + residual), and the signs of that * sign_scale + sign_shift. `out` may also be
+    a tensor to write into (x itself, for one in place). Returns (out | None, packed | None)."""
+    x = _dev(x, torch.float32)
+    b, ch = x.shape[0], x.shape[-1]
+    desc, _keep = _scale_desc(scale, sign_scale, sign_shift)
+    res = None if residual is None else _dev(residual, torch.float32)
+    o = out if isinstance(out, torch.Tensor) else (torch.empty_like(x) if out else None)
+    pk = torch.empty(x.shape[:-1] + (cdiv(ch, 32),), dtype=torch.int32,
+                     device=x.device) if packed else None
+    _check(lib().lce_b200_f32_scale_sign(_p(x), C.byref(desc), _p(res), C.c_int(activation),
+                                         C.c_int64(b), C.c_int64(x.numel() // max(b * ch, 1)),
+                                         C.c_int(ch), _p(o), _p(pk), _stream()))
     return o, pk
 
 
@@ -423,6 +452,24 @@ class BConv2d:
         _check(lib().lce_b200_bconv2d_run_fused_gate(self._h, _p(x), C.byref(desc), _p(res),
                                                      C.c_int(add_activation), _p(out), _p(pk),
                                                      _stream()))
+        return out, pk
+
+    def run_fused_scale(self, x: torch.Tensor, scale, residual=None, add_activation=0, sign_scale=None,
+                        sign_shift=None, packed=True, out=None):
+        """lce_b200_bconv2d_run_fused_scale on bitpacked x with scale [OH, OW, C] (or [1, OH, OW, C]):
+        returns (float out, packed signs | None). `out` may be given (the C-ABI refuses one that
+        overlaps the residual or the scale)."""
+        x = _dev(x, torch.int32)
+        if tuple(x.shape[:3]) != (self.desc.batch, self.desc.in_h, self.desc.in_w):
+            self.set_input_shape(*x.shape[:3])
+        out = self._alloc(x, out)
+        pk = torch.empty(out.shape[:3] + (cdiv(out.shape[3], 32),), dtype=torch.int32,
+                         device=x.device) if packed else None
+        res = None if residual is None else _dev(residual, torch.float32)
+        desc, _keep = _scale_desc(scale, sign_scale, sign_shift)
+        _check(lib().lce_b200_bconv2d_run_fused_scale(self._h, _p(x), C.byref(desc), _p(res),
+                                                      C.c_int(add_activation), _p(out), _p(pk),
+                                                      _stream()))
         return out, pk
 
     def run_slice(self, x: torch.Tensor, out: torch.Tensor, offset: int = 0):

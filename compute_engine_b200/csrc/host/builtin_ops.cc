@@ -446,12 +446,13 @@ int64_t PreluAlphaCount(const TfLiteTensor* x, const TfLiteTensor* a) {
 }
 
 // ------------------------------ ADD / MUL / RELU ------------------------------ //
-// The kernels compute out[i] = a[i] (op) b[i % Count(b)], which is TFLite's broadcast for two shapes
-// of b only: a's own shape, and [C] (a's last dimension) with any leading 1s. A b of higher rank
+// The kernels compute out[i] = a[i] (op) b[i % Count(b)], which is TFLite's broadcast whenever b's
+// shape with leading 1s dropped is a's trailing dimensions: a's own shape, [C] (a's last
+// dimension), or a per-position [1,H,W,C], [H,W,C], [W,C] (XNOR-Net++'s scale). A b of higher rank
 // would make the output's rank b's. A b of one element (a scalar, or all dimensions 1) is read as
-// b[0] for every element. MUL's one further broadcast: a [B,H,W,C] tensor by a per-image,
-// per-channel [B,1,1,C] one (the channel gate of Real-to-Binary Net); runs as
-// lce_b200_f32_gate_sign with only the gate set.
+// b[0] for every element. MAXIMUM, MINIMUM and DIV take only the first two and the one element.
+// MUL's one further broadcast: a [B,H,W,C] tensor by a per-image, per-channel [B,1,1,C] one (the
+// channel gate of Real-to-Binary Net); runs as lce_b200_f32_gate_sign with only the gate set.
 bool ImageChannelBroadcast(const TfLiteTensor* a, const TfLiteTensor* b) {
   return a->dims->size == 4 && b->dims->size == 4 && b->dims->data[0] == a->dims->data[0] &&
          b->dims->data[1] == 1 && b->dims->data[2] == 1 && b->dims->data[3] == a->dims->data[3];
@@ -463,12 +464,16 @@ bool PlainBroadcast(const TfLiteTensor* a, const TfLiteTensor* b) {
   return a->dims->size > 0 && b->dims->size <= a->dims->size && nb > 0 &&
          (nb == Count(a) || nb == a->dims->data[a->dims->size - 1] || nb == 1);
 }
+// b's shape with leading 1s dropped is a's trailing dimensions, of at most a's rank
+bool TrailingBroadcast(const TfLiteTensor* a, const TfLiteTensor* b) {
+  return a->dims->size > 0 && b->dims->size <= a->dims->size && PreluAlphaCount(a, b) > 0;
+}
 template <bool MUL>
 TfLiteStatus EltPrepare(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* a = T(c, n->inputs, 0);
   const TfLiteTensor* b = T(c, n->inputs, 1);
   B_ENSURE(c, a && b, "ADD/MUL: two inputs required");
-  const bool plain = PlainBroadcast(a, b);
+  const bool plain = TrailingBroadcast(a, b);
   if (MUL)
     B_ENSURE(c, plain || (Count(b) > 0 && ImageChannelBroadcast(a, b)),
              "MUL: only same-shape, last-dimension or [B,H,W,C] x [B,1,1,C] broadcast is supported");
@@ -485,7 +490,15 @@ TfLiteStatus EltInvoke(TfLiteContext* c, TfLiteNode* n) {
   TfLiteTensor* out = T(c, n->outputs, 0);
   B_ENSURE(c, OnDevice(b->data.raw), "float builtins need device-resident operands");
   const int64_t na = Count(a);
-  if (MUL && !PlainBroadcast(a, b)) {   // [B,1,1,C] (EltPrepare)
+  if (MUL && TrailingBroadcast(a, b) && !PlainBroadcast(a, b)) {   // per position: [1,H,W,C], [W,C], ...
+    const lce_scale_desc scale{b->data.f, nullptr, nullptr};
+    const int ch = a->dims->data[a->dims->size - 1];
+    const int64_t nb = Count(b);
+    B_CAPI(c, lce_b200_f32_scale_sign(a->data.f, &scale, nullptr, P(n).activation, na / nb, nb / ch, ch,
+                                      out->data.f, nullptr, lce_b200_get_stream()));
+    return kTfLiteOk;
+  }
+  if (MUL && !TrailingBroadcast(a, b)) {   // [B,1,1,C] (EltPrepare)
     const lce_gate_desc gate{b->data.f, nullptr, nullptr, nullptr};
     const int ch = a->dims->data[3];
     B_CAPI(c, lce_b200_f32_gate_sign(a->data.f, &gate, nullptr, P(n).activation, a->dims->data[0],

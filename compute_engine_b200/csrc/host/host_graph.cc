@@ -648,6 +648,91 @@ int Graph::FuseChannelGates() {
   return removed;
 }
 
+extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_SCALE(const TfLiteRegistration* original);
+
+int Graph::FuseSpatialScales() {
+  if (!device_arena_) return 0;
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    NodeRecord& b = *nodes_[i];
+    if (b.name != "LceBconv2d" || b.initialized || b.node.inputs->size != 5 || b.node.outputs->size != 1)
+      continue;
+    TfLiteRegistration* scale_reg = lce_b200_internal_Register_BCONV_2D_SCALE(b.registration);
+    if (scale_reg == nullptr) continue;
+    const int y = b.node.outputs->data[0];
+    const TfLiteIntArray* yd = tensors_[y].dims;
+    if (tensors_[y].type != kTfLiteFloat32 || !yd || yd->size != 4) continue;
+    const int C = yd->data[3];
+    // MUL(y, gamma): gamma a float constant [1, OH, OW, C] or [OH, OW, C], no fused activation
+    const size_t km = SoleConsumer(y);
+    if (km == kNoNode) continue;
+    const NodeRecord& m = *nodes_[km];
+    if (m.name != kMul || m.initialized || m.node.inputs->size != 2 || m.node.outputs->size != 1 ||
+        m.node.inputs->data[0] != y || tensors_[m.node.outputs->data[0]].type != kTfLiteFloat32 ||
+        !Params(m) || Activation(m) != 0)
+      continue;
+    const int gamma = m.node.inputs->data[1];
+    if (gamma < 0 || gamma == y) continue;
+    const TfLiteTensor& gt = tensors_[gamma];
+    const TfLiteIntArray* gd = gt.dims;
+    if (gt.type != kTfLiteFloat32 || gt.allocation_type != kTfLiteMmapRo || !gd ||
+        !(gd->size == 3 || (gd->size == 4 && gd->data[0] == 1)))
+      continue;
+    const int lead = gd->size - 3;
+    if (gd->data[lead] != yd->data[1] || gd->data[lead + 1] != yd->data[2] || gd->data[lead + 2] != C)
+      continue;
+    // ADD(t, shortcut), the shortcut a computed float tensor of y's shape; its activation applies
+    const int t1 = m.node.outputs->data[0];
+    const size_t ka = SoleConsumer(t1);
+    if (ka == kNoNode) continue;
+    const NodeRecord& a = *nodes_[ka];
+    if (a.name != kAdd || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1)
+      continue;
+    const int in0 = a.node.inputs->data[0], in1 = a.node.inputs->data[1];
+    if (in0 == in1 || (in0 != t1 && in1 != t1)) continue;
+    const int r = in0 == t1 ? in1 : in0;
+    if (r < 0 || tensors_[r].type != kTfLiteFloat32 || tensors_[r].allocation_type == kTfLiteMmapRo ||
+        !SameDims(tensors_[r].dims, yd) || !ReadyBefore(r, i))
+      continue;
+    const int o = a.node.outputs->data[0];
+    if (tensors_[o].type != kTfLiteFloat32) continue;
+    const int32_t add_act = Activation(a);
+    std::vector<size_t> absorbed{km, ka};
+    // the next block's BatchNorm and sign: MUL(o, scale) -> ADD(shift) -> LceQuantize, when the
+    // convolution is ungrouped (the fused sign-pack needs groups == 1); o may have other readers
+    int sc = -1, sh = -1, packed = -1;
+    const TfLiteIntArray* xs = tensors_[b.node.inputs->data[0]].dims;
+    const TfLiteIntArray* fs = tensors_[b.node.inputs->data[1]].dims;
+    const bool ungrouped = xs && fs && xs->size == 4 && fs->size == 4 && xs->data[3] == fs->data[3];
+    for (size_t c : Consumers(o)) {
+      if (!ungrouped) break;
+      const int v1 = PerChannelConstOp(c, kMul, o, C);
+      if (v1 < 0) continue;
+      const int t3 = nodes_[c]->node.outputs->data[0];
+      const size_t k2 = SoleConsumer(t3);
+      const int v2 = PerChannelConstOp(k2, kAdd, t3, C);
+      if (v2 < 0) continue;
+      const size_t kq = SoleConsumer(nodes_[k2]->node.outputs->data[0]);
+      if (!IsQuantize(kq)) continue;
+      sc = v1; sh = v2; packed = nodes_[kq]->node.outputs->data[0];
+      absorbed.insert(absorbed.end(), {c, k2, kq});
+      break;
+    }
+    std::vector<int> ins = Ints(b.node.inputs);
+    ins.insert(ins.end(), {r, gamma, sc, sh});
+    std::vector<int> outs{o};
+    if (packed >= 0) outs.push_back(packed);
+    SetNodeIO(b, ins, outs);
+    b.registration = scale_reg;
+    SetBuiltinBlob(b, &add_act, sizeof(add_act));
+    b.name = packed >= 0 ? "LceBconv2d+MUL+ADD+MUL+ADD+LceQuantize" : "LceBconv2d+MUL+ADD";
+    removed += static_cast<int>(absorbed.size());
+    EraseNodes(absorbed);   // all after node i
+  }
+  allocated_ = false;
+  return removed;
+}
+
 extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_DENSE(const TfLiteRegistration* original);
 extern "C" int lce_b200_internal_slice_takes(const lce_bconv2d_desc* d);   // lce_b200.cu
 

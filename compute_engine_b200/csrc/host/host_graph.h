@@ -99,6 +99,22 @@ class Graph {
   // number of nodes removed.
   int FuseChannelGates();
 
+  // XNOR-Net++'s scaled block tail
+  //   LceBconv2d(float y) -> MUL(y, gamma) -> ADD(shortcut)
+  //     [-> MUL(scale) -> ADD(shift) -> LceQuantize, the next block's BatchNorm and sign]
+  // becomes one node "LceBconv2d+MUL+ADD[+MUL+ADD+LceQuantize]" (lce_b200_bconv2d_run_fused_scale):
+  // inputs [in, filter, mul, bias, thr, shortcut, gamma, scale, shift (-1 when the sign tail is
+  // absent)], outputs [sum, packed signs?]. Only when gamma is a float constant of shape
+  // [1, OH, OW, C] or [OH, OW, C] (one value per output position and channel), scale / shift are
+  // float constants of shape [C] or [1, ..., 1, C], the MULs and the BatchNorm ADD have no fused
+  // activation (the shortcut ADD's, any, is applied), y, the MUL's output and the BatchNorm's
+  // intermediates have a single consumer and are not graph outputs (the sum may have other
+  // readers), and the shortcut exists before the convolution runs; otherwise the graph is left as
+  // it is. Run before FuseFloatGlue and FuseActivationChains, which would otherwise take the
+  // BatchNorm's ADD -> LceQuantize as a lone RSign. Bit-identical. Returns the number of nodes
+  // removed.
+  int FuseSpatialScales();
+
   // BinaryAlexNet's and XNOR-Net's pooled BatchNorm and sign
   //   MAX_POOL_2D(x) -> MUL(scale) -> ADD(shift) -> LceQuantize
   // becomes one node "MAX_POOL_2D+MUL+ADD+LceQuantize" (lce_b200_f32_maxpool_affine_sign): inputs

@@ -769,6 +769,56 @@ TfLiteStatus GateEval(TfLiteContext* context, TfLiteNode* node) {
 }
 
 // ------------------------------------------------------------------------- //
+// XNOR-Net++'s scaled block in one node (Graph::FuseSpatialScales):
+// [in, filter, mul, bias, thr, residual, scale [1,OH,OW,C] or [OH,OW,C], sign_scale, sign_shift]
+// -> [out, packed_out?]; absent vectors are -1; builtin_data: the shortcut ADD's activation.
+// ------------------------------------------------------------------------- //
+template <KernelType kt>
+TfLiteStatus ScalePrepare(TfLiteContext* context, TfLiteNode* node) {
+  LCE_ENSURE(context, node->inputs->size == 9);
+  GateBlockView v(node);
+  if (BconvPrepare<kt, true>(context, &v.node) != kTfLiteOk) return kTfLiteError;
+  const lce_bconv2d_desc& d = static_cast<BconvOpData*>(node->user_data)->desc;
+  const TfLiteTensor* out = GetOutput(context, node, 0);
+  const TfLiteTensor* scale = GetInput(context, node, 6);
+  const int r = scale ? NumDims(scale) : 0;
+  LCE_ENSURE_MSG(context,
+                 scale != nullptr && scale->type == kTfLiteFloat32 && (r == 3 || (r == 4 && Dim(scale, 0) == 1)) &&
+                     Dim(scale, r - 3) == Dim(out, 1) && Dim(scale, r - 2) == Dim(out, 2) &&
+                     Dim(scale, r - 1) == d.channels_out,
+                 "scaled LceBconv2d: the scale must be a float32 [1, out_h, out_w, channels_out] tensor");
+  for (int k = 7; k < 9; ++k) {
+    const TfLiteTensor* t = GetInput(context, node, k);
+    LCE_ENSURE(context, t == nullptr || (t->type == kTfLiteFloat32 && NumElements(t) == d.channels_out));
+  }
+  return kTfLiteOk;
+}
+
+TfLiteStatus ScaleEval(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<BconvOpData*>(node->user_data);
+  if (BconvEnsurePlan(context, node) != kTfLiteOk) return kTfLiteError;
+  const TfLiteTensor* input = GetInput(context, node, 0);
+  const TfLiteTensor* residual = GetInput(context, node, 5);
+  const TfLiteTensor* scale = GetInput(context, node, 6);
+  TfLiteTensor* output = GetOutput(context, node, 0);
+  TfLiteTensor* packed = node->outputs->size > 1 ? GetOutput(context, node, 1) : nullptr;
+  int add_act = LCE_ACT_NONE;
+  if (node->builtin_data) add_act = *static_cast<const int32_t*>(node->builtin_data);
+  LCE_ENSURE_MSG(context, OnDevice(input->data.raw) && OnDevice(output->data.raw) &&
+                              OnDevice(residual->data.raw) && OnDevice(scale->data.raw),
+                 "scaled LceBconv2d needs a device arena");
+  auto vec = [&](int k) {
+    const TfLiteTensor* v = GetInput(context, node, k);
+    return v ? v->data.f : nullptr;
+  };
+  const lce_scale_desc sd{scale->data.f, vec(7), vec(8)};
+  LCE_ENSURE_CAPI(context, lce_b200_bconv2d_run_fused_scale(
+                               op->plan, input->data.i32, &sd, residual->data.f, add_act,
+                               output->data.f, packed ? packed->data.i32 : nullptr, g_stream));
+  return kTfLiteOk;
+}
+
+// ------------------------------------------------------------------------- //
 // A BinaryDenseNet dense layer or a MeliusNet improvement layer in one node
 // (Graph::FuseDenseBlocks): [src, scale, shift, filter, mul, bias, thr] -> [X]. X is the block's
 // final map [B, H, W, C_L]; builtin_data: int32 {C_L, the layer kind (kDenseLayer /
@@ -902,6 +952,12 @@ TfLiteRegistration* BconvGateRegistration() {
 }
 
 template <KernelType kt>
+TfLiteRegistration* BconvScaleRegistration() {
+  static TfLiteRegistration r = {BconvInit, BconvFree, ScalePrepare<kt>, ScaleEval};
+  return &r;
+}
+
+template <KernelType kt>
 TfLiteRegistration* BconvPairRegistration() {
   static TfLiteRegistration r = {PairInit, PairFree, PairPrepare<kt>, PairEval};
   return &r;
@@ -970,6 +1026,19 @@ TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_GATE(const TfLiteRegistr
     return BconvGateRegistration<KernelType::kOptimizedBGEMM>();
   if (original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
     return BconvGateRegistration<KernelType::kOptimizedIndirectBGEMM>();
+  return nullptr;
+}
+
+// host-internal: the scaled-block node created by Graph::FuseSpatialScales from a plain LceBconv2d
+// node of this registration (nullptr: not one of this library's LceBconv2d registrations)
+TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_SCALE(const TfLiteRegistration* original) {
+  if (original == BconvRegistration<KernelType::kCuda>()) return BconvScaleRegistration<KernelType::kCuda>();
+  if (original == BconvRegistration<KernelType::kReference>())
+    return BconvScaleRegistration<KernelType::kReference>();
+  if (original == BconvRegistration<KernelType::kOptimizedBGEMM>())
+    return BconvScaleRegistration<KernelType::kOptimizedBGEMM>();
+  if (original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
+    return BconvScaleRegistration<KernelType::kOptimizedIndirectBGEMM>();
   return nullptr;
 }
 

@@ -192,19 +192,21 @@ size_t imma_smem_budget(int V, bool b1) {
   return (227u * 1024u / ctas - 1024u - 256u) & ~size_t{127};
 }
 
-template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false>
+template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
+          bool SPATIAL = false>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(imma_smem_budget(V, B1))));
-  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE><<<grid, lce::kIThreads, smem, s>>>(p);
+  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL><<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
 // Epilogue tails of the float output beyond run_fused's (bconv_run_impl decides).
-enum class Tail { kNone, kChain, kGate, kSlice };   // p.chain / p.gate / p.out_stride in the epilogue
+// kScale: p.gate indexed by position within the image (lce_b200_bconv2d_run_fused_scale)
+enum class Tail { kNone, kChain, kGate, kScale, kSlice };   // p.chain / p.gate / p.out_stride in the epilogue
 
 template <int V>
 int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, dim3 grid,
@@ -216,6 +218,10 @@ int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, d
   if (tail == Tail::kGate) {
     if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, true>(p, grid, smem, s);
     return launch_imma_vo<V, LCE_OUT_FLOAT, false, false, true>(p, grid, smem, s);
+  }
+  if (tail == Tail::kScale) {
+    if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, true, false, true>(p, grid, smem, s);
+    return launch_imma_vo<V, LCE_OUT_FLOAT, false, false, true, false, true>(p, grid, smem, s);
   }
   if (tail == Tail::kSlice) {
     if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, false, true>(p, grid, smem, s);
@@ -278,7 +284,7 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, Tail tail = Ta
       default: return launch_imma_v<1>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
     }
   }
-  if (tail != Tail::kNone) return fail("bconv2d: the chain, gate and slice epilogues need the mma.sync kernel");
+  if (tail != Tail::kNone) return fail("bconv2d: the chain, gate, scale and slice epilogues need the mma.sync kernel");
   if (c.tc_ok) {
     // wgmma inner product: persistent 128 x BN tiles
     const int rc = tc_launch(c, p, s);
@@ -1100,7 +1106,7 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
                           const float* residual, int residual_act, int32_t* packed_out,
                           const lce_chain_desc* chain, void* stream,
                           const lce_gate_desc* gate = nullptr, int64_t out_stride = 0,
-                          float* scratch = nullptr) {
+                          float* scratch = nullptr, bool gate_per_position = false) {
   const lce_bconv2d_desc& d = plan->d;
   GemmCore& c = plan->core;
   cudaStream_t s = as_stream(stream);
@@ -1156,17 +1162,24 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     return lce_b200_f32_chain_sign(out, chain, p.M, c.cout, out, packed_out, stream);
   }
   if (gate != nullptr) {
+    // gate_per_position: gate->gate is a scale [OH * OW][C] and gate->alpha is NULL
     if (!zp_float && takes_imma(c, p) && p.M < (1LL << 31)) {   // the epilogue's 32-bit image index
       p.gate = *gate;
-      return launch_conv(c, p, s, Tail::kGate);
+      return launch_conv(c, p, s, gate_per_position ? Tail::kScale : Tail::kGate);
     }
     // every other kernel: the convolution alone, then the whole tail in one pass in place
     const int rc = bconv_run_impl(plan, in_dev, out_dev, nullptr, LCE_ACT_NONE, nullptr, nullptr,
                                   stream);
     if (rc) return rc;
     float* out = static_cast<float*>(out_dev);
-    return lce_b200_f32_gate_sign(out, gate, residual, residual_act, d.batch,
-                                  static_cast<int64_t>(p.OH) * p.OW, c.cout, out, packed_out, stream);
+    const int64_t pixels = static_cast<int64_t>(p.OH) * p.OW;
+    if (gate_per_position) {
+      const lce_scale_desc sd{gate->gate, gate->sign_scale, gate->sign_shift};
+      return lce_b200_f32_scale_sign(out, &sd, residual, residual_act, d.batch, pixels, c.cout, out,
+                                     packed_out, stream);
+    }
+    return lce_b200_f32_gate_sign(out, gate, residual, residual_act, d.batch, pixels, c.cout, out,
+                                  packed_out, stream);
   }
   // run_slice / run_slice_add: the mma.sync kernel's strided store, and the residual read at the
   // same strided address (the caller checked that the kernel takes the plan)
@@ -1274,6 +1287,40 @@ int lce_b200_bconv2d_run_fused_gate(lce_b200_bconv2d* plan, const int32_t* in_de
     return fail("bconv2d_run_fused_gate: output must not overlap the gate");
   return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev,
                         nullptr, stream, gate);
+}
+
+int lce_b200_bconv2d_run_fused_scale(lce_b200_bconv2d* plan, const int32_t* in_dev,
+                                     const lce_scale_desc* scale, const float* residual_dev,
+                                     int add_activation, float* out_dev, int32_t* packed_out_dev,
+                                     void* stream) {
+  const lce_bconv2d_desc& d = plan->d;
+  if (d.out_type != LCE_OUT_FLOAT)
+    return fail("bconv2d_run_fused_scale: only float-output plans can take a scale");
+  if (packed_out_dev && d.groups != 1)
+    return fail("bconv2d_run_fused_scale: packed output needs groups == 1");
+  if (!scale || !scale->scale) return fail("bconv2d_run_fused_scale: the scale tensor is required");
+  if (add_activation < LCE_ACT_NONE || add_activation > LCE_ACT_RELU6)
+    return fail("bconv2d_run_fused_scale: unknown ADD activation %d", add_activation);
+  if (residual_dev && !aligned16(residual_dev))
+    return fail("bconv2d_run_fused_scale: residual must be 16-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(scale->scale) & 7u) != 0)
+    return fail("bconv2d_run_fused_scale: the scale must be 8-byte aligned");
+  for (const float* v : {scale->scale, scale->sign_scale, scale->sign_shift})
+    if (v && !is_device_ptr(v)) return fail("bconv2d_run_fused_scale: scale vectors must be device memory");
+  // the epilogue reads the shortcut and the scale rows other CTAs may write: out must not alias them
+  const uintptr_t o0 = reinterpret_cast<uintptr_t>(out_dev);
+  const uintptr_t o1 = o0 + bconv_out_bytes(plan);
+  auto overlaps = [&](const void* v, size_t bytes) {
+    const uintptr_t v0 = reinterpret_cast<uintptr_t>(v);
+    return v != nullptr && v0 < o1 && o0 < v0 + bytes;
+  };
+  if (overlaps(residual_dev, bconv_out_bytes(plan)))
+    return fail("bconv2d_run_fused_scale: output must not overlap the residual");
+  if (overlaps(scale->scale, static_cast<size_t>(plan->out_h) * plan->out_w * d.channels_out * sizeof(float)))
+    return fail("bconv2d_run_fused_scale: output must not overlap the scale");
+  const lce_gate_desc gate{scale->scale, nullptr, scale->sign_scale, scale->sign_shift};
+  return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev,
+                        nullptr, stream, &gate, 0, nullptr, /*gate_per_position=*/true);
 }
 
 int lce_b200_bconv2d_run_slice(lce_b200_bconv2d* plan, const int32_t* in_dev, float* out_dev,

@@ -1044,8 +1044,9 @@ __global__ void __launch_bounds__(256) chain_sign_kernel(const float* x, const l
 }
 
 // lce_b200_f32_gate_sign: one pass of the gated tail (lce_b200_chain.cuh) over [batch][pixels][C],
-// threads laid out as in chain_sign_kernel. x and out may be the same buffer.
-template <bool PACK, typename I>
+// threads laid out as in chain_sign_kernel. x and out may be the same buffer. SPATIAL
+// (lce_b200_f32_scale_sign): the gate row is the position row % pixels, not the image.
+template <bool PACK, typename I, bool SPATIAL = false>
 __global__ void __launch_bounds__(256) gate_sign_kernel(const float* x, const lce_gate_desc gd,
                                                         const float* __restrict__ residual, int act,
                                                         I rows, I pixels, int channels, int cw,
@@ -1062,7 +1063,8 @@ __global__ void __launch_bounds__(256) gate_sign_kernel(const float* x, const lc
     if (!PACK || c < channels) {
       const I e = row * channels + c;
       const I b = row / pixels;
-      float o = lce::gate_prelu(x[e], __ldg(gd.gate + b * channels + c), has_a,
+      const I gi = SPATIAL ? row - b * pixels : b;
+      float o = lce::gate_prelu(x[e], __ldg(gd.gate + gi * channels + c), has_a,
                                 has_a ? __ldg(gd.alpha + c) : 0.0f);
       if (residual) o = __fadd_rn(o, residual[e]);
       o = apply_act(o, act);
@@ -2251,6 +2253,40 @@ int lce_b200_f32_gate_sign(const float* x, const lce_gate_desc* gate, const floa
                                                               cw, out, packed);
   }
   return launch_check("gate_sign_kernel");
+}
+
+int lce_b200_f32_scale_sign(const float* x, const lce_scale_desc* scale, const float* residual, int act,
+                            int64_t batch, int64_t pixels, int channels, float* out, int32_t* packed,
+                            void* stream) {
+  if (batch < 0 || pixels < 0 || channels <= 0)
+    return fail("scale_sign: bad shape (%lld images, %lld pixels, %d channels)",
+                static_cast<long long>(batch), static_cast<long long>(pixels), channels);
+  if (!scale || !scale->scale) return fail("scale_sign: the scale tensor is required");
+  if (act < LCE_ACT_NONE || act > LCE_ACT_RELU6) return fail("scale_sign: unknown activation %d", act);
+  const long long rows = batch * pixels;
+  if (rows == 0 || (out == nullptr && packed == nullptr)) return 0;
+  const lce_gate_desc gd{scale->scale, nullptr, scale->sign_scale, scale->sign_shift};
+  const int cw = (channels + 31) / 32;
+  const long long n = packed ? rows * cw * 32 : rows * static_cast<long long>(channels);
+  const int grid = grid_for(n, 256);
+  cudaStream_t s = as_stream(stream);
+  const bool narrow = n + 256LL * grid < (1LL << 31);   // pixels * channels <= rows * channels too
+  if (packed) {
+    if (narrow)
+      gate_sign_kernel<true, int, true><<<grid, 256, 0, s>>>(x, gd, residual, act, static_cast<int>(rows),
+                                                             static_cast<int>(pixels), channels, cw, out, packed);
+    else
+      gate_sign_kernel<true, long long, true><<<grid, 256, 0, s>>>(x, gd, residual, act, rows, pixels,
+                                                                   channels, cw, out, packed);
+  } else {
+    if (narrow)
+      gate_sign_kernel<false, int, true><<<grid, 256, 0, s>>>(x, gd, residual, act, static_cast<int>(rows),
+                                                              static_cast<int>(pixels), channels, cw, out, packed);
+    else
+      gate_sign_kernel<false, long long, true><<<grid, 256, 0, s>>>(x, gd, residual, act, rows, pixels,
+                                                                    channels, cw, out, packed);
+  }
+  return launch_check("gate_sign_kernel (per position)");
 }
 
 int lce_b200_f32_affine_sign(const float* x, int64_t x_pixel_stride, int64_t rows, int channels,

@@ -306,15 +306,18 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // shift_out | sign_shift | mul | bias] x 64 channels in shared memory: holding them all in
 // registers would exceed the b1 instances' 128-register cap. GATE (float output): Real-to-Binary's
 // gated tail (p.gate) before the shortcut ADD, from chain_s = [- | alpha | sign_scale | sign_shift
-// | mul | bias]; the gate row is each row's own image's (a tile can span several images).
+// | mul | bias]; the gate row is each row's own image's (a tile can span several images). With
+// SPATIAL it is the row's position within its image instead: XNOR-Net++'s scale Gamma[OH*OW][C]
+// (lce_b200_bconv2d_run_fused_scale, alpha absent).
 // SLICE (float output, no signs): row m goes to out + m * p.out_stride, a channel slice of a
 // wider map; a shortcut is read at the same strided address, which may be the output itself.
 // BITPACKED: the row's two output words, bit = acc > p.thr[c], packed like the float output's signs.
-template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false>
+template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false, bool SPATIAL = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
                                               int tig, const float* chain_s = nullptr) {
   static_assert(!(CHAIN && GATE), "one epilogue tail at a time");
+  static_assert(!SPATIAL || GATE, "a spatial scale is the gate tail's");
   static_assert(!SLICE || (OUT == LCE_OUT_FLOAT && !CHAIN && !GATE), "a plain float slice");
   static_assert(OUT != LCE_OUT_BITPACKED || !(CHAIN || GATE || SLICE), "float tails only");
   constexpr bool STAGED = CHAIN || GATE;
@@ -393,9 +396,12 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           }
         }
         if constexpr (GATE) {
-          // MUL(gate) -> PRELU(alpha): gate row b = m / (OH * OW) (M < 2^31, host-checked)
+          // MUL(gate) -> PRELU(alpha): gate row b = m / (OH * OW), or with SPATIAL the position
+          // m - b * OH * OW (M < 2^31, host-checked)
           const uint32_t b = fdiv(static_cast<uint32_t>(m), p.fd_ohw);
-          const float* gr = p.gate.gate + static_cast<size_t>(b) * p.cout + cth;
+          const uint32_t gi =
+              SPATIAL ? static_cast<uint32_t>(m) - b * (static_cast<uint32_t>(p.OH) * p.OW) : b;
+          const float* gr = p.gate.gate + static_cast<size_t>(gi) * p.cout + cth;
           const bool has_a = p.gate.alpha != nullptr;
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns) {
@@ -511,10 +517,12 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 // B1 selects the inner product: packed b1 fragments (accumulators at scale 1) or int8 ones
 // (scale 8). Both produce the same int32 accumulators. CHAIN (float output): the epilogue also
 // applies p.chain (lce_b200_bconv2d_run_fused_chain); GATE (float output): p.gate
-// (lce_b200_bconv2d_run_fused_gate); SLICE (float output): the strided store of
+// (lce_b200_bconv2d_run_fused_gate), with SPATIAL p.gate indexed by position
+// (lce_b200_bconv2d_run_fused_scale); SLICE (float output): the strided store of
 // lce_b200_bconv2d_run_slice, and its read-add-write in lce_b200_bconv2d_run_slice_add. The other
 // instances compile as without them.
-template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false>
+template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
+          bool SPATIAL = false>
 __global__ void __launch_bounds__(kIThreads, B1 ? kB1Ctas : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
   using Vec = typename VecT<V>::T;
@@ -653,7 +661,7 @@ bconv_imma_kernel(const ConvKParams p) {
       cs[i] = v != nullptr ? __ldg(v + c_tile + (i & (kBN - 1))) : 0.0f;
     }
     __syncthreads();
-    epilogue_imma<OUT, S, false, true>(p, acc, m0, c_tile, warp, gid, tig, cs);
+    epilogue_imma<OUT, S, false, true, false, SPATIAL>(p, acc, m0, c_tile, warp, gid, tig, cs);
   } else {
     epilogue_imma<OUT, S, false, false, SLICE>(p, acc, m0, c_tile, warp, gid, tig);
   }

@@ -200,6 +200,12 @@ class HostGraph:
         Call before fuse_activation_chains and allocate_tensors."""
         return lib().lce_host_fuse_channel_gates(self._g)
 
+    def fuse_spatial_scales(self):
+        """LceBconv2d -> MUL(constant scale [1,OH,OW,C]) -> ADD(shortcut) [-> MUL -> ADD -> LceQuantize]
+        (XNOR-Net++'s scaled block and the next block's BatchNorm and sign) => one node. Call
+        before fuse_float_glue, fuse_activation_chains and allocate_tensors."""
+        return lib().lce_host_fuse_spatial_scales(self._g)
+
     def fuse_pooled_signs(self):
         """MAX_POOL_2D -> MUL(scale) -> ADD(shift) -> LceQuantize (BinaryAlexNet's and XNOR-Net's
         pooled BatchNorm and sign) => one node that writes only the signs. Call before
@@ -232,7 +238,8 @@ class HostGraph:
         return lib().lce_host_fuse_residual_pairs(self._g)
 
     def fuse_all(self):
-        return (self.fuse_dense_blocks() + self.fuse_residual_blocks() + self.fuse_float_glue()
+        return (self.fuse_dense_blocks() + self.fuse_residual_blocks() + self.fuse_spatial_scales()
+                + self.fuse_float_glue()
                 + self.fuse_grouped_conv_affine() + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
                 + self.fuse_residual_pairs())
 

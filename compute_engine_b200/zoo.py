@@ -152,12 +152,13 @@ class _Builder:
         return y
 
     def bconv(self, xq, xs, cout, k=3, stride=1, pad_values=1, activation="RELU", dilation=1,
-              padding="SAME", bitpacked=False):
+              padding="SAME", bitpacked=False, fold_bn=True):
         """LceBconv2d with float output; BN (and for Bi-RealNet the kernel scale)
         folded into post_activation_multiplier / bias like the converter does
         (LCE/mlir/transforms/optimize_patterns_common.td:39-113). bitpacked: int32 output, the
         signs the next binary layer reads, with synthetic int32 thresholds [cout] around half the
-        accumulators' range K = k * k * cin (inputs 2 and 3 absent) in place of the BN."""
+        accumulators' range K = k * k * cin (inputs 2 and 3 absent) in place of the BN.
+        fold_bn=False: nothing is folded, post_activation_multiplier 1 and bias 0."""
         b, h, w, cin = xs
         signs = self.rng.integers(0, 2, (cout, k, k, cin), dtype=np.int8) * 2 - 1
         bits = np.zeros((cout, k, k, ((cin + 31) // 32) * 32), np.uint32)
@@ -178,8 +179,11 @@ class _Builder:
             self.m.add_op("LceBconv2d", [xq, self.const(filt, np.int32, "bfilter"), -1, -1,
                                          self.const(thr, np.int32, "thr")], [y], custom_options=opts)
             return y, (b, oh, ow, cout)
-        s, t = self.bn(cout)
-        mul = (s / np.float32(k * k * cin) * np.float32(4.0)).astype(np.float32)
+        if fold_bn:
+            s, t = self.bn(cout)
+            mul = (s / np.float32(k * k * cin) * np.float32(4.0)).astype(np.float32)
+        else:
+            mul, t = np.ones(cout, np.float32), np.zeros(cout, np.float32)
         y = self.act((b, oh, ow, cout))
         self.m.add_op("LceBconv2d",
                       [xq, self.const(filt, np.int32, "bfilter"), self.const(mul, name="pmul"),
@@ -381,6 +385,49 @@ def realtobinarynet(batch=1, seed=0, image=224, input_type="float32", pad_values
             g.m.add_op("MUL", [y, gt], [u])
             x, xs = g.add(prelu(u, ys), s, ys), ys
     probs = g.head(prelu(x, xs), xs, relu=False)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
+def xnornetpp(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+    """XNOR-Net++, restated from the paper (Bulat & Tzimiropoulos, BMVC 2019) on the ResNet-18
+    backbone of birealnet18, with synthetic weights, in the converter's op order:
+      stem CONV_2D 7x7/s2 3 -> 64 (BN folded, RELU) -> MAX_POOL_2D 3x3/s2 SAME;
+      4 stages x 4 blocks at 64 / 128 / 256 / 512 channels, stride 2 and Cout = 2 Cin on the first
+      block of stages 2-4; each block on x [B,H,W,Cin], in XNOR order: the shortcut first (x, or
+      AVERAGE_POOL_2D 2x2/s2 VALID -> CONV_2D 1x1, BN folded); MUL(x, bn_scale) -> ADD(bn_shift) ->
+      LceQuantize -> LceBconv2d 3x3 SAME (stride s, `pad_values`, no fused activation, float output,
+      post_activation multiplier 1 and bias 0: nothing is folded into it) -> MUL(Gamma) ->
+      ADD(shortcut);
+      head MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX, as in birealnet18.
+    Gamma is the paper's learned output scale in its factorised form alpha[C] x beta[OH] x gamma[OW],
+    all positive, alpha scaled by 1 / K (K = 9 Cin, so Gamma also normalises the accumulator), folded
+    into one constant [1, OH, OW, Cout] as the converter leaves it. 16 LceBconv2d, 16 Gamma MULs."""
+    g = _Builder(seed, batch, "XNORNetPP")
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+    x, xs = g.conv(x, xs, 64, 7, 2, activation="RELU")
+    x, xs = g.pool("MAX_POOL_2D", x, xs, 3, 2, "SAME")
+    for stage, cout in enumerate((64, 128, 256, 512)):
+        for blk in range(4):
+            stride = 2 if (stage > 0 and blk == 0) else 1
+            if stride == 2:
+                s, ss = g.pool("AVERAGE_POOL_2D", x, xs, 2, 2, "VALID")
+                s, _ = g.conv(s, ss, cout, 1, 1)
+            else:
+                s = x
+            t = g.batchnorm(x, xs)
+            y, ys = g.bconv(g.quantize(t, xs), xs, cout, stride=stride, pad_values=pad_values,
+                            activation="NONE", fold_bn=False)
+            _, oh, ow, _ = ys
+            alpha = g.rng.uniform(0.5, 1.5, cout).astype(np.float32) / np.float32(9 * xs[3])
+            beta = g.rng.uniform(0.5, 1.5, oh).astype(np.float32)
+            gamma = g.rng.uniform(0.5, 1.5, ow).astype(np.float32)
+            scale = (beta[:, None, None] * gamma[None, :, None] * alpha[None, None, :]).astype(np.float32)
+            u = g.act(ys)
+            g.m.add_op("MUL", [y, g.const(scale.reshape(1, oh, ow, cout), name="gamma")], [u])
+            x, xs = g.add(u, s, ys), ys
+    probs = g.head(x, xs, relu=False)
     g.m.outputs = [probs]
     return g.m.serialize()
 

@@ -166,6 +166,28 @@ int lce_b200_f32_gate_sign(const float* x_dev, const lce_gate_desc* gate_desc,
                            const float* residual_dev, int activation, int64_t batch,
                            int64_t pixels, int channels, float* out_dev, int32_t* packed_out_dev,
                            void* stream);
+/* XNOR-Net++'s scaled block tail (lce_scale_desc, lce_b200_types.h) behind the convolution:
+ *   out = act(fl(fl(OutputTransform(acc) * scale[p][c]) + residual)),
+ *   packed_out = bitpack(fl(fl(out * sign_scale) + sign_shift)) (optional),
+ * with p = m mod (OH * OW) the output pixel's position within its image. residual may be NULL (then
+ * act applies to the product); add_activation is an LCE_ACT_* code. scale_desc and
+ * scale_desc->scale are required. Float-output plans only; packed_out needs groups == 1; out must
+ * not overlap residual or the scale. The mma.sync kernel applies the tail in its epilogue; plans on
+ * another kernel, or that finish zero padding with the float correction pass, run the convolution
+ * and then lce_b200_f32_scale_sign in place. Bit-identical to the op sequence either way. */
+int lce_b200_bconv2d_run_fused_scale(lce_b200_bconv2d* plan, const int32_t* in_dev,
+                                     const lce_scale_desc* scale_desc, const float* residual_dev,
+                                     int add_activation, float* out_dev, int32_t* packed_out_dev,
+                                     void* stream);
+/* The same tail without a convolution, in one pass over a float [batch, pixels, channels] tensor:
+ * element (b, p, c) takes scale[p][c] and channel c of the other present vectors. residual, out and
+ * packed_out as in lce_b200_f32_gate_sign. With only `scale` set this is the MUL builtin of a
+ * [B,H,W,C] tensor by a [1,H,W,C] one (any b whose shape, leading 1s dropped, is x's trailing
+ * dimensions), out = act(x * scale). */
+int lce_b200_f32_scale_sign(const float* x_dev, const lce_scale_desc* scale_desc,
+                            const float* residual_dev, int activation, int64_t batch,
+                            int64_t pixels, int channels, float* out_dev, int32_t* packed_out_dev,
+                            void* stream);
 /* The sigmoid that ends Real-to-Binary Net's gate, TFLite's LOGISTIC
  * (TF/lite/kernels/internal/reference/logistic.h): out = 1 above 16.619047164916992188, exp(x)
  * below -9, else 1 / (1 + exp(-x)). CUDA's expf is not libm's: within 4 ulp of the formula, not

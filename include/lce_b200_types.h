@@ -110,6 +110,20 @@ typedef struct lce_gate_desc {
   const float* sign_shift;
 } lce_gate_desc;
 
+/* XNOR-Net++'s learned output scale behind a binary convolution (Bulat & Tzimiropoulos, BMVC
+ * 2019): MUL by a constant Gamma of one float per output position and channel (alpha[C] x beta[OH]
+ * x gamma[OW], folded by the converter into one [1, OH, OW, C] tensor), the shortcut ADD, then the
+ * next block's BatchNorm and sign (MUL(sign_scale) -> ADD(sign_shift) -> LceQuantize). `scale` is
+ * a device tensor [OH * OW][channels] and is required; sign_scale / sign_shift are device vectors
+ * with one float per channel, NULL when the op is absent. Per element of position p within its
+ * image, channel c, in TFLite's order and rounding:
+ *   o = act(s * scale[p][c] + residual);  bit = (o * sign_scale + sign_shift) < 0 */
+typedef struct lce_scale_desc {
+  const float* scale;
+  const float* sign_scale;
+  const float* sign_shift;
+} lce_scale_desc;
+
 #ifdef __cplusplus
 }
 #endif
