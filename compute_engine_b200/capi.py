@@ -103,6 +103,9 @@ EXPORTS = [
     "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
     "lce_b200_f32_maximum", "lce_b200_f32_minimum", "lce_b200_f32_div", "lce_b200_f32_round",
     "lce_b200_f32_quant2_planes", "lce_b200_f32_grouped_conv2d",
+    "lce_b200_bconv2d_bases_create", "lce_b200_bconv2d_bases_set_input_shape",
+    "lce_b200_bconv2d_bases_get_desc", "lce_b200_bconv2d_bases_run", "lce_b200_bconv2d_bases_destroy",
+    "lce_b200_f32_shift_sign_planes",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -318,6 +321,82 @@ def quant2_planes(x: torch.Tensor, pool=None):
     _check(lib().lce_b200_f32_quant2_planes(_p(x), b, h, w, c, fh, fw, sh, sw, padding, activation, _p(planes),
                                             _stream()))
     return planes
+
+
+def shift_sign_planes(x: torch.Tensor, shifts):
+    """ABC-Net's shifted signs of a float map x [..., C] (C % 32 == 0): one int32 plane
+    [..., C / 32] per shift, bit = fl(x + shift) < 0. Returns the list of planes."""
+    x = _dev(x, torch.float32)
+    c = x.shape[-1]
+    n = len(shifts)
+    planes = [torch.empty(x.shape[:-1] + (c // 32,), dtype=torch.int32, device=x.device) for _ in range(n)]
+    sh = (C.c_float * max(n, 1))(*[float(s) for s in shifts])
+    ptrs = (C.c_void_p * max(n, 1))(*[p.data_ptr() for p in planes])
+    _check(lib().lce_b200_f32_shift_sign_planes(_p(x), C.c_int64(x.numel() // c if c else 0), C.c_int(c),
+                                                C.c_int(n), sh, ptrs, _stream()))
+    return planes
+
+
+class BConv2dBases:
+    """ABC-Net layer plan (lce_b200_bconv2d_bases_*): M * N LceBconv2d terms, term n * M + m on input
+    plane n with base filter m, summed left to right, then the BatchNorm, an optional shortcut and
+    the next layer's shifted signs, in one kernel."""
+
+    def __init__(self, m_bases, n_planes, desc: BconvDesc, filters, post_muls, post_biases):
+        import numpy as np
+        t = m_bases * n_planes
+        if not (len(filters) == len(post_muls) == len(post_biases) == t):
+            raise LceError("BConv2dBases: M * N filters, multipliers and biases")
+        self._h = C.c_void_p()
+        self.desc = desc
+        self.m, self.n = m_bases, n_planes
+        keep = [np.ascontiguousarray(f, np.int32) for f in filters] + \
+            [np.ascontiguousarray(v, np.float32) for v in list(post_muls) + list(post_biases)]
+        descs = (BconvDesc * t)(*[desc] * t)
+        ptr = [a.ctypes.data_as(C.c_void_p) for a in keep]
+        fs, ms, bs = ((C.c_void_p * t)(*ptr[k * t:(k + 1) * t]) for k in range(3))
+        _check(lib().lce_b200_bconv2d_bases_create(C.c_int(m_bases), C.c_int(n_planes), descs, fs, ms, bs,
+                                                   C.byref(self._h)))
+
+    def out_shape(self):
+        d = BconvDesc()
+        oh, ow = C.c_int(), C.c_int()
+        _check(lib().lce_b200_bconv2d_bases_get_desc(self._h, C.byref(d), C.byref(oh), C.byref(ow)))
+        return (d.batch, oh.value, ow.value, d.channels_out)
+
+    def __call__(self, planes, bn_scale, bn_shift, bn_activation=ACT_NONE, residual=None,
+                 add_activation=ACT_NONE, next_shifts=(), out=True):
+        """planes: N packed inputs. Returns (float out | None, [next planes])."""
+        planes = [_dev(p, torch.int32) for p in planes]
+        b, h, w = planes[0].shape[:3]
+        if (b, h, w) != (self.desc.batch, self.desc.in_h, self.desc.in_w):
+            _check(lib().lce_b200_bconv2d_bases_set_input_shape(self._h, b, h, w))
+            self.desc.batch, self.desc.in_h, self.desc.in_w = b, h, w
+        shape = self.out_shape()
+        dev = planes[0].device
+        o = torch.empty(shape, dtype=torch.float32, device=dev) if out else None
+        nxt = [torch.empty(shape[:3] + (shape[3] // 32,), dtype=torch.int32, device=dev) for _ in next_shifts]
+        vecs = [_dev(v, torch.float32) for v in (bn_scale, bn_shift)]
+        res = None if residual is None else _dev(residual, torch.float32)
+        k = len(next_shifts)
+        pin = (C.c_void_p * len(planes))(*[p.data_ptr() for p in planes])
+        sh = (C.c_float * max(k, 1))(*[float(s) for s in next_shifts])
+        pout = (C.c_void_p * max(k, 1))(*[p.data_ptr() for p in nxt])
+        _check(lib().lce_b200_bconv2d_bases_run(self._h, pin, _p(vecs[0]), _p(vecs[1]), C.c_int(bn_activation),
+                                                _p(res), C.c_int(add_activation), _p(o), C.c_int(k), sh, pout,
+                                                _stream()))
+        return o, nxt
+
+    def close(self):
+        if self._h:
+            lib().lce_b200_bconv2d_bases_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class ConvDesc(C.Structure):

@@ -144,6 +144,7 @@ int lce_host_fuse_residual_blocks(void* g) { return static_cast<Graph*>(g)->Fuse
 int lce_host_fuse_float_glue(void* g) { return static_cast<Graph*>(g)->FuseFloatGlue(); }
 int lce_host_fuse_channel_gates(void* g) { return static_cast<Graph*>(g)->FuseChannelGates(); }
 int lce_host_fuse_spatial_scales(void* g) { return static_cast<Graph*>(g)->FuseSpatialScales(); }
+int lce_host_fuse_binary_bases(void* g) { return static_cast<Graph*>(g)->FuseBinaryBases(); }
 int lce_host_fuse_pooled_signs(void* g) { return static_cast<Graph*>(g)->FusePooledSigns(); }
 int lce_host_fuse_quantized_activations(void* g) {
   return static_cast<Graph*>(g)->FuseQuantizedActivations();

@@ -1061,6 +1061,234 @@ int Graph::FusePooledSigns() {
   return removed;
 }
 
+extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_BASES(const TfLiteRegistration* original);
+extern "C" TfLiteRegistration* lce_b200_internal_Register_SHIFT_SIGN_PLANES(void);
+extern "C" int lce_b200_internal_bases_takes(const lce_bconv2d_desc* d, int m_bases, int n_planes);   // lce_b200.cu
+
+int Graph::FuseBinaryBases() {
+  if (!device_arena_) return 0;
+  constexpr int kMax = 8;   // bases, planes and next planes per node (lce::kMaxBases)
+  auto producer = [&](int t) -> size_t {
+    for (size_t k = 0; k < nodes_.size(); ++k)
+      for (int q = 0; q < nodes_[k]->node.outputs->size; ++q)
+        if (nodes_[k]->node.outputs->data[q] == t) return k;
+    return kNoNode;
+  };
+  auto is_const = [&](int t, TfLiteType type) {
+    return t >= 0 && tensors_[t].type == type && tensors_[t].allocation_type == kTfLiteMmapRo;
+  };
+  // node k = ADD(x, u), u a one-element float constant, no fused activation, whose output only an
+  // LceQuantize reads: that LceQuantize (and *shift = u), else kNoNode
+  auto shift_sign = [&](size_t k, int x, float* shift) -> size_t {
+    if (k >= nodes_.size()) return kNoNode;
+    const NodeRecord& a = *nodes_[k];
+    if (a.name != kAdd || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1 ||
+        a.node.inputs->data[0] != x || !Params(a) || Activation(a) != 0)
+      return kNoNode;
+    const int u = a.node.inputs->data[1];
+    if (!is_const(u, kTfLiteFloat32) || tensors_[u].bytes != sizeof(float)) return kNoNode;
+    const size_t q = SoleConsumer(a.node.outputs->data[0]);
+    if (!IsQuantize(q)) return kNoNode;
+    memcpy(shift, const_host_[u].data(), sizeof(float));
+    return q;
+  };
+  // an unprepared plain LceBconv2d of this library with float output and constant inputs
+  auto plain_term = [&](size_t k) {
+    if (k >= nodes_.size()) return false;
+    const NodeRecord& b = *nodes_[k];
+    if (b.name != "LceBconv2d" || b.initialized || b.node.inputs->size != 5 || b.node.outputs->size != 1 ||
+        tensors_[b.node.outputs->data[0]].type != kTfLiteFloat32 ||
+        lce_b200_internal_Register_BCONV_2D_BASES(b.registration) == nullptr)
+      return false;
+    const int* in = b.node.inputs->data;
+    return is_const(in[1], kTfLiteInt32) && is_const(in[2], kTfLiteFloat32) && is_const(in[3], kTfLiteFloat32);
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size(); ++i) {
+    if (!plain_term(i)) continue;
+    // the sum ADD(...ADD(ADD(t_0, t_1), t_2)..., t_{K-1}), every intermediate read by the next ADD alone
+    std::vector<size_t> terms{i}, absorbed;
+    int cur = nodes_[i]->node.outputs->data[0];
+    for (;;) {
+      const size_t a = SoleConsumer(cur);
+      if (a >= nodes_.size()) break;
+      const NodeRecord& an = *nodes_[a];
+      if (an.name != kAdd || an.initialized || an.node.inputs->size != 2 || an.node.outputs->size != 1 ||
+          an.node.inputs->data[0] != cur || !Params(an) || Activation(an) != 0 ||
+          tensors_[an.node.outputs->data[0]].type != kTfLiteFloat32)
+        break;
+      const int t = an.node.inputs->data[1];
+      const size_t tk = producer(t);
+      if (!plain_term(tk) || SoleConsumer(t) != a) break;
+      terms.push_back(tk);
+      absorbed.push_back(a);
+      cur = an.node.outputs->data[0];
+    }
+    const int K = static_cast<int>(terms.size());
+    if (K < 2) continue;   // a single LceBconv2d is never a bases layer
+    const TfLiteIntArray* yd = tensors_[cur].dims;
+    if (!yd || yd->size != 4) continue;
+    const int C = yd->data[3];
+    // the BatchNorm MUL(bn_scale) -> ADD(bn_shift, any activation)
+    const size_t km = SoleConsumer(cur);
+    const int bn_s = PerChannelConstOp(km, kMul, cur, C);
+    if (bn_s < 0) continue;
+    const int t1 = nodes_[km]->node.outputs->data[0];
+    const size_t kb = SoleConsumer(t1);
+    const int bn_t = PerChannelConstOp(kb, kAdd, t1, C, true);
+    if (bn_t < 0) continue;
+    // the planes: term k reads plane k / M, and each plane is read by its M terms alone
+    std::vector<int> planes;
+    for (size_t k : terms) {
+      const int q = nodes_[k]->node.inputs->data[0];
+      if (std::find(planes.begin(), planes.end(), q) == planes.end()) planes.push_back(q);
+    }
+    const int N = static_cast<int>(planes.size());
+    if (K % N != 0 || N > kMax || K / N > kMax) continue;
+    const int M = K / N;
+    bool ok = true;
+    for (int k = 0; k < K && ok; ++k) ok = nodes_[terms[k]]->node.inputs->data[0] == planes[k / M];
+    for (int n = 0; n < N && ok; ++n)
+      ok = !IsGraphOutput(planes[n]) && static_cast<int>(Consumers(planes[n]).size()) == M &&
+           SameDims(tensors_[planes[n]].dims, tensors_[planes[0]].dims);
+    // identical geometry (options and filter shape); term (n, m) convolves with base m's filter
+    const NodeRecord& t0 = *nodes_[terms[0]];
+    for (int k = 1; k < K && ok; ++k) {
+      const NodeRecord& tk = *nodes_[terms[k]];
+      const int fk = tk.node.inputs->data[1], fm = nodes_[terms[k % M]]->node.inputs->data[1];
+      ok = tk.custom_options == t0.custom_options &&
+           SameDims(tensors_[fk].dims, tensors_[t0.node.inputs->data[1]].dims) &&
+           (fk == fm || const_host_[fk] == const_host_[fm]);
+    }
+    if (!ok) continue;
+    const TfLiteIntArray* xd = tensors_[planes[0]].dims;
+    const TfLiteIntArray* fd = tensors_[t0.node.inputs->data[1]].dims;
+    if (!xd || !fd || xd->size != 4 || fd->size != 4) continue;
+    FlexMap opts(t0.custom_options.data(), t0.custom_options.size());
+    lce_bconv2d_desc d{};
+    d.batch = xd->data[0]; d.in_h = xd->data[1]; d.in_w = xd->data[2];
+    d.channels_in = opts.AsInt32("channels_in");
+    d.channels_out = fd->data[0]; d.filter_h = fd->data[1]; d.filter_w = fd->data[2];
+    d.groups = fd->data[3] == (d.channels_in + 31) / 32 && xd->data[3] == fd->data[3] ? 1 : 0;
+    d.stride_h = opts.AsInt32("stride_height"); d.stride_w = opts.AsInt32("stride_width");
+    d.dilation_h = opts.AsInt32("dilation_height_factor");
+    d.dilation_w = opts.AsInt32("dilation_width_factor");
+    d.padding = opts.AsInt32("padding"); d.pad_value = opts.AsInt32("pad_values");
+    d.activation = opts.AsInt32("fused_activation_function");
+    d.out_type = LCE_OUT_FLOAT;
+    if (d.channels_out != C || !lce_b200_internal_bases_takes(&d, M, N)) continue;
+    // where the planes come from: N pairs ADD(x, u_n) -> LceQuantize of one x, turned into one planes
+    // node below, or the outputs of one earlier fused node that already writes them
+    std::vector<size_t> pairs;   // shift ADD, LceQuantize of each plane
+    std::vector<float> in_shifts;
+    int x = -1;
+    for (int n = 0; n < N && ok; ++n) {
+      const size_t kq = producer(planes[n]);
+      const size_t ks = kq < nodes_.size() && IsQuantize(kq) ? producer(nodes_[kq]->node.inputs->data[0]) : kNoNode;
+      float u = 0.f;
+      if (ks < nodes_.size() && nodes_[ks]->node.inputs->size == 2) {
+        if (x < 0) x = nodes_[ks]->node.inputs->data[0];
+        ok = shift_sign(ks, x, &u) == kq;
+        pairs.insert(pairs.end(), {ks, kq});
+        in_shifts.push_back(u);
+      } else {
+        ok = false;
+      }
+    }
+    if (!ok) {
+      // already fused: every plane is an output of the same earlier node that writes shifted signs
+      const size_t kp = producer(planes[0]);
+      ok = kp < nodes_.size() && (nodes_[kp]->name == "LceBconv2dBases+LceQuantize" ||
+                                  nodes_[kp]->name == "ADD+LceQuantize");
+      for (int n = 1; n < N && ok; ++n) ok = producer(planes[n]) == kp;
+      if (!ok) continue;
+      pairs.clear();
+    } else {
+      // the planes node reads x [.., channels_in]
+      const TfLiteIntArray* xs = tensors_[x].dims;
+      if (tensors_[x].type != kTfLiteFloat32 || !xs || xs->size != 4 || xs->data[3] != d.channels_in) continue;
+    }
+    // the optional shortcut ADD(o, r, any activation), r computed, of o's shape
+    int o = nodes_[kb]->node.outputs->data[0];
+    size_t last = kb;
+    int r = -1;
+    int32_t add_act = 0;
+    const size_t ka = SoleConsumer(o);
+    if (ka < nodes_.size()) {
+      const NodeRecord& a = *nodes_[ka];
+      if (a.name == kAdd && !a.initialized && a.node.inputs->size == 2 && a.node.outputs->size == 1 && Params(a) &&
+          tensors_[a.node.outputs->data[0]].type == kTfLiteFloat32) {
+        const int in0 = a.node.inputs->data[0], in1 = a.node.inputs->data[1];
+        const int rr = in0 == o ? in1 : in0;
+        if (in0 != in1 && rr >= 0 && tensors_[rr].type == kTfLiteFloat32 &&
+            tensors_[rr].allocation_type != kTfLiteMmapRo && SameDims(tensors_[rr].dims, yd) && ReadyBefore(rr, i)) {
+          r = rr;
+          add_act = Activation(a);
+          absorbed.push_back(kb);
+          last = ka;
+          o = a.node.outputs->data[0];
+        }
+      }
+    }
+    // the next layer's shifted signs among o's readers; o itself is stored when anything else reads it
+    std::vector<int> next;
+    std::vector<float> next_shifts;
+    size_t others = 0;
+    for (size_t c : Consumers(o)) {
+      float u = 0.f;
+      const size_t q = next.size() < kMax ? shift_sign(c, o, &u) : kNoNode;
+      if (q == kNoNode) {
+        ++others;
+        continue;
+      }
+      next.push_back(nodes_[q]->node.outputs->data[0]);
+      next_shifts.push_back(u);
+      absorbed.insert(absorbed.end(), {c, q});
+    }
+    const int32_t store = IsGraphOutput(o) || others > 0 || next.empty();
+    // rewrite: node `last` becomes the layer, the first shift ADD the planes node
+    std::vector<int> ins(planes);
+    for (size_t k : terms) {
+      const int* in = nodes_[k]->node.inputs->data;
+      ins.insert(ins.end(), {in[1], in[2], in[3]});
+    }
+    ins.insert(ins.end(), {bn_s, bn_t, r});
+    std::vector<int> outs;
+    if (store) outs.push_back(o);
+    outs.insert(outs.end(), next.begin(), next.end());
+    std::vector<uint8_t> blob(6 * sizeof(int32_t) + next_shifts.size() * sizeof(float));
+    const int32_t head[6] = {M, N, static_cast<int32_t>(next.size()), Activation(*nodes_[kb]), add_act, store};
+    memcpy(blob.data(), head, sizeof(head));
+    if (!next_shifts.empty()) memcpy(blob.data() + sizeof(head), next_shifts.data(), next_shifts.size() * sizeof(float));
+    std::vector<uint8_t> options = t0.custom_options;
+    NodeRecord& f = *nodes_[last];
+    f.registration = lce_b200_internal_Register_BCONV_2D_BASES(t0.registration);
+    SetCustomOptions(f, std::move(options));
+    SetNodeIO(f, ins, outs);
+    SetBuiltinBlob(f, blob.data(), blob.size());
+    f.name = next.empty() ? "LceBconv2dBases" : "LceBconv2dBases+LceQuantize";
+    absorbed.insert(absorbed.end(), terms.begin(), terms.end());
+    absorbed.push_back(km);
+    if (!pairs.empty()) {
+      NodeRecord& pn = *nodes_[pairs[0]];   // the first shift ADD: x exists there
+      std::vector<uint8_t> pblob(sizeof(int32_t) + in_shifts.size() * sizeof(float));
+      const int32_t n32 = N;
+      memcpy(pblob.data(), &n32, sizeof(n32));
+      memcpy(pblob.data() + sizeof(n32), in_shifts.data(), in_shifts.size() * sizeof(float));
+      pn.registration = lce_b200_internal_Register_SHIFT_SIGN_PLANES();
+      SetNodeIO(pn, {x}, planes);
+      SetBuiltinBlob(pn, pblob.data(), pblob.size());
+      pn.name = "ADD+LceQuantize";
+      absorbed.insert(absorbed.end(), pairs.begin() + 1, pairs.end());
+    }
+    removed += static_cast<int>(absorbed.size());
+    EraseNodes(absorbed);
+    i = SIZE_MAX;   // indices moved: scan again from the start
+  }
+  allocated_ = false;
+  return removed;
+}
+
 int Graph::FuseQuantizedActivations() {
   // the host copy of a float constant, else nullptr (data.raw may be its device copy)
   auto float_const = [&](int t) -> const float* {

@@ -115,6 +115,30 @@ class Graph {
   // removed.
   int FuseSpatialScales();
 
+  // ABC-Net's multiple binary bases (Lin et al., NeurIPS 2017): a layer on a float map x with N
+  // shifted signs q_n = LceQuantize(ADD(x, u_n)) and M weight bases,
+  //   t_nm = LceBconv2d(q_n, B_m)  ->  ADD(...ADD(ADD(t_00, t_01), t_02)..., t_{N-1,M-1})  (n outer)
+  //     -> MUL(bn_scale) -> ADD(bn_shift, any activation) [-> ADD(shortcut, any activation)]
+  //     [-> the next layer's ADD(o, u'_k) -> LceQuantize pairs]
+  // becomes one node "LceBconv2dBases[+LceQuantize]" (lce_b200_bconv2d_bases_run): inputs [q_0..q_{N-1},
+  // then filter, mul, bias of each term in (n, m) order, bn_scale, bn_shift, shortcut (-1 when
+  // absent)], outputs [o if anything other than the absorbed pairs reads it or it is a graph output,
+  // then the next planes], builtin_data int32 {M, N, next planes, BatchNorm activation, shortcut
+  // activation, o stored} and the next shifts as floats; options are term 0's. When the q_n come
+  // from unfused pairs, they become one node "ADD+LceQuantize" (lce_b200_f32_shift_sign_planes): inputs
+  // [x], outputs [q_0..q_{N-1}], builtin_data int32 N then the N shifts. Only when every u_n is a
+  // one-element float constant and the ADDs have no fused activation; M * N >= 2 (a single
+  // LceBconv2d never matches) with M, N <= 8; the terms are plain float LceBconv2d nodes with equal
+  // options and filter shapes, constant inputs and term (n, m)'s filter equal to term (0, m)'s; term
+  // k of the chain reads plane k / M, and each plane is read by its M terms alone; the chain's ADDs
+  // take the running sum as their first operand and have no fused activation; bn_scale / bn_shift
+  // are float constants [C] or [1, ..., 1, C]; every intermediate has one consumer and is not a graph
+  // output; and lce_b200_bconv2d_bases_create takes the terms (one-padded or VALID, no fused
+  // activation, channels_out % 64 == 0, the bases' weights within shared memory). Zero-padded layers
+  // stay unfused. Run first: FuseResidualBlocks would take ADD(t_00, t_01) as a residual block.
+  // Bit-identical. Returns the number of nodes removed.
+  int FuseBinaryBases();
+
   // BinaryAlexNet's and XNOR-Net's pooled BatchNorm and sign
   //   MAX_POOL_2D(x) -> MUL(scale) -> ADD(shift) -> LceQuantize
   // becomes one node "MAX_POOL_2D+MUL+ADD+LceQuantize" (lce_b200_f32_maxpool_affine_sign): inputs

@@ -819,6 +819,181 @@ TfLiteStatus ScaleEval(TfLiteContext* context, TfLiteNode* node) {
 }
 
 // ------------------------------------------------------------------------- //
+// An ABC-Net layer in one node (Graph::FuseBinaryBases): [q_0..q_{N-1}, (filter, mul, bias) of each
+// term n * M + m, bn_scale, bn_shift, shortcut] -> [out if stored, next planes...]; builtin_data
+// int32 {M, N, next planes, bn activation, shortcut activation, out stored} then the next shifts as
+// floats; options are the terms' LceBconv2d options.
+// ------------------------------------------------------------------------- //
+struct BasesOpData {
+  BconvOpData* conv = nullptr;   // the terms' parameters (desc)
+  lce_b200_bconv2d_bases* plan = nullptr;
+  ~BasesOpData() {
+    lce_b200_bconv2d_bases_destroy(plan);
+    delete conv;
+  }
+};
+struct BasesNodeParams {
+  int32_t m, n, n_next, bn_act, add_act, store;
+  float shift[8];
+};
+
+void* BasesInit(TfLiteContext* context, const char* buffer, size_t length) {
+  auto* op = new BasesOpData();
+  op->conv = static_cast<BconvOpData*>(BconvInit(context, buffer, length));
+  return op;
+}
+void BasesFree(TfLiteContext*, void* buffer) { delete static_cast<BasesOpData*>(buffer); }
+
+bool BasesParamsOf(const TfLiteNode* node, BasesNodeParams* b) {
+  if (!node->builtin_data) return false;
+  memset(b, 0, sizeof(*b));
+  memcpy(b, node->builtin_data, 6 * sizeof(int32_t));
+  if (b->m < 1 || b->n < 1 || b->m > 8 || b->n > 8 || b->n_next < 0 || b->n_next > 8) return false;
+  memcpy(b->shift, static_cast<const char*>(node->builtin_data) + 6 * sizeof(int32_t), b->n_next * sizeof(float));
+  return true;
+}
+
+TfLiteStatus BasesPrepare(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<BasesOpData*>(node->user_data);
+  if (!op->conv->successfully_initialized) return kTfLiteError;
+  BasesNodeParams bp;
+  LCE_ENSURE(context, BasesParamsOf(node, &bp));
+  const int T = bp.m * bp.n;
+  LCE_ENSURE(context, node->inputs->size == bp.n + 3 * T + 3);
+  LCE_ENSURE(context, node->outputs->size == bp.store + bp.n_next);
+  lce_bconv2d_desc& d = op->conv->desc;
+  const TfLiteTensor* input = GetInput(context, node, 0);
+  const TfLiteTensor* filter = GetInput(context, node, bp.n);
+  LCE_ENSURE(context, input != nullptr && filter != nullptr && NumDims(input) == 4 && NumDims(filter) == 4);
+  LCE_ENSURE(context, input->type == kTfLiteInt32 && filter->type == kTfLiteInt32);
+  for (int k = 1; k < bp.n; ++k) {
+    const TfLiteTensor* q = GetInput(context, node, k);
+    LCE_ENSURE(context, q != nullptr && q->type == kTfLiteInt32 && NumDims(q) == 4);
+    for (int a = 0; a < 4; ++a) LCE_ENSURE(context, Dim(q, a) == Dim(input, a));
+  }
+  d.channels_out = Dim(filter, 0);
+  d.filter_h = Dim(filter, 1);
+  d.filter_w = Dim(filter, 2);
+  d.groups = 1;
+  LCE_ENSURE(context, Dim(filter, 3) == BitpackedSize(d.channels_in) && Dim(input, 3) == Dim(filter, 3));
+  d.out_type = LCE_OUT_FLOAT;
+  d.batch = Dim(input, 0);
+  d.in_h = Dim(input, 1);
+  d.in_w = Dim(input, 2);
+  int out_h, out_w, pad_h, pad_w;
+  LCE_ENSURE_CAPI(context, lce_b200_bconv2d_out_shape(&d, &out_h, &out_w, &pad_h, &pad_w));
+  for (int t = 0; t < T; ++t) {
+    const TfLiteTensor* f = GetInput(context, node, bp.n + 3 * t);
+    const TfLiteTensor* mul = GetInput(context, node, bp.n + 3 * t + 1);
+    const TfLiteTensor* bias = GetInput(context, node, bp.n + 3 * t + 2);
+    LCE_ENSURE(context, f != nullptr && f->type == kTfLiteInt32 && NumElements(f) == NumElements(filter));
+    LCE_ENSURE(context, mul != nullptr && mul->type == kTfLiteFloat32 && NumElements(mul) == d.channels_out);
+    LCE_ENSURE(context, bias != nullptr && bias->type == kTfLiteFloat32 && NumElements(bias) == d.channels_out);
+  }
+  for (int k = 0; k < 2; ++k) {
+    const TfLiteTensor* v = GetInput(context, node, bp.n + 3 * T + k);
+    LCE_ENSURE(context, v != nullptr && v->type == kTfLiteFloat32 && NumElements(v) == d.channels_out);
+  }
+  const TfLiteTensor* residual = GetInput(context, node, bp.n + 3 * T + 2);
+  if (residual != nullptr) {
+    LCE_ENSURE(context, residual->type == kTfLiteFloat32 && NumDims(residual) == 4);
+    LCE_ENSURE(context, Dim(residual, 0) == d.batch && Dim(residual, 1) == out_h && Dim(residual, 2) == out_w &&
+                            Dim(residual, 3) == d.channels_out);
+  }
+  for (int k = 0; k < node->outputs->size; ++k) {
+    TfLiteTensor* o = GetOutput(context, node, k);
+    const bool is_out = bp.store && k == 0;
+    LCE_ENSURE(context, o->type == (is_out ? kTfLiteFloat32 : kTfLiteInt32));
+    TfLiteIntArray* shape = LceB200IntArrayCreate(4);
+    shape->data[0] = d.batch;
+    shape->data[1] = out_h;
+    shape->data[2] = out_w;
+    shape->data[3] = is_out ? d.channels_out : BitpackedSize(d.channels_out);
+    if (context->ResizeTensor(context, o, shape) != kTfLiteOk) return kTfLiteError;
+  }
+  op->conv->plan_stale = true;
+  return kTfLiteOk;
+}
+
+TfLiteStatus BasesEval(TfLiteContext* context, TfLiteNode* node) {
+  auto* op = static_cast<BasesOpData*>(node->user_data);
+  BasesNodeParams bp;
+  LCE_ENSURE(context, BasesParamsOf(node, &bp));
+  const int T = bp.m * bp.n;
+  const lce_bconv2d_desc& d = op->conv->desc;
+  if (op->plan == nullptr) {
+    // the constants are the graph's and do not change; later Prepares only resize the input
+    std::vector<lce_bconv2d_desc> descs(T, d);
+    std::vector<const int32_t*> filters(T);
+    std::vector<const float*> muls(T), biases(T);
+    for (int t = 0; t < T; ++t) {
+      filters[t] = GetInput(context, node, bp.n + 3 * t)->data.i32;
+      muls[t] = GetInput(context, node, bp.n + 3 * t + 1)->data.f;
+      biases[t] = GetInput(context, node, bp.n + 3 * t + 2)->data.f;
+    }
+    LCE_ENSURE_CAPI(context, lce_b200_bconv2d_bases_create(bp.m, bp.n, descs.data(), filters.data(), muls.data(),
+                                                           biases.data(), &op->plan));
+    op->conv->plan_stale = true;
+  }
+  if (op->conv->plan_stale) {
+    LCE_ENSURE_CAPI(context, lce_b200_bconv2d_bases_set_input_shape(op->plan, d.batch, d.in_h, d.in_w));
+    op->conv->plan_stale = false;
+  }
+  const int32_t* planes[8];
+  for (int n = 0; n < bp.n; ++n) {
+    const TfLiteTensor* q = GetInput(context, node, n);
+    LCE_ENSURE_MSG(context, OnDevice(q->data.raw), "LceBconv2dBases needs a device arena");
+    planes[n] = q->data.i32;
+  }
+  const TfLiteTensor* residual = GetInput(context, node, bp.n + 3 * T + 2);
+  float* out = bp.store ? GetOutput(context, node, 0)->data.f : nullptr;
+  int32_t* next[8];
+  for (int k = 0; k < bp.n_next; ++k) next[k] = GetOutput(context, node, bp.store + k)->data.i32;
+  LCE_ENSURE_CAPI(context, lce_b200_bconv2d_bases_run(
+                               op->plan, planes, GetInput(context, node, bp.n + 3 * T)->data.f,
+                               GetInput(context, node, bp.n + 3 * T + 1)->data.f, bp.bn_act,
+                               residual ? residual->data.f : nullptr, bp.add_act, out, bp.n_next, bp.shift,
+                               next, g_stream));
+  return kTfLiteOk;
+}
+
+// ABC-Net's shifted signs of a float map in one node (Graph::FuseBinaryBases): [x] -> [q_0..q_{N-1}];
+// builtin_data int32 N then the N shifts as floats.
+TfLiteStatus ShiftPlanesPrepare(TfLiteContext* context, TfLiteNode* node) {
+  LCE_ENSURE(context, node->inputs->size == 1 && node->builtin_data != nullptr);
+  int32_t n = 0;
+  memcpy(&n, node->builtin_data, sizeof(n));
+  LCE_ENSURE(context, n >= 1 && n <= 8 && node->outputs->size == n);
+  const TfLiteTensor* x = GetInput(context, node, 0);
+  LCE_ENSURE(context, x != nullptr && x->type == kTfLiteFloat32 && NumDims(x) >= 1);
+  LCE_ENSURE(context, Dim(x, NumDims(x) - 1) % 32 == 0);
+  for (int k = 0; k < n; ++k) {
+    TfLiteTensor* q = GetOutput(context, node, k);
+    LCE_ENSURE(context, q->type == kTfLiteInt32);
+    TfLiteIntArray* shape = LceB200IntArrayCreate(NumDims(x));
+    for (int a = 0; a < NumDims(x); ++a) shape->data[a] = Dim(x, a);
+    shape->data[shape->size - 1] = BitpackedSize(Dim(x, NumDims(x) - 1));
+    if (context->ResizeTensor(context, q, shape) != kTfLiteOk) return kTfLiteError;
+  }
+  return kTfLiteOk;
+}
+
+TfLiteStatus ShiftPlanesEval(TfLiteContext* context, TfLiteNode* node) {
+  int32_t n = 0;
+  memcpy(&n, node->builtin_data, sizeof(n));
+  float shifts[8];
+  memcpy(shifts, static_cast<const char*>(node->builtin_data) + sizeof(n), n * sizeof(float));
+  const TfLiteTensor* x = GetInput(context, node, 0);
+  int32_t* planes[8];
+  for (int k = 0; k < n; ++k) planes[k] = GetOutput(context, node, k)->data.i32;
+  LCE_ENSURE_MSG(context, OnDevice(x->data.raw) && OnDevice(planes[0]), "shifted signs need a device arena");
+  const int c = Dim(x, NumDims(x) - 1);
+  LCE_ENSURE_CAPI(context, lce_b200_f32_shift_sign_planes(x->data.f, NumElements(x) / c, c, n, shifts, planes,
+                                                          g_stream));
+  return kTfLiteOk;
+}
+
+// ------------------------------------------------------------------------- //
 // A BinaryDenseNet dense layer or a MeliusNet improvement layer in one node
 // (Graph::FuseDenseBlocks): [src, scale, shift, filter, mul, bias, thr] -> [X]. X is the block's
 // final map [B, H, W, C_L]; builtin_data: int32 {C_L, the layer kind (kDenseLayer /
@@ -1040,6 +1215,24 @@ TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_SCALE(const TfLiteRegist
   if (original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
     return BconvScaleRegistration<KernelType::kOptimizedIndirectBGEMM>();
   return nullptr;
+}
+
+// host-internal: the ABC-Net layer node created by Graph::FuseBinaryBases from plain LceBconv2d nodes
+// of this registration (nullptr: not one of this library's LceBconv2d registrations). The terms are
+// one-padded or VALID, where every registration computes the same integers, so one node serves all.
+TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_BASES(const TfLiteRegistration* original) {
+  static TfLiteRegistration r = {BasesInit, BasesFree, BasesPrepare, BasesEval};
+  if (original == BconvRegistration<KernelType::kCuda>() || original == BconvRegistration<KernelType::kReference>() ||
+      original == BconvRegistration<KernelType::kOptimizedBGEMM>() ||
+      original == BconvRegistration<KernelType::kOptimizedIndirectBGEMM>())
+    return &r;
+  return nullptr;
+}
+
+// host-internal: Graph::FuseBinaryBases's one-pass shifted signs
+TfLiteRegistration* lce_b200_internal_Register_SHIFT_SIGN_PLANES(void) {
+  static TfLiteRegistration r = {nullptr, nullptr, ShiftPlanesPrepare, ShiftPlanesEval};
+  return &r;
 }
 
 // host-internal: the dense- or improvement-layer node created by Graph::FuseDenseBlocks from a plain

@@ -790,6 +790,77 @@ int launch_pair(const lce::PairParams& p, int grid, cudaStream_t s) {
   return launch_check("bconv_pair_kernel");
 }
 
+// OneTimeSetup's fold of the float / int8 output transform (bconv2d.cc:353-389), in double on the
+// host: fm = -mul / scale, fb = (bias + K * mul) / scale + zero_point for each output channel.
+int fold_output_transform(const lce_bconv2d_desc& d, const float* post_mul, const float* post_bias,
+                          float* fm, float* fb) {
+  const int cout = d.channels_out;
+  std::vector<float> pm(cout), pb(cout);
+  if (to_host(post_mul, cout * sizeof(float), pm.data()) || to_host(post_bias, cout * sizeof(float), pb.data()))
+    return 1;
+  const int32_t backtransform_add = d.filter_h * d.filter_w * (d.channels_in / d.groups);
+  const double scale = d.out_type == LCE_OUT_INT8 ? static_cast<double>(d.out_scale) : 1.0;
+  const double zp = d.out_type == LCE_OUT_INT8 ? static_cast<double>(d.out_zero_point) : 0.0;
+  for (int i = 0; i < cout; ++i) {
+    const double m = pm[i], b = pb[i];
+    fm[i] = static_cast<float>(-1 * m / scale);
+    fb[i] = static_cast<float>((b + static_cast<double>(backtransform_add) * m) / scale + zp);
+  }
+  return 0;
+}
+
+// ABC-Net bases kernel (bconv_bases_kernel): the M bases' fragments stay in shared memory, the
+// planes stream through a two-deep ring of whole-K planes (reuse) or of K chunks. Returns what a
+// layer with `n_slices` 8-word k-slices and `m_bases` bases stages, or a refusal.
+constexpr size_t kBasesSmemMax = 226u * 1024u;   // one CTA per SM, its 1 KB of static shared memory aside
+const char* bases_staging(int n_slices, int m_bases, int* chunk_slices, int* chunks, int* reuse,
+                          size_t* smem) {
+  const size_t w = static_cast<size_t>(m_bases) * n_slices * (8 * 32 * 8);
+  const size_t slice_a = static_cast<size_t>(lce::kIBM) * 32;
+  if (w + 2 * slice_a > kBasesSmemMax)
+    return "the bases' weights for one 64-channel tile do not fit in shared memory";
+  const size_t avail = kBasesSmemMax - w;
+  if (2 * n_slices * slice_a <= avail) {
+    *reuse = 1; *chunks = 1; *chunk_slices = n_slices;
+  } else {
+    const int ring = static_cast<int>(avail / (2 * slice_a));
+    *reuse = 0;
+    *chunks = cdiv(n_slices, ring);
+    *chunk_slices = cdiv(n_slices, *chunks);
+  }
+  *smem = w + 2 * static_cast<size_t>(*chunk_slices) * slice_a;
+  return nullptr;
+}
+
+template <int V>
+int launch_bases(const lce::BasesParams& bp, dim3 grid, size_t smem, cudaStream_t s) {
+  static PerDeviceOnce once;
+  if (once.need())
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_bases_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(kBasesSmemMax)));
+  lce::bconv_bases_kernel<V><<<grid, lce::kIThreads, smem, s>>>(bp);
+  g_path[1].fetch_add(1, std::memory_order_relaxed);
+  return launch_check("bconv_bases_kernel");
+}
+
+// What keeps terms of this shape off the bases kernel, or nullptr
+const char* bases_refusal(const lce_bconv2d_desc& d, int m_bases, int n_planes) {
+  if (m_bases < 1 || n_planes < 1 || m_bases > lce::kMaxBases || n_planes > lce::kMaxBases)
+    return "1 to 8 bases and 1 to 8 planes";
+  if (d.out_type != LCE_OUT_FLOAT || d.activation != LCE_ACT_NONE)
+    return "float output without a fused activation";
+  if (d.groups != 1 || d.channels_out % lce::kBN != 0 || d.channels_in % 32 != 0)
+    return "ungrouped terms with channels_in % 32 == 0 and channels_out % 64 == 0";
+  if (d.padding == LCE_PADDING_SAME && d.pad_value == 0)
+    return "one-padded or VALID terms (zero padding needs the per-term float correction)";
+  if (env_off("LCE_B200_BCONV_IMMA") || env_off("LCE_B200_BCONV_B1"))
+    return "the b1 mma.sync inner product (LCE_B200_BCONV_IMMA / _B1 are 0)";
+  const int Kw = d.filter_h * d.filter_w * (d.channels_in / 32);
+  int cs, nc, reuse;
+  size_t smem;
+  return bases_staging(cdiv(Kw, 8), m_bases, &cs, &nc, &reuse, &smem);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------- //
@@ -1000,17 +1071,9 @@ int lce_b200_bconv2d_create(const lce_bconv2d_desc* d, const int32_t* filter,
   const size_t padded = static_cast<size_t>(c.cout) + kChanPad;
   if (!rc && d->out_type != LCE_OUT_BITPACKED) {
     // OneTimeSetup (bconv2d.cc:353-389): fold in double on the host.
-    std::vector<float> pm(c.cout), pb(c.cout), fm(padded, 0.f), fb(padded, 0.f);
-    rc = to_host(post_mul, c.cout * sizeof(float), pm.data()) ||
-         to_host(post_bias, c.cout * sizeof(float), pb.data());
+    std::vector<float> fm(padded, 0.f), fb(padded, 0.f);
+    rc = fold_output_transform(*d, post_mul, post_bias, fm.data(), fb.data());
     const int32_t backtransform_add = d->filter_h * d->filter_w * (d->channels_in / d->groups);
-    const double scale = d->out_type == LCE_OUT_INT8 ? static_cast<double>(d->out_scale) : 1.0;
-    const double zp = d->out_type == LCE_OUT_INT8 ? static_cast<double>(d->out_zero_point) : 0.0;
-    for (int i = 0; i < c.cout; ++i) {
-      const double m = pm[i], b = pb[i];
-      fm[i] = static_cast<float>(-1 * m / scale);
-      fb[i] = static_cast<float>((b + static_cast<double>(backtransform_add) * m) / scale + zp);
-    }
     int32_t nmin, nmax;  // CalculateActivationRange<int32>, kernel_util.h:285-300
     switch (d->activation) {
       case LCE_ACT_RELU: nmin = 0; nmax = INT32_MAX; break;
@@ -1386,6 +1449,12 @@ int lce_b200_internal_slice_takes(const lce_bconv2d_desc* d) {
   return slice_refusal(*d, nullptr) == nullptr;
 }
 
+// host-internal (Graph::FuseBinaryBases): lce_b200_bconv2d_bases_create would take M * N terms of
+// this descriptor; no device needed
+int lce_b200_internal_bases_takes(const lce_bconv2d_desc* d, int m_bases, int n_planes) {
+  return bases_refusal(*d, m_bases, n_planes) == nullptr;
+}
+
 int lce_b200_bconv2d_run_fused_pair(lce_b200_bconv2d* plan1, lce_b200_bconv2d* plan2,
                                     const int32_t* in_dev, const float* residual_dev,
                                     int act1, int act2, float* out_dev, int32_t* packed_out_dev,
@@ -1512,6 +1581,198 @@ void lce_b200_bconv2d_destroy(lce_b200_bconv2d* plan) {
   cudaFree(plan->d2h_out);
   delete plan;
 }
+
+// ------------------------- ABC-Net binary bases -------------------------- //
+struct lce_b200_bconv2d_bases {
+  int M = 0, N = 0;
+  lce_b200_bconv2d* geo = nullptr;   // term (0, 0)'s plan: shape, padding, clamp, K layout
+  int32_t* wt = nullptr;             // [tile][M][n_slices][8][32] b1 fragments
+  int32_t* wpop = nullptr;           // [M][ldc]
+  float* tmul = nullptr;             // [M * N][ldc]
+  float* tbias = nullptr;
+  int ldc = 0, chunk_slices = 0, chunks = 1, reuse = 1;
+  size_t smem = 0;
+  unsigned w_bytes = 0;
+  ~lce_b200_bconv2d_bases() {
+    lce_b200_bconv2d_destroy(geo);
+    cudaFree(wt); cudaFree(wpop); cudaFree(tmul); cudaFree(tbias);
+  }
+};
+
+int lce_b200_bconv2d_bases_create(int m_bases, int n_planes, const lce_bconv2d_desc* terms,
+                                  const int32_t* const* filters, const float* const* post_mul,
+                                  const float* const* post_bias, lce_b200_bconv2d_bases** out_plan) {
+  *out_plan = nullptr;
+  if (lce_b200_device_count() < 1) return fail("no CUDA device: this library has no CPU path");
+  if (!terms || !filters || !post_mul || !post_bias) return fail("bconv2d_bases: null argument");
+  const lce_bconv2d_desc& d = terms[0];
+  int oh, ow, ph, pw;
+  if (lce_b200_bconv2d_out_shape(&d, &oh, &ow, &ph, &pw)) return 1;
+  if (const char* why = bases_refusal(d, m_bases, n_planes))
+    return fail("bconv2d_bases: the terms must be %s", why);
+  const int T = m_bases * n_planes;
+  for (int t = 1; t < T; ++t)
+    if (memcmp(&terms[t], &d, sizeof(d)) != 0)
+      return fail("bconv2d_bases: term %d's descriptor differs from term 0's", t);
+  for (int t = 0; t < T; ++t)
+    if (!filters[t] || !post_mul[t] || !post_bias[t]) return fail("bconv2d_bases: term %d lacks a constant", t);
+  const int cout = d.channels_out;
+  const int Kw = d.filter_h * d.filter_w * (d.channels_in / 32);
+  const size_t fwords = static_cast<size_t>(cout) * Kw;
+  // term (n, m) must convolve with base m's filter
+  {
+    std::vector<int32_t> f0(fwords), fn(fwords);
+    for (int m = 0; m < m_bases; ++m) {
+      if (to_host(filters[m], fwords * 4, f0.data())) return 1;
+      for (int n = 1; n < n_planes; ++n) {
+        if (to_host(filters[n * m_bases + m], fwords * 4, fn.data())) return 1;
+        if (f0 != fn) return fail("bconv2d_bases: term (%d, %d) does not share base %d's filter", n, m, m);
+      }
+    }
+  }
+  auto* plan = new lce_b200_bconv2d_bases();
+  plan->M = m_bases; plan->N = n_planes;
+  plan->ldc = cout + kChanPad;
+  const int n_slices = cdiv(Kw, 8);
+  const size_t tile_bytes = static_cast<size_t>(n_slices) * (8 * 32 * 8);
+  const int tiles = cout / lce::kBN;
+  plan->w_bytes = static_cast<unsigned>(tile_bytes * m_bases);
+  bases_staging(n_slices, m_bases, &plan->chunk_slices, &plan->chunks, &plan->reuse, &plan->smem);
+  auto cleanup = [&](int rc) {
+    delete plan;
+    return rc;
+  };
+  if (cudaMalloc(&plan->wt, static_cast<size_t>(tiles) * plan->w_bytes) != cudaSuccess ||
+      cudaMalloc(&plan->wpop, static_cast<size_t>(m_bases) * plan->ldc * 4) != cudaSuccess ||
+      cudaMemset(plan->wpop, 0, static_cast<size_t>(m_bases) * plan->ldc * 4) != cudaSuccess)
+    return cleanup(fail("bconv2d_bases: out of device memory"));
+  // each base's plan packs its fragments and popcounts; the tiles are interleaved base by base
+  for (int m = 0; m < m_bases; ++m) {
+    lce_b200_bconv2d* b = nullptr;
+    if (lce_b200_bconv2d_create(&d, filters[m], post_mul[m], post_bias[m], nullptr, &b)) return cleanup(1);
+    const GemmCore& c = b->core;
+    if (c.wt_nat == nullptr || !c.imma_b1) {
+      lce_b200_bconv2d_destroy(b);
+      return cleanup(fail("bconv2d_bases: no b1 weight fragments"));
+    }
+    const bool ok =
+        cudaMemcpy2D(reinterpret_cast<unsigned char*>(plan->wt) + m * tile_bytes, plan->w_bytes, c.wt_nat,
+                     tile_bytes, tile_bytes, tiles, cudaMemcpyDeviceToDevice) == cudaSuccess &&
+        cudaMemcpy(plan->wpop + static_cast<size_t>(m) * plan->ldc, c.wpop, static_cast<size_t>(cout) * 4,
+                   cudaMemcpyDeviceToDevice) == cudaSuccess;
+    if (m == 0) plan->geo = b;
+    else lce_b200_bconv2d_destroy(b);
+    if (!ok) return cleanup(fail("bconv2d_bases: weight copy failed"));
+  }
+  std::vector<float> fm(static_cast<size_t>(T) * plan->ldc, 0.f), fb(fm.size(), 0.f);
+  for (int t = 0; t < T; ++t)
+    if (fold_output_transform(d, post_mul[t], post_bias[t], fm.data() + static_cast<size_t>(t) * plan->ldc,
+                              fb.data() + static_cast<size_t>(t) * plan->ldc))
+      return cleanup(1);
+  void *dm = nullptr, *db = nullptr;
+  const int rc = to_device(fm.data(), fm.size() * 4, fm.size() * 4, &dm);
+  plan->tmul = static_cast<float*>(dm);
+  if (rc || to_device(fb.data(), fb.size() * 4, fb.size() * 4, &db)) return cleanup(1);
+  plan->tbias = static_cast<float*>(db);
+  *out_plan = plan;
+  return 0;
+}
+
+int lce_b200_bconv2d_bases_set_input_shape(lce_b200_bconv2d_bases* plan, int batch, int in_h, int in_w) {
+  return lce_b200_bconv2d_set_input_shape(plan->geo, batch, in_h, in_w);
+}
+
+int lce_b200_bconv2d_bases_get_desc(const lce_b200_bconv2d_bases* plan, lce_bconv2d_desc* d, int* out_h,
+                                    int* out_w) {
+  return lce_b200_bconv2d_get_desc(plan->geo, d, out_h, out_w);
+}
+
+int lce_b200_bconv2d_bases_run(lce_b200_bconv2d_bases* plan, const int32_t* const* planes_dev,
+                               const float* bn_scale_dev, const float* bn_shift_dev, int bn_activation,
+                               const float* residual_dev, int add_activation, float* out_dev, int n_next,
+                               const float* next_shifts, int32_t* const* next_planes_dev, void* stream) {
+  const lce_bconv2d_desc& d = plan->geo->d;
+  const GemmCore& c = plan->geo->core;
+  if (!planes_dev) return fail("bconv2d_bases_run: the input planes are required");
+  if (!bn_scale_dev || !bn_shift_dev || !is_device_ptr(bn_scale_dev) || !is_device_ptr(bn_shift_dev))
+    return fail("bconv2d_bases_run: the BatchNorm vectors must be device memory");
+  for (int a : {bn_activation, add_activation})
+    if (a < LCE_ACT_NONE || a > LCE_ACT_RELU6) return fail("bconv2d_bases_run: unknown activation %d", a);
+  if (n_next < 0 || n_next > lce::kMaxBases) return fail("bconv2d_bases_run: 0 to 8 next planes");
+  if (n_next > 0 && (!next_shifts || !next_planes_dev)) return fail("bconv2d_bases_run: next shifts and planes required");
+  if (residual_dev && !aligned16(residual_dev)) return fail("bconv2d_bases_run: residual must be 16-byte aligned");
+  if (out_dev && !aligned16(out_dev)) return fail("bconv2d_bases_run: output must be 16-byte aligned");
+  const long long M = static_cast<long long>(d.batch) * plan->geo->out_h * plan->geo->out_w;
+  const size_t in_bytes = static_cast<size_t>(d.batch) * d.in_h * d.in_w * (d.channels_in / 32) * 4;
+  const size_t out_bytes = static_cast<size_t>(M) * d.channels_out * 4;
+  const size_t pk_bytes = static_cast<size_t>(M) * (d.channels_out / 32) * 4;
+  auto overlaps = [](const void* a, size_t an, const void* b, size_t bn) {
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+    return a && b && a0 < b0 + bn && b0 < a0 + an;
+  };
+  // CTAs gather neighbouring pixels of the planes and read the shortcut: the outputs alias neither
+  for (int n = 0; n < plan->N; ++n) {
+    if (!planes_dev[n]) return fail("bconv2d_bases_run: input plane %d is NULL", n);
+    if ((reinterpret_cast<uintptr_t>(planes_dev[n]) & (4u * c.V - 1)) != 0)
+      return fail("bconv2d_bases_run: input planes must be %d-byte aligned", 4 * c.V);
+    if (overlaps(out_dev, out_bytes, planes_dev[n], in_bytes))
+      return fail("bconv2d_bases_run: the output overlaps an input plane");
+    for (int k = 0; k < n_next; ++k)
+      if (overlaps(next_planes_dev[k], pk_bytes, planes_dev[n], in_bytes))
+        return fail("bconv2d_bases_run: a next plane overlaps an input plane");
+  }
+  for (int k = 0; k < n_next; ++k) {
+    if (!next_planes_dev[k] || (reinterpret_cast<uintptr_t>(next_planes_dev[k]) & 7u) != 0)
+      return fail("bconv2d_bases_run: next planes must be 8-byte aligned");
+    if (overlaps(next_planes_dev[k], pk_bytes, residual_dev, out_bytes))
+      return fail("bconv2d_bases_run: a next plane overlaps the residual");
+  }
+  if (overlaps(out_dev, out_bytes, residual_dev, out_bytes))
+    return fail("bconv2d_bases_run: output must not overlap the residual");
+  lce::BasesParams bp;
+  memset(&bp, 0, sizeof(bp));
+  lce::ConvKParams& p = bp.p;
+  p.wt = plan->wt; p.out = out_dev; p.residual = residual_dev; p.residual_act = add_activation;
+  p.M = M;
+  p.H = d.in_h; p.W = d.in_w;
+  p.Cw_total = d.channels_in / 32; p.Cw_pg = c.Cw_pg; p.CwV = c.Cw_pg / c.V;
+  p.KH = d.filter_h; p.KW = d.filter_w;
+  p.sh = d.stride_h; p.sw = d.stride_w; p.dh = d.dilation_h; p.dw = d.dilation_w;
+  p.ph = plan->geo->pad_h; p.pw = plan->geo->pad_w; p.OH = plan->geo->out_h; p.OW = plan->geo->out_w;
+  p.cout = c.cout; p.cout_pg = c.cout; p.tiles_per_group = c.tiles_per_group;
+  p.Kv = c.Kv; p.Kc_v = plan->chunk_slices * 8 / c.V; p.n_chunks = plan->chunks;
+  p.clamp_min = c.clamp_min; p.clamp_max = c.clamp_max;
+  p.cw_out = d.channels_out / 32;
+  p.fd_ohw = lce::make_fastdiv(static_cast<uint32_t>(p.OH) * p.OW);
+  p.fd_ow = lce::make_fastdiv(p.OW);
+  p.fd_cwv = lce::make_fastdiv(p.CwV);
+  p.fd_kw = lce::make_fastdiv(p.KW);
+  p.fd_tpg = lce::make_fastdiv(p.tiles_per_group);
+  p.img_words = static_cast<long long>(p.H) * p.W * p.Cw_total;
+  for (int n = 0; n < plan->N; ++n) bp.planes[n] = planes_dev[n];
+  bp.tmul = plan->tmul; bp.tbias = plan->tbias; bp.wpop = plan->wpop;
+  bp.ldc = plan->ldc; bp.n_bases = plan->M; bp.n_planes = plan->N; bp.reuse = plan->reuse;
+  bp.bn_scale = bn_scale_dev; bp.bn_shift = bn_shift_dev; bp.bn_act = bn_activation;
+  bp.n_next = n_next;
+  for (int k = 0; k < n_next; ++k) {
+    bp.next_shift[k] = next_shifts[k];
+    bp.next_planes[k] = next_planes_dev[k];
+  }
+  bp.w_bytes = plan->w_bytes;
+  if (M == 0) return 0;
+  const long long m_tiles = (M + lce::kIBM - 1) / lce::kIBM;
+  if (m_tiles > INT_MAX) return fail("bconv2d_bases_run: too many output pixels");
+  if (p.img_words >= (1LL << 31)) return fail("bconv2d_bases_run: input image too large (>= 2^31 packed words)");
+  cudaStream_t s = as_stream(stream);
+  const dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(c.tiles_per_group));
+  switch (c.V) {
+    case 4: return launch_bases<4>(bp, grid, plan->smem, s);
+    case 2: return launch_bases<2>(bp, grid, plan->smem, s);
+    default: return launch_bases<1>(bp, grid, plan->smem, s);
+  }
+}
+
+void lce_b200_bconv2d_bases_destroy(lce_b200_bconv2d_bases* plan) { delete plan; }
 
 // --------------------------------- BGEMM --------------------------------- //
 int lce_b200_bgemm_create(int N, int Kw, const int32_t* W, const lce_bgemm_epilogue* ep,

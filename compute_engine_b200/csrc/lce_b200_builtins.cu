@@ -1196,6 +1196,28 @@ __global__ void __launch_bounds__(256) quant2_planes_kernel(
   }
 }
 
+// lce_b200_f32_shift_sign_planes: ABC-Net's N shifted signs of one float map, N x (ADD(x, shift_k) ->
+// LceQuantize), in one pass; one warp per pixel and 32-channel word, as quant2_planes_kernel.
+struct ShiftPlanes {
+  float shift[8];
+  int32_t* planes[8];
+};
+template <typename I>
+__global__ void __launch_bounds__(256) shift_sign_planes_kernel(const float* __restrict__ x, int C, int cw, int n,
+                                                                const __grid_constant__ ShiftPlanes sp, I words) {
+  const int lane = threadIdx.x & 31;
+  const I warps = static_cast<I>(gridDim.x) * (blockDim.x >> 5);
+  for (I wi = static_cast<I>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); wi < words; wi += warps) {
+    const I pix = wi / cw;
+    const int word = static_cast<int>(wi - pix * cw);
+    const float v = __ldg(x + pix * C + word * 32 + lane);
+    for (int k = 0; k < n; ++k) {
+      const unsigned b = __ballot_sync(0xffffffffu, __fadd_rn(v, sp.shift[k]) < 0.0f);
+      if (lane == 0) sp.planes[k][wi] = static_cast<int32_t>(b);
+    }
+  }
+}
+
 // LOGISTIC, TFLite's float reference (reference/logistic.h) with CUDA's expf
 __global__ void __launch_bounds__(256) logistic_kernel(const float* __restrict__ in,
                                                        float* __restrict__ out, long long n) {
@@ -2392,6 +2414,32 @@ int lce_b200_f32_quant2_planes(const float* x, int batch, int in_h, int in_w, in
   }
 #undef LCE_QUANT2
   return launch_check("quant2_planes_kernel");
+}
+
+int lce_b200_f32_shift_sign_planes(const float* x, int64_t pixels, int channels, int n_planes,
+                                   const float* shifts, int32_t* const* planes, void* stream) {
+  if (pixels < 0 || channels <= 0) return fail("shift_sign_planes: bad shape (%lld x %d)",
+                                               static_cast<long long>(pixels), channels);
+  if (channels % 32) return fail("shift_sign_planes: channels (%d) must be a multiple of 32", channels);
+  if (n_planes < 1 || n_planes > 8) return fail("shift_sign_planes: 1 to 8 planes, not %d", n_planes);
+  if (!shifts || !planes) return fail("shift_sign_planes: the shifts and planes are required");
+  ShiftPlanes sp{};
+  for (int k = 0; k < n_planes; ++k) {
+    if (!planes[k]) return fail("shift_sign_planes: plane %d is NULL", k);
+    sp.shift[k] = shifts[k];
+    sp.planes[k] = planes[k];
+  }
+  if (pixels == 0) return 0;
+  const int cw = channels / 32;
+  const long long words = pixels * cw;
+  const int grid = grid_for(words * 32, 256);
+  cudaStream_t s = as_stream(stream);
+  // 32-bit index arithmetic where the input and the word count fit
+  if (pixels * channels + 8LL * 32 * grid < (1LL << 31))
+    shift_sign_planes_kernel<int><<<grid, 256, 0, s>>>(x, channels, cw, n_planes, sp, static_cast<int>(words));
+  else
+    shift_sign_planes_kernel<long long><<<grid, 256, 0, s>>>(x, channels, cw, n_planes, sp, words);
+  return launch_check("shift_sign_planes_kernel");
 }
 
 int lce_b200_f32_grouped_conv2d(const lce_f32_conv_desc* d, int groups, const float* in, const float* filter,

@@ -667,5 +667,207 @@ bconv_imma_kernel(const ConvKParams p) {
   }
 }
 
+// ---- ABC-Net's multiple binary bases (lce_b200_bconv2d_bases_run) ----
+// One layer y = sum over n, m of t_nm, t_nm = OutputTransform_nm(bconv(A_n, B_m)), with N input
+// planes A_n and M weight bases B_m, then the BatchNorm, the optional shortcut and the next
+// layer's shifted signs. The M bases' b1 fragments for the CTA's 64-channel tile stay in shared
+// memory for the whole CTA (one TMA copy); the input planes stream through a two-deep ring:
+// with reuse, one whole-K plane per ring slot, multiplied by all M bases; otherwise one K chunk
+// per slot, gathered again for every base. One accumulator set: each finished term is folded
+// into a float running sum exactly as its own plan would output it (clamp, then the unfused
+// multiply and add), the sum starting from t_00 and adding the terms left to right in (n, m)
+// order, as the converter's ADD chain does.
+constexpr int kMaxBases = 8;
+struct BasesParams {
+  ConvKParams p;   // geometry, ring sizes, clamp, wt = [tile][M][n_slices] fragments,
+                   // residual / residual_act (the shortcut ADD), out (NULL: not stored), cw_out
+  const int32_t* planes[kMaxBases];   // the N packed input planes
+  const float* tmul;                  // [M * N][ldc] folded multipliers, term n * M + m
+  const float* tbias;                 // [M * N][ldc] folded biases
+  const int32_t* wpop;                // [M][ldc] popcount of each base's filter rows
+  int ldc, n_bases, n_planes, reuse;
+  const float* bn_scale;              // MUL(bn_scale) -> ADD(bn_shift, bn_act)
+  const float* bn_shift;
+  int bn_act;
+  int n_next;                         // the next layer's planes: bit = fl(out + shift) < 0
+  float next_shift[kMaxBases];
+  int32_t* next_planes[kMaxBases];
+  unsigned w_bytes;                   // one tile's fragments of all M bases
+};
+
+// TFLite's fused activation as the float builtins apply it
+__device__ __forceinline__ float bases_act(float x, int act) {
+  switch (act) {
+    case LCE_ACT_RELU: return fmaxf(x, 0.0f);
+    case LCE_ACT_RELU_N1_TO_1: return fminf(fmaxf(x, -1.0f), 1.0f);
+    case LCE_ACT_RELU6: return fminf(fmaxf(x, 0.0f), 6.0f);
+    default: return x;
+  }
+}
+
+template <int V>
+__global__ void __launch_bounds__(kIThreads, 1) bconv_bases_kernel(const __grid_constant__ BasesParams bp) {
+  const ConvKParams& p = bp.p;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ __align__(8) uint64_t wbar;
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int gid = lane >> 2, tig = lane & 3;
+  const int nt = blockIdx.y;
+  const long long m0 = static_cast<long long>(blockIdx.x) * kIBM;
+  const int c_tile = nt * kBN, cth = c_tile + tig * 2;
+  const int Kv_end = b1_padded_vectors(p.Kv, V);
+  const int n_slices = (Kv_end * V + 7) >> 3;
+  const int chunk_slices = (p.Kc_v * V + 7) >> 3;
+  const int M = bp.n_bases, nc = p.n_chunks;
+  const uint2* W_s = reinterpret_cast<const uint2*>(smem_raw);
+  unsigned char* A_base = smem_raw + bp.w_bytes;
+  const size_t a_bytes = static_cast<size_t>(chunk_slices) * kIBM * 32;
+
+  if (tid == 0) {
+    mbar_init(&wbar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&wbar, bp.w_bytes);
+    bulk_g2s(smem_raw, reinterpret_cast<const unsigned char*>(p.wt) + static_cast<size_t>(nt) * bp.w_bytes,
+             bp.w_bytes, &wbar);
+  }
+  // unit u of the ring: plane n, chunk ch (reuse: the whole K of plane u)
+  const int per_plane = bp.reuse ? 1 : M * nc;
+  const int U = bp.n_planes * per_plane;
+  auto stage = [&](int u) {
+    const int n = u / per_plane;
+    const int ch = bp.reuse ? 0 : (u - n * per_plane) % nc;
+    const int kv0 = ch * p.Kc_v;
+    const int kv1 = min(kv0 + p.Kc_v, Kv_end);
+    gather_tile<V, kIBM, kIThreads, true>(p, reinterpret_cast<typename VecT<V>::T*>(A_base + (u & 1) * a_bytes),
+                                         m0, 0, kv0, kv1, tid, bp.planes[n]);
+    cp_async_commit();
+  };
+
+  int acc[2][8][4];
+  int pa[2][4];
+  float sum[2][2][16];
+  auto clear = [&]() {
+#pragma unroll
+    for (int ms = 0; ms < 2; ++ms) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) pa[ms][e] = 0;
+#pragma unroll
+      for (int ns = 0; ns < 8; ++ns)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[ms][ns][e] = 0;
+    }
+  };
+  clear();
+  stage(0);
+  for (int u = 0; u < U; ++u) {
+    const bool more = u + 1 < U;
+    if (more) stage(u + 1);   // its slot was released by the barrier that ended unit u - 1
+    if (more) asm volatile("cp.async.wait_group 1;" ::: "memory");
+    else asm volatile("cp.async.wait_group 0;" ::: "memory");
+    if (u == 0) mbar_wait(&wbar, 0);
+    __syncthreads();
+    const uint32_t* A_b = reinterpret_cast<const uint32_t*>(A_base + (u & 1) * a_bytes);
+    const int n = u / per_plane;
+    const int r = u - n * per_plane;
+    const int m_lo = bp.reuse ? 0 : r / nc, m_hi = bp.reuse ? M : m_lo + 1;
+    const int ch = bp.reuse ? 0 : r % nc;
+    const int kv0 = ch * p.Kc_v;
+    const int words = (min(kv0 + p.Kc_v, Kv_end) - kv0) * V;
+    for (int m = m_lo; m < m_hi; ++m) {
+      compute_chunk_b1(A_b, W_s + (static_cast<size_t>(m) * n_slices + ch * chunk_slices) * 256, words,
+                       warp, gid, tig, lane, acc, pa);
+      if (ch != nc - 1) continue;
+      // the finished term t_nm: popc(a ^ w), OutputTransform, then into the running sum
+      const int term = n * M + m;
+      const float* tm = bp.tmul + static_cast<size_t>(term) * bp.ldc + cth;
+      const float* tb = bp.tbias + static_cast<size_t>(term) * bp.ldc + cth;
+      const int32_t* wp = bp.wpop + static_cast<size_t>(m) * bp.ldc + cth;
+#pragma unroll
+      for (int ns = 0; ns < 8; ++ns) {
+        const int2 pw = __ldg(reinterpret_cast<const int2*>(wp + ns * 8));
+        const float2 mu = __ldg(reinterpret_cast<const float2*>(tm + ns * 8));
+        const float2 bi = __ldg(reinterpret_cast<const float2*>(tb + ns * 8));
+#pragma unroll
+        for (int ms = 0; ms < 2; ++ms)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int x0 = (pw.x + pa[ms][h * 2] - 2 * acc[ms][ns][h * 2]) << 1;
+            const int x1 = (pw.y + pa[ms][h * 2 + 1] - 2 * acc[ms][ns][h * 2 + 1]) << 1;
+            const float y0 = transform_float_x2(x0, p.clamp_min, p.clamp_max, mu.x, bi.x);
+            const float y1 = transform_float_x2(x1, p.clamp_min, p.clamp_max, mu.y, bi.y);
+            sum[ms][h][2 * ns] = term == 0 ? y0 : __fadd_rn(sum[ms][h][2 * ns], y0);
+            sum[ms][h][2 * ns + 1] = term == 0 ? y1 : __fadd_rn(sum[ms][h][2 * ns + 1], y1);
+          }
+      }
+      clear();
+    }
+    __syncthreads();
+  }
+
+  // MUL(bn_scale) -> ADD(bn_shift, bn_act) [-> ADD(shortcut, residual_act)], then the next planes
+  const bool has_res = p.residual != nullptr;
+  float* out = static_cast<float*>(p.out);
+#pragma unroll
+  for (int ms = 0; ms < 2; ++ms) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long long m = m0 + warp * 32 + ms * 16 + h * 8 + gid;
+      const bool row_ok = m < p.M;
+      float* y = sum[ms][h];
+      if (row_ok) {
+        const size_t e0 = static_cast<size_t>(m) * p.cout + cth;
+#pragma unroll
+        for (int ns = 0; ns < 8; ++ns) {
+          const float2 s = __ldg(reinterpret_cast<const float2*>(bp.bn_scale + cth + ns * 8));
+          const float2 t = __ldg(reinterpret_cast<const float2*>(bp.bn_shift + cth + ns * 8));
+          y[2 * ns] = bases_act(__fadd_rn(__fmul_rn(y[2 * ns], s.x), t.x), bp.bn_act);
+          y[2 * ns + 1] = bases_act(__fadd_rn(__fmul_rn(y[2 * ns + 1], s.y), t.y), bp.bn_act);
+        }
+        if (has_res) {
+#pragma unroll
+          for (int ns = 0; ns < 8; ++ns) {
+            const float2 rv = __ldg(reinterpret_cast<const float2*>(p.residual + e0 + ns * 8));
+            y[2 * ns] = bases_act(__fadd_rn(y[2 * ns], rv.x), p.residual_act);
+            y[2 * ns + 1] = bases_act(__fadd_rn(y[2 * ns + 1], rv.y), p.residual_act);
+          }
+        }
+        if (out != nullptr) {
+#pragma unroll
+          for (int ns = 0; ns < 8; ++ns)
+            *reinterpret_cast<float2*>(out + e0 + ns * 8) = make_float2(y[2 * ns], y[2 * ns + 1]);
+        }
+      }
+      // LceQuantize(ADD(out, shift)): bit = fl(out + shift) < 0 (bitpack.h:159); the shuffles are
+      // uniform across the warp
+      for (int k = 0; k < bp.n_next; ++k) {
+        const float sh = bp.next_shift[k];
+        uint32_t bits0 = 0, bits1 = 0;
+#pragma unroll
+        for (int ns = 0; ns < 4; ++ns) {
+          bits0 |= ((__fadd_rn(y[2 * ns], sh) < 0.0f ? 1u : 0u) |
+                    (__fadd_rn(y[2 * ns + 1], sh) < 0.0f ? 2u : 0u)) << (ns * 8);
+          bits1 |= ((__fadd_rn(y[2 * ns + 8], sh) < 0.0f ? 1u : 0u) |
+                    (__fadd_rn(y[2 * ns + 9], sh) < 0.0f ? 2u : 0u)) << (ns * 8);
+        }
+        bits0 <<= tig * 2;
+        bits1 <<= tig * 2;
+        bits0 |= __shfl_xor_sync(0xffffffffu, bits0, 1);
+        bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 1);
+        bits0 |= __shfl_xor_sync(0xffffffffu, bits0, 2);
+        bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 2);
+        if (row_ok && tig == 0) {
+          int32_t* pk = bp.next_planes[k] + static_cast<size_t>(m) * p.cw_out + (c_tile >> 5);
+          pk[0] = static_cast<int32_t>(bits0);
+          pk[1] = static_cast<int32_t>(bits1);
+        }
+      }
+    }
+  }
+}
+
 }  // namespace lce
 #endif

@@ -279,9 +279,11 @@ __device__ __forceinline__ void split_pixel(const ConvKParams& p, long long m, l
 // zero-filling cp.async. Thread t handles pixel t % BM and every second k-vector.
 // kSliceRows: the layout is A_buf[k-slice][pixel][8 words] instead (k = (kv - kv0) * V words into
 // the chunk), and vectors at kv >= p.Kv -- the K tail padding -- are zero-filled.
+// `in` (optional) replaces p.in as the packed input: one of several input planes.
 template <int V, int BM_ = kBM, int NT_ = kThreads, bool kSliceRows = false>
 __device__ __forceinline__ void gather_tile(const ConvKParams& p, typename VecT<V>::T* A_buf,
-                                            long long m0, int g, int kv0, int kv1, int tid) {
+                                            long long m0, int g, int kv0, int kv1, int tid,
+                                            const int32_t* in = nullptr) {
   using Vec = typename VecT<V>::T;
   constexpr int kStep = NT_ / BM_;  // threads per pixel: each takes every kStep-th k-vector
   const int lp = tid & (BM_ - 1);
@@ -289,14 +291,15 @@ __device__ __forceinline__ void gather_tile(const ConvKParams& p, typename VecT<
   const long long gm = m0 + lp;
   const bool pix_valid = gm < p.M;
   int iy0 = 0, ix0 = 0;
-  const int32_t* img = p.in;
+  const int32_t* src_in = in != nullptr ? in : p.in;
+  const int32_t* img = src_in;
   if (pix_valid) {
     long long b;
     int oy, ox;
     split_pixel(p, gm, &b, &oy, &ox);
     iy0 = oy * p.sh - p.ph;
     ix0 = ox * p.sw - p.pw;
-    img = p.in + b * p.img_words + g * p.Cw_pg;
+    img = src_in + b * p.img_words + g * p.Cw_pg;
   }
   int kv = kv0 + half;
   int tap = static_cast<int>(fdiv(static_cast<uint32_t>(kv), p.fd_cwv));
@@ -312,7 +315,7 @@ __device__ __forceinline__ void gather_tile(const ConvKParams& p, typename VecT<
                         static_cast<unsigned>(ix) < static_cast<unsigned>(p.W);
     // offsets inside one image fit 32 bits (img_words < 2^31)
     const int off = (iy * p.W + ix) * p.Cw_total + cv * V;
-    const int32_t* src = inside ? img + off : p.in;
+    const int32_t* src = inside ? img + off : src_in;
     uint32_t d = dst;
     if constexpr (kSliceRows) {
       const uint32_t k = static_cast<uint32_t>(kv - kv0) * V;

@@ -206,6 +206,13 @@ class HostGraph:
         before fuse_float_glue, fuse_activation_chains and allocate_tensors."""
         return lib().lce_host_fuse_spatial_scales(self._g)
 
+    def fuse_binary_bases(self):
+        """ABC-Net's layer: N x (ADD(x, u_n) -> LceQuantize), M * N LceBconv2d terms, their
+        left-to-right ADD chain, MUL -> ADD (BatchNorm) [-> ADD(shortcut)] [-> the next layer's
+        shifted signs] => one node; planes of a map without such a producer => one node. Call
+        first in fuse_all: fuse_residual_blocks would take ADD(t_00, t_01) as a residual block."""
+        return lib().lce_host_fuse_binary_bases(self._g)
+
     def fuse_pooled_signs(self):
         """MAX_POOL_2D -> MUL(scale) -> ADD(shift) -> LceQuantize (BinaryAlexNet's and XNOR-Net's
         pooled BatchNorm and sign) => one node that writes only the signs. Call before
@@ -238,7 +245,8 @@ class HostGraph:
         return lib().lce_host_fuse_residual_pairs(self._g)
 
     def fuse_all(self):
-        return (self.fuse_dense_blocks() + self.fuse_residual_blocks() + self.fuse_spatial_scales()
+        return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_residual_blocks()
+                + self.fuse_spatial_scales()
                 + self.fuse_float_glue()
                 + self.fuse_grouped_conv_affine() + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
                 + self.fuse_residual_pairs())

@@ -432,6 +432,69 @@ def xnornetpp(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
     return g.m.serialize()
 
 
+def abcnet(batch=1, seed=0, image=224, input_type="float32", bases=(3, 3), pad_values=1):
+    """ABC-Net (Lin et al., NeurIPS 2017), restated from the paper on the ResNet-18 backbone with
+    synthetic weights, in the converter's op order; bases = (M, N) weight bases and shifted
+    activation signs.
+      ABC(x, C_out, k, stride): for n = 0..N-1, s_n = ADD(x, u_n) with u_n a one-element float
+      constant (the paper's v_n - 0.5, spread around 0) -> q_n = LceQuantize(s_n); then, n outer and
+      m inner, t_nm = LceBconv2d(q_n, B_m) k x k SAME (stride, `pad_values`, float output, no fused
+      activation, post_activation_multiplier gamma_nm [C_out] = the synthetic alpha_m * beta_n,
+      post_activation_bias 0), the M filters B_m shared by every n; y = ADD(...ADD(ADD(t_00, t_01),
+      t_02)..., t_{N-1,M-1}), left to right in that order.
+      stem CONV_2D 7x7/s2 3 -> 64 (BN folded, RELU) -> MAX_POOL_2D 3x3/s2 SAME;
+      4 stages x 2 basic blocks at 64 / 128 / 256 / 512 channels, stride 2 on the first block of
+      stages 2-4; a block on x: the shortcut first (x, or CONV_2D 1x1 with the block's stride, BN
+      folded); h = ADD(MUL(ABC(x, f, 3, s), bn_scale), bn_shift, RELU);
+      z = ADD(MUL(ABC(h, f, 3, 1), bn_scale'), bn_shift'); out = ADD(z, shortcut, RELU);
+      head MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX.
+    16 ABC layers, 16 * M * N LceBconv2d. Not in MODELS."""
+    m_bases, n_planes = bases
+    g = _Builder(seed, batch, "ABCNet")
+    xs = (batch, image, image, 3)
+    x = g.image_input(xs, input_type)
+    x, xs = g.conv(x, xs, 64, 7, 2, activation="RELU")
+    x, xs = g.pool("MAX_POOL_2D", x, xs, 3, 2, "SAME")
+    shifts = [0.0] if n_planes == 1 else list(np.linspace(-0.6, 0.6, n_planes))
+
+    def abc(t, ts, cout, k, stride):
+        b, h, w, cin = ts
+        qs = [g.quantize(g.add(t, g.const(np.array(u, np.float32), name="shift"), ts), ts) for u in shifts]
+        filts = []
+        for _ in range(m_bases):
+            signs = g.rng.integers(0, 2, (cout, k, k, cin), dtype=np.int8) * 2 - 1
+            bits = (signs < 0).astype(np.uint32).reshape(cout, k, k, cin // 32, 32)
+            filt = (bits << np.arange(32, dtype=np.uint32)).sum(-1, dtype=np.uint64).astype(np.uint32).view(np.int32)
+            filts.append(g.const(filt, np.int32, "bfilter"))
+        alpha = [g.rng.uniform(0.5, 1.5, cout).astype(np.float32) * np.float32(4.0 / (k * k * cin))
+                 for _ in range(m_bases)]
+        beta = g.rng.uniform(0.5, 1.5, n_planes).astype(np.float32)
+        oh, ow = -(-h // stride), -(-w // stride)
+        ys = (b, oh, ow, cout)
+        opts = bconv2d_options(cin, (stride, stride), (1, 1), 0, pad_values, 0)
+        y = None
+        for n in range(n_planes):
+            for m in range(m_bases):
+                t_nm = g.act(ys)
+                g.m.add_op("LceBconv2d", [qs[n], filts[m], g.const((alpha[m] * beta[n]).astype(np.float32), name="pmul"),
+                                          g.const(np.zeros(cout, np.float32), name="pbias"), -1], [t_nm],
+                           custom_options=opts)
+                y = t_nm if y is None else g.add(y, t_nm, ys)
+        return y, ys
+
+    for stage, f in enumerate((64, 128, 256, 512)):
+        for blk in range(2):
+            stride = 2 if (stage > 0 and blk == 0) else 1
+            s = g.conv(x, xs, f, 1, stride)[0] if stride == 2 or xs[3] != f else x
+            y, ys = abc(x, xs, f, 3, stride)
+            h = g.batchnorm(y, ys, "RELU")
+            z = g.batchnorm(abc(h, ys, f, 3, 1)[0], ys)
+            x, xs = g.add(z, s, ys, "RELU"), ys
+    probs = g.head(x, xs, relu=False)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
 def binarydensenet(batch=1, seed=0, image=224, input_type="float32", pad_values=0,
                    layers=(6, 6, 6, 5), reduction=(2.7, 2.7, 2.2), dilation=(1, 1, 1, 1),
                    name="BinaryDenseNet28"):

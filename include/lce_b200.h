@@ -263,6 +263,49 @@ int lce_b200_f32_round(const float* in_dev, float* out_dev, int64_t n, void* str
 int lce_b200_f32_quant2_planes(const float* x_dev, int batch, int in_h, int in_w, int channels,
                                int filter_h, int filter_w, int stride_h, int stride_w, int padding,
                                int activation, int32_t* planes_out_dev, void* stream);
+/* ---- ABC-Net's multiple binary bases (Lin et al., NeurIPS 2017) ---------
+ * One layer y = sum over n < N, m < M of t_nm, where t_nm is an LceBconv2d (float output) of input
+ * plane A_n with base filter B_m, followed by the BatchNorm, an optional shortcut and the next
+ * layer's shifted signs:
+ *   y = (...((t_00 + t_01) + t_02) ... + t_{N-1,M-1})   (left to right, n outer, m inner)
+ *   o = bn_act(fl(fl(y * bn_scale[c]) + bn_shift[c]));  out = residual ? add_act(fl(o + residual)) : o
+ *   next_planes[k] = bitpack(fl(out + next_shifts[k]) < 0)
+ * Each t_nm is exactly what lce_b200_bconv2d_run computes for term (n, m)'s own plan, and the sums and
+ * the tail round as TFLite's ADD and MUL do, so the result is bit-identical to the M * N + N + 3 ops.
+ * bases_create takes the M * N terms in that order (index n * M + m): their descriptors (all equal),
+ * filters (term (n, m)'s filter must equal term (0, m)'s) and post_mul / post_bias (host or device).
+ * It refuses, with a message: terms that are not float output without a fused activation; grouped
+ * terms; channels_in % 32 != 0 or channels_out % 64 != 0; zero padding (SAME with pad_values 0,
+ * whose optimised result needs a per-term float correction: run such terms unfused); more than 8
+ * bases or planes; M bases whose b1 fragments for one 64-channel tile (M * ceil(k*k*channels_in/256)
+ * * 2 KB) leave no room for two 4 KB input slices in one CTA's 227 KB of shared memory; and
+ * LCE_B200_BCONV_IMMA or _B1 set to 0.
+ * bases_run: planes_dev[N] are the packed inputs [batch, in_h, in_w, channels_in / 32]; bn_scale /
+ * bn_shift are required device vectors [channels_out]; residual (may be NULL) and out (may be NULL:
+ * not stored) are float [batch, out_h, out_w, channels_out]; next_shifts[n_next] (host floats) and
+ * next_planes_dev[n_next] ([batch, out_h, out_w, channels_out / 32], 8-byte aligned) with n_next in
+ * 0..8. Activations are LCE_ACT_* codes. The outputs must not overlap the input planes or the
+ * residual. The M bases' fragments stay in shared memory for the whole CTA. */
+typedef struct lce_b200_bconv2d_bases lce_b200_bconv2d_bases;
+int lce_b200_bconv2d_bases_create(int m_bases, int n_planes, const lce_bconv2d_desc* terms,
+                                  const int32_t* const* filters, const float* const* post_mul,
+                                  const float* const* post_bias, lce_b200_bconv2d_bases** plan);
+int lce_b200_bconv2d_bases_set_input_shape(lce_b200_bconv2d_bases* plan, int batch, int in_h,
+                                           int in_w);
+int lce_b200_bconv2d_bases_get_desc(const lce_b200_bconv2d_bases* plan, lce_bconv2d_desc* d,
+                                    int* out_h, int* out_w);
+int lce_b200_bconv2d_bases_run(lce_b200_bconv2d_bases* plan, const int32_t* const* planes_dev,
+                               const float* bn_scale_dev, const float* bn_shift_dev,
+                               int bn_activation, const float* residual_dev, int add_activation,
+                               float* out_dev, int n_next, const float* next_shifts,
+                               int32_t* const* next_planes_dev, void* stream);
+void lce_b200_bconv2d_bases_destroy(lce_b200_bconv2d_bases* plan);
+/* ABC-Net's shifted signs of a float map without a fused producer, N x (ADD(x, shifts[k]) ->
+ * LceQuantize), in one pass over x [pixels, channels] (channels % 32 == 0):
+ *   planes[k][pixel][channels / 32] = bitpack(fl(x + shifts[k]) < 0),  1 <= n_planes <= 8,
+ * shifts on the host, planes device pointers. Bit-identical to the 2 N ops. */
+int lce_b200_f32_shift_sign_planes(const float* x_dev, int64_t pixels, int channels, int n_planes,
+                                   const float* shifts, int32_t* const* planes_dev, void* stream);
 /* Grouped CONV_2D (TF/lite/kernels/conv.cc with groups = in_c / filter_in): x NHWC [batch, in_h,
  * in_w, d->in_c], filter OHWI [d->out_c, filter_h, filter_w, d->in_c / groups]; output channel o reads
  * the input channels [(o / (out_c / groups)) * in_c / groups, ...). `groups` must divide in_c and
