@@ -441,6 +441,7 @@ void Graph::SetCustomOptions(NodeRecord& n, std::vector<uint8_t> options) {
 }
 
 extern "C" TfLiteRegistration* lce_b200_internal_Register_BCONV_2D_FUSED(const TfLiteRegistration* original);
+extern "C" int lce_b200_internal_grouped_packs(const lce_bconv2d_desc* d);   // lce_b200.cu
 
 int Graph::FuseResidualBlocks() {
   if (!device_arena_) return 0;
@@ -462,12 +463,24 @@ int Graph::FuseResidualBlocks() {
     if (tensors_[r].type != kTfLiteFloat32 || tensors_[r].allocation_type == kTfLiteMmapRo) continue;
     // Preconditions of the fused kernel, checked before the graph is rewritten (both graphs below
     // run correctly unfused): the shortcut has exactly the convolution's shape (ADD would also
-    // accept a broadcast over the last dimension), and the convolution is not grouped (the fused
-    // sign-pack needs groups == 1): filter words per pixel == input words per pixel.
+    // accept a broadcast over the last dimension), and the convolution is ungrouped (filter words
+    // per pixel == input words per pixel) or grouped such that the fused sign-pack takes it. Of the
+    // grouped layers only those with channels_in == channels_out are fused: binary MobileNets'
+    // layers in place of depthwise convolutions, the case this fusion is measured on; other
+    // grouped layers run unfused.
     if (!SameDims(tensors_[y].dims, tensors_[r].dims)) continue;
     const TfLiteIntArray* xs = tensors_[b.node.inputs->data[0]].dims;
     const TfLiteIntArray* fs = tensors_[b.node.inputs->data[1]].dims;
-    if (!xs || !fs || xs->size != 4 || fs->size != 4 || xs->data[3] != fs->data[3]) continue;
+    if (!xs || !fs || xs->size != 4 || fs->size != 4 || fs->data[3] < 1 || xs->data[3] % fs->data[3] != 0)
+      continue;
+    if (xs->data[3] != fs->data[3]) {
+      lce_bconv2d_desc d{};
+      d.channels_in = FlexMap(b.custom_options.data(), b.custom_options.size()).AsInt32("channels_in");
+      d.channels_out = fs->data[0];
+      d.groups = xs->data[3] / fs->data[3];
+      d.out_type = LCE_OUT_FLOAT;
+      if (d.channels_in != d.channels_out || !lce_b200_internal_grouped_packs(&d)) continue;
+    }
     // the shortcut must already exist when the bconv runs
     if (!ReadyBefore(r, i)) continue;
     const int o = a.node.outputs->data[0];

@@ -22,6 +22,9 @@
 #include "lce_b200.h"
 #include "lce_b200_tflite.h"
 
+// lce_b200.cu: whether run_fused / run_fused_chain take packed output for a plan of *d
+extern "C" int lce_b200_internal_grouped_packs(const lce_bconv2d_desc* d);
+
 namespace {
 
 // The stream the ops launch on: set by the graph host before it walks its nodes. Thread local:
@@ -331,7 +334,7 @@ TfLiteStatus BconvPrepare(TfLiteContext* context, TfLiteNode* node) {
                                            NumElements(v) == d.channels_out));
     }
     if (node->outputs->size > 1) {
-      LCE_ENSURE(context, d.groups == 1);
+      LCE_ENSURE(context, lce_b200_internal_grouped_packs(&d));
       TfLiteIntArray* packed_shape = LceB200IntArrayCreate(4);
       packed_shape->data[0] = d.batch;
       packed_shape->data[1] = out_h;

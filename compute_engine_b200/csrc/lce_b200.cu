@@ -144,6 +144,7 @@ struct GemmCore {
   int32_t* wt_nat = nullptr;    // weights in mma B-fragment order: packed b1, or expanded to int8
   int32_t* wpop = nullptr;      // popcount of each channel's filter row (padded by BN)
   bool imma_b1 = false;         // b1 fragments (default) or int8 ones (LCE_B200_BCONV_B1=0)
+  bool imma_win = false;        // b1 group windows: groups of 32 * odd output channels (GW)
   // a 32-channel layer the pair kernel takes: its b1 fragments for that kernel alone (wpop filled
   // too); the plan's own launches stay on the kernels below, which take every other channel count
   int32_t* pair_wt = nullptr;
@@ -193,20 +194,37 @@ size_t imma_smem_budget(int V, bool b1) {
 }
 
 template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
-          bool SPATIAL = false>
+          bool SPATIAL = false, bool GW = false>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(imma_smem_budget(V, B1))));
-  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL><<<grid, lce::kIThreads, smem, s>>>(p);
+  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW><<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
 // Epilogue tails of the float output beyond run_fused's (bconv_run_impl decides).
 // kScale: p.gate indexed by position within the image (lce_b200_bconv2d_run_fused_scale)
 enum class Tail { kNone, kChain, kGate, kScale, kSlice };   // p.chain / p.gate / p.out_stride in the epilogue
+
+// group-window plans (b1 only): every tail but the slice store
+template <int V>
+int launch_imma_win_v(int out_type, Tail tail, const lce::ConvKParams& p, dim3 grid, size_t smem,
+                      cudaStream_t s) {
+  constexpr int F = LCE_OUT_FLOAT;
+  switch (tail) {
+    case Tail::kChain: return launch_imma_vo<V, F, true, true, false, false, false, true>(p, grid, smem, s);
+    case Tail::kGate: return launch_imma_vo<V, F, true, false, true, false, false, true>(p, grid, smem, s);
+    case Tail::kScale: return launch_imma_vo<V, F, true, false, true, false, true, true>(p, grid, smem, s);
+    case Tail::kSlice: return fail("bconv2d: the slice store takes no grouped plan with 32 * odd channels per group");
+    case Tail::kNone: break;
+  }
+  if (out_type == LCE_OUT_BITPACKED)
+    return launch_imma_vo<V, LCE_OUT_BITPACKED, true, false, false, false, false, true>(p, grid, smem, s);
+  return launch_imma_vo<V, F, true, false, false, false, false, true>(p, grid, smem, s);
+}
 
 template <int V>
 int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, dim3 grid,
@@ -278,6 +296,19 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, Tail tail = Ta
     const size_t ismem = c.imma_smem;
     dim3 igrid(static_cast<unsigned>((p.M + lce::kIBM - 1) / lce::kIBM),
                static_cast<unsigned>(c.groups * c.tiles_per_group));
+    if (c.imma_win) {
+      // K = taps x the window's two groups of input words; 64-channel tiles over all channels
+      q.Kv = 2 * p.Kv;
+      q.CwV = 2 * p.CwV;
+      q.fd_cwv = lce::make_fastdiv(q.CwV);
+      q.win_step = 8 % (2 * c.Cw_pg);
+      igrid.y = static_cast<unsigned>(cdiv(c.cout, lce::kBN));
+      switch (c.V) {
+        case 4: return launch_imma_win_v<4>(c.out_type, tail, q, igrid, ismem, s);
+        case 2: return launch_imma_win_v<2>(c.out_type, tail, q, igrid, ismem, s);
+        default: return launch_imma_win_v<1>(c.out_type, tail, q, igrid, ismem, s);
+      }
+    }
     switch (c.V) {
       case 4: return launch_imma_v<4>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
       case 2: return launch_imma_v<2>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
@@ -665,21 +696,27 @@ int build_core_weights(GemmCore* c, const int32_t* filter, bool want_tap_popc, b
   // tiles, float, bitpacked or raw-accumulator output. LCE_B200_BCONV_IMMA=0 leaves every plan
   // to the wgmma / XOR + POPC kernels (bench.py reports both). LCE_B200_BCONV_B1=0 keeps the
   // int8 fragments instead of the packed b1 ones; both give the same accumulators.
-  if (!env_off("LCE_B200_BCONV_IMMA") && c->cout_pg % lce::kBN == 0 && c->out_type != LCE_OUT_INT8) {
+  // Grouped plans with 32 * odd output channels per group take the b1 fragments over group
+  // windows (bconv_imma_kernel's GW); with int8 fragments they stay on the kernels below.
+  const bool imma_on = !env_off("LCE_B200_BCONV_IMMA") && c->out_type != LCE_OUT_INT8;
+  c->imma_win = imma_on && c->groups > 1 && c->cout_pg % lce::kBN == 32 && !env_off("LCE_B200_BCONV_B1");
+  if (imma_on && (c->cout_pg % lce::kBN == 0 || c->imma_win)) {
     const int Kw = c->taps * c->Cw_pg;
     c->imma_b1 = !env_off("LCE_B200_BCONV_B1");
     const size_t budget = imma_smem_budget(c->V, c->imma_b1);
     if (c->imma_b1) {
-      const int n_slices = cdiv(Kw, 8);  // 8-word k-slices, the last one padded to 4 or 8 words
-      const long long total = static_cast<long long>(c->groups) * c->tiles_per_group * n_slices * 256;
+      const int win = c->imma_win ? 2 : 1;   // a group window holds two groups' words per tap
+      const int n_slices = cdiv(win * Kw, 8);  // 8-word k-slices, the last one padded to 4 or 8 words
+      const long long n_tiles = c->imma_win ? cdiv(c->cout, lce::kBN) : c->groups * c->tiles_per_group;
+      const long long total = n_tiles * n_slices * 256;
       CUDA_OK(cudaMalloc(&c->wt_nat, total * 8));
       lce::pack_weights_b1_kernel<<<grid_for(total, 256, 1 << 22), 256>>>(
-          d_filter, reinterpret_cast<uint2*>(c->wt_nat), c->cout_pg, c->tiles_per_group, Kw,
-          n_slices, total);
+          d_filter, reinterpret_cast<uint2*>(c->wt_nat), c->cout_pg, c->tiles_per_group, win * Kw,
+          n_slices, total, c->imma_win ? c->Cw_pg : 0, c->groups);
       if (launch_check("pack_weights_b1_kernel")) return 1;
       // K staging: one chunk when it fits kB1SmemCtas CTAs per SM, else a two-deep ring of
       // chunks of whole 8-word slices
-      const int Kvp = lce::b1_padded_vectors(c->Kv, c->V);
+      const int Kvp = lce::b1_padded_vectors(win * c->Kv, c->V);
       const size_t slice_bytes = lce::kB1BytesPerSlice;
       if (n_slices * slice_bytes <= budget) {
         c->imma_chunks = 1;
@@ -776,6 +813,17 @@ const char* slice_refusal(const lce_bconv2d_desc& d, const GemmCore* c) {
   if (!imma)
     return "the mma.sync weight fragments (channels_out a multiple of 64, LCE_B200_BCONV_IMMA not 0)";
   return nullptr;
+}
+
+// Whether lce_b200_bconv2d_run_fused / _run_fused_chain take packed output for the plan: every
+// ungrouped plan, and grouped float-output plans with channels_out / groups a multiple of 32 on the
+// b1 mma.sync weight fragments, whose epilogue packs whole 32-channel words of one CTA.
+// c == nullptr: for a plan not created yet (LCE_B200_BCONV_IMMA and _B1 not 0).
+bool grouped_packs(const lce_bconv2d_desc& d, const GemmCore* c) {
+  if (d.groups == 1) return true;
+  if (d.out_type != LCE_OUT_FLOAT || d.groups < 1 || (d.channels_out / d.groups) % 32 != 0) return false;
+  if (c != nullptr) return c->wt_nat != nullptr && c->imma_b1;
+  return !env_off("LCE_B200_BCONV_IMMA") && !env_off("LCE_B200_BCONV_B1");
 }
 
 template <int CW>
@@ -1294,8 +1342,9 @@ int lce_b200_bconv2d_run_fused(lce_b200_bconv2d* plan, const int32_t* in_dev,
                                int32_t* packed_out_dev, void* stream) {
   if (plan->d.out_type != LCE_OUT_FLOAT)
     return fail("bconv2d_run_fused: only float-output plans can take a residual");
-  if (packed_out_dev && plan->d.groups != 1)
-    return fail("bconv2d_run_fused: packed output needs groups == 1");
+  if (packed_out_dev && !grouped_packs(plan->d, &plan->core))
+    return fail("bconv2d_run_fused: packed output needs groups == 1, or channels_out / groups a "
+                "multiple of 32 on the b1 mma.sync kernel");
   if (residual_dev && (reinterpret_cast<uintptr_t>(residual_dev) & 15u) != 0)
     return fail("bconv2d_run_fused: residual must be 16-byte aligned");
   return bconv_run_impl(plan, in_dev, out_dev, residual_dev, add_activation, packed_out_dev,
@@ -1308,8 +1357,9 @@ int lce_b200_bconv2d_run_fused_chain(lce_b200_bconv2d* plan, const int32_t* in_d
                                      int32_t* packed_out_dev, void* stream) {
   if (plan->d.out_type != LCE_OUT_FLOAT)
     return fail("bconv2d_run_fused_chain: only float-output plans can take a chain");
-  if (packed_out_dev && plan->d.groups != 1)
-    return fail("bconv2d_run_fused_chain: packed output needs groups == 1");
+  if (packed_out_dev && !grouped_packs(plan->d, &plan->core))
+    return fail("bconv2d_run_fused_chain: packed output needs groups == 1, or channels_out / groups "
+                "a multiple of 32 on the b1 mma.sync kernel");
   if (residual_dev && (reinterpret_cast<uintptr_t>(residual_dev) & 15u) != 0)
     return fail("bconv2d_run_fused_chain: residual must be 16-byte aligned");
   if (chain)
@@ -1447,6 +1497,12 @@ int lce_b200_bconv2d_run_slice_add(lce_b200_bconv2d* plan, const int32_t* in_dev
 // (Graph::FuseDenseBlocks asks before it rewrites the graph).
 int lce_b200_internal_slice_takes(const lce_bconv2d_desc* d) {
   return slice_refusal(*d, nullptr) == nullptr;
+}
+
+// host-internal (Graph::FuseResidualBlocks, BconvPrepare): run_fused / run_fused_chain take
+// packed output for a plan created now from *d; no device needed
+int lce_b200_internal_grouped_packs(const lce_bconv2d_desc* d) {
+  return grouped_packs(*d, nullptr);
 }
 
 // host-internal (Graph::FuseBinaryBases): lce_b200_bconv2d_bases_create would take M * N terms of

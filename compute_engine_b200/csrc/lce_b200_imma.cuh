@@ -61,6 +61,8 @@ constexpr int kIBytesPerWord = kIBM * 4 + 8 * 32 * 8;  // smem per K word: packe
 // holds for every QuickNet layer; the register cap allows kB1Ctas.
 constexpr int kB1BytesPerSlice = kIBM * 32 + 8 * 32 * 8;
 constexpr int kB1Ctas = 4;
+// the bitpacked group-window instance needs more than 128 registers: 3 CTAs per SM (168)
+__host__ __device__ constexpr int b1_ctas_per_sm(bool gw, int out) { return gw && out == LCE_OUT_BITPACKED ? 3 : kB1Ctas; }
 constexpr int kB1SmemCtas = 2;
 // K words padded up to the b1 instructions' granularity (4 words = m16n8k128), in vectors of V
 __host__ __device__ constexpr int b1_padded_vectors(int Kv, int V) { return ((Kv * V + 3) & ~3) / V; }
@@ -186,9 +188,13 @@ __device__ __forceinline__ void bmma_k128(int (&c)[4], uint32_t a0, uint32_t a1,
 // channel ns*8 + lane/4 that `lane` feeds to the b1 mma (see above); two neighbouring sub-tiles
 // side by side so one 128-bit LDS fetches both. A k128 tail slice has {word tig, 0}. Words past
 // Kw and channels past the group's end are 0.
+// win_cw > 0: a group-window plan (see bconv_imma_kernel's GW), Cw_pg = win_cw, `groups` groups;
+// tiles run over all channels (tiles_per_group unused) and K = taps x [window group 0's win_cw
+// words | window group 1's], Kw = taps * 2 * win_cw. Each channel's filter words sit in its own
+// group's half of the window and the other half is 0: the fragments are block-diagonal.
 __global__ void pack_weights_b1_kernel(const int32_t* __restrict__ filter, uint2* __restrict__ wtb,
                                        int cout_pg, int tiles_per_group, int Kw, int n_slices,
-                                       long long total) {
+                                       long long total, int win_cw = 0, int groups = 1) {
   const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (idx >= total) return;
   const int ns = static_cast<int>(((idx >> 6) & 3) * 2 + (idx & 1));
@@ -196,25 +202,49 @@ __global__ void pack_weights_b1_kernel(const int32_t* __restrict__ filter, uint2
   const long long r = idx >> 8;
   const int s = static_cast<int>(r % n_slices);
   const int nt = static_cast<int>(r / n_slices);
-  const int g = nt / tiles_per_group, tg = nt - g * tiles_per_group;
-  const int ch = tg * kBN + ns * 8 + (lane >> 2);
   const int tig = lane & 3;
   const bool tail = s * 8 + 4 >= ((Kw + 3) & ~3);
   const int k0 = s * 8 + (tail ? tig : 2 * tig);
-  const int32_t* row = filter + (static_cast<long long>(g) * cout_pg + ch) * Kw;
-  const bool ch_ok = ch < cout_pg;
-  const uint32_t w0 = ch_ok && k0 < Kw ? static_cast<uint32_t>(row[k0]) : 0u;
-  const uint32_t w1 = ch_ok && !tail && k0 + 1 < Kw ? static_cast<uint32_t>(row[k0 + 1]) : 0u;
+  uint32_t w0, w1;
+  if (win_cw > 0) {
+    const int c = nt * kBN + ns * 8 + (lane >> 2);
+    const int gb = min(nt * kBN / cout_pg, groups - 2), gc = c / cout_pg;
+    auto word = [&](int k) -> uint32_t {
+      const int tap = k / (2 * win_cw), wi = k - tap * 2 * win_cw;
+      if (c >= cout_pg * groups || k >= Kw || gb + wi / win_cw != gc) return 0u;
+      return static_cast<uint32_t>(filter[static_cast<long long>(c) * (Kw / 2) + tap * win_cw + wi % win_cw]);
+    };
+    w0 = word(k0);
+    w1 = tail ? 0u : word(k0 + 1);
+  } else {
+    const int g = nt / tiles_per_group, tg = nt - g * tiles_per_group;
+    const int ch = tg * kBN + ns * 8 + (lane >> 2);
+    const int32_t* row = filter + (static_cast<long long>(g) * cout_pg + ch) * Kw;
+    const bool ch_ok = ch < cout_pg;
+    w0 = ch_ok && k0 < Kw ? static_cast<uint32_t>(row[k0]) : 0u;
+    w1 = ch_ok && !tail && k0 + 1 < Kw ? static_cast<uint32_t>(row[k0 + 1]) : 0u;
+  }
   wtb[idx] = make_uint2(w0, w1);
 }
 
-// acc += popc(a & w) and pa += popc(a) over `words` K words (a multiple of 4) of one chunk
+// acc += popc(a & w) and pa += popc(a) over `words` K words (a multiple of 4) of one chunk.
+// GW (group window, K = taps x [window group 0's cw words | window group 1's], the chunk starting
+// at window word k0): pa column n counts only window group (n & 1)'s bits. The popc BMMA's B
+// fragment is that group's mask instead of all ones, so pa[ms][e] holds group e & 1's popcount.
+template <bool GW = false>
 __device__ __forceinline__ void compute_chunk_b1(const uint32_t* A_s, const uint2* B_s, int words,
                                                  int warp, int gid, int tig, int lane,
-                                                 int (&acc)[2][8][4], int (&pa)[2][4]) {
+                                                 int (&acc)[2][8][4], int (&pa)[2][4], int k0 = 0,
+                                                 int cw = 0, int step = 0) {
   const uint4* b4 = reinterpret_cast<const uint4*>(B_s) + lane;
   const uint2* a2 = reinterpret_cast<const uint2*>(A_s) + (warp * 32 + gid) * 4 + tig;
   const int full = words >> 3;
+  // GW: r = the window position of this thread's word 2 * tig of the slice, advanced 8 (step =
+  // 8 % cw2) per slice
+  const int cw2 = 2 * cw;
+  auto mask = [&](int q) { return (q >= cw) != (gid & 1) ? 0u : ~0u; };
+  int r = 0;
+  if constexpr (GW) r = (k0 + 2 * tig) % cw2;
 #pragma unroll 2
   for (int s = 0; s < full; ++s) {
     uint32_t a[2][4];
@@ -232,8 +262,15 @@ __device__ __forceinline__ void compute_chunk_b1(const uint32_t* A_s, const uint
       bmma_k256(acc[0][2 * np + 1], a[0], b.z, b.w);
       bmma_k256(acc[1][2 * np + 1], a[1], b.z, b.w);
     }
-    bmma_k256(pa[0], a[0], ~0u, ~0u);
-    bmma_k256(pa[1], a[1], ~0u, ~0u);
+    uint32_t m0 = ~0u, m1 = ~0u;
+    if constexpr (GW) {
+      m0 = mask(r);
+      m1 = mask(r + 1 == cw2 ? 0 : r + 1);
+      r += step;
+      if (r >= cw2) r -= cw2;
+    }
+    bmma_k256(pa[0], a[0], m0, m1);
+    bmma_k256(pa[1], a[1], m0, m1);
   }
   if (words & 4) {
     const uint32_t* a1 = A_s + (full * kIBM + warp * 32 + gid) * 8 + tig;
@@ -252,8 +289,10 @@ __device__ __forceinline__ void compute_chunk_b1(const uint32_t* A_s, const uint
         bmma_k128(acc[ms][2 * np + 1], lo[ms], hi[ms], b.z);
       }
     }
+    uint32_t m = ~0u;
+    if constexpr (GW) m = mask((k0 + full * 8 + tig) % cw2);
 #pragma unroll
-    for (int ms = 0; ms < 2; ++ms) bmma_k128(pa[ms], lo[ms], hi[ms], ~0u);
+    for (int ms = 0; ms < 2; ++ms) bmma_k128(pa[ms], lo[ms], hi[ms], m);
   }
 }
 
@@ -312,7 +351,10 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // SLICE (float output, no signs): row m goes to out + m * p.out_stride, a channel slice of a
 // wider map; a shortcut is read at the same strided address, which may be the output itself.
 // BITPACKED: the row's two output words, bit = acc > p.thr[c], packed like the float output's signs.
-template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false, bool SPATIAL = false>
+// GW (group-window plans): the last tile may hold only 32 channels (channels_out % 64 == 32); its
+// upper half (ns 4..7, the second output word) is then neither read nor written.
+template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false, bool SPATIAL = false,
+          bool GW = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
                                               int tig, const float* chain_s = nullptr) {
@@ -322,6 +364,7 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
   static_assert(OUT != LCE_OUT_BITPACKED || !(CHAIN || GATE || SLICE), "float tails only");
   constexpr bool STAGED = CHAIN || GATE;
   const int cth = c_tile + tig * 2;
+  const bool hi = !GW || c_tile + 32 < p.cout;
   float2 mul_r[8], bias_r[8];
   int2 thr_r[8];
   if (OUT == LCE_OUT_FLOAT && !STAGED) {
@@ -356,8 +399,9 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           int* o = static_cast<int*>(p.out) + e0;
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns)
-            *reinterpret_cast<int2*>(o + ns * 8) =
-                make_int2(acc[ms][ns][h * 2] >> S, acc[ms][ns][h * 2 + 1] >> S);
+            if (ns < 4 || hi)
+              *reinterpret_cast<int2*>(o + ns * 8) =
+                  make_int2(acc[ms][ns][h * 2] >> S, acc[ms][ns][h * 2 + 1] >> S);
         }
         continue;
       }
@@ -405,7 +449,8 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           const bool has_a = p.gate.alpha != nullptr;
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns) {
-            const float2 gv = __ldg(reinterpret_cast<const float2*>(gr + ns * 8));
+            const float2 gv = ns < 4 || hi ? __ldg(reinterpret_cast<const float2*>(gr + ns * 8))
+                                           : make_float2(0.0f, 0.0f);
             const float2 al = *reinterpret_cast<const float2*>(chain_s + kBN + tig * 2 + ns * 8);
             y[2 * ns] = gate_prelu(y[2 * ns], gv.x, has_a, al.x);
             y[2 * ns + 1] = gate_prelu(y[2 * ns + 1], gv.y, has_a, al.y);
@@ -420,8 +465,9 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           // (non-coherent) path
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns)
-            rv[ns] = SLICE ? __ldcg(reinterpret_cast<const float2*>(r + ns * 8))
-                           : __ldg(reinterpret_cast<const float2*>(r + ns * 8));
+            rv[ns] = !(ns < 4 || hi) ? make_float2(0.0f, 0.0f)
+                     : SLICE         ? __ldcg(reinterpret_cast<const float2*>(r + ns * 8))
+                                     : __ldg(reinterpret_cast<const float2*>(r + ns * 8));
 #pragma unroll
           for (int ns = 0; ns < 8; ++ns) {
             y[2 * ns] = __fadd_rn(y[2 * ns], rv[ns].x);
@@ -455,7 +501,7 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
         float* o = static_cast<float*>(p.out) + e0;
 #pragma unroll
         for (int ns = 0; ns < 8; ++ns)
-          *reinterpret_cast<float2*>(o + ns * 8) = make_float2(y[2 * ns], y[2 * ns + 1]);
+          if (ns < 4 || hi) *reinterpret_cast<float2*>(o + ns * 8) = make_float2(y[2 * ns], y[2 * ns + 1]);
         if (has_pk) {
           if constexpr (CHAIN) {
             // RSign: LceQuantize of the value just written plus sign_shift
@@ -507,7 +553,7 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           int32_t* pk = (OUT == LCE_OUT_BITPACKED ? static_cast<int32_t*>(p.out) : p.packed_out) +
                         static_cast<size_t>(m) * p.cw_out + (c_tile >> 5);
           pk[0] = static_cast<int32_t>(bits0);
-          pk[1] = static_cast<int32_t>(bits1);
+          if (hi) pk[1] = static_cast<int32_t>(bits1);
         }
       }
     }
@@ -521,10 +567,18 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 // (lce_b200_bconv2d_run_fused_scale); SLICE (float output): the strided store of
 // lce_b200_bconv2d_run_slice, and its read-add-write in lce_b200_bconv2d_run_slice_add. The other
 // instances compile as without them.
+// GW (b1 only): a grouped plan whose groups hold 32 * odd output channels, so a 64-channel tile on
+// 64-aligned channels may span two groups. Tile nt covers channels nt * 64 .. nt * 64 + 63 and
+// gathers, per tap, the contiguous input words of two neighbouring groups (its window, from group
+// gb = min(first channel's group, groups - 2)): p.Kv and p.CwV count the window's vectors, p.Cw_pg
+// one group's words. The fragments are block-diagonal (pack_weights_b1_kernel) and pa counts each
+// window group's bits apart (compute_chunk_b1), so every channel gets popc(a ^ w) over its own
+// group alone: the XOR + POPC kernel's integers.
 template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
-          bool SPATIAL = false>
-__global__ void __launch_bounds__(kIThreads, B1 ? kB1Ctas : imma_ctas_per_sm(V))
+          bool SPATIAL = false, bool GW = false>
+__global__ void __launch_bounds__(kIThreads, B1 ? b1_ctas_per_sm(GW, OUT) : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
+  static_assert(!GW || (B1 && !SLICE), "group windows: b1, no slice store");
   using Vec = typename VecT<V>::T;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   // two buffers of { A: [Kc_v][128] packed vectors, B: [Kc_v*V][8][32] int8 fragments }, or for
@@ -535,10 +589,12 @@ bconv_imma_kernel(const ConvKParams p) {
   const int warp = tid >> 5, lane = tid & 31;
   const int gid = lane >> 2, tig = lane & 3;
   const int nt = blockIdx.y;
-  const int g = static_cast<int>(fdiv(static_cast<uint32_t>(nt), p.fd_tpg));
-  const int tg = nt - g * p.tiles_per_group;
+  // GW: g = the window's first group
+  const int g = GW ? min(nt * kBN / p.cout_pg, p.cout / p.cout_pg - 2)
+                   : static_cast<int>(fdiv(static_cast<uint32_t>(nt), p.fd_tpg));
+  const int tg = GW ? 0 : nt - g * p.tiles_per_group;
   const long long m0 = static_cast<long long>(blockIdx.x) * kIBM;
-  const int c_tile = g * p.cout_pg + tg * kBN;
+  const int c_tile = GW ? nt * kBN : g * p.cout_pg + tg * kBN;
   // B1: K runs to the padded vector count, in 8-word slices (the last may be a 4-word one)
   const int Kv_end = B1 ? b1_padded_vectors(p.Kv, V) : p.Kv;
   const int n_slices = (Kv_end * V + 7) >> 3;
@@ -569,7 +625,8 @@ bconv_imma_kernel(const ConvKParams p) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const long long m = m0 + warp * 32 + i * 8 + gid;
-      if (m < p.M) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + m * p.cout + c_tile + tig * 16));
+      if (m < p.M && (!GW || c_tile + tig * 16 < p.cout))
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + m * p.cout + c_tile + tig * 16));
     }
   }
 
@@ -609,8 +666,8 @@ bconv_imma_kernel(const ConvKParams p) {
     const int kv0 = ch * p.Kc_v;
     const int nkv = min(kv0 + p.Kc_v, Kv_end) - kv0;
     if constexpr (B1)
-      compute_chunk_b1(reinterpret_cast<const uint32_t*>(base), B_b, nkv * V, warp, gid, tig,
-                       lane, acc, pa);
+      compute_chunk_b1<GW>(reinterpret_cast<const uint32_t*>(base), B_b, nkv * V, warp, gid, tig,
+                           lane, acc, pa, kv0 * V, p.Cw_pg, p.win_step);
     else
       compute_chunk_imma<V>(reinterpret_cast<const Vec*>(base), B_b, nkv, warp, gid, tig, lane,
                             acc);
@@ -619,14 +676,19 @@ bconv_imma_kernel(const ConvKParams p) {
   constexpr int S = B1 ? 0 : 3;
   if constexpr (B1) {
     // popc(a ^ w) = popc(w) + popc(a) - 2 * popc(a & w); out-of-bounds taps (a = 0) give popc(w)
+    // GW: wg0 / wg1 = the window group of the tile's channels 0-31 / 32-63
+    const bool wg0 = GW && c_tile / p.cout_pg != g, wg1 = GW && (c_tile + 32) / p.cout_pg != g;
 #pragma unroll
     for (int ns = 0; ns < 8; ++ns) {
       const int2 pw = *reinterpret_cast<const int2*>(p.wpop + c_tile + ns * 8 + tig * 2);
 #pragma unroll
       for (int ms = 0; ms < 2; ++ms)
 #pragma unroll
-        for (int e = 0; e < 4; ++e)
-          acc[ms][ns][e] = (e & 1 ? pw.y : pw.x) + pa[ms][e] - 2 * acc[ms][ns][e];
+        for (int e = 0; e < 4; ++e) {
+          // GW: the popcount of the channel's own window group (pa[ms][e] holds group e & 1's)
+          const int a = !GW ? pa[ms][e] : (ns < 4 ? wg0 : wg1) ? pa[ms][e | 1] : pa[ms][e & 2];
+          acc[ms][ns][e] = (e & 1 ? pw.y : pw.x) + a - 2 * acc[ms][ns][e];
+        }
     }
   }
   if (p.tap_popc != nullptr) zero_pad_correction_imma<S>(p, acc, m0, c_tile, warp, gid, tig);
@@ -642,10 +704,12 @@ bconv_imma_kernel(const ConvKParams p) {
                        : k == 3 ? p.chain.sign_shift
                        : k == 4 ? p.mul
                                 : p.bias;
-      cs[i] = v != nullptr ? __ldg(v + c_tile + (i & (kBN - 1))) : 0.0f;
+      cs[i] = v != nullptr && (!GW || c_tile + (i & (kBN - 1)) < p.cout)
+                  ? __ldg(v + c_tile + (i & (kBN - 1)))
+                  : 0.0f;
     }
     __syncthreads();
-    epilogue_imma<OUT, S, true>(p, acc, m0, c_tile, warp, gid, tig, cs);
+    epilogue_imma<OUT, S, true, false, false, false, GW>(p, acc, m0, c_tile, warp, gid, tig, cs);
   } else if constexpr (GATE) {
     // likewise the gated tail's per-channel vectors (slot 0 unused); the gate itself is per image
     // and is read per row
@@ -658,12 +722,14 @@ bconv_imma_kernel(const ConvKParams p) {
                        : k == 4 ? p.mul
                        : k == 5 ? p.bias
                                 : nullptr;
-      cs[i] = v != nullptr ? __ldg(v + c_tile + (i & (kBN - 1))) : 0.0f;
+      cs[i] = v != nullptr && (!GW || c_tile + (i & (kBN - 1)) < p.cout)
+                  ? __ldg(v + c_tile + (i & (kBN - 1)))
+                  : 0.0f;
     }
     __syncthreads();
-    epilogue_imma<OUT, S, false, true, false, SPATIAL>(p, acc, m0, c_tile, warp, gid, tig, cs);
+    epilogue_imma<OUT, S, false, true, false, SPATIAL, GW>(p, acc, m0, c_tile, warp, gid, tig, cs);
   } else {
-    epilogue_imma<OUT, S, false, false, SLICE>(p, acc, m0, c_tile, warp, gid, tig);
+    epilogue_imma<OUT, S, false, false, SLICE, false, GW>(p, acc, m0, c_tile, warp, gid, tig);
   }
 }
 

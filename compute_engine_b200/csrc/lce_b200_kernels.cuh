@@ -101,6 +101,9 @@ struct ConvKParams {
   // SLICE instances only: output pixel m's cout floats start at out + m * out_stride, and so do
   // the residual's (lce_b200_bconv2d_run_slice, lce_b200_bconv2d_run_slice_add)
   long long out_stride;
+  // mma.sync kernel, group-window (GW) instances only: 8 % (2 * Cw_pg), a k-slice's step through
+  // the window
+  int win_step;
 };
 
 // --------------------------- PTX helpers ---------------------------------- //

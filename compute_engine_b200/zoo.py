@@ -152,19 +152,39 @@ class _Builder:
         return y
 
     def bconv(self, xq, xs, cout, k=3, stride=1, pad_values=1, activation="RELU", dilation=1,
-              padding="SAME", bitpacked=False, fold_bn=True):
+              padding="SAME", bitpacked=False, fold_bn=True, groups=1):
         """LceBconv2d with float output; BN (and for Bi-RealNet the kernel scale)
         folded into post_activation_multiplier / bias like the converter does
         (LCE/mlir/transforms/optimize_patterns_common.td:39-113). bitpacked: int32 output, the
         signs the next binary layer reads, with synthetic int32 thresholds [cout] around half the
         accumulators' range K = k * k * cin (inputs 2 and 3 absent) in place of the BN.
-        fold_bn=False: nothing is folded, post_activation_multiplier 1 and bias 0."""
+        fold_bn=False: nothing is folded, post_activation_multiplier 1 and bias 0.
+        groups > 1: a grouped layer, filter [cout, k, k, cin / groups / 32 words] (cin / groups a
+        multiple of 32), channels_in still cin. Each group's signs and then its BN (or thresholds)
+        are drawn in turn, as `groups` ungrouped layers of cin / groups -> cout / groups would
+        draw them, and concatenated along the output channels."""
         b, h, w, cin = xs
-        signs = self.rng.integers(0, 2, (cout, k, k, cin), dtype=np.int8) * 2 - 1
-        bits = np.zeros((cout, k, k, ((cin + 31) // 32) * 32), np.uint32)
-        bits[..., :cin] = signs < 0
-        filt = (bits.reshape(cout, k, k, -1, 32) << np.arange(32, dtype=np.uint32)).sum(
-            -1, dtype=np.uint64).astype(np.uint32).view(np.int32)
+        if cin % groups or cout % groups or (groups > 1 and (cin // groups) % 32):
+            raise ValueError(f"groups={groups} needs cin / groups a multiple of 32 and cout divisible")
+        cin_g, cout_g = cin // groups, cout // groups
+        kk = k * k * cin_g
+        filts, thrs, muls, shifts = [], [], [], []
+        for _ in range(groups):
+            signs = self.rng.integers(0, 2, (cout_g, k, k, cin_g), dtype=np.int8) * 2 - 1
+            bits = np.zeros((cout_g, k, k, ((cin_g + 31) // 32) * 32), np.uint32)
+            bits[..., :cin_g] = signs < 0
+            filts.append((bits.reshape(cout_g, k, k, -1, 32) << np.arange(32, dtype=np.uint32)).sum(
+                -1, dtype=np.uint64).astype(np.uint32).view(np.int32))
+            if bitpacked:
+                thrs.append(np.rint(kk / 2 + self.rng.standard_normal(cout_g) * np.sqrt(kk) * 0.75).astype(np.int32))
+            elif fold_bn:
+                s, t = self.bn(cout_g)
+                muls.append((s / np.float32(kk) * np.float32(4.0)).astype(np.float32))
+                shifts.append(t)
+            else:
+                muls.append(np.ones(cout_g, np.float32))
+                shifts.append(np.zeros(cout_g, np.float32))
+        filt = np.concatenate(filts)
         if padding == "SAME":
             oh, ow = -(-h // stride), -(-w // stride)
         else:
@@ -173,17 +193,12 @@ class _Builder:
         opts = bconv2d_options(cin, (stride, stride), (dilation, dilation), {"SAME": 0, "VALID": 1}[padding],
                                pad_values, act_code)
         if bitpacked:
-            kk = k * k * cin
-            thr = np.rint(kk / 2 + self.rng.standard_normal(cout) * np.sqrt(kk) * 0.75).astype(np.int32)
+            thr = np.concatenate(thrs)
             y = self.act((b, oh, ow, (cout + 31) // 32), np.int32)
             self.m.add_op("LceBconv2d", [xq, self.const(filt, np.int32, "bfilter"), -1, -1,
                                          self.const(thr, np.int32, "thr")], [y], custom_options=opts)
             return y, (b, oh, ow, cout)
-        if fold_bn:
-            s, t = self.bn(cout)
-            mul = (s / np.float32(k * k * cin) * np.float32(4.0)).astype(np.float32)
-        else:
-            mul, t = np.ones(cout, np.float32), np.zeros(cout, np.float32)
+        mul, t = np.concatenate(muls), np.concatenate(shifts)
         y = self.act((b, oh, ow, cout))
         self.m.add_op("LceBconv2d",
                       [xq, self.const(filt, np.int32, "bfilter"), self.const(mul, name="pmul"),
@@ -279,7 +294,15 @@ def reactnet_a(batch=1, seed=0, image=224, input_type="float32"):
       -> ADD(out1) (width doubling: two such 1x1 convolutions on the same signs, each + out1,
       then CONCATENATION on channels) -> RPReLU.
     Head MEAN -> FULLY_CONNECTED 1000 -> SOFTMAX. 31 LceBconv2d, 26 PRELU."""
-    g = _Builder(seed, batch, "ReActNetA")
+    def conv3x3(g, q, xs, c, stride):
+        return g.bconv(q, xs, c, stride=stride, pad_values=1, activation="NONE")
+    return _reactnet_backbone(batch, seed, image, input_type, "ReActNetA", conv3x3)
+
+
+def _reactnet_backbone(batch, seed, image, input_type, name, conv3x3):
+    """ReActNet-A's graph (see reactnet_a) with each block's 3x3 binary convolution written by
+    conv3x3(g, signs, xs, C, stride) -> (y, ys)."""
+    g = _Builder(seed, batch, name)
     xs = (batch, image, image, 3)
     x = g.image_input(xs, input_type)
     x, xs = g.conv(x, xs, 32, 3, 2)
@@ -301,7 +324,7 @@ def reactnet_a(batch=1, seed=0, image=224, input_type="float32"):
         stride = 2 if cout != cin and cin != 32 else 1
         # the shortcut first: the convolution's epilogue can then add it (Graph::FuseResidualBlocks)
         sc = x if stride == 1 else g.pool("AVERAGE_POOL_2D", x, xs, 2, 2, "VALID")[0]
-        y, ys = g.bconv(rsign(x, xs), xs, cin, stride=stride, pad_values=1, activation="NONE")
+        y, ys = conv3x3(g, rsign(x, xs), xs, cin, stride)
         out1 = rprelu(g.add(y, sc, ys), ys)
         q = rsign(out1, ys)
         halves = []
@@ -318,6 +341,43 @@ def reactnet_a(batch=1, seed=0, image=224, input_type="float32"):
     probs = g.head(x, xs, relu=False)
     g.m.outputs = [probs]
     return g.m.serialize()
+
+
+def binary_mobilenet(batch=1, seed=0, image=224, input_type="float32", group_channels=32,
+                     group_conv="native"):
+    """A binary MobileNet in the manner of Phan et al. ("Binarizing MobileNet via Evolution-based
+    Searching", CVPR 2020): grouped binary convolutions in place of the depthwise ones. The paper's
+    searched per-layer group counts are not available offline, so the topology is restated with a
+    fixed group width on ReActNet-A's MobileNet-V1 backbone and converter op order (reactnet_a):
+    each block's 3x3 LceBconv2d C -> C runs in C / group_channels groups (the first block's
+    32-channel layer, with group_channels = 32, stays one group); the 1x1 halves, shortcuts, RSign
+    and RPReLU are ReActNet-A's.
+    group_conv="native": each grouped layer is one grouped LceBconv2d (filter [C, 3, 3,
+    group_channels / 32 words], channels_in C). group_conv="split": SPLIT of the packed signs on
+    axis 3 into the groups' words, one ungrouped LceBconv2d per group, CONCATENATION on channels:
+    the same weights, drawn in the same order, and bit for bit the same result."""
+    if group_conv not in ("split", "native"):
+        raise ValueError(f"group_conv must be 'split' or 'native', not {group_conv!r}")
+    if group_channels < 32 or group_channels % 32:
+        raise ValueError(f"group_channels must be a positive multiple of 32, not {group_channels}")
+
+    def conv3x3(g, q, xs, c, stride):
+        groups = max(c // group_channels, 1)
+        if group_conv == "native" or groups == 1:
+            return g.bconv(q, xs, c, stride=stride, pad_values=1, activation="NONE", groups=groups)
+        b, h, w, _ = xs
+        cg = c // groups
+        axis = g.const(np.array(3, np.int32), np.int32, "axis")
+        parts = [g.act((b, h, w, cg // 32), np.int32) for _ in range(groups)]
+        g.m.add_op("SPLIT", [axis, q], parts, num_splits=groups)
+        ys = [g.bconv(p, (b, h, w, cg), cg, stride=stride, pad_values=1, activation="NONE") for p in parts]
+        out_s = ys[0][1][:3] + (c,)
+        z = g.act(out_s)
+        g.m.add_op("CONCATENATION", [y for y, _ in ys], [z], axis=3)
+        return z, out_s
+
+    name = "BinaryMobileNet" if group_conv == "native" else "BinaryMobileNetSplit"
+    return _reactnet_backbone(batch, seed, image, input_type, name, conv3x3)
 
 
 def realtobinarynet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):

@@ -109,7 +109,9 @@ int lce_b200_bconv2d_run_f32(lce_b200_bconv2d* plan, const float* in_dev,
  *   LceBconv2d(float out) -> ADD(shortcut) [-> LceQuantize of the sum]):
  *   out = act_add(OutputTransform(acc) + residual);  packed_out = bitpack(out) (optional).
  * Bit-identical to running the three ops one after the other. Float output plans only;
- * packed_out additionally needs groups == 1. residual / packed_out may be NULL. */
+ * packed_out additionally needs groups == 1, or channels_out / groups a multiple of 32 on the b1
+ * mma.sync kernel (LCE_B200_BCONV_IMMA and _B1 not 0 when the plan was created); the same holds
+ * for run_fused_chain. residual / packed_out may be NULL. */
 int lce_b200_bconv2d_run_fused(lce_b200_bconv2d* plan, const int32_t* in_dev,
                                const float* residual_dev, int add_activation,
                                float* out_dev, int32_t* packed_out_dev, void* stream);
