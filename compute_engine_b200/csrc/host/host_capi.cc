@@ -165,6 +165,9 @@ int lce_host_node_num_inputs(void* g, int node) {
 int lce_host_node_input(void* g, int node, int k) {
   return static_cast<Graph*>(g)->node(node).node.inputs->data[k];
 }
+int lce_host_node_num_outputs(void* g, int node) {
+  return static_cast<Graph*>(g)->node(node).node.outputs->size;
+}
 int lce_host_node_output(void* g, int node, int k) {
   return static_cast<Graph*>(g)->node(node).node.outputs->data[k];
 }
@@ -184,6 +187,9 @@ int lce_host_tensor_dim(void* g, int i, int d) {
 }
 size_t lce_host_tensor_bytes(void* g, int i) { return static_cast<Graph*>(g)->tensor(i)->bytes; }
 void* lce_host_tensor_data(void* g, int i) { return static_cast<Graph*>(g)->tensor(i)->data.raw; }
+int lce_host_tensor_in_arena(void* g, int i) {
+  return static_cast<Graph*>(g)->tensor(i)->allocation_type == kTfLiteArenaRw;
+}
 const char* lce_host_tensor_name(void* g, int i) { return static_cast<Graph*>(g)->tensor(i)->name; }
 float lce_host_tensor_scale(void* g, int i) { return static_cast<Graph*>(g)->tensor(i)->params.scale; }
 int lce_host_tensor_zero_point(void* g, int i) {

@@ -269,6 +269,11 @@ class HostGraph:
         return ([lib().lce_host_node_input(self._g, i, k) for k in range(n)],
                 [lib().lce_host_node_output(self._g, i, 0)])
 
+    def node_outputs(self, i):
+        """Every output of node i (node_io lists output 0 only)."""
+        return [lib().lce_host_node_output(self._g, i, k)
+                for k in range(lib().lce_host_node_num_outputs(self._g, i))]
+
     def synchronize(self):
         self._check(lib().lce_host_synchronize(self._g), "Synchronize")
 
@@ -319,6 +324,13 @@ class HostGraph:
 
     def data_ptr(self, t):
         return lib().lce_host_tensor_data(self._g, t)
+
+    def in_arena(self, t):
+        """Whether tensor t lives in the tensor arena (a constant does not)."""
+        return bool(lib().lce_host_tensor_in_arena(self._g, t))
+
+    def num_tensors(self):
+        return lib().lce_host_num_tensors(self._g)
 
     def arena_bytes(self):
         return int(lib().lce_host_arena_bytes(self._g))

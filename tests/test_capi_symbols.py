@@ -78,6 +78,16 @@ def test_no_cpu_fallback_without_device(lib):
                      np.ones(8, np.float32))
 
 
+def test_host_library_exports_the_graph_accessors():
+    """The graph host's read-only accessors the arena tests use (tests/test_arena_independence.py):
+    a node's outputs beyond the first, and whether a tensor lives in the arena."""
+    from compute_engine_b200 import host
+    L = host.lib()
+    for n in ("lce_host_node_num_outputs", "lce_host_node_output", "lce_host_tensor_in_arena",
+              "lce_host_tensor_data", "lce_host_arena_bytes", "lce_host_num_tensors"):
+        assert hasattr(L, n), f"{n} not exported by liblce_b200_host.so"
+
+
 def test_builtin_kernels_header_symbols_are_exported(lib):
     names = declared_symbols("lce_b200_builtins.h")
     assert len(names) == 17
