@@ -619,12 +619,21 @@ int pw_tf32_conv(const float* in, const float* filter, const float* bias, float*
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return fail("cuTensorMapEncodeTiled (pointwise filter) failed");
   }
-  p.out = out;
+  CUtensorMap tm_o;
+  {
+    // the output, stored by TMA from 64-row x 32-column SWIZZLE_128B staging boxes
+    cuuint64_t gd[2] = {static_cast<cuuint64_t>(p.N), static_cast<cuuint64_t>(p.M)};
+    cuuint64_t gs[1] = {static_cast<cuuint64_t>(p.N) * 4};
+    cuuint32_t box_o[2] = {32, 64};
+    if (enc(&tm_o, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, out, gd, gs, box_o, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+      return fail("cuTensorMapEncodeTiled (pointwise output) failed");
+  }
   static PerDeviceOnce once;
   if (once.need())
     CUDA_OK(cudaFuncSetAttribute(P::pw_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(P::kPwSmem)));
   const int grid = static_cast<int>(std::min<long long>(m_tiles * p.n_tiles, num_sms()));
-  P::pw_tf32_kernel<<<grid, P::kPwThreads, P::kPwSmem, static_cast<cudaStream_t>(stream)>>>(tm_a, tm_w, p);
+  P::pw_tf32_kernel<<<grid, P::kPwThreads, P::kPwSmem, static_cast<cudaStream_t>(stream)>>>(tm_a, tm_w, tm_o, p);
   g_pw_launches.fetch_add(1, std::memory_order_relaxed);
   return launch_check("pw_tf32_kernel");
 }

@@ -833,6 +833,13 @@ __global__ void __launch_bounds__(256) pool_v4_kernel(const float4* __restrict__
 // one output pixel x 4 channels; the 4x4 input window is loaded once (16 x LDG.128), the nine
 // pooled values are formed in registers and multiplied in the same (fy, fx) order as
 // depthwise_v4_kernel, so the result is bit-identical to the two-kernel sequence.
+// On an H100 80GB HBM3 at a 700 W power limit, QuickNet batch 256 (per-node CUDA events, 200
+// steps): 111.8 / 60.8 / 34.3 us for 56x56x64 / 28x28x128 / 14x14x256, 2.30 / 2.11 / 1.87 TB/s
+// of operands read once and results written once. A tiled kernel that stages each tile's input
+// window (4 output rows x 8 columns x 32 channels) in shared memory by cp.async, forms every
+// pooled value once and blurs from there measured slower on the same card: 143.6 / 82.7 / 43.0 us
+// one tile per CTA, 180.5 / 98.8 / 49.4 us persistent with a two-deep window buffer. So the
+// one-thread-per-output kernel stays, and the reuse stays with L1.
 #ifndef LCE_POOL_MINBLOCKS
 #define LCE_POOL_MINBLOCKS 4
 #endif
