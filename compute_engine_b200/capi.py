@@ -106,6 +106,7 @@ EXPORTS = [
     "lce_b200_bconv2d_bases_create", "lce_b200_bconv2d_bases_set_input_shape",
     "lce_b200_bconv2d_bases_get_desc", "lce_b200_bconv2d_bases_run", "lce_b200_bconv2d_bases_destroy",
     "lce_b200_f32_shift_sign_planes",
+    "lce_b200_f32_resize_nearest", "lce_b200_f32_resize_bilinear", "lce_b200_f32_upsample_add_sign",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -335,6 +336,36 @@ def shift_sign_planes(x: torch.Tensor, shifts):
     _check(lib().lce_b200_f32_shift_sign_planes(_p(x), C.c_int64(x.numel() // c if c else 0), C.c_int(c),
                                                 C.c_int(n), sh, ptrs, _stream()))
     return planes
+
+
+def resize(x: torch.Tensor, size, bilinear=False, align_corners=False, half_pixel_centers=False):
+    """RESIZE_NEAREST_NEIGHBOR (or with bilinear RESIZE_BILINEAR) of a float NHWC map to
+    size = (new_height, new_width), bit for bit TFLite's reference kernel."""
+    x = _dev(x, torch.float32)
+    b, h, w, c = x.shape
+    oh, ow = int(size[0]), int(size[1])
+    out = torch.empty((b, oh, ow, c), dtype=torch.float32, device=x.device)
+    fn = lib().lce_b200_f32_resize_bilinear if bilinear else lib().lce_b200_f32_resize_nearest
+    _check(fn(_p(x), b, h, w, c, oh, ow, int(bool(align_corners)), int(bool(half_pixel_centers)), _p(out),
+              _stream()))
+    return out
+
+
+def upsample_add_sign(u: torch.Tensor, skip: torch.Tensor, align_corners=False, half_pixel_centers=False,
+                      activation=ACT_NONE, out=True, packed=True):
+    """RESIZE_NEAREST_NEIGHBOR(u) to skip's size -> ADD(skip) with its activation [-> LceQuantize] in
+    one pass. Returns (sum | None, packed signs | None)."""
+    u, skip = _dev(u, torch.float32), _dev(skip, torch.float32)
+    b, h, w, c = u.shape
+    oh, ow = skip.shape[1], skip.shape[2]
+    if skip.shape[0] != b or skip.shape[3] != c:
+        raise LceError("upsample_add_sign: skip must be [B, new_height, new_width, C]")
+    o = torch.empty_like(skip) if out else None
+    pk = torch.empty((b, oh, ow, cdiv(c, 32)), dtype=torch.int32, device=u.device) if packed else None
+    _check(lib().lce_b200_f32_upsample_add_sign(_p(u), b, h, w, c, oh, ow, int(bool(align_corners)),
+                                                int(bool(half_pixel_centers)), _p(skip), C.c_int(activation),
+                                                _p(o), _p(pk), _stream()))
+    return o, pk
 
 
 class BConv2dBases:

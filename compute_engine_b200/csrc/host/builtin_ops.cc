@@ -816,6 +816,104 @@ TfLiteStatus PadInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// -------------------- RESIZE_BILINEAR / RESIZE_NEAREST_NEIGHBOR -------------------- //
+// inputs [x (float32 [B,H,W,C]), size (constant int32 [2] = new_height, new_width, read on the host
+// as PAD reads its paddings)]; output [B, new_height, new_width, C], so the batch follows x's
+// (TF/lite/kernels/resize_bilinear.cc, resize_nearest_neighbor.cc).
+const int32_t* HostInts(const TfLiteTensor* t);
+const char* ResizeGeometry(TfLiteContext* c, TfLiteNode* n, bool bilinear, const BuiltinParams& p,
+                           int32_t* out_h, int32_t* out_w) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const TfLiteTensor* size = T(c, n->inputs, 1);
+  if (!x || x->type != kTfLiteFloat32 || x->dims->size != 4)
+    return bilinear ? "RESIZE_BILINEAR: the input must be a 4-D float32 tensor"
+                    : "RESIZE_NEAREST_NEIGHBOR: the input must be a 4-D float32 tensor";
+  if (!size || size->allocation_type != kTfLiteMmapRo || !HostInts(size) || Count(size) != 2)
+    return bilinear ? "RESIZE_BILINEAR: the size must be a constant int32 tensor of 2 values"
+                    : "RESIZE_NEAREST_NEIGHBOR: the size must be a constant int32 tensor of 2 values";
+  if (size->data.i32[0] <= 0 || size->data.i32[1] <= 0)
+    return bilinear ? "RESIZE_BILINEAR: the size must be positive"
+                    : "RESIZE_NEAREST_NEIGHBOR: the size must be positive";
+  if (bilinear && p.align_corners && p.half_pixel_centers)
+    return "RESIZE_BILINEAR: align_corners and half_pixel_centers cannot both be set";
+  *out_h = size->data.i32[0];
+  *out_w = size->data.i32[1];
+  return nullptr;
+}
+template <bool BILINEAR>
+TfLiteStatus ResizePrepare(TfLiteContext* c, TfLiteNode* n) {
+  int32_t oh, ow;
+  const char* why = ResizeGeometry(c, n, BILINEAR, P(n), &oh, &ow);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteIntArray* d = T(c, n->inputs, 0)->dims;
+  return Resize(c, T(c, n->outputs, 0), {d->data[0], oh, ow, d->data[3]});
+}
+template <bool BILINEAR>
+TfLiteStatus ResizeInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const TfLiteTensor* o = T(c, n->outputs, 0);
+  const BuiltinParams& p = P(n);
+  const int* d = x->dims->data;
+  if (BILINEAR)
+    B_CAPI(c, lce_b200_f32_resize_bilinear(x->data.f, d[0], d[1], d[2], d[3], o->dims->data[1], o->dims->data[2],
+                                           p.align_corners, p.half_pixel_centers, o->data.f,
+                                           lce_b200_get_stream()));
+  else
+    B_CAPI(c, lce_b200_f32_resize_nearest(x->data.f, d[0], d[1], d[2], d[3], o->dims->data[1], o->dims->data[2],
+                                          p.align_corners, p.half_pixel_centers, o->data.f,
+                                          lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// ------------- fused RESIZE_NEAREST_NEIGHBOR -> ADD [-> LceQuantize]: a decoder merge ------------- //
+// Created by Graph::FuseUpsampleMerges; builtin_data = { BuiltinParams resize, BuiltinParams add };
+// inputs [u, size, skip], outputs [sum (-1 when only the signs are read), packed signs?].
+struct MergeParams {
+  BuiltinParams resize, add;
+};
+void* MergeInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* p = new MergeParams();
+  memset(p, 0, sizeof(*p));
+  if (buffer && length >= sizeof(MergeParams)) memcpy(p, buffer, sizeof(MergeParams));
+  return p;
+}
+void MergeFree(TfLiteContext*, void* p) { delete static_cast<MergeParams*>(p); }
+TfLiteStatus MergePrepare(TfLiteContext* c, TfLiteNode* n) {
+  const auto& mp = *static_cast<const MergeParams*>(n->user_data);
+  B_ENSURE(c, n->inputs->size == 3 && n->outputs->size >= 1 && n->outputs->size <= 2,
+           "RESIZE_NEAREST_NEIGHBOR+ADD: inputs [u, size, skip] and one or two outputs expected");
+  int32_t oh, ow;
+  const char* why = ResizeGeometry(c, n, false, mp.resize, &oh, &ow);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteIntArray* u = T(c, n->inputs, 0)->dims;
+  const TfLiteTensor* skip = T(c, n->inputs, 2);
+  B_ENSURE(c, skip && skip->type == kTfLiteFloat32 && skip->dims->size == 4 && skip->dims->data[0] == u->data[0] &&
+                  skip->dims->data[1] == oh && skip->dims->data[2] == ow && skip->dims->data[3] == u->data[3],
+           "RESIZE_NEAREST_NEIGHBOR+ADD: the skip map must have the resized map's shape");
+  TfLiteTensor* o = T(c, n->outputs, 0);
+  if (o && Resize(c, o, {u->data[0], oh, ow, u->data[3]}) != kTfLiteOk) return kTfLiteError;
+  if (n->outputs->size == 2) {
+    TfLiteTensor* pk = T(c, n->outputs, 1);
+    B_ENSURE(c, pk && pk->type == kTfLiteInt32, "RESIZE_NEAREST_NEIGHBOR+ADD+LceQuantize: packed output must be int32");
+    if (Resize(c, pk, {u->data[0], oh, ow, (u->data[3] + 31) / 32}) != kTfLiteOk) return kTfLiteError;
+  }
+  return kTfLiteOk;
+}
+TfLiteStatus MergeInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const auto& mp = *static_cast<const MergeParams*>(n->user_data);
+  const TfLiteTensor* u = T(c, n->inputs, 0);
+  const TfLiteTensor* skip = T(c, n->inputs, 2);
+  TfLiteTensor* o = T(c, n->outputs, 0);
+  TfLiteTensor* pk = n->outputs->size > 1 ? T(c, n->outputs, 1) : nullptr;
+  const int* d = u->dims->data;
+  B_CAPI(c, lce_b200_f32_upsample_add_sign(u->data.f, d[0], d[1], d[2], d[3], skip->dims->data[1],
+                                           skip->dims->data[2], mp.resize.align_corners,
+                                           mp.resize.half_pixel_centers, skip->data.f, mp.add.activation,
+                                           o ? o->data.f : nullptr, pk ? pk->data.i32 : nullptr,
+                                           lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // ------------------------------ CONCATENATION ------------------------------ //
 // Strided device copies (one cudaMemcpy2DAsync per input): no kernel of ours.
 TfLiteStatus ConcatPrepare(TfLiteContext* c, TfLiteNode* n) {
@@ -1019,6 +1117,10 @@ const TfLiteRegistration* GroupedConvAffineRegistration() {
   static TfLiteRegistration r = {ConvAffineInit, ConvAffineFree, ConvAffinePrepare, ConvAffineInvoke};
   return &r;
 }
+const TfLiteRegistration* UpsampleMergeRegistration() {
+  static TfLiteRegistration r = {MergeInit, MergeFree, MergePrepare, MergeInvoke};
+  return &r;
+}
 
 void RegisterBuiltinOps(OpResolver* r) {
   static TfLiteRegistration conv = {Init, Free, ConvPrepare<false>, ConvInvoke<false>};
@@ -1067,6 +1169,10 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(45, &strided_slice);  // STRIDED_SLICE
   static TfLiteRegistration split = {Init, Free, SplitPrepare, SplitInvoke};
   r->AddBuiltin(49, &split);  // SPLIT
+  static TfLiteRegistration resize_bilinear = {Init, Free, ResizePrepare<true>, ResizeInvoke<true>};
+  static TfLiteRegistration resize_nearest = {Init, Free, ResizePrepare<false>, ResizeInvoke<false>};
+  r->AddBuiltin(23, &resize_bilinear);  // RESIZE_BILINEAR
+  r->AddBuiltin(97, &resize_nearest);   // RESIZE_NEAREST_NEIGHBOR
 }
 
 }  // namespace lce_b200

@@ -20,6 +20,8 @@ struct BuiltinParams {
   // STRIDED_SLICE (StridedSliceOptions) and SPLIT (SplitOptions)
   int32_t begin_mask, end_mask, ellipsis_mask, new_axis_mask, shrink_axis_mask, offset;
   int32_t num_splits;
+  // RESIZE_BILINEAR (ResizeBilinearOptions) and RESIZE_NEAREST_NEIGHBOR (ResizeNearestNeighborOptions)
+  int32_t align_corners, half_pixel_centers;
 };
 
 // STRIDED_SLICE's bounds for an input of dims[0..rank) and n = the length of begin / end / strides,

@@ -311,6 +311,7 @@ constexpr const char* kDepthwiseConv2d = "builtin:4";
 constexpr const char* kDequantize = "builtin:6";
 constexpr const char* kFullyConnected = "builtin:9";
 constexpr const char* kMaxPool2d = "builtin:17";
+constexpr const char* kResizeNearest = "builtin:97";
 constexpr const char* kMul = "builtin:18";
 constexpr const char* kRelu = "builtin:19";
 constexpr const char* kMean = "builtin:40";
@@ -1683,6 +1684,63 @@ int Graph::FuseFloatGlue() {
     pool.name = "MAX_POOL_2D+DEPTHWISE_CONV_2D";
     EraseNode(di);
     ++removed;
+  }
+  allocated_ = false;
+  return removed;
+}
+
+const TfLiteRegistration* UpsampleMergeRegistration();   // builtin_ops.cc
+
+int Graph::FuseUpsampleMerges() {
+  if (!device_arena_) return 0;
+  auto fuse = [&](size_t i) -> int {   // nodes removed by fusing the resize at i, 0 when it stays
+    NodeRecord& r = *nodes_[i];
+    if (r.name != kResizeNearest || r.initialized || r.node.inputs->size != 2 || r.node.outputs->size != 1 ||
+        !Params(r))
+      return 0;
+    const int u = r.node.inputs->data[0], size = r.node.inputs->data[1], v = r.node.outputs->data[0];
+    if (u < 0 || size < 0 || tensors_[u].type != kTfLiteFloat32 || tensors_[v].type != kTfLiteFloat32) return 0;
+    const TfLiteIntArray* vd = tensors_[v].dims;
+    if (!vd || vd->size != 4) return 0;
+    const size_t ai = SoleConsumer(v);
+    if (ai == kNoNode || ai <= i) return 0;
+    NodeRecord& a = *nodes_[ai];
+    if (a.name != kAdd || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1 || !Params(a))
+      return 0;
+    const int in0 = a.node.inputs->data[0], in1 = a.node.inputs->data[1];
+    if (in0 == in1) return 0;
+    const int skip = in0 == v ? in1 : in0;
+    if (skip < 0 || tensors_[skip].type != kTfLiteFloat32 || !SameDims(vd, tensors_[skip].dims)) return 0;
+    const int s = a.node.outputs->data[0];
+    if (tensors_[s].type != kTfLiteFloat32) return 0;
+    // the sign tail: the sum's only LceQuantize reader, on whole 32-channel words
+    const std::vector<size_t> readers = Consumers(s);
+    size_t kq = kNoNode;
+    int quantizers = 0;
+    for (size_t k : readers)
+      if (nodes_[k]->name == "LceQuantize") { ++quantizers; kq = k; }
+    const bool tail = quantizers == 1 && IsQuantize(kq) && kq > ai && vd->data[3] % 32 == 0;
+    const bool store = !tail || readers.size() > 1 || IsGraphOutput(s);
+    std::vector<int> outs{store ? s : -1};
+    if (tail) outs.push_back(nodes_[kq]->node.outputs->data[0]);
+    const BuiltinParams two[2] = {*Params(r), *Params(a)};
+    // the ADD's node becomes the merge: u and skip both exist where it runs
+    SetNodeIO(a, {u, size, skip}, outs);
+    SetBuiltinBlob(a, two, sizeof(two));
+    a.registration = UpsampleMergeRegistration();
+    a.name = tail ? "RESIZE_NEAREST_NEIGHBOR+ADD+LceQuantize" : "RESIZE_NEAREST_NEIGHBOR+ADD";
+    if (tail) {
+      EraseNodes({i, kq});
+      return 2;
+    }
+    EraseNode(i);
+    return 1;
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size();) {
+    const int k = fuse(i);
+    removed += k;
+    if (k == 0) ++i;   // else node i is erased and its successor moved up
   }
   allocated_ = false;
   return removed;

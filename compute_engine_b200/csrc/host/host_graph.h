@@ -237,6 +237,22 @@ class Graph {
   int FuseConvQuantize();  // part of FuseFloatGlue: CONV_2D -> LceQuantize => conv with 2 outputs
   int FuseStem();  // part of FuseFloatGlue: [DEQUANTIZE +] stem conv + depthwise conv -> one node
 
+  // A segmentation decoder's merge
+  //   RESIZE_NEAREST_NEIGHBOR(u) -> ADD(v, skip) [-> LceQuantize]
+  // becomes one node "RESIZE_NEAREST_NEIGHBOR+ADD[+LceQuantize]" (lce_b200_f32_upsample_add_sign),
+  // which reads u at each output pixel's nearest source pixel, so the upsampled copy of u is never
+  // written and the sum is read by nobody to make its signs: inputs [u, size, skip], outputs [sum (-1
+  // when only the absorbed LceQuantize reads it and it is not a graph output), packed signs?],
+  // builtin_data { the resize's, the ADD's BuiltinParams }; the ADD's activation is applied. v may be
+  // either operand of the ADD. Only when v has one consumer, the ADD, and is not a graph output; u,
+  // v and skip are float32 and v and skip have the same 4-D shape (no broadcast); otherwise the graph
+  // is left as it is. The LceQuantize is absorbed only when C % 32 == 0 and it is the sum's only
+  // LceQuantize reader. No other pass matches a RESIZE_NEAREST_NEIGHBOR, so the pass may run anywhere;
+  // fuse_all runs it after FuseFloatGlue and before FuseChannelGates / FuseActivationChains, the
+  // passes that look for a lone ADD -> LceQuantize sign tail, so that none of them can take the
+  // merge's sign first. Bit-identical. Returns the number of nodes removed.
+  int FuseUpsampleMerges();
+
   // init (first time) + prepare of every node in order, then arena allocation.
   TfLiteStatus AllocateTensors();
   TfLiteStatus ResizeInputTensor(int tensor, const std::vector<int>& dims);

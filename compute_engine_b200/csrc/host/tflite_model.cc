@@ -317,6 +317,14 @@ bool BuildGraphFromTflite(const uint8_t* data, size_t size, const OpResolver& re
       case 49:  // SPLIT: SplitOptions
         bp.num_splits = o.scalar<int32_t>(0, 0);
         break;
+      case 23:  // RESIZE_BILINEAR: ResizeBilinearOptions (fields 0 and 1 are the deprecated sizes)
+        bp.align_corners = o.scalar<int8_t>(2, 0);
+        bp.half_pixel_centers = o.scalar<int8_t>(3, 0);
+        break;
+      case 97:  // RESIZE_NEAREST_NEIGHBOR: ResizeNearestNeighborOptions
+        bp.align_corners = o.scalar<int8_t>(0, 0);
+        bp.half_pixel_centers = o.scalar<int8_t>(1, 0);
+        break;
       default:
         break;
     }

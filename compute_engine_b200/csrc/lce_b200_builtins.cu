@@ -1225,6 +1225,136 @@ __global__ void __launch_bounds__(256) shift_sign_planes_kernel(const float* __r
   }
 }
 
+// RESIZE_NEAREST_NEIGHBOR / RESIZE_BILINEAR (reference/resize_nearest_neighbor.h, resize_bilinear.h).
+// One axis of the resize: the host computes `scale` as the reference does, in float; every step here
+// is one explicitly rounded operation so that nvcc contracts nothing into an FMA.
+struct ResizeAxis {
+  int in, out;
+  float scale;
+};
+struct ResizeGeom {
+  ResizeAxis y, x;
+  int batch, C;
+  int align_corners, half_pixel_centers;
+};
+// GetNearestNeighbor: the source index of output index o
+__device__ __forceinline__ int nearest_src(int o, const ResizeAxis& a, int align, int half) {
+  const float v = __fmul_rn(__fadd_rn(static_cast<float>(o), half ? 0.5f : 0.0f), a.scale);
+  int s = min(align ? static_cast<int>(roundf(v)) : static_cast<int>(floorf(v)), a.in - 1);
+  if (half) s = max(s, 0);
+  return s;
+}
+// ComputeInterpolationValues: the source coordinate v and its clamped neighbours lo, hi
+__device__ __forceinline__ float bilinear_src(int o, const ResizeAxis& a, int half, int* lo, int* hi) {
+  const float of = static_cast<float>(o);
+  const float v = half ? __fsub_rn(__fmul_rn(__fadd_rn(of, 0.5f), a.scale), 0.5f) : __fmul_rn(of, a.scale);
+  *lo = max(static_cast<int>(floorf(v)), 0);
+  *hi = min(static_cast<int>(ceilf(v)), a.in - 1);
+  return v;
+}
+
+// The resize kernels walk the output by rows: blockIdx.y strides over the B * OH output rows, so each
+// row's source rows (and for the bilinear one its vertical weight) are found once per thread and row,
+// and blockIdx.x / threadIdx.x stride over the row's OW * C floats, taken VEC = 4 at a time when the
+// row is a whole number of 16-byte float4s (a float4 may span two pixels when C % 4 != 0, as at the
+// 21 classes of a segmentation head), else one at a time. Element offsets are 64-bit; a row's own
+// index is 32-bit (the host refuses rows within 2^22 floats of 2^31).
+template <int VEC>
+__global__ void __launch_bounds__(256) resize_nearest_kernel(const float* __restrict__ in,
+                                                             float* __restrict__ out, ResizeGeom g) {
+  const int row_len = g.x.out * g.C;
+  for (long long row = blockIdx.y; row < static_cast<long long>(g.y.out) * g.batch; row += gridDim.y) {
+    const long long b = row / g.y.out;
+    const int sy = nearest_src(static_cast<int>(row - b * g.y.out), g.y, g.align_corners, g.half_pixel_centers);
+    const float* src = in + (b * g.y.in + sy) * g.x.in * g.C;
+    float* dst = out + row * row_len;
+    for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * VEC; j < row_len; j += gridDim.x * blockDim.x * VEC) {
+      int ox = j / g.C, c = j - ox * g.C;
+      float v[VEC];
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) {
+        v[k] = __ldg(src + nearest_src(ox, g.x, g.align_corners, g.half_pixel_centers) * g.C + c);
+        if (++c == g.C) { c = 0; ++ox; }
+      }
+      if (VEC == 4) reinterpret_cast<float4*>(dst)[j >> 2] = make_float4(v[0], v[1], v[2], v[3]);
+      else dst[j] = v[0];
+    }
+  }
+}
+
+__device__ __forceinline__ float bilinear_mix(float x00, float x10, float x01, float x11, float dy, float dx) {
+  // x00*(1-dy)*(1-dx) + x10*dy*(1-dx) + x01*(1-dy)*dx + x11*dy*dx, left to right, every step rounded
+  const float ey = __fsub_rn(1.0f, dy), ex = __fsub_rn(1.0f, dx);
+  float s = __fmul_rn(__fmul_rn(x00, ey), ex);
+  s = __fadd_rn(s, __fmul_rn(__fmul_rn(x10, dy), ex));
+  s = __fadd_rn(s, __fmul_rn(__fmul_rn(x01, ey), dx));
+  return __fadd_rn(s, __fmul_rn(__fmul_rn(x11, dy), dx));
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(256) resize_bilinear_kernel(const float* __restrict__ in,
+                                                              float* __restrict__ out, ResizeGeom g) {
+  const int row_len = g.x.out * g.C;
+  for (long long row = blockIdx.y; row < static_cast<long long>(g.y.out) * g.batch; row += gridDim.y) {
+    const long long b = row / g.y.out;
+    int y0, y1;
+    const float vy = bilinear_src(static_cast<int>(row - b * g.y.out), g.y, g.half_pixel_centers, &y0, &y1);
+    // the weights come from the clamped lower neighbours, as in the reference
+    const float dy = __fsub_rn(vy, static_cast<float>(y0));
+    const float* src0 = in + (b * g.y.in + y0) * g.x.in * g.C;
+    const float* src1 = in + (b * g.y.in + y1) * g.x.in * g.C;
+    float* dst = out + row * row_len;
+    for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * VEC; j < row_len; j += gridDim.x * blockDim.x * VEC) {
+      int ox = j / g.C, c = j - ox * g.C;
+      float v[VEC];
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) {
+        int x0, x1;
+        const float vx = bilinear_src(ox, g.x, g.half_pixel_centers, &x0, &x1);
+        const float dx = __fsub_rn(vx, static_cast<float>(x0));
+        v[k] = bilinear_mix(__ldg(src0 + x0 * g.C + c), __ldg(src1 + x0 * g.C + c), __ldg(src0 + x1 * g.C + c),
+                            __ldg(src1 + x1 * g.C + c), dy, dx);
+        if (++c == g.C) { c = 0; ++ox; }
+      }
+      if (VEC == 4) reinterpret_cast<float4*>(dst)[j >> 2] = make_float4(v[0], v[1], v[2], v[3]);
+      else dst[j] = v[0];
+    }
+  }
+}
+
+// lce_b200_f32_upsample_add_sign: a decoder merge RESIZE_NEAREST_NEIGHBOR(u) -> ADD(skip) [->
+// LceQuantize] in one pass, by output rows as the resize kernels. One warp per output pixel and
+// 32-channel word, as shift_sign_planes_kernel: lane l reads channel 32 * word + l of u at the nearest
+// source pixel and of skip, adds them as the ADD builtin does (one rounding, then its activation),
+// stores the sum when `out` is set and ballots the signs into the packed word when `packed` is set
+// (lanes past C vote 0).
+__global__ void __launch_bounds__(256) upsample_add_sign_kernel(const float* __restrict__ u,
+                                                                const float* __restrict__ skip, ResizeGeom g,
+                                                                int cw, int act, float* __restrict__ out,
+                                                                int32_t* __restrict__ packed) {
+  const int lane = threadIdx.x & 31;
+  const int row_words = g.x.out * cw;
+  for (long long row = blockIdx.y; row < static_cast<long long>(g.y.out) * g.batch; row += gridDim.y) {
+    const long long b = row / g.y.out;
+    const int sy = nearest_src(static_cast<int>(row - b * g.y.out), g.y, g.align_corners, g.half_pixel_centers);
+    const float* src = u + (b * g.y.in + sy) * g.x.in * g.C;
+    for (int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < row_words; w += gridDim.x * (blockDim.x >> 5)) {
+      const int ox = w / cw;
+      const int c = (w - ox * cw) * 32 + lane;
+      bool bit = false;
+      if (c < g.C) {
+        const long long at = (row * g.x.out + ox) * g.C + c;
+        const int sx = nearest_src(ox, g.x, g.align_corners, g.half_pixel_centers);
+        const float s = apply_act(__fadd_rn(__ldg(src + sx * g.C + c), __ldg(skip + at)), act);
+        if (out) out[at] = s;
+        bit = lce::chain_sign(s, false, 0.0f);
+      }
+      const unsigned word = __ballot_sync(0xffffffffu, bit);
+      if (packed && lane == 0) packed[row * row_words + w] = static_cast<int32_t>(word);
+    }
+  }
+}
+
 // LOGISTIC, TFLite's float reference (reference/logistic.h) with CUDA's expf
 __global__ void __launch_bounds__(256) logistic_kernel(const float* __restrict__ in,
                                                        float* __restrict__ out, long long n) {
@@ -2486,6 +2616,89 @@ int lce_b200_f32_logistic(const float* in, float* out, int64_t n, void* stream) 
   if (n == 0) return 0;
   logistic_kernel<<<grid_for(n, 256), 256, 0, as_stream(stream)>>>(in, out, n);
   return launch_check("logistic_kernel");
+}
+
+}  // extern "C"
+
+namespace {
+// The reference's scale, in float: in / out, or (in - 1) / (out - 1) with align_corners and out > 1
+ResizeAxis resize_axis(int in, int out, int align_corners) {
+  const float scale = align_corners && out > 1 ? static_cast<float>(in - 1) / static_cast<float>(out - 1)
+                                               : static_cast<float>(in) / static_cast<float>(out);
+  return ResizeAxis{in, out, scale};
+}
+int resize_geom(const char* op, int batch, int in_h, int in_w, int channels, int out_h, int out_w,
+                int align_corners, int half_pixel_centers, ResizeGeom* g) {
+  if (batch < 0 || in_h <= 0 || in_w <= 0 || channels <= 0 || out_h <= 0 || out_w <= 0)
+    return fail("%s: bad shape (%d x %d x %d x %d to %d x %d)", op, batch, in_h, in_w, channels, out_h, out_w);
+  if (static_cast<long long>(std::max(in_w, out_w)) * ((channels + 31) / 32 * 32) >= (1LL << 31) - (1LL << 22))
+    return fail("%s: a row of %d x %d floats is too wide", op, std::max(in_w, out_w), channels);
+  g->y = resize_axis(in_h, out_h, align_corners);
+  g->x = resize_axis(in_w, out_w, align_corners);
+  g->batch = batch;
+  g->C = channels;
+  g->align_corners = align_corners ? 1 : 0;
+  g->half_pixel_centers = half_pixel_centers ? 1 : 0;
+  return 0;
+}
+// blockIdx.y over the output rows, blockIdx.x over one row's `per_row` units of work
+dim3 row_grid(long long rows, long long per_row, int per_block) {
+  return dim3(static_cast<unsigned>(std::min<long long>((per_row + per_block - 1) / per_block, 1024)),
+              static_cast<unsigned>(std::min<long long>(rows, 65535)));
+}
+template <bool BILINEAR>
+int resize_run(const char* op, const float* in, int batch, int in_h, int in_w, int channels, int out_h,
+               int out_w, int align_corners, int half_pixel_centers, float* out, void* stream) {
+  ResizeGeom g;
+  if (resize_geom(op, batch, in_h, in_w, channels, out_h, out_w, align_corners, half_pixel_centers, &g)) return 1;
+  if (BILINEAR && align_corners && half_pixel_centers)
+    return fail("%s: align_corners and half_pixel_centers cannot both be set", op);
+  if (batch == 0) return 0;
+  if (!in || !out) return fail("%s: null tensor", op);
+  const long long row_len = static_cast<long long>(out_w) * channels;
+  const bool vec = row_len % 4 == 0 && !((uintptr_t)out & 15);
+  const dim3 grid = row_grid(static_cast<long long>(batch) * out_h, vec ? row_len / 4 : row_len, 256);
+  cudaStream_t s = as_stream(stream);
+  if (BILINEAR) {
+    if (vec) resize_bilinear_kernel<4><<<grid, 256, 0, s>>>(in, out, g);
+    else resize_bilinear_kernel<1><<<grid, 256, 0, s>>>(in, out, g);
+    return launch_check("resize_bilinear_kernel");
+  }
+  if (vec) resize_nearest_kernel<4><<<grid, 256, 0, s>>>(in, out, g);
+  else resize_nearest_kernel<1><<<grid, 256, 0, s>>>(in, out, g);
+  return launch_check("resize_nearest_kernel");
+}
+}  // namespace
+
+extern "C" {
+
+int lce_b200_f32_resize_nearest(const float* in, int batch, int in_h, int in_w, int channels, int out_h, int out_w,
+                                int align_corners, int half_pixel_centers, float* out, void* stream) {
+  return resize_run<false>("resize_nearest", in, batch, in_h, in_w, channels, out_h, out_w, align_corners,
+                           half_pixel_centers, out, stream);
+}
+
+int lce_b200_f32_resize_bilinear(const float* in, int batch, int in_h, int in_w, int channels, int out_h,
+                                 int out_w, int align_corners, int half_pixel_centers, float* out, void* stream) {
+  return resize_run<true>("resize_bilinear", in, batch, in_h, in_w, channels, out_h, out_w, align_corners,
+                          half_pixel_centers, out, stream);
+}
+
+int lce_b200_f32_upsample_add_sign(const float* u, int batch, int in_h, int in_w, int channels, int out_h,
+                                   int out_w, int align_corners, int half_pixel_centers, const float* skip,
+                                   int activation, float* out, int32_t* packed, void* stream) {
+  ResizeGeom g;
+  if (resize_geom("upsample_add_sign", batch, in_h, in_w, channels, out_h, out_w, align_corners,
+                  half_pixel_centers, &g))
+    return 1;
+  if (activation < LCE_ACT_NONE || activation > LCE_ACT_RELU6)
+    return fail("upsample_add_sign: unknown activation %d", activation);
+  if (!u || !skip) return fail("upsample_add_sign: u and skip are required");
+  if (batch == 0 || (out == nullptr && packed == nullptr)) return 0;
+  const int cw = (channels + 31) / 32;
+  const dim3 grid = row_grid(static_cast<long long>(batch) * out_h, static_cast<long long>(out_w) * cw, 8);
+  upsample_add_sign_kernel<<<grid, 256, 0, as_stream(stream)>>>(u, skip, g, cw, activation, out, packed);
+  return launch_check("upsample_add_sign_kernel");
 }
 
 int lce_b200_f32_mean_hw_act(const float* in, float* out, int batch, int h, int w, int c, int pre_activation,

@@ -239,6 +239,12 @@ class HostGraph:
         Call after fuse_residual_blocks and before allocate_tensors."""
         return lib().lce_host_fuse_activation_chains(self._g)
 
+    def fuse_upsample_merges(self):
+        """RESIZE_NEAREST_NEIGHBOR(u) -> ADD(skip) [-> LceQuantize] (a segmentation decoder's merge)
+        => one node that reads u at each output pixel's nearest source pixel. Call before
+        fuse_activation_chains and allocate_tensors."""
+        return lib().lce_host_fuse_upsample_merges(self._g)
+
     def fuse_residual_pairs(self):
         """Two consecutive LceBconv2d+ADD[+LceQuantize] blocks whose intermediate nothing else
         reads => one node that keeps it on chip. Call after the other fusions."""
@@ -247,7 +253,7 @@ class HostGraph:
     def fuse_all(self):
         return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_residual_blocks()
                 + self.fuse_spatial_scales()
-                + self.fuse_float_glue()
+                + self.fuse_float_glue() + self.fuse_upsample_merges()
                 + self.fuse_grouped_conv_affine() + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
                 + self.fuse_residual_pairs())
 

@@ -226,12 +226,21 @@ def quicknet(batch=1, blocks=(4, 4, 4, 4), filters=(64, 128, 256, 512), seed=0, 
              name="QuickNet", input_type="float32"):
     """Returns the serialized .tflite bytes."""
     g = _Builder(seed, batch, name)
+    x, xs = _quicknet_encoder(g, batch, image, input_type, blocks, filters)[-1]
+    probs = g.head(x, xs)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
+def _quicknet_encoder(g, batch, image, input_type, blocks, filters):
+    """QuickNet's stem, sections and transitions; returns each section's final map (x, shape)."""
     xs = (batch, image, image, 3)
     x = g.image_input(xs, input_type)
     # stem
     x, xs = g.conv(x, xs, filters[0] // 4, 3, 2, activation="RELU")
     x, xs = g.depthwise(x, xs, 3, 2, bn=True)
     x, xs = g.conv(x, xs, filters[0], 1, 1)
+    sections = []
     for si, (nb, f) in enumerate(zip(blocks, filters)):
         if si > 0:   # transition block
             x, xs = g.pool("MAX_POOL_2D", x, xs, 2, 1, "VALID")
@@ -241,8 +250,47 @@ def quicknet(batch=1, blocks=(4, 4, 4, 4), filters=(64, 128, 256, 512), seed=0, 
             q = g.quantize(x, xs)
             y, _ = g.bconv(q, xs, f, pad_values=1, activation="RELU")
             x = g.add(y, x, xs)
-    probs = g.head(x, xs)
-    g.m.outputs = [probs]
+        sections.append((x, xs))
+    return sections
+
+
+def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, decoder_blocks=2):
+    """A binary segmentation network: QuickNet's encoder, then a decoder of three stages that merge
+    the coarse map with the encoder's skip maps as TF2's UpSampling2D and Keras' Add emit them, then a
+    per-pixel classifier at full resolution. Each stage, for (coarse, skip) = (s4, s3), (d3, s2),
+    (d2, s1): CONV_2D 1x1 to the skip's channels (BatchNorm folded, no activation) ->
+    RESIZE_NEAREST_NEIGHBOR x2 (half_pixel_centers) -> ADD(skip) -> `decoder_blocks` residual blocks
+    [LceQuantize -> LceBconv2d 3x3 (one-padding, ReLU, BatchNorm folded) -> ADD shortcut]. Head:
+    CONV_2D 1x1 64 -> classes with bias -> RESIZE_BILINEAR to (image, image) (half_pixel_centers), the
+    logits [B, image, image, classes]. image must be a multiple of 32 (the encoder halves it five
+    times and the decoder doubles it back)."""
+    if image % 32:
+        raise ValueError(f"quicknet_seg needs an image size that is a multiple of 32, not {image}")
+    g = _Builder(seed, batch, "QuickNetSeg")
+    sections = _quicknet_encoder(g, batch, image, input_type, (4, 4, 4, 4), (64, 128, 256, 512))
+    x, xs = sections[-1]
+
+    def size(h, w):
+        return g.const(np.array([h, w], np.int32), np.int32, "size")
+
+    for skip, ss in reversed(sections[:-1]):
+        x, xs = g.conv(x, xs, ss[3], 1, 1)
+        up = g.act(ss)
+        g.m.add_op("RESIZE_NEAREST_NEIGHBOR", [x, size(ss[1], ss[2])], [up], half_pixel_centers=True)
+        x, xs = g.add(up, skip, ss), ss
+        for _ in range(decoder_blocks):
+            q = g.quantize(x, xs)
+            y, _ = g.bconv(q, xs, xs[3], pad_values=1, activation="RELU")
+            x = g.add(y, x, xs)
+    b, h, w, c = xs
+    wt = g.rng.standard_normal((classes, 1, 1, c)).astype(np.float32) / np.float32(np.sqrt(c))
+    bias = g.rng.uniform(-0.5, 0.5, classes).astype(np.float32)
+    logits = g.act((b, h, w, classes))
+    g.m.add_op("CONV_2D", [x, g.const(wt), g.const(bias, name="b")], [logits], padding="SAME",
+               stride=(1, 1), activation="NONE")
+    out = g.act((b, image, image, classes))
+    g.m.add_op("RESIZE_BILINEAR", [logits, size(image, image)], [out], half_pixel_centers=True)
+    g.m.outputs = [out]
     return g.m.serialize()
 
 

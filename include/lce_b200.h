@@ -308,6 +308,33 @@ void lce_b200_bconv2d_bases_destroy(lce_b200_bconv2d_bases* plan);
  * shifts on the host, planes device pointers. Bit-identical to the 2 N ops. */
 int lce_b200_f32_shift_sign_planes(const float* x_dev, int64_t pixels, int channels, int n_planes,
                                    const float* shifts, int32_t* const* planes_dev, void* stream);
+/* TFLite's RESIZE_NEAREST_NEIGHBOR and RESIZE_BILINEAR (TF/lite/kernels/internal/reference/
+ * resize_nearest_neighbor.h, resize_bilinear.h) of a float NHWC map [batch, in_h, in_w, channels] to
+ * [batch, out_h, out_w, channels]. Per axis, scale = in / (float)out, or with align_corners and
+ * out > 1 (in - 1) / (float)(out - 1), computed in float on the host.
+ * Nearest: source = min(align_corners ? roundf((o + off) * scale) : floorf((o + off) * scale), in - 1)
+ * with off = half_pixel_centers ? 0.5 : 0, and with half_pixel_centers clamped below at 0 too.
+ * Bilinear: v = half_pixel_centers ? (o + 0.5) * scale - 0.5 : o * scale, lo = max(floor(v), 0),
+ * hi = min(ceil(v), in - 1) per axis, and out = x[lo_y,lo_x]*(1-dy)*(1-dx) + x[hi_y,lo_x]*dy*(1-dx)
+ * + x[lo_y,hi_x]*(1-dy)*dx + x[hi_y,hi_x]*dy*dx with dy = v_y - lo_y, dx = v_x - lo_x, left to
+ * right with every product and sum rounded; refuses align_corners with half_pixel_centers, as
+ * TFLite's Prepare does. Every float step is one IEEE operation, so both are the reference kernels'
+ * results bit for bit. */
+int lce_b200_f32_resize_nearest(const float* in_dev, int batch, int in_h, int in_w, int channels, int out_h,
+                                int out_w, int align_corners, int half_pixel_centers, float* out_dev,
+                                void* stream);
+int lce_b200_f32_resize_bilinear(const float* in_dev, int batch, int in_h, int in_w, int channels, int out_h,
+                                 int out_w, int align_corners, int half_pixel_centers, float* out_dev,
+                                 void* stream);
+/* A decoder merge, RESIZE_NEAREST_NEIGHBOR(u) -> ADD(skip) [-> LceQuantize], in one pass that reads u
+ * at each output pixel's nearest source pixel (u [batch, in_h, in_w, channels]; skip, out
+ * [batch, out_h, out_w, channels]):
+ *   out = act(fl(u[source] + skip)),  packed_out[pixel][ceil(channels/32)] = bitpack(out < 0),
+ * the source as lce_b200_f32_resize_nearest finds it, act an LCE_ACT_* code, tail bits 0. out or
+ * packed_out may be NULL (not written). Bit-identical to the three ops one after the other. */
+int lce_b200_f32_upsample_add_sign(const float* u_dev, int batch, int in_h, int in_w, int channels, int out_h,
+                                   int out_w, int align_corners, int half_pixel_centers, const float* skip_dev,
+                                   int activation, float* out_dev, int32_t* packed_out_dev, void* stream);
 /* Grouped CONV_2D (TF/lite/kernels/conv.cc with groups = in_c / filter_in): x NHWC [batch, in_h,
  * in_w, d->in_c], filter OHWI [d->out_c, filter_h, filter_w, d->in_c / groups]; output channel o reads
  * the input channels [(o / (out_c / groups)) * in_c / groups, ...). `groups` must divide in_c and
