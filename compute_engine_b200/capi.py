@@ -107,6 +107,7 @@ EXPORTS = [
     "lce_b200_bconv2d_bases_get_desc", "lce_b200_bconv2d_bases_run", "lce_b200_bconv2d_bases_destroy",
     "lce_b200_f32_shift_sign_planes",
     "lce_b200_f32_resize_nearest", "lce_b200_f32_resize_bilinear", "lce_b200_f32_upsample_add_sign",
+    "lce_b200_detection_max_anchors", "lce_b200_detection_workspace_bytes", "lce_b200_f32_detection_postprocess",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
     "lce_b200_bgemm_destroy", "lce_b200_launch_count",
@@ -366,6 +367,38 @@ def upsample_add_sign(u: torch.Tensor, skip: torch.Tensor, align_corners=False, 
                                                 int(bool(half_pixel_centers)), _p(skip), C.c_int(activation),
                                                 _p(o), _p(pk), _stream()))
     return o, pk
+
+
+class DetectionOptions(C.Structure):
+    """lce_b200_detection_options (TFLite_Detection_PostProcess's custom_options)."""
+    _fields_ = [("max_detections", C.c_int), ("max_classes_per_detection", C.c_int),
+                ("detections_per_class", C.c_int), ("num_classes", C.c_int), ("use_regular_nms", C.c_int),
+                ("nms_score_threshold", C.c_float), ("nms_iou_threshold", C.c_float), ("y_scale", C.c_float),
+                ("x_scale", C.c_float), ("h_scale", C.c_float), ("w_scale", C.c_float)]
+
+
+def detection_max_anchors():
+    return int(lib().lce_b200_detection_max_anchors())
+
+
+def detection_postprocess(boxes: torch.Tensor, scores: torch.Tensor, anchors: torch.Tensor, **options):
+    """TFLite_Detection_PostProcess of float box encodings [B, N, K >= 4], class predictions
+    [B, N, C + label_offset] and anchors [N, 4], each image as TFLite's kernel computes it alone.
+    options: the DetectionOptions fields. Returns (boxes [B, D, 4], classes [B, D], scores [B, D],
+    num_detections [B]) with D = max_detections * max_classes_per_detection."""
+    boxes, scores, anchors = (_dev(t, torch.float32) for t in (boxes, scores, anchors))
+    o = DetectionOptions(**options)
+    b, n, k = boxes.shape
+    d = o.max_detections * o.max_classes_per_detection
+    f = dict(dtype=torch.float32, device=boxes.device)
+    out = (torch.empty((b, d, 4), **f), torch.empty((b, d), **f), torch.empty((b, d), **f), torch.empty((b,), **f))
+    L = lib()
+    L.lce_b200_detection_workspace_bytes.restype = C.c_size_t
+    ws_bytes = L.lce_b200_detection_workspace_bytes(b, n, C.byref(o))
+    ws = torch.empty(max(int(ws_bytes), 16), dtype=torch.uint8, device=boxes.device)
+    _check(L.lce_b200_f32_detection_postprocess(_p(boxes), _p(scores), b, n, k, scores.shape[2], _p(anchors),
+                                                C.byref(o), *(_p(t) for t in out), _p(ws), _stream()))
+    return out
 
 
 class BConv2dBases:

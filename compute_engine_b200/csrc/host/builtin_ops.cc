@@ -6,9 +6,11 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 
 #include "builtin_params.h"
+#include "flexbuffer_map.h"
 #include "host_graph.h"
 #include "lce_b200.h"
 #include "lce_b200_builtins.h"
@@ -1060,6 +1062,125 @@ TfLiteStatus SplitInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+
+// -------------------------- TFLite_Detection_PostProcess -------------------------- //
+// The custom op that ends a TF Object Detection API SSD (TF/lite/kernels/detection_postprocess.cc),
+// float32 inputs only, over the whole batch. inputs [box encodings [B, N, K >= 4], class predictions
+// [B, N, num_classes + label_offset], anchors (constant [N, 4])], outputs [boxes [B, D, 4], classes
+// [B, D], scores [B, D], num_detections [B]] with D = max_detections * max_classes_per_detection, one
+// temporary: lce_b200_f32_detection_postprocess's workspace. The anchors are a constant of a custom op,
+// so the reader leaves them on the host; Prepare validates them there and copies them to device memory
+// the op owns, once.
+struct DetectionOp {
+  lce_b200_detection_options o;
+  float* anchors_dev = nullptr;
+};
+void* DetectionInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* op = new DetectionOp();
+  const FlexMap m(reinterpret_cast<const uint8_t*>(buffer), length);
+  lce_b200_detection_options& o = op->o;
+  o.max_detections = m.AsInt32("max_detections");
+  o.max_classes_per_detection = m.AsInt32("max_classes_per_detection");
+  o.detections_per_class = m.Has("detections_per_class") ? m.AsInt32("detections_per_class") : 100;
+  o.num_classes = m.AsInt32("num_classes");
+  o.use_regular_nms = m.AsBool("use_regular_nms", false) ? 1 : 0;
+  o.nms_score_threshold = m.AsFloat("nms_score_threshold", 0.0f);
+  o.nms_iou_threshold = m.AsFloat("nms_iou_threshold", 0.0f);
+  o.y_scale = m.AsFloat("y_scale", 0.0f);
+  o.x_scale = m.AsFloat("x_scale", 0.0f);
+  o.h_scale = m.AsFloat("h_scale", 0.0f);
+  o.w_scale = m.AsFloat("w_scale", 0.0f);
+  return op;
+}
+void DetectionFree(TfLiteContext*, void* p) {
+  auto* op = static_cast<DetectionOp*>(p);
+  if (op->anchors_dev) cudaFree(op->anchors_dev);
+  delete op;
+}
+TfLiteStatus DetectionPrepare(TfLiteContext* c, TfLiteNode* n) {
+  auto* op = static_cast<DetectionOp*>(n->user_data);
+  const lce_b200_detection_options& o = op->o;
+  B_ENSURE(c, n->inputs->size == 3 && n->outputs->size == 4,
+           "TFLite_Detection_PostProcess: three inputs and four outputs expected");
+  const TfLiteTensor* boxes = T(c, n->inputs, 0);
+  const TfLiteTensor* scores = T(c, n->inputs, 1);
+  const TfLiteTensor* anchors = T(c, n->inputs, 2);
+  B_ENSURE(c, boxes && scores && anchors && boxes->type == kTfLiteFloat32 && scores->type == kTfLiteFloat32 &&
+                  anchors->type == kTfLiteFloat32,
+           "TFLite_Detection_PostProcess: box encodings, class predictions and anchors must be float32 "
+           "(quantized post-processing is not supported)");
+  B_ENSURE(c, boxes->dims->size == 3 && scores->dims->size == 3 && anchors->dims->size == 2,
+           "TFLite_Detection_PostProcess: box encodings and class predictions must be 3-D, anchors 2-D");
+  const int B = boxes->dims->data[0], N = boxes->dims->data[1], K = boxes->dims->data[2];
+  const int S = scores->dims->data[2];
+  B_ENSURE(c, scores->dims->data[0] == B && scores->dims->data[1] == N && anchors->dims->data[0] == N &&
+                  anchors->dims->data[1] == 4 && K >= 4 && N >= 1 && S >= 1,
+           "TFLite_Detection_PostProcess: shapes must be box encodings [B, N, >= 4], class predictions "
+           "[B, N, C] and anchors [N, 4]");
+  B_ENSURE(c, o.num_classes >= 1 && o.num_classes <= S,
+           "TFLite_Detection_PostProcess: num_classes must be in [1, the class predictions' last dimension]");
+  B_ENSURE(c, o.max_detections >= 1, "TFLite_Detection_PostProcess: max_detections must be at least 1");
+  B_ENSURE(c, o.max_classes_per_detection >= 1,
+           "TFLite_Detection_PostProcess: max_classes_per_detection must be at least 1");
+  B_ENSURE(c, !o.use_regular_nms || o.detections_per_class >= 1,
+           "TFLite_Detection_PostProcess: detections_per_class must be at least 1");
+  B_ENSURE(c, o.nms_iou_threshold > 0.0f && o.nms_iou_threshold <= 1.0f,
+           "TFLite_Detection_PostProcess: nms_iou_threshold must be in (0, 1]");
+  if (N > lce_b200_detection_max_anchors()) {
+    c->ReportError(c, "TFLite_Detection_PostProcess: %d anchors are more than the %d one image's NMS holds in "
+                   "shared memory", N, lce_b200_detection_max_anchors());
+    return kTfLiteError;
+  }
+  B_ENSURE(c, anchors->allocation_type == kTfLiteMmapRo && anchors->data.raw && !OnDevice(anchors->data.raw),
+           "TFLite_Detection_PostProcess: the anchors must be a constant tensor");
+  for (int i = 0; i < N; ++i) {
+    const float h = anchors->data.f[4 * i + 2], w = anchors->data.f[4 * i + 3];
+    B_ENSURE(c, std::isfinite(h) && std::isfinite(w) && h >= 0.0f && w >= 0.0f,
+             "TFLite_Detection_PostProcess: anchor heights and widths must be finite and non-negative");
+  }
+  if (!op->anchors_dev) {   // no device on a host-arena graph: Invoke then reports it
+    void* d = nullptr;
+    if (cudaMalloc(&d, sizeof(float) * 4 * N) == cudaSuccess &&
+        cudaMemcpy(d, anchors->data.raw, sizeof(float) * 4 * N, cudaMemcpyHostToDevice) == cudaSuccess) {
+      op->anchors_dev = static_cast<float*>(d);
+    } else {
+      if (d) cudaFree(d);
+      cudaGetLastError();
+    }
+  }
+  if (n->temporaries->size != 1) {
+    int first = 0;
+    if (c->AddTensors(c, 1, &first) != kTfLiteOk) return kTfLiteError;
+    LceB200IntArrayFree(n->temporaries);
+    n->temporaries = LceB200IntArrayCreate(1);
+    n->temporaries->data[0] = first;
+  }
+  TfLiteTensor* ws = &c->tensors[n->temporaries->data[0]];   // c->tensors may have moved
+  ws->type = kTfLiteUInt8;
+  const size_t bytes = lce_b200_detection_workspace_bytes(std::max(B, 1), N, &o);
+  B_ENSURE(c, bytes > 0 && bytes <= static_cast<size_t>(INT32_MAX),
+           "TFLite_Detection_PostProcess: the batch needs too large a workspace");
+  if (Resize(c, ws, {static_cast<int>(bytes)}) != kTfLiteOk) return kTfLiteError;
+  const int D = o.max_detections * o.max_classes_per_detection;
+  if (Resize(c, T(c, n->outputs, 0), {B, D, 4}) != kTfLiteOk || Resize(c, T(c, n->outputs, 1), {B, D}) != kTfLiteOk ||
+      Resize(c, T(c, n->outputs, 2), {B, D}) != kTfLiteOk || Resize(c, T(c, n->outputs, 3), {B}) != kTfLiteOk)
+    return kTfLiteError;
+  for (int k = 0; k < 4; ++k)
+    B_ENSURE(c, T(c, n->outputs, k)->type == kTfLiteFloat32, "TFLite_Detection_PostProcess: outputs must be float32");
+  return kTfLiteOk;
+}
+TfLiteStatus DetectionInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const auto* op = static_cast<const DetectionOp*>(n->user_data);
+  B_ENSURE(c, op->anchors_dev, "TFLite_Detection_PostProcess: the anchors could not be copied to the device");
+  const TfLiteTensor* boxes = T(c, n->inputs, 0);
+  const TfLiteTensor* scores = T(c, n->inputs, 1);
+  const int* d = boxes->dims->data;
+  B_CAPI(c, lce_b200_f32_detection_postprocess(
+                boxes->data.f, scores->data.f, d[0], d[1], d[2], scores->dims->data[2], op->anchors_dev, &op->o,
+                T(c, n->outputs, 0)->data.f, T(c, n->outputs, 1)->data.f, T(c, n->outputs, 2)->data.f,
+                T(c, n->outputs, 3)->data.f, c->tensors[n->temporaries->data[0]].data.raw, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
 }  // namespace
 
 const char* StridedSliceBounds(const int32_t* dims, int rank, const int32_t* begin, const int32_t* end,
@@ -1173,6 +1294,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   static TfLiteRegistration resize_nearest = {Init, Free, ResizePrepare<false>, ResizeInvoke<false>};
   r->AddBuiltin(23, &resize_bilinear);  // RESIZE_BILINEAR
   r->AddBuiltin(97, &resize_nearest);   // RESIZE_NEAREST_NEIGHBOR
+  static TfLiteRegistration detection = {DetectionInit, DetectionFree, DetectionPrepare, DetectionInvoke};
+  r->AddCustom("TFLite_Detection_PostProcess", &detection);
 }
 
 }  // namespace lce_b200

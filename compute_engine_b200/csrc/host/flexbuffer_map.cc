@@ -30,17 +30,22 @@ struct Cursor {
   }
 };
 
-bool ReadScalar(const Cursor& c, size_t slot, int slot_width, uint8_t packed, int64_t* out) {
+// *out is the scalar as AsInt32 converts it, *real the same scalar as a double.
+bool ReadScalar(const Cursor& c, size_t slot, int slot_width, uint8_t packed, int64_t* out, double* real) {
   const int type = packed >> 2;
   const int child_width = 1 << (packed & 3);
+  *real = 0.0;
   switch (type) {
     case kInt:
-      return c.ReadI(slot, slot_width, out);
+      if (!c.ReadI(slot, slot_width, out)) return false;
+      *real = static_cast<double>(*out);
+      return true;
     case kUInt:
     case kBool: {
       uint64_t u;
       if (!c.ReadU(slot, slot_width, &u)) return false;
       *out = static_cast<int64_t>(u);
+      *real = static_cast<double>(u);
       return true;
     }
     case kFloat: {
@@ -49,6 +54,7 @@ bool ReadScalar(const Cursor& c, size_t slot, int slot_width, uint8_t packed, in
         if (!c.in(slot, 4)) return false;
         memcpy(&f, c.base + slot, 4);
         *out = static_cast<int64_t>(f);
+        *real = f;
         return true;
       }
       if (slot_width == 8) {
@@ -56,6 +62,7 @@ bool ReadScalar(const Cursor& c, size_t slot, int slot_width, uint8_t packed, in
         if (!c.in(slot, 8)) return false;
         memcpy(&d, c.base + slot, 8);
         *out = static_cast<int64_t>(d);
+        *real = d;
         return true;
       }
       return false;
@@ -110,8 +117,11 @@ FlexMap::FlexMap(const uint8_t* buffer, size_t length) {
     if (!nul) return;
     keys_.emplace_back(reinterpret_cast<const char*>(buffer + kaddr));
     int64_t v;
-    if (!ReadScalar(c, map + i * w, w, buffer[types + i], &v)) return;
+    double real;
+    if (!ReadScalar(c, map + i * w, w, buffer[types + i], &v, &real)) return;
     values_.push_back(v);
+    reals_.push_back(real);
+    types_.push_back(buffer[types + i] >> 2);
   }
   ok_ = true;
 }
@@ -126,6 +136,31 @@ int32_t FlexMap::AsInt32(const char* key) const {
   for (size_t i = 0; i < keys_.size(); ++i)
     if (keys_[i] == key) return static_cast<int32_t>(values_[i]);
   return 0;
+}
+
+int FlexMap::Find(const char* key) const {
+  if (!ok_) return -1;
+  for (size_t i = 0; i < keys_.size(); ++i)
+    if (keys_[i] == key) return static_cast<int>(i);
+  return -1;
+}
+
+bool FlexMap::IsNumber(int i) const {
+  return i >= 0 && (types_[i] == kInt || types_[i] == kUInt || types_[i] == kFloat || types_[i] == kBool ||
+                    types_[i] == kIndirectInt || types_[i] == kIndirectUInt);
+}
+
+float FlexMap::AsFloat(const char* key, float default_value) const {
+  const int i = Find(key);
+  if (!IsNumber(i)) return default_value;
+  return (types_[i] == kIndirectInt || types_[i] == kIndirectUInt) ? static_cast<float>(values_[i])
+                                                                   : static_cast<float>(reals_[i]);
+}
+
+bool FlexMap::AsBool(const char* key, bool default_value) const {
+  const int i = Find(key);
+  if (!IsNumber(i)) return default_value;
+  return types_[i] == kFloat ? reals_[i] != 0.0 : values_[i] != 0;
 }
 
 std::vector<uint8_t> WriteFlexIntMap(std::vector<std::pair<std::string, int64_t>> items) {

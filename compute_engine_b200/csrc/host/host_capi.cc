@@ -215,6 +215,12 @@ int lce_host_flex_get_int(const uint8_t* buf, size_t len, const char* key, int* 
   *found = m.Has(key) ? 1 : 0;
   return m.AsInt32(key);
 }
+float lce_host_flex_get_float(const uint8_t* buf, size_t len, const char* key, float default_value) {
+  return lce_b200::FlexMap(buf, len).AsFloat(key, default_value);
+}
+int lce_host_flex_get_bool(const uint8_t* buf, size_t len, const char* key, int default_value) {
+  return lce_b200::FlexMap(buf, len).AsBool(key, default_value != 0) ? 1 : 0;
+}
 int lce_host_flex_map_size(const uint8_t* buf, size_t len) {
   lce_b200::FlexMap m(buf, len);
   return m.ok() ? static_cast<int>(m.size()) : -1;

@@ -47,6 +47,8 @@ def lib():
         L.lce_host_tensor_scale.restype = C.c_float
         L.lce_host_node_time_ms.restype = C.c_double
         L.lce_host_node_name.restype = C.c_char_p
+        L.lce_host_flex_get_float.restype = C.c_float
+        L.lce_host_flex_get_float.argtypes = [C.c_void_p, C.c_size_t, C.c_char_p, C.c_float]
         for name in ("lce_host_graph_destroy", "lce_host_last_error", "lce_host_allocate_tensors",
                      "lce_host_invoke", "lce_host_num_tensors", "lce_host_num_nodes",
                      "lce_host_arena_bytes", "lce_host_stream", "lce_host_num_inputs",
@@ -71,6 +73,17 @@ def flex_get_int(blob: bytes, key: str):
     buf = (C.c_uint8 * len(blob)).from_buffer_copy(blob) if blob else None
     v = lib().lce_host_flex_get_int(buf, C.c_size_t(len(blob)), key.encode(), C.byref(found))
     return v if found.value else None
+
+
+def flex_get_float(blob: bytes, key: str, default=0.0):
+    """FlexMap::AsFloat: a FLOAT, INT, UINT or BOOL value as float32; default for a missing key."""
+    buf = (C.c_uint8 * len(blob)).from_buffer_copy(blob) if blob else None
+    return lib().lce_host_flex_get_float(buf, C.c_size_t(len(blob)), key.encode(), C.c_float(default))
+
+
+def flex_get_bool(blob: bytes, key: str, default=False):
+    buf = (C.c_uint8 * len(blob)).from_buffer_copy(blob) if blob else None
+    return bool(lib().lce_host_flex_get_bool(buf, C.c_size_t(len(blob)), key.encode(), int(bool(default))))
 
 
 def flex_map_size(blob: bytes):

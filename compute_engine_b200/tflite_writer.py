@@ -254,19 +254,29 @@ class TFLiteModel:
 
 
 # --------------------------------------------------------------------------- #
-# FlexBuffers map of integers (the LCE ops' custom_options), in pure
-# Python so that a model can be serialised without loading any native library. Emits the same
-# bytes as csrc/host/flexbuffer_map.cc::WriteFlexIntMap (tests/test_host_ops.py compares them,
-# and both reproduce the blobs the real flatbuffers library wrote into
-# LCE/mlir/tests/legalize-lce.mlir:9,21).
+# FlexBuffers maps of scalars (the custom ops' custom_options), in pure Python so that a model can
+# be serialised without loading any native library. An int map is the same bytes as
+# csrc/host/flexbuffer_map.cc::WriteFlexIntMap (tests/test_host_ops.py compares them, and both
+# reproduce the blobs the real flatbuffers library wrote into LCE/mlir/tests/legalize-lce.mlir:9,21).
 # --------------------------------------------------------------------------- #
-_FBT_INT, _FBT_MAP = 1, 9
+_FBT_INT, _FBT_FLOAT, _FBT_MAP, _FBT_BOOL = 1, 3, 9, 26
 
 
-def flex_int_map(items: dict) -> bytes:
+def flex_map(items: dict) -> bytes:
+    """A map of int, bool and float scalars as flexbuffers::Builder writes it: keys sorted by their
+    bytes, every value at the map's one byte width (the least that fits all of them). A Python float
+    is Builder::Float (float32, at least 4 bytes), a numpy float64 Builder::Double (8 bytes); a float
+    at byte width 8 is stored as a double, as the builder stores it."""
     keys = list(items)
     order = sorted(range(len(keys)), key=lambda i: keys[i].encode())
-    for log2w in range(3):
+    vals = [items[k] for k in keys]
+    min_log2w = 0
+    for v in vals:
+        if isinstance(v, np.float64):
+            min_log2w = 3
+        elif isinstance(v, (float, np.floating)):
+            min_log2w = max(min_log2w, 2)
+    for log2w in range(min_log2w, 4):
         w = 1 << log2w
         lim = 1 << (8 * w - 1)
         out = bytearray()
@@ -296,13 +306,23 @@ def flex_int_map(items: dict) -> bytes:
         put(w)
         put(len(keys))
         mp = len(out)
+        types = []
         for i in order:
-            v = int(items[keys[i]])
-            if v >= lim or v < -lim:
-                fits = False
-            put(v)
-        for _ in keys:
-            out.append((_FBT_INT << 2) | log2w)
+            v = vals[i]
+            if isinstance(v, (bool, np.bool_)):
+                put(int(v))
+                types.append(_FBT_BOOL)
+            elif isinstance(v, (float, np.floating)):
+                out.extend(struct.pack("<f" if w == 4 else "<d", float(v)))
+                types.append(_FBT_FLOAT)
+            else:
+                v = int(v)
+                if v >= lim or v < -lim:
+                    fits = False
+                put(v)
+                types.append(_FBT_INT)
+        for t in types:
+            out.append((t << 2) | log2w)
         align()
         if len(out) - mp >= (1 << (8 * w)):
             fits = False
@@ -312,7 +332,32 @@ def flex_int_map(items: dict) -> bytes:
         out.append((_FBT_MAP << 2) | log2w)
         out.append(w)
         return bytes(out)
-    raise ValueError("flexbuffer map does not fit 32-bit offsets")
+    raise ValueError("flexbuffer map does not fit 64-bit offsets")
+
+
+def flex_int_map(items: dict) -> bytes:
+    """A map of integers (the LCE ops' attributes): byte widths 1, 2 or 4."""
+    out = flex_map({k: int(v) for k, v in items.items()})
+    if out[-1] > 4:
+        raise ValueError("flexbuffer map does not fit 32-bit offsets")
+    return out
+
+
+def detection_postprocess_options(max_detections=100, max_classes_per_detection=1, detections_per_class=100,
+                                  num_classes=90, use_regular_nms=False, nms_score_threshold=1e-8,
+                                  nms_iou_threshold=0.6, y_scale=10.0, x_scale=10.0, h_scale=5.0,
+                                  w_scale=5.0, converter_keys=True) -> bytes:
+    """custom_options of TFLite_Detection_PostProcess, with the keys the TF Object Detection API's
+    export writes (export_tflite_ssd_graph_lib.py) and, with converter_keys, the two flags TF's
+    converter adds."""
+    items = {"max_detections": max_detections, "max_classes_per_detection": max_classes_per_detection,
+             "detections_per_class": detections_per_class, "use_regular_nms": bool(use_regular_nms),
+             "nms_score_threshold": float(nms_score_threshold), "nms_iou_threshold": float(nms_iou_threshold),
+             "num_classes": num_classes, "y_scale": float(y_scale), "x_scale": float(x_scale),
+             "h_scale": float(h_scale), "w_scale": float(w_scale)}
+    if converter_keys:
+        items.update({"_output_quantized": True, "_support_output_type_float_in_quantized_op": True})
+    return flex_map(items)
 
 
 def bconv2d_options(channels_in, stride=(1, 1), dilation=(1, 1), padding=0, pad_values=1,

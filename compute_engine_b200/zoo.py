@@ -24,9 +24,9 @@ import numpy as np
 # native library is loaded, so bench.py's reference arm can synthesise the very same model bytes
 # by loading these two files alone (importlib, not the package).
 try:
-    from .tflite_writer import TFLiteModel, bconv2d_options
+    from .tflite_writer import TFLiteModel, bconv2d_options, detection_postprocess_options
 except ImportError:      # loaded as a stand-alone file next to tflite_writer.py
-    from tflite_writer import TFLiteModel, bconv2d_options
+    from tflite_writer import TFLiteModel, bconv2d_options, detection_postprocess_options
 
 
 # Quantisation of an int8 image input (`input_type="int8"`): what the converter attaches to the
@@ -106,7 +106,7 @@ class _Builder:
                       [y], padding=padding, stride=(stride, stride), activation=activation)
         return y, (b, oh, ow, cout)
 
-    def depthwise(self, x, xs, k, stride, padding="SAME", blur=False, bn=False):
+    def depthwise(self, x, xs, k, stride, padding="SAME", blur=False, bn=False, activation="NONE"):
         b, h, w, c = xs
         if blur:   # blurpool: fixed binomial kernel
             a = np.array([1.0, 2.0, 1.0], np.float32)
@@ -123,7 +123,7 @@ class _Builder:
         ow = -(-w // stride) if padding == "SAME" else (w - k) // stride + 1
         y = self.act((b, oh, ow, c))
         self.m.add_op("DEPTHWISE_CONV_2D", [x, self.const(wt), self.const(bias, name="b")], [y],
-                      padding=padding, stride=(stride, stride), depth_multiplier=1)
+                      padding=padding, stride=(stride, stride), depth_multiplier=1, activation=activation)
         return y, (b, oh, ow, c)
 
     def pool(self, kind, x, xs, k, stride, padding):
@@ -291,6 +291,81 @@ def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, d
     out = g.act((b, image, image, classes))
     g.m.add_op("RESIZE_BILINEAR", [logits, size(image, image)], [out], half_pixel_centers=True)
     g.m.outputs = [out]
+    return g.m.serialize()
+
+
+def ssd_anchors(grids, min_scale=0.2, max_scale=0.95):
+    """The TF Object Detection API's SSD anchors (anchor_generators/multiple_grid_anchor_generator.py,
+    create_ssd_anchors with its defaults) for feature maps of `grids` [(h, w), ...], in float32 as
+    TFLite_Detection_PostProcess reads them: [N, 4] rows of (y_center, x_center, height, width),
+    ordered by (row, column, anchor) as a head's [B, h, w, A * 4] map reshapes to [B, h * w * A, 4].
+    The lowest map gets (0.1, 1), (s, 2), (s, 1/2); every other map (s, r) for the aspect ratios
+    r in (1, 2, 3, 1/2, 1/3) and (sqrt(s * s_next), 1), with the scales s spread evenly over
+    [min_scale, max_scale] and 1 after the last."""
+    f32 = np.float32
+    n = len(grids)
+    scales = [min_scale + (max_scale - min_scale) * i / (n - 1) for i in range(n)] + [1.0]
+    out = []
+    for layer, (h, w) in enumerate(grids):
+        s, s_next = scales[layer], scales[layer + 1]
+        if layer == 0:
+            specs = [(0.1, 1.0), (s, 2.0), (s, 0.5)]
+        else:
+            specs = [(s, r) for r in (1.0, 2.0, 3.0, 0.5, 1.0 / 3.0)] + [(np.sqrt(s * s_next), 1.0)]
+        sc = np.array([p[0] for p in specs], f32)
+        ar = np.sqrt(np.array([p[1] for p in specs], f32))
+        heights, widths = sc / ar, sc * ar
+        yc = (np.arange(h, dtype=f32) * f32(1.0 / h) + f32(0.5 / h)).astype(f32)
+        xc = (np.arange(w, dtype=f32) * f32(1.0 / w) + f32(0.5 / w)).astype(f32)
+        a = np.empty((h, w, len(specs), 4), f32)
+        a[..., 0] = yc[:, None, None]
+        a[..., 1] = xc[None, :, None]
+        a[..., 2] = heights
+        a[..., 3] = widths
+        out.append(a.reshape(-1, 4))
+    return np.concatenate(out).astype(f32)
+
+
+def quicknet_ssd(batch=1, seed=0, image=224, input_type="float32", classes=20, postprocess=True,
+                 use_regular_nms=False):
+    """A binary SSDLite detector: QuickNet's encoder, then on its 28x28x128, 14x14x256 and 7x7x512
+    maps (at 224) a head of A = 3, 6 and 6 anchors per cell: DEPTHWISE_CONV_2D 3x3 (BatchNorm folded,
+    RELU) -> CONV_2D 1x1 to A * 4 box encodings and another to A * (classes + 1) class logits, each
+    RESHAPEd to [B, h * w * A, 4 | classes + 1]. The maps are joined by CONCATENATION on axis 1, the
+    logits go through LOGISTIC, and TFLite_Detection_PostProcess (the TF OD API's export defaults:
+    100 detections, 1 class each, 100 per class, score threshold 1e-8, IoU threshold 0.6, scales
+    10, 10, 5, 5) turns them into the outputs [boxes [B, 100, 4], classes, scores [B, 100],
+    num_detections [B]], with the anchors of ssd_anchors(). postprocess=False leaves the op out: the
+    outputs are then the box encodings [B, N, 4] and the class scores [B, N, classes + 1]."""
+    if image % 32:
+        raise ValueError(f"quicknet_ssd needs an image size that is a multiple of 32, not {image}")
+    g = _Builder(seed, batch, "QuickNetSSD")
+    sections = _quicknet_encoder(g, batch, image, input_type, (4, 4, 4, 4), (64, 128, 256, 512))
+    boxes, logits, grids = [], [], []
+    for (x, xs), a in zip(sections[1:], (3, 6, 6)):
+        b, h, w, _ = xs
+        t, ts = g.depthwise(x, xs, 3, 1, bn=True, activation="RELU")
+        for width, maps in ((4, boxes), (classes + 1, logits)):
+            y, _ = g.conv(t, ts, a * width, 1, 1)
+            r = g.act((b, h * w * a, width))
+            g.m.add_op("RESHAPE", [y], [r], new_shape=[-1, h * w * a, width])
+            maps.append(r)
+        grids.append((h, w))
+    anchors = ssd_anchors(grids)
+    n = anchors.shape[0]
+    enc = g.act((batch, n, 4))
+    g.m.add_op("CONCATENATION", boxes, [enc], axis=1)
+    cat = g.act((batch, n, classes + 1))
+    g.m.add_op("CONCATENATION", logits, [cat], axis=1)
+    scores = g.act((batch, n, classes + 1))
+    g.m.add_op("LOGISTIC", [cat], [scores])
+    if not postprocess:
+        g.m.outputs = [enc, scores]
+        return g.m.serialize()
+    outs = [g.act((batch, 100, 4)), g.act((batch, 100)), g.act((batch, 100)), g.act((batch,))]
+    g.m.add_op("TFLite_Detection_PostProcess", [enc, scores, g.const(anchors, name="anchors")], outs,
+               custom_options=detection_postprocess_options(num_classes=classes, use_regular_nms=use_regular_nms))
+    g.m.outputs = outs
     return g.m.serialize()
 
 

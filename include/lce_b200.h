@@ -335,6 +335,34 @@ int lce_b200_f32_resize_bilinear(const float* in_dev, int batch, int in_h, int i
 int lce_b200_f32_upsample_add_sign(const float* u_dev, int batch, int in_h, int in_w, int channels, int out_h,
                                    int out_w, int align_corners, int half_pixel_centers, const float* skip_dev,
                                    int activation, float* out_dev, int32_t* packed_out_dev, void* stream);
+/* TFLite_Detection_PostProcess (TF/lite/kernels/detection_postprocess.cc) with its float32 inputs,
+ * applied to every image of a batch as TFLite applies it to its single image. */
+typedef struct {
+  int max_detections, max_classes_per_detection, detections_per_class, num_classes, use_regular_nms;
+  float nms_score_threshold, nms_iou_threshold, y_scale, x_scale, h_scale, w_scale;
+} lce_b200_detection_options;
+/* The largest anchor count one image's (or one class's) NMS holds in shared memory. */
+int lce_b200_detection_max_anchors(void);
+/* Device workspace bytes lce_b200_f32_detection_postprocess needs (0 for invalid arguments). */
+size_t lce_b200_detection_workspace_bytes(int batch, int num_anchors, const lce_b200_detection_options* opts);
+/* boxes [batch, num_anchors, box_dim >= 4] (y, x, h, w encodings; the first 4 of each row are read),
+ * scores [batch, num_anchors, score_dim] (class c at c + score_dim - num_classes), anchors
+ * [num_anchors, 4] (y, x, h, w), all device float32. Outputs, D = max_detections *
+ * max_classes_per_detection: det_boxes [batch, D, 4] (ymin, xmin, ymax, xmax; 16-byte aligned),
+ * det_classes and det_scores [batch, D], num_detections [batch]; every element is written, the slots
+ * TFLite leaves alone as 0. Decode: ycenter = y / y_scale * ha + ya, half_h = 0.5f * exp(h / h_scale) * ha
+ * and so on, each step rounded in float, exp in double rounded once. A score is kept when
+ * >= nms_score_threshold; candidates go by score descending (-0 as +0), ties to the lower anchor; a
+ * candidate is dropped when its IoU with a selected box (TFLite's formula; 0 for a box of non-positive
+ * area) is > nms_iou_threshold. Fast mode: NMS on each anchor's best score (ArgMaxVector for one class
+ * per detection; several go by score descending, class ascending, NaN last). Regular mode: NMS per class
+ * up to detections_per_class, then the stable top-max_detections of the class lists in class order.
+ * Refuses more than lce_b200_detection_max_anchors() anchors. No allocation, no synchronisation. */
+int lce_b200_f32_detection_postprocess(const float* boxes_dev, const float* scores_dev, int batch, int num_anchors,
+                                       int box_dim, int score_dim, const float* anchors_dev,
+                                       const lce_b200_detection_options* opts, float* det_boxes_dev,
+                                       float* det_classes_dev, float* det_scores_dev, float* num_detections_dev,
+                                       void* workspace_dev, void* stream);
 /* Grouped CONV_2D (TF/lite/kernels/conv.cc with groups = in_c / filter_in): x NHWC [batch, in_h,
  * in_w, d->in_c], filter OHWI [d->out_c, filter_h, filter_w, d->in_c / groups]; output channel o reads
  * the input channels [(o / (out_c / groups)) * in_c / groups, ...). `groups` must divide in_c and
