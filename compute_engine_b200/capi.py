@@ -12,6 +12,7 @@ LceBconv2d (Init/Prepare/Eval as constructor / set_input_shape / __call__),
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 
 import torch
@@ -107,6 +108,7 @@ EXPORTS = [
     "lce_b200_bconv2d_bases_get_desc", "lce_b200_bconv2d_bases_run", "lce_b200_bconv2d_bases_destroy",
     "lce_b200_f32_shift_sign_planes",
     "lce_b200_f32_resize_nearest", "lce_b200_f32_resize_bilinear", "lce_b200_f32_upsample_add_sign",
+    "lce_b200_f32_argmax", "lce_b200_resize_bilinear_argmax_max_row_floats", "lce_b200_f32_resize_bilinear_argmax",
     "lce_b200_detection_max_anchors", "lce_b200_detection_workspace_bytes", "lce_b200_f32_detection_postprocess",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
@@ -349,6 +351,42 @@ def resize(x: torch.Tensor, size, bilinear=False, align_corners=False, half_pixe
     fn = lib().lce_b200_f32_resize_bilinear if bilinear else lib().lce_b200_f32_resize_nearest
     _check(fn(_p(x), b, h, w, c, oh, ow, int(bool(align_corners)), int(bool(half_pixel_centers)), _p(out),
               _stream()))
+    return out
+
+
+def argmax(x: torch.Tensor, axis=-1, out_dtype=torch.int64):
+    """ARG_MAX of a float tensor over `axis`, bit for bit TFLite's reference loop (ties to the lowest
+    index, a NaN at index 0 gives 0, a NaN elsewhere is never chosen); int64 or int32 labels."""
+    x = _dev(x, torch.float32)
+    if out_dtype not in (torch.int64, torch.int32):
+        raise LceError("argmax: out_dtype must be torch.int64 or torch.int32")
+    a = axis + x.dim() if axis < 0 else axis
+    if x.dim() < 1 or not 0 <= a < x.dim():
+        raise LceError(f"argmax: axis {axis} is out of range for rank {x.dim()}")
+    outer, inner = math.prod(x.shape[:a]), math.prod(x.shape[a + 1:])
+    out = torch.empty(x.shape[:a] + x.shape[a + 1:], dtype=out_dtype, device=x.device)
+    _check(lib().lce_b200_f32_argmax(_p(x), C.c_int64(outer), C.c_int(x.shape[a]), C.c_int64(inner),
+                                     int(out_dtype == torch.int64), _p(out), _stream()))
+    return out
+
+
+def resize_bilinear_argmax_max_row_floats():
+    return int(lib().lce_b200_resize_bilinear_argmax_max_row_floats())
+
+
+def resize_bilinear_argmax(x: torch.Tensor, size, align_corners=False, half_pixel_centers=False,
+                           out_dtype=torch.int64):
+    """ARG_MAX over the channels of RESIZE_BILINEAR(x) to size = (new_height, new_width), in one pass
+    that never writes the resized map: the labels [B, new_height, new_width], bit for bit the two ops'."""
+    x = _dev(x, torch.float32)
+    if out_dtype not in (torch.int64, torch.int32):
+        raise LceError("resize_bilinear_argmax: out_dtype must be torch.int64 or torch.int32")
+    b, h, w, c = x.shape
+    oh, ow = int(size[0]), int(size[1])
+    out = torch.empty((b, oh, ow), dtype=out_dtype, device=x.device)
+    _check(lib().lce_b200_f32_resize_bilinear_argmax(_p(x), b, h, w, c, oh, ow, int(bool(align_corners)),
+                                                     int(bool(half_pixel_centers)), int(out_dtype == torch.int64),
+                                                     _p(out), _stream()))
     return out
 
 

@@ -916,6 +916,89 @@ TfLiteStatus MergeInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// --------------------------------- ARG_MAX --------------------------------- //
+// inputs [x (float32, rank >= 1), axis (read on the host, as the resizes read their size)]; output x's
+// shape without the axis, of ArgMaxOptions.output_type (int32 or int64) (TF/lite/kernels/arg_min_max.cc).
+// Checks x = input 0, the axis at input `axis_input` and output 0; returns nullptr, or why they are refused.
+const char* ArgMaxChecks(TfLiteContext* c, TfLiteNode* n, int axis_input, const BuiltinParams& p, int* axis) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  if (!x || x->type != kTfLiteFloat32 || x->dims->size < 1)
+    return "ARG_MAX: the input must be a float32 tensor of rank 1 or more";
+  const char* why = ArgMaxAxis(T(c, n->inputs, axis_input), x->dims->size, axis);
+  if (why) return why;
+  if (x->dims->data[*axis] <= 0) return "ARG_MAX: the reduced axis is empty";
+  if (p.output_type != 2 && p.output_type != 4) return "ARG_MAX: output_type must be int32 or int64";
+  const TfLiteTensor* o = T(c, n->outputs, 0);
+  if (!o || o->type != (p.output_type == 4 ? kTfLiteInt64 : kTfLiteInt32))
+    return "ARG_MAX: the output tensor's type differs from output_type";
+  return nullptr;
+}
+TfLiteStatus ArgMaxPrepare(TfLiteContext* c, TfLiteNode* n) {
+  B_ENSURE(c, n->inputs->size == 2 && n->outputs->size == 1, "ARG_MAX: inputs [x, axis] and one output expected");
+  int axis;
+  const char* why = ArgMaxChecks(c, n, 1, P(n), &axis);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteIntArray* d = T(c, n->inputs, 0)->dims;
+  TfLiteIntArray* dims = LceB200IntArrayCreate(d->size - 1);
+  for (int k = 0, j = 0; k < d->size; ++k)
+    if (k != axis) dims->data[j++] = d->data[k];
+  return c->ResizeTensor(c, T(c, n->outputs, 0), dims);
+}
+TfLiteStatus ArgMaxInvoke(TfLiteContext* c, TfLiteNode* n) {
+  int axis;
+  const char* why = ArgMaxChecks(c, n, 1, P(n), &axis);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  TfLiteTensor* o = T(c, n->outputs, 0);
+  int64_t outer = 1, inner = 1;
+  for (int k = 0; k < axis; ++k) outer *= x->dims->data[k];
+  for (int k = axis + 1; k < x->dims->size; ++k) inner *= x->dims->data[k];
+  B_CAPI(c, lce_b200_f32_argmax(x->data.f, outer, x->dims->data[axis], inner, o->type == kTfLiteInt64,
+                                o->data.raw, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// ------------------ fused RESIZE_BILINEAR -> ARG_MAX: a segmentation head ------------------ //
+// Created by Graph::FuseResizeArgmax; builtin_data = { BuiltinParams resize, BuiltinParams argmax };
+// inputs [x, size, axis (the channel axis)], outputs [labels [B, new_height, new_width]].
+struct ResizeArgmaxParams {
+  BuiltinParams resize, argmax;
+};
+void* ResizeArgmaxInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* p = new ResizeArgmaxParams();
+  memset(p, 0, sizeof(*p));
+  if (buffer && length >= sizeof(ResizeArgmaxParams)) memcpy(p, buffer, sizeof(ResizeArgmaxParams));
+  return p;
+}
+void ResizeArgmaxFree(TfLiteContext*, void* p) { delete static_cast<ResizeArgmaxParams*>(p); }
+TfLiteStatus ResizeArgmaxPrepare(TfLiteContext* c, TfLiteNode* n) {
+  const auto& rp = *static_cast<const ResizeArgmaxParams*>(n->user_data);
+  B_ENSURE(c, n->inputs->size == 3 && n->outputs->size == 1,
+           "RESIZE_BILINEAR+ARG_MAX: inputs [x, size, axis] and one output expected");
+  int32_t oh, ow;
+  const char* why = ResizeGeometry(c, n, true, rp.resize, &oh, &ow);
+  B_ENSURE(c, why == nullptr, why);
+  int axis;
+  why = ArgMaxChecks(c, n, 2, rp.argmax, &axis);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteIntArray* d = T(c, n->inputs, 0)->dims;
+  B_ENSURE(c, axis == 3, "RESIZE_BILINEAR+ARG_MAX: the axis must be the channel axis");
+  B_ENSURE(c, static_cast<int64_t>(d->data[2]) * d->data[3] <= lce_b200_resize_bilinear_argmax_max_row_floats(),
+           "RESIZE_BILINEAR+ARG_MAX: the source rows do not fit shared memory");
+  return Resize(c, T(c, n->outputs, 0), {d->data[0], oh, ow});
+}
+TfLiteStatus ResizeArgmaxInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const auto& rp = *static_cast<const ResizeArgmaxParams*>(n->user_data);
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  TfLiteTensor* o = T(c, n->outputs, 0);
+  const int* d = x->dims->data;
+  B_CAPI(c, lce_b200_f32_resize_bilinear_argmax(x->data.f, d[0], d[1], d[2], d[3], o->dims->data[1],
+                                                o->dims->data[2], rp.resize.align_corners,
+                                                rp.resize.half_pixel_centers, o->type == kTfLiteInt64,
+                                                o->data.raw, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // ------------------------------ CONCATENATION ------------------------------ //
 // Strided device copies (one cudaMemcpy2DAsync per input): no kernel of ours.
 TfLiteStatus ConcatPrepare(TfLiteContext* c, TfLiteNode* n) {
@@ -1214,6 +1297,22 @@ const char* StridedSliceBounds(const int32_t* dims, int rank, const int32_t* beg
   return nullptr;
 }
 
+const char* ArgMaxAxis(const TfLiteTensor* axis, int rank, int* out) {
+  if (!axis || axis->allocation_type != kTfLiteMmapRo || !axis->data.raw || OnDevice(axis->data.raw))
+    return "ARG_MAX: the axis must be a constant tensor";
+  if (axis->type != kTfLiteInt32 && axis->type != kTfLiteInt64) return "ARG_MAX: the axis must be int32 or int64";
+  if (axis->dims->size > 1 || Count(axis) != 1) return "ARG_MAX: the axis must have exactly one element";
+  int64_t a;
+  if (axis->type == kTfLiteInt32) {
+    a = axis->data.i32[0];
+  } else {
+    memcpy(&a, axis->data.raw, sizeof(a));
+  }
+  if (a < -rank || a >= rank) return "ARG_MAX: the axis is out of range";
+  *out = static_cast<int>(a < 0 ? a + rank : a);
+  return nullptr;
+}
+
 const TfLiteRegistration* FusedStemRegistration() {
   static TfLiteRegistration r = {StemInit, StemFree, StemPrepare, StemInvoke};
   return &r;
@@ -1236,6 +1335,10 @@ const TfLiteRegistration* PooledSignRegistration() {
 }
 const TfLiteRegistration* GroupedConvAffineRegistration() {
   static TfLiteRegistration r = {ConvAffineInit, ConvAffineFree, ConvAffinePrepare, ConvAffineInvoke};
+  return &r;
+}
+const TfLiteRegistration* ResizeArgmaxRegistration() {
+  static TfLiteRegistration r = {ResizeArgmaxInit, ResizeArgmaxFree, ResizeArgmaxPrepare, ResizeArgmaxInvoke};
   return &r;
 }
 const TfLiteRegistration* UpsampleMergeRegistration() {
@@ -1294,6 +1397,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   static TfLiteRegistration resize_nearest = {Init, Free, ResizePrepare<false>, ResizeInvoke<false>};
   r->AddBuiltin(23, &resize_bilinear);  // RESIZE_BILINEAR
   r->AddBuiltin(97, &resize_nearest);   // RESIZE_NEAREST_NEIGHBOR
+  static TfLiteRegistration arg_max = {Init, Free, ArgMaxPrepare, ArgMaxInvoke};
+  r->AddBuiltin(56, &arg_max);   // ARG_MAX
   static TfLiteRegistration detection = {DetectionInit, DetectionFree, DetectionPrepare, DetectionInvoke};
   r->AddCustom("TFLite_Detection_PostProcess", &detection);
 }

@@ -6,6 +6,8 @@
 #define LCE_B200_HOST_BUILTIN_PARAMS_H_
 #include <cstdint>
 
+#include "lce_b200_tflite.h"
+
 namespace lce_b200 {
 struct BuiltinParams {
   int32_t builtin_code;
@@ -22,7 +24,14 @@ struct BuiltinParams {
   int32_t num_splits;
   // RESIZE_BILINEAR (ResizeBilinearOptions) and RESIZE_NEAREST_NEIGHBOR (ResizeNearestNeighborOptions)
   int32_t align_corners, half_pixel_centers;
+  // ARG_MAX (ArgMaxOptions): the output's TensorType code
+  int32_t output_type;
 };
+
+// ARG_MAX's axis: a constant int32 or int64 tensor of one element (0-D or [1]) in host memory, within
+// [-rank, rank) and normalised to [0, rank). Returns nullptr, or why the axis is refused.
+// builtin_ops.cc; Graph::FuseResizeArgmax reads the axis through it too.
+const char* ArgMaxAxis(const TfLiteTensor* axis, int rank, int* out);
 
 // STRIDED_SLICE's bounds for an input of dims[0..rank) and n = the length of begin / end / strides,
 // normalised as TFLite's strided_slice.cc does (masks, negative indices, clamping): the output is

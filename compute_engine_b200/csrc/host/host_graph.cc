@@ -312,6 +312,8 @@ constexpr const char* kDequantize = "builtin:6";
 constexpr const char* kFullyConnected = "builtin:9";
 constexpr const char* kMaxPool2d = "builtin:17";
 constexpr const char* kResizeNearest = "builtin:97";
+constexpr const char* kResizeBilinear = "builtin:23";
+constexpr const char* kArgMax = "builtin:56";
 constexpr const char* kMul = "builtin:18";
 constexpr const char* kRelu = "builtin:19";
 constexpr const char* kMean = "builtin:40";
@@ -1741,6 +1743,47 @@ int Graph::FuseUpsampleMerges() {
     const int k = fuse(i);
     removed += k;
     if (k == 0) ++i;   // else node i is erased and its successor moved up
+  }
+  allocated_ = false;
+  return removed;
+}
+
+const TfLiteRegistration* ResizeArgmaxRegistration();   // builtin_ops.cc
+
+int Graph::FuseResizeArgmax() {
+  if (!device_arena_) return 0;
+  auto fuse = [&](size_t i) -> bool {   // the resize at i is fused into its ARG_MAX and erased
+    NodeRecord& r = *nodes_[i];
+    if (r.name != kResizeBilinear || r.initialized || r.node.inputs->size != 2 || r.node.outputs->size != 1 ||
+        !Params(r))
+      return false;
+    const int x = r.node.inputs->data[0], size = r.node.inputs->data[1], v = r.node.outputs->data[0];
+    if (x < 0 || size < 0 || tensors_[x].type != kTfLiteFloat32 || tensors_[v].type != kTfLiteFloat32) return false;
+    const TfLiteIntArray* xd = tensors_[x].dims;
+    if (!xd || xd->size != 4 || !tensors_[v].dims || tensors_[v].dims->size != 4) return false;
+    const size_t ai = SoleReaderAsFirstInput(v);
+    if (ai == kNoNode || ai <= i) return false;
+    NodeRecord& a = *nodes_[ai];
+    if (a.name != kArgMax || a.initialized || a.node.inputs->size != 2 || a.node.outputs->size != 1 || !Params(a))
+      return false;
+    const int axis_t = a.node.inputs->data[1];
+    int axis;
+    if (axis_t < 0 || ArgMaxAxis(&tensors_[axis_t], 4, &axis) != nullptr || axis != 3) return false;
+    if (static_cast<int64_t>(xd->data[2]) * xd->data[3] > lce_b200_resize_bilinear_argmax_max_row_floats())
+      return false;
+    const BuiltinParams two[2] = {*Params(r), *Params(a)};
+    // the ARG_MAX's node becomes the fused one: x exists where it runs
+    SetNodeIO(a, {x, size, axis_t}, Ints(a.node.outputs));
+    SetBuiltinBlob(a, two, sizeof(two));
+    a.registration = ResizeArgmaxRegistration();
+    a.name = "RESIZE_BILINEAR+ARG_MAX";
+    EraseNode(i);
+    return true;
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size();) {
+    if (fuse(i)) ++removed;   // node i is erased and its successor moved up
+    else ++i;
   }
   allocated_ = false;
   return removed;

@@ -253,6 +253,18 @@ class Graph {
   // merge's sign first. Bit-identical. Returns the number of nodes removed.
   int FuseUpsampleMerges();
 
+  // A segmentation head that ends in a per-pixel label
+  //   RESIZE_BILINEAR(x) -> ARG_MAX(v, axis = the channel axis)
+  // becomes one node "RESIZE_BILINEAR+ARG_MAX" (lce_b200_f32_resize_bilinear_argmax), which computes
+  // each output pixel's resized values from two source rows staged on chip and stores only their
+  // label, so the resized map v is never written: inputs [x, size, axis], outputs [labels], builtin_data
+  // { the resize's, the ARG_MAX's BuiltinParams }. Only when v is float32 and 4-D, has one consumer,
+  // the ARG_MAX, which reads it as input 0, and is not a graph output; the axis is a constant that
+  // normalises to 3; and x's rows (in_w * C floats) fit lce_b200_resize_bilinear_argmax_max_row_floats().
+  // Otherwise the graph is left as it is. No other pass matches either op, so the pass may run
+  // anywhere; fuse_all runs it after FuseUpsampleMerges. Bit-identical. Returns the nodes removed.
+  int FuseResizeArgmax();
+
   // init (first time) + prepare of every node in order, then arena allocation.
   TfLiteStatus AllocateTensors();
   TfLiteStatus ResizeInputTensor(int tensor, const std::vector<int>& dims);

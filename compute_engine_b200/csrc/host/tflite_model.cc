@@ -325,6 +325,9 @@ bool BuildGraphFromTflite(const uint8_t* data, size_t size, const OpResolver& re
         bp.align_corners = o.scalar<int8_t>(0, 0);
         bp.half_pixel_centers = o.scalar<int8_t>(1, 0);
         break;
+      case 56:  // ARG_MAX: ArgMaxOptions
+        bp.output_type = o.scalar<int8_t>(0, 0);
+        break;
       default:
         break;
     }

@@ -1355,6 +1355,127 @@ __global__ void __launch_bounds__(256) upsample_add_sign_kernel(const float* __r
   }
 }
 
+// ARG_MAX (reference/arg_min_max.h, ArgMinMax with std::greater) over x [outer, n, inner]: for each
+// (outer, inner) position v = x[0], idx = 0, then x[i] is taken only when x[i] > v. So ties go to the
+// lowest index (-0.0 == +0.0), a NaN at index 0 gives 0 and a NaN elsewhere is never taken. Split
+// across lanes, the same result is 0 when x[0] is NaN and otherwise the max of the non-NaN values by
+// (value, lowest index): an associative and commutative merge.
+struct ArgBest {
+  float v;
+  int i;   // -1: no non-NaN value seen yet
+};
+// x[i], with i increasing from one call to the next
+__device__ __forceinline__ void argbest_take(ArgBest& a, float v, int i) {
+  if (!isnan(v) && (a.i < 0 || v > a.v)) {
+    a.v = v;
+    a.i = i;
+  }
+}
+__device__ __forceinline__ ArgBest argbest_merge(ArgBest a, ArgBest b) {
+  if (b.i < 0) return a;
+  return a.i < 0 || b.v > a.v || (b.v == a.v && b.i < a.i) ? b : a;
+}
+
+// One thread per (outer, inner) position, walking the axis as the reference does: adjacent threads
+// read adjacent inner positions, so the loads coalesce when inner > 1; at inner == 1 (short rows)
+// each thread reads its own row.
+template <typename OutT>
+__global__ void __launch_bounds__(256) argmax_kernel(const float* __restrict__ in, long long outer, int n,
+                                                     long long inner, OutT* __restrict__ out) {
+  const long long total = outer * inner;
+  for (long long p = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; p < total;
+       p += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long o = p / inner;
+    const float* x = in + o * n * inner + (p - o * inner);
+    float v = __ldg(x);
+    int idx = 0;
+    for (int i = 1; i < n; ++i) {
+      const float xi = __ldg(x + i * inner);
+      if (xi > v) {
+        v = xi;
+        idx = i;
+      }
+    }
+    out[p] = static_cast<OutT>(idx);
+  }
+}
+
+// One warp per row at inner == 1 (long rows): lane l takes elements l, l + 32, ... in order, then the
+// lanes merge their (value, index) pairs.
+template <typename OutT>
+__global__ void __launch_bounds__(256) argmax_warp_kernel(const float* __restrict__ in, long long rows, int n,
+                                                          OutT* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
+  for (long long r = blockIdx.x * static_cast<long long>(blockDim.x >> 5) + (threadIdx.x >> 5); r < rows;
+       r += warps) {
+    const float* x = in + r * n;
+    ArgBest b{0.0f, -1};
+    for (int i = lane; i < n; i += 32) argbest_take(b, __ldg(x + i), i);
+#pragma unroll
+    for (int off = 16; off; off >>= 1) {
+      const ArgBest o{__shfl_xor_sync(0xffffffffu, b.v, off), __shfl_xor_sync(0xffffffffu, b.i, off)};
+      b = argbest_merge(b, o);
+    }
+    if (lane == 0) out[r] = static_cast<OutT>(isnan(__ldg(x)) ? 0 : b.i);
+  }
+}
+
+// RESIZE_BILINEAR -> ARG_MAX over the channel axis in one pass, by output rows as
+// resize_bilinear_kernel: blockIdx.y strides over the B * OH output rows. The CTA stages the row's two
+// source rows y0 and y1 (in_w * C floats each, as float4s when both are 16-byte aligned) in shared
+// memory; then each thread takes one output pixel, computes its C values with bilinear_src and
+// bilinear_mix exactly as the resize kernel does and keeps ARG_MAX's running index over them. Only the
+// label is stored; the resized map is never written.
+template <typename OutT>
+__global__ void __launch_bounds__(256) bilinear_argmax_kernel(const float* __restrict__ in, ResizeGeom g,
+                                                              OutT* __restrict__ out) {
+  extern __shared__ float4 stage4[];
+  const int src_len = g.x.in * g.C;
+  float* s0 = reinterpret_cast<float*>(stage4);
+  float* s1 = s0 + src_len;
+  for (long long row = blockIdx.y; row < static_cast<long long>(g.y.out) * g.batch; row += gridDim.y) {
+    const long long b = row / g.y.out;
+    int y0, y1;
+    const float vy = bilinear_src(static_cast<int>(row - b * g.y.out), g.y, g.half_pixel_centers, &y0, &y1);
+    const float dy = __fsub_rn(vy, static_cast<float>(y0));
+    const float* src0 = in + (b * g.y.in + y0) * src_len;
+    const float* src1 = in + (b * g.y.in + y1) * src_len;
+    __syncthreads();   // every thread is done with the previous row's stage
+    if (src_len % 4 == 0 && !((reinterpret_cast<uintptr_t>(src0) | reinterpret_cast<uintptr_t>(src1)) & 15)) {
+      for (int j = threadIdx.x; j < src_len / 4; j += blockDim.x) {
+        reinterpret_cast<float4*>(s0)[j] = __ldg(reinterpret_cast<const float4*>(src0) + j);
+        reinterpret_cast<float4*>(s1)[j] = __ldg(reinterpret_cast<const float4*>(src1) + j);
+      }
+    } else {
+      for (int j = threadIdx.x; j < src_len; j += blockDim.x) {
+        s0[j] = __ldg(src0 + j);
+        s1[j] = __ldg(src1 + j);
+      }
+    }
+    __syncthreads();
+    for (int ox = threadIdx.x; ox < g.x.out; ox += blockDim.x) {
+      int x0, x1;
+      const float vx = bilinear_src(ox, g.x, g.half_pixel_centers, &x0, &x1);
+      const float dx = __fsub_rn(vx, static_cast<float>(x0));
+      const float* p00 = s0 + x0 * g.C;
+      const float* p10 = s1 + x0 * g.C;
+      const float* p01 = s0 + x1 * g.C;
+      const float* p11 = s1 + x1 * g.C;
+      float v = bilinear_mix(p00[0], p10[0], p01[0], p11[0], dy, dx);
+      int idx = 0;
+      for (int c = 1; c < g.C; ++c) {
+        const float vc = bilinear_mix(p00[c], p10[c], p01[c], p11[c], dy, dx);
+        if (vc > v) {
+          v = vc;
+          idx = c;
+        }
+      }
+      out[row * g.x.out + ox] = static_cast<OutT>(idx);
+    }
+  }
+}
+
 // LOGISTIC, TFLite's float reference (reference/logistic.h) with CUDA's expf
 __global__ void __launch_bounds__(256) logistic_kernel(const float* __restrict__ in,
                                                        float* __restrict__ out, long long n) {
@@ -2699,6 +2820,57 @@ int lce_b200_f32_upsample_add_sign(const float* u, int batch, int in_h, int in_w
   const dim3 grid = row_grid(static_cast<long long>(batch) * out_h, static_cast<long long>(out_w) * cw, 8);
   upsample_add_sign_kernel<<<grid, 256, 0, as_stream(stream)>>>(u, skip, g, cw, activation, out, packed);
   return launch_check("upsample_add_sign_kernel");
+}
+
+// Rows of at least this many elements (at inner == 1) take a warp each; shorter rows a thread each.
+constexpr int kArgmaxWarpRow = 64;
+
+int lce_b200_f32_argmax(const float* in, int64_t outer, int n, int64_t inner, int out_int64, void* out,
+                        void* stream) {
+  if (outer < 0 || inner < 0 || n <= 0)
+    return fail("argmax: bad shape (%lld x %d x %lld)", static_cast<long long>(outer), n,
+                static_cast<long long>(inner));
+  if (outer == 0 || inner == 0) return 0;
+  if (!in || !out) return fail("argmax: null tensor");
+  cudaStream_t s = as_stream(stream);
+  if (inner == 1 && n >= kArgmaxWarpRow) {
+    const int grid = grid_for(outer, 8);
+    if (out_int64) argmax_warp_kernel<int64_t><<<grid, 256, 0, s>>>(in, outer, n, static_cast<int64_t*>(out));
+    else argmax_warp_kernel<int32_t><<<grid, 256, 0, s>>>(in, outer, n, static_cast<int32_t*>(out));
+    return launch_check("argmax_warp_kernel");
+  }
+  const int grid = grid_for(outer * inner, 256);
+  if (out_int64) argmax_kernel<int64_t><<<grid, 256, 0, s>>>(in, outer, n, inner, static_cast<int64_t*>(out));
+  else argmax_kernel<int32_t><<<grid, 256, 0, s>>>(in, outer, n, inner, static_cast<int32_t*>(out));
+  return launch_check("argmax_kernel");
+}
+
+// The two staged source rows of bilinear_argmax_kernel fit the default 48 KB of dynamic shared memory.
+constexpr int kBilinearArgmaxMaxRowFloats = 48 * 1024 / 2 / static_cast<int>(sizeof(float));
+
+int lce_b200_resize_bilinear_argmax_max_row_floats(void) { return kBilinearArgmaxMaxRowFloats; }
+
+int lce_b200_f32_resize_bilinear_argmax(const float* in, int batch, int in_h, int in_w, int channels, int out_h,
+                                        int out_w, int align_corners, int half_pixel_centers, int out_int64,
+                                        void* out, void* stream) {
+  ResizeGeom g;
+  if (resize_geom("resize_bilinear_argmax", batch, in_h, in_w, channels, out_h, out_w, align_corners,
+                  half_pixel_centers, &g))
+    return 1;
+  if (align_corners && half_pixel_centers)
+    return fail("resize_bilinear_argmax: align_corners and half_pixel_centers cannot both be set");
+  if (static_cast<long long>(in_w) * channels > kBilinearArgmaxMaxRowFloats)
+    return fail("resize_bilinear_argmax: a source row of %d x %d floats does not fit shared memory (at most %d)",
+                in_w, channels, kBilinearArgmaxMaxRowFloats);
+  if (batch == 0) return 0;
+  if (!in || !out) return fail("resize_bilinear_argmax: null tensor");
+  const dim3 grid = row_grid(static_cast<long long>(batch) * out_h, 1, 1);
+  const int threads = std::min(256, (out_w + 31) / 32 * 32);
+  const size_t smem = 2 * static_cast<size_t>(in_w) * channels * sizeof(float);
+  cudaStream_t s = as_stream(stream);
+  if (out_int64) bilinear_argmax_kernel<int64_t><<<grid, threads, smem, s>>>(in, g, static_cast<int64_t*>(out));
+  else bilinear_argmax_kernel<int32_t><<<grid, threads, smem, s>>>(in, g, static_cast<int32_t*>(out));
+  return launch_check("bilinear_argmax_kernel");
 }
 
 int lce_b200_f32_mean_hw_act(const float* in, float* out, int batch, int h, int w, int c, int pre_activation,

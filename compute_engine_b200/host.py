@@ -258,6 +258,11 @@ class HostGraph:
         fuse_activation_chains and allocate_tensors."""
         return lib().lce_host_fuse_upsample_merges(self._g)
 
+    def fuse_resize_argmax(self):
+        """RESIZE_BILINEAR -> ARG_MAX over the channel axis (a segmentation head's labels) => one
+        node that never writes the resized map. Call before allocate_tensors."""
+        return lib().lce_host_fuse_resize_argmax(self._g)
+
     def fuse_residual_pairs(self):
         """Two consecutive LceBconv2d+ADD[+LceQuantize] blocks whose intermediate nothing else
         reads => one node that keeps it on chip. Call after the other fusions."""
@@ -266,7 +271,7 @@ class HostGraph:
     def fuse_all(self):
         return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_residual_blocks()
                 + self.fuse_spatial_scales()
-                + self.fuse_float_glue() + self.fuse_upsample_merges()
+                + self.fuse_float_glue() + self.fuse_upsample_merges() + self.fuse_resize_argmax()
                 + self.fuse_grouped_conv_affine() + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
                 + self.fuse_residual_pairs())
 

@@ -254,7 +254,7 @@ def _quicknet_encoder(g, batch, image, input_type, blocks, filters):
     return sections
 
 
-def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, decoder_blocks=2):
+def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, decoder_blocks=2, labels=None):
     """A binary segmentation network: QuickNet's encoder, then a decoder of three stages that merge
     the coarse map with the encoder's skip maps as TF2's UpSampling2D and Keras' Add emit them, then a
     per-pixel classifier at full resolution. Each stage, for (coarse, skip) = (s4, s3), (d3, s2),
@@ -262,10 +262,14 @@ def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, d
     RESIZE_NEAREST_NEIGHBOR x2 (half_pixel_centers) -> ADD(skip) -> `decoder_blocks` residual blocks
     [LceQuantize -> LceBconv2d 3x3 (one-padding, ReLU, BatchNorm folded) -> ADD shortcut]. Head:
     CONV_2D 1x1 64 -> classes with bias -> RESIZE_BILINEAR to (image, image) (half_pixel_centers), the
-    logits [B, image, image, classes]. image must be a multiple of 32 (the encoder halves it five
-    times and the decoder doubles it back)."""
+    logits [B, image, image, classes]. With labels="int64" or "int32" the head ends in ARG_MAX over
+    the channel axis (the axis a constant int32 -1), as tf.argmax(logits, axis=-1) converts, and the
+    output is the label map [B, image, image] of that type. image must be a multiple of 32 (the
+    encoder halves it five times and the decoder doubles it back)."""
     if image % 32:
         raise ValueError(f"quicknet_seg needs an image size that is a multiple of 32, not {image}")
+    if labels not in (None, "int32", "int64"):
+        raise ValueError(f"quicknet_seg labels must be None, 'int32' or 'int64', not {labels!r}")
     g = _Builder(seed, batch, "QuickNetSeg")
     sections = _quicknet_encoder(g, batch, image, input_type, (4, 4, 4, 4), (64, 128, 256, 512))
     x, xs = sections[-1]
@@ -290,6 +294,10 @@ def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, d
                stride=(1, 1), activation="NONE")
     out = g.act((b, image, image, classes))
     g.m.add_op("RESIZE_BILINEAR", [logits, size(image, image)], [out], half_pixel_centers=True)
+    if labels is not None:
+        logits, out = out, g.act((b, image, image), np.dtype(labels))
+        g.m.add_op("ARG_MAX", [logits, g.const(np.array(-1, np.int32), np.int32, "axis")], [out],
+                   output_type=np.dtype(labels))
     g.m.outputs = [out]
     return g.m.serialize()
 

@@ -335,6 +335,24 @@ int lce_b200_f32_resize_bilinear(const float* in_dev, int batch, int in_h, int i
 int lce_b200_f32_upsample_add_sign(const float* u_dev, int batch, int in_h, int in_w, int channels, int out_h,
                                    int out_w, int align_corners, int half_pixel_centers, const float* skip_dev,
                                    int activation, float* out_dev, int32_t* packed_out_dev, void* stream);
+/* TFLite's float ARG_MAX (TF/lite/kernels/internal/reference/arg_min_max.h with std::greater) of a float
+ * tensor viewed as [outer, n, inner], reduced over n (n >= 1): out[o][i] = the reference's sequential
+ * result, v = x[o][0][i], idx = 0, and for k = 1 .. n-1 take x[o][k][i] only when x[o][k][i] > v. Ties go
+ * to the lowest index (-0.0 equals +0.0), a NaN at index 0 gives 0, a NaN elsewhere is never chosen.
+ * out_dev is int64 [outer, inner] when out_int64 is set, else int32; every element is written. */
+int lce_b200_f32_argmax(const float* in_dev, int64_t outer, int n, int64_t inner, int out_int64, void* out_dev,
+                        void* stream);
+/* The largest in_w * channels lce_b200_f32_resize_bilinear_argmax takes: it stages two source rows of
+ * that many floats in shared memory. */
+int lce_b200_resize_bilinear_argmax_max_row_floats(void);
+/* lce_b200_f32_resize_bilinear followed by lce_b200_f32_argmax over the channel axis, in one pass that
+ * never writes the resized map: out [batch, out_h, out_w] (int64 when out_int64 is set, else int32)
+ * is the index ARG_MAX picks from each output pixel's channels, each value computed as
+ * lce_b200_f32_resize_bilinear computes it, so the labels equal the two ops' bit for bit. Refuses
+ * in_w * channels above lce_b200_resize_bilinear_argmax_max_row_floats(). */
+int lce_b200_f32_resize_bilinear_argmax(const float* in_dev, int batch, int in_h, int in_w, int channels,
+                                        int out_h, int out_w, int align_corners, int half_pixel_centers,
+                                        int out_int64, void* out_dev, void* stream);
 /* TFLite_Detection_PostProcess (TF/lite/kernels/detection_postprocess.cc) with its float32 inputs,
  * applied to every image of a batch as TFLite applies it to its single image. */
 typedef struct {
