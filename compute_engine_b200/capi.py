@@ -109,6 +109,7 @@ EXPORTS = [
     "lce_b200_f32_shift_sign_planes",
     "lce_b200_f32_resize_nearest", "lce_b200_f32_resize_bilinear", "lce_b200_f32_upsample_add_sign",
     "lce_b200_f32_argmax", "lce_b200_resize_bilinear_argmax_max_row_floats", "lce_b200_f32_resize_bilinear_argmax",
+    "lce_b200_f32_depth_to_space", "lce_b200_subpixel_conv_max_out_channels", "lce_b200_f32_subpixel_conv",
     "lce_b200_detection_max_anchors", "lce_b200_detection_workspace_bytes", "lce_b200_f32_detection_postprocess",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
@@ -530,6 +531,46 @@ def grouped_conv2d(x: torch.Tensor, filt: torch.Tensor, bias=None, stride=(1, 1)
     _check(lib().lce_b200_f32_grouped_conv2d(C.byref(d), C.c_int(cin // fin), _p(x), _p(filt), _p(vecs[0]),
                                              _p(vecs[1]), _p(vecs[2]), C.c_int(post_activation), _p(out),
                                              _stream()))
+    return out
+
+
+def depth_to_space(x: torch.Tensor, block_size: int):
+    """DEPTH_TO_SPACE of a float NHWC map [B, H, W, C] to [B, H * r, W * r, C / r^2]: the values
+    moved as TFLite's reference moves them."""
+    x = _dev(x, torch.float32)
+    b, h, w, c = x.shape
+    r = int(block_size)
+    if r <= 0 or c % (r * r):
+        raise LceError(f"depth_to_space: {c} channels are not a multiple of block_size^2 (block size {r})")
+    out = torch.empty((b, h * r, w * r, c // (r * r)), dtype=torch.float32, device=x.device)
+    _check(lib().lce_b200_f32_depth_to_space(_p(x), b, h, w, c, r, _p(out), _stream()))
+    return out
+
+
+def subpixel_conv_max_out_channels():
+    return int(lib().lce_b200_subpixel_conv_max_out_channels())
+
+
+def subpixel_conv(x: torch.Tensor, filt: torch.Tensor, bias, block_size: int, img=None, align_corners=False,
+                  half_pixel_centers=False, activation=ACT_NONE, add_activation=ACT_NONE):
+    """A super-resolution tail in one pass: CONV_2D(x, filt [C_out, kh, kw, C_in], bias, stride 1, SAME,
+    activation) -> DEPTH_TO_SPACE(block_size) [-> ADD(RESIZE_BILINEAR(img) to the output's size, with
+    add_activation)], [B, H * r, W * r, C_out / r^2]; bit for bit the ops one by one."""
+    x = _dev(x, torch.float32)
+    filt = _dev(filt, torch.float32)
+    bias = None if bias is None else _dev(bias, torch.float32)
+    img = None if img is None else _dev(img, torch.float32)
+    b, h, w, cin = x.shape
+    cout, kh, kw, _ = filt.shape
+    r = int(block_size)
+    if r <= 0 or cout % (r * r):
+        raise LceError(f"subpixel_conv: {cout} output channels are not a multiple of block_size^2 (block size {r})")
+    d = ConvDesc(b, h, w, cin, kh, kw, cout, 1, 1, 1, 1, PADDING_SAME, activation)
+    out = torch.empty((b, h * r, w * r, cout // (r * r)), dtype=torch.float32, device=x.device)
+    ih, iw = (img.shape[1], img.shape[2]) if img is not None else (0, 0)
+    _check(lib().lce_b200_f32_subpixel_conv(C.byref(d), _p(x), _p(filt), _p(bias), r, _p(img), ih, iw,
+                                            int(bool(align_corners)), int(bool(half_pixel_centers)),
+                                            int(add_activation), _p(out), _stream()))
     return out
 
 

@@ -999,6 +999,98 @@ TfLiteStatus ResizeArgmaxInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// ------------------------------ DEPTH_TO_SPACE ------------------------------ //
+// inputs [x (float32 [B, H, W, C])], output [B, H * r, W * r, C / r^2] (TF/lite/kernels/depth_to_space.cc:
+// rank 4, block_size > 0, C % r^2 == 0, input and output of one type; float32 only here).
+const char* DepthToSpaceChecks(const TfLiteTensor* x, const TfLiteTensor* o, int r) {
+  if (!x || x->dims->size != 4) return "DEPTH_TO_SPACE: the input must be a 4-D tensor";
+  if (x->type != kTfLiteFloat32) return "DEPTH_TO_SPACE: only float32 is supported";
+  if (!o || o->type != x->type) return "DEPTH_TO_SPACE: the output's type differs from the input's";
+  if (r <= 0) return "DEPTH_TO_SPACE: block_size must be positive";
+  if (x->dims->data[3] % (static_cast<int64_t>(r) * r))
+    return "DEPTH_TO_SPACE: the input's channels must be a multiple of block_size^2";
+  return nullptr;
+}
+TfLiteStatus DepthToSpacePrepare(TfLiteContext* c, TfLiteNode* n) {
+  B_ENSURE(c, n->inputs->size == 1 && n->outputs->size == 1, "DEPTH_TO_SPACE: one input and one output expected");
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const int r = P(n).block_size;
+  const char* why = DepthToSpaceChecks(x, T(c, n->outputs, 0), r);
+  B_ENSURE(c, why == nullptr, why);
+  const int* d = x->dims->data;
+  B_ENSURE(c, static_cast<int64_t>(d[1]) * r <= INT32_MAX && static_cast<int64_t>(d[2]) * r <= INT32_MAX,
+           "DEPTH_TO_SPACE: the output is too large");
+  return Resize(c, T(c, n->outputs, 0), {d[0], d[1] * r, d[2] * r, d[3] / (r * r)});
+}
+TfLiteStatus DepthToSpaceInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const int* d = x->dims->data;
+  B_CAPI(c, lce_b200_f32_depth_to_space(x->data.f, d[0], d[1], d[2], d[3], P(n).block_size,
+                                        T(c, n->outputs, 0)->data.f, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// ----- fused CONV_2D -> DEPTH_TO_SPACE [-> ADD(RESIZE_BILINEAR(img))]: a super-resolution tail ----- //
+// Created by Graph::FuseSubpixelConvs; builtin_data = { BuiltinParams conv, depth_to_space, resize, add }
+// (the last two zero without the residual); inputs [x, filter, bias (-1 when absent)] or [x, filter,
+// bias, img, size], outputs [y [B, H * r, W * r, C']]. Runs lce_b200_f32_subpixel_conv.
+struct SubpixelParams {
+  BuiltinParams conv, d2s, resize, add;
+};
+void* SubpixelInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* p = new SubpixelParams();
+  memset(p, 0, sizeof(*p));
+  if (buffer && length >= sizeof(SubpixelParams)) memcpy(p, buffer, sizeof(SubpixelParams));
+  return p;
+}
+void SubpixelFree(TfLiteContext*, void* p) { delete static_cast<SubpixelParams*>(p); }
+TfLiteStatus SubpixelPrepare(TfLiteContext* c, TfLiteNode* n) {
+  const auto& sp = *static_cast<const SubpixelParams*>(n->user_data);
+  B_ENSURE(c, (n->inputs->size == 3 || n->inputs->size == 5) && n->outputs->size == 1,
+           "CONV_2D+DEPTH_TO_SPACE: inputs [x, filter, bias] or [x, filter, bias, img, size] and one output expected");
+  lce_f32_conv_desc d;
+  int groups = 1;
+  B_ENSURE(c, ConvDesc(c, n, false, &d, &groups) && groups == 1,
+           "CONV_2D+DEPTH_TO_SPACE: bad input / filter shapes");
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  B_ENSURE(c, x->type == kTfLiteFloat32, "CONV_2D+DEPTH_TO_SPACE: only float32 is supported");
+  B_ENSURE(c, d.stride_h == 1 && d.stride_w == 1 && d.dilation_h == 1 && d.dilation_w == 1 &&
+                  d.padding == LCE_PADDING_SAME,
+           "CONV_2D+DEPTH_TO_SPACE: the convolution must have stride 1, dilation 1 and SAME padding");
+  const int r = sp.d2s.block_size;
+  B_ENSURE(c, r > 0 && d.out_c % (r * r) == 0,
+           "CONV_2D+DEPTH_TO_SPACE: the conv's channels must be a multiple of block_size^2");
+  B_ENSURE(c, d.out_c <= lce_b200_subpixel_conv_max_out_channels(),
+           "CONV_2D+DEPTH_TO_SPACE: the conv has too many output channels");
+  const int cp = d.out_c / (r * r);
+  if (n->inputs->size == 5) {
+    const TfLiteTensor* img = T(c, n->inputs, 3);
+    const TfLiteTensor* size = T(c, n->inputs, 4);
+    B_ENSURE(c, img && img->type == kTfLiteFloat32 && img->dims->size == 4 && img->dims->data[0] == d.batch &&
+                    img->dims->data[3] == cp,
+             "CONV_2D+DEPTH_TO_SPACE+RESIZE_BILINEAR+ADD: img must be float32 [B, h, w, C']");
+    B_ENSURE(c, size && size->allocation_type == kTfLiteMmapRo && HostInts(size) && Count(size) == 2 &&
+                    size->data.i32[0] == d.in_h * r && size->data.i32[1] == d.in_w * r,
+             "CONV_2D+DEPTH_TO_SPACE+RESIZE_BILINEAR+ADD: the size must be the constant output size");
+    B_ENSURE(c, !(sp.resize.align_corners && sp.resize.half_pixel_centers),
+             "RESIZE_BILINEAR: align_corners and half_pixel_centers cannot both be set");
+  }
+  return Resize(c, T(c, n->outputs, 0), {d.batch, d.in_h * r, d.in_w * r, cp});
+}
+TfLiteStatus SubpixelInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const auto& sp = *static_cast<const SubpixelParams*>(n->user_data);
+  lce_f32_conv_desc d;
+  ConvDesc(c, n, false, &d);
+  const TfLiteTensor* bias = T(c, n->inputs, 2);
+  const TfLiteTensor* img = n->inputs->size == 5 ? T(c, n->inputs, 3) : nullptr;
+  B_CAPI(c, lce_b200_f32_subpixel_conv(&d, T(c, n->inputs, 0)->data.f, T(c, n->inputs, 1)->data.f,
+                                       bias ? bias->data.f : nullptr, sp.d2s.block_size, img ? img->data.f : nullptr,
+                                       img ? img->dims->data[1] : 0, img ? img->dims->data[2] : 0,
+                                       sp.resize.align_corners, sp.resize.half_pixel_centers, sp.add.activation,
+                                       T(c, n->outputs, 0)->data.f, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // ------------------------------ CONCATENATION ------------------------------ //
 // Strided device copies (one cudaMemcpy2DAsync per input): no kernel of ours.
 TfLiteStatus ConcatPrepare(TfLiteContext* c, TfLiteNode* n) {
@@ -1341,6 +1433,10 @@ const TfLiteRegistration* ResizeArgmaxRegistration() {
   static TfLiteRegistration r = {ResizeArgmaxInit, ResizeArgmaxFree, ResizeArgmaxPrepare, ResizeArgmaxInvoke};
   return &r;
 }
+const TfLiteRegistration* SubpixelConvRegistration() {
+  static TfLiteRegistration r = {SubpixelInit, SubpixelFree, SubpixelPrepare, SubpixelInvoke};
+  return &r;
+}
 const TfLiteRegistration* UpsampleMergeRegistration() {
   static TfLiteRegistration r = {MergeInit, MergeFree, MergePrepare, MergeInvoke};
   return &r;
@@ -1399,6 +1495,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(97, &resize_nearest);   // RESIZE_NEAREST_NEIGHBOR
   static TfLiteRegistration arg_max = {Init, Free, ArgMaxPrepare, ArgMaxInvoke};
   r->AddBuiltin(56, &arg_max);   // ARG_MAX
+  static TfLiteRegistration depth_to_space = {Init, Free, DepthToSpacePrepare, DepthToSpaceInvoke};
+  r->AddBuiltin(5, &depth_to_space);   // DEPTH_TO_SPACE
   static TfLiteRegistration detection = {DetectionInit, DetectionFree, DetectionPrepare, DetectionInvoke};
   r->AddCustom("TFLite_Detection_PostProcess", &detection);
 }

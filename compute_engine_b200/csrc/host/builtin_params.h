@@ -26,6 +26,8 @@ struct BuiltinParams {
   int32_t align_corners, half_pixel_centers;
   // ARG_MAX (ArgMaxOptions): the output's TensorType code
   int32_t output_type;
+  // DEPTH_TO_SPACE (DepthToSpaceOptions)
+  int32_t block_size;
 };
 
 // ARG_MAX's axis: a constant int32 or int64 tensor of one element (0-D or [1]) in host memory, within

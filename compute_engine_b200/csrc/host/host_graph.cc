@@ -314,6 +314,7 @@ constexpr const char* kMaxPool2d = "builtin:17";
 constexpr const char* kResizeNearest = "builtin:97";
 constexpr const char* kResizeBilinear = "builtin:23";
 constexpr const char* kArgMax = "builtin:56";
+constexpr const char* kDepthToSpace = "builtin:5";
 constexpr const char* kMul = "builtin:18";
 constexpr const char* kRelu = "builtin:19";
 constexpr const char* kMean = "builtin:40";
@@ -1784,6 +1785,108 @@ int Graph::FuseResizeArgmax() {
   for (size_t i = 0; i < nodes_.size();) {
     if (fuse(i)) ++removed;   // node i is erased and its successor moved up
     else ++i;
+  }
+  allocated_ = false;
+  return removed;
+}
+
+const TfLiteRegistration* SubpixelConvRegistration();   // builtin_ops.cc
+extern "C" int lce_b200_internal_conv_runs_igemm(int in_h, int in_w, int in_c, int filter_h, int filter_w,
+                                                 int stride_h, int stride_w, int dilation_h, int dilation_w,
+                                                 int out_c);   // lce_b200_builtins.cu
+
+int Graph::FuseSubpixelConvs() {
+  if (!device_arena_) return 0;
+  auto is_const = [&](int t, TfLiteType type) {
+    return t >= 0 && tensors_[t].type == type && tensors_[t].allocation_type == kTfLiteMmapRo;
+  };
+  auto Elements = [&](int t) {
+    int64_t n = 1;
+    for (int k = 0; tensors_[t].dims && k < tensors_[t].dims->size; ++k) n *= tensors_[t].dims->data[k];
+    return n;
+  };
+  auto fuse = [&](size_t i) -> int {   // nodes removed by fusing the conv at i, 0 when it stays
+    NodeRecord& cv = *nodes_[i];
+    const BuiltinParams* cp = Params(cv);
+    if (cv.name != kConv2d || cv.initialized || cv.node.inputs->size < 2 || cv.node.inputs->size > 3 ||
+        cv.node.outputs->size != 1 || !cp)
+      return 0;
+    const int x = cv.node.inputs->data[0], f = cv.node.inputs->data[1], y = cv.node.outputs->data[0];
+    const int bias = cv.node.inputs->size == 3 ? cv.node.inputs->data[2] : -1;
+    if (x < 0 || tensors_[x].type != kTfLiteFloat32 || tensors_[y].type != kTfLiteFloat32) return 0;
+    const TfLiteIntArray* xd = tensors_[x].dims;
+    const TfLiteIntArray* fd = is_const(f, kTfLiteFloat32) ? tensors_[f].dims : nullptr;
+    if (!xd || xd->size != 4 || !fd || fd->size != 4 || fd->data[1] != 3 || fd->data[2] != 3 ||
+        fd->data[3] != xd->data[3])
+      return 0;
+    const int cin = xd->data[3], cout = fd->data[0];
+    if (bias >= 0 && (!is_const(bias, kTfLiteFloat32) || Elements(bias) != cout)) return 0;
+    if (cp->stride_h != 1 || cp->stride_w != 1 || cp->dilation_h != 1 || cp->dilation_w != 1 ||
+        cp->padding != LCE_PADDING_SAME || cin % 4 != 0 || cout > lce_b200_subpixel_conv_max_out_channels() ||
+        !lce_b200_internal_conv_runs_igemm(xd->data[1], xd->data[2], cin, 3, 3, 1, 1, 1, 1, cout))
+      return 0;
+    const size_t di = SoleReaderAsFirstInput(y);
+    if (di == kNoNode || di <= i) return 0;
+    NodeRecord& ds = *nodes_[di];
+    if (ds.name != kDepthToSpace || ds.initialized || ds.node.inputs->size != 1 || ds.node.outputs->size != 1 ||
+        !Params(ds))
+      return 0;
+    const int r = Params(ds)->block_size, s = ds.node.outputs->data[0];
+    if (r < 2 || cout % (r * r) != 0 || tensors_[s].type != kTfLiteFloat32) return 0;
+    BuiltinParams four[4] = {*cp, *Params(ds), {}, {}};
+    // the residual: s's one reader an ADD whose other operand is a RESIZE_BILINEAR output of s's shape
+    // that only the ADD reads, resized from a float32 4-D image by a constant size
+    size_t ai = SoleConsumer(s), ri = kNoNode;
+    int img = -1, size = -1;
+    if (ai != kNoNode && ai > di) {
+      NodeRecord& a = *nodes_[ai];
+      const int in0 = a.node.inputs->size == 2 ? a.node.inputs->data[0] : -1;
+      const int in1 = a.node.inputs->size == 2 ? a.node.inputs->data[1] : -1;
+      const int v = in0 == s ? in1 : in0;
+      if (a.name == kAdd && !a.initialized && a.node.outputs->size == 1 && Params(a) && in0 != in1 && v >= 0 &&
+          tensors_[a.node.outputs->data[0]].type == kTfLiteFloat32 && tensors_[v].type == kTfLiteFloat32 &&
+          SameDims(tensors_[v].dims, tensors_[s].dims) && tensors_[s].dims && tensors_[s].dims->size == 4 &&
+          SoleConsumer(v) == ai) {
+        for (size_t k = 0; k < ai && ri == kNoNode; ++k)
+          if (nodes_[k]->node.outputs->size == 1 && nodes_[k]->node.outputs->data[0] == v) ri = k;
+      }
+      if (ri != kNoNode) {
+        NodeRecord& rz = *nodes_[ri];
+        img = rz.node.inputs->size == 2 ? rz.node.inputs->data[0] : -1;
+        size = rz.node.inputs->size == 2 ? rz.node.inputs->data[1] : -1;
+        if (rz.name != kResizeBilinear || rz.initialized || !Params(rz) || img < 0 ||
+            tensors_[img].type != kTfLiteFloat32 || !tensors_[img].dims || tensors_[img].dims->size != 4 ||
+            !is_const(size, kTfLiteInt32) || Elements(size) != 2)
+          ri = kNoNode;
+      }
+    }
+    std::vector<int> ins{x, f, bias};
+    if (ri != kNoNode) {
+      NodeRecord& a = *nodes_[ai];
+      four[2] = *Params(*nodes_[ri]);
+      four[3] = *Params(a);
+      ins.push_back(img);
+      ins.push_back(size);
+      // the ADD's node becomes the fused one: x and img both exist where it runs
+      SetNodeIO(a, ins, Ints(a.node.outputs));
+      SetBuiltinBlob(a, four, sizeof(four));
+      a.registration = SubpixelConvRegistration();
+      a.name = "CONV_2D+DEPTH_TO_SPACE+RESIZE_BILINEAR+ADD";
+      EraseNodes({i, di, ri});
+      return 3;
+    }
+    SetNodeIO(ds, ins, {s});
+    SetBuiltinBlob(ds, four, sizeof(four));
+    ds.registration = SubpixelConvRegistration();
+    ds.name = "CONV_2D+DEPTH_TO_SPACE";
+    EraseNode(i);
+    return 1;
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size();) {
+    const int k = fuse(i);
+    removed += k;
+    if (k == 0) ++i;   // else node i is erased and its successor moved up
   }
   allocated_ = false;
   return removed;

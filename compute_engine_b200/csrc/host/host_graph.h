@@ -265,6 +265,26 @@ class Graph {
   // anywhere; fuse_all runs it after FuseUpsampleMerges. Bit-identical. Returns the nodes removed.
   int FuseResizeArgmax();
 
+  // A super-resolution network's sub-pixel tail
+  //   CONV_2D(x) -> DEPTH_TO_SPACE(y, r) [-> ADD(s, RESIZE_BILINEAR(img))]
+  // becomes one node (lce_b200_f32_subpixel_conv) that computes each low-resolution pixel's conv
+  // channels, stores them at their high-resolution addresses and adds the resized image there, so
+  // y, s and the resized image are never written: "CONV_2D+DEPTH_TO_SPACE+RESIZE_BILINEAR+ADD", inputs
+  // [x, filter, bias (-1 when absent), img, size], or without the ADD part "CONV_2D+DEPTH_TO_SPACE",
+  // inputs [x, filter, bias]; builtin_data { the conv's, the DEPTH_TO_SPACE's, the resize's, the ADD's
+  // BuiltinParams } (the last two zero without the ADD). Only when the conv is float32 and ungrouped,
+  // with a constant [Cout, 3, 3, Cin] filter and a constant bias or none, stride 1, dilation 1, SAME,
+  // Cin % 4 == 0, Cout <= lce_b200_subpixel_conv_max_out_channels(), and runs on the implicit-GEMM
+  // kernels unfused (lce_b200_internal_conv_runs_igemm, the predicate conv2d_impl dispatches by), whose
+  // chain the fused kernel repeats; y has one reader, the DEPTH_TO_SPACE, and is not a graph output;
+  // r >= 2. The ADD part joins only when s's one reader is an ADD (either operand), the other operand
+  // is a RESIZE_BILINEAR output of s's 4-D shape (no broadcast) read by the ADD alone, resized from a
+  // float32 4-D img by a constant size, and neither s nor the resized map is a graph output; otherwise
+  // the ADD and the resize stay as they are. Otherwise the graph is left as it is. No other pass
+  // matches a DEPTH_TO_SPACE, so the pass may run anywhere; fuse_all runs it after FuseResizeArgmax.
+  // Bit-identical. Returns the nodes removed.
+  int FuseSubpixelConvs();
+
   // init (first time) + prepare of every node in order, then arena allocation.
   TfLiteStatus AllocateTensors();
   TfLiteStatus ResizeInputTensor(int tensor, const std::vector<int>& dims);

@@ -328,6 +328,9 @@ bool BuildGraphFromTflite(const uint8_t* data, size_t size, const OpResolver& re
       case 56:  // ARG_MAX: ArgMaxOptions
         bp.output_type = o.scalar<int8_t>(0, 0);
         break;
+      case 5:  // DEPTH_TO_SPACE: DepthToSpaceOptions
+        bp.block_size = o.scalar<int32_t>(0, 0);
+        break;
       default:
         break;
     }

@@ -1476,6 +1476,210 @@ __global__ void __launch_bounds__(256) bilinear_argmax_kernel(const float* __res
   }
 }
 
+// DEPTH_TO_SPACE (reference/depth_to_space.h): out[b, y*r + i, x*r + j, c] = in[b, y, x, (i*r + j)*C' + c]
+// with C' = C / r^2. By output rows as the resize kernels: blockIdx.y strides over the B * H * r output
+// rows, and an output row (b, Y) is W runs of r * C' contiguous floats, run x read from LR pixel
+// (b, Y / r, x) at channel (Y % r) * r * C'. Consecutive threads store consecutive floats (VEC = 4 at a
+// time when a run is a whole number of float4s). Element offsets are 64-bit; an index within a row is
+// 32-bit (the host refuses rows within 2^22 floats of 2^31).
+template <int VEC>
+__global__ void __launch_bounds__(256) depth_to_space_kernel(const float* __restrict__ in, float* __restrict__ out,
+                                                             int H, int W, int C, int r, long long rows) {
+  const int run = C / r;   // r * C'
+  const int row_len = W * run;
+  for (long long row = blockIdx.y; row < rows; row += gridDim.y) {
+    const long long by = row / r;   // b * H + y
+    const int i = static_cast<int>(row - by * r);
+    const float* src = in + by * W * C + i * run;
+    float* dst = out + row * row_len;
+    for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * VEC; j < row_len; j += gridDim.x * blockDim.x * VEC) {
+      const int x = j / run, t = j - x * run;
+      const float* s = src + static_cast<long long>(x) * C + t;
+      if (VEC == 4) reinterpret_cast<float4*>(dst)[j >> 2] = __ldg(reinterpret_cast<const float4*>(s));
+      else dst[j] = __ldg(s);
+    }
+  }
+}
+
+// The sub-pixel tail of a super-resolution network,
+//   CONV_2D(x, KHxKW, stride 1, SAME) -> DEPTH_TO_SPACE(r) [-> ADD(RESIZE_BILINEAR(img))],
+// in one pass (Graph::FuseSubpixelConvs). A CTA computes BM low-resolution pixels x BN >= Cout conv
+// channels as conv_igemm8x8_kernel does: the input patches and filter rows staged KC k at a time, each
+// thread 8 pixels x TN channels, and every output the igemm kernels' own chain: acc = 0, fmaf in
+// k = (fy * KW + fx) * Cin + ci order with a padded tap as fmaf(0, w, acc), then zero terms up to a
+// multiple of kIK, then apply_act(acc + bias). The CTA's tile goes to shared memory, from where the
+// pixels' channels n = (i * r + j) * C' + c are stored at their high-resolution addresses
+// (b, y * r + i, x * r + j, c): each of the r passes writes runs of r * C' floats, consecutive threads
+// consecutive floats. With img, each value is first added to img's bilinear value at that pixel (the
+// resize kernel's bilinear_src / bilinear_mix, then the ADD builtin's add and activation). The conv
+// output, the shuffled map and the resized image are never written.
+struct SubpixelGeom {
+  int B, H, W, Cin, KH, KW, ph, pw, Cout, r, Cp;   // Cout = Cp * r * r
+  int act, add_act;
+  ResizeGeom img;   // img [B, ih, iw, Cp] to (H * r, W * r), when the residual is present
+};
+constexpr int kSpKC = 8;   // k per staged chunk; kIK (16) is a multiple, so the K padding is igemm's
+template <int NCOL, int TN>
+struct SubpixelTile {
+  static constexpr int kRowThreads = 128 / NCOL, BM = kRowThreads * 8, BN = NCOL * TN;
+  static constexpr int kStageFloats = 2 * kSpKC * (BM + 4) + 2 * kSpKC * (BN + 4);
+  static constexpr int kOutFloats = BM * (BN + 1);
+  static constexpr int kFloats = kStageFloats > kOutFloats ? kStageFloats : kOutFloats;
+};
+template <int NCOL, int TN>
+__global__ void __launch_bounds__(128) subpixel_conv_kernel(const float* __restrict__ in,
+                                                            const float* __restrict__ filter,
+                                                            const float* __restrict__ bias,
+                                                            const float* __restrict__ img,
+                                                            float* __restrict__ out, SubpixelGeom g,
+                                                            unsigned M) {
+  using Tile = SubpixelTile<NCOL, TN>;
+  constexpr int BM = Tile::BM, BN = Tile::BN, RPT = BM / 128, TQ = TN / 4;
+  extern __shared__ __align__(16) float sp_smem[];
+  float (*A_s)[kSpKC][BM + 4] = reinterpret_cast<float (*)[kSpKC][BM + 4]>(sp_smem);
+  float (*B_s)[kSpKC][BN + 4] = reinterpret_cast<float (*)[kSpKC][BN + 4]>(sp_smem + 2 * kSpKC * (BM + 4));
+  float* out_s = sp_smem;   // [BM][BN + 1], after the K loop
+  const int K = g.KH * g.KW * g.Cin;
+  const int Kpad = (K + kIK - 1) / kIK * kIK;
+  int* koff = reinterpret_cast<int*>(sp_smem + Tile::kFloats);
+  int* kdydx = koff + Kpad;
+  const int tid = threadIdx.x;
+  for (int k = tid; k < Kpad; k += 128) {
+    if (k < K) {
+      const int tap = k / g.Cin, ci = k - tap * g.Cin;
+      const int fy = tap / g.KW, fx = tap - fy * g.KW;
+      koff[k] = (fy * g.W + fx) * g.Cin + ci;
+      kdydx[k] = (fy << 16) | fx;
+    } else {
+      koff[k] = 0;
+      kdydx[k] = 0x7fff7fff;   // fails every bounds test
+    }
+  }
+  const unsigned m0 = blockIdx.x * static_cast<unsigned>(BM);
+  const unsigned hw = static_cast<unsigned>(g.H) * g.W;
+  int iy0[RPT], ix0[RPT];
+  bool row_ok[RPT];
+  const float* base[RPT];
+#pragma unroll
+  for (int q = 0; q < RPT; ++q) {
+    const unsigned m = m0 + tid + 128 * q;
+    row_ok[q] = m < M;
+    const unsigned mm = row_ok[q] ? m : 0u;
+    const unsigned b = mm / hw, rem = mm - b * hw;
+    const int y = static_cast<int>(rem / g.W), x = static_cast<int>(rem - (rem / g.W) * g.W);
+    iy0[q] = y - g.ph;
+    ix0[q] = x - g.pw;
+    base[q] = in + ((static_cast<long long>(b) * g.H + iy0[q]) * g.W + ix0[q]) * g.Cin;   // read only in bounds
+  }
+  __syncthreads();
+
+  float ra[RPT][kSpKC], rb[BN * kSpKC / 128];
+  auto fetch = [&](int k0) {
+#pragma unroll
+    for (int e = 0; e < kSpKC; ++e) {
+      const int d = kdydx[k0 + e], o = koff[k0 + e];
+#pragma unroll
+      for (int q = 0; q < RPT; ++q) {
+        const int iy = iy0[q] + (d >> 16), ix = ix0[q] + (d & 0xffff);
+        const bool ok = row_ok[q] && static_cast<unsigned>(iy) < static_cast<unsigned>(g.H) &&
+                        static_cast<unsigned>(ix) < static_cast<unsigned>(g.W);
+        ra[q][e] = ok ? __ldg(base[q] + o) : 0.0f;
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < BN * kSpKC / 128; ++e) {
+      const int idx = tid + 128 * e, n = idx / kSpKC, k = k0 + idx % kSpKC;
+      rb[e] = (n < g.Cout && k < K) ? __ldg(filter + static_cast<size_t>(n) * K + k) : 0.0f;
+    }
+  };
+  auto stash = [&](int buf) {
+#pragma unroll
+    for (int q = 0; q < RPT; ++q)
+#pragma unroll
+      for (int e = 0; e < kSpKC; ++e) A_s[buf][e][tid + 128 * q] = ra[q][e];
+#pragma unroll
+    for (int e = 0; e < BN * kSpKC / 128; ++e) {
+      const int idx = tid + 128 * e;
+      B_s[buf][idx % kSpKC][idx / kSpKC] = rb[e];
+    }
+  };
+  const int tx = tid % NCOL, ty = tid / NCOL;
+  float acc[8][TN];
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int j = 0; j < TN; ++j) acc[i][j] = 0.0f;
+  fetch(0);
+  stash(0);
+  __syncthreads();
+  const int nk = Kpad / kSpKC;
+  for (int it = 0; it < nk; ++it) {
+    const int buf = it & 1;
+    if (it + 1 < nk) fetch((it + 1) * kSpKC);
+#pragma unroll
+    for (int kk = 0; kk < kSpKC; ++kk) {
+      const float4 a0 = *reinterpret_cast<const float4*>(&A_s[buf][kk][ty * 4]);
+      const float4 a1 = *reinterpret_cast<const float4*>(&A_s[buf][kk][BM / 2 + ty * 4]);
+      const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+      float bv[TN];
+#pragma unroll
+      for (int q = 0; q < TQ; ++q) {
+        const float4 b = *reinterpret_cast<const float4*>(&B_s[buf][kk][q * (BN / TQ) + tx * 4]);
+        bv[4 * q] = b.x;
+        bv[4 * q + 1] = b.y;
+        bv[4 * q + 2] = b.z;
+        bv[4 * q + 3] = b.w;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+    }
+    if (it + 1 < nk) {
+      stash(buf ^ 1);
+      __syncthreads();
+    }
+  }
+  __syncthreads();   // out_s reuses the staging memory
+  constexpr int SP = BN + 1;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int row = i < 4 ? ty * 4 + i : BM / 2 + ty * 4 + (i - 4);
+#pragma unroll
+    for (int j = 0; j < TN; ++j) {
+      const int n = (j / 4) * (BN / TQ) + tx * 4 + (j & 3);
+      if (n < g.Cout) out_s[row * SP + n] = apply_act(acc[i][j] + (bias ? bias[n] : 0.0f), g.act);
+    }
+  }
+  __syncthreads();
+  const int rows = static_cast<int>(min(static_cast<unsigned>(BM), M - m0));
+  const int run = g.r * g.Cp;   // floats of one LR pixel in one HR row
+  const long long hr_row = static_cast<long long>(g.W) * run;
+  for (int i = 0; i < g.r; ++i) {
+    for (int e = tid; e < rows * run; e += 128) {
+      const int p = e / run, t = e - p * run;
+      const unsigned m = m0 + p;
+      const unsigned b = m / hw, rem = m - b * hw;
+      const int y = static_cast<int>(rem / g.W), x = static_cast<int>(rem - (rem / g.W) * g.W);
+      const int Y = y * g.r + i;
+      float v = out_s[p * SP + i * run + t];
+      if (img) {
+        const int jx = t / g.Cp, c = t - jx * g.Cp;
+        int y0, y1, x0, x1;
+        const float vy = bilinear_src(Y, g.img.y, g.img.half_pixel_centers, &y0, &y1);
+        const float vx = bilinear_src(x * g.r + jx, g.img.x, g.img.half_pixel_centers, &x0, &x1);
+        const float* src0 = img + (static_cast<long long>(b) * g.img.y.in + y0) * g.img.x.in * g.Cp + c;
+        const float* src1 = img + (static_cast<long long>(b) * g.img.y.in + y1) * g.img.x.in * g.Cp + c;
+        const float rv = bilinear_mix(__ldg(src0 + x0 * g.Cp), __ldg(src1 + x0 * g.Cp), __ldg(src0 + x1 * g.Cp),
+                                      __ldg(src1 + x1 * g.Cp), __fsub_rn(vy, static_cast<float>(y0)),
+                                      __fsub_rn(vx, static_cast<float>(x0)));
+        v = apply_act(v + rv, g.add_act);
+      }
+      out[(static_cast<long long>(b) * g.H * g.r + Y) * hr_row + static_cast<long long>(x) * run + t] = v;
+    }
+  }
+}
+
 // LOGISTIC, TFLite's float reference (reference/logistic.h) with CUDA's expf
 __global__ void __launch_bounds__(256) logistic_kernel(const float* __restrict__ in,
                                                        float* __restrict__ out, long long n) {
@@ -2127,6 +2331,63 @@ int lce_b200_internal_conv_packs_alike(int filter_h, int filter_w, int stride_h,
   return !(pw && out_c % 32 == 0 && out_c % 128 != 0);
 }
 
+// The direct kernel's K threshold; LCE_B200_DIRECT_MAXK overrides it for experiments.
+static int direct_max_k() {
+  static const int k = [] {
+    const char* e = getenv("LCE_B200_DIRECT_MAXK");
+    return e ? atoi(e) : kDirectMaxK;
+  }();
+  return k;
+}
+
+// Whether conv2d_impl runs an ungrouped convolution of this geometry on the implicit-GEMM kernels
+// (conv_igemm8x8_kernel, or conv_igemm_kernel under LCE_B200_IGEMM_8X4: the same chain per output)
+// whatever its batch and wherever its tensors sit. conv2d_impl takes that path first for such a
+// convolution, and Graph::FuseSubpixelConvs asks here before it replaces one by a kernel that
+// repeats the igemm kernels' chain, so the two cannot disagree. Never: 1x1 stride-1 convolutions
+// (tf32 pointwise and GEMM kernels), the 7x7 stride-2 3 -> 64 stem, K up to the direct kernel's
+// threshold. A convolution refused here may still reach the igemm kernels as a fallback.
+int lce_b200_internal_conv_runs_igemm(int in_h, int in_w, int in_c, int filter_h, int filter_w, int stride_h,
+                                      int stride_w, int dilation_h, int dilation_w, int out_c) {
+  if (filter_h == 1 && filter_w == 1 && stride_h == 1 && stride_w == 1) return 0;
+  if (filter_h == 7 && filter_w == 7 && in_c == 3 && out_c == 64 && stride_h == 2 && stride_w == 2 &&
+      dilation_h == 1 && dilation_w == 1)
+    return 0;
+  const long long K = static_cast<long long>(filter_h) * filter_w * in_c;
+  if (K <= direct_max_k()) return 0;
+  return K <= kIKMax && static_cast<long long>(in_h) * in_w * in_c < (1LL << 31);
+}
+
+static int igemm_conv(const ConvGeom& g, long long M, const float* in, const float* filter, const float* bias,
+                      float* out, void* stream) {
+  const int K = g.KH * g.KW * g.Cin;
+  dim3 igrid(static_cast<unsigned>((M + kIM - 1) / kIM), (g.Cout + kIN - 1) / kIN);
+  const size_t ksmem = static_cast<size_t>((K + kIK - 1) / kIK * kIK) * 2 * sizeof(int);
+  static const bool use8x4 = [] {
+    const char* e = getenv("LCE_B200_IGEMM_8X4");
+    return e && e[0] == '1';
+  }();
+  // with the kernels' static tiles, the offset table of a K above about 3000 (DoReFaNet's 3x3x384
+  // layers as float convolutions) passes the 48 KB a launch gets without opting in
+  {
+    static bool attr[64] = {};   // the attribute is per device
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64 || !attr[dev]) {
+      const int most = kIKMax * 2 * static_cast<int>(sizeof(int));
+      cudaFuncSetAttribute(conv_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+      cudaFuncSetAttribute(conv_igemm8x8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+      if (dev >= 0 && dev < 64) attr[dev] = true;
+    }
+  }
+  if (use8x4) {
+    conv_igemm_kernel<<<igrid, 256, ksmem, as_stream(stream)>>>(in, filter, bias, out, g, M);
+    return launch_check("conv_igemm_kernel");
+  }
+  conv_igemm8x8_kernel<<<igrid, 128, ksmem, as_stream(stream)>>>(in, filter, bias, out, g, M);
+  return launch_check("conv_igemm8x8_kernel");
+}
+
 // `packed` (optional): LceQuantize of the output. Kernels that can emit it in their epilogue do
 // and set *packed_done; the caller packs with the stand-alone kernel otherwise.
 static int conv2d_impl(const lce_f32_conv_desc* d, const float* in, const float* filter,
@@ -2137,11 +2398,8 @@ static int conv2d_impl(const lce_f32_conv_desc* d, const float* in, const float*
   const long long M = static_cast<long long>(g.B) * g.OH * g.OW;
   if (M == 0) return 0;
   const int K = g.KH * g.KW * g.Cin;
-  // experiments: LCE_B200_DIRECT_MAXK overrides the small-K threshold of the direct kernel
-  static const int direct_max_k = [] {
-    const char* e = getenv("LCE_B200_DIRECT_MAXK");
-    return e ? atoi(e) : kDirectMaxK;
-  }();
+  if (lce_b200_internal_conv_runs_igemm(g.H, g.W, g.Cin, g.KH, g.KW, g.sh, g.sw, g.dh, g.dw, g.Cout))
+    return igemm_conv(g, M, in, filter, bias, out, stream);
   // 1x1 stride-1 convolutions are plain GEMMs over the pixels: tensor cores first
   if (g.KH == 1 && g.KW == 1 && g.sh == 1 && g.sw == 1) {
     int32_t* pk = (packed && (g.Cout & 31) == 0) ? packed : nullptr;
@@ -2160,7 +2418,7 @@ static int conv2d_impl(const lce_f32_conv_desc* d, const float* in, const float*
   const int Gd = (g.Cout + 15) / 16;
   const size_t direct_smem =
       (static_cast<size_t>(K) * Gd * kDirectGroupStride + Gd * 16) * sizeof(float);
-  if (K <= direct_max_k && g.Cout <= kDirectMaxCout && !((uintptr_t)out & 15) &&
+  if (K <= direct_max_k() && g.Cout <= kDirectMaxCout && !((uintptr_t)out & 15) &&
       M * Gd < (1LL << 30) && direct_smem <= 96 * 1024) {
     const int G = Gd;
     const long long threads = M * G;
@@ -2234,33 +2492,8 @@ static int conv2d_impl(const lce_f32_conv_desc* d, const float* in, const float*
                                                              g.act, pk);
     return launch_check("conv_gemm128_kernel");
   }
-  if (K <= kIKMax && static_cast<long long>(g.H) * g.W * g.Cin < (1LL << 31)) {
-    dim3 igrid(static_cast<unsigned>((M + kIM - 1) / kIM), (g.Cout + kIN - 1) / kIN);
-    const size_t ksmem = static_cast<size_t>((K + kIK - 1) / kIK * kIK) * 2 * sizeof(int);
-    static const bool use8x4 = [] {
-      const char* e = getenv("LCE_B200_IGEMM_8X4");
-      return e && e[0] == '1';
-    }();
-    // with the kernels' static tiles, the offset table of a K above about 3000 (DoReFaNet's 3x3x384
-    // layers as float convolutions) passes the 48 KB a launch gets without opting in
-    {
-      static bool attr[64] = {};   // the attribute is per device
-      int dev = 0;
-      cudaGetDevice(&dev);
-      if (dev < 0 || dev >= 64 || !attr[dev]) {
-        const int most = kIKMax * 2 * static_cast<int>(sizeof(int));
-        cudaFuncSetAttribute(conv_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
-        cudaFuncSetAttribute(conv_igemm8x8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
-        if (dev >= 0 && dev < 64) attr[dev] = true;
-      }
-    }
-    if (use8x4) {
-      conv_igemm_kernel<<<igrid, 256, ksmem, as_stream(stream)>>>(in, filter, bias, out, g, M);
-      return launch_check("conv_igemm_kernel");
-    }
-    conv_igemm8x8_kernel<<<igrid, 128, ksmem, as_stream(stream)>>>(in, filter, bias, out, g, M);
-    return launch_check("conv_igemm8x8_kernel");
-  }
+  if (K <= kIKMax && static_cast<long long>(g.H) * g.W * g.Cin < (1LL << 31))
+    return igemm_conv(g, M, in, filter, bias, out, stream);
   dim3 grid(static_cast<unsigned>((M + kGM - 1) / kGM), (g.Cout + kGN - 1) / kGN);
   conv_gemm_kernel<<<grid, 256, 0, as_stream(stream)>>>(in, filter, bias, out, g, M);
   return launch_check("conv_gemm_kernel");
@@ -2789,6 +3022,25 @@ int resize_run(const char* op, const float* in, int batch, int in_h, int in_w, i
   else resize_nearest_kernel<1><<<grid, 256, 0, s>>>(in, out, g);
   return launch_check("resize_nearest_kernel");
 }
+
+template <int NCOL, int TN>
+int subpixel_launch(const float* in, const float* filter, const float* bias, const float* img, float* out,
+                    const SubpixelGeom& g, unsigned M, cudaStream_t s) {
+  using Tile = SubpixelTile<NCOL, TN>;
+  const int Kpad = (g.KH * g.KW * g.Cin + kIK - 1) / kIK * kIK;
+  const size_t smem = Tile::kFloats * sizeof(float) + 2 * static_cast<size_t>(Kpad) * sizeof(int);
+  static bool attr[64] = {};   // the attribute is per device
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64 || !attr[dev]) {
+    cudaFuncSetAttribute(subpixel_conv_kernel<NCOL, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         static_cast<int>(Tile::kFloats * sizeof(float) + 2 * kIKMax * sizeof(int)));
+    if (dev >= 0 && dev < 64) attr[dev] = true;
+  }
+  const unsigned blocks = (M + Tile::BM - 1) / Tile::BM;
+  subpixel_conv_kernel<NCOL, TN><<<blocks, 128, smem, s>>>(in, filter, bias, img, out, g, M);
+  return launch_check("subpixel_conv_kernel");
+}
 }  // namespace
 
 extern "C" {
@@ -2871,6 +3123,69 @@ int lce_b200_f32_resize_bilinear_argmax(const float* in, int batch, int in_h, in
   if (out_int64) bilinear_argmax_kernel<int64_t><<<grid, threads, smem, s>>>(in, g, static_cast<int64_t*>(out));
   else bilinear_argmax_kernel<int32_t><<<grid, threads, smem, s>>>(in, g, static_cast<int32_t*>(out));
   return launch_check("bilinear_argmax_kernel");
+}
+
+int lce_b200_f32_depth_to_space(const float* in, int batch, int in_h, int in_w, int channels, int block_size,
+                                float* out, void* stream) {
+  if (batch < 0 || in_h <= 0 || in_w <= 0 || channels <= 0 || block_size <= 0)
+    return fail("depth_to_space: bad shape (%d x %d x %d x %d, block size %d)", batch, in_h, in_w, channels,
+                block_size);
+  const int r = block_size;
+  if (channels % (static_cast<long long>(r) * r))
+    return fail("depth_to_space: %d channels are not a multiple of block_size^2 = %lld", channels,
+                static_cast<long long>(r) * r);
+  const int run = channels / r;   // r * C'
+  const long long row_len = static_cast<long long>(in_w) * run;
+  if (row_len >= (1LL << 31) - (1LL << 22) || static_cast<long long>(in_h) * r > INT_MAX)
+    return fail("depth_to_space: an output row of %lld floats is too wide", row_len);
+  if (batch == 0) return 0;
+  if (!in || !out) return fail("depth_to_space: null tensor");
+  const bool vec = run % 4 == 0 && !((uintptr_t)in & 15) && !((uintptr_t)out & 15);
+  const long long rows = static_cast<long long>(batch) * in_h * r;
+  const dim3 grid = row_grid(rows, vec ? row_len / 4 : row_len, 256);
+  cudaStream_t s = as_stream(stream);
+  if (vec) depth_to_space_kernel<4><<<grid, 256, 0, s>>>(in, out, in_h, in_w, channels, r, rows);
+  else depth_to_space_kernel<1><<<grid, 256, 0, s>>>(in, out, in_h, in_w, channels, r, rows);
+  return launch_check("depth_to_space_kernel");
+}
+
+int lce_b200_subpixel_conv_max_out_channels(void) { return SubpixelTile<8, 8>::BN; }
+
+int lce_b200_f32_subpixel_conv(const lce_f32_conv_desc* d, const float* in, const float* filter, const float* bias,
+                               int block_size, const float* img, int img_h, int img_w, int align_corners,
+                               int half_pixel_centers, int add_activation, float* out, void* stream) {
+  ConvGeom cg;
+  if (make_geom(d, &cg)) return 1;
+  const int r = block_size;
+  if (cg.sh != 1 || cg.sw != 1 || cg.dh != 1 || cg.dw != 1 || d->padding != LCE_PADDING_SAME)
+    return fail("subpixel_conv: the convolution must have stride 1, dilation 1 and SAME padding");
+  if (r <= 0 || cg.Cout % (r * r))
+    return fail("subpixel_conv: %d output channels are not a multiple of block_size^2 (block size %d)", cg.Cout, r);
+  if (cg.Cout > lce_b200_subpixel_conv_max_out_channels())
+    return fail("subpixel_conv: %d output channels are more than %d", cg.Cout,
+                lce_b200_subpixel_conv_max_out_channels());
+  const long long K = static_cast<long long>(cg.KH) * cg.KW * cg.Cin;
+  const long long M = static_cast<long long>(cg.B) * cg.H * cg.W;
+  if (K > kIKMax || static_cast<long long>(cg.H) * cg.W * cg.Cin >= (1LL << 31) || M > (1LL << 31))
+    return fail("subpixel_conv: the convolution is too large (K = %lld, %lld pixels)", K, M);
+  SubpixelGeom g{cg.B, cg.H, cg.W, cg.Cin, cg.KH, cg.KW, cg.ph, cg.pw, cg.Cout, r, cg.Cout / (r * r),
+                 cg.act, add_activation, {}};
+  if (static_cast<long long>(cg.H) * r > INT_MAX || static_cast<long long>(cg.W) * r * g.Cp >= (1LL << 31) - (1LL << 22))
+    return fail("subpixel_conv: an output row of %d x %d floats is too wide", cg.W * r, g.Cp);
+  if (img) {
+    if (resize_geom("subpixel_conv", cg.B, img_h, img_w, g.Cp, cg.H * r, cg.W * r, align_corners, half_pixel_centers,
+                    &g.img))
+      return 1;
+    if (align_corners && half_pixel_centers)
+      return fail("subpixel_conv: align_corners and half_pixel_centers cannot both be set");
+  }
+  if (M == 0) return 0;
+  if (!in || !filter || !out) return fail("subpixel_conv: null tensor");
+  cudaStream_t s = as_stream(stream);
+  const unsigned m = static_cast<unsigned>(M);
+  if (cg.Cout <= SubpixelTile<4, 4>::BN) return subpixel_launch<4, 4>(in, filter, bias, img, out, g, m, s);
+  if (cg.Cout <= SubpixelTile<4, 8>::BN) return subpixel_launch<4, 8>(in, filter, bias, img, out, g, m, s);
+  return subpixel_launch<8, 8>(in, filter, bias, img, out, g, m, s);
 }
 
 int lce_b200_f32_mean_hw_act(const float* in, float* out, int batch, int h, int w, int c, int pre_activation,

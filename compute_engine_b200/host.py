@@ -263,6 +263,12 @@ class HostGraph:
         node that never writes the resized map. Call before allocate_tensors."""
         return lib().lce_host_fuse_resize_argmax(self._g)
 
+    def fuse_subpixel_convs(self):
+        """CONV_2D -> DEPTH_TO_SPACE [-> ADD(RESIZE_BILINEAR(img))] (a super-resolution tail) => one
+        node that never writes the conv output, the shuffled map or the resized image. Call before
+        allocate_tensors."""
+        return lib().lce_host_fuse_subpixel_convs(self._g)
+
     def fuse_residual_pairs(self):
         """Two consecutive LceBconv2d+ADD[+LceQuantize] blocks whose intermediate nothing else
         reads => one node that keeps it on chip. Call after the other fusions."""
@@ -272,6 +278,7 @@ class HostGraph:
         return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_residual_blocks()
                 + self.fuse_spatial_scales()
                 + self.fuse_float_glue() + self.fuse_upsample_merges() + self.fuse_resize_argmax()
+                + self.fuse_subpixel_convs()
                 + self.fuse_grouped_conv_affine() + self.fuse_quantized_activations() + self.fuse_pooled_signs() + self.fuse_channel_gates() + self.fuse_activation_chains()
                 + self.fuse_residual_pairs())
 

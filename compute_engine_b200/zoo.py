@@ -302,6 +302,51 @@ def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, d
     return g.m.serialize()
 
 
+def binary_srnet(batch=1, seed=0, image=64, input_type="float32", scale=2, channels=64, blocks=16, residual=True):
+    """A binary super-resolution network in EDSR-baseline's layout. Head: CONV_2D 3x3, 3 -> `channels`,
+    with bias. Body: `blocks` residual blocks [LceQuantize -> LceBconv2d 3x3 (one-padding, BatchNorm
+    folded, no activation) -> ADD shortcut], then the long skip ADD(body, head). Tail: CONV_2D 3x3,
+    `channels` -> 3 * scale^2, with bias -> DEPTH_TO_SPACE(scale), and with `residual` an ADD of the
+    image resized to the output's size by RESIZE_BILINEAR (half_pixel_centers), so the network learns
+    the difference to a bilinear upscale. The tail is ESPCN's single sub-pixel convolution, not EDSR's
+    wider upsampler (a 64 -> 256 convolution and a shuffle per factor 2). image is an int or an (h, w)
+    pair; the output is [B, scale * h, scale * w, 3]. With input_type="int8" the DEQUANTIZE output
+    feeds both the head and the resize."""
+    if scale not in (2, 3, 4):
+        raise ValueError(f"binary_srnet needs scale 2, 3 or 4, not {scale}")
+    h, w = (image, image) if isinstance(image, int) else (int(image[0]), int(image[1]))
+    g = _Builder(seed, batch, "BinarySRNet")
+    xs = (batch, h, w, 3)
+    img = g.image_input(xs, input_type)
+
+    def conv3x3(t, cin, cout):
+        wt = g.rng.standard_normal((cout, 3, 3, cin)).astype(np.float32) * np.float32(1.0 / np.sqrt(9 * cin))
+        bias = g.rng.uniform(-0.1, 0.1, cout).astype(np.float32)
+        y = g.act((batch, h, w, cout))
+        g.m.add_op("CONV_2D", [t, g.const(wt), g.const(bias, name="b")], [y], padding="SAME", stride=(1, 1),
+                   activation="NONE")
+        return y
+
+    ts = (batch, h, w, channels)
+    head = x = conv3x3(img, 3, channels)
+    for _ in range(blocks):
+        q = g.quantize(x, ts)
+        y, _ = g.bconv(q, ts, channels, pad_values=1, activation="NONE")
+        x = g.add(y, x, ts)
+    x = g.add(x, head, ts)
+    sub = conv3x3(x, channels, 3 * scale * scale)
+    out_shape = (batch, scale * h, scale * w, 3)
+    out = g.act(out_shape)
+    g.m.add_op("DEPTH_TO_SPACE", [sub], [out], block_size=scale)
+    if residual:
+        up = g.act(out_shape)
+        size = g.const(np.array([scale * h, scale * w], np.int32), np.int32, "size")
+        g.m.add_op("RESIZE_BILINEAR", [img, size], [up], half_pixel_centers=True)
+        out = g.add(out, up, out_shape)
+    g.m.outputs = [out]
+    return g.m.serialize()
+
+
 def ssd_anchors(grids, min_scale=0.2, max_scale=0.95):
     """The TF Object Detection API's SSD anchors (anchor_generators/multiple_grid_anchor_generator.py,
     create_ssd_anchors with its defaults) for feature maps of `grids` [(h, w), ...], in float32 as

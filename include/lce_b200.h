@@ -353,6 +353,26 @@ int lce_b200_resize_bilinear_argmax_max_row_floats(void);
 int lce_b200_f32_resize_bilinear_argmax(const float* in_dev, int batch, int in_h, int in_w, int channels,
                                         int out_h, int out_w, int align_corners, int half_pixel_centers,
                                         int out_int64, void* out_dev, void* stream);
+/* TFLite's float DEPTH_TO_SPACE (TF/lite/kernels/internal/reference/depth_to_space.h): in [batch, in_h,
+ * in_w, channels] to out [batch, in_h * block_size, in_w * block_size, channels / block_size^2] with
+ * out[b, y*r + i, x*r + j, c] = in[b, y, x, (i*r + j) * C' + c] (r = block_size, C' = channels / r^2);
+ * the values are moved, not computed. Refuses block_size <= 0 and channels % r^2 != 0. */
+int lce_b200_f32_depth_to_space(const float* in_dev, int batch, int in_h, int in_w, int channels, int block_size,
+                                float* out_dev, void* stream);
+/* The largest out_c lce_b200_f32_subpixel_conv takes: every CTA computes all the conv's channels. */
+int lce_b200_subpixel_conv_max_out_channels(void);
+/* A super-resolution network's sub-pixel tail in one pass: lce_b200_f32_conv2d(d) (stride 1, dilation 1,
+ * SAME; out_c = C' * block_size^2 <= lce_b200_subpixel_conv_max_out_channels(); K = filter_h * filter_w *
+ * in_c <= 4096), then lce_b200_f32_depth_to_space(block_size), then, when img_dev is set, an ADD (with
+ * add_activation) of lce_b200_f32_resize_bilinear(img [batch, img_h, img_w, C'] to (in_h * block_size,
+ * in_w * block_size), align_corners, half_pixel_centers). out [batch, in_h * r, in_w * r, C'] equals the
+ * ops run one by one bit for bit where lce_b200_f32_conv2d runs the convolution on its implicit-GEMM
+ * kernels; the conv output, the shuffled map and the resized image are never written. */
+struct lce_f32_conv_desc; /* lce_b200_builtins.h */
+int lce_b200_f32_subpixel_conv(const struct lce_f32_conv_desc* d, const float* in_dev, const float* filter_dev,
+                               const float* bias_dev, int block_size, const float* img_dev, int img_h, int img_w,
+                               int align_corners, int half_pixel_centers, int add_activation, float* out_dev,
+                               void* stream);
 /* TFLite_Detection_PostProcess (TF/lite/kernels/detection_postprocess.cc) with its float32 inputs,
  * applied to every image of a batch as TFLite applies it to its single image. */
 typedef struct {
