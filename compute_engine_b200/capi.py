@@ -99,7 +99,7 @@ EXPORTS = [
     "lce_b200_bconv2d_run", "lce_b200_bconv2d_run_fused", "lce_b200_bconv2d_run_fused_chain",
     "lce_b200_bconv2d_run_fused_pair",
     "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_fused_scale",
-    "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add",
+    "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add", "lce_b200_bconv2d_run_fused_shuffle",
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_scale_sign", "lce_b200_f32_logistic",
     "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
     "lce_b200_f32_maximum", "lce_b200_f32_minimum", "lce_b200_f32_div", "lce_b200_f32_round",
@@ -110,6 +110,7 @@ EXPORTS = [
     "lce_b200_f32_resize_nearest", "lce_b200_f32_resize_bilinear", "lce_b200_f32_upsample_add_sign",
     "lce_b200_f32_argmax", "lce_b200_resize_bilinear_argmax_max_row_floats", "lce_b200_f32_resize_bilinear_argmax",
     "lce_b200_f32_depth_to_space", "lce_b200_subpixel_conv_max_out_channels", "lce_b200_f32_subpixel_conv",
+    "lce_b200_f32_transpose_conv2d",
     "lce_b200_detection_max_anchors", "lce_b200_detection_workspace_bytes", "lce_b200_f32_detection_postprocess",
     "lce_b200_bconv2d_run_f32", "lce_b200_bconv2d_run_host",
     "lce_b200_bconv2d_destroy", "lce_b200_bgemm_create", "lce_b200_bgemm_run",
@@ -544,6 +545,36 @@ def depth_to_space(x: torch.Tensor, block_size: int):
         raise LceError(f"depth_to_space: {c} channels are not a multiple of block_size^2 (block size {r})")
     out = torch.empty((b, h * r, w * r, c // (r * r)), dtype=torch.float32, device=x.device)
     _check(lib().lce_b200_f32_depth_to_space(_p(x), b, h, w, c, r, _p(out), _stream()))
+    return out
+
+
+class TransposeConvDesc(C.Structure):
+    """``lce_f32_transpose_conv_desc`` (include/lce_b200_types.h)."""
+    _fields_ = [(n, C.c_int32) for n in (
+        "batch", "in_h", "in_w", "in_c", "filter_h", "filter_w", "out_c", "out_h", "out_w", "stride_h",
+        "stride_w", "pad_h", "pad_w", "activation")]
+
+
+def transpose_conv2d(x: torch.Tensor, filt: torch.Tensor, bias, out_hw, stride, padding=PADDING_SAME,
+                     activation=ACT_NONE):
+    """TFLite's float TRANSPOSE_CONV of an NHWC map x [B, H, W, C_in] with weights [C_out, kh, kw, C_in]
+    to [B, out_h, out_w, C_out]: TFLite's padding for that output size (the floor half), each output one
+    fmaf chain in the reference's order, then the bias (may be None) and the activation."""
+    x = _dev(x, torch.float32)
+    filt = _dev(filt, torch.float32)
+    bias = None if bias is None else _dev(bias, torch.float32)
+    b, h, w, cin = x.shape
+    cout, kh, kw, _ = filt.shape
+    (oh, ow), (sh, sw) = out_hw, stride
+    want = [(o + s - 1) // s if padding == PADDING_SAME else (o + s - k) // s
+            for o, s, k in ((oh, sh, kh), (ow, sw, kw))]
+    if filt.shape[3] != cin or want != [h, w]:
+        raise LceError(f"transpose_conv2d: input {tuple(x.shape)} is not what a convolution with filter "
+                       f"{tuple(filt.shape)}, stride {stride} gives from output {out_hw}")
+    ph, pw = (max((n - 1) * s + k - o, 0) // 2 for n, s, k, o in ((h, sh, kh, oh), (w, sw, kw, ow)))
+    d = TransposeConvDesc(b, h, w, cin, kh, kw, cout, oh, ow, sh, sw, ph, pw, activation)
+    out = torch.empty((b, oh, ow, cout), dtype=torch.float32, device=x.device)
+    _check(lib().lce_b200_f32_transpose_conv2d(C.byref(d), _p(x), _p(filt), _p(bias), _p(out), _stream()))
     return out
 
 

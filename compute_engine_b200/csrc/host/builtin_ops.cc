@@ -1091,6 +1091,160 @@ TfLiteStatus SubpixelInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// ------------------------------ TRANSPOSE_CONV ------------------------------ //
+// inputs [output_shape (constant int32 [4], read on the host as the resizes read their size), weights
+// [Cout, kh, kw, Cin], x [B, H, W, Cin], bias [Cout] (-1 when absent)], output [B, output_shape[1],
+// output_shape[2], Cout]: the batch follows x's, as the resizes' does, so a batch resize keeps the
+// model's output_shape (output_shape[0] is not read). Float32 only. The padding is TFLite's
+// (TF/lite/kernels/transpose_conv.cc): ComputePaddingHeightWidth run on the output's size, the floor
+// half of the total, and x's H and W must be what a convolution with this filter, stride and padding
+// gives from the output's (TF's consistency condition; Keras' output_padding < stride meets it).
+// Fills *d, or returns why the node is refused.
+int TransposeConvInputSize(int padding, int out, int k, int s) {
+  return padding == LCE_PADDING_SAME ? (out + s - 1) / s : (out + s - k) / s;
+}
+const char* TransposeConvChecks(TfLiteContext* c, TfLiteNode* n, const BuiltinParams& p,
+                                lce_f32_transpose_conv_desc* d) {
+  if ((n->inputs->size != 3 && n->inputs->size != 4) || n->outputs->size != 1)
+    return "TRANSPOSE_CONV: inputs [output_shape, weights, input, bias] and one output expected";
+  const TfLiteTensor* shape = T(c, n->inputs, 0);
+  const TfLiteTensor* w = T(c, n->inputs, 1);
+  const TfLiteTensor* x = T(c, n->inputs, 2);
+  const TfLiteTensor* bias = n->inputs->size == 4 ? T(c, n->inputs, 3) : nullptr;
+  const TfLiteTensor* o = T(c, n->outputs, 0);
+  if (!shape || shape->allocation_type != kTfLiteMmapRo || !HostInts(shape) || Count(shape) != 4)
+    return "TRANSPOSE_CONV: output_shape must be a constant int32 tensor of 4 elements";
+  if (!w || !x || !o || w->type != kTfLiteFloat32 || x->type != kTfLiteFloat32 || o->type != kTfLiteFloat32 ||
+      (bias && bias->type != kTfLiteFloat32))
+    return "TRANSPOSE_CONV: only float32 is supported";
+  if (w->dims->size != 4 || x->dims->size != 4) return "TRANSPOSE_CONV: the weights and the input must be 4-D";
+  const int cout = w->dims->data[0], kh = w->dims->data[1], kw = w->dims->data[2];
+  if (w->dims->data[3] != x->dims->data[3]) return "TRANSPOSE_CONV: the weights' input channels differ from the input's";
+  if (bias && (bias->dims->size != 1 || bias->dims->data[0] != cout))
+    return "TRANSPOSE_CONV: the bias must have shape [Cout]";
+  const int32_t* os = shape->data.i32;
+  if (os[3] != cout) return "TRANSPOSE_CONV: output_shape[3] differs from the weights' output channels";
+  if (p.stride_h <= 0 || p.stride_w <= 0) return "TRANSPOSE_CONV: strides must be positive";
+  if (p.activation < LCE_ACT_NONE || p.activation > LCE_ACT_RELU6)
+    return "TRANSPOSE_CONV: the fused activation must be NONE, RELU, RELU_N1_TO_1 or RELU6";
+  if (p.padding != LCE_PADDING_SAME && p.padding != LCE_PADDING_VALID) return "TRANSPOSE_CONV: unknown padding";
+  if (os[1] <= 0 || os[2] <= 0 || kh <= 0 || kw <= 0 || cout <= 0)
+    return "TRANSPOSE_CONV: the output and the filter must not be empty";
+  if (x->dims->data[1] != TransposeConvInputSize(p.padding, os[1], kh, p.stride_h) ||
+      x->dims->data[2] != TransposeConvInputSize(p.padding, os[2], kw, p.stride_w))
+    return "TRANSPOSE_CONV: the input's height and width are not what a convolution with this filter, stride "
+           "and padding gives from output_shape";
+  auto pad = [](int in, int k, int s, int out) {   // ComputePaddingWithOffset(s, 1, out, k, in), floor half
+    const int64_t total = static_cast<int64_t>(in - 1) * s + k - out;
+    return static_cast<int>(total > 0 ? total / 2 : 0);
+  };
+  *d = {x->dims->data[0], x->dims->data[1], x->dims->data[2], x->dims->data[3], kh, kw, cout, os[1], os[2],
+        p.stride_h, p.stride_w, pad(x->dims->data[1], kh, p.stride_h, os[1]),
+        pad(x->dims->data[2], kw, p.stride_w, os[2]), p.activation};
+  return nullptr;
+}
+TfLiteStatus TransposeConvPrepare(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_transpose_conv_desc d;
+  const char* why = TransposeConvChecks(c, n, P(n), &d);
+  B_ENSURE(c, why == nullptr, why);
+  return Resize(c, T(c, n->outputs, 0), {d.batch, d.out_h, d.out_w, d.out_c});
+}
+TfLiteStatus TransposeConvInvoke(TfLiteContext* c, TfLiteNode* n) {
+  lce_f32_transpose_conv_desc d;
+  TransposeConvChecks(c, n, P(n), &d);
+  const TfLiteTensor* bias = n->inputs->size == 4 ? T(c, n->inputs, 3) : nullptr;
+  B_CAPI(c, lce_b200_f32_transpose_conv2d(&d, T(c, n->inputs, 2)->data.f, T(c, n->inputs, 1)->data.f,
+                                          bias ? bias->data.f : nullptr, T(c, n->outputs, 0)->data.f,
+                                          lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// --- fused LceDequantize -> TRANSPOSE_CONV (+-1, k = s) [-> ADD(skip)] [-> LceQuantize]: a binary upsampler --- //
+// Created by Graph::FuseBinaryTransposeConvs; builtin_data = BinaryTConvParams; inputs [q (packed signs
+// [B, H, W, ceil(Cin / 32)]), filter (the weights' signs as a packed 1x1 LceBconv2d filter [s_h * s_w *
+// C, 1, 1, ceil(Cin / 32)], rows in (i, j, c) order), bias ([C] or -1), skip ([B, H * s_h, W * s_w, C]
+// or -1)], outputs [sum [B, H * s_h, W * s_w, C], packed signs?]. The node owns a 1x1 LceBconv2d plan
+// and runs lce_b200_bconv2d_run_fused_shuffle, which takes the +-1 dot product from its accumulators.
+struct BinaryTConvParams {
+  BuiltinParams tconv, add;
+  int32_t channels_in;
+};
+struct BinaryTConvOp {
+  BinaryTConvParams p;
+  lce_b200_bconv2d* plan = nullptr;
+};
+void* BinaryTConvInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* op = new BinaryTConvOp();
+  memset(&op->p, 0, sizeof(op->p));
+  if (buffer && length >= sizeof(BinaryTConvParams)) memcpy(&op->p, buffer, sizeof(BinaryTConvParams));
+  return op;
+}
+void BinaryTConvFree(TfLiteContext*, void* p) {
+  auto* op = static_cast<BinaryTConvOp*>(p);
+  lce_b200_bconv2d_destroy(op->plan);
+  delete op;
+}
+TfLiteStatus BinaryTConvPrepare(TfLiteContext* c, TfLiteNode* n) {
+  auto* op = static_cast<BinaryTConvOp*>(n->user_data);
+  const BinaryTConvParams& bp = op->p;
+  B_ENSURE(c, n->inputs->size == 4 && n->outputs->size >= 1 && n->outputs->size <= 2,
+           "LceBconv2dTranspose: inputs [q, filter, bias, skip] and one or two outputs expected");
+  const TfLiteTensor* q = T(c, n->inputs, 0);
+  const TfLiteTensor* f = T(c, n->inputs, 1);
+  const TfLiteTensor* bias = T(c, n->inputs, 2);
+  const TfLiteTensor* skip = T(c, n->inputs, 3);
+  const int sh = bp.tconv.stride_h, sw = bp.tconv.stride_w, cin = bp.channels_in;
+  B_ENSURE(c, sh > 0 && sw > 0 && cin > 0, "LceBconv2dTranspose: bad strides or input channels");
+  B_ENSURE(c, q && q->type == kTfLiteInt32 && q->dims->size == 4 && q->dims->data[3] == (cin + 31) / 32,
+           "LceBconv2dTranspose: the input must be the packed signs [B, H, W, ceil(Cin / 32)]");
+  B_ENSURE(c, f && f->type == kTfLiteInt32 && f->allocation_type == kTfLiteMmapRo && f->dims->size == 4 &&
+                  f->dims->data[1] == 1 && f->dims->data[2] == 1 && f->dims->data[3] == (cin + 31) / 32 &&
+                  f->dims->data[0] % (sh * sw) == 0,
+           "LceBconv2dTranspose: the filter must be a constant packed [s_h * s_w * C, 1, 1, ceil(Cin / 32)]");
+  const int C = f->dims->data[0] / (sh * sw);
+  B_ENSURE(c, !bias || (bias->type == kTfLiteFloat32 && bias->allocation_type == kTfLiteMmapRo &&
+                        Count(bias) == C),
+           "LceBconv2dTranspose: the bias must be a constant float32 [C]");
+  const int B = q->dims->data[0], H = q->dims->data[1], W = q->dims->data[2];
+  B_ENSURE(c, static_cast<int64_t>(H) * sh <= INT32_MAX && static_cast<int64_t>(W) * sw <= INT32_MAX,
+           "LceBconv2dTranspose: the output is too large");
+  const int OH = H * sh, OW = W * sw;
+  B_ENSURE(c, !skip || (skip->type == kTfLiteFloat32 && skip->dims->size == 4 && skip->dims->data[0] == B &&
+                        skip->dims->data[1] == OH && skip->dims->data[2] == OW && skip->dims->data[3] == C),
+           "LceBconv2dTranspose+ADD: the skip map must have the output's shape");
+  if (Resize(c, T(c, n->outputs, 0), {B, OH, OW, C}) != kTfLiteOk) return kTfLiteError;
+  if (n->outputs->size == 2) {
+    TfLiteTensor* pk = T(c, n->outputs, 1);
+    B_ENSURE(c, pk && pk->type == kTfLiteInt32, "LceBconv2dTranspose+LceQuantize: packed output must be int32");
+    if (Resize(c, pk, {B, OH, OW, (C + 31) / 32}) != kTfLiteOk) return kTfLiteError;
+  }
+  if (op->plan) {
+    B_CAPI(c, lce_b200_bconv2d_set_input_shape(op->plan, B, H, W));
+    return kTfLiteOk;
+  }
+  lce_bconv2d_desc d;
+  memset(&d, 0, sizeof(d));
+  d.batch = B; d.in_h = H; d.in_w = W; d.channels_in = cin;
+  d.filter_h = 1; d.filter_w = 1; d.channels_out = sh * sw * C; d.groups = 1;
+  d.stride_h = 1; d.stride_w = 1; d.dilation_h = 1; d.dilation_w = 1;
+  d.padding = LCE_PADDING_VALID; d.pad_value = 1; d.activation = LCE_ACT_NONE; d.out_type = LCE_OUT_FLOAT;
+  const std::vector<float> ones(d.channels_out, 1.0f), zeros(d.channels_out, 0.0f);
+  B_CAPI(c, lce_b200_bconv2d_create(&d, f->data.i32, ones.data(), zeros.data(), nullptr, &op->plan));
+  return kTfLiteOk;
+}
+TfLiteStatus BinaryTConvInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const auto* op = static_cast<const BinaryTConvOp*>(n->user_data);
+  const TfLiteTensor* bias = T(c, n->inputs, 2);
+  const TfLiteTensor* skip = T(c, n->inputs, 3);
+  TfLiteTensor* pk = n->outputs->size > 1 ? T(c, n->outputs, 1) : nullptr;
+  B_CAPI(c, lce_b200_bconv2d_run_fused_shuffle(op->plan, T(c, n->inputs, 0)->data.i32, op->p.tconv.stride_h,
+                                               op->p.tconv.stride_w, bias ? bias->data.f : nullptr,
+                                               op->p.tconv.activation, skip ? skip->data.f : nullptr,
+                                               op->p.add.activation, T(c, n->outputs, 0)->data.f,
+                                               pk ? pk->data.i32 : nullptr, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // ------------------------------ CONCATENATION ------------------------------ //
 // Strided device copies (one cudaMemcpy2DAsync per input): no kernel of ours.
 TfLiteStatus ConcatPrepare(TfLiteContext* c, TfLiteNode* n) {
@@ -1433,6 +1587,10 @@ const TfLiteRegistration* ResizeArgmaxRegistration() {
   static TfLiteRegistration r = {ResizeArgmaxInit, ResizeArgmaxFree, ResizeArgmaxPrepare, ResizeArgmaxInvoke};
   return &r;
 }
+const TfLiteRegistration* BinaryTransposeConvRegistration() {
+  static TfLiteRegistration r = {BinaryTConvInit, BinaryTConvFree, BinaryTConvPrepare, BinaryTConvInvoke};
+  return &r;
+}
 const TfLiteRegistration* SubpixelConvRegistration() {
   static TfLiteRegistration r = {SubpixelInit, SubpixelFree, SubpixelPrepare, SubpixelInvoke};
   return &r;
@@ -1497,6 +1655,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(56, &arg_max);   // ARG_MAX
   static TfLiteRegistration depth_to_space = {Init, Free, DepthToSpacePrepare, DepthToSpaceInvoke};
   r->AddBuiltin(5, &depth_to_space);   // DEPTH_TO_SPACE
+  static TfLiteRegistration transpose_conv = {Init, Free, TransposeConvPrepare, TransposeConvInvoke};
+  r->AddBuiltin(67, &transpose_conv);   // TRANSPOSE_CONV
   static TfLiteRegistration detection = {DetectionInit, DetectionFree, DetectionPrepare, DetectionInvoke};
   r->AddCustom("TFLite_Detection_PostProcess", &detection);
 }

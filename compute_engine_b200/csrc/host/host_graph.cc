@@ -315,6 +315,7 @@ constexpr const char* kResizeNearest = "builtin:97";
 constexpr const char* kResizeBilinear = "builtin:23";
 constexpr const char* kArgMax = "builtin:56";
 constexpr const char* kDepthToSpace = "builtin:5";
+constexpr const char* kTransposeConv = "builtin:67";
 constexpr const char* kMul = "builtin:18";
 constexpr const char* kRelu = "builtin:19";
 constexpr const char* kMean = "builtin:40";
@@ -1887,6 +1888,128 @@ int Graph::FuseSubpixelConvs() {
     const int k = fuse(i);
     removed += k;
     if (k == 0) ++i;   // else node i is erased and its successor moved up
+  }
+  allocated_ = false;
+  return removed;
+}
+
+const TfLiteRegistration* BinaryTransposeConvRegistration();   // builtin_ops.cc
+extern "C" int lce_b200_internal_shuffle_takes(const lce_bconv2d_desc* d, int s_h, int s_w);   // lce_b200.cu
+
+int Graph::FuseBinaryTransposeConvs() {
+  if (!device_arena_) return 0;
+  auto fuse = [&](size_t i) -> int {   // nodes removed by fusing the TRANSPOSE_CONV at i, 0 when it stays
+    NodeRecord& tc = *nodes_[i];
+    const BuiltinParams* tp = Params(tc);
+    if (tc.name != kTransposeConv || tc.initialized || !tp || tc.node.inputs->size < 3 || tc.node.inputs->size > 4 ||
+        tc.node.outputs->size != 1)
+      return 0;
+    const int shape = tc.node.inputs->data[0], w = tc.node.inputs->data[1], x = tc.node.inputs->data[2];
+    const int bias = tc.node.inputs->size == 4 ? tc.node.inputs->data[3] : -1, y = tc.node.outputs->data[0];
+    const int sh = tp->stride_h, sw = tp->stride_w;
+    if (shape < 0 || w < 0 || x < 0 || tensors_[shape].type != kTfLiteInt32 ||
+        tensors_[shape].allocation_type != kTfLiteMmapRo || tensors_[w].type != kTfLiteFloat32 ||
+        tensors_[w].allocation_type != kTfLiteMmapRo || tensors_[x].type != kTfLiteFloat32 ||
+        tensors_[y].type != kTfLiteFloat32 || tp->activation < LCE_ACT_NONE || tp->activation > LCE_ACT_RELU6 ||
+        sh <= 0 || sw <= 0 || sh * sw < 2)
+      return 0;
+    const TfLiteIntArray* wd = tensors_[w].dims;
+    const TfLiteIntArray* xd = tensors_[x].dims;
+    if (!wd || wd->size != 4 || !xd || xd->size != 4 || wd->data[1] != sh || wd->data[2] != sw ||
+        wd->data[3] != xd->data[3] || const_host_[shape].size() < 4 * sizeof(int32_t) ||
+        tensors_[shape].bytes != 4 * sizeof(int32_t))
+      return 0;
+    const int C = wd->data[0], cin = xd->data[3];
+    // the output exactly in * s: no output_padding rows (which would hold the bias alone)
+    int32_t os[4];
+    memcpy(os, const_host_[shape].data(), sizeof(os));
+    if (os[1] != static_cast<int64_t>(xd->data[1]) * sh || os[2] != static_cast<int64_t>(xd->data[2]) * sw ||
+        os[3] != C)
+      return 0;
+    if (bias >= 0 && (tensors_[bias].type != kTfLiteFloat32 || tensors_[bias].allocation_type != kTfLiteMmapRo ||
+                      !tensors_[bias].dims || tensors_[bias].dims->size != 1 || tensors_[bias].dims->data[0] != C))
+      return 0;
+    // every weight exactly +1.0f or -1.0f (not -0.0, not 0.5)
+    const size_t nw = static_cast<size_t>(C) * sh * sw * cin;
+    if (const_host_[w].size() < nw * sizeof(float)) return 0;
+    std::vector<uint32_t> wb(nw);
+    memcpy(wb.data(), const_host_[w].data(), nw * sizeof(float));
+    for (uint32_t v : wb)
+      if (v != 0x3f800000u && v != 0xbf800000u) return 0;
+    lce_bconv2d_desc d;
+    memset(&d, 0, sizeof(d));
+    d.batch = xd->data[0]; d.in_h = xd->data[1]; d.in_w = xd->data[2]; d.channels_in = cin;
+    d.filter_h = 1; d.filter_w = 1; d.channels_out = sh * sw * C; d.groups = 1;
+    d.stride_h = 1; d.stride_w = 1; d.dilation_h = 1; d.dilation_w = 1;
+    d.padding = LCE_PADDING_VALID; d.pad_value = 1; d.activation = LCE_ACT_NONE; d.out_type = LCE_OUT_FLOAT;
+    if (!lce_b200_internal_shuffle_takes(&d, sh, sw)) return 0;   // C % 64 == 0, the b1 mma.sync kernel
+    // x: an LceDequantize of packed signs q, read by the TRANSPOSE_CONV alone
+    size_t di = kNoNode;
+    for (size_t k = 0; k < i && di == kNoNode; ++k)
+      if (nodes_[k]->node.outputs->size == 1 && nodes_[k]->node.outputs->data[0] == x) di = k;
+    if (di == kNoNode || SoleConsumer(x) != i) return 0;
+    const NodeRecord& dq = *nodes_[di];
+    const int q = dq.node.inputs->size == 1 ? dq.node.inputs->data[0] : -1;
+    if (dq.name != "LceDequantize" || dq.initialized || q < 0 || tensors_[q].type != kTfLiteInt32) return 0;
+    // the ADD: y's one reader, the other operand of y's shape (no broadcast) and ready before it
+    size_t ai = SoleConsumer(y);
+    int skip = -1;
+    if (ai != kNoNode) {
+      const NodeRecord& a = *nodes_[ai];
+      const int in0 = a.node.inputs->size == 2 ? a.node.inputs->data[0] : -1;
+      const int in1 = a.node.inputs->size == 2 ? a.node.inputs->data[1] : -1;
+      skip = in0 == y ? in1 : in0;
+      if (ai <= i || a.name != kAdd || a.initialized || a.node.outputs->size != 1 || !Params(a) || in0 == in1 ||
+          skip < 0 || tensors_[skip].type != kTfLiteFloat32 || tensors_[a.node.outputs->data[0]].type != kTfLiteFloat32 ||
+          !SameDims(tensors_[skip].dims, tensors_[y].dims) || !ReadyBefore(skip, ai)) {
+        ai = kNoNode;
+        skip = -1;
+      }
+    }
+    const int s = ai != kNoNode ? nodes_[ai]->node.outputs->data[0] : y;
+    // the signs: the sum's only LceQuantize reader; the sum itself stays stored
+    size_t kq = kNoNode;
+    int quantizers = 0;
+    for (size_t k : Consumers(s))
+      if (nodes_[k]->name == "LceQuantize") { ++quantizers; kq = k; }
+    const bool tail = quantizers == 1 && IsQuantize(kq) && kq > (ai != kNoNode ? ai : i);
+    std::vector<int> outs{s};
+    if (tail) outs.push_back(nodes_[kq]->node.outputs->data[0]);
+    // the filter: each weight's sign bit, rows (i, j, c) of the 1x1 GEMM, ceil(Cin / 32) words per row
+    const int cw = (cin + 31) / 32;
+    std::vector<int32_t> filt(static_cast<size_t>(d.channels_out) * cw, 0);
+    for (int c = 0; c < C; ++c)
+      for (int fi = 0; fi < sh; ++fi)
+        for (int fj = 0; fj < sw; ++fj) {
+          const size_t src = ((static_cast<size_t>(c) * sh + fi) * sw + fj) * cin;
+          int32_t* row = filt.data() + (static_cast<size_t>(fi * sw + fj) * C + c) * cw;
+          for (int ci = 0; ci < cin; ++ci)
+            if (wb[src + ci] >> 31) row[ci >> 5] |= static_cast<int32_t>(1u << (ci & 31));
+        }
+    const int ft = AddTensor(kTfLiteInt32, {d.channels_out, 1, 1, cw}, filt.data(), filt.size() * sizeof(int32_t),
+                             false, 0.0f, 0, names_[w] + "_packed", /*const_on_device=*/true);
+    struct {
+      BuiltinParams tconv, add;
+      int32_t channels_in;
+    } params{*tp, ai != kNoNode ? *Params(*nodes_[ai]) : BuiltinParams{}, cin};
+    // the ADD's node (or without it the TRANSPOSE_CONV's) becomes the fused one: q and the skip exist
+    // where it runs, and every reader of the sum and of the signs comes after it
+    NodeRecord& f = ai != kNoNode ? *nodes_[ai] : tc;
+    SetNodeIO(f, {q, ft, bias, skip}, outs);
+    SetBuiltinBlob(f, &params, sizeof(params));
+    f.registration = BinaryTransposeConvRegistration();
+    f.name = std::string("LceBconv2dTranspose") + (ai != kNoNode ? "+ADD" : "") + (tail ? "+LceQuantize" : "");
+    std::vector<size_t> gone{di};
+    if (ai != kNoNode) gone.push_back(i);
+    if (tail) gone.push_back(kq);
+    EraseNodes(gone);
+    return static_cast<int>(gone.size());
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size();) {
+    const int k = fuse(i);
+    removed += k;
+    i = k > 0 ? 0 : i + 1;   // indices moved: scan again (a fused node no longer matches)
   }
   allocated_ = false;
   return removed;

@@ -285,6 +285,24 @@ class Graph {
   // Bit-identical. Returns the nodes removed.
   int FuseSubpixelConvs();
 
+  // A binary learned upsampler, as a larq QuantConv2DTranspose(ste_sign, ste_sign) converts,
+  //   LceDequantize(q) -> TRANSPOSE_CONV(+-1 weights, kernel = stride s_h x s_w, s_h * s_w >= 2, bias?,
+  //   activation) [-> ADD(skip)] [-> LceQuantize]
+  // becomes one node (lce_b200_bconv2d_run_fused_shuffle) that reads q's packed words, runs the layer as
+  // a 1x1 binary convolution to s_h * s_w * C columns on the b1 mma.sync kernel and stores each column
+  // at its pixel-shuffled address, adding the bias, the activation and the skip there and packing the
+  // signs: "LceBconv2dTranspose[+ADD][+LceQuantize]", inputs [q, packed filter (a new constant), bias
+  // (-1 when absent), skip (-1 when absent)], outputs [sum, signs?]. The sum is always stored (the
+  // decoder's next shortcut reads it). Only when every weight is exactly +1.0f or -1.0f, the output is
+  // exactly in * s (no output_padding), C % 64 == 0 and the plan lands on the b1 mma.sync kernel
+  // (lce_b200_internal_shuffle_takes); the dequantized map is read by the TRANSPOSE_CONV alone and is
+  // not a graph output. The ADD joins only when it is the TRANSPOSE_CONV output's one reader (not a graph
+  // output), without broadcast, with the skip ready before it; the LceQuantize joins when it is the
+  // sum's only sign reader. Otherwise the graph is left as it is. Bit-identical: every product is +-1,
+  // so the dot product is exact in any order. fuse_all runs it before FuseResidualBlocks; no pass before
+  // it matches a TRANSPOSE_CONV, its ADD or its LceQuantize. Returns the nodes removed.
+  int FuseBinaryTransposeConvs();
+
   // init (first time) + prepare of every node in order, then arena allocation.
   TfLiteStatus AllocateTensors();
   TfLiteStatus ResizeInputTensor(int tensor, const std::vector<int>& dims);

@@ -331,6 +331,12 @@ bool BuildGraphFromTflite(const uint8_t* data, size_t size, const OpResolver& re
       case 5:  // DEPTH_TO_SPACE: DepthToSpaceOptions
         bp.block_size = o.scalar<int32_t>(0, 0);
         break;
+      case 67:  // TRANSPOSE_CONV: TransposeConvOptions
+        bp.padding = o.scalar<int8_t>(0, 0);
+        bp.stride_w = o.scalar<int32_t>(1, 0);
+        bp.stride_h = o.scalar<int32_t>(2, 0);
+        bp.activation = o.scalar<int8_t>(3, 0);
+        break;
       default:
         break;
     }

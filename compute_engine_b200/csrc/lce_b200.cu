@@ -194,20 +194,21 @@ size_t imma_smem_budget(int V, bool b1) {
 }
 
 template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
-          bool SPATIAL = false, bool GW = false>
+          bool SPATIAL = false, bool GW = false, bool SHUFFLE = false>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW, SHUFFLE>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(imma_smem_budget(V, B1))));
-  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW><<<grid, lce::kIThreads, smem, s>>>(p);
+  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW, SHUFFLE><<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
 // Epilogue tails of the float output beyond run_fused's (bconv_run_impl decides).
 // kScale: p.gate indexed by position within the image (lce_b200_bconv2d_run_fused_scale)
-enum class Tail { kNone, kChain, kGate, kScale, kSlice };   // p.chain / p.gate / p.out_stride in the epilogue
+// kShuffle: the pixel-shuffled store of lce_b200_bconv2d_run_fused_shuffle (p.shuf_*), b1 only
+enum class Tail { kNone, kChain, kGate, kScale, kSlice, kShuffle };   // p.chain / p.gate / p.out_stride in the epilogue
 
 // group-window plans (b1 only): every tail but the slice store
 template <int V>
@@ -219,6 +220,7 @@ int launch_imma_win_v(int out_type, Tail tail, const lce::ConvKParams& p, dim3 g
     case Tail::kGate: return launch_imma_vo<V, F, true, false, true, false, false, true>(p, grid, smem, s);
     case Tail::kScale: return launch_imma_vo<V, F, true, false, true, false, true, true>(p, grid, smem, s);
     case Tail::kSlice: return fail("bconv2d: the slice store takes no grouped plan with 32 * odd channels per group");
+    case Tail::kShuffle: return fail("bconv2d: the shuffle store takes no grouped plan");
     case Tail::kNone: break;
   }
   if (out_type == LCE_OUT_BITPACKED)
@@ -244,6 +246,10 @@ int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, d
   if (tail == Tail::kSlice) {
     if (b1) return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, false, true>(p, grid, smem, s);
     return launch_imma_vo<V, LCE_OUT_FLOAT, false, false, false, true>(p, grid, smem, s);
+  }
+  if (tail == Tail::kShuffle) {
+    if (!b1) return fail("bconv2d: the shuffle store needs the b1 inner product");
+    return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, false, false, false, false, true>(p, grid, smem, s);
   }
   if (b1) {
     if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, true>(p, grid, smem, s);
@@ -315,7 +321,8 @@ int launch_conv(GemmCore& c, lce::ConvKParams& p, cudaStream_t s, Tail tail = Ta
       default: return launch_imma_v<1>(c.out_type, c.imma_b1, tail, q, igrid, ismem, s);
     }
   }
-  if (tail != Tail::kNone) return fail("bconv2d: the chain, gate, scale and slice epilogues need the mma.sync kernel");
+  if (tail != Tail::kNone)
+    return fail("bconv2d: the chain, gate, scale, slice and shuffle epilogues need the mma.sync kernel");
   if (c.tc_ok) {
     // wgmma inner product: persistent 128 x BN tiles
     const int rc = tc_launch(c, p, s);
@@ -824,6 +831,23 @@ const char* slice_refusal(const lce_bconv2d_desc& d, const GemmCore* c) {
   return nullptr;
 }
 
+// What keeps a plan off lce_b200_bconv2d_run_fused_shuffle with an s_h x s_w shuffle, or nullptr: an
+// ungrouped 1x1 / stride 1 / dilation 1 plan with float output, no fused activation and no zero
+// padding, channels_out = s_h * s_w * C with C a multiple of 64, on the b1 mma.sync weight fragments.
+// c == nullptr: for a plan not created yet.
+const char* shuffle_refusal(const lce_bconv2d_desc& d, int s_h, int s_w, const GemmCore* c) {
+  if (d.out_type != LCE_OUT_FLOAT || d.activation != LCE_ACT_NONE) return "float output without a fused activation";
+  if (d.groups != 1 || d.filter_h != 1 || d.filter_w != 1 || d.stride_h != 1 || d.stride_w != 1 ||
+      d.dilation_h != 1 || d.dilation_w != 1 || (d.padding == LCE_PADDING_SAME && d.pad_value == 0))
+    return "an ungrouped 1x1 convolution with stride 1, dilation 1 and no zero padding";
+  if (s_h <= 0 || s_w <= 0 || d.channels_out % (s_h * s_w) != 0 || (d.channels_out / (s_h * s_w)) % lce::kBN != 0)
+    return "channels_out = s_h * s_w * C with C a multiple of 64";
+  const bool b1 = c != nullptr ? c->wt_nat != nullptr && c->imma_b1 && !c->imma_win
+                               : !env_off("LCE_B200_BCONV_IMMA") && !env_off("LCE_B200_BCONV_B1");
+  if (!b1) return "the b1 mma.sync inner product (LCE_B200_BCONV_IMMA / _B1 are 0)";
+  return nullptr;
+}
+
 // Whether lce_b200_bconv2d_run_fused / _run_fused_chain take packed output for the plan: every
 // ungrouped plan, and grouped float-output plans with channels_out / groups a multiple of 32 on the
 // b1 mma.sync weight fragments, whose epilogue packs whole 32-channel words of one CTA.
@@ -1226,7 +1250,8 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
                           const float* residual, int residual_act, int32_t* packed_out,
                           const lce_chain_desc* chain, void* stream,
                           const lce_gate_desc* gate = nullptr, int64_t out_stride = 0,
-                          float* scratch = nullptr, bool gate_per_position = false) {
+                          float* scratch = nullptr, bool gate_per_position = false,
+                          const lce::ConvKParams* shuffle = nullptr) {
   const lce_bconv2d_desc& d = plan->d;
   GemmCore& c = plan->core;
   cudaStream_t s = as_stream(stream);
@@ -1300,6 +1325,15 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     }
     return lce_b200_f32_gate_sign(out, gate, residual, residual_act, d.batch, pixels, c.cout, out,
                                   packed_out, stream);
+  }
+  if (shuffle != nullptr) {
+    // run_fused_shuffle (the caller checked that the b1 mma.sync kernel takes the plan): its shuf_*
+    // fields, and the signs' words per output pixel of C channels
+    p.shuf_sh = shuffle->shuf_sh; p.shuf_sw = shuffle->shuf_sw; p.shuf_c = shuffle->shuf_c;
+    p.shuf_act = shuffle->shuf_act; p.shuf_bias = shuffle->shuf_bias; p.shuf_k = shuffle->shuf_k;
+    p.cw_out = shuffle->shuf_c / 32;
+    if (!takes_imma(c, p)) return fail("bconv2d_run_fused_shuffle: the plan does not run on the mma.sync kernel");
+    return launch_conv(c, p, s, Tail::kShuffle);
   }
   // run_slice / run_slice_add: the mma.sync kernel's strided store, and the residual read at the
   // same strided address (the caller checked that the kernel takes the plan)
@@ -1500,6 +1534,49 @@ int lce_b200_bconv2d_run_slice_add(lce_b200_bconv2d* plan, const int32_t* in_dev
   }
   return bconv_run_impl(plan, in_dev, io_dev, io_dev, LCE_ACT_NONE, nullptr, nullptr, stream, nullptr,
                         io_pixel_stride, corr ? scratch_dev : nullptr);
+}
+
+int lce_b200_bconv2d_run_fused_shuffle(lce_b200_bconv2d* plan, const int32_t* in_dev, int s_h, int s_w,
+                                       const float* bias_dev, int activation, const float* skip_dev,
+                                       int add_activation, float* out_dev, int32_t* packed_out_dev,
+                                       void* stream) {
+  const lce_bconv2d_desc& d = plan->d;
+  if (const char* why = shuffle_refusal(d, s_h, s_w, &plan->core))
+    return fail("bconv2d_run_fused_shuffle: the plan needs %s", why);
+  for (int a : {activation, add_activation})
+    if (a < LCE_ACT_NONE || a > LCE_ACT_RELU6) return fail("bconv2d_run_fused_shuffle: unknown activation %d", a);
+  if (!aligned16(out_dev) || (skip_dev && !aligned16(skip_dev)) ||
+      (bias_dev && (reinterpret_cast<uintptr_t>(bias_dev) & 7u) != 0))
+    return fail("bconv2d_run_fused_shuffle: out and skip must be 16-byte aligned, bias 8-byte aligned");
+  if (bias_dev && !is_device_ptr(bias_dev)) return fail("bconv2d_run_fused_shuffle: bias must be device memory");
+  const long long px = static_cast<long long>(d.batch) * plan->out_h * plan->out_w;
+  if (px >= (1LL << 31) - lce::kIBM) return fail("bconv2d_run_fused_shuffle: too many input pixels (%lld)", px);
+  if (px == 0) return 0;
+  // the epilogue reads the skip and the input other CTAs' rows may land on: out must not alias them
+  const uintptr_t o0 = reinterpret_cast<uintptr_t>(out_dev);
+  const uintptr_t o1 = o0 + bconv_out_bytes(plan);   // px * s_h * s_w * C floats
+  auto overlaps = [&](const void* v, size_t bytes) {
+    const uintptr_t v0 = reinterpret_cast<uintptr_t>(v);
+    return v != nullptr && v0 < o1 && o0 < v0 + bytes;
+  };
+  if (overlaps(skip_dev, bconv_out_bytes(plan)) ||
+      overlaps(in_dev, static_cast<size_t>(px) * cdiv(d.channels_in, 32) * 4))
+    return fail("bconv2d_run_fused_shuffle: out must not overlap the skip or the input");
+  const lce::ConvKParams shuf = [&] {
+    lce::ConvKParams q;
+    memset(&q, 0, sizeof(q));
+    q.shuf_sh = s_h; q.shuf_sw = s_w; q.shuf_c = d.channels_out / (s_h * s_w);
+    q.shuf_act = activation; q.shuf_bias = bias_dev; q.shuf_k = d.channels_in;
+    return q;
+  }();
+  return bconv_run_impl(plan, in_dev, out_dev, skip_dev, add_activation, packed_out_dev, nullptr, stream, nullptr,
+                        0, nullptr, false, &shuf);
+}
+
+// host-internal (Graph::FuseBinaryTransposeConvs): lce_b200_bconv2d_run_fused_shuffle takes an s_h x s_w
+// shuffle of a plan created now from *d; no device needed
+int lce_b200_internal_shuffle_takes(const lce_bconv2d_desc* d, int s_h, int s_w) {
+  return shuffle_refusal(*d, s_h, s_w, nullptr) == nullptr;
 }
 
 // Whether lce_b200_bconv2d_run_slice will take a plan created now from *d

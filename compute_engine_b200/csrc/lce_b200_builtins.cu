@@ -1501,6 +1501,76 @@ __global__ void __launch_bounds__(256) depth_to_space_kernel(const float* __rest
   }
 }
 
+// TRANSPOSE_CONV (reference/transpose_conv.h) as a gather: output pixel (oy, ox) of phase
+// ((oy + pad_h) mod s_h, (ox + pad_w) mod s_w) is a stride-1 convolution over the input with only the
+// taps fy = oy + pad_h - iy * s_h, fx = ox + pad_w - ix * s_w that land in the filter. Each thread
+// computes one output pixel x 4 consecutive channels; consecutive threads take consecutive channel
+// groups of one pixel, so the input row is a broadcast and the stores are coalesced. Every output is
+// one fmaf chain from 0.0f over the taps in the reference's scatter order (input rows, then columns,
+// ascending) and, within a tap, the input channels ascending; then one __fadd_rn of the bias and the
+// activation, as the reference zeroes, accumulates, adds the bias and clamps. No atomics: the result
+// does not depend on scheduling. VEC4: in_c % 4 == 0 and 16-byte aligned input and filter.
+struct TConvGeom {
+  int B, H, W, Cin, KH, KW, Cout, OH, OW, sh, sw, ph, pw, act;
+};
+template <bool VEC4>
+__global__ void __launch_bounds__(256) transpose_conv_kernel(const float* __restrict__ in, const float* __restrict__ w,
+                                                             const float* __restrict__ bias, float* __restrict__ out,
+                                                             const TConvGeom g, long long total) {
+  const int groups = (g.Cout + 3) >> 2;
+  const long long step = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long t = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; t < total; t += step) {
+    const long long pix = t / groups;
+    const int co = static_cast<int>(t - pix * groups) * 4;
+    const long long by = pix / g.OW;
+    const int ox = static_cast<int>(pix - by * g.OW);
+    const long long b = by / g.OH;
+    const int oy = static_cast<int>(by - b * g.OH);
+    const int nq = min(4, g.Cout - co);
+    const int vy = oy + g.ph, vx = ox + g.pw;
+    // the input rows / columns whose tap lands in the filter: 0 <= v - i * s < K
+    const int ly = vy - g.KH + 1, lx = vx - g.KW + 1;
+    const int iy0 = ly <= 0 ? 0 : (ly + g.sh - 1) / g.sh, iy1 = min(vy / g.sh, g.H - 1);
+    const int ix0 = lx <= 0 ? 0 : (lx + g.sw - 1) / g.sw, ix1 = min(vx / g.sw, g.W - 1);
+    // filter rows of the thread's channels; a channel past Cout reads the last one and is not stored
+    const float* wr[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) wr[q] = w + static_cast<long long>(co + min(q, nq - 1)) * g.KH * g.KW * g.Cin;
+    float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    for (int iy = iy0; iy <= iy1; ++iy) {
+      const int fy = vy - iy * g.sh;
+      for (int ix = ix0; ix <= ix1; ++ix) {
+        const int fx = vx - ix * g.sw;
+        const float* xr = in + ((b * g.H + iy) * g.W + ix) * g.Cin;
+        const long long wo = (static_cast<long long>(fy) * g.KW + fx) * g.Cin;
+        if (VEC4) {
+          for (int ci = 0; ci < g.Cin; ci += 4) {
+            const float4 x = __ldg(reinterpret_cast<const float4*>(xr + ci));
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float4 f = __ldg(reinterpret_cast<const float4*>(wr[q] + wo + ci));
+              acc[q] = fmaf(x.x, f.x, acc[q]);
+              acc[q] = fmaf(x.y, f.y, acc[q]);
+              acc[q] = fmaf(x.z, f.z, acc[q]);
+              acc[q] = fmaf(x.w, f.w, acc[q]);
+            }
+          }
+        } else {
+          for (int ci = 0; ci < g.Cin; ++ci) {
+            const float x = __ldg(xr + ci);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) acc[q] = fmaf(x, __ldg(wr[q] + wo + ci), acc[q]);
+          }
+        }
+      }
+    }
+    float* o = out + pix * g.Cout + co;
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      if (q < nq) o[q] = apply_act(bias ? __fadd_rn(acc[q], __ldg(bias + co + q)) : acc[q], g.act);
+  }
+}
+
 // The sub-pixel tail of a super-resolution network,
 //   CONV_2D(x, KHxKW, stride 1, SAME) -> DEPTH_TO_SPACE(r) [-> ADD(RESIZE_BILINEAR(img))],
 // in one pass (Graph::FuseSubpixelConvs). A CTA computes BM low-resolution pixels x BN >= Cout conv
@@ -3147,6 +3217,31 @@ int lce_b200_f32_depth_to_space(const float* in, int batch, int in_h, int in_w, 
   if (vec) depth_to_space_kernel<4><<<grid, 256, 0, s>>>(in, out, in_h, in_w, channels, r, rows);
   else depth_to_space_kernel<1><<<grid, 256, 0, s>>>(in, out, in_h, in_w, channels, r, rows);
   return launch_check("depth_to_space_kernel");
+}
+
+int lce_b200_f32_transpose_conv2d(const lce_f32_transpose_conv_desc* d, const float* in, const float* filter,
+                                  const float* bias, float* out, void* stream) {
+  if (!d) return fail("transpose_conv2d: null descriptor");
+  const TConvGeom g{d->batch, d->in_h, d->in_w, d->in_c, d->filter_h, d->filter_w, d->out_c, d->out_h, d->out_w,
+                    d->stride_h, d->stride_w, d->pad_h, d->pad_w, d->activation};
+  if (g.B < 0 || g.H <= 0 || g.W <= 0 || g.Cin <= 0 || g.KH <= 0 || g.KW <= 0 || g.Cout <= 0 || g.OH <= 0 ||
+      g.OW <= 0)
+    return fail("transpose_conv2d: bad shape (input %d x %d x %d x %d, filter %d x %d x %d, output %d x %d)", g.B,
+                g.H, g.W, g.Cin, g.Cout, g.KH, g.KW, g.OH, g.OW);
+  if (g.sh <= 0 || g.sw <= 0) return fail("transpose_conv2d: strides must be positive");
+  if (g.ph < 0 || g.pw < 0) return fail("transpose_conv2d: padding must not be negative");
+  if (g.act < LCE_ACT_NONE || g.act > LCE_ACT_RELU6) return fail("transpose_conv2d: unknown activation %d", g.act);
+  if (static_cast<long long>(g.OH) + g.ph + g.KH >= INT_MAX || static_cast<long long>(g.OW) + g.pw + g.KW >= INT_MAX)
+    return fail("transpose_conv2d: the output is too large");
+  const long long total = static_cast<long long>(g.B) * g.OH * g.OW * ((g.Cout + 3) / 4);
+  if (total == 0) return 0;
+  if (!in || !filter || !out) return fail("transpose_conv2d: null tensor");
+  const bool vec = g.Cin % 4 == 0 && !((uintptr_t)in & 15) && !((uintptr_t)filter & 15);
+  cudaStream_t s = as_stream(stream);
+  const unsigned grid = grid_for(total, 256);
+  if (vec) transpose_conv_kernel<true><<<grid, 256, 0, s>>>(in, filter, bias, out, g, total);
+  else transpose_conv_kernel<false><<<grid, 256, 0, s>>>(in, filter, bias, out, g, total);
+  return launch_check("transpose_conv_kernel");
 }
 
 int lce_b200_subpixel_conv_max_out_channels(void) { return SubpixelTile<8, 8>::BN; }

@@ -353,21 +353,34 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // BITPACKED: the row's two output words, bit = acc > p.thr[c], packed like the float output's signs.
 // GW (group-window plans): the last tile may hold only 32 channels (channels_out % 64 == 32); its
 // upper half (ns 4..7, the second output word) is then neither read nor written.
+// SHUFFLE (float output, 1x1 plan, lce_b200_bconv2d_run_fused_shuffle): column (i * sw + j) * C + c of
+// row m = (b * OH + y) * OW + x goes to pixel ((b * OH + y) * sh + i) * OW * sw + x * sw + j of a
+// [B, OH * sh, OW * sw, C] map, C = p.shuf_c a multiple of 64, so the tile's 64 columns are one phase
+// (i, j)'s contiguous channels of that pixel; the shortcut and the signs are read and written there.
+// The plan's output transform is not applied: y = D = p.shuf_k - 2 popc(a ^ w), the +-1 dot product,
+// exact, then p.shuf_bias added with one rounding and p.shuf_act applied (TRANSPOSE_CONV's), then the
+// shortcut. No per-channel vectors stay in registers, which keeps the instance within the b1 cap.
 template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false, bool SPATIAL = false,
-          bool GW = false>
+          bool GW = false, bool SHUFFLE = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
                                               long long m0, int c_tile, int warp, int gid,
                                               int tig, const float* chain_s = nullptr) {
   static_assert(!(CHAIN && GATE), "one epilogue tail at a time");
   static_assert(!SPATIAL || GATE, "a spatial scale is the gate tail's");
   static_assert(!SLICE || (OUT == LCE_OUT_FLOAT && !CHAIN && !GATE), "a plain float slice");
+  static_assert(!SHUFFLE || (OUT == LCE_OUT_FLOAT && !CHAIN && !GATE && !SLICE && !GW), "a plain float shuffle");
   static_assert(OUT != LCE_OUT_BITPACKED || !(CHAIN || GATE || SLICE), "float tails only");
   constexpr bool STAGED = CHAIN || GATE;
   const int cth = c_tile + tig * 2;
+  // SHUFFLE: the tile's phase (si, sj) and first channel c_sh
+  const int phase = SHUFFLE ? c_tile / p.shuf_c : 0;
+  const int c_sh = SHUFFLE ? c_tile - phase * p.shuf_c : c_tile;
+  const int si = SHUFFLE ? phase / p.shuf_sw : 0;
+  const int sj = phase - si * p.shuf_sw;
   const bool hi = !GW || c_tile + 32 < p.cout;
   float2 mul_r[8], bias_r[8];
   int2 thr_r[8];
-  if (OUT == LCE_OUT_FLOAT && !STAGED) {
+  if (OUT == LCE_OUT_FLOAT && !STAGED && !SHUFFLE) {
 #pragma unroll
     for (int ns = 0; ns < 8; ++ns) {
       mul_r[ns] = *reinterpret_cast<const float2*>(p.mul + cth + ns * 8);
@@ -392,8 +405,17 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
       const int lrow = warp * 32 + ms * 16 + h * 8 + gid;
       const long long m = m0 + lrow;
       const bool row_ok = m < p.M;
-      const size_t e0 = SLICE ? static_cast<size_t>(m) * p.out_stride + cth
-                              : static_cast<size_t>(m) * p.cout + cth;
+      // SHUFFLE: the output pixel of row m (M < 2^31, host-checked)
+      long long opix = m;
+      if constexpr (SHUFFLE) {
+        const uint32_t yy = fdiv(static_cast<uint32_t>(m), p.fd_ow);   // b * OH + y
+        const long long x = m - static_cast<long long>(yy) * p.OW;
+        opix = (static_cast<long long>(yy) * p.shuf_sh + si) * (static_cast<long long>(p.OW) * p.shuf_sw) +
+               x * p.shuf_sw + sj;
+      }
+      const size_t e0 = SLICE     ? static_cast<size_t>(m) * p.out_stride + cth
+                        : SHUFFLE ? static_cast<size_t>(opix) * p.shuf_c + c_sh + tig * 2
+                                  : static_cast<size_t>(m) * p.cout + cth;
       if (OUT == LCE_OUT_RAW_ACC) {
         if (row_ok) {
           int* o = static_cast<int*>(p.out) + e0;
@@ -428,7 +450,10 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           } else {
             x0 <<= 1; x1 <<= 1;
           }
-          if constexpr (STAGED) {
+          if constexpr (SHUFFLE) {
+            y[2 * ns] = static_cast<float>(p.shuf_k - x0);
+            y[2 * ns + 1] = static_cast<float>(p.shuf_k - x1);
+          } else if constexpr (STAGED) {
             const float2 mu = *reinterpret_cast<const float2*>(chain_s + 4 * kBN + tig * 2 + ns * 8);
             const float2 bi = *reinterpret_cast<const float2*>(chain_s + 5 * kBN + tig * 2 + ns * 8);
             y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mu.x, bi.x);
@@ -437,6 +462,26 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
             y[2 * ns] = transform_float_x2(x0, p.clamp_min, p.clamp_max, mul_r[ns].x, bias_r[ns].x);
             y[2 * ns + 1] =
                 transform_float_x2(x1, p.clamp_min, p.clamp_max, mul_r[ns].y, bias_r[ns].y);
+          }
+        }
+        if constexpr (SHUFFLE) {
+          // TRANSPOSE_CONV's bias, one rounding, then its activation
+          if (p.shuf_bias != nullptr) {
+            const float* sb = p.shuf_bias + c_sh + tig * 2;
+#pragma unroll
+            for (int ns = 0; ns < 8; ++ns) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(sb + ns * 8));
+              y[2 * ns] = __fadd_rn(y[2 * ns], b.x);
+              y[2 * ns + 1] = __fadd_rn(y[2 * ns + 1], b.y);
+            }
+          }
+          const int sact = p.shuf_act;
+          if (sact != LCE_ACT_NONE) {
+            const float s_lo = sact == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
+            const float s_hi =
+                sact == LCE_ACT_RELU ? __int_as_float(0x7f800000) : (sact == LCE_ACT_RELU6 ? 6.0f : 1.0f);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], s_lo), s_hi);
           }
         }
         if constexpr (GATE) {
@@ -551,7 +596,7 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
         bits1 |= __shfl_xor_sync(0xffffffffu, bits1, 2);
         if (row_ok && tig == 0) {
           int32_t* pk = (OUT == LCE_OUT_BITPACKED ? static_cast<int32_t*>(p.out) : p.packed_out) +
-                        static_cast<size_t>(m) * p.cw_out + (c_tile >> 5);
+                        static_cast<size_t>(opix) * p.cw_out + (c_sh >> 5);
           pk[0] = static_cast<int32_t>(bits0);
           if (hi) pk[1] = static_cast<int32_t>(bits1);
         }
@@ -565,7 +610,8 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 // applies p.chain (lce_b200_bconv2d_run_fused_chain); GATE (float output): p.gate
 // (lce_b200_bconv2d_run_fused_gate), with SPATIAL p.gate indexed by position
 // (lce_b200_bconv2d_run_fused_scale); SLICE (float output): the strided store of
-// lce_b200_bconv2d_run_slice, and its read-add-write in lce_b200_bconv2d_run_slice_add. The other
+// lce_b200_bconv2d_run_slice, and its read-add-write in lce_b200_bconv2d_run_slice_add; SHUFFLE (b1,
+// float output): the pixel-shuffled store of lce_b200_bconv2d_run_fused_shuffle. The other
 // instances compile as without them.
 // GW (b1 only): a grouped plan whose groups hold 32 * odd output channels, so a 64-channel tile on
 // 64-aligned channels may span two groups. Tile nt covers channels nt * 64 .. nt * 64 + 63 and
@@ -575,10 +621,11 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 // window group's bits apart (compute_chunk_b1), so every channel gets popc(a ^ w) over its own
 // group alone: the XOR + POPC kernel's integers.
 template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
-          bool SPATIAL = false, bool GW = false>
+          bool SPATIAL = false, bool GW = false, bool SHUFFLE = false>
 __global__ void __launch_bounds__(kIThreads, B1 ? b1_ctas_per_sm(GW, OUT) : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
   static_assert(!GW || (B1 && !SLICE), "group windows: b1, no slice store");
+  static_assert(!SHUFFLE || B1, "the shuffle store: b1 only");
   using Vec = typename VecT<V>::T;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   // two buffers of { A: [Kc_v][128] packed vectors, B: [Kc_v*V][8][32] int8 fragments }, or for
@@ -621,7 +668,7 @@ bconv_imma_kernel(const ConvKParams p) {
       acc[ms][ns][2] = pw.x * 8; acc[ms][ns][3] = pw.y * 8;
     }
   }
-  if (OUT == LCE_OUT_FLOAT && !SLICE && p.residual != nullptr) {
+  if (OUT == LCE_OUT_FLOAT && !SLICE && !SHUFFLE && p.residual != nullptr) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const long long m = m0 + warp * 32 + i * 8 + gid;
@@ -729,7 +776,7 @@ bconv_imma_kernel(const ConvKParams p) {
     __syncthreads();
     epilogue_imma<OUT, S, false, true, false, SPATIAL, GW>(p, acc, m0, c_tile, warp, gid, tig, cs);
   } else {
-    epilogue_imma<OUT, S, false, false, SLICE, false, GW>(p, acc, m0, c_tile, warp, gid, tig);
+    epilogue_imma<OUT, S, false, false, SLICE, false, GW, SHUFFLE>(p, acc, m0, c_tile, warp, gid, tig);
   }
 }
 

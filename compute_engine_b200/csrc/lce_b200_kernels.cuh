@@ -101,6 +101,12 @@ struct ConvKParams {
   // SLICE instances only: output pixel m's cout floats start at out + m * out_stride, and so do
   // the residual's (lce_b200_bconv2d_run_slice, lce_b200_bconv2d_run_slice_add)
   long long out_stride;
+  // mma.sync kernel, SHUFFLE instances only (lce_b200_bconv2d_run_fused_shuffle): a 1x1 GEMM to
+  // shuf_sh * shuf_sw * shuf_c columns stored pixel-shuffled, out [B, OH * shuf_sh, OW * shuf_sw,
+  // shuf_c]; the +-1 dot product shuf_k - 2 popc (shuf_k = channels_in), shuf_bias (shuf_c floats, or
+  // nullptr) added and shuf_act applied before the shortcut ADD
+  int shuf_sh, shuf_sw, shuf_c, shuf_act, shuf_k;
+  const float* shuf_bias;
   // mma.sync kernel, group-window (GW) instances only: 8 % (2 * Cw_pg), a k-slice's step through
   // the window
   int win_step;

@@ -269,13 +269,21 @@ class HostGraph:
         allocate_tensors."""
         return lib().lce_host_fuse_subpixel_convs(self._g)
 
+    def fuse_binary_transpose_convs(self):
+        """LceDequantize -> TRANSPOSE_CONV (+-1 weights, kernel = stride) [-> ADD(skip)] [-> LceQuantize]
+        (a binary learned upsampler) => one node that runs it as a 1x1 binary convolution on the b1
+        tensor instruction and stores each column at its pixel-shuffled address. Call before
+        fuse_residual_blocks and allocate_tensors."""
+        return lib().lce_host_fuse_binary_transpose_convs(self._g)
+
     def fuse_residual_pairs(self):
         """Two consecutive LceBconv2d+ADD[+LceQuantize] blocks whose intermediate nothing else
         reads => one node that keeps it on chip. Call after the other fusions."""
         return lib().lce_host_fuse_residual_pairs(self._g)
 
     def fuse_all(self):
-        return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_residual_blocks()
+        return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_binary_transpose_convs()
+                + self.fuse_residual_blocks()
                 + self.fuse_spatial_scales()
                 + self.fuse_float_glue() + self.fuse_upsample_merges() + self.fuse_resize_argmax()
                 + self.fuse_subpixel_convs()

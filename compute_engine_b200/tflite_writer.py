@@ -113,12 +113,14 @@ OP = {"ADD": 0, "AVERAGE_POOL_2D": 1, "CONV_2D": 3, "DEPTHWISE_CONV_2D": 4,
       "SOFTMAX": 25, "MEAN": 40, "CUSTOM": 32, "CONCATENATION": 2, "PAD": 34, "PADV2": 60,
       "DEQUANTIZE": 6, "PRELU": 54, "LOGISTIC": 14, "STRIDED_SLICE": 45, "SPLIT": 49,
       "DIV": 42, "MAXIMUM": 55, "MINIMUM": 57, "ROUND": 116, "RESIZE_BILINEAR": 23,
-      "RESIZE_NEAREST_NEIGHBOR": 97, "ARG_MAX": 56, "DEPTH_TO_SPACE": 5}
+      "RESIZE_NEAREST_NEIGHBOR": 97, "ARG_MAX": 56, "DEPTH_TO_SPACE": 5,
+      "TRANSPOSE_CONV": 67}
 # BuiltinOptions union tags (schema_generated.h:1652-1694)
 OPT_TAG = {"CONV_2D": 1, "DEPTHWISE_CONV_2D": 2, "AVERAGE_POOL_2D": 5, "MAX_POOL_2D": 5,
            "FULLY_CONNECTED": 8, "SOFTMAX": 9, "ADD": 11, "MUL": 21, "RESHAPE": 17, "MEAN": 27,
            "CONCATENATION": 10, "PAD": 22, "PADV2": 43, "STRIDED_SLICE": 32, "SPLIT": 35, "DIV": 29,
-           "RESIZE_BILINEAR": 15, "RESIZE_NEAREST_NEIGHBOR": 74, "ARG_MAX": 40, "DEPTH_TO_SPACE": 94}
+           "RESIZE_BILINEAR": 15, "RESIZE_NEAREST_NEIGHBOR": 74, "ARG_MAX": 40, "DEPTH_TO_SPACE": 94,
+           "TRANSPOSE_CONV": 49}
 PADDING = {"SAME": 0, "VALID": 1}
 ACT = {"NONE": 0, "RELU": 1, "RELU_N1_TO_1": 2, "RELU6": 3}
 
@@ -186,6 +188,9 @@ class TFLiteModel:
             return fb.table({0: ("b", TENSOR_TYPE[np.dtype(o["output_type"])])})
         if kind == "DEPTH_TO_SPACE":  # DepthToSpaceOptions: block_size
             return fb.table({0: ("i", int(o["block_size"]))})
+        if kind == "TRANSPOSE_CONV":  # TransposeConvOptions: padding, stride_w, stride_h, fused activation
+            return fb.table({0: ("b", PADDING[o["padding"]]), 1: ("i", o["stride"][1]),
+                             2: ("i", o["stride"][0]), 3: ("b", act)})
         flags = [("b", 1) if o.get(f) else None for f in ("align_corners", "half_pixel_centers")]
         if kind == "RESIZE_BILINEAR":  # ResizeBilinearOptions (0, 1: the deprecated new_height / new_width)
             return fb.table({2: flags[0], 3: flags[1]})

@@ -144,6 +144,26 @@ class _Builder:
         self.m.add_op("RELU", [x], [y])
         return y
 
+    def transpose_conv(self, x, xs, out_shape, binary=False):
+        """TRANSPOSE_CONV 2x2 / stride 2 (SAME) from xs to out_shape with bias. binary: larq's
+        QuantConv2DTranspose(ste_sign, ste_sign) as the converter leaves it, LceQuantize -> LceDequantize
+        -> TRANSPOSE_CONV with +-1 weights."""
+        cin, cout = xs[3], out_shape[3]
+        if binary:
+            x = self.quantize(x, xs)
+            deq = self.act(xs)
+            self.m.add_op("LceDequantize", [x], [deq], custom_options=b"")
+            x = deq
+            wt = (self.rng.integers(0, 2, (cout, 2, 2, cin), dtype=np.int8) * 2 - 1).astype(np.float32)
+        else:
+            wt = self.rng.standard_normal((cout, 2, 2, cin)).astype(np.float32) * np.float32(1.0 / np.sqrt(cin))
+        bias = self.rng.uniform(-0.5, 0.5, cout).astype(np.float32)
+        y = self.act(out_shape)
+        self.m.add_op("TRANSPOSE_CONV", [self.const(np.array(out_shape, np.int32), np.int32, "output_shape"),
+                                         self.const(wt), x, self.const(bias, name="b")], [y],
+                      padding="SAME", stride=(2, 2), activation="NONE")
+        return y
+
     # ---- LCE custom ops ----
     def quantize(self, x, xs):
         b, h, w, c = xs
@@ -254,7 +274,8 @@ def _quicknet_encoder(g, batch, image, input_type, blocks, filters):
     return sections
 
 
-def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, decoder_blocks=2, labels=None):
+def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, decoder_blocks=2, labels=None,
+                 upsample="nearest"):
     """A binary segmentation network: QuickNet's encoder, then a decoder of three stages that merge
     the coarse map with the encoder's skip maps as TF2's UpSampling2D and Keras' Add emit them, then a
     per-pixel classifier at full resolution. Each stage, for (coarse, skip) = (s4, s3), (d3, s2),
@@ -265,7 +286,15 @@ def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, d
     logits [B, image, image, classes]. With labels="int64" or "int32" the head ends in ARG_MAX over
     the channel axis (the axis a constant int32 -1), as tf.argmax(logits, axis=-1) converts, and the
     output is the label map [B, image, image] of that type. image must be a multiple of 32 (the
-    encoder halves it five times and the decoder doubles it back)."""
+    encoder halves it five times and the decoder doubles it back).
+    upsample picks how each stage brings the coarse map to the skip's size and channels:
+    "nearest" the CONV_2D 1x1 -> RESIZE_NEAREST_NEIGHBOR above; "transpose" one float TRANSPOSE_CONV
+    2x2 / stride 2 with bias (Keras' Conv2DTranspose); "binary_transpose" larq's
+    QuantConv2DTranspose(ste_sign, ste_sign) as the converter leaves it without a binary transposed
+    op: LceQuantize -> LceDequantize -> TRANSPOSE_CONV 2x2 / stride 2 with +-1 weights and a bias."""
+    if upsample not in ("nearest", "transpose", "binary_transpose"):
+        raise ValueError(f"quicknet_seg upsample must be 'nearest', 'transpose' or 'binary_transpose', "
+                         f"not {upsample!r}")
     if image % 32:
         raise ValueError(f"quicknet_seg needs an image size that is a multiple of 32, not {image}")
     if labels not in (None, "int32", "int64"):
@@ -278,9 +307,12 @@ def quicknet_seg(batch=1, seed=0, image=224, input_type="float32", classes=21, d
         return g.const(np.array([h, w], np.int32), np.int32, "size")
 
     for skip, ss in reversed(sections[:-1]):
-        x, xs = g.conv(x, xs, ss[3], 1, 1)
-        up = g.act(ss)
-        g.m.add_op("RESIZE_NEAREST_NEIGHBOR", [x, size(ss[1], ss[2])], [up], half_pixel_centers=True)
+        if upsample == "nearest":
+            x, xs = g.conv(x, xs, ss[3], 1, 1)
+            up = g.act(ss)
+            g.m.add_op("RESIZE_NEAREST_NEIGHBOR", [x, size(ss[1], ss[2])], [up], half_pixel_centers=True)
+        else:
+            up = g.transpose_conv(x, xs, ss, binary=upsample == "binary_transpose")
         x, xs = g.add(up, skip, ss), ss
         for _ in range(decoder_blocks):
             q = g.quantize(x, xs)

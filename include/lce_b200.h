@@ -216,6 +216,22 @@ int lce_b200_bconv2d_run_slice(lce_b200_bconv2d* plan, const int32_t* in_dev, fl
  * refuses such a plan without a scratch. Other plans ignore scratch_dev, which may be NULL. */
 int lce_b200_bconv2d_run_slice_add(lce_b200_bconv2d* plan, const int32_t* in_dev, float* io_dev,
                                    int64_t io_pixel_stride, float* scratch_dev, void* stream);
+/* A binary learned upsampler, LceDequantize -> TRANSPOSE_CONV (+-1 weights, kernel = stride s_h x s_w)
+ * [-> ADD(skip)] [-> LceQuantize], as the 1x1 plan's GEMM to s_h * s_w * C columns in (i, j, c) order
+ * followed by a pixel shuffle in the store: GEMM row (b, y, x), column (i * s_w + j) * C + c goes to
+ * out[b, y * s_h + i, x * s_w + j, c], out [batch, in_h * s_h, in_w * s_w, C]. Per element:
+ *   t = act(D + bias[c]);  out = add_act(t + skip) (skip NULL: out = t);  packed_out = bitpack(out),
+ * D the +-1 dot product as an exact integer, one rounding for the bias (bias NULL: t = act(D)) and one
+ * for the skip, which is TFLite's TRANSPOSE_CONV and ADD bit for bit. D = channels_in - 2 popcount(a ^ w)
+ * comes from the accumulators: the plan's post_mul / post_bias are not applied. The plan must be an
+ * ungrouped 1x1 / stride 1 plan with float output, no fused activation and no zero padding,
+ * channels_out = s_h * s_w * C with C % 64 == 0, on the b1 mma.sync kernel
+ * (lce_b200_internal_shuffle_takes); bias holds C device floats, skip and out are [batch, in_h * s_h,
+ * in_w * s_w, C] and packed_out (may be NULL) [.., C / 32]. out must not overlap skip or the input. */
+int lce_b200_bconv2d_run_fused_shuffle(lce_b200_bconv2d* plan, const int32_t* in_dev, int s_h, int s_w,
+                                       const float* bias_dev, int activation, const float* skip_dev,
+                                       int add_activation, float* out_dev, int32_t* packed_out_dev,
+                                       void* stream);
 /* The signs of a dense layer's BatchNorm in one pass over a strided float [rows, channels] map
  * (row r starts at x_dev + r * x_pixel_stride):
  *   packed_out[r][ceil(channels/32)] = bitpack(x * scale[c] + shift[c]),
@@ -359,6 +375,13 @@ int lce_b200_f32_resize_bilinear_argmax(const float* in_dev, int batch, int in_h
  * the values are moved, not computed. Refuses block_size <= 0 and channels % r^2 != 0. */
 int lce_b200_f32_depth_to_space(const float* in_dev, int batch, int in_h, int in_w, int channels, int block_size,
                                 float* out_dev, void* stream);
+/* TFLite's float TRANSPOSE_CONV (TF/lite/kernels/internal/reference/transpose_conv.h) as a gather
+ * (lce_f32_transpose_conv_desc, lce_b200_types.h): each output is one fmaf chain from 0 over its taps in
+ * the reference's order, then the bias (may be NULL) added with one rounding, then the activation; no
+ * atomics, so the result is the same every run. */
+int lce_b200_f32_transpose_conv2d(const lce_f32_transpose_conv_desc* d, const float* in_dev,
+                                  const float* filter_dev, const float* bias_dev, float* out_dev,
+                                  void* stream);
 /* The largest out_c lce_b200_f32_subpixel_conv takes: every CTA computes all the conv's channels. */
 int lce_b200_subpixel_conv_max_out_channels(void);
 /* A super-resolution network's sub-pixel tail in one pass: lce_b200_f32_conv2d(d) (stride 1, dilation 1,

@@ -124,6 +124,20 @@ typedef struct lce_scale_desc {
   const float* sign_shift;
 } lce_scale_desc;
 
+/* One float TRANSPOSE_CONV (TF/lite/kernels/internal/reference/transpose_conv.h): input
+ * [batch, in_h, in_w, in_c], filter [out_c, filter_h, filter_w, in_c], output [batch, out_h, out_w,
+ * out_c]. Input pixel (iy, ix) and tap (fy, fx) reach output pixel (iy * stride_h - pad_h + fy,
+ * ix * stride_w - pad_w + fx); pad_h / pad_w are the floor half of the total padding TFLite computes
+ * for a convolution from the output's size back to the input's. */
+typedef struct lce_f32_transpose_conv_desc {
+  int32_t batch, in_h, in_w, in_c;
+  int32_t filter_h, filter_w, out_c;
+  int32_t out_h, out_w;
+  int32_t stride_h, stride_w;
+  int32_t pad_h, pad_w;
+  int32_t activation; /* LCE_ACT_* */
+} lce_f32_transpose_conv_desc;
+
 #ifdef __cplusplus
 }
 #endif
