@@ -100,6 +100,7 @@ EXPORTS = [
     "lce_b200_bconv2d_run_fused_pair",
     "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_fused_scale",
     "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add", "lce_b200_bconv2d_run_fused_shuffle",
+    "lce_b200_bconv2d_run_fused_fc",
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_scale_sign", "lce_b200_f32_logistic",
     "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
     "lce_b200_f32_maximum", "lce_b200_f32_minimum", "lce_b200_f32_div", "lce_b200_f32_round",
@@ -723,6 +724,29 @@ class BConv2d:
         _check(lib().lce_b200_bconv2d_run_fused_scale(self._h, _p(x), C.byref(desc), _p(res),
                                                       C.c_int(add_activation), _p(out), _p(pk),
                                                       _stream()))
+        return out, pk
+
+    def run_fused_fc(self, x: torch.Tensor, alpha=None, bias=None, activation=0, scale=None, shift=None,
+                     bn_activation=0, packed=True):
+        """lce_b200_bconv2d_run_fused_fc: a binary dense layer on packed x [rows, ceil(K / 32)] (a 1x1 plan
+        with in_h = in_w = 1 and channels_in = K; rows re-plans the batch). Per column c of N:
+        y = activation(fl(fl(alpha[c] * D) + bias[c])), then bn_activation(fl(fl(y * scale[c]) + shift[c])),
+        D the exact +-1 dot product; each vector [N] may be None. Returns (float out [rows, N], packed
+        signs [rows, N / 32] | None)."""
+        x = _dev(x, torch.int32)
+        rows = x.shape[0]
+        if x.dim() != 2 or x.shape[1] != cdiv(self.desc.channels_in, 32):
+            raise LceError("run_fused_fc: x must be packed rows [rows, ceil(channels_in / 32)]")
+        if (rows, self.desc.in_h, self.desc.in_w) != (self.desc.batch, 1, 1):
+            self.set_input_shape(rows, 1, 1)
+        n = self.desc.channels_out
+        vecs = [None if v is None else torch.as_tensor(v, dtype=torch.float32, device=x.device).contiguous()
+                for v in (alpha, bias, scale, shift)]
+        out = torch.empty((rows, n), dtype=torch.float32, device=x.device)
+        pk = torch.empty((rows, cdiv(n, 32)), dtype=torch.int32, device=x.device) if packed else None
+        _check(lib().lce_b200_bconv2d_run_fused_fc(self._h, _p(x), _p(vecs[0]), _p(vecs[1]), C.c_int(activation),
+                                                   _p(vecs[2]), _p(vecs[3]), C.c_int(bn_activation), _p(out),
+                                                   _p(pk), _stream()))
         return out, pk
 
     def run_slice(self, x: torch.Tensor, out: torch.Tensor, offset: int = 0):

@@ -259,7 +259,7 @@ TfLiteStatus PoolInvoke(TfLiteContext* c, TfLiteNode* n) {
 // --------------- fused MAX_POOL_2D -> MUL(scale) -> ADD(shift) -> LceQuantize --------------- //
 // Created by Graph::FusePooledSigns; builtin_data = the pool's BuiltinParams; inputs [x, scale,
 // shift], each constant [C] (or [1, ..., 1, C]) for x [B,H,W,C]; output the packed signs
-// [B,OH,OW,ceil(C/32)].
+// [B,OH,OW,ceil(C/32)], or [B, OH*OW*C/32] when the pass looked through a flattening RESHAPE.
 TfLiteStatus PooledSignPrepare(TfLiteContext* c, TfLiteNode* n) {
   lce_f32_pool_desc d;
   B_ENSURE(c, n->inputs->size == 3 && PoolDesc(c, n, &d) && T(c, n->inputs, 0)->type == kTfLiteFloat32,
@@ -273,6 +273,8 @@ TfLiteStatus PooledSignPrepare(TfLiteContext* c, TfLiteNode* n) {
   B_ENSURE(c, pk && pk->type == kTfLiteInt32, "MAX_POOL_2D+MUL+ADD+LceQuantize: packed output must be int32");
   int oh, ow;
   B_CAPI(c, lce_b200_f32_pool_out_shape(&d, &oh, &ow));
+  // through a flattening RESHAPE (C % 32 == 0): the same words as [B, OH * OW * C / 32]
+  if (pk->dims->size == 2) return Resize(c, pk, {d.batch, oh * ow * (d.channels / 32)});
   return Resize(c, pk, {d.batch, oh, ow, (d.channels + 31) / 32});
 }
 TfLiteStatus PooledSignInvoke(TfLiteContext* c, TfLiteNode* n) {
@@ -1245,6 +1247,86 @@ TfLiteStatus BinaryTConvInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// --- fused LceDequantize -> FULLY_CONNECTED (+-alpha) [-> MUL -> ADD] [-> LceQuantize]: a binary dense layer --- //
+// Created by Graph::FuseBinaryFullyConnected; builtin_data = BinaryFcParams; inputs [q (packed signs whose
+// words are the rows' words, ceil(K / 32) per row), filter (the weights' signs as a packed 1x1 LceBconv2d
+// filter [N, 1, 1, ceil(K / 32)]), alpha ([N] or -1), bias, scale, shift ([N] or -1)], outputs [result
+// [rows, N], packed signs [rows, N / 32]?]. rows follow q's size, so a batch resize re-plans them. The
+// node owns a 1x1 LceBconv2d plan of rows x 1 x 1 and runs lce_b200_bconv2d_run_fused_fc.
+struct BinaryFcParams {
+  BuiltinParams fc, add;
+  int32_t channels_in;
+};
+struct BinaryFcOp {
+  BinaryFcParams p;
+  lce_b200_bconv2d* plan = nullptr;
+};
+void* BinaryFcInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* op = new BinaryFcOp();
+  memset(&op->p, 0, sizeof(op->p));
+  if (buffer && length >= sizeof(BinaryFcParams)) memcpy(&op->p, buffer, sizeof(BinaryFcParams));
+  return op;
+}
+void BinaryFcFree(TfLiteContext*, void* p) {
+  auto* op = static_cast<BinaryFcOp*>(p);
+  lce_b200_bconv2d_destroy(op->plan);
+  delete op;
+}
+TfLiteStatus BinaryFcPrepare(TfLiteContext* c, TfLiteNode* n) {
+  auto* op = static_cast<BinaryFcOp*>(n->user_data);
+  const int K = op->p.channels_in;
+  B_ENSURE(c, n->inputs->size == 6 && n->outputs->size >= 1 && n->outputs->size <= 2 && K > 0,
+           "LceBfc: inputs [q, filter, alpha, bias, scale, shift] and one or two outputs expected");
+  const TfLiteTensor* q = T(c, n->inputs, 0);
+  const TfLiteTensor* f = T(c, n->inputs, 1);
+  const int cw = (K + 31) / 32;
+  B_ENSURE(c, q && q->type == kTfLiteInt32 && q->dims->size >= 1 && Count(q) % cw == 0,
+           "LceBfc: the input must be packed signs of whole rows of ceil(K / 32) words");
+  B_ENSURE(c, f && f->type == kTfLiteInt32 && f->allocation_type == kTfLiteMmapRo && f->dims->size == 4 &&
+                  f->dims->data[1] == 1 && f->dims->data[2] == 1 && f->dims->data[3] == cw,
+           "LceBfc: the filter must be a constant packed [N, 1, 1, ceil(K / 32)]");
+  const int N = f->dims->data[0];
+  for (int k = 2; k < 6; ++k) {
+    const TfLiteTensor* v = T(c, n->inputs, k);
+    B_ENSURE(c, !v || (v->type == kTfLiteFloat32 && v->allocation_type == kTfLiteMmapRo && Count(v) == N),
+             "LceBfc: alpha, bias, scale and shift must be constant float32 [N]");
+  }
+  const int64_t rows = Count(q) / cw;
+  B_ENSURE(c, rows <= INT32_MAX, "LceBfc: too many rows");
+  if (Resize(c, T(c, n->outputs, 0), {static_cast<int>(rows), N}) != kTfLiteOk) return kTfLiteError;
+  if (n->outputs->size == 2) {
+    TfLiteTensor* pk = T(c, n->outputs, 1);
+    B_ENSURE(c, pk && pk->type == kTfLiteInt32, "LceBfc+LceQuantize: packed output must be int32");
+    if (Resize(c, pk, {static_cast<int>(rows), (N + 31) / 32}) != kTfLiteOk) return kTfLiteError;
+  }
+  if (op->plan) {
+    B_CAPI(c, lce_b200_bconv2d_set_input_shape(op->plan, static_cast<int>(rows), 1, 1));
+    return kTfLiteOk;
+  }
+  lce_bconv2d_desc d;
+  memset(&d, 0, sizeof(d));
+  d.batch = static_cast<int>(rows); d.in_h = 1; d.in_w = 1; d.channels_in = K;
+  d.filter_h = 1; d.filter_w = 1; d.channels_out = N; d.groups = 1;
+  d.stride_h = 1; d.stride_w = 1; d.dilation_h = 1; d.dilation_w = 1;
+  d.padding = LCE_PADDING_VALID; d.pad_value = 1; d.activation = LCE_ACT_NONE; d.out_type = LCE_OUT_FLOAT;
+  const std::vector<float> ones(N, 1.0f), zeros(N, 0.0f);
+  B_CAPI(c, lce_b200_bconv2d_create(&d, f->data.i32, ones.data(), zeros.data(), nullptr, &op->plan));
+  return kTfLiteOk;
+}
+TfLiteStatus BinaryFcInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const auto* op = static_cast<const BinaryFcOp*>(n->user_data);
+  auto vec = [&](int k) -> const float* {
+    const TfLiteTensor* v = T(c, n->inputs, k);
+    return v ? v->data.f : nullptr;
+  };
+  TfLiteTensor* pk = n->outputs->size > 1 ? T(c, n->outputs, 1) : nullptr;
+  B_CAPI(c, lce_b200_bconv2d_run_fused_fc(op->plan, T(c, n->inputs, 0)->data.i32, vec(2), vec(3),
+                                          op->p.fc.activation, vec(4), vec(5), op->p.add.activation,
+                                          T(c, n->outputs, 0)->data.f, pk ? pk->data.i32 : nullptr,
+                                          lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // ------------------------------ CONCATENATION ------------------------------ //
 // Strided device copies (one cudaMemcpy2DAsync per input): no kernel of ours.
 TfLiteStatus ConcatPrepare(TfLiteContext* c, TfLiteNode* n) {
@@ -1589,6 +1671,10 @@ const TfLiteRegistration* ResizeArgmaxRegistration() {
 }
 const TfLiteRegistration* BinaryTransposeConvRegistration() {
   static TfLiteRegistration r = {BinaryTConvInit, BinaryTConvFree, BinaryTConvPrepare, BinaryTConvInvoke};
+  return &r;
+}
+const TfLiteRegistration* BinaryFullyConnectedRegistration() {
+  static TfLiteRegistration r = {BinaryFcInit, BinaryFcFree, BinaryFcPrepare, BinaryFcInvoke};
   return &r;
 }
 const TfLiteRegistration* SubpixelConvRegistration() {

@@ -317,6 +317,7 @@ constexpr const char* kArgMax = "builtin:56";
 constexpr const char* kDepthToSpace = "builtin:5";
 constexpr const char* kTransposeConv = "builtin:67";
 constexpr const char* kMul = "builtin:18";
+constexpr const char* kReshape = "builtin:22";
 constexpr const char* kRelu = "builtin:19";
 constexpr const char* kMean = "builtin:40";
 constexpr const char* kDiv = "builtin:42";
@@ -1067,13 +1068,31 @@ int Graph::FusePooledSigns() {
     const size_t ka = SoleConsumer(t1);
     const int shift = PerChannelConstOp(ka, kAdd, t1, C);
     if (shift < 0 || ka <= km) continue;
-    const size_t kq = SoleConsumer(nodes_[ka]->node.outputs->data[0]);
-    if (!IsQuantize(kq) || kq <= ka) continue;
+    // larq's Flatten -> QuantDense: ADD -> RESHAPE [B, OH * OW * C] -> LceQuantize. With C % 32 == 0 the
+    // flattened map packs to the map's own words, so the node writes them as [B, OH * OW * C / 32].
+    const int t2 = nodes_[ka]->node.outputs->data[0];
+    size_t kq = SoleConsumer(t2), kr = kNoNode;
+    if (kq != kNoNode && nodes_[kq]->name == kReshape && !nodes_[kq]->initialized && C % 32 == 0 &&
+        nodes_[kq]->node.inputs->size >= 1 && nodes_[kq]->node.inputs->data[0] == t2 &&
+        nodes_[kq]->node.outputs->size == 1) {
+      const int r = nodes_[kq]->node.outputs->data[0];
+      const TfLiteIntArray* yd = tensors_[y].dims;
+      const TfLiteIntArray* rd = tensors_[r].dims;
+      if (tensors_[r].type == kTfLiteFloat32 && yd && yd->size == 4 && rd && rd->size == 2 &&
+          rd->data[0] == yd->data[0] &&
+          static_cast<int64_t>(rd->data[1]) == static_cast<int64_t>(yd->data[1]) * yd->data[2] * yd->data[3]) {
+        kr = kq;
+        kq = SoleConsumer(r);
+      }
+    }
+    if (!IsQuantize(kq) || kq <= (kr != kNoNode ? kr : ka)) continue;
     SetNodeIO(p, {x, scale, shift}, {nodes_[kq]->node.outputs->data[0]});
     p.registration = PooledSignRegistration();   // builtin_data stays the pool's parameters
-    p.name = "MAX_POOL_2D+MUL+ADD+LceQuantize";
-    EraseNodes({km, ka, kq});
-    removed += 3;
+    p.name = kr != kNoNode ? "MAX_POOL_2D+MUL+ADD+RESHAPE+LceQuantize" : "MAX_POOL_2D+MUL+ADD+LceQuantize";
+    std::vector<size_t> gone{km, ka, kq};
+    if (kr != kNoNode) gone.push_back(kr);
+    EraseNodes(gone);
+    removed += static_cast<int>(gone.size());
   }
   allocated_ = false;
   return removed;
@@ -2001,6 +2020,147 @@ int Graph::FuseBinaryTransposeConvs() {
     f.name = std::string("LceBconv2dTranspose") + (ai != kNoNode ? "+ADD" : "") + (tail ? "+LceQuantize" : "");
     std::vector<size_t> gone{di};
     if (ai != kNoNode) gone.push_back(i);
+    if (tail) gone.push_back(kq);
+    EraseNodes(gone);
+    return static_cast<int>(gone.size());
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size();) {
+    const int k = fuse(i);
+    removed += k;
+    i = k > 0 ? 0 : i + 1;   // indices moved: scan again (a fused node no longer matches)
+  }
+  allocated_ = false;
+  return removed;
+}
+
+const TfLiteRegistration* BinaryFullyConnectedRegistration();   // builtin_ops.cc
+extern "C" int lce_b200_internal_fc_takes(const lce_bconv2d_desc* d);   // lce_b200.cu
+
+int Graph::FuseBinaryFullyConnected() {
+  if (!device_arena_) return 0;
+  // a constant float32 [n] (exactly rank 1), or -1
+  auto vec = [&](int t, int n) {
+    return t >= 0 && tensors_[t].type == kTfLiteFloat32 && tensors_[t].allocation_type == kTfLiteMmapRo &&
+                   tensors_[t].dims && tensors_[t].dims->size == 1 && tensors_[t].dims->data[0] == n
+               ? t
+               : -1;
+  };
+  auto count = [](const TfLiteIntArray* d) {
+    int64_t n = 1;
+    for (int k = 0; k < d->size; ++k) n *= d->data[k];
+    return n;
+  };
+  auto fuse = [&](size_t i) -> int {   // nodes removed by fusing the FULLY_CONNECTED at i, 0 when it stays
+    NodeRecord& fc = *nodes_[i];
+    const BuiltinParams* fp = Params(fc);
+    if (fc.name != kFullyConnected || fc.initialized || !fp || fc.node.inputs->size < 2 || fc.node.inputs->size > 3 ||
+        fc.node.outputs->size != 1)
+      return 0;
+    const int x = fc.node.inputs->data[0], w = fc.node.inputs->data[1], y = fc.node.outputs->data[0];
+    const int bias_in = fc.node.inputs->size == 3 ? fc.node.inputs->data[2] : -1;
+    if (x < 0 || w < 0 || tensors_[w].type != kTfLiteFloat32 || tensors_[w].allocation_type != kTfLiteMmapRo ||
+        tensors_[x].type != kTfLiteFloat32 || tensors_[y].type != kTfLiteFloat32 || fp->keep_dims != 0 ||
+        fp->activation < LCE_ACT_NONE || fp->activation > LCE_ACT_RELU6)
+      return 0;
+    const TfLiteIntArray* wd = tensors_[w].dims;
+    const TfLiteIntArray* xd = tensors_[x].dims;
+    if (!wd || wd->size != 2 || !xd || xd->size < 1 || wd->data[0] <= 0 || wd->data[1] <= 0) return 0;
+    const int N = wd->data[0], K = wd->data[1];
+    const int bias = vec(bias_in, N);
+    if (bias_in >= 0 && bias < 0) return 0;
+    // every row o exactly +-alpha_o: one positive, finite magnitude, bitwise, in the whole row (no 0.0 or
+    // -0.0, no 0.5 among 1.0s)
+    const size_t nw = static_cast<size_t>(N) * K;
+    if (const_host_[w].size() < nw * sizeof(float)) return 0;
+    std::vector<uint32_t> wb(nw);
+    memcpy(wb.data(), const_host_[w].data(), nw * sizeof(float));
+    std::vector<float> alpha(N);
+    bool unit = true;
+    for (int o = 0; o < N; ++o) {
+      const uint32_t mag = wb[static_cast<size_t>(o) * K] & 0x7fffffffu;
+      if (mag == 0 || mag >= 0x7f800000u) return 0;
+      for (int k = 1; k < K; ++k)
+        if ((wb[static_cast<size_t>(o) * K + k] & 0x7fffffffu) != mag) return 0;
+      memcpy(&alpha[o], &mag, sizeof(float));
+      unit = unit && mag == 0x3f800000u;
+    }
+    // x: an LceDequantize of packed signs q, read by the FULLY_CONNECTED alone
+    size_t di = kNoNode;
+    for (size_t k = 0; k < i && di == kNoNode; ++k)
+      if (nodes_[k]->node.outputs->size == 1 && nodes_[k]->node.outputs->data[0] == x) di = k;
+    if (di == kNoNode || SoleConsumer(x) != i) return 0;
+    const NodeRecord& dq = *nodes_[di];
+    const int q = dq.node.inputs->size == 1 ? dq.node.inputs->data[0] : -1;
+    if (dq.name != "LceDequantize" || dq.initialized || q < 0 || tensors_[q].type != kTfLiteInt32) return 0;
+    // q's words are the rows' words: each row is x's last axis (any K), or whole words of a map whose
+    // last axis packs without a padded word (C % 32 == 0, K % 32 == 0)
+    const TfLiteIntArray* qd = tensors_[q].dims;
+    const int last = xd->data[xd->size - 1];
+    if (!qd || qd->size != xd->size || qd->data[qd->size - 1] != (last + 31) / 32) return 0;
+    for (int k = 0; k + 1 < xd->size; ++k)
+      if (qd->data[k] != xd->data[k]) return 0;
+    if (last != K && (last % 32 != 0 || K % 32 != 0)) return 0;
+    const int64_t elems = count(xd);
+    if (elems % K != 0 || elems / K > INT32_MAX) return 0;
+    lce_bconv2d_desc d;
+    memset(&d, 0, sizeof(d));
+    d.batch = static_cast<int>(elems / K); d.in_h = 1; d.in_w = 1; d.channels_in = K;
+    d.filter_h = 1; d.filter_w = 1; d.channels_out = N; d.groups = 1;
+    d.stride_h = 1; d.stride_w = 1; d.dilation_h = 1; d.dilation_w = 1;
+    d.padding = LCE_PADDING_VALID; d.pad_value = 1; d.activation = LCE_ACT_NONE; d.out_type = LCE_OUT_FLOAT;
+    if (!lce_b200_internal_fc_takes(&d)) return 0;   // N % 64 == 0, the b1 mma.sync kernel
+    // the BatchNorm: MUL(scale [N]) as y's one reader, then ADD(shift [N]) as the product's one reader
+    size_t km = SoleConsumer(y), ka = kNoNode;
+    int scale = vec(PerChannelConstOp(km, kMul, y, N), N), shift = -1;
+    if (scale >= 0 && km > i) {
+      const int t1 = nodes_[km]->node.outputs->data[0];
+      ka = SoleConsumer(t1);
+      shift = vec(PerChannelConstOp(ka, kAdd, t1, N, /*any_activation=*/true), N);
+      if (shift < 0 || ka <= km || Activation(*nodes_[ka]) < LCE_ACT_NONE || Activation(*nodes_[ka]) > LCE_ACT_RELU6)
+        ka = kNoNode;
+    }
+    if (ka == kNoNode) {
+      km = kNoNode;
+      scale = shift = -1;
+    }
+    const int s = ka != kNoNode ? nodes_[ka]->node.outputs->data[0] : y;
+    // the signs: the result's only LceQuantize reader; the result itself stays stored
+    size_t kq = kNoNode;
+    int quantizers = 0;
+    for (size_t k : Consumers(s))
+      if (nodes_[k]->name == "LceQuantize") { ++quantizers; kq = k; }
+    const bool tail = quantizers == 1 && IsQuantize(kq) && kq > (ka != kNoNode ? ka : i);
+    std::vector<int> outs{s};
+    if (tail) outs.push_back(nodes_[kq]->node.outputs->data[0]);
+    // the filter: each weight's sign bit, ceil(K / 32) words per output row
+    const int cw = (K + 31) / 32;
+    std::vector<int32_t> filt(static_cast<size_t>(N) * cw, 0);
+    for (int o = 0; o < N; ++o)
+      for (int k = 0; k < K; ++k)
+        if (wb[static_cast<size_t>(o) * K + k] >> 31) filt[static_cast<size_t>(o) * cw + (k >> 5)] |= static_cast<int32_t>(1u << (k & 31));
+    const int ft = AddTensor(kTfLiteInt32, {N, 1, 1, cw}, filt.data(), filt.size() * sizeof(int32_t), false, 0.0f, 0,
+                             names_[w] + "_packed", /*const_on_device=*/true);
+    // alpha = 1.0 everywhere multiplies by nothing: the node reads no vector for it
+    const int at = unit ? -1
+                        : AddTensor(kTfLiteFloat32, {N}, alpha.data(), alpha.size() * sizeof(float), false, 0.0f, 0,
+                                    names_[w] + "_alpha", /*const_on_device=*/true);
+    struct {
+      BuiltinParams fc, add;
+      int32_t channels_in;
+    } params{*fp, ka != kNoNode ? *Params(*nodes_[ka]) : BuiltinParams{}, K};
+    // the ADD's node (or without it the FULLY_CONNECTED's) becomes the fused one: q exists where it runs,
+    // and every reader of the result and of the signs comes after it
+    NodeRecord& f = ka != kNoNode ? *nodes_[ka] : fc;
+    SetNodeIO(f, {q, ft, at, bias, scale, shift}, outs);
+    SetBuiltinBlob(f, &params, sizeof(params));
+    f.registration = BinaryFullyConnectedRegistration();
+    f.name = std::string("LceBfc") + (ka != kNoNode ? "+MUL+ADD" : "") + (tail ? "+LceQuantize" : "");
+    std::vector<size_t> gone{di};
+    if (ka != kNoNode) {
+      gone.push_back(i);
+      gone.push_back(km);
+    }
     if (tail) gone.push_back(kq);
     EraseNodes(gone);
     return static_cast<int>(gone.size());

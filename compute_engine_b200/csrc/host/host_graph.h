@@ -303,6 +303,28 @@ class Graph {
   // it matches a TRANSPOSE_CONV, its ADD or its LceQuantize. Returns the nodes removed.
   int FuseBinaryTransposeConvs();
 
+  // A binary dense layer, as a larq QuantDense(ste_sign, ste_sign) converts (LCE has no binary dense op),
+  //   LceDequantize(q) -> FULLY_CONNECTED(+-alpha_o weights, bias?, activation)
+  //   [-> MUL(scale [N]) -> ADD(shift [N], activation)] [-> LceQuantize]
+  // becomes one node (lce_b200_bconv2d_run_fused_fc) that reads q's packed words and runs the layer as
+  // a 1x1 binary convolution of rows = the FULLY_CONNECTED's rows on the b1 mma.sync kernel, applying
+  // alpha, the bias, the activation, the BatchNorm and its activation to the exact +-1 dot product D in
+  // its store and packing the signs: "LceBfc[+MUL+ADD][+LceQuantize]", inputs [q, packed filter (a new
+  // constant), alpha (a new constant [N], -1 when every alpha_o is 1.0), bias, scale, shift (-1 when
+  // absent)], outputs [result, signs?]. The result is always stored. Only when every row o of the
+  // constant [N, K] weights is exactly +-alpha_o with one positive finite magnitude bitwise (no 0.0 or
+  // -0.0), the bias is a constant float32 [N], N % 64 == 0 and the plan lands on the b1 mma.sync kernel
+  // (lce_b200_internal_fc_takes), the dequantized map is read by the FULLY_CONNECTED alone and is not a
+  // graph output, and q's words are the rows' words (x's last axis is K, or it is a multiple of 32 and
+  // so is K). The MUL and ADD join only as the sole readers of the previous result with constant
+  // float32 [N] operands; the LceQuantize when it is the result's only sign reader. Otherwise the graph
+  // is left as it is. Each step rounds as TFLite's ops do, so with every alpha_o a power of two (1.0
+  // included) it is bit-identical; otherwise fl(fl(alpha * D) + b) is the real value rounded twice
+  // where TFLite's loop rounds after each of its K terms: the two differ by up to about
+  // K * 2^-24 * K * alpha_o, which can flip the next sign at a near-tie. fuse_all runs it right after
+  // FuseBinaryTransposeConvs; no pass before it matches a FULLY_CONNECTED. Returns the nodes removed.
+  int FuseBinaryFullyConnected();
+
   // init (first time) + prepare of every node in order, then arena allocation.
   TfLiteStatus AllocateTensors();
   TfLiteStatus ResizeInputTensor(int tensor, const std::vector<int>& dims);

@@ -1331,8 +1331,10 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     // fields, and the signs' words per output pixel of C channels
     p.shuf_sh = shuffle->shuf_sh; p.shuf_sw = shuffle->shuf_sw; p.shuf_c = shuffle->shuf_c;
     p.shuf_act = shuffle->shuf_act; p.shuf_bias = shuffle->shuf_bias; p.shuf_k = shuffle->shuf_k;
+    p.shuf_alpha = shuffle->shuf_alpha; p.shuf_scale = shuffle->shuf_scale; p.shuf_shift = shuffle->shuf_shift;
+    p.shuf_act2 = shuffle->shuf_act2;
     p.cw_out = shuffle->shuf_c / 32;
-    if (!takes_imma(c, p)) return fail("bconv2d_run_fused_shuffle: the plan does not run on the mma.sync kernel");
+    if (!takes_imma(c, p)) return fail("bconv2d_run_fused_shuffle / _fc: the plan does not run on the mma.sync kernel");
     return launch_conv(c, p, s, Tail::kShuffle);
   }
   // run_slice / run_slice_add: the mma.sync kernel's strided store, and the residual read at the
@@ -1578,6 +1580,59 @@ int lce_b200_bconv2d_run_fused_shuffle(lce_b200_bconv2d* plan, const int32_t* in
 int lce_b200_internal_shuffle_takes(const lce_bconv2d_desc* d, int s_h, int s_w) {
   return shuffle_refusal(*d, s_h, s_w, nullptr) == nullptr;
 }
+
+// What keeps a plan off lce_b200_bconv2d_run_fused_fc, or nullptr: the shuffle store's plan with s_h =
+// s_w = 1 (channels_out % 64 == 0, the b1 mma.sync kernel) on a 1 x 1 input, so that its rows are the
+// dense layer's rows.
+static const char* fc_refusal(const lce_bconv2d_desc& d, const GemmCore* c) {
+  if (d.in_h != 1 || d.in_w != 1) return "in_h = in_w = 1 (one row per image)";
+  return shuffle_refusal(d, 1, 1, c);
+}
+
+int lce_b200_bconv2d_run_fused_fc(lce_b200_bconv2d* plan, const int32_t* in_dev, const float* alpha_dev,
+                                  const float* bias_dev, int activation, const float* scale_dev,
+                                  const float* shift_dev, int bn_activation, float* out_dev,
+                                  int32_t* packed_out_dev, void* stream) {
+  const lce_bconv2d_desc& d = plan->d;
+  if (const char* why = fc_refusal(d, &plan->core)) return fail("bconv2d_run_fused_fc: the plan needs %s", why);
+  for (int a : {activation, bn_activation})
+    if (a < LCE_ACT_NONE || a > LCE_ACT_RELU6) return fail("bconv2d_run_fused_fc: unknown activation %d", a);
+  if (!aligned16(out_dev)) return fail("bconv2d_run_fused_fc: out must be 16-byte aligned");
+  for (const float* v : {alpha_dev, bias_dev, scale_dev, shift_dev}) {
+    if (v && (reinterpret_cast<uintptr_t>(v) & 7u) != 0)
+      return fail("bconv2d_run_fused_fc: alpha, bias, scale and shift must be 8-byte aligned");
+    if (v && !is_device_ptr(v)) return fail("bconv2d_run_fused_fc: alpha, bias, scale and shift must be device memory");
+  }
+  const long long rows = d.batch;
+  if (rows >= (1LL << 31) - lce::kIBM) return fail("bconv2d_run_fused_fc: too many rows (%lld)", rows);
+  if (rows == 0) return 0;
+  // other CTAs read the input rows this CTA's store may land on
+  const uintptr_t o0 = reinterpret_cast<uintptr_t>(out_dev);
+  const uintptr_t o1 = o0 + bconv_out_bytes(plan);   // rows * N floats
+  const size_t in_bytes = static_cast<size_t>(rows) * cdiv(d.channels_in, 32) * 4;
+  const size_t pk_bytes = static_cast<size_t>(rows) * (d.channels_out / 32) * 4;
+  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+    return a != nullptr && b != nullptr && a0 < b0 + nb && b0 < a0 + na;
+  };
+  if (overlap(in_dev, in_bytes, out_dev, o1 - o0) || overlap(packed_out_dev, pk_bytes, out_dev, o1 - o0) ||
+      overlap(packed_out_dev, pk_bytes, in_dev, in_bytes))
+    return fail("bconv2d_run_fused_fc: out, packed_out and the input must not overlap");
+  const lce::ConvKParams fc = [&] {
+    lce::ConvKParams q;
+    memset(&q, 0, sizeof(q));
+    q.shuf_sh = 1; q.shuf_sw = 1; q.shuf_c = d.channels_out; q.shuf_k = d.channels_in;
+    q.shuf_act = activation; q.shuf_bias = bias_dev; q.shuf_alpha = alpha_dev;
+    q.shuf_scale = scale_dev; q.shuf_shift = shift_dev; q.shuf_act2 = bn_activation;
+    return q;
+  }();
+  return bconv_run_impl(plan, in_dev, out_dev, nullptr, LCE_ACT_NONE, packed_out_dev, nullptr, stream, nullptr, 0,
+                        nullptr, false, &fc);
+}
+
+// host-internal (Graph::FuseBinaryFullyConnected): lce_b200_bconv2d_run_fused_fc takes a plan created
+// now from *d; no device needed
+int lce_b200_internal_fc_takes(const lce_bconv2d_desc* d) { return fc_refusal(*d, nullptr) == nullptr; }
 
 // Whether lce_b200_bconv2d_run_slice will take a plan created now from *d
 // (Graph::FuseDenseBlocks asks before it rewrites the graph).

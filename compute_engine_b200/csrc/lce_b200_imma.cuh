@@ -360,6 +360,9 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
 // The plan's output transform is not applied: y = D = p.shuf_k - 2 popc(a ^ w), the +-1 dot product,
 // exact, then p.shuf_bias added with one rounding and p.shuf_act applied (TRANSPOSE_CONV's), then the
 // shortcut. No per-channel vectors stay in registers, which keeps the instance within the b1 cap.
+// The same instance runs lce_b200_bconv2d_run_fused_fc: with sh = sw = 1 and OH = OW = 1 the address
+// is row-major [M, cout], and D is scaled by p.shuf_alpha before the bias and followed by the
+// BatchNorm p.shuf_scale, p.shuf_shift and p.shuf_act2, each step rounded on its own.
 template <int OUT, int S, bool CHAIN = false, bool GATE = false, bool SLICE = false, bool SPATIAL = false,
           bool GW = false, bool SHUFFLE = false>
 __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2][8][4],
@@ -465,12 +468,22 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           }
         }
         if constexpr (SHUFFLE) {
-          // TRANSPOSE_CONV's bias, one rounding, then its activation
-          if (p.shuf_bias != nullptr) {
-            const float* sb = p.shuf_bias + c_sh + tig * 2;
+          // FULLY_CONNECTED's alpha (run_fused_fc), one rounding; TRANSPOSE_CONV's or FULLY_CONNECTED's
+          // bias, one rounding, then its activation; then run_fused_fc's BatchNorm, MUL and ADD rounded
+          // apart as TFLite's ops round them, and the ADD's activation. Each vector is read per ns.
+          const int cv = c_sh + tig * 2;
+          if (p.shuf_alpha != nullptr) {
 #pragma unroll
             for (int ns = 0; ns < 8; ++ns) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(sb + ns * 8));
+              const float2 a = __ldg(reinterpret_cast<const float2*>(p.shuf_alpha + cv + ns * 8));
+              y[2 * ns] = __fmul_rn(y[2 * ns], a.x);
+              y[2 * ns + 1] = __fmul_rn(y[2 * ns + 1], a.y);
+            }
+          }
+          if (p.shuf_bias != nullptr) {
+#pragma unroll
+            for (int ns = 0; ns < 8; ++ns) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.shuf_bias + cv + ns * 8));
               y[2 * ns] = __fadd_rn(y[2 * ns], b.x);
               y[2 * ns + 1] = __fadd_rn(y[2 * ns + 1], b.y);
             }
@@ -480,6 +493,30 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
             const float s_lo = sact == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
             const float s_hi =
                 sact == LCE_ACT_RELU ? __int_as_float(0x7f800000) : (sact == LCE_ACT_RELU6 ? 6.0f : 1.0f);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], s_lo), s_hi);
+          }
+          if (p.shuf_scale != nullptr) {
+#pragma unroll
+            for (int ns = 0; ns < 8; ++ns) {
+              const float2 a = __ldg(reinterpret_cast<const float2*>(p.shuf_scale + cv + ns * 8));
+              y[2 * ns] = __fmul_rn(y[2 * ns], a.x);
+              y[2 * ns + 1] = __fmul_rn(y[2 * ns + 1], a.y);
+            }
+          }
+          if (p.shuf_shift != nullptr) {
+#pragma unroll
+            for (int ns = 0; ns < 8; ++ns) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.shuf_shift + cv + ns * 8));
+              y[2 * ns] = __fadd_rn(y[2 * ns], b.x);
+              y[2 * ns + 1] = __fadd_rn(y[2 * ns + 1], b.y);
+            }
+          }
+          const int sact2 = p.shuf_act2;
+          if (sact2 != LCE_ACT_NONE) {
+            const float s_lo = sact2 == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
+            const float s_hi =
+                sact2 == LCE_ACT_RELU ? __int_as_float(0x7f800000) : (sact2 == LCE_ACT_RELU6 ? 6.0f : 1.0f);
 #pragma unroll
             for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], s_lo), s_hi);
           }

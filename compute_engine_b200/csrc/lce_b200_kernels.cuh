@@ -107,6 +107,14 @@ struct ConvKParams {
   // nullptr) added and shuf_act applied before the shortcut ADD
   int shuf_sh, shuf_sw, shuf_c, shuf_act, shuf_k;
   const float* shuf_bias;
+  // SHUFFLE instances, lce_b200_bconv2d_run_fused_fc (shuf_sh = shuf_sw = 1, OH = OW = 1, shuf_c =
+  // cout): shuf_alpha multiplies the dot product before the bias, then after shuf_act a BatchNorm
+  // shuf_scale, shuf_shift and shuf_act2 (each vector shuf_c floats or nullptr; run_fused_shuffle
+  // passes none of them and shuf_act2 = NONE)
+  const float* shuf_alpha;
+  const float* shuf_scale;
+  const float* shuf_shift;
+  int shuf_act2;
   // mma.sync kernel, group-window (GW) instances only: 8 % (2 * Cw_pg), a k-slice's step through
   // the window
   int win_step;

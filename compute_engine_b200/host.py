@@ -276,6 +276,14 @@ class HostGraph:
         fuse_residual_blocks and allocate_tensors."""
         return lib().lce_host_fuse_binary_transpose_convs(self._g)
 
+    def fuse_binary_fully_connected(self):
+        """LceDequantize -> FULLY_CONNECTED (+-alpha_o weights, N % 64 == 0) [-> MUL -> ADD] [-> LceQuantize]
+        (a binary dense layer) => one node that runs it as a 1x1 binary convolution of its rows on the b1
+        tensor instruction, with alpha, the bias, the BatchNorm and the next sign in the store.
+        Bit-identical when every alpha_o is a power of two; otherwise within the bound
+        Graph::FuseBinaryFullyConnected states. Call before allocate_tensors."""
+        return lib().lce_host_fuse_binary_fully_connected(self._g)
+
     def fuse_residual_pairs(self):
         """Two consecutive LceBconv2d+ADD[+LceQuantize] blocks whose intermediate nothing else
         reads => one node that keeps it on chip. Call after the other fusions."""
@@ -283,7 +291,7 @@ class HostGraph:
 
     def fuse_all(self):
         return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_binary_transpose_convs()
-                + self.fuse_residual_blocks()
+                + self.fuse_binary_fully_connected() + self.fuse_residual_blocks()
                 + self.fuse_spatial_scales()
                 + self.fuse_float_glue() + self.fuse_upsample_merges() + self.fuse_resize_argmax()
                 + self.fuse_subpixel_convs()

@@ -42,13 +42,19 @@ class Interpreter:
         (the optimised kernels' rules and their float zero-padding correction).
         batch_size: mini-batch used by predict (default: all). fuse: apply the graph-level fusions
         (residual-block tail into LceBconv2d's epilogue, max-pool + blur-pool); the outputs are
-        bit-identical either way, with one exception: a 2-bit-activation layer (DoReFaNet's quantiser
+        bit-identical either way, with two exceptions: a 2-bit-activation layer (DoReFaNet's quantiser
         in front of a float CONV_2D or FULLY_CONNECTED with +-alpha weights) runs fused as an exact
         integer binary convolution over bit planes, whose result is the real value rounded twice,
         where the float layer rounds after each of its K terms; the two differ by up to about
         K * 2^-24 * sum |a| |w| per output, which can flip a level of the next quantiser at a near-tie
-        (HostGraph.fuse_quantized_activations). devices: CUDA device indices to shard mini-batches over
-        (default: the current device only)."""
+        (HostGraph.fuse_quantized_activations). And a binary dense layer (LceDequantize ->
+        FULLY_CONNECTED with +-alpha_o weights) whose alpha_o are not all powers of two (XNOR-Net's
+        scaled or BatchNorm-folded kernels) runs fused as fl(fl(alpha_o * D) + bias) with D the exact
+        +-1 dot product, the real value rounded twice, where the float layer rounds after each of its K
+        terms; the two differ by up to about K * 2^-24 * K * alpha_o per output (sum |a| |w| = K *
+        alpha_o), which can flip the next sign at a near-tie (HostGraph.fuse_binary_fully_connected);
+        with every alpha_o a power of two (+-1.0 kernels included) it is bit-identical. devices: CUDA
+        device indices to shard mini-batches over (default: the current device only)."""
         if use_reference_bconv and use_indirect_bgemm:
             import warnings
             warnings.warn("'use_reference_bconv' and `use_indirect_bgemm` are both set to true. "

@@ -923,29 +923,56 @@ def meliusnet22(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
     return meliusnet(batch, seed, image, input_type, pad_values)
 
 
-def _alexnet(g, x, xs, widths, pad_values):
+def _alexnet(g, x, xs, widths, pad_values, flatten=False):
     """The binary trunk BinaryAlexNet and XNOR-Net share, after the stem's map x: pooled sign ->
     LceBconv2d 5x5 (float) -> pooled sign -> two LceBconv2d 3x3 with bitpacked output -> LceBconv2d
     3x3 (float) -> pooled sign -> LceBconv2d VALID over the whole pooled map (bitpacked). A pooled
     sign is MAX_POOL_2D 3x3/s2 VALID -> MUL(bn_scale) -> ADD(bn_shift) -> LceQuantize. Returns the
-    packed signs of the last layer and their shape."""
+    packed signs of the last layer and their shape.
+    flatten (widths without the last): the trunk ends at the last pooled BatchNorm, flattened as larq's
+    Flatten converts, ADD -> RESHAPE [-1, OH * OW * C]; returns that float map and its width."""
     def pooled_sign(t, ts):
         t, ts = g.pool("MAX_POOL_2D", t, ts, 3, 2, "VALID")
         return g.quantize(g.batchnorm(t, ts), ts), ts
 
-    c2, c3, c4, c5, c6 = widths
+    c2, c3, c4, c5 = widths[:4]
     q, qs = pooled_sign(x, xs)
     y, ys = g.bconv(q, qs, c2, k=5, pad_values=pad_values, activation="NONE")
     q, qs = pooled_sign(y, ys)
     q, qs = g.bconv(q, qs, c3, pad_values=pad_values, activation="NONE", bitpacked=True)
     q, qs = g.bconv(q, qs, c4, pad_values=pad_values, activation="NONE", bitpacked=True)
     y, ys = g.bconv(q, qs, c5, pad_values=pad_values, activation="NONE")
+    if flatten:
+        y, ys = g.pool("MAX_POOL_2D", y, ys, 3, 2, "VALID")
+        y = g.batchnorm(y, ys)
+        k = ys[1] * ys[2] * ys[3]
+        flat = g.act((ys[0], k))
+        g.m.add_op("RESHAPE", [y], [flat], new_shape=[-1, k])
+        return flat, k
     q, qs = pooled_sign(y, ys)
-    return g.bconv(q, qs, c6, k=qs[1], pad_values=pad_values, activation="NONE", padding="VALID",
+    return g.bconv(q, qs, widths[4], k=qs[1], pad_values=pad_values, activation="NONE", padding="VALID",
                    bitpacked=True)
 
 
-def binaryalexnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+def _binary_dense(g, x, k, n, alpha=None, bias=None, activation="NONE"):
+    """larq's QuantDense(ste_sign, ste_sign) on a float [B, k] map as the converter leaves it (LCE has no
+    binary dense op): LceQuantize -> LceDequantize -> FULLY_CONNECTED with weights +-alpha_o (alpha None:
+    +-1.0, larq's ste_sign kernel) and the bias (None: absent). Returns the [B, n] output."""
+    b = g.batch
+    q = g.act((b, (k + 31) // 32), np.int32)
+    g.m.add_op("LceQuantize", [x], [q], custom_options=b"")
+    deq = g.act((b, k))
+    g.m.add_op("LceDequantize", [q], [deq], custom_options=b"")
+    wt = (g.rng.integers(0, 2, (n, k), dtype=np.int8) * 2 - 1).astype(np.float32)
+    if alpha is not None:
+        wt = wt * alpha[:, None]
+    y = g.act((b, n))
+    g.m.add_op("FULLY_CONNECTED", [deq, g.const(wt), -1 if bias is None else g.const(bias, name="b")], [y],
+               activation=activation)
+    return y
+
+
+def binaryalexnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0, dense="conv"):
     """BinaryAlexNet, restated from larq-zoo with synthetic weights, in the converter's op order
     (shapes at 224):
       stem CONV_2D 11x11/s4 SAME 3 -> 64 with +-1 float weights (a binary kernel on the float image,
@@ -962,11 +989,27 @@ def binaryalexnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0
     Simplification: larq-zoo flattens the pooled map and applies dense layers; flattening an NHWC
     map and a dense layer over it is exactly a VALID convolution over the whole map, which keeps
     those layers binary. The BatchNorm that follows each binary layer with bitpacked output is
-    folded into its thresholds. 7 LceBconv2d (4 bitpacked), 3 pooled signs."""
+    folded into its thresholds. 7 LceBconv2d (4 bitpacked), 3 pooled signs.
+    dense="fully_connected": larq-zoo's head as the converter leaves it instead: the last pooled
+    BatchNorm flattened (ADD -> RESHAPE [-1, 9216]), then three times LceQuantize -> LceDequantize ->
+    FULLY_CONNECTED (+-1.0 weights, no bias) -> MUL -> ADD (the BatchNorm, not folded), 4096, 4096 and
+    1000 wide, then SOFTMAX. 4 LceBconv2d (2 bitpacked), 2 pooled signs and the flattened one."""
+    if dense not in ("conv", "fully_connected"):
+        raise ValueError(f"binaryalexnet dense must be 'conv' or 'fully_connected', not {dense!r}")
     g = _Builder(seed, batch, "BinaryAlexNet")
     xs = (batch, image, image, 3)
     x = g.image_input(xs, input_type)
     x, xs = g.conv(x, xs, 64, 11, 4, bn=False, use_bias=False, binary=True)
+    if dense == "fully_connected":
+        x, k = _alexnet(g, x, xs, (192, 384, 384, 256), pad_values, flatten=True)
+        for n in (4096, 4096, 1000):
+            y = _binary_dense(g, x, k, n)
+            x = g.batchnorm(y, (batch, 1, 1, n))
+            k = n
+        probs = g.act((batch, 1000))
+        g.m.add_op("SOFTMAX", [x], [probs], beta=1.0)
+        g.m.outputs = [probs]
+        return g.m.serialize()
     q, qs = _alexnet(g, x, xs, (192, 384, 384, 256, 4096), pad_values)
     q, qs = g.bconv(q, qs, 4096, k=1, pad_values=pad_values, activation="NONE", padding="VALID",
                     bitpacked=True)
@@ -979,7 +1022,7 @@ def binaryalexnet(batch=1, seed=0, image=224, input_type="float32", pad_values=0
     return g.m.serialize()
 
 
-def xnornet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
+def xnornet(batch=1, seed=0, image=224, input_type="float32", pad_values=0, dense="conv"):
     """XNOR-Net, restated from larq-zoo with synthetic weights, in the converter's op order (shapes
     at 224):
       stem CONV_2D 11x11/s4 SAME 3 -> 96 (BN folded, RELU) -> [B,56,56,96];
@@ -993,15 +1036,32 @@ def xnornet(batch=1, seed=0, image=224, input_type="float32", pad_values=0):
     The per-channel weight scale of XNOR-Net's binary layers folds into each post-activation
     multiplier, so with synthetic weights it changes nothing. The first dense layer is restated as
     a VALID convolution over the whole pooled map, as in binaryalexnet. 6 LceBconv2d (3
-    bitpacked), 3 pooled signs."""
+    bitpacked), 3 pooled signs.
+    dense="fully_connected": the two 4096-wide layers as the converter leaves larq's QuantDense with
+    XNOR-Net's kernel scale instead: the last pooled BatchNorm flattened (ADD -> RESHAPE [-1, 9216]),
+    then LceQuantize -> LceDequantize -> FULLY_CONNECTED 9216 -> 4096 and LceQuantize -> LceDequantize
+    -> FULLY_CONNECTED 4096 -> 4096 (RELU), each with weights +-alpha_o, alpha_o the row's mean |w|
+    times its folded BatchNorm scale (not powers of two), and the folded shift as the bias; then the
+    float classifier as above. 4 LceBconv2d (2 bitpacked), 2 pooled signs and the flattened one."""
+    if dense not in ("conv", "fully_connected"):
+        raise ValueError(f"xnornet dense must be 'conv' or 'fully_connected', not {dense!r}")
     g = _Builder(seed, batch, "XNORNet")
     xs = (batch, image, image, 3)
     x = g.image_input(xs, input_type)
     x, xs = g.conv(x, xs, 96, 11, 4, activation="RELU")
-    q, qs = _alexnet(g, x, xs, (256, 384, 384, 256, 4096), pad_values)
-    y, ys = g.bconv(q, qs, 4096, k=1, pad_values=pad_values, activation="RELU", padding="VALID")
-    flat = g.act((batch, 4096))
-    g.m.add_op("RESHAPE", [y], [flat], new_shape=[-1, 4096])
+    if dense == "fully_connected":
+        x, k = _alexnet(g, x, xs, (256, 384, 384, 256), pad_values, flatten=True)
+        for act in ("NONE", "RELU"):
+            s, t = g.bn(4096)
+            alpha = (g.rng.uniform(0.5, 1.5, 4096).astype(np.float32) * s / np.float32(np.sqrt(k)))
+            x = _binary_dense(g, x, k, 4096, alpha=alpha, bias=t, activation=act)
+            k = 4096
+        flat = x
+    else:
+        q, qs = _alexnet(g, x, xs, (256, 384, 384, 256, 4096), pad_values)
+        y, ys = g.bconv(q, qs, 4096, k=1, pad_values=pad_values, activation="RELU", padding="VALID")
+        flat = g.act((batch, 4096))
+        g.m.add_op("RESHAPE", [y], [flat], new_shape=[-1, 4096])
     wt = g.rng.standard_normal((1000, 4096)).astype(np.float32) / np.float32(np.sqrt(4096))
     s, t = g.bn(1000)
     logits = g.act((batch, 1000))

@@ -232,6 +232,25 @@ int lce_b200_bconv2d_run_fused_shuffle(lce_b200_bconv2d* plan, const int32_t* in
                                        const float* bias_dev, int activation, const float* skip_dev,
                                        int add_activation, float* out_dev, int32_t* packed_out_dev,
                                        void* stream);
+/* A binary dense layer, LceDequantize -> FULLY_CONNECTED (weights +-alpha_c, [bias]) [-> MUL(scale) ->
+ * ADD(shift)] [-> LceQuantize], as the plan's 1x1 GEMM of batch rows (in_h = in_w = 1) on the instance of
+ * the b1 mma.sync kernel run_fused_shuffle uses, with s_h = s_w = 1. Per row m, column c < N =
+ * channels_out:
+ *   y = activation(fl(fl(alpha[c] * D) + bias[c]));
+ *   y = bn_activation(fl(fl(y * scale[c]) + shift[c]));   out[m][c] = y;   packed_out = bitpack(y),
+ * D the +-1 dot product channels_in - 2 popcount(a ^ w) as an exact integer, each step rounded on its
+ * own as TFLite's FULLY_CONNECTED, MUL and ADD round the result (a NULL vector drops its step;
+ * bn_activation applies either way). With every alpha a power of two that is TFLite's FULLY_CONNECTED
+ * bit for bit; otherwise TFLite's loop rounds after each of its K terms and the results can differ by
+ * about K * 2^-24 * K * alpha. The plan must be an ungrouped 1x1 / stride 1 plan of in_h = in_w = 1 with
+ * float output, no fused activation and no zero padding, N % 64 == 0, on the b1 mma.sync kernel
+ * (lce_b200_internal_fc_takes); the post_mul / post_bias are not applied. alpha, bias, scale and shift
+ * hold N device floats each (8-byte aligned) or are NULL; out is [batch, N] (16-byte aligned) and
+ * packed_out (may be NULL) [batch, N / 32]; out, packed_out and the input must not overlap. */
+int lce_b200_bconv2d_run_fused_fc(lce_b200_bconv2d* plan, const int32_t* in_dev, const float* alpha_dev,
+                                  const float* bias_dev, int activation, const float* scale_dev,
+                                  const float* shift_dev, int bn_activation, float* out_dev,
+                                  int32_t* packed_out_dev, void* stream);
 /* The signs of a dense layer's BatchNorm in one pass over a strided float [rows, channels] map
  * (row r starts at x_dev + r * x_pixel_stride):
  *   packed_out[r][ceil(channels/32)] = bitpack(x * scale[c] + shift[c]),
