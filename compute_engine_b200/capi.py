@@ -100,7 +100,7 @@ EXPORTS = [
     "lce_b200_bconv2d_run_fused_pair",
     "lce_b200_bconv2d_run_fused_gate", "lce_b200_bconv2d_run_fused_scale",
     "lce_b200_bconv2d_run_slice", "lce_b200_bconv2d_run_slice_add", "lce_b200_bconv2d_run_fused_shuffle",
-    "lce_b200_bconv2d_run_fused_fc",
+    "lce_b200_bconv2d_run_fused_fc", "lce_b200_bconv2d_run_fused_fc_max",
     "lce_b200_f32_chain_sign", "lce_b200_f32_gate_sign", "lce_b200_f32_scale_sign", "lce_b200_f32_logistic",
     "lce_b200_f32_affine_sign", "lce_b200_f32_maxpool_affine_sign",
     "lce_b200_f32_maximum", "lce_b200_f32_minimum", "lce_b200_f32_div", "lce_b200_f32_round",
@@ -109,7 +109,7 @@ EXPORTS = [
     "lce_b200_bconv2d_bases_get_desc", "lce_b200_bconv2d_bases_run", "lce_b200_bconv2d_bases_destroy",
     "lce_b200_f32_shift_sign_planes",
     "lce_b200_f32_resize_nearest", "lce_b200_f32_resize_bilinear", "lce_b200_f32_upsample_add_sign",
-    "lce_b200_f32_argmax", "lce_b200_resize_bilinear_argmax_max_row_floats", "lce_b200_f32_resize_bilinear_argmax",
+    "lce_b200_f32_argmax", "lce_b200_f32_reduce_max", "lce_b200_resize_bilinear_argmax_max_row_floats", "lce_b200_f32_resize_bilinear_argmax",
     "lce_b200_f32_depth_to_space", "lce_b200_subpixel_conv_max_out_channels", "lce_b200_f32_subpixel_conv",
     "lce_b200_f32_transpose_conv2d",
     "lce_b200_detection_max_anchors", "lce_b200_detection_workspace_bytes", "lce_b200_f32_detection_postprocess",
@@ -370,6 +370,25 @@ def argmax(x: torch.Tensor, axis=-1, out_dtype=torch.int64):
     out = torch.empty(x.shape[:a] + x.shape[a + 1:], dtype=out_dtype, device=x.device)
     _check(lib().lce_b200_f32_argmax(_p(x), C.c_int64(outer), C.c_int(x.shape[a]), C.c_int64(inner),
                                      int(out_dtype == torch.int64), _p(out), _stream()))
+    return out
+
+
+def reduce_max(x: torch.Tensor, axes, keep_dims=False):
+    """REDUCE_MAX of a float tensor over `axes` (contiguous once normalised; negative and duplicate axes as
+    in TFLite), TFLite's reference rule bit for bit: cur = -FLT_MAX, then cur = x > cur ? x : cur in index
+    order (a NaN is never chosen, the first of equal values wins, an all-NaN / all--inf / empty slice gives
+    -FLT_MAX)."""
+    x = _dev(x, torch.float32)
+    r = x.dim()
+    red = sorted({a + r if a < 0 else a for a in ([axes] if isinstance(axes, int) else axes)})
+    if not red or red[0] < 0 or red[-1] >= r or red != list(range(red[0], red[-1] + 1)):
+        raise LceError(f"reduce_max: axes {axes} must be non-empty, in range and contiguous for rank {r}")
+    a, b = red[0], red[-1] + 1
+    outer, n, inner = math.prod(x.shape[:a]), math.prod(x.shape[a:b]), math.prod(x.shape[b:])
+    shape = x.shape[:a] + ((1,) * (b - a) if keep_dims else ()) + x.shape[b:]
+    out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    _check(lib().lce_b200_f32_reduce_max(_p(x), C.c_int64(outer), C.c_int64(n), C.c_int64(inner), _p(out),
+                                         _stream()))
     return out
 
 
@@ -747,6 +766,28 @@ class BConv2d:
         _check(lib().lce_b200_bconv2d_run_fused_fc(self._h, _p(x), _p(vecs[0]), _p(vecs[1]), C.c_int(activation),
                                                    _p(vecs[2]), _p(vecs[3]), C.c_int(bn_activation), _p(out),
                                                    _p(pk), _stream()))
+        return out, pk
+
+    def run_fused_fc_max(self, x: torch.Tensor, points: int, alpha=None, bias=None, activation=0, scale=None,
+                         shift=None, bn_activation=0, store_max=True, packed=True):
+        """lce_b200_bconv2d_run_fused_fc_max: run_fused_fc's layer on packed x [rows, ceil(K / 32)], rows =
+        B * points, then each image's column max by TFLite's REDUCE_MAX rule. Returns (float max [B, N] |
+        None, packed signs [B, N / 32] | None)."""
+        x = _dev(x, torch.int32)
+        rows = x.shape[0]
+        if x.dim() != 2 or x.shape[1] != cdiv(self.desc.channels_in, 32):
+            raise LceError("run_fused_fc_max: x must be packed rows [rows, ceil(channels_in / 32)]")
+        if (rows, self.desc.in_h, self.desc.in_w) != (self.desc.batch, 1, 1):
+            self.set_input_shape(rows, 1, 1)
+        n, b = self.desc.channels_out, rows // max(points, 1)
+        vecs = [None if v is None else torch.as_tensor(v, dtype=torch.float32, device=x.device).contiguous()
+                for v in (alpha, bias, scale, shift)]
+        keys = torch.empty((max(b, 1), n), dtype=torch.int64, device=x.device)
+        out = torch.empty((b, n), dtype=torch.float32, device=x.device) if store_max else None
+        pk = torch.empty((b, cdiv(n, 32)), dtype=torch.int32, device=x.device) if packed else None
+        _check(lib().lce_b200_bconv2d_run_fused_fc_max(self._h, _p(x), _p(vecs[0]), _p(vecs[1]), C.c_int(activation),
+                                                       _p(vecs[2]), _p(vecs[3]), C.c_int(bn_activation),
+                                                       C.c_int(points), _p(keys), _p(out), _p(pk), _stream()))
         return out, pk
 
     def run_slice(self, x: torch.Tensor, out: torch.Tensor, offset: int = 0):

@@ -48,6 +48,11 @@ TfLiteStatus Resize(TfLiteContext* c, TfLiteTensor* t, std::initializer_list<int
   for (int d : dims) a->data[i++] = d;
   return c->ResizeTensor(c, t, a);
 }
+TfLiteStatus ResizeTo(TfLiteContext* c, TfLiteTensor* t, const std::vector<int>& dims) {
+  TfLiteIntArray* a = LceB200IntArrayCreate(static_cast<int>(dims.size()));
+  for (size_t i = 0; i < dims.size(); ++i) a->data[i] = dims[i];
+  return c->ResizeTensor(c, t, a);
+}
 bool OnDevice(const void* p) {
   cudaPointerAttributes a;
   if (!p || cudaPointerGetAttributes(&a, p) != cudaSuccess) {
@@ -205,7 +210,14 @@ TfLiteStatus FcPrepare(TfLiteContext* c, TfLiteNode* n) {
   B_ENSURE(c, in && w && w->dims->size == 2, "FULLY_CONNECTED: weights must be [out, in]");
   const int k = w->dims->data[1];
   B_ENSURE(c, k > 0 && Count(in) % k == 0, "FULLY_CONNECTED: input size mismatch");
-  return Resize(c, T(c, n->outputs, 0), {static_cast<int>(Count(in) / k), w->dims->data[0]});
+  if (!P(n).keep_dims) return Resize(c, T(c, n->outputs, 0), {static_cast<int>(Count(in) / k), w->dims->data[0]});
+  // keep_num_dims: the input's shape with its last axis, which must be the weights' input size, now N
+  B_ENSURE(c, in->dims->size >= 1 && in->dims->data[in->dims->size - 1] == k,
+           "FULLY_CONNECTED: keep_num_dims needs the input's last axis to be the weights' input size");
+  TfLiteIntArray* dims = LceB200IntArrayCreate(in->dims->size);
+  for (int i = 0; i < in->dims->size; ++i) dims->data[i] = in->dims->data[i];
+  dims->data[dims->size - 1] = w->dims->data[0];
+  return c->ResizeTensor(c, T(c, n->outputs, 0), dims);
 }
 TfLiteStatus FcInvoke(TfLiteContext* c, TfLiteNode* n) {
   const TfLiteTensor* in = T(c, n->inputs, 0);
@@ -960,6 +972,61 @@ TfLiteStatus ArgMaxInvoke(TfLiteContext* c, TfLiteNode* n) {
   return kTfLiteOk;
 }
 
+// -------------------------------- REDUCE_MAX -------------------------------- //
+// inputs [x (float32, rank 1-5), axes (a constant int32 tensor, 0-D or 1-D, read on the host)]; output
+// x's shape with the reduced axes kept as 1 (ReducerOptions.keep_dims) or dropped. Negative axes count
+// from the end and duplicates are allowed, as in TFLite; the reduced axes must be contiguous, so the
+// op is [outer, n, inner] reduced over n. Returns nullptr, or why the node is refused.
+const char* ReduceMaxChecks(TfLiteContext* c, TfLiteNode* n, int* first, int* last) {
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  const TfLiteTensor* axes = T(c, n->inputs, 1);
+  const TfLiteTensor* o = T(c, n->outputs, 0);
+  if (!x || x->type != kTfLiteFloat32) return "REDUCE_MAX: the input must be float32";
+  if (!o || o->type != kTfLiteFloat32) return "REDUCE_MAX: the output must be float32";
+  if (!axes || axes->allocation_type != kTfLiteMmapRo || !axes->data.raw || OnDevice(axes->data.raw))
+    return "REDUCE_MAX: the axes must be a constant tensor";
+  if (axes->type != kTfLiteInt32 || axes->dims->size > 1) return "REDUCE_MAX: the axes must be a 0-D or 1-D int32 tensor";
+  const int rank = x->dims->size;
+  if (rank < 1 || rank > 5) return "REDUCE_MAX: the input's rank must be 1 to 5";
+  if (Count(axes) < 1) return "REDUCE_MAX: no axis to reduce";
+  bool red[5] = {};
+  for (int64_t k = 0; k < Count(axes); ++k) {
+    const int a = axes->data.i32[k];
+    if (a < -rank || a >= rank) return "REDUCE_MAX: an axis is out of range";
+    red[a < 0 ? a + rank : a] = true;
+  }
+  *first = 0;
+  while (!red[*first]) ++*first;
+  *last = *first;
+  while (*last + 1 < rank && red[*last + 1]) ++*last;
+  for (int k = *last + 1; k < rank; ++k)
+    if (red[k]) return "REDUCE_MAX: the reduced axes must be contiguous";
+  return nullptr;
+}
+TfLiteStatus ReduceMaxPrepare(TfLiteContext* c, TfLiteNode* n) {
+  B_ENSURE(c, n->inputs->size == 2 && n->outputs->size == 1, "REDUCE_MAX: inputs [x, axes] and one output expected");
+  int first, last;
+  const char* why = ReduceMaxChecks(c, n, &first, &last);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteIntArray* d = T(c, n->inputs, 0)->dims;
+  std::vector<int> dims;
+  for (int k = 0; k < d->size; ++k)
+    if (k < first || k > last) dims.push_back(d->data[k]);
+    else if (P(n).keep_dims) dims.push_back(1);
+  return ResizeTo(c, T(c, n->outputs, 0), dims);
+}
+TfLiteStatus ReduceMaxInvoke(TfLiteContext* c, TfLiteNode* n) {
+  int first, last;
+  const char* why = ReduceMaxChecks(c, n, &first, &last);
+  B_ENSURE(c, why == nullptr, why);
+  const TfLiteTensor* x = T(c, n->inputs, 0);
+  int64_t outer = 1, r = 1, inner = 1;
+  for (int k = 0; k < x->dims->size; ++k)
+    (k < first ? outer : k > last ? inner : r) *= x->dims->data[k];
+  B_CAPI(c, lce_b200_f32_reduce_max(x->data.f, outer, r, inner, T(c, n->outputs, 0)->data.f, lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
 // ------------------ fused RESIZE_BILINEAR -> ARG_MAX: a segmentation head ------------------ //
 // Created by Graph::FuseResizeArgmax; builtin_data = { BuiltinParams resize, BuiltinParams argmax };
 // inputs [x, size, axis (the channel axis)], outputs [labels [B, new_height, new_width]].
@@ -1293,11 +1360,21 @@ TfLiteStatus BinaryFcPrepare(TfLiteContext* c, TfLiteNode* n) {
   }
   const int64_t rows = Count(q) / cw;
   B_ENSURE(c, rows <= INT32_MAX, "LceBfc: too many rows");
-  if (Resize(c, T(c, n->outputs, 0), {static_cast<int>(rows), N}) != kTfLiteOk) return kTfLiteError;
+  // FULLY_CONNECTED's keep_num_dims: q's leading axes (the input's), then N (the pass took it only when
+  // the input's last axis is K, so q holds one row per leading index)
+  auto shape = [&](int last) {
+    std::vector<int> d{static_cast<int>(rows), last};
+    if (op->p.fc.keep_dims) {
+      d.assign(q->dims->data, q->dims->data + q->dims->size);
+      d.back() = last;
+    }
+    return d;
+  };
+  if (ResizeTo(c, T(c, n->outputs, 0), shape(N)) != kTfLiteOk) return kTfLiteError;
   if (n->outputs->size == 2) {
     TfLiteTensor* pk = T(c, n->outputs, 1);
     B_ENSURE(c, pk && pk->type == kTfLiteInt32, "LceBfc+LceQuantize: packed output must be int32");
-    if (Resize(c, pk, {static_cast<int>(rows), (N + 31) / 32}) != kTfLiteOk) return kTfLiteError;
+    if (ResizeTo(c, pk, shape((N + 31) / 32)) != kTfLiteOk) return kTfLiteError;
   }
   if (op->plan) {
     B_CAPI(c, lce_b200_bconv2d_set_input_shape(op->plan, static_cast<int>(rows), 1, 1));
@@ -1324,6 +1401,106 @@ TfLiteStatus BinaryFcInvoke(TfLiteContext* c, TfLiteNode* n) {
                                           op->p.fc.activation, vec(4), vec(5), op->p.add.activation,
                                           T(c, n->outputs, 0)->data.f, pk ? pk->data.i32 : nullptr,
                                           lce_b200_get_stream()));
+  return kTfLiteOk;
+}
+
+// --- fused LceDequantize -> FULLY_CONNECTED [-> MUL -> ADD] -> REDUCE_MAX(points) [-> LceQuantize] --- //
+// Created by Graph::FuseBinaryFcMax; builtin_data = BinaryFcMaxParams; inputs as LceBfc's, outputs [max
+// [B, N] (or [B, 1, N] with keep_dims)?, packed signs [B, N / 32]?] as the params say, temporaries [keys:
+// B * N 64-bit words]. The rows follow q's size (B * points), so a batch resize re-plans them. The node
+// owns a 1x1 LceBconv2d plan of rows x 1 x 1 and runs lce_b200_bconv2d_run_fused_fc_max, which
+// initialises the keys itself.
+struct BinaryFcMaxOp {
+  BinaryFcMaxParams p;
+  lce_b200_bconv2d* plan = nullptr;
+};
+void* BinaryFcMaxInit(TfLiteContext*, const char* buffer, size_t length) {
+  auto* op = new BinaryFcMaxOp();
+  memset(&op->p, 0, sizeof(op->p));
+  if (buffer && length >= sizeof(BinaryFcMaxParams)) memcpy(&op->p, buffer, sizeof(BinaryFcMaxParams));
+  return op;
+}
+void BinaryFcMaxFree(TfLiteContext*, void* p) {
+  auto* op = static_cast<BinaryFcMaxOp*>(p);
+  lce_b200_bconv2d_destroy(op->plan);
+  delete op;
+}
+TfLiteStatus BinaryFcMaxPrepare(TfLiteContext* c, TfLiteNode* n) {
+  auto* op = static_cast<BinaryFcMaxOp*>(n->user_data);
+  const BinaryFcMaxParams& p = op->p;
+  const int K = p.channels_in, P = p.points;
+  B_ENSURE(c, n->inputs->size == 6 && K > 0 && P > 0 && (p.store_max || p.store_signs) &&
+                  n->outputs->size == p.store_max + p.store_signs,
+           "LceBfc+REDUCE_MAX: inputs [q, filter, alpha, bias, scale, shift] and the max and/or its signs expected");
+  const TfLiteTensor* q = T(c, n->inputs, 0);
+  const TfLiteTensor* f = T(c, n->inputs, 1);
+  const int cw = (K + 31) / 32;
+  B_ENSURE(c, q && q->type == kTfLiteInt32 && q->dims->size == 3 && q->dims->data[1] == P && q->dims->data[2] == cw,
+           "LceBfc+REDUCE_MAX: the input must be packed signs [B, points, ceil(K / 32)]");
+  B_ENSURE(c, f && f->type == kTfLiteInt32 && f->allocation_type == kTfLiteMmapRo && f->dims->size == 4 &&
+                  f->dims->data[1] == 1 && f->dims->data[2] == 1 && f->dims->data[3] == cw,
+           "LceBfc+REDUCE_MAX: the filter must be a constant packed [N, 1, 1, ceil(K / 32)]");
+  const int N = f->dims->data[0];
+  B_ENSURE(c, N % 32 == 0, "LceBfc+REDUCE_MAX: N must be a multiple of 32");
+  for (int k = 2; k < 6; ++k) {
+    const TfLiteTensor* v = T(c, n->inputs, k);
+    B_ENSURE(c, !v || (v->type == kTfLiteFloat32 && v->allocation_type == kTfLiteMmapRo && Count(v) == N),
+             "LceBfc+REDUCE_MAX: alpha, bias, scale and shift must be constant float32 [N]");
+  }
+  const int B = q->dims->data[0];
+  const int64_t rows = static_cast<int64_t>(B) * P;
+  B_ENSURE(c, rows <= INT32_MAX, "LceBfc+REDUCE_MAX: too many rows");
+  int o = 0;
+  if (p.store_max) {
+    TfLiteTensor* mx = T(c, n->outputs, o++);
+    B_ENSURE(c, mx && mx->type == kTfLiteFloat32, "LceBfc+REDUCE_MAX: the max must be float32");
+    if (ResizeTo(c, mx, p.reduce.keep_dims ? std::vector<int>{B, 1, N} : std::vector<int>{B, N}) != kTfLiteOk)
+      return kTfLiteError;
+  }
+  if (p.store_signs) {
+    TfLiteTensor* pk = T(c, n->outputs, o);
+    B_ENSURE(c, pk && pk->type == kTfLiteInt32, "LceBfc+REDUCE_MAX+LceQuantize: packed output must be int32");
+    if (ResizeTo(c, pk, p.reduce.keep_dims ? std::vector<int>{B, 1, N / 32} : std::vector<int>{B, N / 32}) !=
+        kTfLiteOk)
+      return kTfLiteError;
+  }
+  if (n->temporaries->size != 1) {
+    int first = 0;
+    if (c->AddTensors(c, 1, &first) != kTfLiteOk) return kTfLiteError;
+    LceB200IntArrayFree(n->temporaries);
+    n->temporaries = LceB200IntArrayCreate(1);
+    n->temporaries->data[0] = first;
+  }
+  TfLiteTensor* keys = &c->tensors[n->temporaries->data[0]];   // c->tensors may have moved
+  keys->type = kTfLiteInt64;
+  if (Resize(c, keys, {std::max(B, 1) * N}) != kTfLiteOk) return kTfLiteError;
+  if (op->plan) {
+    B_CAPI(c, lce_b200_bconv2d_set_input_shape(op->plan, static_cast<int>(rows), 1, 1));
+    return kTfLiteOk;
+  }
+  lce_bconv2d_desc d;
+  memset(&d, 0, sizeof(d));
+  d.batch = static_cast<int>(rows); d.in_h = 1; d.in_w = 1; d.channels_in = K;
+  d.filter_h = 1; d.filter_w = 1; d.channels_out = N; d.groups = 1;
+  d.stride_h = 1; d.stride_w = 1; d.dilation_h = 1; d.dilation_w = 1;
+  d.padding = LCE_PADDING_VALID; d.pad_value = 1; d.activation = LCE_ACT_NONE; d.out_type = LCE_OUT_FLOAT;
+  const std::vector<float> ones(N, 1.0f), zeros(N, 0.0f);
+  B_CAPI(c, lce_b200_bconv2d_create(&d, f->data.i32, ones.data(), zeros.data(), nullptr, &op->plan));
+  return kTfLiteOk;
+}
+TfLiteStatus BinaryFcMaxInvoke(TfLiteContext* c, TfLiteNode* n) {
+  const auto* op = static_cast<const BinaryFcMaxOp*>(n->user_data);
+  const BinaryFcMaxParams& p = op->p;
+  auto vec = [&](int k) -> const float* {
+    const TfLiteTensor* v = T(c, n->inputs, k);
+    return v ? v->data.f : nullptr;
+  };
+  float* mx = p.store_max ? T(c, n->outputs, 0)->data.f : nullptr;
+  int32_t* pk = p.store_signs ? T(c, n->outputs, p.store_max)->data.i32 : nullptr;
+  B_CAPI(c, lce_b200_bconv2d_run_fused_fc_max(op->plan, T(c, n->inputs, 0)->data.i32, vec(2), vec(3), p.fc.activation,
+                                              vec(4), vec(5), p.add.activation, p.points,
+                                              c->tensors[n->temporaries->data[0]].data.raw, mx, pk,
+                                              lce_b200_get_stream()));
   return kTfLiteOk;
 }
 
@@ -1677,6 +1854,10 @@ const TfLiteRegistration* BinaryFullyConnectedRegistration() {
   static TfLiteRegistration r = {BinaryFcInit, BinaryFcFree, BinaryFcPrepare, BinaryFcInvoke};
   return &r;
 }
+const TfLiteRegistration* BinaryFcMaxRegistration() {
+  static TfLiteRegistration r = {BinaryFcMaxInit, BinaryFcMaxFree, BinaryFcMaxPrepare, BinaryFcMaxInvoke};
+  return &r;
+}
 const TfLiteRegistration* SubpixelConvRegistration() {
   static TfLiteRegistration r = {SubpixelInit, SubpixelFree, SubpixelPrepare, SubpixelInvoke};
   return &r;
@@ -1739,6 +1920,8 @@ void RegisterBuiltinOps(OpResolver* r) {
   r->AddBuiltin(97, &resize_nearest);   // RESIZE_NEAREST_NEIGHBOR
   static TfLiteRegistration arg_max = {Init, Free, ArgMaxPrepare, ArgMaxInvoke};
   r->AddBuiltin(56, &arg_max);   // ARG_MAX
+  static TfLiteRegistration reduce_max = {Init, Free, ReduceMaxPrepare, ReduceMaxInvoke};
+  r->AddBuiltin(82, &reduce_max);   // REDUCE_MAX
   static TfLiteRegistration depth_to_space = {Init, Free, DepthToSpacePrepare, DepthToSpaceInvoke};
   r->AddBuiltin(5, &depth_to_space);   // DEPTH_TO_SPACE
   static TfLiteRegistration transpose_conv = {Init, Free, TransposeConvPrepare, TransposeConvInvoke};

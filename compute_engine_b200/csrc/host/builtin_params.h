@@ -30,6 +30,14 @@ struct BuiltinParams {
   int32_t block_size;
 };
 
+// builtin_data of the "LceBfc[+MUL+ADD]+REDUCE_MAX[+LceQuantize]" node Graph::FuseBinaryFcMax creates
+// (builtin_ops.cc runs it): the FULLY_CONNECTED's, the ADD's (zeros without it) and the REDUCE_MAX's
+// parameters, K, the points per image, and whether the node stores the float max and its signs.
+struct BinaryFcMaxParams {
+  BuiltinParams fc, add, reduce;
+  int32_t channels_in, points, store_max, store_signs;
+};
+
 // ARG_MAX's axis: a constant int32 or int64 tensor of one element (0-D or [1]) in host memory, within
 // [-rank, rank) and normalised to [0, rank). Returns nullptr, or why the axis is refused.
 // builtin_ops.cc; Graph::FuseResizeArgmax reads the axis through it too.

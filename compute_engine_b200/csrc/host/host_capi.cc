@@ -157,6 +157,7 @@ int lce_host_fuse_resize_argmax(void* g) { return static_cast<Graph*>(g)->FuseRe
 int lce_host_fuse_subpixel_convs(void* g) { return static_cast<Graph*>(g)->FuseSubpixelConvs(); }
 int lce_host_fuse_binary_transpose_convs(void* g) { return static_cast<Graph*>(g)->FuseBinaryTransposeConvs(); }
 int lce_host_fuse_binary_fully_connected(void* g) { return static_cast<Graph*>(g)->FuseBinaryFullyConnected(); }
+int lce_host_fuse_binary_fc_max(void* g) { return static_cast<Graph*>(g)->FuseBinaryFcMax(); }
 int lce_host_fuse_residual_pairs(void* g) { return static_cast<Graph*>(g)->FuseResidualPairs(); }
 void lce_host_enable_profiling(void* g, int on) { static_cast<Graph*>(g)->EnableProfiling(on != 0); }
 void lce_host_reset_profile(void* g) { static_cast<Graph*>(g)->ResetProfile(); }

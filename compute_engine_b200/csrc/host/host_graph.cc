@@ -318,6 +318,7 @@ constexpr const char* kDepthToSpace = "builtin:5";
 constexpr const char* kTransposeConv = "builtin:67";
 constexpr const char* kMul = "builtin:18";
 constexpr const char* kReshape = "builtin:22";
+constexpr const char* kReduceMax = "builtin:82";
 constexpr const char* kRelu = "builtin:19";
 constexpr const char* kMean = "builtin:40";
 constexpr const char* kDiv = "builtin:42";
@@ -2035,10 +2036,23 @@ int Graph::FuseBinaryTransposeConvs() {
 }
 
 const TfLiteRegistration* BinaryFullyConnectedRegistration();   // builtin_ops.cc
+const TfLiteRegistration* BinaryFcMaxRegistration();            // builtin_ops.cc
 extern "C" int lce_b200_internal_fc_takes(const lce_bconv2d_desc* d);   // lce_b200.cu
+extern "C" int lce_b200_internal_fc_max_takes(const lce_bconv2d_desc* d, int points);   // lce_b200.cu
 
-int Graph::FuseBinaryFullyConnected() {
-  if (!device_arena_) return 0;
+namespace {
+lce_bconv2d_desc FcDesc(int64_t rows, int K, int N) {   // a binary dense layer's rows x 1 x 1 plan
+  lce_bconv2d_desc d;
+  memset(&d, 0, sizeof(d));
+  d.batch = static_cast<int>(rows); d.in_h = 1; d.in_w = 1; d.channels_in = K;
+  d.filter_h = 1; d.filter_w = 1; d.channels_out = N; d.groups = 1;
+  d.stride_h = 1; d.stride_w = 1; d.dilation_h = 1; d.dilation_w = 1;
+  d.padding = LCE_PADDING_VALID; d.pad_value = 1; d.activation = LCE_ACT_NONE; d.out_type = LCE_OUT_FLOAT;
+  return d;
+}
+}  // namespace
+
+bool Graph::MatchBinaryFc(size_t i, BinaryFcMatch* m) const {
   // a constant float32 [n] (exactly rank 1), or -1
   auto vec = [&](int t, int n) {
     return t >= 0 && tensors_[t].type == kTfLiteFloat32 && tensors_[t].allocation_type == kTfLiteMmapRo &&
@@ -2046,120 +2060,202 @@ int Graph::FuseBinaryFullyConnected() {
                ? t
                : -1;
   };
-  auto count = [](const TfLiteIntArray* d) {
-    int64_t n = 1;
-    for (int k = 0; k < d->size; ++k) n *= d->data[k];
-    return n;
-  };
+  if (i >= nodes_.size()) return false;
+  const NodeRecord& fc = *nodes_[i];
+  const BuiltinParams* fp = Params(fc);
+  if (fc.name != kFullyConnected || fc.initialized || !fp || fc.node.inputs->size < 2 || fc.node.inputs->size > 3 ||
+      fc.node.outputs->size != 1)
+    return false;
+  const int x = fc.node.inputs->data[0], w = fc.node.inputs->data[1], y = fc.node.outputs->data[0];
+  const int bias_in = fc.node.inputs->size == 3 ? fc.node.inputs->data[2] : -1;
+  if (x < 0 || w < 0 || tensors_[w].type != kTfLiteFloat32 || tensors_[w].allocation_type != kTfLiteMmapRo ||
+      tensors_[x].type != kTfLiteFloat32 || tensors_[y].type != kTfLiteFloat32 || fp->activation < LCE_ACT_NONE ||
+      fp->activation > LCE_ACT_RELU6)
+    return false;
+  const TfLiteIntArray* wd = tensors_[w].dims;
+  const TfLiteIntArray* xd = tensors_[x].dims;
+  if (!wd || wd->size != 2 || !xd || xd->size < 1 || wd->data[0] <= 0 || wd->data[1] <= 0) return false;
+  const int N = wd->data[0], K = wd->data[1];
+  const int bias = vec(bias_in, N);
+  if (bias_in >= 0 && bias < 0) return false;
+  // keep_num_dims keeps x's leading axes, so each row must be x's last axis
+  if (fp->keep_dims != 0 && xd->data[xd->size - 1] != K) return false;
+  // every row o exactly +-alpha_o: one positive, finite magnitude, bitwise, in the whole row (no 0.0 or
+  // -0.0, no 0.5 among 1.0s)
+  const size_t nw = static_cast<size_t>(N) * K;
+  if (const_host_[w].size() < nw * sizeof(float)) return false;
+  m->wb.resize(nw);
+  memcpy(m->wb.data(), const_host_[w].data(), nw * sizeof(float));
+  m->alpha.assign(N, 0.0f);
+  m->unit = true;
+  for (int o = 0; o < N; ++o) {
+    const uint32_t mag = m->wb[static_cast<size_t>(o) * K] & 0x7fffffffu;
+    if (mag == 0 || mag >= 0x7f800000u) return false;
+    for (int k = 1; k < K; ++k)
+      if ((m->wb[static_cast<size_t>(o) * K + k] & 0x7fffffffu) != mag) return false;
+    memcpy(&m->alpha[o], &mag, sizeof(float));
+    m->unit = m->unit && mag == 0x3f800000u;
+  }
+  // x: an LceDequantize of packed signs q, read by the FULLY_CONNECTED alone
+  size_t di = kNoNode;
+  for (size_t k = 0; k < i && di == kNoNode; ++k)
+    if (nodes_[k]->node.outputs->size == 1 && nodes_[k]->node.outputs->data[0] == x) di = k;
+  if (di == kNoNode || SoleConsumer(x) != i) return false;
+  const NodeRecord& dq = *nodes_[di];
+  const int q = dq.node.inputs->size == 1 ? dq.node.inputs->data[0] : -1;
+  if (dq.name != "LceDequantize" || dq.initialized || q < 0 || tensors_[q].type != kTfLiteInt32) return false;
+  // q's words are the rows' words: each row is x's last axis (any K), or whole words of a map whose
+  // last axis packs without a padded word (C % 32 == 0, K % 32 == 0)
+  const TfLiteIntArray* qd = tensors_[q].dims;
+  const int last = xd->data[xd->size - 1];
+  if (!qd || qd->size != xd->size || qd->data[qd->size - 1] != (last + 31) / 32) return false;
+  for (int k = 0; k + 1 < xd->size; ++k)
+    if (qd->data[k] != xd->data[k]) return false;
+  if (last != K && (last % 32 != 0 || K % 32 != 0)) return false;
+  int64_t elems = 1;
+  for (int k = 0; k < xd->size; ++k) elems *= xd->data[k];
+  if (elems % K != 0 || elems / K > INT32_MAX) return false;
+  m->rows = elems / K;
+  const lce_bconv2d_desc d = FcDesc(m->rows, K, N);
+  if (!lce_b200_internal_fc_takes(&d)) return false;   // N % 64 == 0, the b1 mma.sync kernel
+  // the BatchNorm: MUL(scale [N]) as y's one reader, then ADD(shift [N]) as the product's one reader
+  size_t km = SoleConsumer(y), ka = kNoNode;
+  int scale = vec(PerChannelConstOp(km, kMul, y, N), N), shift = -1;
+  if (scale >= 0 && km > i) {
+    const int t1 = nodes_[km]->node.outputs->data[0];
+    ka = SoleConsumer(t1);
+    shift = vec(PerChannelConstOp(ka, kAdd, t1, N, /*any_activation=*/true), N);
+    if (shift < 0 || ka <= km || Activation(*nodes_[ka]) < LCE_ACT_NONE || Activation(*nodes_[ka]) > LCE_ACT_RELU6)
+      ka = kNoNode;
+  }
+  if (ka == kNoNode) {
+    km = kNoNode;
+    scale = shift = -1;
+  }
+  m->fc = i; m->dq = di; m->km = km; m->ka = ka;
+  m->q = q; m->w = w; m->K = K; m->N = N; m->bias = bias; m->scale = scale; m->shift = shift;
+  m->result = ka != kNoNode ? nodes_[ka]->node.outputs->data[0] : y;
+  return true;
+}
+
+void Graph::BinaryFcConstants(const BinaryFcMatch& m, int* filter, int* alpha) {
+  // the filter: each weight's sign bit, ceil(K / 32) words per output row
+  const int N = m.N, K = m.K, cw = (K + 31) / 32;
+  std::vector<int32_t> filt(static_cast<size_t>(N) * cw, 0);
+  for (int o = 0; o < N; ++o)
+    for (int k = 0; k < K; ++k)
+      if (m.wb[static_cast<size_t>(o) * K + k] >> 31) filt[static_cast<size_t>(o) * cw + (k >> 5)] |= static_cast<int32_t>(1u << (k & 31));
+  const std::string name = names_[m.w];
+  *filter = AddTensor(kTfLiteInt32, {N, 1, 1, cw}, filt.data(), filt.size() * sizeof(int32_t), false, 0.0f, 0,
+                      name + "_packed", /*const_on_device=*/true);
+  // alpha = 1.0 everywhere multiplies by nothing: the node reads no vector for it
+  *alpha = m.unit ? -1
+                  : AddTensor(kTfLiteFloat32, {N}, m.alpha.data(), m.alpha.size() * sizeof(float), false, 0.0f, 0,
+                              name + "_alpha", /*const_on_device=*/true);
+}
+
+int Graph::FuseBinaryFullyConnected() {
+  if (!device_arena_) return 0;
   auto fuse = [&](size_t i) -> int {   // nodes removed by fusing the FULLY_CONNECTED at i, 0 when it stays
-    NodeRecord& fc = *nodes_[i];
-    const BuiltinParams* fp = Params(fc);
-    if (fc.name != kFullyConnected || fc.initialized || !fp || fc.node.inputs->size < 2 || fc.node.inputs->size > 3 ||
-        fc.node.outputs->size != 1)
-      return 0;
-    const int x = fc.node.inputs->data[0], w = fc.node.inputs->data[1], y = fc.node.outputs->data[0];
-    const int bias_in = fc.node.inputs->size == 3 ? fc.node.inputs->data[2] : -1;
-    if (x < 0 || w < 0 || tensors_[w].type != kTfLiteFloat32 || tensors_[w].allocation_type != kTfLiteMmapRo ||
-        tensors_[x].type != kTfLiteFloat32 || tensors_[y].type != kTfLiteFloat32 || fp->keep_dims != 0 ||
-        fp->activation < LCE_ACT_NONE || fp->activation > LCE_ACT_RELU6)
-      return 0;
-    const TfLiteIntArray* wd = tensors_[w].dims;
-    const TfLiteIntArray* xd = tensors_[x].dims;
-    if (!wd || wd->size != 2 || !xd || xd->size < 1 || wd->data[0] <= 0 || wd->data[1] <= 0) return 0;
-    const int N = wd->data[0], K = wd->data[1];
-    const int bias = vec(bias_in, N);
-    if (bias_in >= 0 && bias < 0) return 0;
-    // every row o exactly +-alpha_o: one positive, finite magnitude, bitwise, in the whole row (no 0.0 or
-    // -0.0, no 0.5 among 1.0s)
-    const size_t nw = static_cast<size_t>(N) * K;
-    if (const_host_[w].size() < nw * sizeof(float)) return 0;
-    std::vector<uint32_t> wb(nw);
-    memcpy(wb.data(), const_host_[w].data(), nw * sizeof(float));
-    std::vector<float> alpha(N);
-    bool unit = true;
-    for (int o = 0; o < N; ++o) {
-      const uint32_t mag = wb[static_cast<size_t>(o) * K] & 0x7fffffffu;
-      if (mag == 0 || mag >= 0x7f800000u) return 0;
-      for (int k = 1; k < K; ++k)
-        if ((wb[static_cast<size_t>(o) * K + k] & 0x7fffffffu) != mag) return 0;
-      memcpy(&alpha[o], &mag, sizeof(float));
-      unit = unit && mag == 0x3f800000u;
-    }
-    // x: an LceDequantize of packed signs q, read by the FULLY_CONNECTED alone
-    size_t di = kNoNode;
-    for (size_t k = 0; k < i && di == kNoNode; ++k)
-      if (nodes_[k]->node.outputs->size == 1 && nodes_[k]->node.outputs->data[0] == x) di = k;
-    if (di == kNoNode || SoleConsumer(x) != i) return 0;
-    const NodeRecord& dq = *nodes_[di];
-    const int q = dq.node.inputs->size == 1 ? dq.node.inputs->data[0] : -1;
-    if (dq.name != "LceDequantize" || dq.initialized || q < 0 || tensors_[q].type != kTfLiteInt32) return 0;
-    // q's words are the rows' words: each row is x's last axis (any K), or whole words of a map whose
-    // last axis packs without a padded word (C % 32 == 0, K % 32 == 0)
-    const TfLiteIntArray* qd = tensors_[q].dims;
-    const int last = xd->data[xd->size - 1];
-    if (!qd || qd->size != xd->size || qd->data[qd->size - 1] != (last + 31) / 32) return 0;
-    for (int k = 0; k + 1 < xd->size; ++k)
-      if (qd->data[k] != xd->data[k]) return 0;
-    if (last != K && (last % 32 != 0 || K % 32 != 0)) return 0;
-    const int64_t elems = count(xd);
-    if (elems % K != 0 || elems / K > INT32_MAX) return 0;
-    lce_bconv2d_desc d;
-    memset(&d, 0, sizeof(d));
-    d.batch = static_cast<int>(elems / K); d.in_h = 1; d.in_w = 1; d.channels_in = K;
-    d.filter_h = 1; d.filter_w = 1; d.channels_out = N; d.groups = 1;
-    d.stride_h = 1; d.stride_w = 1; d.dilation_h = 1; d.dilation_w = 1;
-    d.padding = LCE_PADDING_VALID; d.pad_value = 1; d.activation = LCE_ACT_NONE; d.out_type = LCE_OUT_FLOAT;
-    if (!lce_b200_internal_fc_takes(&d)) return 0;   // N % 64 == 0, the b1 mma.sync kernel
-    // the BatchNorm: MUL(scale [N]) as y's one reader, then ADD(shift [N]) as the product's one reader
-    size_t km = SoleConsumer(y), ka = kNoNode;
-    int scale = vec(PerChannelConstOp(km, kMul, y, N), N), shift = -1;
-    if (scale >= 0 && km > i) {
-      const int t1 = nodes_[km]->node.outputs->data[0];
-      ka = SoleConsumer(t1);
-      shift = vec(PerChannelConstOp(ka, kAdd, t1, N, /*any_activation=*/true), N);
-      if (shift < 0 || ka <= km || Activation(*nodes_[ka]) < LCE_ACT_NONE || Activation(*nodes_[ka]) > LCE_ACT_RELU6)
-        ka = kNoNode;
-    }
-    if (ka == kNoNode) {
-      km = kNoNode;
-      scale = shift = -1;
-    }
-    const int s = ka != kNoNode ? nodes_[ka]->node.outputs->data[0] : y;
+    BinaryFcMatch m;
+    if (!MatchBinaryFc(i, &m)) return 0;
     // the signs: the result's only LceQuantize reader; the result itself stays stored
     size_t kq = kNoNode;
     int quantizers = 0;
-    for (size_t k : Consumers(s))
+    for (size_t k : Consumers(m.result))
       if (nodes_[k]->name == "LceQuantize") { ++quantizers; kq = k; }
-    const bool tail = quantizers == 1 && IsQuantize(kq) && kq > (ka != kNoNode ? ka : i);
-    std::vector<int> outs{s};
+    const bool tail = quantizers == 1 && IsQuantize(kq) && kq > (m.ka != kNoNode ? m.ka : i);
+    std::vector<int> outs{m.result};
     if (tail) outs.push_back(nodes_[kq]->node.outputs->data[0]);
-    // the filter: each weight's sign bit, ceil(K / 32) words per output row
-    const int cw = (K + 31) / 32;
-    std::vector<int32_t> filt(static_cast<size_t>(N) * cw, 0);
-    for (int o = 0; o < N; ++o)
-      for (int k = 0; k < K; ++k)
-        if (wb[static_cast<size_t>(o) * K + k] >> 31) filt[static_cast<size_t>(o) * cw + (k >> 5)] |= static_cast<int32_t>(1u << (k & 31));
-    const int ft = AddTensor(kTfLiteInt32, {N, 1, 1, cw}, filt.data(), filt.size() * sizeof(int32_t), false, 0.0f, 0,
-                             names_[w] + "_packed", /*const_on_device=*/true);
-    // alpha = 1.0 everywhere multiplies by nothing: the node reads no vector for it
-    const int at = unit ? -1
-                        : AddTensor(kTfLiteFloat32, {N}, alpha.data(), alpha.size() * sizeof(float), false, 0.0f, 0,
-                                    names_[w] + "_alpha", /*const_on_device=*/true);
+    int ft, at;
+    BinaryFcConstants(m, &ft, &at);
     struct {
       BuiltinParams fc, add;
       int32_t channels_in;
-    } params{*fp, ka != kNoNode ? *Params(*nodes_[ka]) : BuiltinParams{}, K};
+    } params{*Params(*nodes_[i]), m.ka != kNoNode ? *Params(*nodes_[m.ka]) : BuiltinParams{}, m.K};
     // the ADD's node (or without it the FULLY_CONNECTED's) becomes the fused one: q exists where it runs,
     // and every reader of the result and of the signs comes after it
-    NodeRecord& f = ka != kNoNode ? *nodes_[ka] : fc;
-    SetNodeIO(f, {q, ft, at, bias, scale, shift}, outs);
+    NodeRecord& f = m.ka != kNoNode ? *nodes_[m.ka] : *nodes_[i];
+    SetNodeIO(f, {m.q, ft, at, m.bias, m.scale, m.shift}, outs);
     SetBuiltinBlob(f, &params, sizeof(params));
     f.registration = BinaryFullyConnectedRegistration();
-    f.name = std::string("LceBfc") + (ka != kNoNode ? "+MUL+ADD" : "") + (tail ? "+LceQuantize" : "");
-    std::vector<size_t> gone{di};
-    if (ka != kNoNode) {
+    f.name = std::string("LceBfc") + (m.ka != kNoNode ? "+MUL+ADD" : "") + (tail ? "+LceQuantize" : "");
+    std::vector<size_t> gone{m.dq};
+    if (m.ka != kNoNode) {
       gone.push_back(i);
-      gone.push_back(km);
+      gone.push_back(m.km);
+    }
+    if (tail) gone.push_back(kq);
+    EraseNodes(gone);
+    return static_cast<int>(gone.size());
+  };
+  int removed = 0;
+  for (size_t i = 0; i < nodes_.size();) {
+    const int k = fuse(i);
+    removed += k;
+    i = k > 0 ? 0 : i + 1;   // indices moved: scan again (a fused node no longer matches)
+  }
+  allocated_ = false;
+  return removed;
+}
+
+int Graph::FuseBinaryFcMax() {
+  if (!device_arena_) return 0;
+  auto fuse = [&](size_t i) -> int {   // nodes removed by fusing the FULLY_CONNECTED at i, 0 when it stays
+    BinaryFcMatch m;
+    if (!MatchBinaryFc(i, &m)) return 0;
+    // the layer's result: [B, P, N], read by a REDUCE_MAX over axis 1 alone and not a graph output
+    const TfLiteIntArray* rd = tensors_[m.result].dims;
+    const size_t kr = SoleConsumer(m.result);
+    if (!rd || rd->size != 3 || rd->data[2] != m.N || rd->data[1] <= 0 || kr >= nodes_.size() ||
+        kr <= (m.ka != kNoNode ? m.ka : i))
+      return 0;
+    const NodeRecord& r = *nodes_[kr];
+    if (r.name != kReduceMax || r.initialized || !Params(r) || r.node.inputs->size != 2 || r.node.outputs->size != 1 ||
+        r.node.inputs->data[0] != m.result)
+      return 0;
+    const int axes = r.node.inputs->data[1], mx = r.node.outputs->data[0];
+    if (axes < 0 || tensors_[axes].type != kTfLiteInt32 || tensors_[axes].allocation_type != kTfLiteMmapRo ||
+        tensors_[mx].type != kTfLiteFloat32)
+      return 0;
+    const TfLiteIntArray* ad = tensors_[axes].dims;
+    int64_t na = 1;
+    for (int k = 0; ad && k < ad->size; ++k) na *= ad->data[k];
+    if (!ad || ad->size > 1 || const_host_[axes].size() < static_cast<size_t>(na) * sizeof(int32_t)) return 0;
+    std::vector<int32_t> av(static_cast<size_t>(na));
+    memcpy(av.data(), const_host_[axes].data(), av.size() * sizeof(int32_t));
+    if (av.empty()) return 0;
+    for (int32_t a : av)   // exactly the point axis (duplicates allowed)
+      if (a != 1 && a != -2) return 0;
+    const int points = rd->data[1];
+    const lce_bconv2d_desc d = FcDesc(m.rows, m.K, m.N);
+    if (m.rows != static_cast<int64_t>(rd->data[0]) * points || !lce_b200_internal_fc_max_takes(&d, points)) return 0;
+    // the signs: the max's only LceQuantize reader; the floats are stored only when something else reads them
+    size_t kq = kNoNode;
+    int quantizers = 0;
+    const std::vector<size_t> readers = Consumers(mx);
+    for (size_t k : readers)
+      if (nodes_[k]->name == "LceQuantize") { ++quantizers; kq = k; }
+    const bool tail = quantizers == 1 && IsQuantize(kq) && kq > kr;
+    const bool store = !tail || readers.size() > 1 || IsGraphOutput(mx);
+    std::vector<int> outs;
+    if (store) outs.push_back(mx);
+    if (tail) outs.push_back(nodes_[kq]->node.outputs->data[0]);
+    int ft, at;
+    BinaryFcConstants(m, &ft, &at);
+    BinaryFcMaxParams params{*Params(*nodes_[i]), m.ka != kNoNode ? *Params(*nodes_[m.ka]) : BuiltinParams{},
+                             *Params(r), m.K, points, store ? 1 : 0, tail ? 1 : 0};
+    // the REDUCE_MAX's node becomes the fused one: q exists where it runs, and every reader of the max
+    // and of its signs comes after it
+    NodeRecord& f = *nodes_[kr];
+    SetNodeIO(f, {m.q, ft, at, m.bias, m.scale, m.shift}, outs);
+    SetBuiltinBlob(f, &params, sizeof(params));
+    f.registration = BinaryFcMaxRegistration();
+    f.name = std::string("LceBfc") + (m.ka != kNoNode ? "+MUL+ADD" : "") + "+REDUCE_MAX" + (tail ? "+LceQuantize" : "");
+    std::vector<size_t> gone{m.dq, i};
+    if (m.ka != kNoNode) {
+      gone.push_back(m.km);
+      gone.push_back(m.ka);
     }
     if (tail) gone.push_back(kq);
     EraseNodes(gone);

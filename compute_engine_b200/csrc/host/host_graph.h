@@ -322,8 +322,27 @@ class Graph {
   // included) it is bit-identical; otherwise fl(fl(alpha * D) + b) is the real value rounded twice
   // where TFLite's loop rounds after each of its K terms: the two differ by up to about
   // K * 2^-24 * K * alpha_o, which can flip the next sign at a near-tie. fuse_all runs it right after
-  // FuseBinaryTransposeConvs; no pass before it matches a FULLY_CONNECTED. Returns the nodes removed.
+  // FuseBinaryTransposeConvs and FuseBinaryFcMax; no other pass before it matches a FULLY_CONNECTED.
+  // With keep_num_dims (the layer's input's last axis then being K) the result keeps the input's
+  // leading axes. Returns the nodes removed.
   int FuseBinaryFullyConnected();
+
+  // A binary point-wise layer and the max over its points, as a BiPointNet's last shared MLP layer and
+  // its global max-pool convert:
+  //   LceDequantize(q) -> FULLY_CONNECTED(+-alpha_o weights, bias?, activation, keep_num_dims)
+  //   [-> MUL(scale [N]) -> ADD(shift [N], activation)] -> REDUCE_MAX(axis 1 of [B, P, N]) [-> LceQuantize]
+  // becomes one node (lce_b200_bconv2d_run_fused_fc_max), "LceBfc[+MUL+ADD]+REDUCE_MAX[+LceQuantize]",
+  // inputs [q, packed filter, alpha, bias, scale, shift] as FuseBinaryFullyConnected's, outputs [max?,
+  // signs?], one temporary (the per-(image, column) keys). The [B, P, N] map is never stored; the max
+  // [B, N] only when a node other than the LceQuantize reads it or it is a graph output. Only under
+  // FuseBinaryFullyConnected's conditions, when the layer's result is [B, P, N], read by the REDUCE_MAX
+  // alone as its input and not a graph output, and the REDUCE_MAX's constant int32 axes are all the
+  // point axis (1 or -2). The LceQuantize joins when it is the max's only sign reader. Otherwise the
+  // graph is left as it is. Every value is the one FuseBinaryFullyConnected's node computes, and the
+  // max is TFLite's reference rule over them (NaN never chosen, the first of equal values), so the
+  // node's bits are the unfused pair's. fuse_all runs it right before FuseBinaryFullyConnected.
+  // Returns the nodes removed.
+  int FuseBinaryFcMax();
 
   // init (first time) + prepare of every node in order, then arena allocation.
   TfLiteStatus AllocateTensors();
@@ -388,6 +407,20 @@ class Graph {
   int PerChannelConstOp(size_t k, const char* op, int x, int C, bool any_activation = false) const;
   // Node k is an unprepared LceQuantize with one input and one int32 output (false for kNoNode).
   bool IsQuantize(size_t k) const;
+  // FuseBinaryFullyConnected's and FuseBinaryFcMax's match: the FULLY_CONNECTED at fc, the LceDequantize
+  // dq of q before it, its BatchNorm's MUL km and ADD ka (kNoNode without them), the constants, and the
+  // tensor the layer ends in (the ADD's output, or the FULLY_CONNECTED's).
+  struct BinaryFcMatch {
+    size_t fc, dq, km, ka;
+    int q, w, K, N, bias, scale, shift, result;
+    int64_t rows;
+    bool unit;                  // every alpha_o is 1.0
+    std::vector<uint32_t> wb;   // the [N, K] weights' bits
+    std::vector<float> alpha;
+  };
+  bool MatchBinaryFc(size_t i, BinaryFcMatch* m) const;
+  // The match's packed filter [N, 1, 1, ceil(K / 32)] and alpha [N] (-1 when unit) as new constants.
+  void BinaryFcConstants(const BinaryFcMatch& m, int* filter, int* alpha);
 
   // How the passes rewrite it. Each clears allocated_. A node they rewrite has not been prepared,
   // so its temporaries are the ones its pass gives it.

@@ -297,7 +297,8 @@ bool BuildGraphFromTflite(const uint8_t* data, size_t size, const OpResolver& re
         bp.axis = o.scalar<int32_t>(0, 0);
         bp.activation = o.scalar<int8_t>(1, 0);
         break;
-      case 40:  // MEAN: ReducerOptions (schema.fbs:1106)
+      case 40:
+      case 82:  // MEAN / REDUCE_MAX: ReducerOptions (schema.fbs:1106)
         bp.keep_dims = o.scalar<int8_t>(0, 0);
         break;
       case 22: {  // RESHAPE (schema.fbs:1044)

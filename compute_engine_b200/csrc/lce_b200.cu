@@ -194,21 +194,23 @@ size_t imma_smem_budget(int V, bool b1) {
 }
 
 template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
-          bool SPATIAL = false, bool GW = false, bool SHUFFLE = false>
+          bool SPATIAL = false, bool GW = false, bool SHUFFLE = false, bool FCMAX = false>
 int launch_imma_vo(const lce::ConvKParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.need())
-    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW, SHUFFLE>,
+    CUDA_OK(cudaFuncSetAttribute(lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW, SHUFFLE, FCMAX>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(imma_smem_budget(V, B1))));
-  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW, SHUFFLE><<<grid, lce::kIThreads, smem, s>>>(p);
+  lce::bconv_imma_kernel<V, OUT, B1, CHAIN, GATE, SLICE, SPATIAL, GW, SHUFFLE, FCMAX>
+      <<<grid, lce::kIThreads, smem, s>>>(p);
   g_path[1].fetch_add(1, std::memory_order_relaxed);
   return launch_check("bconv_imma_kernel");
 }
 // Epilogue tails of the float output beyond run_fused's (bconv_run_impl decides).
 // kScale: p.gate indexed by position within the image (lce_b200_bconv2d_run_fused_scale)
 // kShuffle: the pixel-shuffled store of lce_b200_bconv2d_run_fused_shuffle (p.shuf_*), b1 only
-enum class Tail { kNone, kChain, kGate, kScale, kSlice, kShuffle };   // p.chain / p.gate / p.out_stride in the epilogue
+// kFcMax: lce_b200_bconv2d_run_fused_fc_max's per-image column max (p.shuf_*, p.max_keys), b1 only
+enum class Tail { kNone, kChain, kGate, kScale, kSlice, kShuffle, kFcMax };   // p.chain / p.gate / p.out_stride in the epilogue
 
 // group-window plans (b1 only): every tail but the slice store
 template <int V>
@@ -220,7 +222,8 @@ int launch_imma_win_v(int out_type, Tail tail, const lce::ConvKParams& p, dim3 g
     case Tail::kGate: return launch_imma_vo<V, F, true, false, true, false, false, true>(p, grid, smem, s);
     case Tail::kScale: return launch_imma_vo<V, F, true, false, true, false, true, true>(p, grid, smem, s);
     case Tail::kSlice: return fail("bconv2d: the slice store takes no grouped plan with 32 * odd channels per group");
-    case Tail::kShuffle: return fail("bconv2d: the shuffle store takes no grouped plan");
+    case Tail::kShuffle:
+    case Tail::kFcMax: return fail("bconv2d: the shuffle store takes no grouped plan");
     case Tail::kNone: break;
   }
   if (out_type == LCE_OUT_BITPACKED)
@@ -250,6 +253,10 @@ int launch_imma_v(int out_type, bool b1, Tail tail, const lce::ConvKParams& p, d
   if (tail == Tail::kShuffle) {
     if (!b1) return fail("bconv2d: the shuffle store needs the b1 inner product");
     return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, false, false, false, false, true>(p, grid, smem, s);
+  }
+  if (tail == Tail::kFcMax) {
+    if (!b1) return fail("bconv2d: the max epilogue needs the b1 inner product");
+    return launch_imma_vo<V, LCE_OUT_FLOAT, true, false, false, false, false, false, false, true>(p, grid, smem, s);
   }
   if (b1) {
     if (out_type == LCE_OUT_FLOAT) return launch_imma_vo<V, LCE_OUT_FLOAT, true>(p, grid, smem, s);
@@ -1333,9 +1340,10 @@ static int bconv_run_impl(lce_b200_bconv2d* plan, const int32_t* in_dev, void* o
     p.shuf_act = shuffle->shuf_act; p.shuf_bias = shuffle->shuf_bias; p.shuf_k = shuffle->shuf_k;
     p.shuf_alpha = shuffle->shuf_alpha; p.shuf_scale = shuffle->shuf_scale; p.shuf_shift = shuffle->shuf_shift;
     p.shuf_act2 = shuffle->shuf_act2;
+    p.max_keys = shuffle->max_keys; p.fd_pts = shuffle->fd_pts;
     p.cw_out = shuffle->shuf_c / 32;
     if (!takes_imma(c, p)) return fail("bconv2d_run_fused_shuffle / _fc: the plan does not run on the mma.sync kernel");
-    return launch_conv(c, p, s, Tail::kShuffle);
+    return launch_conv(c, p, s, shuffle->max_keys != nullptr ? Tail::kFcMax : Tail::kShuffle);
   }
   // run_slice / run_slice_add: the mma.sync kernel's strided store, and the residual read at the
   // same strided address (the caller checked that the kernel takes the plan)
@@ -1633,6 +1641,87 @@ int lce_b200_bconv2d_run_fused_fc(lce_b200_bconv2d* plan, const int32_t* in_dev,
 // host-internal (Graph::FuseBinaryFullyConnected): lce_b200_bconv2d_run_fused_fc takes a plan created
 // now from *d; no device needed
 int lce_b200_internal_fc_takes(const lce_bconv2d_desc* d) { return fc_refusal(*d, nullptr) == nullptr; }
+
+// The keys of lce_b200_bconv2d_run_fused_fc_max as floats (max_key_value), one thread per (image,
+// column), and each 32 columns' signs packed by a ballot (N % 32 == 0): keys [B][N], out [B][N] or
+// null, packed [B][N / 32] or null.
+__global__ void __launch_bounds__(256) fc_max_finalize_kernel(const unsigned long long* __restrict__ keys,
+                                                              long long total, float* __restrict__ out,
+                                                              int32_t* __restrict__ packed) {
+  // total % 32 == 0: every warp is whole
+  for (long long i = blockIdx.x * 256LL + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * 256) {
+    const float v = lce::max_key_value(keys[i]);
+    if (out) out[i] = v;
+    const unsigned bits = __ballot_sync(0xffffffffu, v < 0.0f);
+    if (packed && (threadIdx.x & 31) == 0) packed[i / 32] = static_cast<int32_t>(bits);
+  }
+}
+
+static const char* fc_max_refusal(const lce_bconv2d_desc& d, int points, const GemmCore* c) {
+  if (points <= 0 || d.batch % points != 0) return "batch rows a whole number of images of `points` rows";
+  return fc_refusal(d, c);
+}
+
+int lce_b200_bconv2d_run_fused_fc_max(lce_b200_bconv2d* plan, const int32_t* in_dev, const float* alpha_dev,
+                                      const float* bias_dev, int activation, const float* scale_dev,
+                                      const float* shift_dev, int bn_activation, int points, void* keys_dev,
+                                      float* max_out_dev, int32_t* packed_out_dev, void* stream) {
+  const lce_bconv2d_desc& d = plan->d;
+  if (const char* why = fc_max_refusal(d, points, &plan->core))
+    return fail("bconv2d_run_fused_fc_max: the plan needs %s", why);
+  for (int a : {activation, bn_activation})
+    if (a < LCE_ACT_NONE || a > LCE_ACT_RELU6) return fail("bconv2d_run_fused_fc_max: unknown activation %d", a);
+  if (!aligned16(keys_dev)) return fail("bconv2d_run_fused_fc_max: keys must be 16-byte aligned");
+  if (!max_out_dev && !packed_out_dev) return fail("bconv2d_run_fused_fc_max: max_out and packed_out are both null");
+  for (const float* v : {alpha_dev, bias_dev, scale_dev, shift_dev}) {
+    if (v && (reinterpret_cast<uintptr_t>(v) & 7u) != 0)
+      return fail("bconv2d_run_fused_fc_max: alpha, bias, scale and shift must be 8-byte aligned");
+    if (v && !is_device_ptr(v))
+      return fail("bconv2d_run_fused_fc_max: alpha, bias, scale and shift must be device memory");
+  }
+  const long long rows = d.batch;
+  if (rows >= (1LL << 31) - lce::kIBM) return fail("bconv2d_run_fused_fc_max: too many rows (%lld)", rows);
+  if (rows == 0) return 0;
+  const int n = d.channels_out;
+  const long long images = rows / points, total = images * n;
+  const size_t in_bytes = static_cast<size_t>(rows) * cdiv(d.channels_in, 32) * 4;
+  const size_t key_bytes = static_cast<size_t>(total) * 8, out_bytes = static_cast<size_t>(total) * 4;
+  const size_t pk_bytes = static_cast<size_t>(total / 32) * 4;
+  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+    return a != nullptr && b != nullptr && a0 < b0 + nb && b0 < a0 + na;
+  };
+  if (overlap(keys_dev, key_bytes, in_dev, in_bytes) || overlap(keys_dev, key_bytes, max_out_dev, out_bytes) ||
+      overlap(keys_dev, key_bytes, packed_out_dev, pk_bytes) || overlap(max_out_dev, out_bytes, packed_out_dev, pk_bytes))
+    return fail("bconv2d_run_fused_fc_max: keys, max_out and packed_out must not overlap each other or the input");
+  cudaStream_t s = as_stream(stream);
+  // every key starts below every value's: replays and reused memory give the same bits
+  CUDA_OK(cudaMemsetAsync(keys_dev, 0, key_bytes, s));
+  const lce::ConvKParams fc = [&] {
+    lce::ConvKParams q;
+    memset(&q, 0, sizeof(q));
+    q.shuf_sh = 1; q.shuf_sw = 1; q.shuf_c = n; q.shuf_k = d.channels_in;
+    q.shuf_act = activation; q.shuf_bias = bias_dev; q.shuf_alpha = alpha_dev;
+    q.shuf_scale = scale_dev; q.shuf_shift = shift_dev; q.shuf_act2 = bn_activation;
+    q.max_keys = static_cast<unsigned long long*>(keys_dev);
+    q.fd_pts = lce::make_fastdiv(static_cast<uint32_t>(points));
+    return q;
+  }();
+  // keys_dev stands in for the output: the instance stores nothing there but reads its alignment
+  const int rc = bconv_run_impl(plan, in_dev, keys_dev, nullptr, LCE_ACT_NONE, nullptr, nullptr, stream, nullptr, 0,
+                                nullptr, false, &fc);
+  if (rc) return rc;
+  const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 148LL * 16));
+  fc_max_finalize_kernel<<<grid, 256, 0, s>>>(static_cast<const unsigned long long*>(keys_dev), total, max_out_dev,
+                                              packed_out_dev);
+  return launch_check("fc_max_finalize_kernel");
+}
+
+// host-internal (Graph::FuseBinaryFcMax): lce_b200_bconv2d_run_fused_fc_max takes a plan created now
+// from *d with images of `points` rows; no device needed
+int lce_b200_internal_fc_max_takes(const lce_bconv2d_desc* d, int points) {
+  return fc_max_refusal(*d, points, nullptr) == nullptr;
+}
 
 // Whether lce_b200_bconv2d_run_slice will take a plan created now from *d
 // (Graph::FuseDenseBlocks asks before it rewrites the graph).

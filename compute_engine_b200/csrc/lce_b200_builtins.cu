@@ -1421,6 +1421,57 @@ __global__ void __launch_bounds__(256) argmax_warp_kernel(const float* __restric
   }
 }
 
+// REDUCE_MAX (lce_b200_f32_reduce_max). One thread per (outer, inner) position, walking the axis as the
+// reference does (cur = -FLT_MAX, then cur = x > cur ? x : cur): adjacent threads read adjacent inner
+// positions, so the loads coalesce when inner > 1; at inner == 1 (short rows) each thread reads its own row.
+__global__ void __launch_bounds__(256) reduce_max_kernel(const float* __restrict__ in, long long outer, long long n,
+                                                         long long inner, float* __restrict__ out) {
+  const long long total = outer * inner;
+  for (long long p = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; p < total;
+       p += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long o = p / inner;
+    const float* x = in + o * n * inner + (p - o * inner);
+    float cur = -FLT_MAX;
+    for (long long i = 0; i < n; ++i) {
+      const float xi = __ldg(x + i * inner);
+      cur = xi > cur ? xi : cur;
+    }
+    out[p] = cur;
+  }
+}
+
+// One warp per row at inner == 1 (long rows): lane l walks elements l, l + 32, ... by the same rule and
+// keeps the index of its value (-1 for the initial one); the lanes then merge, the larger value or of
+// equal ones the lower index winning, which is what the sequential walk keeps.
+__global__ void __launch_bounds__(256) reduce_max_warp_kernel(const float* __restrict__ in, long long rows,
+                                                              long long n, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
+  for (long long r = blockIdx.x * static_cast<long long>(blockDim.x >> 5) + (threadIdx.x >> 5); r < rows;
+       r += warps) {
+    const float* x = in + r * n;
+    float v = -FLT_MAX;
+    long long idx = LLONG_MAX;
+    for (long long i = lane; i < n; i += 32) {
+      const float xi = __ldg(x + i);
+      if (xi > v) {
+        v = xi;
+        idx = i;
+      }
+    }
+#pragma unroll
+    for (int off = 16; off; off >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, v, off);
+      const long long oi = __shfl_xor_sync(0xffffffffu, idx, off);
+      if (ov > v || (ov == v && oi < idx)) {
+        v = ov;
+        idx = oi;
+      }
+    }
+    if (lane == 0) out[r] = v;
+  }
+}
+
 // RESIZE_BILINEAR -> ARG_MAX over the channel axis in one pass, by output rows as
 // resize_bilinear_kernel: blockIdx.y strides over the B * OH output rows. The CTA stages the row's two
 // source rows y0 and y1 (in_w * C floats each, as float4s when both are 16-byte aligned) in shared
@@ -3165,6 +3216,21 @@ int lce_b200_f32_argmax(const float* in, int64_t outer, int n, int64_t inner, in
   if (out_int64) argmax_kernel<int64_t><<<grid, 256, 0, s>>>(in, outer, n, inner, static_cast<int64_t*>(out));
   else argmax_kernel<int32_t><<<grid, 256, 0, s>>>(in, outer, n, inner, static_cast<int32_t*>(out));
   return launch_check("argmax_kernel");
+}
+
+int lce_b200_f32_reduce_max(const float* in, int64_t outer, int64_t n, int64_t inner, float* out, void* stream) {
+  if (outer < 0 || inner < 0 || n < 0)
+    return fail("reduce_max: bad shape (%lld x %lld x %lld)", static_cast<long long>(outer), static_cast<long long>(n),
+                static_cast<long long>(inner));
+  if (outer == 0 || inner == 0) return 0;
+  if (!out || (n > 0 && !in)) return fail("reduce_max: null tensor");
+  cudaStream_t s = as_stream(stream);
+  if (inner == 1 && n >= kArgmaxWarpRow) {
+    reduce_max_warp_kernel<<<grid_for(outer, 8), 256, 0, s>>>(in, outer, n, out);
+    return launch_check("reduce_max_warp_kernel");
+  }
+  reduce_max_kernel<<<grid_for(outer * inner, 256), 256, 0, s>>>(in, outer, n, inner, out);
+  return launch_check("reduce_max_kernel");
 }
 
 // The two staged source rows of bilinear_argmax_kernel fit the default 48 KB of dynamic shared memory.

@@ -338,6 +338,42 @@ __device__ __forceinline__ void zero_pad_correction_imma(const ConvKParams& p,
   }
 }
 
+// Columns c and c + 1 of the SHUFFLE store, from the +-1 dot products y0, y1: FULLY_CONNECTED's alpha
+// (run_fused_fc), one rounding; TRANSPOSE_CONV's or FULLY_CONNECTED's bias, one rounding, then its
+// activation; then run_fused_fc's BatchNorm, MUL and ADD rounded apart as TFLite's ops round them, and
+// the ADD's activation. Each vector is read here, per column pair, so none stays in registers.
+__device__ __forceinline__ float act_clamp(float y, int act) {
+  if (act == LCE_ACT_NONE) return y;
+  const float lo = act == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
+  const float hi = act == LCE_ACT_RELU ? __int_as_float(0x7f800000) : (act == LCE_ACT_RELU6 ? 6.0f : 1.0f);
+  return fminf(fmaxf(y, lo), hi);
+}
+__device__ __forceinline__ float2 fc_steps(const ConvKParams& p, int c, float y0, float y1) {
+  if (p.shuf_alpha != nullptr) {
+    const float2 a = __ldg(reinterpret_cast<const float2*>(p.shuf_alpha + c));
+    y0 = __fmul_rn(y0, a.x);
+    y1 = __fmul_rn(y1, a.y);
+  }
+  if (p.shuf_bias != nullptr) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(p.shuf_bias + c));
+    y0 = __fadd_rn(y0, b.x);
+    y1 = __fadd_rn(y1, b.y);
+  }
+  y0 = act_clamp(y0, p.shuf_act);
+  y1 = act_clamp(y1, p.shuf_act);
+  if (p.shuf_scale != nullptr) {
+    const float2 a = __ldg(reinterpret_cast<const float2*>(p.shuf_scale + c));
+    y0 = __fmul_rn(y0, a.x);
+    y1 = __fmul_rn(y1, a.y);
+  }
+  if (p.shuf_shift != nullptr) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(p.shuf_shift + c));
+    y0 = __fadd_rn(y0, b.x);
+    y1 = __fadd_rn(y1, b.y);
+  }
+  return make_float2(act_clamp(y0, p.shuf_act2), act_clamp(y1, p.shuf_act2));
+}
+
 // Accumulator (ms, ns, e) of thread (gid, tig): pixel m0 + warp*32 + ms*16 + (e/2)*8 + gid,
 // channel c_tile + ns*8 + tig*2 + (e & 1), at scale 2^S. Full 64-channel tiles only
 // (host-checked). CHAIN (float output): ReActNet's chain on the fused sum. Its four vectors and
@@ -468,57 +504,12 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
           }
         }
         if constexpr (SHUFFLE) {
-          // FULLY_CONNECTED's alpha (run_fused_fc), one rounding; TRANSPOSE_CONV's or FULLY_CONNECTED's
-          // bias, one rounding, then its activation; then run_fused_fc's BatchNorm, MUL and ADD rounded
-          // apart as TFLite's ops round them, and the ADD's activation. Each vector is read per ns.
           const int cv = c_sh + tig * 2;
-          if (p.shuf_alpha != nullptr) {
 #pragma unroll
-            for (int ns = 0; ns < 8; ++ns) {
-              const float2 a = __ldg(reinterpret_cast<const float2*>(p.shuf_alpha + cv + ns * 8));
-              y[2 * ns] = __fmul_rn(y[2 * ns], a.x);
-              y[2 * ns + 1] = __fmul_rn(y[2 * ns + 1], a.y);
-            }
-          }
-          if (p.shuf_bias != nullptr) {
-#pragma unroll
-            for (int ns = 0; ns < 8; ++ns) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.shuf_bias + cv + ns * 8));
-              y[2 * ns] = __fadd_rn(y[2 * ns], b.x);
-              y[2 * ns + 1] = __fadd_rn(y[2 * ns + 1], b.y);
-            }
-          }
-          const int sact = p.shuf_act;
-          if (sact != LCE_ACT_NONE) {
-            const float s_lo = sact == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
-            const float s_hi =
-                sact == LCE_ACT_RELU ? __int_as_float(0x7f800000) : (sact == LCE_ACT_RELU6 ? 6.0f : 1.0f);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], s_lo), s_hi);
-          }
-          if (p.shuf_scale != nullptr) {
-#pragma unroll
-            for (int ns = 0; ns < 8; ++ns) {
-              const float2 a = __ldg(reinterpret_cast<const float2*>(p.shuf_scale + cv + ns * 8));
-              y[2 * ns] = __fmul_rn(y[2 * ns], a.x);
-              y[2 * ns + 1] = __fmul_rn(y[2 * ns + 1], a.y);
-            }
-          }
-          if (p.shuf_shift != nullptr) {
-#pragma unroll
-            for (int ns = 0; ns < 8; ++ns) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.shuf_shift + cv + ns * 8));
-              y[2 * ns] = __fadd_rn(y[2 * ns], b.x);
-              y[2 * ns + 1] = __fadd_rn(y[2 * ns + 1], b.y);
-            }
-          }
-          const int sact2 = p.shuf_act2;
-          if (sact2 != LCE_ACT_NONE) {
-            const float s_lo = sact2 == LCE_ACT_RELU_N1_TO_1 ? -1.0f : 0.0f;
-            const float s_hi =
-                sact2 == LCE_ACT_RELU ? __int_as_float(0x7f800000) : (sact2 == LCE_ACT_RELU6 ? 6.0f : 1.0f);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = fminf(fmaxf(y[j], s_lo), s_hi);
+          for (int ns = 0; ns < 8; ++ns) {
+            const float2 r = fc_steps(p, cv + ns * 8, y[2 * ns], y[2 * ns + 1]);
+            y[2 * ns] = r.x;
+            y[2 * ns + 1] = r.y;
           }
         }
         if constexpr (GATE) {
@@ -642,14 +633,68 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
   }
 }
 
+// FCMAX (b1, lce_b200_bconv2d_run_fused_fc_max): the columns run_fused_fc stores (SHUFFLE with sh =
+// sw = 1, fc_steps), but each column's max over the rows of each image instead of the rows. Row m
+// belongs to image m / points (p.fd_pts); the thread's four rows m0 + warp * 32 + {0, 8, 16, 24} + gid
+// come in row order, so it keeps one key (max_key) per image run and column and merges a run into
+// p.max_keys[image][column] with atomicMax when its image ends. When the warp's 32 rows all belong to
+// one image, its eight lanes of each column merge first and one of them writes. Column pair by column
+// pair, so the accumulators of a pair die as it is done.
+__device__ __forceinline__ void epilogue_fc_max(const ConvKParams& p, int (&acc)[2][8][4], long long m0,
+                                                int c_tile, int warp, int gid, int tig) {
+  const long long mw = m0 + warp * 32;   // the warp's first row (M < 2^31, host-checked)
+  uint32_t img[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) img[r] = fdiv(static_cast<uint32_t>(mw + r * 8 + gid), p.fd_pts);
+  const bool one = mw + 31 < p.M &&
+                   fdiv(static_cast<uint32_t>(mw), p.fd_pts) == fdiv(static_cast<uint32_t>(mw + 31), p.fd_pts);
+  auto merge = [&](uint32_t b, int c, unsigned long long k0, unsigned long long k1) {
+    unsigned long long* kp = p.max_keys + static_cast<size_t>(b) * p.cout + c;
+    if (k0) atomicMax(kp, k0);
+    if (k1) atomicMax(kp + 1, k1);
+  };
+#pragma unroll
+  for (int ns = 0; ns < 8; ++ns) {
+    const int c = c_tile + ns * 8 + tig * 2;
+    unsigned long long k0 = 0, k1 = 0;
+    uint32_t cur = img[0];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const long long m = mw + r * 8 + gid;
+      if (m >= p.M) break;
+      if (img[r] != cur) {
+        merge(cur, c, k0, k1);
+        k0 = k1 = 0;
+        cur = img[r];
+      }
+      // the +-1 dot product D = K - 2 popc(a ^ w), as the SHUFFLE store takes it
+      const int x0 = acc[r >> 1][ns][(r & 1) * 2] << 1, x1 = acc[r >> 1][ns][(r & 1) * 2 + 1] << 1;
+      const float2 y = fc_steps(p, c, static_cast<float>(p.shuf_k - x0), static_cast<float>(p.shuf_k - x1));
+      k0 = max(k0, max_key(y.x, static_cast<uint32_t>(m)));
+      k1 = max(k1, max_key(y.y, static_cast<uint32_t>(m)));
+    }
+    if (one) {   // uniform across the warp
+#pragma unroll
+      for (int off = 4; off < 32; off <<= 1) {
+        k0 = max(k0, __shfl_xor_sync(0xffffffffu, k0, off));
+        k1 = max(k1, __shfl_xor_sync(0xffffffffu, k1, off));
+      }
+      if (gid == 0) merge(cur, c, k0, k1);
+    } else {
+      merge(cur, c, k0, k1);
+    }
+  }
+}
+
 // B1 selects the inner product: packed b1 fragments (accumulators at scale 1) or int8 ones
 // (scale 8). Both produce the same int32 accumulators. CHAIN (float output): the epilogue also
 // applies p.chain (lce_b200_bconv2d_run_fused_chain); GATE (float output): p.gate
 // (lce_b200_bconv2d_run_fused_gate), with SPATIAL p.gate indexed by position
 // (lce_b200_bconv2d_run_fused_scale); SLICE (float output): the strided store of
 // lce_b200_bconv2d_run_slice, and its read-add-write in lce_b200_bconv2d_run_slice_add; SHUFFLE (b1,
-// float output): the pixel-shuffled store of lce_b200_bconv2d_run_fused_shuffle. The other
-// instances compile as without them.
+// float output): the pixel-shuffled store of lce_b200_bconv2d_run_fused_shuffle; FCMAX (b1): its
+// run_fused_fc columns reduced to each image's max (epilogue_fc_max). The other instances compile as
+// without them.
 // GW (b1 only): a grouped plan whose groups hold 32 * odd output channels, so a 64-channel tile on
 // 64-aligned channels may span two groups. Tile nt covers channels nt * 64 .. nt * 64 + 63 and
 // gathers, per tap, the contiguous input words of two neighbouring groups (its window, from group
@@ -658,11 +703,13 @@ __device__ __forceinline__ void epilogue_imma(const ConvKParams& p, int (&acc)[2
 // window group's bits apart (compute_chunk_b1), so every channel gets popc(a ^ w) over its own
 // group alone: the XOR + POPC kernel's integers.
 template <int V, int OUT, bool B1, bool CHAIN = false, bool GATE = false, bool SLICE = false,
-          bool SPATIAL = false, bool GW = false, bool SHUFFLE = false>
+          bool SPATIAL = false, bool GW = false, bool SHUFFLE = false, bool FCMAX = false>
 __global__ void __launch_bounds__(kIThreads, B1 ? b1_ctas_per_sm(GW, OUT) : imma_ctas_per_sm(V))
 bconv_imma_kernel(const ConvKParams p) {
   static_assert(!GW || (B1 && !SLICE), "group windows: b1, no slice store");
   static_assert(!SHUFFLE || B1, "the shuffle store: b1 only");
+  static_assert(!FCMAX || (B1 && OUT == LCE_OUT_FLOAT && !CHAIN && !GATE && !SLICE && !GW && !SHUFFLE),
+                "the max epilogue: b1, float columns, no other tail");
   using Vec = typename VecT<V>::T;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   // two buffers of { A: [Kc_v][128] packed vectors, B: [Kc_v*V][8][32] int8 fragments }, or for
@@ -812,6 +859,8 @@ bconv_imma_kernel(const ConvKParams p) {
     }
     __syncthreads();
     epilogue_imma<OUT, S, false, true, false, SPATIAL, GW>(p, acc, m0, c_tile, warp, gid, tig, cs);
+  } else if constexpr (FCMAX) {
+    epilogue_fc_max(p, acc, m0, c_tile, warp, gid, tig);
   } else {
     epilogue_imma<OUT, S, false, false, SLICE, false, GW, SHUFFLE>(p, acc, m0, c_tile, warp, gid, tig);
   }

@@ -60,6 +60,30 @@ __device__ __forceinline__ uint32_t fdiv(uint32_t n, FastDiv d) {
   return static_cast<uint32_t>((static_cast<unsigned long long>(n) * d.mul) >> d.shift);
 }
 
+// REDUCE_MAX's rule (TFLite's reference reduction: cur = lowest(), then cur = in > cur ? in : cur in
+// index order) as a 64-bit key that atomicMax can merge in any order. High word: the value's
+// order-preserving key, -0.0 and +0.0 one key; low word: the complemented row index (rows < 2^31),
+// so that the first of equal values wins, and below it the value's sign bit, which tells the zeros
+// apart. A NaN is never chosen: its key is 0, below every value's.
+__device__ __forceinline__ uint32_t max_key_hi(float v) {
+  uint32_t b = __float_as_uint(v);
+  if ((b & 0x7fffffffu) == 0) b = 0;
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ unsigned long long max_key(float v, uint32_t row) {
+  if (v != v) return 0ull;
+  return (static_cast<unsigned long long>(max_key_hi(v)) << 32) | ((0x7fffffffu - row) << 1) |
+         (__float_as_uint(v) >> 31);
+}
+// The key's value: -FLT_MAX when no key beats the initial value's (no value, NaNs, -inf only).
+__device__ __forceinline__ float max_key_value(unsigned long long key) {
+  const uint32_t hi = static_cast<uint32_t>(key >> 32);
+  if (hi <= max_key_hi(-3.402823466e38f)) return -3.402823466e38f;
+  uint32_t b = (hi & 0x80000000u) ? (hi & 0x7fffffffu) : ~hi;
+  if (b == 0 && (key & 1ull)) b = 0x80000000u;
+  return __uint_as_float(b);
+}
+
 // Fused shortcut: each thread parks its own 4 x 8 residual values (8 x 16 B) in shared memory
 // with cp.async at kernel start, so the epilogue never waits on L2 / HBM.
 constexpr int kResStageBytes = kThreads * 8 * 16;
@@ -115,6 +139,10 @@ struct ConvKParams {
   const float* shuf_scale;
   const float* shuf_shift;
   int shuf_act2;
+  // FCMAX instances only (lce_b200_bconv2d_run_fused_fc_max): the same columns, never stored; each
+  // one's max over the rows of each image (fd_pts: / points per image) goes into max_keys [B][cout]
+  unsigned long long* max_keys;
+  FastDiv fd_pts;
   // mma.sync kernel, group-window (GW) instances only: 8 % (2 * Cw_pg), a k-slice's step through
   // the window
   int win_step;

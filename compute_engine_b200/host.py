@@ -284,6 +284,14 @@ class HostGraph:
         Graph::FuseBinaryFullyConnected states. Call before allocate_tensors."""
         return lib().lce_host_fuse_binary_fully_connected(self._g)
 
+    def fuse_binary_fc_max(self):
+        """LceDequantize -> FULLY_CONNECTED (+-alpha_o weights, N % 64 == 0) [-> MUL -> ADD] -> REDUCE_MAX
+        over the points of [B, P, N] [-> LceQuantize] (a binary PointNet's last shared layer and its max
+        pool) => one node that runs the layer on the b1 tensor instruction and reduces each image's
+        columns in its store, never writing the [B, P, N] map. The same bits as the unfused ops under
+        fuse_binary_fully_connected. Call before fuse_binary_fully_connected and allocate_tensors."""
+        return lib().lce_host_fuse_binary_fc_max(self._g)
+
     def fuse_residual_pairs(self):
         """Two consecutive LceBconv2d+ADD[+LceQuantize] blocks whose intermediate nothing else
         reads => one node that keeps it on chip. Call after the other fusions."""
@@ -291,7 +299,7 @@ class HostGraph:
 
     def fuse_all(self):
         return (self.fuse_binary_bases() + self.fuse_dense_blocks() + self.fuse_binary_transpose_convs()
-                + self.fuse_binary_fully_connected() + self.fuse_residual_blocks()
+                + self.fuse_binary_fc_max() + self.fuse_binary_fully_connected() + self.fuse_residual_blocks()
                 + self.fuse_spatial_scales()
                 + self.fuse_float_glue() + self.fuse_upsample_merges() + self.fuse_resize_argmax()
                 + self.fuse_subpixel_convs()

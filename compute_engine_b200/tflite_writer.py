@@ -114,13 +114,13 @@ OP = {"ADD": 0, "AVERAGE_POOL_2D": 1, "CONV_2D": 3, "DEPTHWISE_CONV_2D": 4,
       "DEQUANTIZE": 6, "PRELU": 54, "LOGISTIC": 14, "STRIDED_SLICE": 45, "SPLIT": 49,
       "DIV": 42, "MAXIMUM": 55, "MINIMUM": 57, "ROUND": 116, "RESIZE_BILINEAR": 23,
       "RESIZE_NEAREST_NEIGHBOR": 97, "ARG_MAX": 56, "DEPTH_TO_SPACE": 5,
-      "TRANSPOSE_CONV": 67}
+      "TRANSPOSE_CONV": 67, "REDUCE_MAX": 82}
 # BuiltinOptions union tags (schema_generated.h:1652-1694)
 OPT_TAG = {"CONV_2D": 1, "DEPTHWISE_CONV_2D": 2, "AVERAGE_POOL_2D": 5, "MAX_POOL_2D": 5,
            "FULLY_CONNECTED": 8, "SOFTMAX": 9, "ADD": 11, "MUL": 21, "RESHAPE": 17, "MEAN": 27,
            "CONCATENATION": 10, "PAD": 22, "PADV2": 43, "STRIDED_SLICE": 32, "SPLIT": 35, "DIV": 29,
            "RESIZE_BILINEAR": 15, "RESIZE_NEAREST_NEIGHBOR": 74, "ARG_MAX": 40, "DEPTH_TO_SPACE": 94,
-           "TRANSPOSE_CONV": 49}
+           "TRANSPOSE_CONV": 49, "REDUCE_MAX": 27}
 PADDING = {"SAME": 0, "VALID": 1}
 ACT = {"NONE": 0, "RELU": 1, "RELU_N1_TO_1": 2, "RELU6": 3}
 
@@ -163,15 +163,16 @@ class TFLiteModel:
             return fb.table({0: ("b", PADDING[o["padding"]]), 1: ("i", o["stride"][1]),
                              2: ("i", o["stride"][0]), 3: ("i", o["filter"][1]),
                              4: ("i", o["filter"][0]), 5: ("b", act)})
-        if kind == "FULLY_CONNECTED":
-            return fb.table({0: ("b", act)})
+        if kind == "FULLY_CONNECTED":   # field 2, keep_num_dims, only when passed: other models keep their bytes
+            keep = ("b", 1 if o["keep_num_dims"] else 0) if "keep_num_dims" in o else None
+            return fb.table({0: ("b", act), 2: keep})
         if kind == "SOFTMAX":
             return fb.table({0: ("f", float(o.get("beta", 1.0)))})
         if kind in ("ADD", "MUL", "DIV"):
             return fb.table({0: ("b", act)})
         if kind == "RESHAPE":
             return fb.table({0: ("o", fb.scalar_vector("i", o["new_shape"]))})
-        if kind == "MEAN":
+        if kind in ("MEAN", "REDUCE_MAX"):   # ReducerOptions: keep_dims
             return fb.table({0: ("b", 1 if o.get("keep_dims", False) else 0)})
         if kind == "CONCATENATION":
             return fb.table({0: ("i", int(o.get("axis", 0))), 1: ("b", act)})

@@ -1151,6 +1151,79 @@ def dorefanet(batch=1, seed=0, image=224, input_type="float32"):
     return g.m.serialize()
 
 
+def binary_pointnet(batch=1, seed=0, points=1024, classes=40, widths=(64, 64, 64, 128, 1024), head=(512, 256),
+                    alpha=None):
+    """BiPointNet (Qin et al., ICLR 2021): vanilla PointNet classification without the T-Nets, its shared
+    MLPs binary, with synthetic weights, in the op order the converter leaves larq's layers in:
+      input float32 [B, P, 3] (P = `points`);
+      stem FULLY_CONNECTED 3 -> widths[0] (float weights, bias, keep_num_dims) -> MUL -> ADD, the BatchNorm
+      unfolded, without a RELU: the next layer takes its signs, which after a RELU would all be +1;
+      each further width n: LceQuantize -> LceDequantize -> FULLY_CONNECTED(+-alpha weights, no bias,
+      keep_num_dims) [B, P, n] -> MUL -> ADD (the BatchNorm), larq's QuantDense on [B, P, C];
+      REDUCE_MAX over the points (axis 1) -> [B, widths[-1]], the global max pool (BiPointNet's EMA-max
+      offset, here about the expected max of the last layer's dot products over P points, is a constant
+      before the max, so it is folded into the last shift);
+      the head: for each width in `head` LceQuantize -> LceDequantize -> FULLY_CONNECTED(+-alpha) -> MUL
+      -> ADD, then a float FULLY_CONNECTED -> `classes` with bias and SOFTMAX.
+    alpha=None: +-1.0 weights. alpha="lsr": each binary layer's weights +-alpha with one scale per layer
+    that is not a power of two, BiPointNet's layer-wise scale recovery. Not in MODELS."""
+    if alpha not in (None, "lsr"):
+        raise ValueError(f"binary_pointnet alpha must be None or 'lsr', not {alpha!r}")
+    g = _Builder(seed, batch, "BiPointNet")
+    b = batch
+    x = g.m.add_tensor("input", (b, points, 3), np.float32)
+    g.m.inputs = [x]
+
+    def bn_tail(y, shape, n, activation="NONE", offset=0.0):
+        scale, shift = g.bn(n)
+        shift = (shift - np.float32(offset) * scale).astype(np.float32)
+        u = g.act(shape)
+        g.m.add_op("MUL", [y, g.const(scale, name="bn_scale")], [u])
+        return g.add(u, g.const(shift, name="bn_shift"), shape, activation)
+
+    def binary_layer(x, lead, k, n, offset=0.0):
+        q = g.act(lead + ((k + 31) // 32,), np.int32)
+        g.m.add_op("LceQuantize", [x], [q], custom_options=b"")
+        deq = g.act(lead + (k,))
+        g.m.add_op("LceDequantize", [q], [deq], custom_options=b"")
+        wt = (g.rng.integers(0, 2, (n, k), dtype=np.int8) * 2 - 1).astype(np.float32)
+        if alpha == "lsr":
+            a = np.float32(g.rng.uniform(0.3, 0.9))   # never a power of two
+            wt = wt * a
+        y = g.act(lead + (n,))
+        keep = {"keep_num_dims": True} if len(lead) > 1 else {}
+        g.m.add_op("FULLY_CONNECTED", [deq, g.const(wt), -1], [y], activation="NONE", **keep)
+        return bn_tail(y, lead + (n,), n, offset=offset * float(np.abs(wt[0, 0])))
+
+    wt = g.rng.standard_normal((widths[0], 3)).astype(np.float32) / np.float32(np.sqrt(3.0))
+    y = g.act((b, points, widths[0]))
+    g.m.add_op("FULLY_CONNECTED", [x, g.const(wt), g.const(g.rng.uniform(-0.5, 0.5, widths[0]).astype(np.float32),
+                                                            name="b")],
+               [y], activation="NONE", keep_num_dims=True)
+    x = bn_tail(y, (b, points, widths[0]), widths[0])
+    # the EMA-max offset: about the expected max over P points of a +-1 dot product of K terms (sd sqrt(K)),
+    # so the pooled features' signs depend on the points
+    lnp = np.log(max(points, 2))
+    e_max = np.sqrt(2 * lnp) - (np.log(lnp) + np.log(4 * np.pi)) / (2 * np.sqrt(2 * lnp))
+    for i, (k, n) in enumerate(zip(widths[:-1], widths[1:])):
+        last = i == len(widths) - 2
+        x = binary_layer(x, (b, points), k, n, offset=np.sqrt(k) * e_max if last and points > 1 else 0.0)
+    feat = g.act((b, widths[-1]))
+    g.m.add_op("REDUCE_MAX", [x, g.const(np.array([1], np.int32), np.int32, "axes")], [feat], keep_dims=False)
+    x, k = feat, widths[-1]
+    for n in head:
+        x = binary_layer(x, (b,), k, n)
+        k = n
+    wt = g.rng.standard_normal((classes, k)).astype(np.float32) / np.float32(np.sqrt(k))
+    logits = g.act((b, classes))
+    g.m.add_op("FULLY_CONNECTED", [x, g.const(wt), g.const(np.zeros(classes, np.float32), name="b")], [logits],
+               activation="NONE")
+    probs = g.act((b, classes))
+    g.m.add_op("SOFTMAX", [logits], [probs], beta=1.0)
+    g.m.outputs = [probs]
+    return g.m.serialize()
+
+
 MODELS = {"quicknet": quicknet, "quicknet_large": quicknet_large, "quicknet_small": quicknet_small,
           "birealnet18": birealnet18,
           "reactnet_a": reactnet_a, "realtobinarynet": realtobinarynet,

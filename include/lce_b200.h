@@ -251,6 +251,20 @@ int lce_b200_bconv2d_run_fused_fc(lce_b200_bconv2d* plan, const int32_t* in_dev,
                                   const float* bias_dev, int activation, const float* scale_dev,
                                   const float* shift_dev, int bn_activation, float* out_dev,
                                   int32_t* packed_out_dev, void* stream);
+/* lce_b200_bconv2d_run_fused_fc's binary dense layer followed by REDUCE_MAX over each image's rows, the
+ * plan's batch rows being images of `points` consecutive rows: max_out[b][c] is TFLite's reference
+ * reduction (cur = -FLT_MAX, then cur = y > cur ? y : cur in row order) of column c of rows b * points ..
+ * b * points + points - 1, each y computed as run_fused_fc computes it, and packed_out[b] = bitpack of
+ * max_out[b]. A NaN is never chosen, of equal values (-0.0, +0.0) the first row's wins, and an image
+ * whose values are all NaN or -inf gives -FLT_MAX. The columns are never stored: each CTA merges its
+ * rows into keys_dev, B * N 64-bit words (16-byte aligned) of workspace this call initialises, with
+ * atomicMax, so the result does not depend on the CTAs' order. max_out [B, N] and packed_out [B, N / 32]
+ * may each be NULL but not both; keys, max_out, packed_out and the input must not overlap. The plan is
+ * run_fused_fc's, with batch a multiple of points. */
+int lce_b200_bconv2d_run_fused_fc_max(lce_b200_bconv2d* plan, const int32_t* in_dev, const float* alpha_dev,
+                                      const float* bias_dev, int activation, const float* scale_dev,
+                                      const float* shift_dev, int bn_activation, int points, void* keys_dev,
+                                      float* max_out_dev, int32_t* packed_out_dev, void* stream);
 /* The signs of a dense layer's BatchNorm in one pass over a strided float [rows, channels] map
  * (row r starts at x_dev + r * x_pixel_stride):
  *   packed_out[r][ceil(channels/32)] = bitpack(x * scale[c] + shift[c]),
@@ -377,6 +391,13 @@ int lce_b200_f32_upsample_add_sign(const float* u_dev, int batch, int in_h, int 
  * out_dev is int64 [outer, inner] when out_int64 is set, else int32; every element is written. */
 int lce_b200_f32_argmax(const float* in_dev, int64_t outer, int n, int64_t inner, int out_int64, void* out_dev,
                         void* stream);
+/* TFLite's float REDUCE_MAX (TF/lite/kernels/internal/reference/reduce.h, from memory) of a float tensor
+ * viewed as [outer, n, inner], reduced over n (n >= 0): out[o][i] = the sequential result of cur =
+ * -FLT_MAX, then cur = x > cur ? x : cur for x = x[o][0][i] .. x[o][n-1][i]. A NaN is never chosen, of
+ * equal values (-0.0, +0.0) the first wins, and an all-NaN, all--inf or empty slice gives -FLT_MAX.
+ * Offsets are 64-bit. */
+int lce_b200_f32_reduce_max(const float* in_dev, int64_t outer, int64_t n, int64_t inner, float* out_dev,
+                            void* stream);
 /* The largest in_w * channels lce_b200_f32_resize_bilinear_argmax takes: it stages two source rows of
  * that many floats in shared memory. */
 int lce_b200_resize_bilinear_argmax_max_row_floats(void);
